@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — subscriber-AOI-queries/s of the spatial hot path (BASELINE.json metric) on N B200s.
+"""bench.py — subscriber-AOI-queries/s of the spatial hot path (BASELINE.json metric) on N H100s.
 
 A step = one batched tick over one synthetic snapshot: spatial-hash build of all entities (positions change
 every step, so the hash is rebuilt and handover candidates detected) -> AOI query + interest diff for every
@@ -56,6 +56,8 @@ def parse():
     ap.add_argument("--scaling", default="strong", choices=["strong", "weak"],
                     help="N>1: strong = the named config sharded over N GPUs (BASELINE config #4); weak = the world, the entities and "
                          "the subscribers grow N-fold in X (per-GPU work fixed)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the results of the last one as DIR/<name>.npy (float64, at most 64 MB in all)")
     return ap.parse_args()
 
 
@@ -85,7 +87,7 @@ def config_dict(wc, world, scaling):
             "tick": "build+query+interest-diff+emit-visible+fanout, positions change every step",
             "positions": "float32-valued (unrealpb.FVector widened by float64(), pkg/unrealpb/extension.go:10-24), computed on as float64",
             "l2": "inputs larger than L2 in effect: every step streams the expanded visible list (4 bytes x V, about 1.95 GB on the "
-                  "1M/100K workload) through the 126 MB L2, evicting the step's inputs; no explicit flush"}
+                  "1M/100K workload) through the 50 MB L2, evicting the step's inputs; no explicit flush"}
 
 
 def oracle_grid(wc):
@@ -222,6 +224,59 @@ def pinned(shape, dtype):
 
     t = torch.empty(shape, dtype=dtype, pin_memory=True)
     return t, t.numpy()
+
+
+DUMP_ARRAY_BYTES = 4 << 20   # per result array; the visible-list sample gets 4x that: 52 MB in all at most
+DUMP_VISIBLE_SLOTS = 256
+
+
+def dump_outputs(e, sm, S, out_dir):
+    """Writes what the last timed tick handed its caller, one float64 array per result, so that two builds can be compared
+    output for output: the tick summary, the (subscriber, cell, dist, interval) pairs, query statuses, the interest diff, visible
+    offsets, the visible lists of a fixed seeded sample of subscribers, the fan-out due list, the handover list and the cell CSR.
+    Lists whose order is not part of the result (diff, due, handover) are sorted by row.  64-bit integers are split into two
+    32-bit columns (hi, lo) so that float64 holds them exactly.  An array over its byte budget keeps evenly spaced rows."""
+    from channeld_b200 import capi
+
+    os.makedirs(out_dir, exist_ok=True)
+
+    def put(name, cols, sort_rows=False, budget=DUMP_ARRAY_BYTES):
+        split = []
+        for c in cols:
+            c = np.asarray(c)
+            if c.dtype.itemsize == 8 and c.dtype.kind in "iu":
+                u = c.view(np.uint64)
+                split += [u >> np.uint64(32), u & np.uint64(0xFFFFFFFF)]
+            else:
+                split.append(c)
+        a = np.stack([c.astype(np.float64) for c in split], axis=1) if split else np.zeros((0, 0))
+        if sort_rows and len(a):
+            a = a[np.lexsort(a.T[::-1])]
+        rows = max(1, budget // (8 * max(a.shape[1], 1)))
+        if len(a) > rows:
+            a = a[np.linspace(0, len(a) - 1, rows).astype(np.int64)]
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a))
+
+    put("summary", [np.array([getattr(sm, f) for f, _ in sm._fields_], np.uint64)])
+    pairs = e.get_pairs(sm.n_pairs)
+    sub_of_pair = np.repeat(np.arange(len(pairs["off"]) - 1, dtype=np.uint32), np.diff(pairs["off"].astype(np.int64)))
+    put("pairs", [sub_of_pair, pairs["channel"], pairs["dist"], pairs["interval"]])
+    put("query_status", [e.get_query_status(S)])
+    (new_sub, new_ch), (un_sub, un_ch) = e.get_diff(sm.n_sub_new, sm.n_unsub)
+    put("interest_diff", [np.r_[np.zeros(len(new_sub)), np.ones(len(un_sub))], np.r_[new_sub, un_sub], np.r_[new_ch, un_ch]], sort_rows=True)
+    voff = np.zeros(e.n_slots + 1, np.uint64)
+    e._ck(e.L.chd_get_visible(e.h, capi.ptr(voff), None))
+    put("visible_offsets", [voff])
+    slots = np.sort(np.random.default_rng(12345).choice(S, min(S, DUMP_VISIBLE_SLOTS), replace=False)) if S else np.zeros(0, np.int64)
+    vis = [e.get_visible_slot(int(j)) for j in slots]
+    put("visible_sample", [np.repeat(slots.astype(np.uint32), [len(v) for v in vis]), np.concatenate(vis) if vis else np.zeros(0)],
+        budget=4 * DUMP_ARRAY_BYTES)
+    due = e.get_due(sm.n_due)
+    put("due", [due[f] for f in due.dtype.names], sort_rows=True)
+    put("handover", list(e.get_handover(sm.n_handover)), sort_rows=True)
+    cs, se = e.get_cells()
+    put("cell_start", [cs])
+    put("sorted_entities", [se])
 
 
 def run_ours(args):
@@ -448,6 +503,8 @@ def run_ours(args):
         launches = e.launch_count() - launches0
         clocks = sampler.stop(tb, te) if rank == 0 else None
         sm = e.summary()  # raises on any capacity overflow during the timed steps
+        if args.dump_outputs:
+            dump_outputs(e, sm, S, args.dump_outputs if world == 1 else os.path.join(args.dump_outputs, "rank%d" % rank))
         ek_tot, ek_n = e.profile_get(capi.STAGE_EMIT_KERNEL)
         emit_kernel_ms_timed = ek_tot / max(ek_n, 1)
         e.profile_enable(True)  # instrumented pass (not timed): every stage, same inputs
@@ -750,26 +807,19 @@ def run_ours(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
             peak, peak_src = float(peaks["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
         except Exception:
-            peak = 6650.0
-            peak_src = "fallback 6.65 TB/s (B200_PROFILING.md)"
+            peak = 3350.0
+            peak_src = "fallback 3.35 TB/s (H100 SXM data sheet, HBM3)"
         ms_step = ms / args.steps
         value = S_total * args.steps / (ms * 1e-3)
         # Roofline of the dominant kernel (emit_visible), DRAM basis.  Algorithmic DRAM bytes per launch = 4 V (every visible
         # entry written once) + 4 N (the cell CSR payload read once; its re-reads are L2 hits by design: 16 MB of phase copies
-        # against a 126 MB L2).  SURVEY §8d's 8 V counts the L2-side re-reads as well: reported as l2_side_gbs, not as the
-        # fraction.  `traffic` = dram__bytes_read.sum + dram__bytes_write.sum of one launch from an `ncu --set full` pass over
-        # this tree (profiles/r2_emit_traffic.json names the commit it was taken on), null if that file is absent.
+        # against a 50 MB L2).  SURVEY §8d's 8 V counts the L2-side re-reads as well: reported as l2_side_gbs, not as the
+        # fraction.
         v_rank = float(sm.n_visible)
         n_sorted = float(sm.n_entities_in_world)
         ek_ms = stage["emit_kernel"]
         dram_bytes = 4.0 * v_rank + 4.0 * n_sorted
         achieved = (dram_bytes / (ek_ms * 1e-3)) / 1e9 if ek_ms > 0 else 0.0
-        traffic, traffic_src = None, None
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "r2_emit_traffic.json")))
-            traffic, traffic_src = tj["dram_bytes_per_launch"], tj.get("source")
-        except Exception:
-            pass
         out = {
             "metric": METRIC, "value": value, "unit": "queries/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms_step, "higher_is_better": True, "scaling": args.scaling if world > 1 else "strong", "vs_baseline": None,
@@ -804,7 +854,7 @@ def run_ours(args):
             "collectives": {"exchange": {0: None, 1: "one ncclAllGather per tick", 2: "peer windows: stores over NVLink into CUDA-IPC-mapped receive buffers + 64-bit flags, no collective call on the tick path"}[e.exchange_mode()],
                             "nccl_all_gathers_issued_by_the_library_rank0": e.collective_count(), "where": "chd_tick_sharded (libchd_b200.so)"} if world > 1 else None,
             "roofline": {"bound": "hbm", "kernel": "emit_visible_kernel", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak if peak else None, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                         "frac": achieved / peak if peak else None, "peak_source": peak_src,
                          "algorithmic_dram_bytes_per_launch": dram_bytes, "algorithmic_dram_bytes": "4*V + 4*N (writes + one read of the CSR)",
                          "kernel_ms": ek_ms, "l2_side_gbs": (8.0 * v_rank / (ek_ms * 1e-3)) / 1e9 if ek_ms > 0 else None,
                          "write_only_peak_gbs_this_run": wp,

@@ -1,6 +1,6 @@
-"""In-tree build of libchd_b200.so (hand-written CUDA for sm_100a + the C ABI of include/chd_gpu.h).
+"""In-tree build of libchd_b200.so (hand-written CUDA for sm_90a, the H100 + the C ABI of include/chd_gpu.h).
 
-nvcc cross-compiles without a GPU.  The .so is git-ignored but travels to the GPU box with the snapshot.
+nvcc cross-compiles without a GPU.  The .so is a build product: git-ignored, rebuilt when a source is newer.
 """
 import os
 import subprocess
@@ -12,7 +12,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libchd_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-fmad=false",            # belt and braces: all parity-critical FP64 uses explicit _rn intrinsics anyway
     "--expt-relaxed-constexpr",
@@ -41,7 +41,7 @@ def needs_build():
 
 
 def build(force=False, verbose=False, extra_flags=(), out=None):
-    """extra_flags / out: experiment builds (tools/), e.g. -DCHD_EMIT_ROWS=8 into another file; the product is LIB."""
+    """extra_flags / out: experiment builds, e.g. -DCHD_EMIT_ROWS=4 into another file; the product is LIB."""
     if out is None and not force and not needs_build():
         return LIB
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -131,7 +131,7 @@ def lib():
     if _lib is not None:
         return _lib
     path = _build.build()
-    if os.environ.get("CHD_EXPERIMENT_LIB"):  # tools/ only: an experiment build of the same sources (different tile constants)
+    if os.environ.get("CHD_EXPERIMENT_LIB"):  # experiments only: an experiment build of the same sources (different tile constants)
         path = os.environ["CHD_EXPERIMENT_LIB"]
     L = C.CDLL(path)
     vp = C.c_void_p

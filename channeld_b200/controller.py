@@ -120,7 +120,7 @@ def pack_queries(queries: Sequence[SpatialInterestQuery], subs=None):
 
 
 class GpuStaticGrid2DSpatialController:
-    """Drop-in for StaticGrid2DSpatialController (spatial.go:89-124) backed by the B200 engine."""
+    """Drop-in for StaticGrid2DSpatialController (spatial.go:89-124) backed by the GPU engine."""
 
     def __init__(self, device=0, max_entities=1 << 16, max_subscribers=1 << 12, **limits):
         self._device, self._ne, self._ns, self._limits = device, max_entities, max_subscribers, limits

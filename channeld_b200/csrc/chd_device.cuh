@@ -84,7 +84,7 @@ __device__ __host__ __forceinline__ uint32_t damping_interval_ms(uint32_t dist, 
 }
 
 // Go math.Cos (src/math/sin.go; Cephes polynomials + 3-part pi/4 reduction), call site spatial.go:295.
-// Restated from the published algorithm (the Go stdlib source is not under /root/reference: parity of the
+// Restated from the published algorithm (the Go stdlib source is not in the reference tree: parity of the
 // cone AOI is pinned only by TestConeAOI).  ok=false for |x| >= 2^29 (Payne-Hanek branch not reproduced).
 __device__ __forceinline__ double go_cos(double x, bool& ok) {
     ok = true;

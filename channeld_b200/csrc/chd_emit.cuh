@@ -5,9 +5,7 @@
 // Decomposition: the OUTPUT array is cut into fixed tiles of EMIT_TILE entries (load-balanced regardless of
 // how entities are distributed over cells).  A partition pass records the first pair of each tile; one CTA copies one
 // tile.  Every thread moves 16-byte chunks: stores are fully coalesced; loads are co-aligned 16-byte reads out of the
-// L2-resident phase copies of the cell CSR (4 x 4 B x N: 16 MB at 1 M entities, far below the 126 MB L2).
-// History (profiles/README.md): v1 4-byte moves, issue-bound, 0.75 ms -> v2/v3 phase-matched 16-byte moves on a persistent
-// grid of warp tiles, 0.355 ms -> this shape (round 2).
+// L2-resident phase copies of the cell CSR (4 x 4 B x N: 16 MB at 1 M entities, a third of the H100's 50 MB L2).
 #pragma once
 #include "chd_types.cuh"
 
@@ -142,12 +140,8 @@ __device__ __forceinline__ void emit_tile_general(uint64_t t, uint64_t n_tiles, 
     }
 }
 
-// One CTA per 16 KB tile of the output (EMIT_TILE = 4096 entries: EMIT_ROWS rows of 256 x 16 bytes), dispatched by the
-// hardware block scheduler.  Measured on B200 (tools/write_probe.cu, profiles/r2_write_probe.json): the same streaming copy
-// out of an L2-resident pool runs at 6.96 TB/s of writes with one CTA per 16 KB chunk, against 6.2 TB/s with a persistent
-// grid that walks the chunks round-robin (the round-1 shape) and 7.48 TB/s for a pure fill; 4 rows per thread beat 1 (more
-// loads in flight), streaming stores (st.global.cs) beat write-back ones by 15 % (the write stream does not evict the
-// L2-resident sources).
+// One CTA per 8 KB tile of the output (EMIT_TILE = 2048 entries: EMIT_ROWS rows of 256 x 16 bytes), dispatched by the
+// hardware block scheduler.  Streaming stores (st.global.cs) keep the write stream from evicting the L2-resident sources.
 // This kernel copies the SIMPLE tiles only (at most two segments: everything a thread needs is the 16-byte descriptor
 // {base0, base1, ends, p0}; the bases are phase-adjusted so every move is a co-aligned LDG.128 -> STG.128) and nothing else
 // lives in it, so that it fits 32 registers = 8 CTAs (all 64 warps) per SM; tiles with more segments are listed by the
@@ -233,9 +227,9 @@ __global__ void __launch_bounds__(EMIT_THREADS)
 
 
 // General kernel (round 1's shape): a persistent grid, every WARP owns whole 4 KB tiles (no block barrier anywhere), the segment
-// table of a tile lives in a warp-private slice of shared memory.  Used when cells are small against a 16 KB tile (many segments
+// table of a tile lives in a warp-private slice of shared memory.  Used when cells are small against a CTA tile (many segments
 // per tile: config #5's 152 entities per cell) or when the CSR payload does not fit the L2 (config #3: the copy is then DRAM-bound
-// on both sides and this shape reaches 0.95 of the copy peak, where the CTA-tile kernel above reaches 0.80).
+// on both sides).
 __global__ void __launch_bounds__(EMIT_THREADS, 4)
     emit_visible_warp_kernel(const uint32_t* __restrict__ n_pairs_ptr, uint64_t pair_cap, const uint64_t* __restrict__ voff,
                         const uint32_t* __restrict__ pair_cell, const uint32_t* __restrict__ cell_start,

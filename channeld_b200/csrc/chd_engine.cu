@@ -272,6 +272,7 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
         CCU(cudaStreamCreateWithPriority(&e->prep_stream, cudaStreamNonBlocking, hi_prio2));
     }
     CCU(cudaDeviceGetAttribute(&e->sm_count, cudaDevAttrMultiProcessorCount, device));
+    CCU(cudaDeviceGetAttribute(&e->l2_bytes, cudaDevAttrL2CacheSize, device));
 
     GridDev& g = e->g;
     g.off_x = cfg->world_offset_x; g.off_z = cfg->world_offset_z; g.w = cfg->grid_width; g.h = cfg->grid_height;

@@ -40,7 +40,8 @@ struct chd_engine {
     std::recursive_mutex mu;
     mutable std::string err;
     std::vector<void*> allocs;
-    int sm_count = 148;
+    int sm_count = 132;
+    int l2_bytes = 50 << 20;  // both read from the device in chd_create
     uint64_t n_launch = 0;  // kernels launched by this engine (bench.py reports it as gpu_launches)
     // CUDA graphs: the launch-bound small-kernel stages are captured once per (shape, parity) and replayed.
     struct GraphSlot {
@@ -207,7 +208,7 @@ struct chd_engine {
     bool early_ready = false;  // ev_join + ev_prep_done of the last tick are recorded
     bool early_results_tick = false;  // CHD_TICK_EARLY_RESULTS of the tick being enqueued
     // CHD_TICK_EARLY_RESULTS: the expanded-list kernel starts after the aux chain (interest + fan-out), so every host-facing
-    // result is final while it is still streaming (alternatives measured in round 1: profiles/README.md)
+    // result is final while it is still streaming
     cudaEvent_t wait_before_emit_kernel = nullptr;
     uint64_t *d_voff = nullptr, *d_vis_off = nullptr;
     uint64_t max_tiles = 0;

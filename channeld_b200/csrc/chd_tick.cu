@@ -10,13 +10,14 @@
 extern "C" {
 
 // Which copy kernel (host-known inputs only: nothing here waits for the device):
-//   CTA tiles + per-tile descriptors  when cells are large against a 16 KB tile (<= 2 segments per tile is the common case)
-//                                     AND the CSR's four phase copies stay L2-resident (the copy is then a pure write stream);
+//   CTA tiles + per-tile descriptors  when cells are large against a tile (<= 2 segments per tile is the common case)
+//                                     AND the CSR's four phase copies fit in half the L2 (they stay resident next to the write
+//                                     stream: the copy is then a pure write stream);
 //   warp tiles (round 1's kernel)     otherwise: many segments per tile (config #5) or sources streamed from DRAM (config #3).
 static bool emit_uses_cta_tiles(const chd_engine* e) {
     const uint64_t n_build = (uint64_t)e->n_own + (e->halo_on_device ? (uint64_t)e->border_cap : (uint64_t)e->n_halo);
     const uint64_t own_cells = (uint64_t)(e->g.col_hi - e->g.col_lo) * e->g.rows;  // (the whole grid on one GPU, the slab on N)
-    return (uint64_t)e->n_own / (own_cells ? own_cells : 1) >= (uint64_t)EMIT_TILE / 2 && n_build * 16ull <= (64ull << 20);
+    return (uint64_t)e->n_own / (own_cells ? own_cells : 1) >= (uint64_t)EMIT_TILE / 2 && n_build * 16ull <= (uint64_t)e->l2_bytes / 2;
 }
 
 // emit preparation on e->stream: per-pair output offsets (scan), per-tile first pairs / descriptors, per-subscriber offsets, V
@@ -48,7 +49,7 @@ static chd_status emit_kernel_enqueue(chd_engine* e, bool cta_tiles) {
     const uint64_t P = e->lim.max_pairs;
     StageTimer kt(e, CHD_STAGE_EMIT_KERNEL);
     if (cta_tiles) {
-        // One CTA per 16 KB tile, dispatched by the hardware block scheduler.  The tile count lives on the device; the grid is
+        // One CTA per tile, dispatched by the hardware block scheduler.  The tile count lives on the device; the grid is
         // sized from the last visible count the host has seen (+3 %: the kernel loops if that was too few, surplus CTAs exit
         // at once), from the capacity before that.
         const uint64_t cap_tiles = (e->lim.max_visible + EMIT_TILE - 1) / EMIT_TILE;

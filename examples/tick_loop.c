@@ -5,7 +5,7 @@
  *
  *   gcc -std=c99 -Iinclude examples/tick_loop.c -Lchanneld_b200 -lchd_b200 -Wl,-rpath,$PWD/channeld_b200 -lm -o tick_loop
  *
- * tests/test_abi.py compiles and links this file on every run (it needs a B200 to actually execute).
+ * tests/test_abi.py compiles and links this file on every run (it needs an H100 to actually execute).
  */
 #include <stdio.h>
 #include <stdlib.h>

@@ -1,5 +1,5 @@
 /*
- * chd_gpu.h — C ABI of the B200-native spatial interest-management + fan-out engine (libchd_b200.so).
+ * chd_gpu.h — C ABI of the H100-native spatial interest-management + fan-out engine (libchd_b200.so).
  *
  * This is the drop-in boundary behind channeld's SpatialController plugin surface
  * (reference: channeldorg/channeld @ 61fa8add, pkg/channeld/spatial.go:17-35).  A cgo shim binds exactly
@@ -19,7 +19,7 @@
  * take an internal mutex and may be called from any thread (the reference calls GetChannelId /
  * QueryChannelIds concurrently from channel goroutines, spatial.go:20-29).
  *
- * There is NO CPU fallback: every compute entry point runs sm_100a kernels and returns CHD_ERR_CUDA if no
+ * There is NO CPU fallback: every compute entry point runs sm_90a kernels and returns CHD_ERR_CUDA if no
  * device is usable.
  */
 #ifndef CHD_GPU_H

@@ -164,7 +164,7 @@ double orc_grid_size(const orc_grid* g) {  // spatial.go:134-139
 }
 
 // Go math.Cos (src/math/sin.go; Cephes cosf/sinf polynomials, 3-part pi/4 reduction).  The Go source is not
-// in /root/reference; this restates the published algorithm.  |x| >= 2^29 uses Payne-Hanek in Go; that branch
+// in the reference tree; this restates the published algorithm.  |x| >= 2^29 uses Payne-Hanek in Go; that branch
 // is not restated: QueryChannelIds rejects such cone angles (ORC_ERR_ANGLE_RANGE); this function alone falls back to libm.
 double orc_go_cos(double x) {
     static const double kSin[6] = {1.58962301576546568060e-10, -2.50507477628578072866e-8, 2.75573136213857245213e-6,

@@ -19,7 +19,7 @@
  *     TestGetAdjacentChannels) — transcribed in tests/test_oracle_kat.py.
  *   - fan-out windows: PINNED by data_test.go:98-166 (F0,F7,F2,F8,F3; doc/design.md:94-109).
  *     data_test.go:168-197 does not follow from the code as written (SURVEY.md §4) and is not used.
- *   - math.Cos (Go stdlib, go 1.25 per go.mod:3; source NOT under /root/reference): restated
+ *   - math.Cos (Go stdlib, go 1.25 per go.mod:3; source NOT in the reference tree): restated
  *     from the published Cephes-derived algorithm; cone AOI is "parity unpinned" beyond TestConeAOI.
  *   - SpotsAOI, dist values, damping, interest diff, visible-entity sets, the ADJACENT_CHANNELS broadcast
  *     branch (message.go:188-239): no reference test exists ("parity unpinned" by the reference); the

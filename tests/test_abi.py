@@ -1,5 +1,5 @@
-"""CPU-side checks of the drop-in boundary: the C-ABI library builds for sm_100a, loads, and exports every
-symbol include/chd_gpu.h declares.  No compute calls (there is no GPU in the build container)."""
+"""CPU-side checks of the drop-in boundary: the C-ABI library builds for sm_90a, loads, and exports every
+symbol include/chd_gpu.h declares.  No compute calls: these run without a GPU."""
 import ctypes as C
 import os
 import re

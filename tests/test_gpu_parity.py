@@ -1,6 +1,6 @@
 """GPU parity tests: the CUDA path, called through the C ABI, against the CPU oracle on the same inputs.
 Bit-exact: integer/index work, and FP64 work that must reproduce Go's rounding operation by operation.
-Run on the B200 box:  python -m pytest tests -m gpu
+Run on an H100:  python -m pytest tests -m gpu
 """
 import ctypes as C
 import math
@@ -1064,7 +1064,7 @@ def test_emit_descriptor_base_wraps_below_zero(chd, oracle):
     centres = [(wc.offx + (c + 0.5) * wc.w, wc.offz + (r + 0.5) * wc.h) for r in range(wc.rows) for c in range(wc.cols)]
     ids = oracle.cell_of(og, np.array([c[0] for c in centres]), np.array([c[1] for c in centres]))
     centres = [centres[k] for k in np.argsort(ids)]  # ascending cell index = CSR order
-    counts = [1001, 5000, 8192 + 2005, 0]  # cell 1 starts at 1001; the big cell ends 2005 entries into its third tile: 2005 % 4 == 1001 % 4
+    counts = [1001, 5000, 8192 + 2005, 0]  # cell 1 starts at 1001; the big cell ends 2005 entries into the tile that starts at 8192: 2005 % 4 == 1001 % 4
     rng = np.random.default_rng(5)
     xs, zs = [], []
     for (cx_, cz_), n in zip(centres, counts):

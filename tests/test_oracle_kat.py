@@ -1,9 +1,9 @@
 """Pins the CPU oracle against every known-answer test the reference holds for the spatial hot path.
 
-Transcribed (inputs + expected results only) from /root/reference/pkg/channeld/spatial_test.go:
+Transcribed (inputs + expected results only) from the reference's pkg/channeld/spatial_test.go:
   TestGetChannelId1 :803-848, TestGetChannelId2 :762-801, TestSphereAOI :244-360, TestBoxAOI :362-491,
   TestConeAOI :21-242, TestGetAdjacentChannels :493-526
-and /root/reference/pkg/channeld/data_test.go TestFanOutChannelData :98-166 (doc/design.md:94-109).
+and the reference's pkg/channeld/data_test.go TestFanOutChannelData :98-166 (doc/design.md:94-109).
 SpatialChannelIdStart = 65536 (settings.go:94).
 """
 import math
