@@ -31,10 +31,10 @@ bool chd_is_device_ptr(const chd_engine* e, const void* p) {
     return a.type == cudaMemoryTypeDevice && a.device == e->device;
 }
 
-chd_status chd_epoch_tick(chd_engine* e, int stage) {
+chd_status chd_epoch_tick(chd_engine* e, cudaStream_t s, int stage) {
     if ((++e->stage_execs[stage] & ((1ull << 20) - 1)) != 0) return CHD_OK;
     for (ScanSite* site : e->sites)
-        if (site->stage == stage && site->desc) CU(e, cudaMemsetAsync(site->desc, 0, site->tiles * 8, e->stream));
+        if (site->stage == stage && site->desc) CU(e, cudaMemsetAsync(site->desc, 0, site->tiles * 8, s));
     return CHD_OK;
 }
 
@@ -422,7 +422,7 @@ chd_status chd_profile_timeline(chd_engine* e, int stage, double* start_ms, doub
     if (!e || stage < 0 || stage >= CHD_STAGE_COUNT || !start_ms || !stop_ms || !e->ev) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
     CU(e, cudaStreamSynchronize(e->stream));
-    if (e->aux_stream) CU(e, cudaStreamSynchronize(e->aux_stream));
+    CU(e, cudaStreamSynchronize(e->aux_stream));
     if (!e->stage_n[CHD_STAGE_TICK] || !e->stage_n[stage]) return CHD_ERR_STATE;
     cudaEvent_t t0 = e->evt(CHD_STAGE_TICK, e->stage_n[CHD_STAGE_TICK] - 1, 0);
     float a = 0, b = 0;

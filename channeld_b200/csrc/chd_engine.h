@@ -35,8 +35,8 @@ struct chd_engine {
     int device = 0;
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    // Guards (a) the shared query scratch between the stateless query entry points and the tick driver and (b) the
-    // temporary redirection of `stream` to aux_stream while the interest / fan-out chain is being enqueued.
+    // Guards (a) the shared query scratch between the stateless query entry points and the interest update and (b) a CUDA
+    // graph capture on `stream` against launches of the stateless entry points, which may run on other threads.
     std::recursive_mutex mu;
     mutable std::string err;
     std::vector<void*> allocs;
@@ -50,7 +50,6 @@ struct chd_engine {
         uint64_t nodes = 0;
     };
     bool use_graphs = true;
-    bool overlap_fanout = true;        // chd_tick runs interest + fan-out on aux_stream concurrently with build + emit
     cudaStream_t aux_stream = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_interest = nullptr, ev_pairs = nullptr;
     bool interest_pending = false, pending_fanout = false;  // chd_begin_interest issued, not yet joined by chd_tick
@@ -206,10 +205,6 @@ struct chd_engine {
     uint64_t fetch_issued = 0, fetch_waited = 0;
     bool fetch_guard = false;
     bool early_ready = false;  // ev_join + ev_prep_done of the last tick are recorded
-    bool early_results_tick = false;  // CHD_TICK_EARLY_RESULTS of the tick being enqueued
-    // CHD_TICK_EARLY_RESULTS: the expanded-list kernel starts after the aux chain (interest + fan-out), so every host-facing
-    // result is final while it is still streaming
-    cudaEvent_t wait_before_emit_kernel = nullptr;
     uint64_t *d_voff = nullptr, *d_vis_off = nullptr;
     uint64_t max_tiles = 0;
     uint64_t vis_estimate = 0;  // n_visible of the last summary the host decoded (0 = none yet): sizes the emit grid
@@ -297,16 +292,18 @@ struct chd_engine {
         CU(e, cudaGetLastError());                    \
     } while (0)
 
-struct StageTimer {  // records a CUDA-event pair around a stage on the engine stream when profiling is on
+struct StageTimer {  // records a CUDA-event pair around a stage on stream `s` when profiling is on
     chd_engine* e;
+    cudaStream_t s;
     int stage;
     bool on;
-    StageTimer(chd_engine* e_, int stage_) : e(e_), stage(stage_), on(e_->profiling == 1 || (e_->profiling == 2 && stage_ == CHD_STAGE_EMIT_KERNEL)) {
-        if (on) cudaEventRecord(e->evt(stage, e->stage_n[stage], 0), e->stream);
+    StageTimer(chd_engine* e_, cudaStream_t s_, int stage_)
+        : e(e_), s(s_), stage(stage_), on(e_->profiling == 1 || (e_->profiling == 2 && stage_ == CHD_STAGE_EMIT_KERNEL)) {
+        if (on) cudaEventRecord(e->evt(stage, e->stage_n[stage], 0), s);
     }
     ~StageTimer() {
         if (on) {
-            cudaEventRecord(e->evt(stage, e->stage_n[stage], 1), e->stream);
+            cudaEventRecord(e->evt(stage, e->stage_n[stage], 1), s);
             e->stage_n[stage]++;
         }
     }
@@ -340,18 +337,22 @@ void chd_dfree(chd_engine* e, void* p);
 chd_status chd_ensure_upload_stream(chd_engine* e);
 chd_status chd_read_u32(chd_engine* e, const uint32_t* d, uint32_t* v);
 chd_status chd_decode_summary(chd_engine* e, chd_tick_summary* out);
-chd_status chd_assign_cells_impl(chd_engine* e);
-chd_status chd_note_pos_read(chd_engine* e);
+chd_status chd_assign_cells_impl(chd_engine* e, cudaStream_t s);
+chd_status chd_note_pos_read(chd_engine* e, cudaStream_t s);
 // Called on the host wherever a stage's epoch is about to be bumped on the device: every 2^20 executions of a stage the
-// descriptors of its scan sites are cleared, so no descriptor can survive until the 22-bit epoch repeats.
-chd_status chd_epoch_tick(chd_engine* e, int stage);
+// descriptors of its scan sites are cleared, so no descriptor can survive until the 22-bit epoch repeats.  `s` is the
+// stream the stage runs on, so the clear is ordered before the stage's scans.
+chd_status chd_epoch_tick(chd_engine* e, cudaStream_t s, int stage);
 // lifecycle / migration calls may name slots beyond the current count: extends the slot table (new slots hold no pairs)
 chd_status chd_grow_slots(chd_engine* e, uint32_t new_n);
-chd_status chd_fetch_guard(chd_engine* e);
+chd_status chd_fetch_guard(chd_engine* e, cudaStream_t s);
+// chd_build / chd_update_interest without the fetch guard, enqueued on `s` (chd_tick runs the interest update on aux_stream)
+chd_status chd_build_on(chd_engine* e, cudaStream_t s);
+chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query_batch* q, int64_t now_ns);
 // what the fan-out / payload kernels read: the host-owned CSR snapshot (staged or zero-copy) or the device-owned rings
 RingDev chd_ring_view(const chd_engine* e);
 // one stable LSD radix pass (histogram, look-back scan, scatter) over 32-bit keys; chd_entities.cu
-chd_status chd_sort_pass_any(chd_engine* e, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in, uint32_t n,
+chd_status chd_sort_pass_any(chd_engine* e, cudaStream_t s, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in, uint32_t n,
                              const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits, uint32_t* key_out,
                              uint32_t* val_out, ScatterExtras ex = ScatterExtras{0, nullptr, 0, nullptr}, unsigned long long* bump = nullptr);
 }
@@ -363,15 +364,15 @@ static inline uint64_t mix_key(uint64_t h, uint64_t v) {
     return h;
 }
 
-// Runs `enqueue` (kernel launches + memsets only, no host sync) either directly or as a replayed CUDA graph.
+// Runs `enqueue` (kernel launches + memsets on `s` only, no host sync) either directly or as a CUDA graph replayed on `s`.
 // A graph is captured only after the same key was seen twice in a row, so workloads whose batch shape changes
 // every tick simply run direct launches.
 template <typename F>
-static chd_status run_stage(chd_engine* e, chd_engine::GraphSlot& slot, uint64_t key, F&& enqueue) {
+static chd_status run_stage(chd_engine* e, cudaStream_t s, chd_engine::GraphSlot& slot, uint64_t key, F&& enqueue) {
     key |= 1;  // never 0
-    if (!e->use_graphs || e->stream == nullptr) return enqueue();
+    if (!e->use_graphs || s == nullptr) return enqueue();
     if (slot.exec && slot.key == key) {
-        CU(e, cudaGraphLaunch(slot.exec, e->stream));
+        CU(e, cudaGraphLaunch(slot.exec, s));
         e->n_launch += slot.nodes;
         e->graph_launches++;
         return CHD_OK;
@@ -385,13 +386,13 @@ static chd_status run_stage(chd_engine* e, chd_engine::GraphSlot& slot, uint64_t
         slot.exec = nullptr;
     }
     const uint64_t l0 = e->n_launch;
-    // Stateless entry points (chd_cell_of, chd_query_channel_ids) may be called from other threads and launch into the same
+    // Stateless entry points (chd_cell_of, chd_query_channel_ids) may be called from other threads and launch into the engine
     // stream: they hold the engine mutex for their whole call, so taking it here keeps their work out of the capture.
     std::lock_guard<std::recursive_mutex> capture_lock(e->mu);
-    CU(e, cudaStreamBeginCapture(e->stream, cudaStreamCaptureModeThreadLocal));
+    CU(e, cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
     chd_status st = enqueue();
     cudaGraph_t g = nullptr;
-    cudaError_t r = cudaStreamEndCapture(e->stream, &g);
+    cudaError_t r = cudaStreamEndCapture(s, &g);
     if (st != CHD_OK || r != cudaSuccess || !g) {
         if (g) cudaGraphDestroy(g);
         if (st == CHD_OK) {
@@ -416,7 +417,7 @@ static chd_status run_stage(chd_engine* e, chd_engine::GraphSlot& slot, uint64_t
     e->n_launch = l0;
     slot.key = key;
     e->graph_captures++;
-    CU(e, cudaGraphLaunch(slot.exec, e->stream));
+    CU(e, cudaGraphLaunch(slot.exec, s));
     e->n_launch += slot.nodes;
     e->graph_launches++;
     return CHD_OK;

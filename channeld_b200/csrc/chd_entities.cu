@@ -12,7 +12,7 @@ struct FusedAssign {
     HandoverOut ho;
 };
 template <int BINS>
-static chd_status sort_pass(chd_engine* e, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in, uint32_t n,
+static chd_status sort_pass(chd_engine* e, cudaStream_t s, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in, uint32_t n,
                             const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits, uint32_t* key_out,
                             uint32_t* val_out, ScatterExtras ex, unsigned long long* bump, const FusedAssign* assign = nullptr, int half = 0) {
     // half: 0 = the whole pass, 1 = histogram + scan only, 2 = scatter only (single-pass builds are split so that the emit
@@ -20,38 +20,38 @@ static chd_status sort_pass(chd_engine* e, uint32_t* hist, const ScanSite& site,
     const uint32_t mask = (1u << bits) - 1u;
     if (half == 2) goto scatter;
     if (assign)
-        assign_hist_kernel<BINS><<<nblocks, BUILD_THREADS, 0, e->stream>>>(e->g, assign->x, assign->z, n, assign->key, assign->prev, assign->ho, per_block, mask,
-                                                                           hist, nblocks, bump);
+        assign_hist_kernel<BINS><<<nblocks, BUILD_THREADS, 0, s>>>(e->g, assign->x, assign->z, n, assign->key, assign->prev, assign->ho, per_block, mask,
+                                                                   hist, nblocks, bump);
     else
-        radix_hist_kernel<BINS><<<nblocks, BUILD_THREADS, 0, e->stream>>>(key_in, n, n_ptr, per_block, shift, mask, hist, nblocks, bump);
+        radix_hist_kernel<BINS><<<nblocks, BUILD_THREADS, 0, s>>>(key_in, n, n_ptr, per_block, shift, mask, hist, nblocks, bump);
     KCHECK(e);
-    SCAN(e, exclusive_scan_1p<uint32_t, uint32_t>(hist, hist, (uint64_t)BINS * nblocks, site, e->stream));
+    SCAN(e, exclusive_scan_1p<uint32_t, uint32_t>(hist, hist, (uint64_t)BINS * nblocks, site, s));
     if (half == 1) return CHD_OK;
 scatter:
     // bandwidth-bound regime: reorder each tile by digit in shared memory first (coalesced runs); small inputs are latency-bound
     // and take the plain scatter (fewer barriers per tile)
     if (n > (2u << 20))
-        radix_scatter_sorted_kernel<BINS><<<nblocks, BUILD_THREADS, 0, e->stream>>>(key_in, val_in, n, n_ptr, per_block, shift, mask, hist, nblocks,
-                                                                                   key_out, val_out, ex);
+        radix_scatter_sorted_kernel<BINS><<<nblocks, BUILD_THREADS, 0, s>>>(key_in, val_in, n, n_ptr, per_block, shift, mask, hist, nblocks,
+                                                                           key_out, val_out, ex);
     else
-        radix_scatter_kernel<BINS><<<nblocks, BUILD_THREADS, 0, e->stream>>>(key_in, val_in, n, n_ptr, per_block, shift, mask, hist, nblocks,
-                                                                            key_out, val_out, ex);
+        radix_scatter_kernel<BINS><<<nblocks, BUILD_THREADS, 0, s>>>(key_in, val_in, n, n_ptr, per_block, shift, mask, hist, nblocks,
+                                                                    key_out, val_out, ex);
     KCHECK(e);
     return CHD_OK;
 }
 
-static chd_status sort_pass_fused(chd_engine* e, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in, uint32_t n,
-                                  const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits, uint32_t* key_out,
+static chd_status sort_pass_fused(chd_engine* e, cudaStream_t s, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in,
+                                  uint32_t n, const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits, uint32_t* key_out,
                                   uint32_t* val_out, ScatterExtras ex, unsigned long long* bump, const FusedAssign* assign, int half = 0) {
-    if (bits <= 8) return sort_pass<256>(e, hist, site, key_in, val_in, n, n_ptr, per_block, nblocks, shift, bits, key_out, val_out, ex, bump, assign, half);
-    return sort_pass<1024>(e, hist, site, key_in, val_in, n, n_ptr, per_block, nblocks, shift, bits, key_out, val_out, ex, bump, assign, half);
+    if (bits <= 8) return sort_pass<256>(e, s, hist, site, key_in, val_in, n, n_ptr, per_block, nblocks, shift, bits, key_out, val_out, ex, bump, assign, half);
+    return sort_pass<1024>(e, s, hist, site, key_in, val_in, n, n_ptr, per_block, nblocks, shift, bits, key_out, val_out, ex, bump, assign, half);
 }
 
-chd_status chd_sort_pass_any(chd_engine* e, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in,
+chd_status chd_sort_pass_any(chd_engine* e, cudaStream_t s, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in,
                                 uint32_t n, const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits,
                                 uint32_t* key_out, uint32_t* val_out, ScatterExtras ex,
                                 unsigned long long* bump) {
-    return sort_pass_fused(e, hist, site, key_in, val_in, n, n_ptr, per_block, nblocks, shift, bits, key_out, val_out, ex, bump, nullptr);
+    return sort_pass_fused(e, s, hist, site, key_in, val_in, n, n_ptr, per_block, nblocks, shift, bits, key_out, val_out, ex, bump, nullptr);
 }
 
 extern "C" {
@@ -249,30 +249,28 @@ chd_status chd_set_entity_ids(chd_engine* e, const uint32_t* gid, uint32_t n) {
 
 // The engine's position buffers are double-buffered for chd_prefetch_entities: remember (outside any graph capture)
 // the last kernel that read the front pair, so an upload into it can be ordered after that read.
-chd_status chd_note_pos_read(chd_engine* e) {
+chd_status chd_note_pos_read(chd_engine* e, cudaStream_t s) {
     if (e->pos_x != e->d_x || !e->ev_pos_read[e->pos_buf]) return CHD_OK;
-    CU(e, cudaEventRecord(e->ev_pos_read[e->pos_buf], e->stream));
+    CU(e, cudaEventRecord(e->ev_pos_read[e->pos_buf], s));
     e->pos_read_recorded[e->pos_buf] = true;
     return CHD_OK;
 }
 
-chd_status chd_assign_cells_impl(chd_engine* e);
-
 chd_status chd_assign_cells(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     {
-        chd_status gs_ = chd_fetch_guard(e);
+        chd_status gs_ = chd_fetch_guard(e, e->stream);
         if (gs_ != CHD_OK) return gs_;
     }
     const bool was_assigned = e->assigned;
-    chd_status st = chd_assign_cells_impl(e);
-    if (st == CHD_OK && !was_assigned) st = chd_note_pos_read(e);
+    chd_status st = chd_assign_cells_impl(e, e->stream);
+    if (st == CHD_OK && !was_assigned) st = chd_note_pos_read(e, e->stream);
     return st;
 }
 
 // host-side half of a cell assignment: the key buffers swap (handover detection compares against the keys of the previous
 // assignment, same entity count; swapped, never copied), the handover counter is zeroed.  Returns the previous keys or nullptr.
-static chd_status assign_prepare(chd_engine* e, uint32_t** prev_out, HandoverOut* ho) {
+static chd_status assign_prepare(chd_engine* e, cudaStream_t s, uint32_t** prev_out, HandoverOut* ho) {
     uint32_t* prev = nullptr;
     if (e->have_prev_key) {
         uint32_t* t = e->d_key;
@@ -281,21 +279,21 @@ static chd_status assign_prepare(chd_engine* e, uint32_t** prev_out, HandoverOut
         prev = e->d_prev_key;
     }
     *ho = HandoverOut{e->d_ho_entity, e->d_ho_src, e->d_ho_dst, &e->d_ctr->n_handover, e->ho_cap};
-    CU(e, cudaMemsetAsync(&e->d_ctr->n_handover, 0, 4, e->stream));
+    CU(e, cudaMemsetAsync(&e->d_ctr->n_handover, 0, 4, s));
     *prev_out = prev;
     return CHD_OK;
 }
 
-chd_status chd_assign_cells_impl(chd_engine* e) {
+chd_status chd_assign_cells_impl(chd_engine* e, cudaStream_t s) {
     CU(e, cudaSetDevice(e->device));
     if (e->assigned) return CHD_OK;
     uint32_t* prev = nullptr;
     HandoverOut ho{};
-    chd_status st = assign_prepare(e, &prev, &ho);
+    chd_status st = assign_prepare(e, s, &prev, &ho);
     if (st != CHD_OK) return st;
     if (e->n_own) {
-        assign_cells_kernel<<<blocks_for(e->n_own, 256), 256, 0, e->stream>>>(e->g, e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z,
-                                                                              e->n_own, e->d_key, prev, ho, e->assign_bump);
+        assign_cells_kernel<<<blocks_for(e->n_own, 256), 256, 0, s>>>(e->g, e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z,
+                                                                      e->n_own, e->d_key, prev, ho, e->assign_bump);
         KCHECK(e);
         e->have_prev_key = true;
         e->assign_bump = nullptr;  // consumed
@@ -307,7 +305,7 @@ chd_status chd_assign_cells_impl(chd_engine* e) {
 
 // part: 0 = the whole build; single-pass builds only: 1 = cell assignment + histogram + scan + CSR offsets, 2 = scatter (+ phase
 // copies).  The cell CSR offsets are final after part 1.
-static chd_status build_enqueue(chd_engine* e, bool with_assign, int part = 0) {
+static chd_status build_enqueue(chd_engine* e, cudaStream_t s, bool with_assign, int part = 0) {
     chd_status st;
     FusedAssign fa{};
     const FusedAssign* fap = nullptr;
@@ -316,7 +314,7 @@ static chd_status build_enqueue(chd_engine* e, bool with_assign, int part = 0) {
             // single-GPU build: GetChannelId per entity is fused into the first pass's histogram kernel
             uint32_t* prev = nullptr;
             HandoverOut ho{};
-            st = assign_prepare(e, &prev, &ho);
+            st = assign_prepare(e, s, &prev, &ho);
             if (st != CHD_OK) return st;
             fa = FusedAssign{e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z, e->d_key, prev, ho};
             fap = &fa;
@@ -324,7 +322,7 @@ static chd_status build_enqueue(chd_engine* e, bool with_assign, int part = 0) {
             e->n_halo = 0;
             e->assigned = true;
         } else {
-            st = chd_assign_cells_impl(e);
+            st = chd_assign_cells_impl(e, s);
             if (st != CHD_OK) return st;
         }
     }
@@ -344,44 +342,41 @@ static chd_status build_enqueue(chd_engine* e, bool with_assign, int part = 0) {
     uint32_t nblocks = (n + per_block - 1) / per_block;
     if (nblocks == 0) nblocks = 1;
     const uint32_t* vals = e->have_gid ? e->d_gid : nullptr;
-    // Phase copies: written by a separate fully-coalesced pass after the scatter.  (Fusing them into the scatter saves a launch but
-    // does 4 scattered 4-byte stores per entity: measured slower at every size — 69 vs 59 us per build at N = 1 M, 325 vs 205 us
-    // at N = 10 M.)
-    const bool fuse_phases = false;
-    const uint32_t fused_stride = fuse_phases ? e->phase_stride : 0u;
+    // The scatters write no phase copies (ScatterExtras stride 0): a separate fully-coalesced pass writes them afterwards.  (Fusing
+    // them into the scatter saves a launch but does 4 scattered 4-byte stores per entity: measured slower at every size — 69 vs
+    // 59 us per build at N = 1 M, 325 vs 205 us at N = 10 M.)
     if (passes == 1 && part != 0) {
         if (part == 1) {
-            st = sort_pass_fused(e, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent,
+            st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent,
                                  ScatterExtras{0, nullptr, C, nullptr}, e->d_epoch + EP_BUILD, fap, 1);
             if (st != CHD_OK) return st;
-            publish_cell_start_kernel<<<blocks_for((uint64_t)C + 2, 256), 256, 0, e->stream>>>(e->d_hist, nblocks, C, n, n_ptr, e->d_cell_start,
-                                                                                                 &e->d_ctr->n_entities_in_world);
+            publish_cell_start_kernel<<<blocks_for((uint64_t)C + 2, 256), 256, 0, s>>>(e->d_hist, nblocks, C, n, n_ptr, e->d_cell_start,
+                                                                                         &e->d_ctr->n_entities_in_world);
             KCHECK(e);
             return CHD_OK;
         }
-        st = sort_pass_fused(e, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent,
-                             ScatterExtras{fused_stride, nullptr, C, nullptr}, nullptr, nullptr, 2);
+        st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent,
+                             ScatterExtras{0, nullptr, C, nullptr}, nullptr, nullptr, 2);
         if (st != CHD_OK) return st;
     } else if (passes == 1) {
         // single pass: digit == key, so the scatter also publishes the CSR offsets
-        ScatterExtras ex{fused_stride, e->d_cell_start, C, &e->d_ctr->n_entities_in_world};
-        st = sort_pass_fused(e, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent, ex,
+        ScatterExtras ex{0, e->d_cell_start, C, &e->d_ctr->n_entities_in_world};
+        st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent, ex,
                              e->d_epoch + EP_BUILD, fap);
         if (st != CHD_OK) return st;
     } else {
-        st = sort_pass_fused(e, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, e->d_tmp_key, e->d_tmp_val,
+        st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, e->d_tmp_key, e->d_tmp_val,
                              ScatterExtras{0, nullptr, 0, nullptr}, e->d_epoch + EP_BUILD, fap);
         if (st != CHD_OK) return st;
-        ScatterExtras ex{fused_stride, nullptr, C, nullptr};
-        st = chd_sort_pass_any(e, e->d_hist, e->site_hist_b, e->d_tmp_key, e->d_tmp_val, n, n_ptr, per_block, nblocks, bits0, bits1, e->d_sorted_key,
-                           e->d_sorted_ent, ex);
+        st = chd_sort_pass_any(e, s, e->d_hist, e->site_hist_b, e->d_tmp_key, e->d_tmp_val, n, n_ptr, per_block, nblocks, bits0, bits1, e->d_sorted_key,
+                               e->d_sorted_ent, ScatterExtras{0, nullptr, C, nullptr});
         if (st != CHD_OK) return st;
-        cell_bounds_kernel<<<blocks_for((uint64_t)n + 1, 256), 256, 0, e->stream>>>(e->d_sorted_key, n, n_ptr, C, e->d_cell_start,
-                                                                                      &e->d_ctr->n_entities_in_world);
+        cell_bounds_kernel<<<blocks_for((uint64_t)n + 1, 256), 256, 0, s>>>(e->d_sorted_key, n, n_ptr, C, e->d_cell_start,
+                                                                              &e->d_ctr->n_entities_in_world);
         KCHECK(e);
     }
-    if (!fuse_phases && n) {
-        replicate_phases_kernel<<<blocks_for(n, 256), 256, 0, e->stream>>>(e->d_sorted_ent, n, n_ptr, e->phase_stride, e->d_sorted4);
+    if (n) {
+        replicate_phases_kernel<<<blocks_for(n, 256), 256, 0, s>>>(e->d_sorted_ent, n, n_ptr, e->phase_stride, e->d_sorted4);
         KCHECK(e);
     }
     return CHD_OK;
@@ -390,12 +385,13 @@ static chd_status build_enqueue(chd_engine* e, bool with_assign, int part = 0) {
 chd_status chd_build(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
-    {
-        chd_status gs_ = chd_fetch_guard(e);
-        if (gs_ != CHD_OK) return gs_;
-    }
-    StageTimer timer(e, CHD_STAGE_BUILD);
-    chd_status st = chd_epoch_tick(e, EP_BUILD);
+    chd_status st = chd_fetch_guard(e, e->stream);
+    return st != CHD_OK ? st : chd_build_on(e, e->stream);
+}
+
+chd_status chd_build_on(chd_engine* e, cudaStream_t s) {
+    StageTimer timer(e, s, CHD_STAGE_BUILD);
+    chd_status st = chd_epoch_tick(e, s, EP_BUILD);
     if (st != CHD_OK) return st;
     bool counts_recorded = false;
     if (!e->assigned && !e->halo_on_device) {
@@ -408,7 +404,7 @@ chd_status chd_build(chd_engine* e) {
         // single-pass builds (<= 1023 cells) run as two replayable halves with an event in between: the cell CSR offsets are
         // final after the first (assignment + histogram + scan), so the emit preparation overlaps the scatter
         const bool split = e->g.cells + 1 <= BUILD_MAX_BINS && e->n_own > 0;
-        st = run_stage(e, e->g_build[slot], key, [&]() { return build_enqueue(e, true, split ? 1 : 0); });
+        st = run_stage(e, s, e->g_build[slot], key, [&]() { return build_enqueue(e, s, true, split ? 1 : 0); });
         if (st == CHD_OK && !e->assigned) {  // replayed graph: mirror the host-side bookkeeping of chd_assign_cells
             if (e->have_prev_key) {
                 uint32_t* t = e->d_key;
@@ -420,24 +416,24 @@ chd_status chd_build(chd_engine* e) {
             e->assigned = true;
         }
         if (st == CHD_OK && split) {
-            CU(e, cudaEventRecord(e->ev_counts, e->stream));
+            CU(e, cudaEventRecord(e->ev_counts, s));
             counts_recorded = true;
-            st = run_stage(e, e->g_build_b[slot], mix_key(key, 0x62), [&]() { return build_enqueue(e, false, 2); });
+            st = run_stage(e, s, e->g_build_b[slot], mix_key(key, 0x62), [&]() { return build_enqueue(e, s, false, 2); });
         }
-        if (st == CHD_OK) st = chd_note_pos_read(e);
+        if (st == CHD_OK) st = chd_note_pos_read(e, s);
     } else if (e->assigned && e->halo_on_device) {
         // multi-GPU flow: cells were assigned by chd_export_border and the halo appended on the device; the sort over
         // own + halo entities is sized by capacity (device-side length) and therefore replayable as well.
         const int slot = e->d_key == e->d_key_a ? 0 : 1;
         uint64_t key = mix_key(mix_key(mix_key(0x736f7274ull, e->lim.max_entities), e->have_gid), (uint64_t)(uintptr_t)e->d_key);
-        st = run_stage(e, e->g_build[slot], key, [&]() { return build_enqueue(e, false); });
+        st = run_stage(e, s, e->g_build[slot], key, [&]() { return build_enqueue(e, s, false); });
     } else {
         const bool with_assign = !e->assigned;
-        st = build_enqueue(e, with_assign);
-        if (st == CHD_OK && with_assign) st = chd_note_pos_read(e);
+        st = build_enqueue(e, s, with_assign);
+        if (st == CHD_OK && with_assign) st = chd_note_pos_read(e, s);
     }
     if (st != CHD_OK) return st;
-    if (!counts_recorded) CU(e, cudaEventRecord(e->ev_counts, e->stream));  // (cell counts final = build done)
+    if (!counts_recorded) CU(e, cudaEventRecord(e->ev_counts, s));  // (cell counts final = build done)
     e->n_sorted = e->n_own + e->n_halo;
     e->built = true;
     e->entities_dirty = false;

@@ -38,7 +38,7 @@ chd_status chd_due_classes(chd_engine* e, uint32_t* out_class_of, uint32_t* out_
     CU(e, cudaMemsetAsync(e->d_cls_rep, 0xFF, 4ull * T, s));
     CU(e, cudaMemsetAsync(e->d_cls_cnt, 0, 4ull * T, s));
     const uint32_t* n_ptr = &e->d_ctr->n_due;
-    st = chd_epoch_tick(e, EP_CLASS);
+    st = chd_epoch_tick(e, s, EP_CLASS);
     if (st != CHD_OK) return st;
     const unsigned blocks = blocks_for(n_due, 256);
     class_insert_kernel<<<blocks, 256, 0, s>>>(e->d_due, e->d_due_key, n_ptr, e->lim.max_due, e->d_cls_table, T - 1, e->d_cls_slot, e->d_cls_rep,
@@ -106,7 +106,7 @@ chd_status chd_adjacent_broadcast(chd_engine* e, const chd_broadcast_batch* b, u
         return CHD_OK;
     }
     cudaStream_t s = e->stream;
-    if (e->aux_stream) CU(e, cudaStreamSynchronize(e->aux_stream));  // an interest update in flight is rewriting the pairs / by-cell order
+    CU(e, cudaStreamSynchronize(e->aux_stream));  // an interest update in flight is rewriting the pairs / by-cell order
     if (n > e->bc_msg_cap) {
         const uint64_t c = std::max<uint64_t>(1024, (uint64_t)n + n / 2);
         chd_dfree(e, e->d_bc_in); chd_dfree(e, e->d_bc_cnt); chd_dfree(e, e->d_bc_off); chd_dfree(e, e->d_bc_msgoff); chd_dfree(e, e->site_bcast.desc);
@@ -133,7 +133,7 @@ chd_status chd_adjacent_broadcast(chd_engine* e, const chd_broadcast_batch* b, u
     const uint8_t* types = e->have_conn_type ? e->d_conn_type : nullptr;
     const unsigned blocks = blocks_for(9ull * n * 32, 256);
     {
-        chd_status st0 = chd_epoch_tick(e, EP_BCAST);
+        chd_status st0 = chd_epoch_tick(e, s, EP_BCAST);
         if (st0 != CHD_OK) return st0;
     }
     bcast_kernel<false><<<blocks, 256, 0, s>>>(e->g, bd, pb.off + S, P, pb, e->d_by_cell, e->d_conn, types, e->d_bc_cnt, nullptr, nullptr, 0,

@@ -7,8 +7,8 @@
 
 extern "C" {
 
-static chd_status upload_queries(chd_engine* e, const chd_query_batch* q, QueryDev* out, bool need_sub, chd_engine::QStage* stage = nullptr,
-                                 cudaStream_t on_stream = nullptr);
+static chd_status upload_queries(chd_engine* e, cudaStream_t s, const chd_query_batch* q, QueryDev* out, bool need_sub,
+                                 chd_engine::QStage* stage = nullptr);
 
 chd_status chd_prefetch_queries(chd_engine* e, const chd_query_batch* q) {
     if (!e || !q) return CHD_ERR_INVALID;
@@ -31,7 +31,7 @@ chd_status chd_prefetch_queries(chd_engine* e, const chd_query_batch* q) {
     }
     if (e->q_read_recorded[set]) CU(e, cudaStreamWaitEvent(e->up_stream, e->ev_q_read[set], 0));  // its previous batch has been consumed
     QueryDev d;
-    st = upload_queries(e, q, &d, true, &qs, e->up_stream);
+    st = upload_queries(e, e->up_stream, q, &d, true, &qs);
     if (st != CHD_OK) return st;
     CU(e, cudaEventRecord(e->ev_upload_q, e->up_stream));
     e->staged_qd = d;
@@ -126,9 +126,9 @@ chd_status chd_remove_subscribers(chd_engine* e, const uint32_t* slot, uint32_t 
     return CHD_OK;
 }
 
-// copies the batch into the engine's device SoA and returns the device view
-static chd_status upload_queries(chd_engine* e, const chd_query_batch* q, QueryDev* out, bool need_sub, chd_engine::QStage* stage,
-                                 cudaStream_t on_stream) {
+// copies the batch into the engine's device SoA (or a prefetch staging set) on `s` and returns the device view
+static chd_status upload_queries(chd_engine* e, cudaStream_t s, const chd_query_batch* q, QueryDev* out, bool need_sub,
+                                 chd_engine::QStage* stage) {
     if (!q) return CHD_ERR_INVALID;
     chd_engine::QStage& dq = stage ? *stage : e->dq;
     const uint32_t n = q->n;
@@ -138,13 +138,12 @@ static chd_status upload_queries(chd_engine* e, const chd_query_batch* q, QueryD
     }
     QueryDev d{};
     d.n = n;
-    cudaStream_t st = stage ? on_stream : e->stream;
 #define UP(field, T)                                                                                      \
     if (q->field) {                                                                                       \
         if (chd_is_device_ptr(e, q->field)) {                                                                 \
             d.field = q->field; /* device-resident batch: consumed in place */                            \
         } else {                                                                                          \
-            CU(e, cudaMemcpyAsync(dq.field, q->field, sizeof(T) * n, cudaMemcpyDefault, st));          \
+            CU(e, cudaMemcpyAsync(dq.field, q->field, sizeof(T) * n, cudaMemcpyDefault, s));           \
             d.field = dq.field;                                                                        \
         }                                                                                                 \
     }
@@ -168,22 +167,22 @@ static chd_status upload_queries(chd_engine* e, const chd_query_batch* q, QueryD
     if (q->spot_off) {
         // spot_off may live on the host or on the device; its last element sizes the spot arrays
         uint32_t total = 0;
-        CU(e, cudaMemcpyAsync(dq.spot_off, q->spot_off, sizeof(uint32_t) * ((uint64_t)n + 1), cudaMemcpyDefault, st));
-        CU(e, cudaMemcpyAsync(e->h_u32, dq.spot_off + n, 4, cudaMemcpyDeviceToHost, st));
-        CU(e, cudaStreamSynchronize(st));
+        CU(e, cudaMemcpyAsync(dq.spot_off, q->spot_off, sizeof(uint32_t) * ((uint64_t)n + 1), cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(e->h_u32, dq.spot_off + n, 4, cudaMemcpyDeviceToHost, s));
+        CU(e, cudaStreamSynchronize(s));
         total = *e->h_u32;
         if (total > e->lim.max_spots) {
             e->fail("%u spots > max_spots %u", total, e->lim.max_spots);
             return CHD_ERR_CAPACITY;
         }
         if (total && (!q->spot_x || !q->spot_z)) return CHD_ERR_INVALID;
-        CU(e, cudaMemcpyAsync(dq.spot_x, q->spot_x, sizeof(double) * total, cudaMemcpyDefault, st));
-        CU(e, cudaMemcpyAsync(dq.spot_z, q->spot_z, sizeof(double) * total, cudaMemcpyDefault, st));
-        if (q->spot_dist) CU(e, cudaMemcpyAsync(dq.spot_dist, q->spot_dist, sizeof(uint32_t) * total, cudaMemcpyDefault, st));
-        else CU(e, cudaMemsetAsync(dq.spot_dist, 0, sizeof(uint32_t) * total, st));
+        CU(e, cudaMemcpyAsync(dq.spot_x, q->spot_x, sizeof(double) * total, cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(dq.spot_z, q->spot_z, sizeof(double) * total, cudaMemcpyDefault, s));
+        if (q->spot_dist) CU(e, cudaMemcpyAsync(dq.spot_dist, q->spot_dist, sizeof(uint32_t) * total, cudaMemcpyDefault, s));
+        else CU(e, cudaMemsetAsync(dq.spot_dist, 0, sizeof(uint32_t) * total, s));
         d.spot_off = dq.spot_off; d.spot_x = dq.spot_x; d.spot_z = dq.spot_z; d.spot_dist = dq.spot_dist;
         if (!q->spot_ndist) {
-            CU(e, cudaMemsetAsync(dq.spot_ndist, 0, sizeof(uint32_t) * n, st));
+            CU(e, cudaMemsetAsync(dq.spot_ndist, 0, sizeof(uint32_t) * n, s));
             d.spot_ndist = dq.spot_ndist;
         }
     }
@@ -194,11 +193,11 @@ static chd_status upload_queries(chd_engine* e, const chd_query_batch* q, QueryD
 // Q1 + scan + Q2: fills bbox / window / side lists / status / qcount for the batch
 // bounding box -> window scratch -> lattice walk, one launch: fills bbox / window / side lists / status / qcount for the batch.
 // The caller has zeroed the window cursor (stage_begin_kernel / a memset on the stateless path).
-static chd_status run_query_kernel(chd_engine* e, const QueryDev& d, uint32_t* status) {
+static chd_status run_query_kernel(chd_engine* e, cudaStream_t s, const QueryDev& d, uint32_t* status) {
     const uint32_t n = d.n;
     if (n == 0) return CHD_OK;
-    query_kernel<<<blocks_for(n, 128), 128, 0, e->stream>>>(e->g, d, e->d_bbox, e->d_win_off, e->lim.max_window_cells, e->d_win_cursor, e->d_window,
-                                                            e->d_side_cell, e->d_side_dist, e->d_side_cnt, status, e->d_qcount, &e->d_ctr->overflow);
+    query_kernel<<<blocks_for(n, 128), 128, 0, s>>>(e->g, d, e->d_bbox, e->d_win_off, e->lim.max_window_cells, e->d_win_cursor, e->d_window,
+                                                    e->d_side_cell, e->d_side_dist, e->d_side_cnt, status, e->d_qcount, &e->d_ctr->overflow);
     KCHECK(e);
     return CHD_OK;
 }
@@ -208,9 +207,9 @@ chd_status chd_query_channel_ids(chd_engine* e, const chd_query_batch* q, uint32
     if (!e || !q) return CHD_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lk(e->mu);
     CU(e, cudaSetDevice(e->device));
-    if (e->aux_stream) CU(e, cudaStreamSynchronize(e->aux_stream));  // an in-flight interest update shares the query scratch
+    CU(e, cudaStreamSynchronize(e->aux_stream));  // an in-flight interest update shares the query scratch
     QueryDev d;
-    chd_status st = upload_queries(e, q, &d, false);
+    chd_status st = upload_queries(e, e->stream, q, &d, false);
     if (st != CHD_OK) return st;
     const uint32_t n = d.n;
     if (n == 0) {
@@ -222,11 +221,11 @@ chd_status chd_query_channel_ids(chd_engine* e, const chd_query_batch* q, uint32
         return CHD_OK;
     }
     // own status array: the statuses of the last interest batch (chd_get_query_status / chd_fetch_results) are not disturbed
-    chd_epoch_tick(e, EP_QUERY);
+    chd_epoch_tick(e, e->stream, EP_QUERY);
     bump_epoch_kernel<<<1, 1, 0, e->stream>>>(e->d_epoch + EP_QUERY);
     KCHECK(e);
     CU(e, cudaMemsetAsync(e->d_win_cursor, 0, 8, e->stream));
-    st = run_query_kernel(e, d, e->d_qstatus);
+    st = run_query_kernel(e, e->stream, d, e->d_qstatus);
     if (st != CHD_OK) return st;
     SCAN(e, exclusive_scan_1p<uint32_t, uint64_t>(e->d_qcount, e->d_qoff, n, e->site_qoff, e->stream));
     const uint64_t dev_cap = e->lim.max_pairs;
@@ -266,15 +265,14 @@ chd_status chd_query_channel_ids(chd_engine* e, const chd_query_batch* q, uint32
 
 // part 0: query -> new subscription pairs (everything emit needs); part 1: pairs grouped by cell + diff lists
 // (needed by the fan-out pass and the host only).  An event between the two lets emit start early.
-static chd_status interest_enqueue(chd_engine* e, const QueryDev& d, int part) {
+static chd_status interest_enqueue(chd_engine* e, cudaStream_t s, const QueryDev& d, int part) {
     const uint32_t n = d.n, S = e->n_slots;
-    cudaStream_t s = e->stream;
     chd_status st = CHD_OK;
     PairBuf& prev = e->pairs[e->cur];
     PairBuf& cur = e->pairs[e->cur ^ 1];
     const uint64_t P = e->lim.max_pairs;
     if (part == 0) {
-    st = run_query_kernel(e, d, e->d_status);
+    st = run_query_kernel(e, s, d, e->d_status);
     if (st != CHD_OK) return st;
     // sub == NULL is the identity batch (query i <-> subscriber slot i): no slot table needed
     const int32_t* slot_query = d.sub ? e->d_slot_query : nullptr;
@@ -309,17 +307,15 @@ static chd_status interest_enqueue(chd_engine* e, const QueryDev& d, int part) {
         const uint32_t nb = e->pc_blocks;
         uint32_t per_block = (uint32_t)((P + nb - 1) / nb);
         per_block = ((per_block + BUILD_TILE - 1) / BUILD_TILE) * BUILD_TILE;
-        cudaStream_t keep = e->stream;  // sort_pass launches on e->stream, which already is `s`
-        (void)keep;
         if (passes == 1) {
-            st = chd_sort_pass_any(e, e->d_pc_hist, e->site_pchist, cur.cell, nullptr, (uint32_t)P, cur.off + S, per_block, nb, 0, bits0, nullptr,
+            st = chd_sort_pass_any(e, s, e->d_pc_hist, e->site_pchist, cur.cell, nullptr, (uint32_t)P, cur.off + S, per_block, nb, 0, bits0, nullptr,
                                e->d_by_cell);
             if (st != CHD_OK) return st;
         } else {
-            st = chd_sort_pass_any(e, e->d_pc_hist, e->site_pchist, cur.cell, nullptr, (uint32_t)P, cur.off + S, per_block, nb, 0, bits0,
+            st = chd_sort_pass_any(e, s, e->d_pc_hist, e->site_pchist, cur.cell, nullptr, (uint32_t)P, cur.off + S, per_block, nb, 0, bits0,
                                e->d_pc_tmp_key, e->d_pc_tmp_val);
             if (st != CHD_OK) return st;
-            st = chd_sort_pass_any(e, e->d_pc_hist, e->site_pchist_b, e->d_pc_tmp_key, e->d_pc_tmp_val, (uint32_t)P, cur.off + S, per_block, nb, bits0,
+            st = chd_sort_pass_any(e, s, e->d_pc_hist, e->site_pchist_b, e->d_pc_tmp_key, e->d_pc_tmp_val, (uint32_t)P, cur.off + S, per_block, nb, bits0,
                                bits1, nullptr, e->d_by_cell);
             if (st != CHD_OK) return st;
         }
@@ -329,13 +325,14 @@ static chd_status interest_enqueue(chd_engine* e, const QueryDev& d, int part) {
 
 chd_status chd_update_interest(chd_engine* e, const chd_query_batch* q, int64_t now_ns) {
     if (!e) return CHD_ERR_INVALID;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
     CU(e, cudaSetDevice(e->device));
-    {
-        chd_status gs_ = chd_fetch_guard(e);
-        if (gs_ != CHD_OK) return gs_;
-    }
-    StageTimer timer(e, CHD_STAGE_INTEREST);
+    chd_status st = chd_fetch_guard(e, e->stream);
+    return st != CHD_OK ? st : chd_update_interest_on(e, e->stream, q, now_ns);
+}
+
+chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query_batch* q, int64_t now_ns) {
+    std::lock_guard<std::recursive_mutex> lk(e->mu);  // the query scratch
+    StageTimer timer(e, s, CHD_STAGE_INTEREST);
     QueryDev d;
     chd_status st;
     int pf_set = -1;  // prefetch staging set this batch lives in
@@ -352,18 +349,18 @@ chd_status chd_update_interest(chd_engine* e, const chd_query_batch* q, int64_t 
             return CHD_ERR_INVALID;
         }
         if (e->wait_q) {
-            CU(e, cudaStreamWaitEvent(e->stream, e->ev_upload_q, 0));
+            CU(e, cudaStreamWaitEvent(s, e->ev_upload_q, 0));
             e->wait_q = false;
         }
     } else {
-        st = upload_queries(e, q, &d, true);  // H2D / D2D copies into the engine's SoA: outside the graph
+        st = upload_queries(e, s, q, &d, true);  // H2D / D2D copies into the engine's SoA: outside the graph
         if (st != CHD_OK) return st;
     }
     const int gslot = e->cur + (pf_set == 1 ? 2 : 0);
     // (outside the replayed graphs: the tick time is a launch argument) tick time, new scan epoch, zeroed counters
     // n_query_errors / n_sub_new / n_unsub / n_kept and window cursor
-    chd_epoch_tick(e, EP_QUERY);
-    stage_begin_kernel<<<1, 1, 0, e->stream>>>(e->d_time, now_ns, e->d_epoch + EP_QUERY, &e->d_ctr->n_query_errors, 4, e->d_win_cursor);
+    chd_epoch_tick(e, s, EP_QUERY);
+    stage_begin_kernel<<<1, 1, 0, s>>>(e->d_time, now_ns, e->d_epoch + EP_QUERY, &e->d_ctr->n_query_errors, 4, e->d_win_cursor);
     KCHECK(e);
     // the graph bakes in which staging arrays are live, the batch size and the pair-buffer parity
     uint64_t key = mix_key(mix_key(mix_key(0x696e74ull, d.n), e->n_slots), (uint64_t)e->cur);
@@ -371,13 +368,13 @@ chd_status chd_update_interest(chd_engine* e, const chd_query_batch* q, int64_t 
     const void* baked[] = {d.sub, d.kind, d.sph_cx, d.sph_cz, d.sph_r, d.box_cx, d.box_cz, d.box_ex, d.box_ez, d.cone_cx, d.cone_cz,
                            d.cone_dx, d.cone_dz, d.cone_angle, d.cone_r, d.spot_off, d.spot_ndist, d.spot_x, d.spot_z, d.spot_dist};
     for (const void* p : baked) key = mix_key(key, (uint64_t)(uintptr_t)p);  // pointers are baked into the captured launches
-    st = run_stage(e, e->g_interest[gslot], key, [&]() { return interest_enqueue(e, d, 0); });
+    st = run_stage(e, s, e->g_interest[gslot], key, [&]() { return interest_enqueue(e, s, d, 0); });
     if (st != CHD_OK) return st;
-    CU(e, cudaEventRecord(e->ev_pairs, e->stream));  // the new pairs exist: emit may start (chd_tick waits on this)
-    st = run_stage(e, e->g_interest_b[gslot], mix_key(key, 0xb), [&]() { return interest_enqueue(e, d, 1); });
+    CU(e, cudaEventRecord(e->ev_pairs, s));  // the new pairs exist: emit may start (chd_tick waits on this)
+    st = run_stage(e, s, e->g_interest_b[gslot], mix_key(key, 0xb), [&]() { return interest_enqueue(e, s, d, 1); });
     if (st != CHD_OK) return st;
     if (pf_set >= 0) {  // the staging set may be refilled once these kernels have run
-        CU(e, cudaEventRecord(e->ev_q_read[pf_set], e->stream));
+        CU(e, cudaEventRecord(e->ev_q_read[pf_set], s));
         e->q_read_recorded[pf_set] = true;
     }
     e->cur ^= 1;

@@ -100,7 +100,7 @@ chd_status chd_assemble_payloads(chd_engine* e, uint32_t* out_n_classes, uint64_
     const RingDev ring = chd_ring_view(e);
     const PayloadIn in{(const unsigned long long*)P.d_entry_off, P.d_entry_bytes, (const unsigned long long*)P.d_full_off, P.d_full_bytes, P.d_url, P.url_len,
                        P.msg_type};
-    st = chd_epoch_tick(e, EP_PAYLOAD);
+    st = chd_epoch_tick(e, s, EP_PAYLOAD);
     if (st != CHD_OK) return st;
     payload_size_kernel<<<blocks_for(n_classes, 128), 128, 0, s>>>(n_classes, e->d_cls_out_rep, e->d_due, e->d_due_key, ring, e->d_conn, in, P.d_cls_len,
                                                                   e->d_epoch + EP_PAYLOAD);
@@ -172,7 +172,7 @@ chd_status chd_frame_packets(chd_engine* e, const uint8_t* compression, uint64_t
     CU(e, cudaMemsetAsync(P.d_fc_cursor, 0, 4ull * (S + 1), s));
     CU(e, cudaMemsetAsync(P.d_ndrop, 0, 4, s));
     if (compression) CU(e, cudaMemcpyAsync(P.d_comp, compression, S, cudaMemcpyDefault, s));
-    st = chd_epoch_tick(e, EP_PAYLOAD);
+    st = chd_epoch_tick(e, s, EP_PAYLOAD);
     if (st != CHD_OK) return st;
     frame_count_kernel<<<blocks_for(n_due ? n_due : 1, 256), 256, 0, s>>>(e->d_due, n_due, S, P.d_fc_cnt, e->d_epoch + EP_PAYLOAD);
     KCHECK(e);

@@ -189,11 +189,11 @@ chd_status chd_fetch_results(chd_engine* e, const chd_result_buffers* b, chd_tic
     chd_status st;
     cudaStream_t s = e->stream;
     cudaStream_t main_stream = e->stream;
-    const bool early = e->early_ready && e->dl_stream;
+    const bool early = e->early_ready;
     // error exits: no copy into the caller's buffers may still be in flight when this returns
     auto drain = [&](chd_status r) {
-        if (e->dl_stream) cudaStreamSynchronize(e->dl_stream);
-        if (e->dl_stream_b) cudaStreamSynchronize(e->dl_stream_b);
+        cudaStreamSynchronize(e->dl_stream);
+        cudaStreamSynchronize(e->dl_stream_b);
         cudaStreamSynchronize(main_stream);
         return r;
     };
@@ -288,7 +288,7 @@ chd_status chd_fetch_results(chd_engine* e, const chd_result_buffers* b, chd_tic
 
 chd_status chd_fetch_results_async(chd_engine* e, const chd_result_buffers* b, void* pinned_header) {
     if (!e || !b || !pinned_header) return CHD_ERR_INVALID;
-    if (!e->early_ready || !e->dl_stream) {
+    if (!e->early_ready) {
         e->fail("chd_fetch_results_async needs a two-stream tick (chd_tick with emit, or chd_begin_interest + chd_tick) just before it");
         return CHD_ERR_STATE;
     }

@@ -72,18 +72,18 @@ chd_status chd_set_slab(chd_engine* e, uint32_t col_lo, uint32_t col_hi, uint32_
 chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_records, uint32_t* out_count) {
     if (!e || !d_records) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    cudaStream_t s = e->stream;
     {
-        chd_status gs_ = chd_fetch_guard(e);
+        chd_status gs_ = chd_fetch_guard(e, s);
         if (gs_ != CHD_OK) return gs_;
     }
-    cudaStream_t s = e->stream;
     const uint32_t n = e->n_own;
     // inside chd_tick_sharded with the peer exchange the records go straight into the peers' windows afterwards: no padding needed
     const bool to_peers = e->peer_push && d_records == e->d_rec_local;
     auto enqueue = [&]() -> chd_status {
         const bool bump_in_assign = !e->assigned && n;
         if (bump_in_assign) e->assign_bump = e->d_epoch + EP_BORDER;
-        chd_status st = chd_assign_cells_impl(e);
+        chd_status st = chd_assign_cells_impl(e, s);
         if (st != CHD_OK) return st;
         if (!bump_in_assign) {
             bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_BORDER);
@@ -103,7 +103,7 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
         }
         return CHD_OK;
     };
-    chd_status st = chd_epoch_tick(e, EP_BORDER);
+    chd_status st = chd_epoch_tick(e, s, EP_BORDER);
     if (st != CHD_OK) return st;
     if (!e->assigned) {
         // replayable: cell assignment + border selection of one tick (two variants: the key buffers ping-pong)
@@ -114,7 +114,7 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
         key = mix_key(mix_key(key, (uint64_t)(uintptr_t)d_records), cap_records);
         key = mix_key(mix_key(mix_key(key, e->g.col_lo), e->g.col_hi), e->g.halo);
         key = mix_key(key, to_peers ? 1 : 0);
-        st = run_stage(e, e->g_export[slot + (to_peers ? 4 : 0)], key, enqueue);
+        st = run_stage(e, s, e->g_export[slot + (to_peers ? 4 : 0)], key, enqueue);
         if (st == CHD_OK && !e->assigned) {  // replayed graph: mirror the host-side bookkeeping of chd_assign_cells
             if (e->have_prev_key) {
                 uint32_t* t = e->d_key;
@@ -125,7 +125,7 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
             e->n_halo = 0;
             e->assigned = true;
         }
-        if (st == CHD_OK) st = chd_note_pos_read(e);
+        if (st == CHD_OK) st = chd_note_pos_read(e, s);
     } else {
         st = enqueue();
     }
@@ -158,7 +158,7 @@ chd_status chd_import_halo(chd_engine* e, const uint32_t* d_records, uint32_t n_
         return CHD_ERR_CAPACITY;
     }
     {
-        chd_status st0 = chd_epoch_tick(e, EP_BORDER);
+        chd_status st0 = chd_epoch_tick(e, s, EP_BORDER);
         if (st0 != CHD_OK) return st0;
         const int slot = e->d_key == e->d_key_a ? 0 : 1;  // the halo keys are appended to the current key buffer
         // peer exchange: the records sit in this tick's buffer of the own window, the live counts come from the flags
@@ -169,7 +169,7 @@ chd_status chd_import_halo(chd_engine* e, const uint32_t* d_records, uint32_t n_
         key = mix_key(mix_key(mix_key(key, (uint64_t)(uintptr_t)d_records), e->n_own), (uint64_t)(uintptr_t)e->d_key);
         key = mix_key(mix_key(mix_key(key, e->g.col_lo), e->g.col_hi), e->g.halo);
         key = mix_key(key, from_peers ? 1 : 0);
-        chd_status st = run_stage(e, e->g_import[slot + 2 * parity], key, [&]() -> chd_status {
+        chd_status st = run_stage(e, s, e->g_import[slot + 2 * parity], key, [&]() -> chd_status {
             const RecView rv{d_records, e->rec_per_rank ? e->rec_per_rank : (n_records ? n_records : 1u),
                              e->rec_per_rank ? e->rec_stride_words : 2ull * (n_records ? n_records : 1u)};
             if (from_peers) {  // (the push kernel of this tick has bumped the compaction site's epoch)
@@ -351,7 +351,7 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
         return CHD_ERR_STATE;
     }
     {
-        chd_status gs_ = chd_fetch_guard(e);
+        chd_status gs_ = chd_fetch_guard(e, e->stream);
         if (gs_ != CHD_OK) return gs_;
     }
     chd_status st;
@@ -366,7 +366,7 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
     if (e->mig_subs && !e->mig_packed) CU(e, cudaMemsetAsync(e->d_rec_local + 2ull * cap, 0, 16, e->stream));  // empty blob header
     e->mig_packed = false;
     {
-        StageTimer tm(e, CHD_STAGE_EXPORT);  // (with the peer exchange: assignment + border selection + the push into the peers' windows)
+        StageTimer tm(e, e->stream, CHD_STAGE_EXPORT);  // (with the peer exchange: assignment + border selection + the push into the peers' windows)
         st = chd_export_border(e, e->d_rec_local, cap, nullptr);
     }
     if (st != CHD_OK) return st;
@@ -376,14 +376,14 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
         gathered = e->d_peer_win + (e->xchg_seq & 1ull) * (uint64_t)e->comm_world * e->rec_stride_words;
     } else {
         NcclApi* api = nccl_api();
-        StageTimer tm(e, CHD_STAGE_EXCHANGE);
+        StageTimer tm(e, e->stream, CHD_STAGE_EXCHANGE);
         NC(e, api, api->AllGather(e->d_rec_local, e->d_rec_all, e->rec_stride_words, ncclUint32, (ncclComm_t)e->comm, e->stream));
         e->n_collectives++;
     }
     {
         // the halo import comes first: with the peer exchange its first kernel is the one that waits for the peers' records, and the
         // immigrants' state (read by the interest update below) sits in the same window
-        StageTimer tm(e, CHD_STAGE_IMPORT);
+        StageTimer tm(e, e->stream, CHD_STAGE_IMPORT);
         st = chd_import_halo(e, gathered, cap * (uint32_t)e->comm_world, (uint32_t)e->comm_rank * cap, cap);
     }
     if (st != CHD_OK) return st;

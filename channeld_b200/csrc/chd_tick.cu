@@ -20,18 +20,17 @@ static bool emit_uses_cta_tiles(const chd_engine* e) {
     return (uint64_t)e->n_own / (own_cells ? own_cells : 1) >= (uint64_t)EMIT_TILE / 2 && n_build * 16ull <= (uint64_t)e->l2_bytes / 2;
 }
 
-// emit preparation on e->stream: per-pair output offsets (scan), per-tile first pairs / descriptors, per-subscriber offsets, V
-static chd_status emit_prep_enqueue(chd_engine* e, bool cta_tiles) {
-    cudaStream_t s = e->stream;
+// emit preparation on `s`: per-pair output offsets (scan), per-tile first pairs / descriptors, per-subscriber offsets, V
+static chd_status emit_prep_enqueue(chd_engine* e, cudaStream_t s, bool cta_tiles) {
     PairBuf& pb = e->pairs[e->cur];
     const uint32_t S = e->n_slots;
     const uint64_t P = e->lim.max_pairs;
     const unsigned grid = (unsigned)e->sm_count * 8;
     const uint32_t tile = cta_tiles ? (uint32_t)EMIT_TILE : (uint32_t)EMIT_WARP_TILE;
     const uint64_t key = mix_key(mix_key(mix_key(mix_key(0x656d6974ull, S), (uint64_t)e->cur), cta_tiles), (uint64_t)(uintptr_t)s);
-    chd_status st = chd_epoch_tick(e, EP_EMIT);
+    chd_status st = chd_epoch_tick(e, s, EP_EMIT);
     if (st != CHD_OK) return st;
-    return run_stage(e, e->g_emit_prep[e->cur], key, [&]() -> chd_status {
+    return run_stage(e, s, e->g_emit_prep[e->cur], key, [&]() -> chd_status {
         // per-pair visible counts are computed by the scan itself; the partition pass opens the next epoch
         SCAN(e, exclusive_scan_fn<PairVcountIn, uint64_t>(PairVcountIn{pb.cell, e->d_cell_start}, e->d_voff, P, e->site_voff, s, pb.off + S));
         emit_partition_kernel<<<grid, 256, 0, s>>>(pb.off + S, P, e->d_voff, pb.cell, e->d_cell_start, e->d_first_pair, cta_tiles ? e->d_tile_desc : nullptr,
@@ -42,12 +41,11 @@ static chd_status emit_prep_enqueue(chd_engine* e, bool cta_tiles) {
     });
 }
 
-static chd_status emit_kernel_enqueue(chd_engine* e, bool cta_tiles) {
-    cudaStream_t s = e->stream;
+static chd_status emit_kernel_enqueue(chd_engine* e, cudaStream_t s, bool cta_tiles) {
     PairBuf& pb = e->pairs[e->cur];
     const uint32_t S = e->n_slots;
     const uint64_t P = e->lim.max_pairs;
-    StageTimer kt(e, CHD_STAGE_EMIT_KERNEL);
+    StageTimer kt(e, s, CHD_STAGE_EMIT_KERNEL);
     if (cta_tiles) {
         // One CTA per tile, dispatched by the hardware block scheduler.  The tile count lives on the device; the grid is
         // sized from the last visible count the host has seen (+3 %: the kernel loops if that was too few, surplus CTAs exit
@@ -70,58 +68,36 @@ static chd_status emit_kernel_enqueue(chd_engine* e, bool cta_tiles) {
     return CHD_OK;
 }
 
+// The emit: the preparation (ending with ev_prep_done), then the copy kernel on `s`, after `kernel_ev` if one is given.  Without
+// `pairs_ev` the preparation runs on `s` too.  In a two-stream tick it needs only the new pairs (`pairs_ev`, second stream) and
+// the cell CSR OFFSETS (ev_counts: recorded between the two halves of a single-pass build), not the sorted entity array — it runs
+// on prep_stream next to the build's scatter; the copy kernel follows on `s` when both are done.
+static chd_status emit_enqueue(chd_engine* e, cudaStream_t s, cudaEvent_t pairs_ev, cudaEvent_t kernel_ev) {
+    if (!e->built) {
+        e->fail("emit before any chd_build");
+        return CHD_ERR_STATE;
+    }
+    const bool cta_tiles = emit_uses_cta_tiles(e);
+    StageTimer timer(e, s, CHD_STAGE_EMIT);
+    const cudaStream_t ps = pairs_ev ? e->prep_stream : s;
+    if (pairs_ev) {
+        CU(e, cudaStreamWaitEvent(ps, e->ev_fork, 0));    // the previous tick's copy kernel (it reads what the preparation rewrites)
+        CU(e, cudaStreamWaitEvent(ps, e->ev_counts, 0));
+        CU(e, cudaStreamWaitEvent(ps, pairs_ev, 0));
+    }
+    chd_status st = emit_prep_enqueue(e, ps, cta_tiles);
+    if (st != CHD_OK) return st;
+    CU(e, cudaEventRecord(e->ev_prep_done, ps));  // visible offsets + counters are final; only the expanded list is still to come
+    if (pairs_ev) CU(e, cudaStreamWaitEvent(s, e->ev_prep_done, 0));
+    if (kernel_ev) CU(e, cudaStreamWaitEvent(s, kernel_ev, 0));
+    return emit_kernel_enqueue(e, s, cta_tiles);
+}
+
 chd_status chd_emit_visible(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
-    if (!e->built) {
-        e->fail("chd_emit_visible before chd_build");
-        return CHD_ERR_STATE;
-    }
-    {
-        chd_status gs_ = chd_fetch_guard(e);
-        if (gs_ != CHD_OK) return gs_;
-    }
-    StageTimer timer(e, CHD_STAGE_EMIT);
-    const bool cta_tiles = emit_uses_cta_tiles(e);
-    chd_status st = emit_prep_enqueue(e, cta_tiles);
-    if (st != CHD_OK) return st;
-    if (e->wait_before_emit_kernel) {
-        CU(e, cudaStreamWaitEvent(e->stream, e->wait_before_emit_kernel, 0));
-        e->wait_before_emit_kernel = nullptr;
-    }
-    CU(e, cudaEventRecord(e->ev_prep_done, e->stream));  // visible offsets + counters are final; only the expanded list is still to come
-    return emit_kernel_enqueue(e, cta_tiles);
-}
-
-// The emit of a two-stream tick: the preparation needs the new pairs (`pairs_ev`, second stream) and the cell CSR OFFSETS
-// (ev_counts: recorded between the two halves of a single-pass build), not the sorted entity array — it runs on its own stream
-// next to the build's scatter; the copy kernel follows on the main stream when both are done.
-static chd_status emit_overlapped(chd_engine* e, cudaEvent_t pairs_ev) {
-    if (!e->built) {
-        e->fail("chd_tick: emit before any build");
-        return CHD_ERR_STATE;
-    }
-    const bool cta_tiles = emit_uses_cta_tiles(e);
-    cudaStream_t main_stream = e->stream, ps = e->prep_stream;
-    CU(e, cudaStreamWaitEvent(ps, e->ev_fork, 0));    // the previous tick's copy kernel (it reads what the preparation rewrites)
-    CU(e, cudaStreamWaitEvent(ps, e->ev_counts, 0));
-    CU(e, cudaStreamWaitEvent(ps, pairs_ev, 0));
-    chd_status st;
-    {
-        std::lock_guard<std::recursive_mutex> redirect(e->mu);  // `stream` is redirected while the preparation is enqueued
-        e->stream = ps;
-        st = emit_prep_enqueue(e, cta_tiles);
-        e->stream = main_stream;
-    }
-    if (st != CHD_OK) return st;
-    CU(e, cudaEventRecord(e->ev_prep_done, ps));
-    StageTimer timer(e, CHD_STAGE_EMIT);
-    CU(e, cudaStreamWaitEvent(main_stream, e->ev_prep_done, 0));
-    if (e->wait_before_emit_kernel) {
-        CU(e, cudaStreamWaitEvent(main_stream, e->wait_before_emit_kernel, 0));
-        e->wait_before_emit_kernel = nullptr;
-    }
-    return emit_kernel_enqueue(e, cta_tiles);
+    chd_status st = chd_fetch_guard(e, e->stream);
+    return st != CHD_OK ? st : emit_enqueue(e, e->stream, nullptr, nullptr);
 }
 
 chd_status chd_set_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
@@ -289,23 +265,16 @@ RingDev chd_ring_view(const chd_engine* e) {
                    e->ring_index_p ? e->ring_index_p : e->d_ring_index, e->have_ch_msg_index ? e->ch_msg_index_p : nullptr, e->d_ring_total, start};
 }
 
-chd_status chd_fanout_tick(chd_engine* e, int64_t t_ns) {
-    if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    cudaStream_t s = e->stream;
+static chd_status fanout_enqueue(chd_engine* e, cudaStream_t s, int64_t t_ns) {
     PairBuf& pb = e->pairs[e->cur];
     const uint32_t S = e->n_slots;
     const uint64_t P = e->lim.max_pairs;
-    {
-        chd_status gs_ = chd_fetch_guard(e);
-        if (gs_ != CHD_OK) return gs_;
-    }
-    StageTimer timer(e, CHD_STAGE_FANOUT);
+    StageTimer timer(e, s, CHD_STAGE_FANOUT);
     if (e->wait_rings) {  // rings handed over by chd_adopt_prefetched: ordered after their upload
         CU(e, cudaStreamWaitEvent(s, e->ev_upload_rings, 0));
         e->wait_rings = false;
     }
-    chd_epoch_tick(e, EP_FANOUT);
+    chd_epoch_tick(e, s, EP_FANOUT);
     stage_begin_kernel<<<1, 1, 0, s>>>(e->d_time + 1, t_ns, e->d_epoch + EP_FANOUT, &e->d_ctr->n_due, 1, nullptr);
     KCHECK(e);
     const RingDev ring = chd_ring_view(e);
@@ -314,7 +283,7 @@ chd_status chd_fanout_tick(chd_engine* e, int64_t t_ns) {
     for (const void* p : {(const void*)ring.off, (const void*)ring.end, (const void*)ring.arrival, (const void*)ring.sender, (const void*)ring.index,
                           (const void*)ring.channel_msg_index, (const void*)ring.start})
         key = mix_key(key, (uint64_t)(uintptr_t)p);  // pointers are baked into the captured launch
-    chd_status st = run_stage(e, e->g_fanout[e->cur + (e->ring_set == 1 ? 2 : 0)], key, [&]() -> chd_status {
+    chd_status st = run_stage(e, s, e->g_fanout[e->cur + (e->ring_set == 1 ? 2 : 0)], key, [&]() -> chd_status {
         const unsigned blocks = (unsigned)std::min<uint64_t>((P + 127) / 128, (uint64_t)e->sm_count * 16);
         fanout_kernel<<<blocks ? blocks : 1, 128, 0, s>>>(pb.off + S, P, pb, e->d_conn, ring, e->d_time + 1, e->g.id_start, e->d_by_cell, e->d_due,
                                                           e->d_due_key, e->lim.max_due, e->d_ctr);
@@ -326,6 +295,13 @@ chd_status chd_fanout_tick(chd_engine* e, int64_t t_ns) {
         e->ring_read_recorded[e->ring_set] = true;
     }
     return st;
+}
+
+chd_status chd_fanout_tick(chd_engine* e, int64_t t_ns) {
+    if (!e) return CHD_ERR_INVALID;
+    CU(e, cudaSetDevice(e->device));
+    chd_status st = chd_fetch_guard(e, e->stream);
+    return st != CHD_OK ? st : fanout_enqueue(e, e->stream, t_ns);
 }
 
 chd_status chd_prefetch_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
@@ -435,6 +411,23 @@ chd_status chd_decode_summary(chd_engine* e, chd_tick_summary* out) {
     return CHD_OK;
 }
 
+// Forks the interest / fan-out chain off `s` onto aux_stream: the interest update (if `interest`; q == NULL = the adopted batch),
+// ev_interest, the fan-out pass (if `fanout`), ev_join.
+static chd_status aux_chain_enqueue(chd_engine* e, cudaStream_t s, const chd_query_batch* q, bool interest, int64_t t_ns, bool fanout) {
+    const cudaStream_t aux = e->aux_stream;
+    CU(e, cudaEventRecord(e->ev_fork, s));
+    CU(e, cudaStreamWaitEvent(aux, e->ev_fork, 0));
+    chd_status st = interest ? chd_update_interest_on(e, aux, q, t_ns) : CHD_OK;
+    if (st != CHD_OK) return st;
+    CU(e, cudaEventRecord(e->ev_interest, aux));
+    if (fanout) {
+        st = fanout_enqueue(e, aux, t_ns);
+        if (st != CHD_OK) return st;
+    }
+    CU(e, cudaEventRecord(e->ev_join, aux));
+    return CHD_OK;
+}
+
 chd_status chd_begin_interest(chd_engine* e, const chd_query_batch* q, int64_t t_ns, int with_fanout) {
     if (!e) return CHD_ERR_INVALID;
     if (!q && !e->have_adopted_q) {
@@ -446,145 +439,99 @@ chd_status chd_begin_interest(chd_engine* e, const chd_query_batch* q, int64_t t
         return CHD_ERR_STATE;
     }
     CU(e, cudaSetDevice(e->device));
-    {
-        chd_status gs = chd_fetch_guard(e);
-        if (gs != CHD_OK) return gs;
-    }
-    if (!e->aux_stream) {  // no second stream: run in place
-        chd_status st = chd_update_interest(e, q, t_ns);
-        if (st == CHD_OK && with_fanout) st = chd_fanout_tick(e, t_ns);
-        return st;
-    }
-    std::lock_guard<std::recursive_mutex> lk(e->mu);  // `stream` is redirected below
-    cudaStream_t main_stream = e->stream;
-    CU(e, cudaEventRecord(e->ev_fork, main_stream));
-    CU(e, cudaStreamWaitEvent(e->aux_stream, e->ev_fork, 0));
-    e->stream = e->aux_stream;
-    chd_status st = chd_update_interest(e, q, t_ns);
-    if (st == CHD_OK && cudaEventRecord(e->ev_interest, e->aux_stream) != cudaSuccess) st = CHD_ERR_CUDA;
-    if (st == CHD_OK && with_fanout) st = chd_fanout_tick(e, t_ns);
-    if (st == CHD_OK && cudaEventRecord(e->ev_join, e->aux_stream) != cudaSuccess) st = CHD_ERR_CUDA;
-    e->stream = main_stream;
+    chd_status st = chd_fetch_guard(e, e->stream);
+    if (st == CHD_OK) st = aux_chain_enqueue(e, e->stream, q, true, t_ns, with_fanout != 0);
     if (st != CHD_OK) return st;
     e->interest_pending = true;
     e->pending_fanout = with_fanout != 0;
     return CHD_OK;
 }
 
-static chd_status chd_tick_impl(chd_engine* e, const chd_query_batch* q, int64_t t_ns, uint32_t flags, chd_tick_summary* out);
+// An asynchronous read-back of the previous tick may still be copying out of the arrays this tick rewrites: order this tick's
+// work after it (device-side wait on `s`; in steady state the copies finished long before).
+chd_status chd_fetch_guard(chd_engine* e, cudaStream_t s) {
+    if (!e->fetch_guard) return CHD_OK;
+    const int fi = (int)((e->fetch_issued - 1) & 1);  // the latest fetch (an older one completed before it: same streams)
+    CU(e, cudaStreamWaitEvent(s, e->ev_fetch_a[fi], 0));
+    CU(e, cudaStreamWaitEvent(s, e->ev_fetch_b[fi], 0));
+    e->fetch_guard = false;
+    return CHD_OK;
+}
+
+// Dependency graph of a tick:   build ----------------+--> emit
+//                               interest --> fan-out  |      (emit needs the cell CSR and the new pairs)
+// The build / emit chain (HBM-bound) runs on the main stream `s`, the interest / fan-out chain (latency-bound, disjoint state)
+// on aux_stream, started here or earlier by chd_begin_interest; the streams are joined before the summary.  A tick with nothing
+// to overlap runs its stages one after the other on `s`.
+static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_batch* q, int64_t t_ns, uint32_t flags) {
+    CU(e, cudaSetDevice(e->device));
+    chd_status st = chd_fetch_guard(e, s);
+    if (st != CHD_OK) return st;
+    const bool need_build = (flags & CHD_TICK_BUILD) && (e->entities_dirty || !e->built);
+    const bool do_emit = flags & CHD_TICK_EMIT;
+    const bool do_fanout = flags & CHD_TICK_FANOUT;
+    const bool started = e->interest_pending;  // the aux chain of this tick was started by chd_begin_interest
+    e->early_ready = false;
+    e->build_done_recorded = false;
+    if (started && q) {
+        e->fail("chd_tick: a query batch was given while chd_begin_interest is pending");
+        return CHD_ERR_STATE;
+    }
+    if (!started && !((q || do_fanout) && (need_build || do_emit))) {
+        if (need_build) {
+            st = chd_build_on(e, s);
+            if (st != CHD_OK) return st;
+        }
+        if (q) {
+            st = chd_update_interest_on(e, s, q, t_ns);
+            if (st != CHD_OK) return st;
+        }
+        if (do_emit) {
+            st = emit_enqueue(e, s, nullptr, nullptr);
+            if (st != CHD_OK) return st;
+        }
+        if (do_fanout) {
+            st = fanout_enqueue(e, s, t_ns);
+            if (st != CHD_OK) return st;
+        }
+        return CHD_OK;
+    }
+    if (!started) {
+        st = aux_chain_enqueue(e, s, q, q != nullptr, t_ns, do_fanout);
+        if (st != CHD_OK) return st;
+    }
+    const bool fanout_done = started ? e->pending_fanout : do_fanout;
+    e->interest_pending = false;
+    if (need_build) {
+        st = chd_build_on(e, s);
+        if (st != CHD_OK) return st;
+        CU(e, cudaEventRecord(e->ev_build_done, s));
+        e->build_done_recorded = true;
+    }
+    if (do_emit) {
+        // the preparation waits for the new pairs (for the fork when this tick updates no interest); CHD_TICK_EARLY_RESULTS: the
+        // copy kernel starts after the whole aux chain, so every host-facing result is final while it is still streaming
+        st = emit_enqueue(e, s, (started || q) ? e->ev_pairs : e->ev_interest, (flags & CHD_TICK_EARLY_RESULTS) ? e->ev_join : nullptr);
+        if (st != CHD_OK) return st;
+    }
+    CU(e, cudaStreamWaitEvent(s, e->ev_join, 0));
+    if (do_fanout && !fanout_done) {
+        st = fanout_enqueue(e, s, t_ns);
+        if (st != CHD_OK) return st;
+    } else {
+        e->early_ready = do_emit;  // everything but the expanded list is final at ev_join + ev_prep_done
+    }
+    return CHD_OK;
+}
 
 chd_status chd_tick(chd_engine* e, const chd_query_batch* q, int64_t t_ns, uint32_t flags, chd_tick_summary* out) {
     if (!e) return CHD_ERR_INVALID;
     chd_status st;
     {
-        StageTimer whole(e, CHD_STAGE_TICK);  // main-stream span of the tick (without the summary read-back)
-        st = chd_tick_impl(e, q, t_ns, flags, nullptr);
+        StageTimer whole(e, e->stream, CHD_STAGE_TICK);  // main-stream span of the tick (without the summary read-back)
+        st = tick_enqueue(e, e->stream, q, t_ns, flags);
     }
     if (st != CHD_OK) return st;
-    if (out) return chd_summary(e, out);
-    return CHD_OK;
-}
-
-// An asynchronous read-back of the previous tick may still be copying out of the arrays this tick rewrites: order this tick's
-// work after it (device-side wait; in steady state the copies finished long before).
-chd_status chd_fetch_guard(chd_engine* e) {
-    if (!e->fetch_guard) return CHD_OK;
-    const int fi = (int)((e->fetch_issued - 1) & 1);  // the latest fetch (an older one completed before it: same streams)
-    CU(e, cudaStreamWaitEvent(e->stream, e->ev_fetch_a[fi], 0));
-    CU(e, cudaStreamWaitEvent(e->stream, e->ev_fetch_b[fi], 0));
-    e->fetch_guard = false;
-    return CHD_OK;
-}
-
-static chd_status chd_tick_impl(chd_engine* e, const chd_query_batch* q, int64_t t_ns, uint32_t flags, chd_tick_summary* out) {
-    chd_status st = chd_fetch_guard(e);
-    if (st != CHD_OK) return st;
-    const bool need_build = (flags & CHD_TICK_BUILD) && (e->entities_dirty || !e->built);
-    const bool do_emit = flags & CHD_TICK_EMIT;
-    bool do_fanout = flags & CHD_TICK_FANOUT;
-    e->early_ready = false;
-    e->build_done_recorded = false;
-    e->early_results_tick = (flags & CHD_TICK_EARLY_RESULTS) != 0;
-    if (e->interest_pending) {
-        // interest (+ fan-out) of this tick were started early with chd_begin_interest and are running on aux_stream
-        if (q) {
-            e->fail("chd_tick: a query batch was given while chd_begin_interest is pending");
-            return CHD_ERR_STATE;
-        }
-        cudaStream_t main_stream = e->stream;
-        e->interest_pending = false;
-        if (need_build) {
-            st = chd_build(e);
-            if (st != CHD_OK) return st;
-            CU(e, cudaEventRecord(e->ev_build_done, main_stream));
-            e->build_done_recorded = true;
-        }
-        if (do_emit) {
-            if (e->early_results_tick) e->wait_before_emit_kernel = e->ev_join;
-            st = emit_overlapped(e, e->ev_pairs);
-            if (st != CHD_OK) return st;
-        }
-        CU(e, cudaStreamWaitEvent(main_stream, e->ev_join, 0));
-        if (do_fanout && !e->pending_fanout) {
-            st = chd_fanout_tick(e, t_ns);
-            if (st != CHD_OK) return st;
-        } else {
-            e->early_ready = do_emit;  // everything but the expanded list is final at ev_join + ev_prep_done
-        }
-        if (out) return chd_summary(e, out);
-        return CHD_OK;
-    }
-    if (e->overlap_fanout && e->aux_stream && (q || do_fanout) && (need_build || do_emit)) {
-        // Dependency graph of a tick:   build ----------------+--> emit
-        //                               interest --> fan-out  |      (emit needs the cell CSR and the new pairs)
-        // The build / emit chain (HBM-bound) runs on the main stream, the interest / fan-out chain
-        // (latency-bound, disjoint state) on aux_stream; they are joined before the summary.
-        cudaStream_t main_stream = e->stream;
-        CU(e, cudaEventRecord(e->ev_fork, main_stream));
-        CU(e, cudaStreamWaitEvent(e->aux_stream, e->ev_fork, 0));
-        std::unique_lock<std::recursive_mutex> redirect(e->mu);  // `stream` is redirected until it is restored below
-        e->stream = e->aux_stream;
-        st = q ? chd_update_interest(e, q, t_ns) : CHD_OK;
-        if (st == CHD_OK) {
-            cudaError_t r = cudaEventRecord(e->ev_interest, e->aux_stream);
-            if (r != cudaSuccess) st = CHD_ERR_CUDA;
-        }
-        if (st == CHD_OK && do_fanout) st = chd_fanout_tick(e, t_ns);
-        e->stream = main_stream;
-        redirect.unlock();
-        if (st != CHD_OK) return st;
-        CU(e, cudaEventRecord(e->ev_join, e->aux_stream));
-        if (need_build) {
-            st = chd_build(e);
-            if (st != CHD_OK) return st;
-            CU(e, cudaEventRecord(e->ev_build_done, main_stream));
-            e->build_done_recorded = true;
-        }
-        if (do_emit) {
-            if (e->early_results_tick) e->wait_before_emit_kernel = e->ev_join;
-            st = emit_overlapped(e, !q ? e->ev_interest : e->ev_pairs);
-            if (st != CHD_OK) return st;
-        }
-        CU(e, cudaStreamWaitEvent(main_stream, e->ev_join, 0));
-        e->early_ready = do_emit;
-    } else {
-        if (need_build) {
-            st = chd_build(e);
-            if (st != CHD_OK) return st;
-        }
-        if (q) {
-            st = chd_update_interest(e, q, t_ns);
-            if (st != CHD_OK) return st;
-        }
-        if (do_emit) {
-            st = chd_emit_visible(e);
-            if (st != CHD_OK) return st;
-        }
-        if (do_fanout) {
-            st = chd_fanout_tick(e, t_ns);
-            if (st != CHD_OK) return st;
-        }
-    }
     if (out) return chd_summary(e, out);
     return CHD_OK;
 }

@@ -290,9 +290,12 @@ enum { CHD_OVF_PAIRS = 1, CHD_OVF_WINDOW = 2, CHD_OVF_VISIBLE = 4, CHD_OVF_DUE =
 /* Synchronises the stream and returns the counters.  CHD_ERR_CAPACITY if any overflow bit is set. */
 chd_status chd_summary(chd_engine* e, chd_tick_summary* out);
 
-/* ---- Channel.Tick for all spatial channels (channel.go:358-387), batched: build (if entities changed) ->
- * update_interest(q) (if q != NULL) -> emit_visible (flags & CHD_TICK_EMIT) -> fanout_tick(t_ns)
- * (flags & CHD_TICK_FANOUT) -> summary.  One stream, no intermediate host sync. */
+/* ---- Channel.Tick for all spatial channels (channel.go:358-387), batched: build (if entities changed),
+ * update_interest(q) (if q != NULL), emit_visible (flags & CHD_TICK_EMIT) and fanout_tick(t_ns) (flags & CHD_TICK_FANOUT),
+ * with the results of those four calls in that order, then the summary.  No intermediate host sync.  Two streams: when
+ * there is something to overlap, the interest update and the fan-out pass run on the engine's second stream next to build
+ * + emit on the engine stream (the emit preparation waits only for the new pairs and the cell counts), and the engine
+ * stream waits for the second one before the summary; otherwise the stages run one after the other on the engine stream. */
 enum {
     CHD_TICK_BUILD = 1, CHD_TICK_EMIT = 2, CHD_TICK_FANOUT = 4, CHD_TICK_ALL = 7,
     /* The host will read this tick's results back (chd_fetch_results): start the expanded-list kernel only after the

@@ -543,6 +543,80 @@ def test_graph_replay_matches_direct_and_oracle(chd, oracle):
     assert sum(r[0]["n_due"] for r in results[True]) > 1000 and sum(r[0]["n_handover"] for r in results[True]) > 100
 
 
+def test_tick_forms_match_step_by_step(chd):
+    """Every way of enqueueing a tick (one stream or two, the interest / fan-out chain started by chd_tick or early by
+    chd_begin_interest with or without the fan-out, the fan-out on the main stream after the join, the early read-back)
+    gives the summary, pairs, visible lists, interest diff, due list and handover list of the four stages called one by one."""
+    import ctypes as C
+
+    wc = chd.synth.scaled(chd.synth.CONFIGS["benchmark"], 30_000, 3_000)
+    A, B, E, F = chd.capi.TICK_ALL, chd.capi.TICK_BUILD, chd.capi.TICK_EMIT, chd.capi.TICK_FANOUT
+
+    def step(e, batch, t):
+        e.build()
+        e.update_interest(batch, t)
+        e.emit_visible()
+        e.fanout_tick(t)
+        return e.summary()
+
+    def early(e, batch, t):
+        e.tick(batch, t, A | chd.capi.TICK_EARLY_RESULTS, want_summary=False)
+        s = chd.capi.TickSummary()
+        e._ck(e.L.chd_fetch_results(e.h, C.byref(chd.capi.ResultBuffers()), C.byref(s)))
+        return s
+
+    def begin(with_fanout):
+        def run(e, batch, t):
+            e.begin_interest(batch, t, with_fanout=with_fanout)
+            return e.tick(None, t, A)
+        return run
+
+    def build_emit_then_fanout(e, batch, t):
+        e.tick(batch, t, B | E, want_summary=False)
+        e.fanout_tick(t)
+        return e.summary()
+
+    forms = {"step": step, "tick": lambda e, batch, t: e.tick(batch, t, A), "early_results": early,
+             "begin_with_fanout": begin(True), "begin_without_fanout": begin(False), "build_emit_then_fanout": build_emit_then_fanout}
+    canon = lambda u, v: np.sort(u.astype(np.uint64) << np.uint64(32) | v.astype(np.uint64))  # noqa: E731
+    results = {}
+    for name, run in forms.items():
+        e = chd.engine.Engine(wc.cfg(), wc.n_entities, wc.n_subscribers, max_visible=1 << 22)
+        ex, ez = chd.synth.entities(wc)
+        conn, _, _, _ = chd.synth.subscribers(wc, ex, ez)
+        e.set_subscribers(conn)
+        ring_state, out = None, []
+        for tick in range(4):
+            t = (tick + 1) * 33_000_000
+            ex, ez = chd.synth.move_entities(wc, ex, ez, tick, 400.0)
+            _, cx, cz, r = chd.synth.subscribers(wc, ex, ez)
+            ring_state, off, arr, snd, idx, cmi = chd.synth.update_rings(wc, tick, t, 33_000_000, 4, len(conn), ring_len=16, state=ring_state)
+            e.set_rings(off, arr, snd, idx, cmi)
+            e.set_entities(ex, ez)
+            batch, keep = chd.engine.make_batch(len(cx), sub=np.arange(len(cx), dtype=np.uint32), sphere=(cx, cz, r))
+            s = run(e, batch, t)
+            pairs = e.get_pairs(s.n_pairs)
+            voff, vis = e.get_visible()
+            (ns, nc), (us, uc) = e.get_diff(s.n_sub_new, s.n_unsub)
+            due = e.get_due(s.n_due)
+            due = due[np.lexsort((due["window_hi"], due["channel_id"], due["sub"]))]
+            ho = np.stack(e.get_handover(s.n_handover), 1)
+            ho = ho[np.lexsort((ho[:, 2], ho[:, 1], ho[:, 0]))]
+            out.append(dict(s=s.as_dict(), pairs=pairs, voff=voff, vis=vis, new=canon(ns, nc), unsub=canon(us, uc), due=due, ho=ho))
+        e.close()
+        results[name] = out
+    want = results.pop("step")
+    for k in ("n_due", "n_handover", "n_sub_new", "n_unsub"):  # every compared list is non-empty in some tick
+        assert sum(w["s"][k] for w in want) > 0, k
+    for name, got in results.items():
+        for tick, (g, w) in enumerate(zip(got, want)):
+            assert g["s"] == w["s"], (name, tick)
+            for k in w["pairs"]:
+                np.testing.assert_array_equal(g["pairs"][k], w["pairs"][k], err_msg=f"{name} tick {tick} pairs {k}")
+            for k in ("voff", "vis", "new", "unsub", "due", "ho"):
+                np.testing.assert_array_equal(g[k], w[k], err_msg=f"{name} tick {tick} {k}")
+
+
 @pytest.mark.parametrize("early", [False, True])
 def test_fetch_results_matches_getters(chd, early):
     """chd_fetch_results (one call) returns exactly what the individual getters return, also when the read-back runs
