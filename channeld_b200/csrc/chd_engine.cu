@@ -50,17 +50,10 @@ void chd_dfree(chd_engine* e, void* p) {
 
 chd_status chd_ensure_upload_stream(chd_engine* e) {
     if (e->up_stream) return CHD_OK;
-    int lo = 0, hi = 0;
-    cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    CU(e, cudaStreamCreateWithPriority(&e->up_stream, cudaStreamNonBlocking, hi));
-    CU(e, cudaEventCreateWithFlags(&e->ev_upload, cudaEventDisableTiming));
-    CU(e, cudaEventCreateWithFlags(&e->ev_upload_q, cudaEventDisableTiming));
-    CU(e, cudaEventCreateWithFlags(&e->ev_upload_rings, cudaEventDisableTiming));
-    for (int i = 0; i < 2; i++) {
-        CU(e, cudaEventCreateWithFlags(&e->ev_q_read[i], cudaEventDisableTiming));
-        CU(e, cudaEventCreateWithFlags(&e->ev_ring_read[i], cudaEventDisableTiming));
-    }
-    return CHD_OK;
+    bool ok = chd_make_stream(e, &e->up_stream);
+    for (cudaEvent_t* ev : {&e->ev_upload, &e->ev_upload_q, &e->ev_upload_rings, &e->ev_q_read[0], &e->ev_ring_read[0], &e->ev_q_read[1], &e->ev_ring_read[1]})
+        ok = ok && chd_make_event(e, ev);
+    return ok ? CHD_OK : CHD_ERR_CUDA;
 }
 
 chd_status chd_read_u32(chd_engine* e, const uint32_t* d, uint32_t* v) {
@@ -131,23 +124,10 @@ void chd_destroy(chd_engine* e) {
     cudaSetDevice(e->device);
     if (e->stream) cudaStreamSynchronize(e->stream);
     chd_comm_destroy(e);
-    if (e->up_stream) cudaStreamSynchronize(e->up_stream);
+    for (cudaStream_t s : e->streams) cudaStreamSynchronize(s);
     for (void* p : e->allocs) cudaFree(p);
-    for (auto* arr : {e->g_emit_prep, e->g_import})
-        for (int i = 0; i < 2; i++)
-            if (arr[i].exec) cudaGraphExecDestroy(arr[i].exec);
-    for (auto* arr : {e->g_build, e->g_build_b, e->g_export, e->g_interest, e->g_interest_b, e->g_fanout})
-        for (int i = 0; i < 4; i++)
-            if (arr[i].exec) cudaGraphExecDestroy(arr[i].exec);
-    for (cudaEvent_t ev : {e->ev_upload_q, e->ev_q_read[0], e->ev_q_read[1], e->ev_upload_rings, e->ev_ring_read[0], e->ev_ring_read[1]})
-        if (ev) cudaEventDestroy(ev);
-    if (e->up_stream) {
-        cudaStreamSynchronize(e->up_stream);
-        cudaStreamDestroy(e->up_stream);
-    }
-    if (e->ev_upload) cudaEventDestroy(e->ev_upload);
-    for (int i = 0; i < 2; i++)
-        if (e->ev_pos_read[i]) cudaEventDestroy(e->ev_pos_read[i]);
+    for (cudaEvent_t ev : e->events) cudaEventDestroy(ev);
+    for (cudaStream_t s : e->streams) cudaStreamDestroy(s);
     if (e->ev) {
         for (size_t i = 0; i < (size_t)CHD_STAGE_COUNT * chd_engine::EV_RING * 2; i++)
             if (e->ev[i]) cudaEventDestroy(e->ev[i]);
@@ -156,25 +136,8 @@ void chd_destroy(chd_engine* e) {
     if (e->h_ctr) cudaFreeHost(e->h_ctr);
     if (e->h_u32) cudaFreeHost(e->h_u32);
     if (e->h_get) cudaFreeHost(e->h_get);
-    if (e->aux_stream) cudaStreamDestroy(e->aux_stream);
-    if (e->dl_stream) cudaStreamDestroy(e->dl_stream);
-    if (e->dl_stream_b) cudaStreamDestroy(e->dl_stream_b);
-    if (e->dl_stream_c) cudaStreamDestroy(e->dl_stream_c);
-    for (int i = 0; i < 2; i++) {
-        if (e->ev_fetch_a[i]) cudaEventDestroy(e->ev_fetch_a[i]);
-        if (e->ev_fetch_b[i]) cudaEventDestroy(e->ev_fetch_b[i]);
-        if (e->ev_fetch_done[i]) cudaEventDestroy(e->ev_fetch_done[i]);
-    }
-    if (e->ev_prep_done) cudaEventDestroy(e->ev_prep_done);
-    if (e->ev_build_done) cudaEventDestroy(e->ev_build_done);
-    if (e->ev_counts) cudaEventDestroy(e->ev_counts);
-    if (e->prep_stream) cudaStreamDestroy(e->prep_stream);
-    if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-    if (e->ev_join) cudaEventDestroy(e->ev_join);
-    if (e->ev_interest) cudaEventDestroy(e->ev_interest);
-    if (e->ev_pairs) cudaEventDestroy(e->ev_pairs);
     if (e->own_stream && e->stream) cudaStreamDestroy(e->stream);
-    delete e;
+    delete e;  // on e->device: the graph slots release their executables
 }
 
 static bool alloc_pairbuf(chd_engine* e, PairBuf& pb) {
@@ -251,26 +214,6 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     CCU(cudaSetDevice(device));
     CCU(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
     e->own_stream = true;
-    {
-        // the aux stream carries short latency-bound kernels that should slot in ahead of the long emit kernel
-        int lo_prio = 0, hi_prio = 0;
-        CCU(cudaDeviceGetStreamPriorityRange(&lo_prio, &hi_prio));
-        CCU(cudaStreamCreateWithPriority(&e->aux_stream, cudaStreamNonBlocking, hi_prio));
-    }
-    CCU(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
-    CCU(cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
-    CCU(cudaEventCreateWithFlags(&e->ev_interest, cudaEventDisableTiming));
-    CCU(cudaEventCreateWithFlags(&e->ev_pairs, cudaEventDisableTiming));
-    CCU(cudaEventCreateWithFlags(&e->ev_prep_done, cudaEventDisableTiming));
-    CCU(cudaEventCreateWithFlags(&e->ev_build_done, cudaEventDisableTiming));
-    CCU(cudaEventCreateWithFlags(&e->ev_counts, cudaEventDisableTiming));
-    {
-        int lo_prio = 0, hi_prio2 = 0;
-        CCU(cudaDeviceGetStreamPriorityRange(&lo_prio, &hi_prio2));
-        CCU(cudaStreamCreateWithPriority(&e->dl_stream, cudaStreamNonBlocking, hi_prio2));
-        CCU(cudaStreamCreateWithPriority(&e->dl_stream_b, cudaStreamNonBlocking, hi_prio2));
-        CCU(cudaStreamCreateWithPriority(&e->prep_stream, cudaStreamNonBlocking, hi_prio2));
-    }
     CCU(cudaDeviceGetAttribute(&e->sm_count, cudaDevAttrMultiProcessorCount, device));
     CCU(cudaDeviceGetAttribute(&e->l2_bytes, cudaDevAttrL2CacheSize, device));
 
@@ -296,10 +239,14 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     if (Q + 1 > scan_n) scan_n = Q + 1;
     if (S + 1 > scan_n) scan_n = S + 1;
     if (N + 1 > scan_n) scan_n = N + 1;
-    bool ok = true;
+    // the aux stream carries short latency-bound kernels that should slot in ahead of the long emit kernel
+    bool ok = chd_make_stream(e, &e->aux_stream) && chd_make_stream(e, &e->dl_stream) && chd_make_stream(e, &e->dl_stream_b) &&
+              chd_make_stream(e, &e->prep_stream);
+    for (cudaEvent_t* ev : {&e->ev_fork, &e->ev_join, &e->ev_interest, &e->ev_pairs, &e->ev_prep_done, &e->ev_build_done, &e->ev_counts,
+                            &e->ev_pos_read[0], &e->ev_pos_read[1]})
+        ok = ok && chd_make_event(e, ev);
     ok = ok && dalloc(e, &e->d_x, N) && dalloc(e, &e->d_z, N) && (e->d_xb[0] = e->d_x, e->d_zb[0] = e->d_z, true) &&
-         cudaEventCreateWithFlags(&e->ev_pos_read[0], cudaEventDisableTiming) == cudaSuccess &&
-         cudaEventCreateWithFlags(&e->ev_pos_read[1], cudaEventDisableTiming) == cudaSuccess && dalloc(e, &e->d_gid, N) && dalloc(e, &e->d_key, N) &&
+         dalloc(e, &e->d_gid, N) && dalloc(e, &e->d_key, N) &&
          dalloc(e, &e->d_prev_key, N) && dalloc(e, &e->d_tmp_key, N) && dalloc(e, &e->d_tmp_val, N) &&
          dalloc(e, &e->d_sorted_key, N) && dalloc(e, &e->d_sorted4, 4 * (((N + 3) / 4) * 4 + 8)) && dalloc(e, &e->d_cell_start, C + 2) &&
          dalloc(e, &e->d_hist, (uint64_t)BUILD_MAX_BINS * e->build_blocks + 2) &&
@@ -315,12 +262,7 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     e->d_key_a = e->d_key;
     ok = ok && dalloc(e, &e->d_conn, S) && dalloc(e, &e->d_slot_ctl, S) && dalloc(e, &e->d_slot_src, S) && dalloc(e, &e->d_lc_slot, S) &&
          dalloc(e, &e->d_lc_aux, S) && alloc_pairbuf(e, e->pairs[0]) && alloc_pairbuf(e, e->pairs[1]);
-    ok = ok && dalloc(e, &e->dq.sub, Q) && dalloc(e, &e->dq.kind, Q) && dalloc(e, &e->dq.sph_cx, Q) && dalloc(e, &e->dq.sph_cz, Q) &&
-         dalloc(e, &e->dq.sph_r, Q) && dalloc(e, &e->dq.box_cx, Q) && dalloc(e, &e->dq.box_cz, Q) && dalloc(e, &e->dq.box_ex, Q) &&
-         dalloc(e, &e->dq.box_ez, Q) && dalloc(e, &e->dq.cone_cx, Q) && dalloc(e, &e->dq.cone_cz, Q) && dalloc(e, &e->dq.cone_dx, Q) &&
-         dalloc(e, &e->dq.cone_dz, Q) && dalloc(e, &e->dq.cone_angle, Q) && dalloc(e, &e->dq.cone_r, Q) &&
-         dalloc(e, &e->dq.spot_off, Q + 1) && dalloc(e, &e->dq.spot_ndist, Q) && dalloc(e, &e->dq.spot_x, (uint64_t)L.max_spots) &&
-         dalloc(e, &e->dq.spot_z, (uint64_t)L.max_spots) && dalloc(e, &e->dq.spot_dist, (uint64_t)L.max_spots);
+    ok = ok && alloc_qstage(e, e->dq);
     ok = ok && dalloc(e, &e->d_bbox, Q) && dalloc(e, &e->d_win_off, Q + 1) && dalloc(e, &e->d_qstatus, Q) && dalloc(e, &e->d_win_cursor, 1) &&
          dalloc(e, &e->d_noff, S + 2) &&
          dalloc(e, &e->d_window, L.max_window_cells) && dalloc(e, &e->d_side_cell, (uint64_t)L.max_spots) &&

@@ -39,7 +39,11 @@ struct chd_engine {
     // graph capture on `stream` against launches of the stateless entry points, which may run on other threads.
     std::recursive_mutex mu;
     mutable std::string err;
+    // what chd_destroy releases: device memory (dalloc), every stream but `stream` (chd_make_stream), every event but the
+    // profiling ring (chd_make_event); each GraphSlot releases its own executable
     std::vector<void*> allocs;
+    std::vector<cudaStream_t> streams;
+    std::vector<cudaEvent_t> events;
     int sm_count = 132;
     int l2_bytes = 50 << 20;  // both read from the device in chd_create
     uint64_t n_launch = 0;  // kernels launched by this engine (bench.py reports it as gpu_launches)
@@ -48,6 +52,14 @@ struct chd_engine {
         cudaGraphExec_t exec = nullptr;
         uint64_t key = 0, pending_key = 0;
         uint64_t nodes = 0;
+        GraphSlot() = default;
+        GraphSlot(const GraphSlot&) = delete;
+        GraphSlot& operator=(const GraphSlot&) = delete;
+        ~GraphSlot() { release(); }
+        void release() {
+            if (exec) cudaGraphExecDestroy(exec);
+            exec = nullptr;
+        }
     };
     bool use_graphs = true;
     cudaStream_t aux_stream = nullptr;
@@ -219,7 +231,7 @@ struct chd_engine {
     uint32_t ring_cap = 0;
     uint32_t *d_rb_begin = nullptr, *d_rb_end = nullptr, *d_upd_off = nullptr, *d_upd_sender = nullptr, *d_ring_flat_off = nullptr;
     int64_t* d_upd_arrival = nullptr;
-    uint64_t upd_cap = 0;
+    uint64_t upd_arrival_cap = 0, upd_sender_cap = 0;
     uint32_t* d_ring_scan_scratch = nullptr;
     uint32_t* d_cell_max_interval = nullptr;  // [C] ChannelData.maxFanOutIntervalMs (subscription.go:84-86)
     int64_t* d_cell_start_ns = nullptr;       // [C] per-channel ChannelTime origin (chd_set_channel_start_times) or nullptr
@@ -323,6 +335,35 @@ static bool dalloc(chd_engine* e, T** p, uint64_t count) {
     return true;
 }
 
+// Every secondary stream: non-blocking and at the device's highest priority, so that its short kernels and copies do not queue
+// behind the emit kernel's grid.  chd_destroy releases it.
+static inline bool chd_make_stream(chd_engine* e, cudaStream_t* s) {
+    int lo = 0, hi = 0;
+    cudaError_t r = cudaDeviceGetStreamPriorityRange(&lo, &hi);
+    if (r == cudaSuccess) r = cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, hi);
+    if (r != cudaSuccess) return e->fail("cudaStreamCreateWithPriority failed: %s", cudaGetErrorString(r));
+    e->streams.push_back(*s);
+    return true;
+}
+
+// An ordering-only event (no timing); chd_destroy releases it.
+static inline bool chd_make_event(chd_engine* e, cudaEvent_t* ev) {
+    cudaError_t r = cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
+    if (r != cudaSuccess) return e->fail("cudaEventCreateWithFlags failed: %s", cudaGetErrorString(r));
+    e->events.push_back(*ev);
+    return true;
+}
+
+// one query staging set: chd_create's dq, chd_prefetch_queries' dq_pf[]
+static inline bool alloc_qstage(chd_engine* e, chd_engine::QStage& qs) {
+    const uint64_t Q = e->lim.max_queries, SP = e->lim.max_spots;
+    return dalloc(e, &qs.sub, Q) && dalloc(e, &qs.kind, Q) && dalloc(e, &qs.sph_cx, Q) && dalloc(e, &qs.sph_cz, Q) && dalloc(e, &qs.sph_r, Q) &&
+           dalloc(e, &qs.box_cx, Q) && dalloc(e, &qs.box_cz, Q) && dalloc(e, &qs.box_ex, Q) && dalloc(e, &qs.box_ez, Q) &&
+           dalloc(e, &qs.cone_cx, Q) && dalloc(e, &qs.cone_cz, Q) && dalloc(e, &qs.cone_dx, Q) && dalloc(e, &qs.cone_dz, Q) &&
+           dalloc(e, &qs.cone_angle, Q) && dalloc(e, &qs.cone_r, Q) && dalloc(e, &qs.spot_off, Q + 1) && dalloc(e, &qs.spot_ndist, Q) &&
+           dalloc(e, &qs.spot_x, SP) && dalloc(e, &qs.spot_z, SP) && dalloc(e, &qs.spot_dist, SP);
+}
+
 enum { EP_BUILD = 0, EP_QUERY, EP_EMIT, EP_FANOUT, EP_BORDER, EP_BCAST, EP_CLASS, EP_PAYLOAD, EP_COUNT };  // d_epoch has 8 slots
 
 // ---- helpers shared by the translation units (C linkage only so that definitions may sit inside their extern "C" blocks)
@@ -357,6 +398,19 @@ chd_status chd_sort_pass_any(chd_engine* e, cudaStream_t s, uint32_t* hist, cons
                              uint32_t* val_out, ScatterExtras ex = ScatterExtras{0, nullptr, 0, nullptr}, unsigned long long* bump = nullptr);
 }
 
+// Grow-on-demand buffer: when `need` elements exceed `*cap`, the buffer is replaced (contents not kept) by one of `count`
+// elements, the caller's growth policy.  *cap is 0 exactly when there is no buffer.
+template <typename T>
+static bool ensure_cap(chd_engine* e, T** p, uint64_t* cap, uint64_t need, uint64_t count) {
+    if (need <= *cap) return true;
+    chd_dfree(e, *p);
+    *p = nullptr;
+    *cap = 0;
+    if (!dalloc(e, p, count)) return false;
+    *cap = count;
+    return true;
+}
+
 static inline unsigned blocks_for(uint64_t n, unsigned threads) { return (unsigned)((n + threads - 1) / threads); }
 
 static inline uint64_t mix_key(uint64_t h, uint64_t v) {
@@ -381,10 +435,7 @@ static chd_status run_stage(chd_engine* e, cudaStream_t s, chd_engine::GraphSlot
         slot.pending_key = key;
         return enqueue();
     }
-    if (slot.exec) {
-        cudaGraphExecDestroy(slot.exec);
-        slot.exec = nullptr;
-    }
+    slot.release();
     const uint64_t l0 = e->n_launch;
     // Stateless entry points (chd_cell_of, chd_query_channel_ids) may be called from other threads and launch into the engine
     // stream: they hold the engine mutex for their whole call, so taking it here keeps their work out of the capture.

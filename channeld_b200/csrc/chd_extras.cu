@@ -148,14 +148,7 @@ chd_status chd_adjacent_broadcast(chd_engine* e, const chd_broadcast_batch* b, u
         e->fail("chd_adjacent_broadcast: %u recipients > capacity %llu", total, (unsigned long long)cap);
         return CHD_ERR_CAPACITY;
     }
-    if (total > e->bc_out_cap) {
-        chd_dfree(e, e->d_bc_out);
-        e->d_bc_out = nullptr;
-        e->bc_out_cap = 0;
-        const uint64_t c = std::max<uint64_t>(1 << 16, (uint64_t)total + total / 2);
-        if (!dalloc(e, &e->d_bc_out, c)) return CHD_ERR_CUDA;
-        e->bc_out_cap = c;
-    }
+    if (!ensure_cap(e, &e->d_bc_out, &e->bc_out_cap, total, std::max<uint64_t>(1 << 16, (uint64_t)total + total / 2))) return CHD_ERR_CUDA;
     if (total) {
         bcast_kernel<true><<<blocks, 256, 0, s>>>(e->g, bd, pb.off + S, P, pb, e->d_by_cell, e->d_conn, types, nullptr, e->d_bc_off, e->d_bc_out,
                                                   e->bc_out_cap, nullptr);

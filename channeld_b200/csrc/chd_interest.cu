@@ -19,14 +19,7 @@ chd_status chd_prefetch_queries(chd_engine* e, const chd_query_batch* q) {
     const int set = e->q_next;
     chd_engine::QStage& qs = e->dq_pf[set];
     if (!e->dq_pf_alloc[set]) {
-        const uint64_t Q = e->lim.max_queries;
-        const bool ok = dalloc(e, &qs.sub, Q) && dalloc(e, &qs.kind, Q) && dalloc(e, &qs.sph_cx, Q) && dalloc(e, &qs.sph_cz, Q) && dalloc(e, &qs.sph_r, Q) &&
-                        dalloc(e, &qs.box_cx, Q) && dalloc(e, &qs.box_cz, Q) && dalloc(e, &qs.box_ex, Q) && dalloc(e, &qs.box_ez, Q) &&
-                        dalloc(e, &qs.cone_cx, Q) && dalloc(e, &qs.cone_cz, Q) && dalloc(e, &qs.cone_dx, Q) && dalloc(e, &qs.cone_dz, Q) &&
-                        dalloc(e, &qs.cone_angle, Q) && dalloc(e, &qs.cone_r, Q) && dalloc(e, &qs.spot_off, Q + 1) && dalloc(e, &qs.spot_ndist, Q) &&
-                        dalloc(e, &qs.spot_x, (uint64_t)e->lim.max_spots) && dalloc(e, &qs.spot_z, (uint64_t)e->lim.max_spots) &&
-                        dalloc(e, &qs.spot_dist, (uint64_t)e->lim.max_spots);
-        if (!ok) return CHD_ERR_CUDA;
+        if (!alloc_qstage(e, qs)) return CHD_ERR_CUDA;
         e->dq_pf_alloc[set] = true;
     }
     if (e->q_read_recorded[set]) CU(e, cudaStreamWaitEvent(e->up_stream, e->ev_q_read[set], 0));  // its previous batch has been consumed

@@ -5,21 +5,10 @@
 
 #include "chd_payload.cuh"
 
-template <typename T>
-static chd_status ensure_cap(chd_engine* e, T** p, uint64_t* cap, uint64_t need) {
-    if (need <= *cap && *p) return CHD_OK;
-    chd_dfree(e, *p);
-    *p = nullptr;
-    *cap = 0;
-    const uint64_t c = need + need / 4 + 256;
-    if (!dalloc(e, p, c)) return CHD_ERR_CUDA;
-    *cap = c;
-    return CHD_OK;
-}
-#define ENSURE(e, ptr, cap, need)                                  \
-    do {                                                           \
-        chd_status _s = ensure_cap(e, &(ptr), &(cap), (need));     \
-        if (_s != CHD_OK) return _s;                               \
+#define ENSURE(e, ptr, cap, need)                                                       \
+    do {                                                                                \
+        const uint64_t _n = (need);                                                     \
+        if (!ensure_cap(e, &(ptr), &(cap), _n, _n + _n / 4 + 256)) return CHD_ERR_CUDA; \
     } while (0)
 
 static chd_status remake_site(chd_engine* e, ScanSite& site, uint64_t* cap, uint64_t need, int stage) {

@@ -310,10 +310,7 @@ chd_status chd_fetch_results_async(chd_engine* e, const chd_result_buffers* b, v
         return CHD_ERR_STATE;
     }
     const int fi = (int)(e->fetch_issued & 1);
-    if (!e->ev_fetch_a[fi]) {
-        CU(e, cudaEventCreateWithFlags(&e->ev_fetch_a[fi], cudaEventDisableTiming));
-        CU(e, cudaEventCreateWithFlags(&e->ev_fetch_b[fi], cudaEventDisableTiming));
-    }
+    if (!e->ev_fetch_a[fi] && !(chd_make_event(e, &e->ev_fetch_a[fi]) && chd_make_event(e, &e->ev_fetch_b[fi]))) return CHD_ERR_CUDA;
     PairBuf& pb = e->pairs[e->cur];
     const uint32_t S = e->n_slots;
     Counters* ctr = e->d_ctr;
@@ -356,19 +353,9 @@ chd_status chd_fetch_results_async(chd_engine* e, const chd_result_buffers* b, v
     for (PackArgs* pa : sets)
         for (int k = 0; k < pa->n; k++) need += up16(std::max<uint64_t>(pa->seg[k].cap, pa->seg[k].fixed) * pa->seg[k].elem_words * 4);
     need += 2 * up16(sizeof(Counters)) + 64;
-    if (e->fetch_stage_bytes[fi] < need) {
-        chd_dfree(e, e->d_fetch_stage[fi]);
-        e->d_fetch_stage[fi] = nullptr;
-        e->fetch_stage_bytes[fi] = 0;
-        if (!dalloc(e, &e->d_fetch_stage[fi], need)) return CHD_ERR_CUDA;
-        e->fetch_stage_bytes[fi] = need;
-    }
-    if (!e->dl_stream_c) {  // high priority like the other read-back streams: its CTAs must not queue behind the emit kernel's grid
-        int lo_p = 0, hi_p = 0;
-        CU(e, cudaDeviceGetStreamPriorityRange(&lo_p, &hi_p));
-        CU(e, cudaStreamCreateWithPriority(&e->dl_stream_c, cudaStreamNonBlocking, hi_p));
-    }
-    if (!e->ev_fetch_done[fi]) CU(e, cudaEventCreateWithFlags(&e->ev_fetch_done[fi], cudaEventDisableTiming));
+    if (!ensure_cap(e, &e->d_fetch_stage[fi], &e->fetch_stage_bytes[fi], need, need)) return CHD_ERR_CUDA;
+    if (!e->dl_stream_c && !chd_make_stream(e, &e->dl_stream_c)) return CHD_ERR_CUDA;
+    if (!e->ev_fetch_done[fi] && !chd_make_event(e, &e->ev_fetch_done[fi])) return CHD_ERR_CUDA;
     uint8_t* cursor = e->d_fetch_stage[fi];
     auto carve = [&](uint64_t bytes) {
         uint8_t* p = cursor;

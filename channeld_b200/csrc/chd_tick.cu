@@ -176,16 +176,9 @@ chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_u
     CU(e, cudaSetDevice(e->device));
     cudaStream_t s = e->stream;
     const uint32_t C = e->g.cells;
-    if (n_updates > e->upd_cap) {
-        chd_dfree(e, e->d_upd_arrival);
-        chd_dfree(e, e->d_upd_sender);
-        e->d_upd_arrival = nullptr;
-        e->d_upd_sender = nullptr;
-        e->upd_cap = 0;
-        const uint64_t c = (uint64_t)n_updates + n_updates / 2 + 1024;
-        if (!dalloc(e, &e->d_upd_arrival, c) || !dalloc(e, &e->d_upd_sender, c)) return CHD_ERR_CUDA;
-        e->upd_cap = c;
-    }
+    const uint64_t grown = (uint64_t)n_updates + n_updates / 2 + 1024;
+    if (!ensure_cap(e, &e->d_upd_arrival, &e->upd_arrival_cap, n_updates, grown) || !ensure_cap(e, &e->d_upd_sender, &e->upd_sender_cap, n_updates, grown))
+        return CHD_ERR_CUDA;
     CU(e, cudaMemcpyAsync(e->d_upd_off, upd_off, sizeof(uint32_t) * ((uint64_t)C + 1), cudaMemcpyDefault, s));
     if (n_updates) {
         CU(e, cudaMemcpyAsync(e->d_upd_arrival, arrival_ns, sizeof(int64_t) * n_updates, cudaMemcpyDefault, s));
