@@ -27,7 +27,7 @@ struct PairVcountIn {
 __global__ void __launch_bounds__(256)
     emit_partition_kernel(const uint32_t* __restrict__ n_pairs_ptr, uint64_t pair_cap, const uint64_t* __restrict__ voff,
                           const uint32_t* __restrict__ pair_cell, const uint32_t* __restrict__ cell_start, uint32_t* __restrict__ first_pair,
-                          TileDesc* __restrict__ desc, uint32_t stride, uint64_t max_tiles, uint32_t n_slots, const uint32_t* __restrict__ pair_off,
+                          TileDesc* __restrict__ desc, uint64_t max_tiles, uint32_t n_slots, const uint32_t* __restrict__ pair_off,
                           uint64_t* __restrict__ vis_off, uint64_t vis_cap, Counters* __restrict__ ctr, unsigned long long* bump_epoch,
                           uint32_t tile, uint32_t* __restrict__ general_tiles, uint32_t* __restrict__ n_general) {
     const uint64_t n = min((uint64_t)*n_pairs_ptr, pair_cap);
@@ -56,10 +56,7 @@ __global__ void __launch_bounds__(256)
             const uint32_t tile_len = (uint32_t)min((uint64_t)tile, V - base);
             TileDesc d;
             d.p0 = (uint32_t)p;
-            // bases are phase-adjusted: the entry that lands on tile slot o is sorted4[base + o] and base + o is a multiple of 4
-            // whenever o is (copy k of the CSR payload holds element i at k * stride + k + i, stride % 4 == 0)
-            const uint32_t s0 = cs + (uint32_t)(base - b), ph0 = (0u - s0) & 3u;
-            d.src0 = ph0 * stride + ph0 + s0;
+            d.src0 = cs + (uint32_t)(base - b);  // tile slot o <- sorted entity src0 + o (phase copy 0)
             const uint32_t end0 = (uint32_t)min((uint64_t)tile, e - base);
             uint32_t end1 = end0;
             d.src1 = 0;
@@ -67,8 +64,7 @@ __global__ void __launch_bounds__(256)
                 uint64_t q = p + 1;
                 while (q < n && voff[q + 1] == e) q++;
                 if (q < n) {
-                    const uint32_t s1 = cell_start[pair_cell[q]] - end0, ph1 = (0u - s1) & 3u;  // (wraps: only base + o, o >= end0, is used)
-                    d.src1 = ph1 * stride + ph1 + s1;
+                    d.src1 = cell_start[pair_cell[q]] - end0;  // (wraps: only src1 + o, o >= end0, is used)
                     end1 = (uint32_t)min((uint64_t)tile, voff[q + 1] - base);
                 }
             }
@@ -140,15 +136,28 @@ __device__ __forceinline__ void emit_tile_general(uint64_t t, uint64_t n_tiles, 
     }
 }
 
+// 16 bytes of a list that starts m entries into chunk a and continues into chunk b
+__device__ __forceinline__ uint4 emit_funnel(uint4 a, uint4 b, uint32_t m) {
+    switch (m) {
+        case 1: return make_uint4(a.y, a.z, a.w, b.x);
+        case 2: return make_uint4(a.z, a.w, b.x, b.y);
+        case 3: return make_uint4(a.w, b.x, b.y, b.z);
+        default: return a;
+    }
+}
+
 // One CTA per 8 KB tile of the output (EMIT_TILE = 2048 entries: EMIT_ROWS rows of 256 x 16 bytes), dispatched by the
 // hardware block scheduler.  Streaming stores (st.global.cs) keep the write stream from evicting the L2-resident sources.
 // This kernel copies the SIMPLE tiles only (at most two segments: everything a thread needs is the 16-byte descriptor
-// {base0, base1, ends, p0}; the bases are phase-adjusted so every move is a co-aligned LDG.128 -> STG.128) and nothing else
-// lives in it, so that it fits 32 registers = 8 CTAs (all 64 warps) per SM; tiles with more segments are listed by the
-// partition pass and copied by emit_visible_general_kernel.  The loop only runs more than once if the host under-estimated
-// the tile count when it sized the grid.
+// {src0, src1, ends, p0}); tiles with more segments are listed by the partition pass and copied by
+// emit_visible_general_kernel.  The loop only runs more than once if the host under-estimated the tile count when it sized
+// the grid.
+// Sources are read from phase copy 0 alone (4 B x N: 4 MB at 1 M entities), not from the four phase copies: with the 16 MB
+// of all four the same kernel runs 25 % slower on an H100, the sources no longer staying in L2 next to the write stream.  A
+// chunk that starts m = src & 3 entries into an aligned 16-byte chunk a takes the rest from chunk a + 1, which the next lane
+// loaded already (shuffle); lane 31, and a lane whose neighbour reads elsewhere, loads it itself.
 __global__ void __launch_bounds__(EMIT_THREADS, CHD_EMIT_MIN_BLOCKS)
-    emit_visible_kernel(const unsigned long long* __restrict__ n_visible_ptr, const uint32_t* __restrict__ sorted4, const TileDesc* __restrict__ desc,
+    emit_visible_kernel(const unsigned long long* __restrict__ n_visible_ptr, const uint32_t* __restrict__ sorted, const TileDesc* __restrict__ desc,
                         uint32_t* __restrict__ vis_entity, uint64_t vis_cap) {
     // V (published by the partition pass) and the CTA's descriptor are loaded back to back: two independent round trips to L2 in
     // flight at once (volatile asm: the compiler would otherwise sink the descriptor load below the early exits)
@@ -160,35 +169,49 @@ __global__ void __launch_bounds__(EMIT_THREADS, CHD_EMIT_MIN_BLOCKS)
     }
     if (V == 0 || V > vis_cap) return;
     const uint32_t n_tiles = (uint32_t)((V + EMIT_TILE - 1) / EMIT_TILE);
-    const uint32_t tid4 = threadIdx.x * 4;
+    const uint32_t tid4 = threadIdx.x * 4, lane = threadIdx.x & 31;
     for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
         if (t != blockIdx.x) dw = __ldg(reinterpret_cast<const uint4*>(desc + t));
         if (dw.z & 0x80000000u) continue;  // CTA-uniform: a general tile
         const uint32_t end0 = dw.z & 0x7FFFu, end1 = (dw.z >> 16) & 0x7FFFu;  // a simple tile's second segment reaches the end of the tile / list
         uint32_t* __restrict__ out = vis_entity + (uint64_t)t * EMIT_TILE;
-        uint4 v[EMIT_ROWS];
+        uint4 va[EMIT_ROWS], vb[EMIT_ROWS];
+        uint32_t si[EMIT_ROWS];
         uint32_t whole = 0;
 #pragma unroll
         for (int r = 0; r < EMIT_ROWS; r++) {
             const uint32_t o = r * (EMIT_THREADS * 4) + tid4;
             const bool in0 = o + 4 <= end0, in1 = o >= end0 && o + 4 <= end1;
+            // 32-bit index arithmetic ON PURPOSE: src1 is stored minus end0 and may have wrapped below zero; src1 + o wraps back
+            si[r] = (in0 ? dw.x : dw.y) + o;
             if (in0 || in1) {
-                // 32-bit index arithmetic ON PURPOSE: base1 is stored minus end0 and may have wrapped below zero; base1 + o wraps back
-                const uint32_t si = (in0 ? dw.x : dw.y) + o;
-                v[r] = __ldg(reinterpret_cast<const uint4*>(sorted4 + si));
+                const uint4* q = reinterpret_cast<const uint4*>(sorted + (si[r] & ~3u));
+                va[r] = __ldg(q);
+                if (lane == 31 && (si[r] & 3u)) vb[r] = __ldg(q + 1);  // (in bounds: the copy is padded by 8 entries)
                 whole |= 1u << r;
             }
         }
+        const uint32_t whole_next = __shfl_down_sync(0xffffffffu, whole, 1);
 #pragma unroll
-        for (int r = 0; r < EMIT_ROWS; r++)
-            if (whole & (1u << r)) __stcs(reinterpret_cast<uint4*>(out + r * (EMIT_THREADS * 4) + tid4), v[r]);
+        for (int r = 0; r < EMIT_ROWS; r++) {
+            const uint4 nb = make_uint4(__shfl_down_sync(0xffffffffu, va[r].x, 1), __shfl_down_sync(0xffffffffu, va[r].y, 1),
+                                        __shfl_down_sync(0xffffffffu, va[r].z, 1), __shfl_down_sync(0xffffffffu, va[r].w, 1));
+            const uint32_t si_next = __shfl_down_sync(0xffffffffu, si[r], 1);
+            if (!(whole & (1u << r))) continue;
+            const uint32_t m = si[r] & 3u;
+            if (m && lane != 31) {
+                if ((whole_next & (1u << r)) && (si_next & ~3u) == (si[r] & ~3u) + 4) vb[r] = nb;
+                else vb[r] = __ldg(reinterpret_cast<const uint4*>(sorted + (si[r] & ~3u)) + 1);
+            }
+            __stcs(reinterpret_cast<uint4*>(out + r * (EMIT_THREADS * 4) + tid4), emit_funnel(va[r], vb[r], m));
+        }
 #pragma unroll
         for (int r = 0; r < EMIT_ROWS; r++) {
             const uint32_t o = r * (EMIT_THREADS * 4) + tid4;
             if (!(whole & (1u << r)) && o < end1)  // the chunk straddles the segment boundary / the end of the list: entry by entry
                 for (uint32_t j = 0; j < 4 && o + j < end1; j++) {
-                    const uint32_t si = (o + j < end0 ? dw.x : dw.y) + o + j;  // (32-bit wrap, as above)
-                    out[o + j] = __ldg(sorted4 + si);
+                    const uint32_t sj = (o + j < end0 ? dw.x : dw.y) + o + j;  // (32-bit wrap, as above)
+                    out[o + j] = __ldg(sorted + sj);
                 }
         }
     }

@@ -108,7 +108,7 @@ __device__ __forceinline__ uint32_t fanout_eval(const RingDev& ring, const Ring&
 // reference issues them from independent per-channel goroutines, i.e. in no global order either).
 constexpr uint32_t FANOUT_STAGE = 640;  // 12.5 KB of shared memory per block
 
-__global__ void __launch_bounds__(128, 8)  // <= 64 registers = 8192 per CTA: a fan-out CTA fits the slot ONE retiring emit CTA (256 x 32) frees
+__global__ void __launch_bounds__(128, 8)  // <= 64 registers = 8192 per CTA: a fan-out CTA fits the slot ONE retiring emit CTA (256 x 40) frees
     fanout_kernel(const uint32_t* __restrict__ n_pairs_ptr, uint64_t pair_cap, PairBuf pb, const uint32_t* __restrict__ conn_id, RingDev ring,
                   const int64_t* __restrict__ t_ptr, uint32_t id_start, const uint32_t* __restrict__ by_cell, chd_due* __restrict__ due,
                   DueKey* __restrict__ due_key, uint32_t due_cap, Counters* __restrict__ ctr) {

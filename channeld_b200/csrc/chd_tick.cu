@@ -34,7 +34,7 @@ static chd_status emit_prep_enqueue(chd_engine* e, cudaStream_t s, bool cta_tile
         // per-pair visible counts are computed by the scan itself; the partition pass opens the next epoch
         SCAN(e, exclusive_scan_fn<PairVcountIn, uint64_t>(PairVcountIn{pb.cell, e->d_cell_start}, e->d_voff, P, e->site_voff, s, pb.off + S));
         emit_partition_kernel<<<grid, 256, 0, s>>>(pb.off + S, P, e->d_voff, pb.cell, e->d_cell_start, e->d_first_pair, cta_tiles ? e->d_tile_desc : nullptr,
-                                                   e->phase_stride, e->max_tiles, S, pb.off, e->d_vis_off, e->lim.max_visible, e->d_ctr, e->d_epoch + EP_EMIT, tile,
+                                                   e->max_tiles, S, pb.off, e->d_vis_off, e->lim.max_visible, e->d_ctr, e->d_epoch + EP_EMIT, tile,
                                                    e->d_general_tiles, e->d_n_general);
         KCHECK(e);
         return CHD_OK;

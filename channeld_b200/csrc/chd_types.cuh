@@ -11,19 +11,19 @@ constexpr int BUILD_ROUNDS = 8;
 constexpr int BUILD_TILE = BUILD_THREADS * BUILD_ROUNDS;  // 2048 entities per tile
 constexpr int BUILD_MAX_BINS = 1024;
 constexpr int EMIT_THREADS = 256;
-// Two rows (an 8 KB tile) keep the two-segment emit kernel within 32 registers on sm_90a, so 8 CTAs fit an SM without spills.
-// Measured on an H100 SXM (80 GB HBM3, 400 W power limit), benchmark config, emit kernel per tick: 0.858 ms with 2 rows and 8
-// CTAs per SM, 0.875 ms with 4 rows and 6 CTAs (40 registers), 1.53 ms with 4 rows and 8 CTAs (32 registers, 72 bytes spilled
-// per thread), 1.29 ms with 8 rows and 3 CTAs.
+// Two rows (an 8 KB tile) of the two-segment emit kernel.  Measured on an H100 SXM (80 GB HBM3, 400 W power limit), benchmark
+// config, emit kernel per tick, when it still read the four phase copies: 0.858 ms with 2 rows and 8 CTAs per SM, 0.875 ms with 4
+// rows and 6 CTAs (40 registers), 1.53 ms with 4 rows and 8 CTAs (32 registers, 72 bytes spilled per thread), 1.29 ms with 8
+// rows and 3 CTAs.  Reading phase copy 0 alone (shuffles between lanes) needs 40 registers: 8 CTAs per SM (32 registers) spill
+// 44 bytes per thread and took 0.851 ms, 6 CTAs per SM took 0.641 ms (H100 SXM, 700 W, the kernel alone at the benchmark shape).
 #ifndef CHD_EMIT_ROWS
 #define CHD_EMIT_ROWS 2
 #endif
 #ifndef CHD_EMIT_MIN_BLOCKS
-#define CHD_EMIT_MIN_BLOCKS 8
+#define CHD_EMIT_MIN_BLOCKS 6
 #endif
-// Dynamic shared memory the two-segment emit kernel asks for WITHOUT using it: 0 lets 8 CTAs (every warp slot and the whole
-// register file of an SM) be emit CTAs; 30 KB caps them at 7 per SM, which keeps one slot (256 threads, 8 K registers, 18 KB)
-// free for the latency-bound kernels of the second stream (fan-out pass) that run next to it.
+// Dynamic shared memory the two-segment emit kernel asks for WITHOUT using it: 0 lets as many CTAs as the register file allows
+// be emit CTAs; a larger value caps them per SM, to keep slots free for the latency-bound kernels of the second stream.
 #ifndef CHD_EMIT_DYN_SMEM
 #define CHD_EMIT_DYN_SMEM 0
 #endif
@@ -45,8 +45,8 @@ constexpr int EMIT_WARP_SMEM_PAIRS = 64;
 // cell start).  A tile is "simple" if at most two pairs' lists intersect it (always the case when cells hold more entities
 // than a tile: 4 444 vs 4 096 on the benchmark config); other tiles take the general path (segment table in shared memory).
 struct TileDesc {
-    uint32_t src0;  // phase-adjusted base of the first segment: slot o of the tile <- sorted4[src0 + o]
-    uint32_t src1;  // the same for the second segment (slots o >= end0)
+    uint32_t src0;  // base of the first segment in the sorted entity array (phase copy 0): slot o of the tile <- sorted[src0 + o]
+    uint32_t src1;  // the same for the second segment (slots o >= end0; stored minus end0, may wrap below zero)
     uint32_t ends;  // end0 | end1 << 16 (relative to the tile base, <= EMIT_TILE); bit 31 = not simple
     uint32_t p0;    // the pair that owns the tile's first slot (general path)
 };
