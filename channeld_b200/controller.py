@@ -219,3 +219,14 @@ class GpuStaticGrid2DSpatialController:
     # -- Tick()   (channel.go:358-387 for all spatial channels at once)
     def Tick(self, batch, t_ns, flags=capi.TICK_ALL):
         return self.engine.tick(batch, t_ns, flags)
+
+    # -- per client, the entities to spawn / despawn since the last delta: the net effect of the FULL data a new subscription
+    # sends, the despawns of an unsubscription and the handovers between cells (spatial.go:612-858,
+    # SpatialChannelData.AddEntity/RemoveEntity).  ReserveVisibleDelta once (and again, larger, after CHD_OVF_DELTA), then
+    # Tick with capi.TICK_VISIBLE_DELTA; GetVisibleDelta only reads the last delta back.
+    def ReserveVisibleDelta(self, cap_entries):
+        self.engine.reserve_visible_delta(cap_entries)
+
+    # -> (enter_off, enter, leave_off, leave): CSR by subscriber slot of entity indices.
+    def GetVisibleDelta(self):
+        return self.engine.get_visible_delta()

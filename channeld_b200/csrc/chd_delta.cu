@@ -1,0 +1,169 @@
+// chd_delta.cu — visible-set deltas: entered / left entities per subscriber slot since the last successful delta (chd_delta.cuh).
+#include "chd_engine.h"
+
+#include "chd_delta.cuh"
+
+static DeltaDev delta_view(chd_engine* e) {
+    chd_engine::Delta& D = e->dl;
+    const PairBuf& pb = e->pairs[e->cur];
+    DeltaDev d{};
+    d.cells = e->g.cells;
+    d.key = e->d_key;
+    d.n = e->n_sorted;
+    d.cell_start = e->d_cell_start;
+    d.sorted = e->d_sorted_ent;
+    d.pair_off = pb.off;
+    d.pair_cell = pb.cell;
+    d.n_slots = e->n_slots;
+    d.snap_key = D.snap_key; d.snap_cell_start = D.snap_cell_start; d.snap_sorted = D.snap_sorted;
+    d.snap_pair_off = D.snap_pair_off; d.snap_pair_cell = D.snap_pair_cell; d.snap_hdr = D.snap_hdr;
+    d.arr_rank = D.arr_rank; d.dep_rank = D.dep_rank; d.arr = D.arr; d.dep = D.dep; d.arr_start = D.arr_start; d.dep_start = D.dep_start;
+    d.cnt_enter = D.cnt_enter; d.cnt_leave = D.cnt_leave; d.enter_off = D.enter_off; d.leave_off = D.leave_off;
+    d.enter = D.enter; d.leave = D.leave; d.enter_cap = D.enter_cap; d.leave_cap = D.leave_cap;
+    d.n_out = D.n_out;
+    d.overflow = &e->d_ctr->overflow;
+    return d;
+}
+
+extern "C" {
+
+chd_status chd_delta_check(chd_engine* e, bool will_build) {
+    if (e->delta_blocked) {
+        e->fail("visible deltas are single-GPU only: this engine used chd_set_slab / chd_set_entity_ids / chd_comm_init");
+        return CHD_ERR_STATE;
+    }
+    if (!e->dl.on) {
+        e->fail("visible delta before chd_reserve_visible_delta");
+        return CHD_ERR_STATE;
+    }
+    if (!will_build && (!e->built || (e->assigned && e->entities_dirty))) {
+        // chd_assign_cells rewrote the keys since the last build: keys and cell CSR no longer describe one state
+        e->fail("visible delta needs a chd_build of the current cell assignment");
+        return CHD_ERR_STATE;
+    }
+    return CHD_OK;
+}
+
+chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
+    chd_engine::Delta& D = e->dl;
+    StageTimer timer(e, s, CHD_STAGE_VISIBLE_DELTA);
+    D.n_out = std::max(D.n_out, e->n_slots);
+    const DeltaDev d = delta_view(e);
+    const uint32_t C = e->g.cells;
+    const uint64_t N = e->lim.max_entities;
+    chd_status st = chd_epoch_tick(e, s, EP_DELTA);
+    if (st != CHD_OK) return st;
+    // sizes and the key / pair buffers in use are baked into the captured launches
+    uint64_t key = mix_key(mix_key(mix_key(mix_key(0x64656c7461ull, d.n), d.n_slots), D.n_out), (uint64_t)e->cur);
+    key = mix_key(mix_key(mix_key(key, (uint64_t)(uintptr_t)d.key), (uint64_t)(uintptr_t)d.enter), (uint64_t)(uintptr_t)d.leave);
+    key = mix_key(mix_key(key, d.enter_cap), d.leave_cap);
+    const int slot = (e->d_key == e->d_key_a ? 0 : 1) + 2 * e->cur;
+    const unsigned grid = (unsigned)e->sm_count * 8;
+    const unsigned slot_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(blocks_for((uint64_t)D.n_out * 32, DELTA_THREADS), (uint64_t)e->sm_count * 32));
+    return run_stage(e, s, D.g[slot], key, [&]() -> chd_status {
+        bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_DELTA);
+        KCHECK(e);
+        SCAN(e, exclusive_scan_fn<DeltaArrivalFlag, uint32_t>(DeltaArrivalFlag{d.sorted, d.key, d.snap_key, d.snap_hdr, C}, D.arr_rank, N, D.site_arr, s,
+                                                              d.cell_start + C));
+        SCAN(e, exclusive_scan_fn<DeltaDepartureFlag, uint32_t>(DeltaDepartureFlag{d.snap_sorted, d.snap_key, d.key, d.n, C}, D.dep_rank, N, D.site_dep, s,
+                                                                d.snap_cell_start + C));
+        delta_moves_kernel<<<grid, DELTA_THREADS, 0, s>>>(d, (uint32_t)N);
+        KCHECK(e);
+        delta_slots_kernel<false><<<slot_grid, DELTA_THREADS, 0, s>>>(d);
+        KCHECK(e);
+        SCAN(e, exclusive_scan_1p<uint32_t, uint64_t>(D.cnt_enter, D.enter_off, D.n_out, D.site_enter, s));
+        SCAN(e, exclusive_scan_1p<uint32_t, uint64_t>(D.cnt_leave, D.leave_off, D.n_out, D.site_leave, s));
+        delta_slots_kernel<true><<<slot_grid, DELTA_THREADS, 0, s>>>(d);
+        KCHECK(e);
+        delta_advance_kernel<<<grid, DELTA_THREADS, 0, s>>>(d, (uint32_t)e->lim.max_pairs);
+        KCHECK(e);
+        return CHD_OK;
+    });
+}
+
+chd_status chd_reserve_visible_delta(chd_engine* e, uint64_t cap_entries) {
+    if (!e) return CHD_ERR_INVALID;
+    if (e->delta_blocked) return chd_delta_check(e, true);
+    CU(e, cudaSetDevice(e->device));
+    // a delta of an earlier tick may still be running (on the engine stream or, inside a tick, on prep_stream)
+    CU(e, cudaStreamSynchronize(e->stream));
+    CU(e, cudaStreamSynchronize(e->prep_stream));
+    chd_engine::Delta& D = e->dl;
+    const uint64_t N = e->lim.max_entities, S = e->lim.max_subscribers, P = e->lim.max_pairs, C = e->g.cells;
+    if (!D.on) {
+        const bool ok = dalloc(e, &D.snap_key, N) && dalloc(e, &D.snap_cell_start, C + 2) && dalloc(e, &D.snap_sorted, N) &&
+                        dalloc(e, &D.snap_pair_off, S + 1) && dalloc(e, &D.snap_pair_cell, P) && dalloc(e, &D.snap_hdr, 2) &&
+                        dalloc(e, &D.arr_rank, N + 1) && dalloc(e, &D.dep_rank, N + 1) && dalloc(e, &D.arr, N) && dalloc(e, &D.dep, N) &&
+                        dalloc(e, &D.arr_start, C + 1) && dalloc(e, &D.dep_start, C + 1) && dalloc(e, &D.cnt_enter, S) &&
+                        dalloc(e, &D.cnt_leave, S) && dalloc(e, &D.enter_off, S + 1) && dalloc(e, &D.leave_off, S + 1) &&
+                        chd_make_site(e, D.site_arr, N + 1, EP_DELTA) && chd_make_site(e, D.site_dep, N + 1, EP_DELTA) &&
+                        chd_make_site(e, D.site_enter, S + 1, EP_DELTA) && chd_make_site(e, D.site_leave, S + 1, EP_DELTA) &&
+                        chd_make_event(e, &D.ev_in) && chd_make_event(e, &D.ev_done);
+        if (!ok) return CHD_ERR_CUDA;
+        for (ScanSite* site : {&D.site_arr, &D.site_dep, &D.site_enter, &D.site_leave}) site->error = &e->d_ctr->overflow;
+        // the empty snapshot: no entities, no cells populated, no slots
+        CU(e, cudaMemsetAsync(D.snap_hdr, 0, 8, e->stream));
+        CU(e, cudaMemsetAsync(D.snap_cell_start, 0, (C + 2) * 4, e->stream));
+        CU(e, cudaMemsetAsync(D.snap_pair_off, 0, (S + 1) * 4, e->stream));
+        CU(e, cudaStreamSynchronize(0));  // (chd_make_site clears its descriptors on the default stream)
+        D.on = true;
+    }
+    if (!ensure_cap(e, &D.enter, &D.enter_cap, cap_entries, cap_entries) || !ensure_cap(e, &D.leave, &D.leave_cap, cap_entries, cap_entries))
+        return CHD_ERR_CUDA;
+    // the lists of the last delta are gone (a grown buffer starts empty): report an empty delta until the next one
+    CU(e, cudaMemsetAsync(D.enter_off, 0, (S + 1) * 8, e->stream));
+    CU(e, cudaMemsetAsync(D.leave_off, 0, (S + 1) * 8, e->stream));
+    CU(e, cudaStreamSynchronize(e->stream));
+    return CHD_OK;
+}
+
+chd_status chd_visible_delta(chd_engine* e) {
+    if (!e) return CHD_ERR_INVALID;
+    chd_status st = chd_delta_check(e, false);
+    if (st != CHD_OK) return st;
+    CU(e, cudaSetDevice(e->device));
+    st = chd_fetch_guard(e, e->stream);
+    return st != CHD_OK ? st : chd_delta_on(e, e->stream);
+}
+
+chd_status chd_get_visible_delta(chd_engine* e, uint64_t* enter_off, uint32_t* enter_entity, uint64_t* leave_off, uint32_t* leave_entity,
+                                 uint64_t cap, uint64_t* n_entered, uint64_t* n_left, uint32_t* n_slots) {
+    if (!e) return CHD_ERR_INVALID;
+    chd_engine::Delta& D = e->dl;
+    if (!D.on) {
+        e->fail("chd_get_visible_delta before chd_reserve_visible_delta");
+        return CHD_ERR_STATE;
+    }
+    CU(e, cudaSetDevice(e->device));
+    cudaStream_t s = e->stream;  // (a tick's delta on prep_stream is joined into the engine stream)
+    const uint32_t S = D.n_out;
+    uint64_t* h64 = (uint64_t*)e->h_get;
+    CU(e, cudaMemcpyAsync(h64, D.enter_off + S, 8, cudaMemcpyDeviceToHost, s));
+    CU(e, cudaMemcpyAsync(h64 + 1, D.leave_off + S, 8, cudaMemcpyDeviceToHost, s));
+    CU(e, cudaStreamSynchronize(s));
+    const uint64_t ne = h64[0], nl = h64[1];
+    if (n_entered) *n_entered = ne;
+    if (n_left) *n_left = nl;
+    if (n_slots) *n_slots = S;
+    if (enter_off) CU(e, cudaMemcpyAsync(enter_off, D.enter_off, 8ull * (S + 1ull), cudaMemcpyDefault, s));
+    if (leave_off) CU(e, cudaMemcpyAsync(leave_off, D.leave_off, 8ull * (S + 1ull), cudaMemcpyDefault, s));
+    if (enter_entity || leave_entity) {
+        if (ne > D.enter_cap || nl > D.leave_cap) {
+            CU(e, cudaStreamSynchronize(s));
+            e->fail("the last visible delta overflowed (CHD_OVF_DELTA): %llu entered / %llu left > capacity %llu",
+                    (unsigned long long)ne, (unsigned long long)nl, (unsigned long long)std::min(D.enter_cap, D.leave_cap));
+            return CHD_ERR_CAPACITY;
+        }
+        if ((enter_entity && ne > cap) || (leave_entity && nl > cap)) {
+            CU(e, cudaStreamSynchronize(s));
+            e->fail("chd_get_visible_delta: %llu entered / %llu left > cap %llu", (unsigned long long)ne, (unsigned long long)nl,
+                    (unsigned long long)cap);
+            return CHD_ERR_CAPACITY;
+        }
+        if (enter_entity && ne) CU(e, cudaMemcpyAsync(enter_entity, D.enter, 4ull * ne, cudaMemcpyDefault, s));
+        if (leave_entity && nl) CU(e, cudaMemcpyAsync(leave_entity, D.leave, 4ull * nl, cudaMemcpyDefault, s));
+    }
+    CU(e, cudaStreamSynchronize(s));
+    return CHD_OK;
+}
+}  // extern "C"

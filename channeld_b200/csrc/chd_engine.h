@@ -105,7 +105,7 @@ struct chd_engine {
     // one look-back scan site per call site: stages run concurrently on two streams and must not share scan state
     unsigned long long* d_epoch = nullptr;  // [EP_COUNT] stage epochs for the look-back scans
     ScanSite site_hist_b{}, site_pchist_b{}, site_hist{}, site_qoff{}, site_slot{}, site_pchist{}, site_voff{}, site_border{};
-    uint64_t stage_execs[8] = {};
+    uint64_t stage_execs[9] = {};  // [EP_COUNT]
     std::vector<ScanSite*> sites;  // every scan site (chd_make_site registers them)
     uint32_t build_blocks = 0;
     bool assigned = false, built = false, have_prev_key = false, entities_dirty = false;
@@ -271,6 +271,23 @@ struct chd_engine {
     // scratch of the tick driver's getters (chd_get_visible*, export counts): separate from h_u32, which the stateless entry
     // points use under the engine mutex from other threads
     uint32_t* h_get = nullptr;
+    // ---- visible-set deltas (chd_delta.cu): everything is allocated by the first chd_reserve_visible_delta
+    struct Delta {
+        bool on = false;
+        uint32_t *snap_key = nullptr, *snap_cell_start = nullptr, *snap_sorted = nullptr, *snap_pair_off = nullptr, *snap_pair_cell = nullptr;
+        uint32_t* snap_hdr = nullptr;  // [0] entity count, [1] slot count of the snapshot
+        uint32_t *arr_rank = nullptr, *dep_rank = nullptr, *arr = nullptr, *dep = nullptr, *arr_start = nullptr, *dep_start = nullptr;
+        uint32_t *cnt_enter = nullptr, *cnt_leave = nullptr;
+        uint64_t *enter_off = nullptr, *leave_off = nullptr;
+        uint32_t *enter = nullptr, *leave = nullptr;
+        uint64_t enter_cap = 0, leave_cap = 0;
+        uint32_t n_out = 0;  // slots the output CSRs cover: max(slots now, slots at any earlier delta) (never shrinks)
+        ScanSite site_arr{}, site_dep{}, site_enter{}, site_leave{};
+        GraphSlot g[4];  // [key buffer][pair-buffer parity]
+        cudaEvent_t ev_in = nullptr, ev_done = nullptr;  // two-stream tick: the build is done / the delta is done
+        bool done_recorded = false;  // the last tick ran the delta off the engine stream: its end (and CHD_OVF_DELTA) is ev_done
+    } dl;
+    bool delta_blocked = false;  // chd_set_slab / chd_set_entity_ids were used: halo indices are not stable, no deltas
 
     bool fail(const char* fmt, ...) const {
         char buf[512];
@@ -364,7 +381,8 @@ static inline bool alloc_qstage(chd_engine* e, chd_engine::QStage& qs) {
            dalloc(e, &qs.spot_x, SP) && dalloc(e, &qs.spot_z, SP) && dalloc(e, &qs.spot_dist, SP);
 }
 
-enum { EP_BUILD = 0, EP_QUERY, EP_EMIT, EP_FANOUT, EP_BORDER, EP_BCAST, EP_CLASS, EP_PAYLOAD, EP_COUNT };  // d_epoch has 8 slots
+enum { EP_BUILD = 0, EP_QUERY, EP_EMIT, EP_FANOUT, EP_BORDER, EP_BCAST, EP_CLASS, EP_PAYLOAD, EP_DELTA, EP_COUNT };  // d_epoch has EP_COUNT slots
+static_assert(EP_COUNT == sizeof(chd_engine::stage_execs) / sizeof(uint64_t), "one execution counter per stage epoch");
 
 // ---- helpers shared by the translation units (C linkage only so that definitions may sit inside their extern "C" blocks)
 extern "C" {
@@ -396,6 +414,9 @@ RingDev chd_ring_view(const chd_engine* e);
 chd_status chd_sort_pass_any(chd_engine* e, cudaStream_t s, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in, uint32_t n,
                              const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits, uint32_t* key_out,
                              uint32_t* val_out, ScatterExtras ex = ScatterExtras{0, nullptr, 0, nullptr}, unsigned long long* bump = nullptr);
+// visible-set delta (chd_delta.cu): whether one may run now (will_build: the caller builds first), and the stage itself on `s`
+chd_status chd_delta_check(chd_engine* e, bool will_build);
+chd_status chd_delta_on(chd_engine* e, cudaStream_t s);
 }
 
 // Grow-on-demand buffer: when `need` elements exceed `*cap`, the buffer is replaced (contents not kept) by one of `count`

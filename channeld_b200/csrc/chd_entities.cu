@@ -237,6 +237,7 @@ chd_status chd_set_entity_count(chd_engine* e, uint32_t n) {
 chd_status chd_set_entity_ids(chd_engine* e, const uint32_t* gid, uint32_t n) {
     if (!e || n > e->lim.max_entities) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    e->delta_blocked = true;  // global ids: the multi-GPU flow (chd_visible_delta is single-GPU only)
     if (!gid) {
         e->have_gid = false;
         return CHD_OK;

@@ -202,6 +202,7 @@ chd_status chd_fetch_results(chd_engine* e, const chd_result_buffers* b, chd_tic
         // The tick is probably still running.  Read back on a separate stream, in the order in which results become final:
         //   phase A  after the interest fill (ev_pairs) and the build: pairs, interest diff, query statuses, handover list, cell CSR
         //   phase B  after the aux chain (ev_join: fan-out) and the emit preparation (ev_prep_done): due list, visible offsets
+        //            (and after the visible delta of a CHD_TICK_VISIBLE_DELTA tick: the counters carry its overflow bit)
         // while the emit kernel is still writing the expanded list.
         CU(e, cudaSetDevice(e->device));
         s = e->dl_stream;
@@ -266,6 +267,7 @@ chd_status chd_fetch_results(chd_engine* e, const chd_result_buffers* b, chd_tic
         s = e->dl_stream_b;
         CU(e, cudaStreamWaitEvent(s, e->ev_join, 0));
         CU(e, cudaStreamWaitEvent(s, e->ev_prep_done, 0));
+        if (e->dl.done_recorded) CU(e, cudaStreamWaitEvent(s, e->dl.ev_done, 0));  // the visible delta (its overflow bit)
         CU(e, cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
         CU(e, cudaStreamSynchronize(s));  // sync B
         st = chd_decode_summary(e, summary);
@@ -415,6 +417,7 @@ chd_status chd_fetch_results_async(chd_engine* e, const chd_result_buffers* b, v
     }
     CU(e, cudaStreamWaitEvent(sb, e->ev_join, 0));
     CU(e, cudaStreamWaitEvent(sb, e->ev_prep_done, 0));
+    if (e->dl.done_recorded) CU(e, cudaStreamWaitEvent(sb, e->dl.ev_done, 0));  // the visible delta (its overflow bit)
     pack_kernel<<<dim3(24, (unsigned)B.n), 256, 0, sb>>>(B);
     KCHECK(e);
     CU(e, cudaEventRecord(e->ev_fetch_b[fi], sb));
@@ -468,7 +471,15 @@ chd_status chd_device_view(chd_engine* e, int which, void** d_ptr, uint64_t* cou
         case CHD_VIEW_VIS_OFF: p = e->d_vis_off; c = (uint64_t)e->n_slots + 1; break;
         case CHD_VIEW_VIS_ENTITY: p = e->d_vis; c = e->lim.max_visible; break;
         case CHD_VIEW_DUE: p = e->d_due; c = e->lim.max_due; break;
+        case CHD_VIEW_DELTA_ENTER_OFF: p = e->dl.enter_off; c = (uint64_t)e->dl.n_out + 1; break;
+        case CHD_VIEW_DELTA_ENTER: p = e->dl.enter; c = e->dl.enter_cap; break;
+        case CHD_VIEW_DELTA_LEAVE_OFF: p = e->dl.leave_off; c = (uint64_t)e->dl.n_out + 1; break;
+        case CHD_VIEW_DELTA_LEAVE: p = e->dl.leave; c = e->dl.leave_cap; break;
         default: return CHD_ERR_INVALID;
+    }
+    if (which >= CHD_VIEW_DELTA_ENTER_OFF && !e->dl.on) {
+        e->fail("chd_device_view: no visible delta before chd_reserve_visible_delta");
+        return CHD_ERR_STATE;
     }
     *d_ptr = p;
     if (count) *count = c;

@@ -66,6 +66,7 @@ chd_status chd_set_slab(chd_engine* e, uint32_t col_lo, uint32_t col_hi, uint32_
     e->g.col_hi = col_hi;
     e->g.halo = halo;
     e->halo_on_device = false;  // set again by chd_import_halo
+    e->delta_blocked = true;
     return CHD_OK;
 }
 

@@ -463,12 +463,18 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
     const bool need_build = (flags & CHD_TICK_BUILD) && (e->entities_dirty || !e->built);
     const bool do_emit = flags & CHD_TICK_EMIT;
     const bool do_fanout = flags & CHD_TICK_FANOUT;
+    const bool do_delta = flags & CHD_TICK_VISIBLE_DELTA;
     const bool started = e->interest_pending;  // the aux chain of this tick was started by chd_begin_interest
     e->early_ready = false;
     e->build_done_recorded = false;
+    e->dl.done_recorded = false;
     if (started && q) {
         e->fail("chd_tick: a query batch was given while chd_begin_interest is pending");
         return CHD_ERR_STATE;
+    }
+    if (do_delta) {
+        st = chd_delta_check(e, need_build);
+        if (st != CHD_OK) return st;
     }
     if (!started && !((q || do_fanout) && (need_build || do_emit))) {
         if (need_build) {
@@ -487,7 +493,7 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
             st = fanout_enqueue(e, s, t_ns);
             if (st != CHD_OK) return st;
         }
-        return CHD_OK;
+        return do_delta ? chd_delta_on(e, s) : CHD_OK;
     }
     if (!started) {
         st = aux_chain_enqueue(e, s, q, q != nullptr, t_ns, do_fanout);
@@ -501,11 +507,24 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
         CU(e, cudaEventRecord(e->ev_build_done, s));
         e->build_done_recorded = true;
     }
+    if (do_delta) CU(e, cudaEventRecord(e->dl.ev_in, s));  // the cell CSR and keys of this tick (or of the last build) are final
     if (do_emit) {
         // the preparation waits for the new pairs (for the fork when this tick updates no interest); CHD_TICK_EARLY_RESULTS: the
         // copy kernel starts after the whole aux chain, so every host-facing result is final while it is still streaming
         st = emit_enqueue(e, s, (started || q) ? e->ev_pairs : e->ev_interest, (flags & CHD_TICK_EARLY_RESULTS) ? e->ev_join : nullptr);
         if (st != CHD_OK) return st;
+    }
+    if (do_delta) {
+        // latency-bound: on prep_stream (after the emit preparation), next to the expanded-list kernel and the aux chain; it needs
+        // the build and the new pairs, and the engine stream waits for it
+        const cudaStream_t ds = e->prep_stream;
+        CU(e, cudaStreamWaitEvent(ds, e->dl.ev_in, 0));
+        if (started || q) CU(e, cudaStreamWaitEvent(ds, e->ev_pairs, 0));
+        st = chd_delta_on(e, ds);
+        if (st != CHD_OK) return st;
+        CU(e, cudaEventRecord(e->dl.ev_done, ds));
+        e->dl.done_recorded = true;  // the early read-back's counters wait for it (CHD_OVF_DELTA belongs to this tick's summary)
+        CU(e, cudaStreamWaitEvent(s, e->dl.ev_done, 0));
     }
     CU(e, cudaStreamWaitEvent(s, e->ev_join, 0));
     if (do_fanout && !fanout_done) {

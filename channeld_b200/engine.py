@@ -340,6 +340,27 @@ class Engine:
         self._ck(self.L.chd_adjacent_broadcast(self.h, C.byref(b), ptr(status), ptr(off), ptr(slot), cap))
         return status, off, slot[:off[-1]]
 
+    # ---- visible-set deltas (entered / left entities per subscriber slot since the last successful delta)
+    def reserve_visible_delta(self, cap_entries):
+        self._ck(self.L.chd_reserve_visible_delta(self.h, int(cap_entries)))
+
+    def visible_delta(self):
+        self._ck(self.L.chd_visible_delta(self.h))
+
+    def visible_delta_counts(self):
+        """-> (n_entered, n_left, n_slots) of the last delta (the required sizes when it overflowed)."""
+        ne, nl, ns = C.c_uint64(), C.c_uint64(), C.c_uint32()
+        self._ck(self.L.chd_get_visible_delta(self.h, None, None, None, None, 0, C.byref(ne), C.byref(nl), C.byref(ns)))
+        return ne.value, nl.value, ns.value
+
+    def get_visible_delta(self):
+        """-> (enter_off[n+1] u64, enter u32, leave_off[n+1] u64, leave u32), n = slots the delta covers."""
+        ne, nl, ns = self.visible_delta_counts()
+        eo, lo = np.zeros(ns + 1, np.uint64), np.zeros(ns + 1, np.uint64)
+        en, le = np.zeros(max(ne, 1), np.uint32), np.zeros(max(nl, 1), np.uint32)
+        self._ck(self.L.chd_get_visible_delta(self.h, ptr(eo), ptr(en), ptr(lo), ptr(le), max(ne, nl, 1), None, None, None))
+        return eo, en[:ne], lo, le[:nl]
+
     def device_view(self, which):
         p, n = C.c_void_p(), C.c_uint64()
         self._ck(self.L.chd_device_view(self.h, which, C.byref(p), C.byref(n)))

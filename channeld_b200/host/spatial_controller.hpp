@@ -3,6 +3,7 @@
 // error behaviour follow the Go interface: Go's `(value, error)` becomes `value` + SpatialError thrown.
 // No hot-path arithmetic lives here: every position -> cell, query and fan-out decision is a libchd_b200.so call.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <map>
 #include <optional>
@@ -253,6 +254,30 @@ class GpuStaticGrid2DSpatialController {
         check(chd_due_classes(engine_, r.class_of.data(), r.rep.data(), r.count.data(), (uint32_t)r.rep.size(), &n));
         r.rep.resize(n);
         r.count.resize(n);
+        return r;
+    }
+
+    // Entities each client should spawn / despawn since the last visible delta (a tick with CHD_TICK_VISIBLE_DELTA, after
+    // chd_reserve_visible_delta): CSR by subscriber slot of entity indices, in visible-list order.
+    struct VisibleDelta {
+        std::vector<uint64_t> enter_off, leave_off;
+        std::vector<uint32_t> enter, leave;
+    };
+    // once before the first tick with CHD_TICK_VISIBLE_DELTA, and again (larger) after CHD_OVF_DELTA
+    void ReserveVisibleDelta(uint64_t cap_entries) { check(chd_reserve_visible_delta(engine_, cap_entries)); }
+    VisibleDelta GetVisibleDelta() {
+        VisibleDelta r;
+        uint64_t ne = 0, nl = 0;
+        uint32_t slots = 0;
+        check(chd_get_visible_delta(engine_, nullptr, nullptr, nullptr, nullptr, 0, &ne, &nl, &slots));
+        r.enter_off.resize((size_t)slots + 1);
+        r.leave_off.resize((size_t)slots + 1);
+        r.enter.resize(ne ? ne : 1);
+        r.leave.resize(nl ? nl : 1);
+        check(chd_get_visible_delta(engine_, r.enter_off.data(), r.enter.data(), r.leave_off.data(), r.leave.data(), std::max<uint64_t>({ne, nl, 1}),
+                                    nullptr, nullptr, nullptr));
+        r.enter.resize(ne);
+        r.leave.resize(nl);
         return r;
     }
 

@@ -404,6 +404,36 @@ func (ctl *GpuStaticGrid2DSpatialController) DueClasses(nDue int) (classOf, rep,
 	return classOf, rep[:n], count[:n], nil
 }
 
+// VisibleDelta returns, per subscriber slot, the entity indices to spawn (enter) and despawn (leave) since the last visible
+// delta: the net effect of the FULL data a new subscription sends, the despawns of an unsubscription and the handovers between
+// cells (spatial.go:612-858).  Call ReserveVisibleDelta once, then tick with CHD_TICK_VISIBLE_DELTA.  UN-RUN like the rest
+// of this file.
+func (ctl *GpuStaticGrid2DSpatialController) ReserveVisibleDelta(capEntries uint64) error {
+	if st := C.chd_reserve_visible_delta(ctl.engine, C.uint64_t(capEntries)); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
+func (ctl *GpuStaticGrid2DSpatialController) VisibleDelta() (enterOff []uint64, enter []uint32, leaveOff []uint64, leave []uint32, err error) {
+	var ne, nl C.uint64_t
+	var slots C.uint32_t
+	if st := C.chd_get_visible_delta(ctl.engine, nil, nil, nil, nil, 0, &ne, &nl, &slots); st != C.CHD_OK {
+		return nil, nil, nil, nil, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	enterOff, leaveOff = make([]uint64, int(slots)+1), make([]uint64, int(slots)+1)
+	enter, leave = make([]uint32, int(ne)+1), make([]uint32, int(nl)+1)
+	capEntries := ne
+	if nl > capEntries {
+		capEntries = nl
+	}
+	if st := C.chd_get_visible_delta(ctl.engine, (*C.uint64_t)(unsafe.Pointer(&enterOff[0])), (*C.uint32_t)(unsafe.Pointer(&enter[0])),
+		(*C.uint64_t)(unsafe.Pointer(&leaveOff[0])), (*C.uint32_t)(unsafe.Pointer(&leave[0])), capEntries+1, nil, nil, nil); st != C.CHD_OK {
+		return nil, nil, nil, nil, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return enterOff, enter[:ne], leaveOff, leave[:nl], nil
+}
+
 // PinnedFloat64s / PinnedUint32s / PinnedInt64s / PinnedUint64s carve staging slices out of page-locked C memory
 // (chd_alloc_pinned): uploads from them are truly asynchronous and, being C memory, they may be referenced by the
 // engine after a cgo call has returned (PrefetchTick).  Release with FreePinned(unsafe.Pointer(&s[0])).

@@ -282,7 +282,8 @@ typedef struct chd_tick_summary {
  *                   chd_fanout_tick); the list holds the decisions that did fit plus CHD_DUE_VOID holes; required_due
  *   CHD_OVF_BORDER  multi-GPU border / halo capacity exceeded: this tick's halo is incomplete */
 enum { CHD_OVF_PAIRS = 1, CHD_OVF_WINDOW = 2, CHD_OVF_VISIBLE = 4, CHD_OVF_DUE = 8, CHD_OVF_BORDER = 16,
-       CHD_OVF_RING = 32 /* a device-owned ring slab was full of live entries: its oldest entry was dropped */ };
+       CHD_OVF_RING = 32, /* a device-owned ring slab was full of live entries: its oldest entry was dropped */
+       CHD_OVF_DELTA = 64 /* the visible-set delta did not fit chd_reserve_visible_delta's capacity: see chd_visible_delta */ };
 /* bit 31: a device-side wait timed out (results invalid, please report).  A macro, not an enumerator: ISO C enumerators
  * must fit an int. */
 #define CHD_OVF_INTERNAL 0x80000000u
@@ -301,7 +302,10 @@ enum {
     /* The host will read this tick's results back (chd_fetch_results): start the expanded-list kernel only after the
      * fan-out pass (it would otherwise starve it of SM slots), so that every host-facing result is final, and is copied
      * to the host, while that kernel is still running.  Costs ~0.06 ms of device time per tick; results are identical. */
-    CHD_TICK_EARLY_RESULTS = 8
+    CHD_TICK_EARLY_RESULTS = 8,
+    /* Run chd_visible_delta after the build and the interest update (with or without CHD_TICK_EMIT).  In a two-stream tick it
+     * runs on a third stream next to the expanded-list kernel and the fan-out pass; the engine stream waits for it. */
+    CHD_TICK_VISIBLE_DELTA = 16
 };
 /* Optional early start: the interest update (and the fan-out pass when with_fanout != 0) do not depend on the entity
  * positions, so a host can start them as soon as the tick's queries and rings are known — on the engine's second
@@ -335,11 +339,45 @@ chd_status chd_get_due(chd_engine* e, chd_due* out, uint32_t cap);
 /* handover candidates of the last build: entity, src channel id, dst channel id (0 = left/entered the world) */
 chd_status chd_get_handover(chd_engine* e, uint32_t* entity, uint32_t* src_channel, uint32_t* dst_channel, uint32_t cap);
 
+/* ---- visible-set deltas: which entities each subscriber slot should spawn / despawn, without reading the expanded lists back.
+ * visible(s) is as for chd_emit_visible: the entities whose current cell is one of slot s's subscribed cells.  For every slot s
+ *     entered(s) = visible_now(s) \ visible_snap(s)        left(s) = visible_snap(s) \ visible_now(s)
+ * where "snap" is the engine state at the last delta that succeeded (before the first one every set is empty, so the first
+ * delta enters the full visible lists).  A delta is measured against that snapshot, not against the previous tick: ticks run
+ * without CHD_TICK_VISIBLE_DELTA, standalone chd_build / chd_update_interest calls and the subscriber lifecycle calls all fold
+ * into the next delta.  So a removed slot (chd_remove_subscribers, chd_set_subscribers) leaves everything it saw, an added slot
+ * enters what its first query makes visible, and a failed query (CHD_Q_ERR_*) changes nothing for its slot.
+ * "now" is the state of the last chd_build and the current subscriptions; CHD_ERR_STATE if chd_assign_cells ran after that build.
+ * Entity identity is the entity index.  An index at or above the entity count of a state, or outside the world in it (NaN-parked
+ * slots included), is absent from that state: appended spawns, a shrunk array and parked slots come out as enter / leave.  An
+ * index reused for a different entity between two deltas is invisible to the engine: the host despawns / spawns it itself.
+ * Order: entered(s) by (current cell asc, entity asc), left(s) by (snapshot cell asc, entity asc): the order of the visible
+ * lists, so results are deterministic.
+ *   chd_reserve_visible_delta  allocates the snapshot (about 8 bytes per entity of capacity) on the first call, which enables the
+ *                              feature, and grows both output lists to cap_entries entries each.  Synchronous, not on the tick path;
+ *                              the last delta's lists are discarded (they read as empty until the next delta).
+ *   chd_visible_delta          computes the delta and advances the snapshot.  Stream-ordered, no host synchronisation.  If a list
+ *                              needs more than the reserved capacity, CHD_OVF_DELTA is raised, nothing is written and the snapshot
+ *                              is NOT advanced: after chd_reserve_visible_delta with the reported counts, the next delta covers
+ *                              everything since the last successful one.
+ *   chd_get_visible_delta      copies the last delta: enter_off / leave_off [*n_slots + 1] (u64 CSR by slot), the entities
+ *                              [cap] each; n_entered / n_left = list lengths (also after an overflow: the required sizes).
+ *                              *n_slots = max(slots now, slots at any earlier delta): slots dropped by chd_set_subscribers still
+ *                              report what they left.  Synchronous; any pointer may be NULL; CHD_ERR_CAPACITY if a requested list
+ *                              does not fit cap or the last delta overflowed.
+ * Single-GPU only: CHD_ERR_STATE on an engine that has used chd_set_slab, chd_set_entity_ids or chd_comm_init (halo entity indices
+ * are not stable from tick to tick there). */
+chd_status chd_reserve_visible_delta(chd_engine* e, uint64_t cap_entries);
+chd_status chd_visible_delta(chd_engine* e);
+chd_status chd_get_visible_delta(chd_engine* e, uint64_t* enter_off, uint32_t* enter_entity, uint64_t* leave_off, uint32_t* leave_entity,
+                                 uint64_t cap, uint64_t* n_entered, uint64_t* n_left, uint32_t* n_slots);
+
 /* ---- all host-facing results of a tick in ONE call instead of one or two synchronisations per getter.  After a
  * two-stream tick (chd_tick with emit, or chd_begin_interest + chd_tick) the lists are copied in the order they become
  * final, on the engine's read-back streams, while the expanded-list kernel may still be running: first the pairs /
  * sub-unsub lists / query statuses / handover list / cell CSR (after the interest fill and the build), then the due list
- * and the visible offsets (after the fan-out pass and the emit preparation; see CHD_TICK_EARLY_RESULTS); the call returns
+ * and the visible offsets (after the fan-out pass, the emit preparation and, with CHD_TICK_VISIBLE_DELTA, the delta, whose
+ * CHD_OVF_DELTA belongs to this summary; see CHD_TICK_EARLY_RESULTS); the call returns
  * when the tick has finished.  Otherwise: waits for the tick, reads the summary, enqueues every copy, waits once.
  * Exact sizes come from the device counters.  Any pointer may be NULL (skipped).  Capacities are in elements; CHD_ERR_CAPACITY if a requested list does not
  * fit (nothing is truncated silently).  This is what a channeld host calls once per tick. */
@@ -379,7 +417,9 @@ chd_status chd_fetch_wait(chd_engine* e, chd_tick_summary* summary);
 /* Device-resident views (valid until the next call that rewrites them) for consumers that stay on the GPU. */
 enum {
     CHD_VIEW_CELL_START = 0, CHD_VIEW_SORTED_ENTITY, CHD_VIEW_ENT_CELL, CHD_VIEW_PAIR_OFF, CHD_VIEW_PAIR_CHANNEL,
-    CHD_VIEW_PAIR_DIST, CHD_VIEW_VIS_OFF, CHD_VIEW_VIS_ENTITY, CHD_VIEW_DUE
+    CHD_VIEW_PAIR_DIST, CHD_VIEW_VIS_OFF, CHD_VIEW_VIS_ENTITY, CHD_VIEW_DUE,
+    /* the visible-set delta (chd_visible_delta): u64 offsets [slots + 1] and u32 entities [capacity] of each list */
+    CHD_VIEW_DELTA_ENTER_OFF, CHD_VIEW_DELTA_ENTER, CHD_VIEW_DELTA_LEAVE_OFF, CHD_VIEW_DELTA_LEAVE
 };
 chd_status chd_device_view(chd_engine* e, int which, void** d_ptr, uint64_t* count);
 
@@ -533,6 +573,7 @@ uint32_t chd_damping_interval_ms(uint32_t dist, uint32_t default_ms);
 enum { CHD_STAGE_BUILD = 0, CHD_STAGE_INTEREST, CHD_STAGE_EMIT, CHD_STAGE_EMIT_KERNEL, CHD_STAGE_FANOUT, CHD_STAGE_TICK,
        CHD_STAGE_EXPORT, CHD_STAGE_EXCHANGE, CHD_STAGE_IMPORT, /* the three steps of chd_tick_sharded before the tick proper */
        CHD_STAGE_READBACK,                                     /* chd_fetch_results_async: the PCIe hop (snapshot -> pinned host) */
+       CHD_STAGE_VISIBLE_DELTA,                                /* chd_visible_delta / CHD_TICK_VISIBLE_DELTA */
        CHD_STAGE_COUNT };
 uint64_t chd_launch_count(const chd_engine* e);
 /* The launch-bound stages (build, interest update, emit preparation, fan-out) are replayed as CUDA graphs once
