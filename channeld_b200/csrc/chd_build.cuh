@@ -189,10 +189,6 @@ __global__ void __launch_bounds__(BUILD_THREADS)
                 const uint32_t dst = s_base[d] + s_wcnt[w][d] + rk[r];
                 val_out[dst] = v[r];
                 if (key_out) key_out[dst] = k[r];
-                if (ex.phase_stride) {
-#pragma unroll
-                    for (uint32_t ph = 1; ph < 4; ph++) val_out[(size_t)ph * ex.phase_stride + ph + dst] = v[r];
-                }
             }
         }
         __syncthreads();
@@ -299,10 +295,6 @@ __global__ void __launch_bounds__(BUILD_THREADS)
             const uint32_t dst = s_base[d] + (j - s_lofs[d]);
             val_out[dst] = s_val[j];
             if (key_out) key_out[dst] = kk;
-            if (ex.phase_stride) {
-#pragma unroll
-                for (uint32_t ph = 1; ph < 4; ph++) val_out[(size_t)ph * ex.phase_stride + ph + dst] = s_val[j];
-            }
         }
         __syncthreads();
         // advance the global bases by the tile's digit totals (= next digit's local offset - this digit's)
@@ -344,21 +336,6 @@ __global__ void __launch_bounds__(256)
         cell_start[c] = i;
         if (c == (int64_t)cells) *n_in_world = i;  // entities with a valid cell precede the key == cells tail
     }
-}
-
-// The cell CSR's entity array is kept in FOUR phase-shifted copies: copy k stores element i at index
-// k*stride + k + i (stride % 4 == 0), i.e. at 16-byte phase (k + i) % 4.  Output chunks are 16-byte aligned, so
-// for a run that starts at source index s the copy k = (-s) & 3 makes source and destination co-aligned and
-// the whole run moves as LDG.128 -> STG.128 with no realignment shuffles.  Cost: 12 extra bytes per entity
-// written once per build (L2-resident), against 8 bytes per VISIBLE entry saved from 4-byte accesses.
-__global__ void __launch_bounds__(256)
-    replicate_phases_kernel(const uint32_t* src, uint32_t n, const uint32_t* __restrict__ n_ptr, uint32_t stride, uint32_t* dst4) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (n_ptr) n = min(n, *n_ptr);
-    if (i >= n) return;
-    const uint32_t v = src[i];
-#pragma unroll
-    for (uint32_t k = 1; k < 4; k++) dst4[(size_t)k * stride + k + i] = v;  // copy 0 is src itself (dst4 == src)
 }
 
 // float -> double widening of a position upload (chd_set_entities_f32): channeld's entity positions arrive as unrealpb.FVector

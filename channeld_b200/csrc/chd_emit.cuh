@@ -4,8 +4,9 @@
 //
 // Decomposition: the OUTPUT array is cut into fixed tiles of EMIT_TILE entries (load-balanced regardless of
 // how entities are distributed over cells).  A partition pass records the first pair of each tile; one CTA copies one
-// tile.  Every thread moves 16-byte chunks: stores are fully coalesced; loads are co-aligned 16-byte reads out of the
-// L2-resident phase copies of the cell CSR (4 x 4 B x N: 16 MB at 1 M entities, a third of the H100's 50 MB L2).
+// tile.  Every thread moves 16-byte chunks: stores are fully coalesced; loads are aligned 16-byte reads of the cell CSR's
+// L2-resident sorted entity array (4 B x N: 4 MB at 1 M entities).  A chunk whose source starts m != 0 entries into an
+// aligned 16-byte chunk is funnelled out of that chunk and the next one (emit_funnel).
 #pragma once
 #include "chd_types.cuh"
 
@@ -56,7 +57,7 @@ __global__ void __launch_bounds__(256)
             const uint32_t tile_len = (uint32_t)min((uint64_t)tile, V - base);
             TileDesc d;
             d.p0 = (uint32_t)p;
-            d.src0 = cs + (uint32_t)(base - b);  // tile slot o <- sorted entity src0 + o (phase copy 0)
+            d.src0 = cs + (uint32_t)(base - b);  // tile slot o <- sorted entity src0 + o
             const uint32_t end0 = (uint32_t)min((uint64_t)tile, e - base);
             uint32_t end1 = end0;
             d.src1 = 0;
@@ -76,10 +77,20 @@ __global__ void __launch_bounds__(256)
     }
 }
 
+// 16 bytes of a list that starts m entries into chunk a and continues into chunk b
+__device__ __forceinline__ uint4 emit_funnel(uint4 a, uint4 b, uint32_t m) {
+    switch (m) {
+        case 1: return make_uint4(a.y, a.z, a.w, b.x);
+        case 2: return make_uint4(a.z, a.w, b.x, b.y);
+        case 3: return make_uint4(a.w, b.x, b.y, b.z);
+        default: return a;
+    }
+}
+
 // General path of one tile: more than two pairs' lists intersect it (cells smaller than a tile).
 __device__ __forceinline__ void emit_tile_general(uint64_t t, uint64_t n_tiles, uint64_t V, uint32_t p0, const uint32_t* __restrict__ n_pairs_ptr,
                                                uint64_t pair_cap, const uint64_t* __restrict__ voff, const uint32_t* __restrict__ pair_cell,
-                                               const uint32_t* __restrict__ cell_start, const uint32_t* __restrict__ sorted4, uint32_t stride,
+                                               const uint32_t* __restrict__ cell_start, const uint32_t* __restrict__ sorted,
                                                const uint32_t* __restrict__ first_pair, uint32_t* __restrict__ vis_entity, uint32_t* s_end,
                                                uint32_t* s_src) {
     const uint32_t tid = threadIdx.x;
@@ -110,14 +121,18 @@ __device__ __forceinline__ void emit_tile_general(uint64_t t, uint64_t n_tiles, 
             const uint32_t beg = k == 0 ? 0u : s_end[k - 1];
             const uint32_t sidx = s_src[k] + (o - beg);
             if (o + 4 <= s_end[k]) {
-                const uint32_t ph = (0u - sidx) & 3u;  // whole chunk inside one segment: phase copy (-sidx) & 3
-                __stcs(reinterpret_cast<uint4*>(out + o), __ldg(reinterpret_cast<const uint4*>(sorted4 + ph * stride + ph + sidx)));
+                // whole chunk inside one segment: the aligned chunk that holds sidx, and the next one if sidx is not aligned
+                // (no shuffle from the neighbouring lane here: a lane may have left the row loop above)
+                const uint4* q = reinterpret_cast<const uint4*>(sorted + (sidx & ~3u));
+                const uint32_t m = sidx & 3u;
+                const uint4 a = __ldg(q);
+                __stcs(reinterpret_cast<uint4*>(out + o), m ? emit_funnel(a, __ldg(q + 1), m) : a);
             } else {
                 uint32_t kk = k;  // the chunk straddles a segment boundary (or the end of the list): entry by entry
                 for (uint32_t j = 0; j < 4 && o + j < tile_len; j++) {
                     while (s_end[kk] <= o + j) kk++;
                     const uint32_t bb = kk == 0 ? 0u : s_end[kk - 1];
-                    out[o + j] = __ldg(sorted4 + s_src[kk] + (o + j - bb));
+                    out[o + j] = __ldg(sorted + s_src[kk] + (o + j - bb));
                 }
             }
         }
@@ -131,18 +146,8 @@ __device__ __forceinline__ void emit_tile_general(uint64_t t, uint64_t n_tiles, 
                 if (voff[mid] <= go) lo = mid; else hi = mid - 1;
             }
             const uint32_t c = pair_cell[lo];
-            vis_entity[go] = sorted4[cell_start[c] + (uint32_t)(go - voff[lo])];
+            vis_entity[go] = sorted[cell_start[c] + (uint32_t)(go - voff[lo])];
         }
-    }
-}
-
-// 16 bytes of a list that starts m entries into chunk a and continues into chunk b
-__device__ __forceinline__ uint4 emit_funnel(uint4 a, uint4 b, uint32_t m) {
-    switch (m) {
-        case 1: return make_uint4(a.y, a.z, a.w, b.x);
-        case 2: return make_uint4(a.z, a.w, b.x, b.y);
-        case 3: return make_uint4(a.w, b.x, b.y, b.z);
-        default: return a;
     }
 }
 
@@ -152,10 +157,9 @@ __device__ __forceinline__ uint4 emit_funnel(uint4 a, uint4 b, uint32_t m) {
 // {src0, src1, ends, p0}); tiles with more segments are listed by the partition pass and copied by
 // emit_visible_general_kernel.  The loop only runs more than once if the host under-estimated the tile count when it sized
 // the grid.
-// Sources are read from phase copy 0 alone (4 B x N: 4 MB at 1 M entities), not from the four phase copies: with the 16 MB
-// of all four the same kernel runs 25 % slower on an H100, the sources no longer staying in L2 next to the write stream.  A
-// chunk that starts m = src & 3 entries into an aligned 16-byte chunk a takes the rest from chunk a + 1, which the next lane
-// loaded already (shuffle); lane 31, and a lane whose neighbour reads elsewhere, loads it itself.
+// A chunk that starts m = src & 3 entries into an aligned 16-byte chunk a takes the rest from chunk a + 1, which the next lane
+// loaded already (shuffle); lane 31, and a lane whose neighbour reads elsewhere, loads it itself.  (Keeping the sources at
+// 4 B x N is what keeps them in L2 next to the write stream: with 16 B x N the same kernel ran 25 % slower, DESIGN §8.)
 __global__ void __launch_bounds__(EMIT_THREADS, CHD_EMIT_MIN_BLOCKS)
     emit_visible_kernel(const unsigned long long* __restrict__ n_visible_ptr, const uint32_t* __restrict__ sorted, const TileDesc* __restrict__ desc,
                         uint32_t* __restrict__ vis_entity, uint64_t vis_cap) {
@@ -187,7 +191,7 @@ __global__ void __launch_bounds__(EMIT_THREADS, CHD_EMIT_MIN_BLOCKS)
             if (in0 || in1) {
                 const uint4* q = reinterpret_cast<const uint4*>(sorted + (si[r] & ~3u));
                 va[r] = __ldg(q);
-                if (lane == 31 && (si[r] & 3u)) vb[r] = __ldg(q + 1);  // (in bounds: the copy is padded by 8 entries)
+                if (lane == 31 && (si[r] & 3u)) vb[r] = __ldg(q + 1);  // (in bounds: the array is padded by 8 entries)
                 whole |= 1u << r;
             }
         }
@@ -222,7 +226,7 @@ __global__ void __launch_bounds__(EMIT_THREADS)
     emit_visible_general_kernel(const uint32_t* __restrict__ general_tiles, uint32_t* __restrict__ n_general_ptr,
                                 const uint32_t* __restrict__ n_pairs_ptr, uint64_t pair_cap, const unsigned long long* __restrict__ n_visible_ptr,
                                 const uint64_t* __restrict__ voff, const uint32_t* __restrict__ pair_cell, const uint32_t* __restrict__ cell_start,
-                                const uint32_t* __restrict__ sorted4, uint32_t stride, const uint32_t* __restrict__ first_pair,
+                                const uint32_t* __restrict__ sorted, const uint32_t* __restrict__ first_pair,
                                 uint32_t* __restrict__ vis_entity, uint64_t vis_cap) {
     __shared__ uint32_t s_end[EMIT_SMEM_PAIRS];  // end of pair (p0+k) relative to the tile base, clamped to EMIT_TILE
     __shared__ uint32_t s_src[EMIT_SMEM_PAIRS];  // source index of the pair's entry that lands on max(voff[p], tile base)
@@ -244,19 +248,19 @@ __global__ void __launch_bounds__(EMIT_THREADS)
     const uint64_t n_tiles = (V + EMIT_TILE - 1) / EMIT_TILE;
     for (uint32_t i = blockIdx.x; i < n_general; i += gridDim.x) {
         const uint32_t t = general_tiles[i];
-        emit_tile_general(t, n_tiles, V, first_pair[t], n_pairs_ptr, pair_cap, voff, pair_cell, cell_start, sorted4, stride, first_pair, vis_entity, s_end, s_src);
+        emit_tile_general(t, n_tiles, V, first_pair[t], n_pairs_ptr, pair_cap, voff, pair_cell, cell_start, sorted, first_pair, vis_entity, s_end, s_src);
     }
 }
 
 
 // General kernel (round 1's shape): a persistent grid, every WARP owns whole 4 KB tiles (no block barrier anywhere), the segment
 // table of a tile lives in a warp-private slice of shared memory.  Used when cells are small against a CTA tile (many segments
-// per tile: config #5's 152 entities per cell) or when the CSR payload does not fit the L2 (config #3: the copy is then DRAM-bound
-// on both sides).
+// per tile: config #5's 152 entities per cell) and for worlds above the CTA kernel's size bound (config #3's 10 M entities,
+// emit_uses_cta_tiles).
 __global__ void __launch_bounds__(EMIT_THREADS, 4)
     emit_visible_warp_kernel(const uint32_t* __restrict__ n_pairs_ptr, uint64_t pair_cap, const uint64_t* __restrict__ voff,
                         const uint32_t* __restrict__ pair_cell, const uint32_t* __restrict__ cell_start,
-                        const uint32_t* __restrict__ sorted4, uint32_t stride, const uint32_t* __restrict__ first_pair,
+                        const uint32_t* __restrict__ sorted, const uint32_t* __restrict__ first_pair,
                         uint32_t* __restrict__ vis_entity, uint64_t vis_cap) {
     __shared__ uint32_t s_end_all[EMIT_WARP_WARPS][EMIT_WARP_SMEM_PAIRS];  // end of pair (p0+k) relative to the tile base, clamped to EMIT_WARP_TILE
     __shared__ uint32_t s_src_all[EMIT_WARP_WARPS][EMIT_WARP_SMEM_PAIRS];  // source index of the pair's entry that lands on max(voff[p], tile base)
@@ -286,8 +290,8 @@ __global__ void __launch_bounds__(EMIT_THREADS, 4)
             }
             __syncwarp();
             uint32_t k = 0;  // segment cursor of this lane (its chunks ascend)
-            uint32_t src[EMIT_WARP_CHUNKS];  // element index into sorted4 (multiple of 4), or 0xFFFFFFFF
-            // phase 1: resolve every chunk's source (nullptr = handled element-wise / out of range)
+            uint32_t src[EMIT_WARP_CHUNKS];  // index into sorted of the chunk's first entry, or 0xFFFFFFFF
+            // phase 1: resolve every chunk's source (0xFFFFFFFF = handled element-wise / out of range)
 #pragma unroll
             for (int it = 0; it < EMIT_WARP_CHUNKS; it++) {
                 const uint32_t o = (it * 32 + lane) * 4;  // first entry of this 16-byte chunk
@@ -297,28 +301,42 @@ __global__ void __launch_bounds__(EMIT_THREADS, 4)
                     const uint32_t beg = k == 0 ? 0u : s_end[k - 1];
                     const uint32_t sidx = s_src[k] + (o - beg);
                     if (o + 4 <= s_end[k]) {
-                        // whole chunk inside one segment: co-aligned 16-byte move out of phase copy (-sidx)&3
-                        const uint32_t ph = (0u - sidx) & 3u;
-                        src[it] = ph * stride + ph + sidx;
+                        src[it] = sidx;  // whole chunk inside one segment
                     } else {
                         // the chunk straddles a segment boundary (or the end of the list): entry by entry
                         uint32_t kk = k;
                         for (uint32_t j = 0; j < 4 && o + j < tile_len; j++) {
                             while (s_end[kk] <= o + j) kk++;
                             const uint32_t bb = kk == 0 ? 0u : s_end[kk - 1];
-                            out[o + j] = __ldg(sorted4 + s_src[kk] + (o + j - bb));
+                            out[o + j] = __ldg(sorted + s_src[kk] + (o + j - bb));
                         }
                     }
                 }
             }
-            // phase 2: all loads in flight, phase 3: streaming stores
+            // phase 2: all loads in flight (the aligned chunk that holds each chunk's first entry)
             uint4 v[EMIT_WARP_CHUNKS];
 #pragma unroll
             for (int it = 0; it < EMIT_WARP_CHUNKS; it++)
-                if (src[it] != 0xFFFFFFFFu) v[it] = __ldg(reinterpret_cast<const uint4*>(sorted4 + src[it]));
+                if (src[it] != 0xFFFFFFFFu) v[it] = __ldg(reinterpret_cast<const uint4*>(sorted + (src[it] & ~3u)));
+            // phase 3: streaming stores.  A lane's chunks are chunk it * 32 + lane of the tile, so the aligned chunk after lane L's
+            // is the one lane L + 1 loaded in the same row, and after lane 31's the one lane 0 loaded in the next row (shuffle).
+            // The last row's lane 31, and a lane whose neighbour read another part of the array, load it themselves.
 #pragma unroll
-            for (int it = 0; it < EMIT_WARP_CHUNKS; it++)
-                if (src[it] != 0xFFFFFFFFu) __stcs(reinterpret_cast<uint4*>(out + (it * 32 + lane) * 4), v[it]);
+            for (int it = 0; it < EMIT_WARP_CHUNKS; it++) {
+                const int nx = it + 1 < EMIT_WARP_CHUNKS ? it + 1 : it;
+                const uint32_t from = (lane + 1) & 31;
+                const uint32_t ns = __shfl_sync(0xffffffffu, lane == 0 ? src[nx] : src[it], from);
+                const uint4 g = lane == 0 ? v[nx] : v[it];
+                const uint4 nb = make_uint4(__shfl_sync(0xffffffffu, g.x, from), __shfl_sync(0xffffffffu, g.y, from),
+                                            __shfl_sync(0xffffffffu, g.z, from), __shfl_sync(0xffffffffu, g.w, from));
+                const uint32_t s = src[it];
+                if (s == 0xFFFFFFFFu) continue;
+                const uint32_t m = s & 3u;
+                uint4 b = nb;
+                const bool shuffled = ns != 0xFFFFFFFFu && (ns & ~3u) == (s & ~3u) + 4 && (lane != 31 || it + 1 < EMIT_WARP_CHUNKS);
+                if (m && !shuffled) b = __ldg(reinterpret_cast<const uint4*>(sorted + (s & ~3u)) + 1);  // (in bounds: padded by 8 entries)
+                __stcs(reinterpret_cast<uint4*>(out + (it * 32 + lane) * 4), emit_funnel(v[it], b, m));
+            }
         } else {
             // more than EMIT_WARP_SMEM_PAIRS pairs inside one tile (tiny / empty cells): per-entry binary search
             for (uint32_t o = lane; o < tile_len; o += 32) {
@@ -329,7 +347,7 @@ __global__ void __launch_bounds__(EMIT_THREADS, 4)
                     if (voff[mid] <= go) lo = mid; else hi = mid - 1;
                 }
                 const uint32_t c = pair_cell[lo];
-                vis_entity[go] = sorted4[cell_start[c] + (uint32_t)(go - voff[lo])];
+                vis_entity[go] = sorted[cell_start[c] + (uint32_t)(go - voff[lo])];
             }
         }
     }

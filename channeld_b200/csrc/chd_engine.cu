@@ -230,7 +230,6 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
 
     const uint64_t N = L.max_entities, S = L.max_subscribers, Q = L.max_queries, P = L.max_pairs, C = g.cells;
     e->build_blocks = (uint32_t)e->sm_count * 4;
-    e->phase_stride = (uint32_t)(((N + 3) / 4) * 4 + 8);
     e->pc_blocks = (uint32_t)std::min<uint64_t>(4096, (P + BUILD_TILE - 1) / BUILD_TILE);
     if (e->pc_blocks == 0) e->pc_blocks = 1;
     e->ho_cap = L.max_entities;
@@ -249,7 +248,10 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     ok = ok && dalloc(e, &e->d_x, N) && dalloc(e, &e->d_z, N) && (e->d_xb[0] = e->d_x, e->d_zb[0] = e->d_z, true) &&
          dalloc(e, &e->d_gid, N) && dalloc(e, &e->d_key, N) &&
          dalloc(e, &e->d_prev_key, N) && dalloc(e, &e->d_tmp_key, N) && dalloc(e, &e->d_tmp_val, N) &&
-         dalloc(e, &e->d_sorted_key, N) && dalloc(e, &e->d_sorted4, 4 * (((N + 3) / 4) * 4 + 8)) && dalloc(e, &e->d_cell_start, C + 2) &&
+         dalloc(e, &e->d_sorted_key, N) &&
+         // padded: an emit chunk that starts m != 0 entries into an aligned 16-byte chunk also loads the next aligned chunk,
+         // which near the end of the array lies past N (chd_emit.cuh)
+         dalloc(e, &e->d_sorted_ent, ((N + 3) / 4) * 4 + 8) && dalloc(e, &e->d_cell_start, C + 2) &&
          dalloc(e, &e->d_hist, (uint64_t)BUILD_MAX_BINS * e->build_blocks + 2) &&
          dalloc(e, &e->d_epoch, EP_COUNT) && chd_init_epochs(e) &&
          chd_make_site(e, e->site_hist, (uint64_t)BUILD_MAX_BINS * e->build_blocks + 1, EP_BUILD) &&
@@ -259,7 +261,6 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
          chd_make_site(e, e->site_border, N + 1, EP_BORDER) &&
          dalloc(e, &e->d_ho_entity, N) && dalloc(e, &e->d_ho_src, N) && dalloc(e, &e->d_ho_dst, N) &&
          dalloc(e, &e->d_bflag, N + 1) && dalloc(e, &e->d_boff, N + 2);
-    e->d_sorted_ent = e->d_sorted4;  // phase copy 0 IS the plain sorted entity array
     e->d_key_a = e->d_key;
     ok = ok && dalloc(e, &e->d_conn, S) && dalloc(e, &e->d_slot_ctl, S) && dalloc(e, &e->d_slot_src, S) && dalloc(e, &e->d_lc_slot, S) &&
          dalloc(e, &e->d_lc_aux, S) && alloc_pairbuf(e, e->pairs[0]) && alloc_pairbuf(e, e->pairs[1]);

@@ -99,8 +99,6 @@ struct chd_engine {
     uint32_t *d_key = nullptr, *d_prev_key = nullptr;  // [max_entities] cell key per entity
     uint32_t *d_tmp_key = nullptr, *d_tmp_val = nullptr, *d_sorted_key = nullptr, *d_sorted_ent = nullptr;
     uint32_t *d_cell_start = nullptr;     // [C+2]
-    uint32_t *d_sorted4 = nullptr;        // 4 phase-shifted copies of d_sorted_ent (chd_emit.cuh), stride = phase_stride
-    uint32_t phase_stride = 0;
     uint32_t *d_hist = nullptr;           // [BUILD_MAX_BINS * nblocks + 1]
     // one look-back scan site per call site: stages run concurrently on two streams and must not share scan state
     unsigned long long* d_epoch = nullptr;  // [EP_COUNT] stage epochs for the look-back scans
@@ -413,7 +411,7 @@ RingDev chd_ring_view(const chd_engine* e);
 // one stable LSD radix pass (histogram, look-back scan, scatter) over 32-bit keys; chd_entities.cu
 chd_status chd_sort_pass_any(chd_engine* e, cudaStream_t s, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in, uint32_t n,
                              const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits, uint32_t* key_out,
-                             uint32_t* val_out, ScatterExtras ex = ScatterExtras{0, nullptr, 0, nullptr}, unsigned long long* bump = nullptr);
+                             uint32_t* val_out, ScatterExtras ex = ScatterExtras{nullptr, 0, nullptr}, unsigned long long* bump = nullptr);
 // visible-set delta (chd_delta.cu): whether one may run now (will_build: the caller builds first), and the stage itself on `s`
 chd_status chd_delta_check(chd_engine* e, bool will_build);
 chd_status chd_delta_on(chd_engine* e, cudaStream_t s);

@@ -1,4 +1,4 @@
-// chd_entities.cu — entity positions, GetChannelId per entity, spatial-hash build (cell CSR + phase copies).
+// chd_entities.cu — entity positions, GetChannelId per entity, spatial-hash build (cell CSR).
 #include "chd_engine.h"
 
 #include "chd_build.cuh"
@@ -304,8 +304,8 @@ chd_status chd_assign_cells_impl(chd_engine* e, cudaStream_t s) {
     return CHD_OK;
 }
 
-// part: 0 = the whole build; single-pass builds only: 1 = cell assignment + histogram + scan + CSR offsets, 2 = scatter (+ phase
-// copies).  The cell CSR offsets are final after part 1.
+// part: 0 = the whole build; single-pass builds only: 1 = cell assignment + histogram + scan + CSR offsets, 2 = scatter.  The
+// cell CSR offsets are final after part 1.
 static chd_status build_enqueue(chd_engine* e, cudaStream_t s, bool with_assign, int part = 0) {
     chd_status st;
     FusedAssign fa{};
@@ -343,13 +343,10 @@ static chd_status build_enqueue(chd_engine* e, cudaStream_t s, bool with_assign,
     uint32_t nblocks = (n + per_block - 1) / per_block;
     if (nblocks == 0) nblocks = 1;
     const uint32_t* vals = e->have_gid ? e->d_gid : nullptr;
-    // The scatters write no phase copies (ScatterExtras stride 0): a separate fully-coalesced pass writes them afterwards.  (Fusing
-    // them into the scatter saves a launch but does 4 scattered 4-byte stores per entity: measured slower at every size — 69 vs
-    // 59 us per build at N = 1 M, 325 vs 205 us at N = 10 M.)
     if (passes == 1 && part != 0) {
         if (part == 1) {
             st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent,
-                                 ScatterExtras{0, nullptr, C, nullptr}, e->d_epoch + EP_BUILD, fap, 1);
+                                 ScatterExtras{nullptr, C, nullptr}, e->d_epoch + EP_BUILD, fap, 1);
             if (st != CHD_OK) return st;
             publish_cell_start_kernel<<<blocks_for((uint64_t)C + 2, 256), 256, 0, s>>>(e->d_hist, nblocks, C, n, n_ptr, e->d_cell_start,
                                                                                          &e->d_ctr->n_entities_in_world);
@@ -357,27 +354,23 @@ static chd_status build_enqueue(chd_engine* e, cudaStream_t s, bool with_assign,
             return CHD_OK;
         }
         st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent,
-                             ScatterExtras{0, nullptr, C, nullptr}, nullptr, nullptr, 2);
+                             ScatterExtras{nullptr, C, nullptr}, nullptr, nullptr, 2);
         if (st != CHD_OK) return st;
     } else if (passes == 1) {
         // single pass: digit == key, so the scatter also publishes the CSR offsets
-        ScatterExtras ex{0, e->d_cell_start, C, &e->d_ctr->n_entities_in_world};
+        ScatterExtras ex{e->d_cell_start, C, &e->d_ctr->n_entities_in_world};
         st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent, ex,
                              e->d_epoch + EP_BUILD, fap);
         if (st != CHD_OK) return st;
     } else {
         st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, e->d_tmp_key, e->d_tmp_val,
-                             ScatterExtras{0, nullptr, 0, nullptr}, e->d_epoch + EP_BUILD, fap);
+                             ScatterExtras{nullptr, 0, nullptr}, e->d_epoch + EP_BUILD, fap);
         if (st != CHD_OK) return st;
         st = chd_sort_pass_any(e, s, e->d_hist, e->site_hist_b, e->d_tmp_key, e->d_tmp_val, n, n_ptr, per_block, nblocks, bits0, bits1, e->d_sorted_key,
-                               e->d_sorted_ent, ScatterExtras{0, nullptr, C, nullptr});
+                               e->d_sorted_ent, ScatterExtras{nullptr, C, nullptr});
         if (st != CHD_OK) return st;
         cell_bounds_kernel<<<blocks_for((uint64_t)n + 1, 256), 256, 0, s>>>(e->d_sorted_key, n, n_ptr, C, e->d_cell_start,
                                                                               &e->d_ctr->n_entities_in_world);
-        KCHECK(e);
-    }
-    if (n) {
-        replicate_phases_kernel<<<blocks_for(n, 256), 256, 0, s>>>(e->d_sorted_ent, n, n_ptr, e->phase_stride, e->d_sorted4);
         KCHECK(e);
     }
     return CHD_OK;

@@ -11,9 +11,10 @@ extern "C" {
 
 // Which copy kernel (host-known inputs only: nothing here waits for the device):
 //   CTA tiles + per-tile descriptors  when cells are large against a tile (<= 2 segments per tile is the common case)
-//                                     AND the CSR's four phase copies fit in half the L2 (they stay resident next to the write
-//                                     stream: the copy is then a pure write stream);
-//   warp tiles (round 1's kernel)     otherwise: many segments per tile (config #5) or sources streamed from DRAM (config #3).
+//                                     AND the world holds at most L2 / 32 entities (1.6 M with the H100's 50 MB): the size
+//                                     bound separates config #2 (1 M entities, CTA tiles) from config #3 (10 M, warp tiles)
+//                                     and has not been re-tuned for the 4-byte-per-entity sources;
+//   warp tiles (round 1's kernel)     otherwise: many segments per tile (config #5) or a world above that bound (config #3).
 static bool emit_uses_cta_tiles(const chd_engine* e) {
     const uint64_t n_build = (uint64_t)e->n_own + (e->halo_on_device ? (uint64_t)e->border_cap : (uint64_t)e->n_halo);
     const uint64_t own_cells = (uint64_t)(e->g.col_hi - e->g.col_lo) * e->g.rows;  // (the whole grid on one GPU, the slab on N)
@@ -55,14 +56,14 @@ static chd_status emit_kernel_enqueue(chd_engine* e, cudaStream_t s, bool cta_ti
         if (tiles == 0) tiles = 1;
         if (tiles > 0x7fffffffull) tiles = 0x7fffffffull;
         tiles = (tiles + EMIT_TILES_PER_CTA - 1) / EMIT_TILES_PER_CTA;
-        emit_visible_kernel<<<(unsigned)tiles, EMIT_THREADS, CHD_EMIT_DYN_SMEM, s>>>(&e->d_ctr->n_visible, e->d_sorted4, e->d_tile_desc, e->d_vis, e->lim.max_visible);
+        emit_visible_kernel<<<(unsigned)tiles, EMIT_THREADS, CHD_EMIT_DYN_SMEM, s>>>(&e->d_ctr->n_visible, e->d_sorted_ent, e->d_tile_desc, e->d_vis, e->lim.max_visible);
         KCHECK(e);
         emit_visible_general_kernel<<<(unsigned)e->sm_count * 2, EMIT_THREADS, 0, s>>>(e->d_general_tiles, e->d_n_general, pb.off + S, P, &e->d_ctr->n_visible,
-                                                                                       e->d_voff, pb.cell, e->d_cell_start, e->d_sorted4, e->phase_stride,
+                                                                                       e->d_voff, pb.cell, e->d_cell_start, e->d_sorted_ent,
                                                                                        e->d_first_pair, e->d_vis, e->lim.max_visible);
     } else {
-        emit_visible_warp_kernel<<<(unsigned)e->sm_count * 4, EMIT_THREADS, 0, s>>>(pb.off + S, P, e->d_voff, pb.cell, e->d_cell_start, e->d_sorted4,
-                                                                                    e->phase_stride, e->d_first_pair, e->d_vis, e->lim.max_visible);
+        emit_visible_warp_kernel<<<(unsigned)e->sm_count * 4, EMIT_THREADS, 0, s>>>(pb.off + S, P, e->d_voff, pb.cell, e->d_cell_start, e->d_sorted_ent,
+                                                                                    e->d_first_pair, e->d_vis, e->lim.max_visible);
     }
     KCHECK(e);
     return CHD_OK;

@@ -45,7 +45,7 @@ constexpr int EMIT_WARP_SMEM_PAIRS = 64;
 // cell start).  A tile is "simple" if at most two pairs' lists intersect it (always the case when cells hold more entities
 // than a tile: 4 444 vs 4 096 on the benchmark config); other tiles take the general path (segment table in shared memory).
 struct TileDesc {
-    uint32_t src0;  // base of the first segment in the sorted entity array (phase copy 0): slot o of the tile <- sorted[src0 + o]
+    uint32_t src0;  // base of the first segment in the sorted entity array: slot o of the tile <- sorted[src0 + o]
     uint32_t src1;  // the same for the second segment (slots o >= end0; stored minus end0, may wrap below zero)
     uint32_t ends;  // end0 | end1 << 16 (relative to the tile base, <= EMIT_TILE); bit 31 = not simple
     uint32_t p0;    // the pair that owns the tile's first slot (general path)
@@ -147,11 +147,9 @@ struct HandoverOut {
 };
 
 // Extras of the FINAL pass of the entity build, fused into the scatter:
-//   phase_stride != 0 : also write the three phase-shifted copies of the payload (chd_emit.cuh)
 //   cell_start != null: single-pass sorts only (digit == key): block 0 publishes the cell CSR offsets straight from
 //                       the scanned histogram (cell_start[c] = #keys < c), replacing a separate boundaries kernel
 struct ScatterExtras {
-    uint32_t phase_stride;
     uint32_t* cell_start;
     uint32_t cells;
     uint32_t* n_in_world;

@@ -1131,7 +1131,7 @@ def test_concurrent_stateless_queries_during_ticks(chd, oracle):
 def test_emit_descriptor_base_wraps_below_zero(chd, oracle):
     """A tile whose second segment is a cell that starts EARLIER in the CSR than the first segment ends in the tile: the descriptor's
     second base is stored minus that end and wraps below zero (32-bit arithmetic on purpose).  With the two ends congruent mod 4 the
-    copy of the second segment comes from phase 0 (no stride added to the base) and the 16-byte chunk across the boundary goes entry
+    second segment's chunks are aligned 16-byte loads of the sorted array and the 16-byte chunk across the boundary goes entry
     by entry — the combination that used to be added in 64 bits (out-of-bounds read)."""
     wc = chd.synth.CONFIGS["2x2"]
     og = _oracle_grid(wc)
