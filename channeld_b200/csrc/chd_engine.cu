@@ -49,12 +49,48 @@ void chd_dfree(chd_engine* e, void* p) {
     cudaFree(p);
 }
 
-chd_status chd_ensure_upload_stream(chd_engine* e) {
-    if (e->up_stream) return CHD_OK;
-    bool ok = chd_make_stream(e, &e->up_stream);
-    for (cudaEvent_t* ev : {&e->ev_upload, &e->ev_upload_q, &e->ev_upload_rings, &e->ev_q_read[0], &e->ev_ring_read[0], &e->ev_q_read[1], &e->ev_ring_read[1]})
-        ok = ok && chd_make_event(e, ev);
-    return ok ? CHD_OK : CHD_ERR_CUDA;
+static bool pf_events(chd_engine* e, Prefetch& p) {
+    if (p.ev_read[1]) return true;  // (made last)
+    return chd_make_event(e, &p.ev_upload) && chd_make_event(e, &p.ev_read[0]) && chd_make_event(e, &p.ev_read[1]);
+}
+
+chd_status chd_pf_begin(chd_engine* e, Prefetch& p, int* set) {
+    if (!e->up_stream && !chd_make_stream(e, &e->up_stream)) return CHD_ERR_CUDA;
+    if (!pf_events(e, p)) return CHD_ERR_CUDA;
+    if (p.read_recorded[p.next]) CU(e, cudaStreamWaitEvent(e->up_stream, p.ev_read[p.next], 0));
+    *set = p.next;
+    p.staged = -1;  // a staged upload is in this set: an upload that fails part way leaves nothing staged
+    return CHD_OK;
+}
+
+chd_status chd_pf_end(chd_engine* e, Prefetch& p) {
+    CU(e, cudaEventRecord(p.ev_upload, e->up_stream));
+    p.staged = p.next;
+    return CHD_OK;
+}
+
+bool chd_pf_adopt(Prefetch& p) {
+    if (p.staged < 0) return false;
+    p.cur = p.staged;
+    p.next = p.staged ^ 1;
+    p.staged = -1;
+    p.wait = true;
+    return true;
+}
+
+chd_status chd_pf_wait(chd_engine* e, Prefetch& p, cudaStream_t s) {
+    if (!p.wait) return CHD_OK;
+    CU(e, cudaStreamWaitEvent(s, p.ev_upload, 0));
+    p.wait = false;
+    return CHD_OK;
+}
+
+chd_status chd_pf_note_read(chd_engine* e, Prefetch& p, int set, cudaStream_t s) {
+    if (set < 0) return CHD_OK;
+    if (!pf_events(e, p)) return CHD_ERR_CUDA;
+    CU(e, cudaEventRecord(p.ev_read[set], s));
+    p.read_recorded[set] = true;
+    return CHD_OK;
 }
 
 chd_status chd_read_u32(chd_engine* e, const uint32_t* d, uint32_t* v) {
@@ -242,9 +278,10 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     // the aux stream carries short latency-bound kernels that should slot in ahead of the long emit kernel
     bool ok = chd_make_stream(e, &e->aux_stream) && chd_make_stream(e, &e->dl_stream) && chd_make_stream(e, &e->dl_stream_b) &&
               chd_make_stream(e, &e->prep_stream);
-    for (cudaEvent_t* ev : {&e->ev_fork, &e->ev_join, &e->ev_interest, &e->ev_pairs, &e->ev_prep_done, &e->ev_build_done, &e->ev_counts,
-                            &e->ev_pos_read[0], &e->ev_pos_read[1]})
+    for (cudaEvent_t* ev : {&e->ev_fork, &e->ev_join, &e->ev_interest, &e->ev_pairs, &e->ev_prep_done, &e->ev_build_done, &e->ev_counts})
         ok = ok && chd_make_event(e, ev);
+    e->pf_pos.cur = 0;  // the pair allocated here is the front one; the first prefetch fills the other
+    e->pf_pos.next = 1;
     ok = ok && dalloc(e, &e->d_x, N) && dalloc(e, &e->d_z, N) && (e->d_xb[0] = e->d_x, e->d_zb[0] = e->d_z, true) &&
          dalloc(e, &e->d_gid, N) && dalloc(e, &e->d_key, N) &&
          dalloc(e, &e->d_prev_key, N) && dalloc(e, &e->d_tmp_key, N) && dalloc(e, &e->d_tmp_val, N) &&
@@ -291,6 +328,7 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
         chd_destroy(e);
         return CHD_ERR_CUDA;
     }
+    e->ring = RingDev{e->d_ring_off, e->d_ring_off + 1, e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, nullptr, e->d_ring_total, nullptr};
     for (ScanSite* site : e->sites)
         site->error = &e->d_ctr->overflow;
     CCU(cudaHostAlloc((void**)&e->h_ctr, sizeof(Counters), cudaHostAllocDefault));

@@ -1,7 +1,7 @@
 // chd_engine.h — internal: the engine object behind include/chd_gpu.h and the helpers its translation units share.
 // Layout of the host code (all device buffers are allocated once in chd_create; the tick path allocates nothing and —
 // apart from chd_summary / the chd_get_* copies — never synchronises with the host):
-//   chd_engine.cu    create / destroy, streams, memory, CUDA-graph stage cache, instrumentation
+//   chd_engine.cu    create / destroy, streams, memory, the prefetch protocol, CUDA-graph stage cache, instrumentation
 //   chd_entities.cu  positions, cell assignment, spatial-hash build, radix sort passes
 //   chd_interest.cu  subscribers (lifecycle), query batches, QueryChannelIds, interest update
 //   chd_tick.cu      emit, rings, fan-out, the batched tick and its two-stream choreography, summary
@@ -27,6 +27,19 @@
 #include "chd_types.cuh"
 
 using namespace chd;
+
+// One kind of per-tick input (positions, queries, rings) that a pipelined host uploads on up_stream into one of two staging sets
+// while a tick is in flight, and hands to the next tick with chd_adopt_prefetched.  The sets' buffers stay with their kind; this
+// holds which set is free, which is staged and which is read, and the events that order the uploads against the reads.  A
+// prefetch fills the set other than the one adopted last, after the last recorded read of it (chd_pf_*).
+struct Prefetch {
+    int next = 0;      // the set the next prefetch fills
+    int staged = -1;   // the set holding an upload not adopted yet (-1: none)
+    int cur = -1;      // the set the engine reads now (-1: none; positions: the front pair, never none)
+    bool wait = false;  // the reader of `cur` has not been ordered after its upload yet
+    cudaEvent_t ev_upload = nullptr, ev_read[2] = {nullptr, nullptr};
+    bool read_recorded[2] = {false, false};
+};
 
 struct chd_engine {
     chd_grid_cfg cfg;
@@ -82,18 +95,15 @@ struct chd_engine {
     bool halo_on_device = false;     // multi-GPU: the build length (own + halo) lives in d_n_build
     uint32_t* d_n_build = nullptr;
     bool have_gid = false;
-    double *d_x = nullptr, *d_z = nullptr;        // engine-owned staging for host inputs (the FRONT buffers)
-    // chd_prefetch_entities: the BACK buffers receive the next tick's positions on `up_stream` while the current tick runs;
-    // chd_adopt_prefetched swaps front and back.  ev_pos_read[b] = last assign_cells that read buffer pair b.
+    double *d_x = nullptr, *d_z = nullptr;        // engine-owned staging for host inputs (the FRONT buffers: d_xb / d_zb[pf_pos.cur])
+    // position pairs: [0] is allocated by chd_create, [1] by the first chd_prefetch_entities; a prefetch fills the BACK pair and
+    // chd_adopt_prefetched makes it the front one.  pos_n: entities a prefetch uploaded into each pair.
     double *d_xb[2] = {nullptr, nullptr}, *d_zb[2] = {nullptr, nullptr};
+    uint32_t pos_n[2] = {0, 0};
+    Prefetch pf_pos;  // pf_pos.cur = the front pair (chd_create sets it to 0)
     uint32_t *d_general_tiles = nullptr, *d_n_general = nullptr;  // tiles with more than two segments: list, {length, consumer ticket}
     float* d_pos_f32[2] = {nullptr, nullptr};  // float staging of chd_set_entities_f32 [0] / chd_prefetch_entities_f32 [1]: x then z
-    int pos_buf = 0;
-    cudaStream_t up_stream = nullptr;
-    cudaEvent_t ev_upload = nullptr, ev_pos_read[2] = {nullptr, nullptr};
-    bool pos_read_recorded[2] = {false, false};
-    bool staged = false;
-    uint32_t staged_n = 0;
+    cudaStream_t up_stream = nullptr;  // every prefetch upload
     const double *pos_x = nullptr, *pos_z = nullptr;  // what the kernels read: the staging buffers, or the caller's device arrays
     uint32_t *d_gid = nullptr;            // [max_entities] global ids (multi-GPU) of own + halo
     uint32_t *d_key = nullptr, *d_prev_key = nullptr;  // [max_entities] cell key per entity
@@ -129,25 +139,17 @@ struct chd_engine {
         double *sph_cx, *sph_cz, *sph_r, *box_cx, *box_cz, *box_ex, *box_ez, *cone_cx, *cone_cz, *cone_dx, *cone_dz, *cone_angle, *cone_r;
         uint32_t *spot_off, *spot_ndist; double *spot_x, *spot_z; uint32_t* spot_dist;
     } dq{};
-    // chd_prefetch_queries / chd_prefetch_rings: two dedicated staging sets each (allocated on first use), filled on
-    // up_stream while a tick is in flight and handed to the next tick by chd_adopt_prefetched
+    // chd_prefetch_queries / chd_prefetch_rings: two staging sets each, allocated by the first prefetch that fills them.
+    // pf_q.cur: the adopted batch the next interest update with q == NULL consumes (-1 once consumed).
     QStage dq_pf[2] = {};
-    bool dq_pf_alloc[2] = {false, false};
-    int q_next = 0;                       // set the next chd_prefetch_queries fills
-    bool staged_q = false, have_adopted_q = false, wait_q = false;
-    int staged_q_set = 0, adopted_q_set = 0;
-    QueryDev staged_qd{}, adopted_qd{};
-    cudaEvent_t ev_upload_q = nullptr, ev_q_read[2] = {nullptr, nullptr};
-    bool q_read_recorded[2] = {false, false};
+    QueryDev dq_pf_view[2] = {};  // the batch each set holds
+    Prefetch pf_q;
     struct RStage {
         uint32_t *off, *sender; int64_t* arrival; uint64_t *index, *cmi;
+        uint32_t total;  // entries uploaded
+        bool has_cmi;    // cmi holds a channel_msg_index
     } ring_pf[2] = {};
-    bool ring_pf_alloc[2] = {false, false};
-    int ring_next = 0, staged_ring_set = 0, ring_set = -1;  // ring_set: prefetch set the current ring pointers refer to (-1: none)
-    bool staged_rings = false, staged_ring_cmi = false, wait_rings = false;
-    uint32_t staged_ring_total = 0;
-    cudaEvent_t ev_upload_rings = nullptr, ev_ring_read[2] = {nullptr, nullptr};
-    bool ring_read_recorded[2] = {false, false};
+    Prefetch pf_ring;  // pf_ring.cur: the set `ring` reads (-1: the rings came from chd_set_rings / chd_rings_init)
     Bbox* d_bbox = nullptr;
     uint32_t *d_window = nullptr, *d_side_cell = nullptr, *d_side_dist = nullptr, *d_side_cnt = nullptr;
     uint64_t* d_win_off = nullptr;
@@ -222,7 +224,6 @@ struct chd_engine {
     uint32_t *d_ring_off = nullptr, *d_ring_sender = nullptr;
     int64_t* d_ring_arrival = nullptr;
     uint64_t *d_ring_index = nullptr, *d_ch_msg_index = nullptr;
-    bool have_ch_msg_index = false;
     // device-owned rings (chd_rings_init: ChannelData.OnUpdate on the GPU, data.go:149-173): per-cell begin / end cursors into
     // slabs of ring_cap entries inside d_ring_arrival / d_ring_sender / d_ring_index; d_ch_msg_index = ChannelData.msgIndex
     bool rings_owned = false;
@@ -234,10 +235,10 @@ struct chd_engine {
     uint32_t* d_cell_max_interval = nullptr;  // [C] ChannelData.maxFanOutIntervalMs (subscription.go:84-86)
     int64_t* d_cell_start_ns = nullptr;       // [C] per-channel ChannelTime origin (chd_set_channel_start_times) or nullptr
     bool have_cell_start = false;
-    // what the fan-out kernel reads: the staging copies above or the caller's device arrays (zero-copy)
-    const uint32_t *ring_off_p = nullptr, *ring_sender_p = nullptr;
-    const int64_t* ring_arrival_p = nullptr;
-    const uint64_t *ring_index_p = nullptr, *ch_msg_index_p = nullptr;
+    // the rings the fan-out and payload kernels read (chd_ring_view adds `start`): the staging copies above, the caller's device
+    // arrays (zero-copy), an adopted prefetch set or the device-owned rings.  Set by chd_create, chd_set_rings, chd_rings_init
+    // and chd_adopt_prefetched.
+    RingDev ring{};
 
     uint32_t *d_by_cell = nullptr, *d_pc_hist = nullptr, *d_pc_tmp_key = nullptr, *d_pc_tmp_val = nullptr;  // pairs grouped by cell
     uint32_t pc_blocks = 0;
@@ -391,10 +392,26 @@ bool chd_make_site(chd_engine* e, ScanSite& site, uint64_t n_max, int stage);
 // and unmodified until the work that reads it has finished (chd_summary / chd_sync / any chd_get_*).
 bool chd_is_device_ptr(const chd_engine* e, const void* p);
 void chd_dfree(chd_engine* e, void* p);
-chd_status chd_ensure_upload_stream(chd_engine* e);
+// The prefetch protocol (struct Prefetch).  begin: creates up_stream and the events on first use, orders up_stream after the
+// last recorded read of the set the prefetch fills and returns that set; the caller then enqueues the upload on up_stream.
+// end: records the upload and stages the set (a second prefetch before an adoption refills it).  adopt: makes the staged set
+// the one read (false: nothing staged).  wait: orders reader stream `s` after the upload, once per adoption.  note_read:
+// records a read of `set` (-1: none) on `s`, outside any graph capture, so that no prefetch overwrites it before that read.
+chd_status chd_pf_begin(chd_engine* e, Prefetch& p, int* set);
+chd_status chd_pf_end(chd_engine* e, Prefetch& p);
+bool chd_pf_adopt(Prefetch& p);
+chd_status chd_pf_wait(chd_engine* e, Prefetch& p, cudaStream_t s);
+chd_status chd_pf_note_read(chd_engine* e, Prefetch& p, int set, cudaStream_t s);
 chd_status chd_read_u32(chd_engine* e, const uint32_t* d, uint32_t* v);
 chd_status chd_decode_summary(chd_engine* e, chd_tick_summary* out);
 chd_status chd_assign_cells_impl(chd_engine* e, cudaStream_t s);
+// Host half of a cell assignment: the key buffers swap (handover detection compares against the keys of the previous
+// assignment, same entity count; swapped, never copied) and the own entities count as assigned.  Returns the previous keys or
+// nullptr.  A replayed assignment graph runs only the device half, so its caller runs this.
+uint32_t* chd_assign_host(chd_engine* e);
+// the current positions were replaced by n others (a set call, chd_set_entity_count, an adopted prefetch): nothing is assigned
+// or built for them yet
+void chd_entities_replaced(chd_engine* e, uint32_t n);
 chd_status chd_note_pos_read(chd_engine* e, cudaStream_t s);
 // Called on the host wherever a stage's epoch is about to be bumped on the device: every 2^20 executions of a stage the
 // descriptors of its scan sites are cleared, so no descriptor can survive until the 22-bit epoch repeats.  `s` is the
@@ -431,6 +448,13 @@ static bool ensure_cap(chd_engine* e, T** p, uint64_t* cap, uint64_t need, uint6
 }
 
 static inline unsigned blocks_for(uint64_t n, unsigned threads) { return (unsigned)((n + threads - 1) / threads); }
+
+// Replayable cell assignments (build, border export) are captured per [key buffer the new keys go to][front position pair]:
+// returns the graph slot and that key buffer.
+static inline int assign_graph_slot(const chd_engine* e, uint32_t** target) {
+    *target = e->have_prev_key ? e->d_prev_key : e->d_key;
+    return (*target == e->d_key_a ? 0 : 1) + 2 * e->pf_pos.cur;
+}
 
 static inline uint64_t mix_key(uint64_t h, uint64_t v) {
     h ^= v + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2);

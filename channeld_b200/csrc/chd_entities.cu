@@ -95,56 +95,6 @@ chd_status chd_cell_of_valid(chd_engine* e, const double* x, const double* z, ui
     return CHD_OK;
 }
 
-chd_status chd_set_entities(chd_engine* e, const double* x, const double* z, uint32_t n) {
-    if (!e || (n && (!x || !z))) return CHD_ERR_INVALID;
-    if (n > e->lim.max_entities) {
-        e->fail("chd_set_entities: %u > max_entities %u", n, e->lim.max_entities);
-        return CHD_ERR_CAPACITY;
-    }
-    CU(e, cudaSetDevice(e->device));
-    if (n != e->n_own) e->have_prev_key = false;
-    if (n && chd_is_device_ptr(e, x) && chd_is_device_ptr(e, z)) {
-        e->pos_x = x;  // device-resident producer: read in place
-        e->pos_z = z;
-    } else {
-        CU(e, cudaMemcpyAsync(e->d_x, x, sizeof(double) * n, cudaMemcpyDefault, e->stream));
-        CU(e, cudaMemcpyAsync(e->d_z, z, sizeof(double) * n, cudaMemcpyDefault, e->stream));
-        e->pos_x = e->d_x;
-        e->pos_z = e->d_z;
-    }
-    e->n_own = n;
-    e->n_halo = 0;
-    e->halo_on_device = false;
-    e->assigned = false;
-    e->entities_dirty = true;
-    return CHD_OK;
-}
-
-chd_status chd_prefetch_entities(chd_engine* e, const double* x, const double* z, uint32_t n) {
-    if (!e || (n && (!x || !z))) return CHD_ERR_INVALID;
-    if (n > e->lim.max_entities) {
-        e->fail("chd_prefetch_entities: %u > max_entities %u", n, e->lim.max_entities);
-        return CHD_ERR_CAPACITY;
-    }
-    CU(e, cudaSetDevice(e->device));
-    const int back = e->pos_buf ^ 1;
-    {
-        chd_status st = chd_ensure_upload_stream(e);
-        if (st != CHD_OK) return st;
-    }
-    if (!e->d_xb[back]) {  // the second pair of position buffers exists only for hosts that prefetch
-        if (!dalloc(e, &e->d_xb[back], e->lim.max_entities) || !dalloc(e, &e->d_zb[back], e->lim.max_entities)) return CHD_ERR_CUDA;
-    }
-    // the back pair was last read by the cell assignment of an earlier tick
-    if (e->pos_read_recorded[back]) CU(e, cudaStreamWaitEvent(e->up_stream, e->ev_pos_read[back], 0));
-    CU(e, cudaMemcpyAsync(e->d_xb[back], x, sizeof(double) * n, cudaMemcpyDefault, e->up_stream));
-    CU(e, cudaMemcpyAsync(e->d_zb[back], z, sizeof(double) * n, cudaMemcpyDefault, e->up_stream));
-    CU(e, cudaEventRecord(e->ev_upload, e->up_stream));
-    e->staged = true;
-    e->staged_n = n;
-    return CHD_OK;
-}
-
 // float uploads (see widen_positions_kernel): the floats land in a staging buffer (or are read in place when they already live on
 // the device) and are widened into the double buffers on the same stream, so everything downstream is unchanged.
 static chd_status widen_upload(chd_engine* e, int which, const float* x, const float* z, uint32_t n, double* dx, double* dz, cudaStream_t s) {
@@ -167,48 +117,66 @@ static chd_status widen_upload(chd_engine* e, int which, const float* x, const f
     return CHD_OK;
 }
 
-chd_status chd_set_entities_f32(chd_engine* e, const float* x, const float* z, uint32_t n) {
-    if (!e || (n && (!x || !z))) return CHD_ERR_INVALID;
-    if (n > e->lim.max_entities) {
-        e->fail("chd_set_entities_f32: %u > max_entities %u", n, e->lim.max_entities);
-        return CHD_ERR_CAPACITY;
-    }
-    CU(e, cudaSetDevice(e->device));
+void chd_entities_replaced(chd_engine* e, uint32_t n) {
     if (n != e->n_own) e->have_prev_key = false;
-    chd_status st = widen_upload(e, 0, x, z, n, e->d_x, e->d_z, e->stream);
-    if (st != CHD_OK) return st;
-    e->pos_x = e->d_x;
-    e->pos_z = e->d_z;
     e->n_own = n;
     e->n_halo = 0;
     e->halo_on_device = false;
     e->assigned = false;
     e->entities_dirty = true;
-    return CHD_OK;
 }
 
-chd_status chd_prefetch_entities_f32(chd_engine* e, const float* x, const float* z, uint32_t n) {
+// Every position upload, f64 or f32: into the front pair on the engine stream (set), or into the pair the next prefetch fills on
+// up_stream (prefetch).  Device-resident doubles given to a set are read in place.
+static chd_status upload_positions(chd_engine* e, const char* fn, const void* x, const void* z, uint32_t n, bool f32, bool prefetch) {
     if (!e || (n && (!x || !z))) return CHD_ERR_INVALID;
     if (n > e->lim.max_entities) {
-        e->fail("chd_prefetch_entities_f32: %u > max_entities %u", n, e->lim.max_entities);
+        e->fail("%s: %u > max_entities %u", fn, n, e->lim.max_entities);
         return CHD_ERR_CAPACITY;
     }
     CU(e, cudaSetDevice(e->device));
-    const int back = e->pos_buf ^ 1;
-    {
-        chd_status st = chd_ensure_upload_stream(e);
+    cudaStream_t s = e->stream;
+    double *dx = e->d_x, *dz = e->d_z;
+    int set = 0;
+    chd_status st;
+    if (prefetch) {
+        st = chd_pf_begin(e, e->pf_pos, &set);
         if (st != CHD_OK) return st;
+        // the second pair of position buffers exists only for hosts that prefetch
+        if (!e->d_zb[set] && !(dalloc(e, &e->d_xb[set], e->lim.max_entities) && dalloc(e, &e->d_zb[set], e->lim.max_entities))) return CHD_ERR_CUDA;
+        s = e->up_stream;
+        dx = e->d_xb[set];
+        dz = e->d_zb[set];
     }
-    if (!e->d_xb[back]) {
-        if (!dalloc(e, &e->d_xb[back], e->lim.max_entities) || !dalloc(e, &e->d_zb[back], e->lim.max_entities)) return CHD_ERR_CUDA;
+    const bool in_place = !f32 && !prefetch && n && chd_is_device_ptr(e, x) && chd_is_device_ptr(e, z);
+    if (f32) {
+        st = widen_upload(e, prefetch ? 1 : 0, (const float*)x, (const float*)z, n, dx, dz, s);
+        if (st != CHD_OK) return st;
+    } else if (!in_place) {
+        CU(e, cudaMemcpyAsync(dx, x, sizeof(double) * n, cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(dz, z, sizeof(double) * n, cudaMemcpyDefault, s));
     }
-    if (e->pos_read_recorded[back]) CU(e, cudaStreamWaitEvent(e->up_stream, e->ev_pos_read[back], 0));
-    chd_status st = widen_upload(e, 1, x, z, n, e->d_xb[back], e->d_zb[back], e->up_stream);
-    if (st != CHD_OK) return st;
-    CU(e, cudaEventRecord(e->ev_upload, e->up_stream));
-    e->staged = true;
-    e->staged_n = n;
+    if (prefetch) {
+        e->pos_n[set] = n;
+        return chd_pf_end(e, e->pf_pos);
+    }
+    e->pos_x = in_place ? (const double*)x : e->d_x;  // device-resident producer: read in place
+    e->pos_z = in_place ? (const double*)z : e->d_z;
+    chd_entities_replaced(e, n);
     return CHD_OK;
+}
+
+chd_status chd_set_entities(chd_engine* e, const double* x, const double* z, uint32_t n) {
+    return upload_positions(e, "chd_set_entities", x, z, n, false, false);
+}
+chd_status chd_prefetch_entities(chd_engine* e, const double* x, const double* z, uint32_t n) {
+    return upload_positions(e, "chd_prefetch_entities", x, z, n, false, true);
+}
+chd_status chd_set_entities_f32(chd_engine* e, const float* x, const float* z, uint32_t n) {
+    return upload_positions(e, "chd_set_entities_f32", x, z, n, true, false);
+}
+chd_status chd_prefetch_entities_f32(chd_engine* e, const float* x, const float* z, uint32_t n) {
+    return upload_positions(e, "chd_prefetch_entities_f32", x, z, n, true, true);
 }
 
 chd_status chd_entity_buffers(chd_engine* e, double** d_x, double** d_z, uint32_t* n) {
@@ -225,12 +193,7 @@ chd_status chd_entity_buffers(chd_engine* e, double** d_x, double** d_z, uint32_
 
 chd_status chd_set_entity_count(chd_engine* e, uint32_t n) {
     if (!e || n > e->lim.max_entities) return CHD_ERR_INVALID;
-    if (n != e->n_own) e->have_prev_key = false;
-    e->n_own = n;
-    e->n_halo = 0;
-    e->halo_on_device = false;
-    e->assigned = false;
-    e->entities_dirty = true;
+    chd_entities_replaced(e, n);
     return CHD_OK;
 }
 
@@ -251,10 +214,7 @@ chd_status chd_set_entity_ids(chd_engine* e, const uint32_t* gid, uint32_t n) {
 // The engine's position buffers are double-buffered for chd_prefetch_entities: remember (outside any graph capture)
 // the last kernel that read the front pair, so an upload into it can be ordered after that read.
 chd_status chd_note_pos_read(chd_engine* e, cudaStream_t s) {
-    if (e->pos_x != e->d_x || !e->ev_pos_read[e->pos_buf]) return CHD_OK;
-    CU(e, cudaEventRecord(e->ev_pos_read[e->pos_buf], s));
-    e->pos_read_recorded[e->pos_buf] = true;
-    return CHD_OK;
+    return chd_pf_note_read(e, e->pf_pos, e->pos_x == e->d_x ? e->pf_pos.cur : -1, s);
 }
 
 chd_status chd_assign_cells(chd_engine* e) {
@@ -269,19 +229,23 @@ chd_status chd_assign_cells(chd_engine* e) {
     return st;
 }
 
-// host-side half of a cell assignment: the key buffers swap (handover detection compares against the keys of the previous
-// assignment, same entity count; swapped, never copied), the handover counter is zeroed.  Returns the previous keys or nullptr.
-static chd_status assign_prepare(chd_engine* e, cudaStream_t s, uint32_t** prev_out, HandoverOut* ho) {
+uint32_t* chd_assign_host(chd_engine* e) {
     uint32_t* prev = nullptr;
     if (e->have_prev_key) {
-        uint32_t* t = e->d_key;
-        e->d_key = e->d_prev_key;
-        e->d_prev_key = t;
+        std::swap(e->d_key, e->d_prev_key);
         prev = e->d_prev_key;
     }
+    if (e->n_own) e->have_prev_key = true;
+    e->n_halo = 0;
+    e->assigned = true;
+    return prev;
+}
+
+// chd_assign_host, the handover output and its counter zeroed on `s`
+static chd_status assign_prepare(chd_engine* e, cudaStream_t s, uint32_t** prev_out, HandoverOut* ho) {
+    *prev_out = chd_assign_host(e);
     *ho = HandoverOut{e->d_ho_entity, e->d_ho_src, e->d_ho_dst, &e->d_ctr->n_handover, e->ho_cap};
     CU(e, cudaMemsetAsync(&e->d_ctr->n_handover, 0, 4, s));
-    *prev_out = prev;
     return CHD_OK;
 }
 
@@ -296,11 +260,8 @@ chd_status chd_assign_cells_impl(chd_engine* e, cudaStream_t s) {
         assign_cells_kernel<<<blocks_for(e->n_own, 256), 256, 0, s>>>(e->g, e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z,
                                                                       e->n_own, e->d_key, prev, ho, e->assign_bump);
         KCHECK(e);
-        e->have_prev_key = true;
         e->assign_bump = nullptr;  // consumed
     }
-    e->n_halo = 0;
-    e->assigned = true;
     return CHD_OK;
 }
 
@@ -319,9 +280,6 @@ static chd_status build_enqueue(chd_engine* e, cudaStream_t s, bool with_assign,
             if (st != CHD_OK) return st;
             fa = FusedAssign{e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z, e->d_key, prev, ho};
             fap = &fa;
-            e->have_prev_key = true;
-            e->n_halo = 0;
-            e->assigned = true;
         } else {
             st = chd_assign_cells_impl(e, s);
             if (st != CHD_OK) return st;
@@ -391,24 +349,15 @@ chd_status chd_build_on(chd_engine* e, cudaStream_t s) {
     if (!e->assigned && !e->halo_on_device) {
         // single-GPU flow: assign + sort as one replayable graph.  The key buffers swap every assignment
         // (handover detection compares against the previous keys), so there are two graph variants.
-        uint32_t* target = e->have_prev_key ? e->d_prev_key : e->d_key;  // buffer the new keys will be written to
-        const int slot = (target == e->d_key_a ? 0 : 1) + 2 * e->pos_buf;
+        uint32_t* target = nullptr;  // buffer the new keys will be written to
+        const int slot = assign_graph_slot(e, &target);
         uint64_t key = mix_key(mix_key(mix_key(0x6275696c64ull, e->n_own), e->have_gid), e->have_prev_key);
         key = mix_key(mix_key(key, (uint64_t)(uintptr_t)target), (uint64_t)(uintptr_t)e->pos_x ^ ((uint64_t)(uintptr_t)e->pos_z << 1));
         // single-pass builds (<= 1023 cells) run as two replayable halves with an event in between: the cell CSR offsets are
         // final after the first (assignment + histogram + scan), so the emit preparation overlaps the scatter
         const bool split = e->g.cells + 1 <= BUILD_MAX_BINS && e->n_own > 0;
         st = run_stage(e, s, e->g_build[slot], key, [&]() { return build_enqueue(e, s, true, split ? 1 : 0); });
-        if (st == CHD_OK && !e->assigned) {  // replayed graph: mirror the host-side bookkeeping of chd_assign_cells
-            if (e->have_prev_key) {
-                uint32_t* t = e->d_key;
-                e->d_key = e->d_prev_key;
-                e->d_prev_key = t;
-            }
-            if (e->n_own) e->have_prev_key = true;
-            e->n_halo = 0;
-            e->assigned = true;
-        }
+        if (st == CHD_OK && !e->assigned) chd_assign_host(e);  // replayed graph
         if (st == CHD_OK && split) {
             CU(e, cudaEventRecord(e->ev_counts, s));
             counts_recorded = true;

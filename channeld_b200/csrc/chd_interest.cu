@@ -14,24 +14,13 @@ chd_status chd_prefetch_queries(chd_engine* e, const chd_query_batch* q) {
     if (!e || !q) return CHD_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lk(e->mu);
     CU(e, cudaSetDevice(e->device));
-    chd_status st = chd_ensure_upload_stream(e);
+    int set = 0;
+    chd_status st = chd_pf_begin(e, e->pf_q, &set);
     if (st != CHD_OK) return st;
-    const int set = e->q_next;
     chd_engine::QStage& qs = e->dq_pf[set];
-    if (!e->dq_pf_alloc[set]) {
-        if (!alloc_qstage(e, qs)) return CHD_ERR_CUDA;
-        e->dq_pf_alloc[set] = true;
-    }
-    if (e->q_read_recorded[set]) CU(e, cudaStreamWaitEvent(e->up_stream, e->ev_q_read[set], 0));  // its previous batch has been consumed
-    QueryDev d;
-    st = upload_queries(e, e->up_stream, q, &d, true, &qs);
-    if (st != CHD_OK) return st;
-    CU(e, cudaEventRecord(e->ev_upload_q, e->up_stream));
-    e->staged_qd = d;
-    e->staged_q_set = set;
-    e->staged_q = true;
-    e->q_next = set ^ 1;
-    return CHD_OK;
+    if (!qs.spot_dist && !alloc_qstage(e, qs)) return CHD_ERR_CUDA;  // (spot_dist is allocated last)
+    st = upload_queries(e, e->up_stream, q, &e->dq_pf_view[set], true, &qs);
+    return st != CHD_OK ? st : chd_pf_end(e, e->pf_q);
 }
 
 /* ------------------------------------------------------------------ subscribers / queries ---- */
@@ -330,21 +319,19 @@ chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query
     chd_status st;
     int pf_set = -1;  // prefetch staging set this batch lives in
     if (!q) {  // the batch uploaded by chd_prefetch_queries and handed over by chd_adopt_prefetched
-        if (!e->have_adopted_q) {
+        if (e->pf_q.cur < 0) {
             e->fail("interest update without a batch: q == NULL needs chd_prefetch_queries + chd_adopt_prefetched first");
             return CHD_ERR_STATE;
         }
-        d = e->adopted_qd;
-        pf_set = e->adopted_q_set;
-        e->have_adopted_q = false;
+        pf_set = e->pf_q.cur;
+        d = e->dq_pf_view[pf_set];
+        e->pf_q.cur = -1;  // consumed
         if (d.n > e->n_slots && !d.sub) {
             e->fail("identity query batch (sub == NULL) of %u queries > %u subscribers", d.n, e->n_slots);
             return CHD_ERR_INVALID;
         }
-        if (e->wait_q) {
-            CU(e, cudaStreamWaitEvent(s, e->ev_upload_q, 0));
-            e->wait_q = false;
-        }
+        st = chd_pf_wait(e, e->pf_q, s);
+        if (st != CHD_OK) return st;
     } else {
         st = upload_queries(e, s, q, &d, true);  // H2D / D2D copies into the engine's SoA: outside the graph
         if (st != CHD_OK) return st;
@@ -366,10 +353,8 @@ chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query
     CU(e, cudaEventRecord(e->ev_pairs, s));  // the new pairs exist: emit may start (chd_tick waits on this)
     st = run_stage(e, s, e->g_interest_b[gslot], mix_key(key, 0xb), [&]() { return interest_enqueue(e, s, d, 1); });
     if (st != CHD_OK) return st;
-    if (pf_set >= 0) {  // the staging set may be refilled once these kernels have run
-        CU(e, cudaEventRecord(e->ev_q_read[pf_set], s));
-        e->q_read_recorded[pf_set] = true;
-    }
+    st = chd_pf_note_read(e, e->pf_q, pf_set, s);  // the staging set may be refilled once these kernels have run
+    if (st != CHD_OK) return st;
     e->cur ^= 1;
     e->last_nq = d.n;
     return CHD_OK;

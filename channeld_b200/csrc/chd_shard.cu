@@ -108,24 +108,15 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
     if (st != CHD_OK) return st;
     if (!e->assigned) {
         // replayable: cell assignment + border selection of one tick (two variants: the key buffers ping-pong)
-        uint32_t* target = e->have_prev_key ? e->d_prev_key : e->d_key;
-        const int slot = (target == e->d_key_a ? 0 : 1) + 2 * e->pos_buf;
+        uint32_t* target = nullptr;
+        const int slot = assign_graph_slot(e, &target);
         uint64_t key = mix_key(mix_key(mix_key(0x6578706full, n), e->have_gid), e->have_prev_key);
         key = mix_key(mix_key(key, (uint64_t)(uintptr_t)target), (uint64_t)(uintptr_t)e->pos_x ^ ((uint64_t)(uintptr_t)e->pos_z << 1));
         key = mix_key(mix_key(key, (uint64_t)(uintptr_t)d_records), cap_records);
         key = mix_key(mix_key(mix_key(key, e->g.col_lo), e->g.col_hi), e->g.halo);
         key = mix_key(key, to_peers ? 1 : 0);
         st = run_stage(e, s, e->g_export[slot + (to_peers ? 4 : 0)], key, enqueue);
-        if (st == CHD_OK && !e->assigned) {  // replayed graph: mirror the host-side bookkeeping of chd_assign_cells
-            if (e->have_prev_key) {
-                uint32_t* t = e->d_key;
-                e->d_key = e->d_prev_key;
-                e->d_prev_key = t;
-            }
-            if (e->n_own) e->have_prev_key = true;
-            e->n_halo = 0;
-            e->assigned = true;
-        }
+        if (st == CHD_OK && !e->assigned) chd_assign_host(e);  // replayed graph
         if (st == CHD_OK) st = chd_note_pos_read(e, s);
     } else {
         st = enqueue();
@@ -356,7 +347,7 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
         if (gs_ != CHD_OK) return gs_;
     }
     chd_status st;
-    const bool has_batch = q || e->have_adopted_q;
+    const bool has_batch = q || e->pf_q.cur >= 0;
     // Without subscriber migration the interest update does not depend on the exchange: it starts first and overlaps it.
     // With migration the immigrants' previous state arrives in the all-gather, so the update starts right after it.
     if (has_batch && !e->mig_subs) {

@@ -101,40 +101,62 @@ chd_status chd_emit_visible(chd_engine* e) {
     return st != CHD_OK ? st : emit_enqueue(e, e->stream, nullptr, nullptr);
 }
 
-chd_status chd_set_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
-                         const uint64_t* index, const uint64_t* ch_msg_index) {
+// argument checks of one tick's host-owned rings (chd_set_rings / chd_prefetch_rings)
+static chd_status check_rings(chd_engine* e, const char* fn, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
+                              const uint64_t* index) {
     if (!e || !ring_off) return CHD_ERR_INVALID;
     if (e->rings_owned) {
-        e->fail("chd_set_rings: the rings are device-owned (chd_rings_init): use chd_rings_append");
+        e->fail("%s: the rings are device-owned (chd_rings_init): use chd_rings_append", fn);
         return CHD_ERR_STATE;
     }
-    CU(e, cudaSetDevice(e->device));
-    const uint32_t C = e->g.cells;
-    const uint32_t total = n_entries;
-    if (total > e->lim.max_ring_entries) {
-        e->fail("%u ring entries > max_ring_entries %u", total, e->lim.max_ring_entries);
+    if (n_entries > e->lim.max_ring_entries) {
+        e->fail("%u ring entries > max_ring_entries %u", n_entries, e->lim.max_ring_entries);
         return CHD_ERR_CAPACITY;
     }
-    if (total && (!arrival || !sender || !index)) return CHD_ERR_INVALID;
+    if (n_entries && (!arrival || !sender || !index)) return CHD_ERR_INVALID;
+    return CHD_OK;
+}
+
+// copies one tick's host-owned rings into staging arrays on `s` and records their entry count and whether they carry
+// channel_msg_index
+static chd_status copy_rings(chd_engine* e, cudaStream_t s, chd_engine::RStage& r, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival,
+                             const uint32_t* sender, const uint64_t* index, const uint64_t* ch_msg_index) {
+    const uint64_t C = e->g.cells;
+    CU(e, cudaMemcpyAsync(r.off, ring_off, sizeof(uint32_t) * (C + 1), cudaMemcpyDefault, s));
+    if (n_entries) {
+        CU(e, cudaMemcpyAsync(r.arrival, arrival, sizeof(int64_t) * n_entries, cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(r.sender, sender, sizeof(uint32_t) * n_entries, cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(r.index, index, sizeof(uint64_t) * n_entries, cudaMemcpyDefault, s));
+    }
+    if (ch_msg_index) CU(e, cudaMemcpyAsync(r.cmi, ch_msg_index, sizeof(uint64_t) * C, cudaMemcpyDefault, s));
+    r.total = n_entries;
+    r.has_cmi = ch_msg_index != nullptr;
+    return CHD_OK;
+}
+
+// staged host-owned rings as the kernels read them: a CSR by cell
+static RingDev staged_ring(const chd_engine* e, const chd_engine::RStage& r) {
+    return RingDev{r.off, r.off + 1, r.arrival, r.sender, r.index, r.has_cmi ? r.cmi : nullptr, e->d_ring_total, nullptr};
+}
+
+chd_status chd_set_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
+                         const uint64_t* index, const uint64_t* ch_msg_index) {
+    chd_status st = check_rings(e, "chd_set_rings", ring_off, n_entries, arrival, sender, index);
+    if (st != CHD_OK) return st;
+    CU(e, cudaSetDevice(e->device));
+    const uint32_t total = n_entries;
     const bool in_place = chd_is_device_ptr(e, ring_off) && (!total || (chd_is_device_ptr(e, arrival) && chd_is_device_ptr(e, sender) && chd_is_device_ptr(e, index))) &&
                           (!ch_msg_index || chd_is_device_ptr(e, ch_msg_index));
     if (in_place) {  // device-resident rings: consumed in place
-        e->ring_off_p = ring_off; e->ring_arrival_p = arrival; e->ring_sender_p = sender; e->ring_index_p = index;
-        e->ch_msg_index_p = ch_msg_index;
+        e->ring = RingDev{ring_off, ring_off + 1, arrival, sender, index, ch_msg_index, e->d_ring_total, nullptr};
     } else {
-        CU(e, cudaMemcpyAsync(e->d_ring_off, ring_off, sizeof(uint32_t) * ((uint64_t)C + 1), cudaMemcpyDefault, e->stream));
-        if (total) {
-            CU(e, cudaMemcpyAsync(e->d_ring_arrival, arrival, sizeof(int64_t) * total, cudaMemcpyDefault, e->stream));
-            CU(e, cudaMemcpyAsync(e->d_ring_sender, sender, sizeof(uint32_t) * total, cudaMemcpyDefault, e->stream));
-            CU(e, cudaMemcpyAsync(e->d_ring_index, index, sizeof(uint64_t) * total, cudaMemcpyDefault, e->stream));
-        }
-        if (ch_msg_index) CU(e, cudaMemcpyAsync(e->d_ch_msg_index, ch_msg_index, sizeof(uint64_t) * C, cudaMemcpyDefault, e->stream));
-        e->ring_off_p = e->d_ring_off; e->ring_arrival_p = e->d_ring_arrival; e->ring_sender_p = e->d_ring_sender;
-        e->ring_index_p = e->d_ring_index; e->ch_msg_index_p = ch_msg_index ? e->d_ch_msg_index : nullptr;
+        chd_engine::RStage r{e->d_ring_off, e->d_ring_sender, e->d_ring_arrival, e->d_ring_index, e->d_ch_msg_index, 0, false};
+        st = copy_rings(e, e->stream, r, ring_off, total, arrival, sender, index, ch_msg_index);
+        if (st != CHD_OK) return st;
+        e->ring = staged_ring(e, r);
     }
-    e->have_ch_msg_index = ch_msg_index != nullptr;
-    e->ring_set = -1;
-    e->wait_rings = false;
+    e->pf_ring.cur = -1;
+    e->pf_ring.wait = false;
     // the fan-out kernel clamps ring_off to this: a lying caller cannot cause out-of-bounds reads
     set_u32_kernel<<<1, 1, 0, e->stream>>>(e->d_ring_total, total);
     KCHECK(e);
@@ -162,9 +184,10 @@ chd_status chd_rings_init(chd_engine* e, uint32_t capacity_per_cell) {
     KCHECK(e);
     e->rings_owned = true;
     e->ring_cap = capacity_per_cell;
-    e->have_ch_msg_index = true;
-    e->ring_set = -1;
-    e->wait_rings = false;
+    e->ring = RingDev{e->d_rb_begin, e->d_rb_end, e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, e->d_ch_msg_index, e->d_ring_total, nullptr};
+    e->pf_ring.cur = -1;
+    e->pf_ring.wait = false;
+    e->pf_ring.staged = -1;  // host-owned rings prefetched before this call are not adopted
     return CHD_OK;
 }
 
@@ -251,12 +274,9 @@ chd_status chd_set_channel_start_times(chd_engine* e, const int64_t* start_ns) {
 }
 
 RingDev chd_ring_view(const chd_engine* e) {
-    const int64_t* start = e->have_cell_start ? e->d_cell_start_ns : nullptr;
-    if (e->rings_owned)
-        return RingDev{e->d_rb_begin, e->d_rb_end, e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, e->d_ch_msg_index, e->d_ring_total, start};
-    const uint32_t* off = e->ring_off_p ? e->ring_off_p : e->d_ring_off;
-    return RingDev{off, off + 1, e->ring_arrival_p ? e->ring_arrival_p : e->d_ring_arrival, e->ring_sender_p ? e->ring_sender_p : e->d_ring_sender,
-                   e->ring_index_p ? e->ring_index_p : e->d_ring_index, e->have_ch_msg_index ? e->ch_msg_index_p : nullptr, e->d_ring_total, start};
+    RingDev ring = e->ring;
+    ring.start = e->have_cell_start ? e->d_cell_start_ns : nullptr;
+    return ring;
 }
 
 static chd_status fanout_enqueue(chd_engine* e, cudaStream_t s, int64_t t_ns) {
@@ -264,31 +284,25 @@ static chd_status fanout_enqueue(chd_engine* e, cudaStream_t s, int64_t t_ns) {
     const uint32_t S = e->n_slots;
     const uint64_t P = e->lim.max_pairs;
     StageTimer timer(e, s, CHD_STAGE_FANOUT);
-    if (e->wait_rings) {  // rings handed over by chd_adopt_prefetched: ordered after their upload
-        CU(e, cudaStreamWaitEvent(s, e->ev_upload_rings, 0));
-        e->wait_rings = false;
-    }
+    chd_status st = chd_pf_wait(e, e->pf_ring, s);  // rings handed over by chd_adopt_prefetched: ordered after their upload
+    if (st != CHD_OK) return st;
     chd_epoch_tick(e, s, EP_FANOUT);
     stage_begin_kernel<<<1, 1, 0, s>>>(e->d_time + 1, t_ns, e->d_epoch + EP_FANOUT, &e->d_ctr->n_due, 1, nullptr);
     KCHECK(e);
     const RingDev ring = chd_ring_view(e);
     const unsigned grid = (unsigned)e->sm_count * 16;
-    uint64_t key = mix_key(mix_key(mix_key(0x66616eull, S), (uint64_t)e->cur), e->have_ch_msg_index);
+    uint64_t key = mix_key(mix_key(mix_key(0x66616eull, S), (uint64_t)e->cur), ring.channel_msg_index != nullptr);
     for (const void* p : {(const void*)ring.off, (const void*)ring.end, (const void*)ring.arrival, (const void*)ring.sender, (const void*)ring.index,
                           (const void*)ring.channel_msg_index, (const void*)ring.start})
         key = mix_key(key, (uint64_t)(uintptr_t)p);  // pointers are baked into the captured launch
-    chd_status st = run_stage(e, s, e->g_fanout[e->cur + (e->ring_set == 1 ? 2 : 0)], key, [&]() -> chd_status {
+    st = run_stage(e, s, e->g_fanout[e->cur + (e->pf_ring.cur == 1 ? 2 : 0)], key, [&]() -> chd_status {
         const unsigned blocks = (unsigned)std::min<uint64_t>((P + 127) / 128, (uint64_t)e->sm_count * 16);
         fanout_kernel<<<blocks ? blocks : 1, 128, 0, s>>>(pb.off + S, P, pb, e->d_conn, ring, e->d_time + 1, e->g.id_start, e->d_by_cell, e->d_due,
                                                           e->d_due_key, e->lim.max_due, e->d_ctr);
         KCHECK(e);
         return CHD_OK;
     });
-    if (st == CHD_OK && e->ring_set >= 0) {
-        CU(e, cudaEventRecord(e->ev_ring_read[e->ring_set], s));
-        e->ring_read_recorded[e->ring_set] = true;
-    }
-    return st;
+    return st != CHD_OK ? st : chd_pf_note_read(e, e->pf_ring, e->pf_ring.cur, s);
 }
 
 chd_status chd_fanout_tick(chd_engine* e, int64_t t_ns) {
@@ -300,81 +314,42 @@ chd_status chd_fanout_tick(chd_engine* e, int64_t t_ns) {
 
 chd_status chd_prefetch_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
                               const uint64_t* index, const uint64_t* ch_msg_index) {
-    if (!e || !ring_off) return CHD_ERR_INVALID;
-    if (n_entries > e->lim.max_ring_entries) {
-        e->fail("%u ring entries > max_ring_entries %u", n_entries, e->lim.max_ring_entries);
-        return CHD_ERR_CAPACITY;
-    }
-    if (n_entries && (!arrival || !sender || !index)) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    chd_status st = chd_ensure_upload_stream(e);
+    chd_status st = check_rings(e, "chd_prefetch_rings", ring_off, n_entries, arrival, sender, index);
     if (st != CHD_OK) return st;
-    const int set = e->ring_next;
+    CU(e, cudaSetDevice(e->device));
+    int set = 0;
+    st = chd_pf_begin(e, e->pf_ring, &set);
+    if (st != CHD_OK) return st;
     chd_engine::RStage& r = e->ring_pf[set];
-    const uint64_t C = e->g.cells;
-    if (!e->ring_pf_alloc[set]) {
-        const uint64_t R = e->lim.max_ring_entries;
-        if (!(dalloc(e, &r.off, C + 1) && dalloc(e, &r.arrival, R) && dalloc(e, &r.sender, R) && dalloc(e, &r.index, R) && dalloc(e, &r.cmi, C)))
-            return CHD_ERR_CUDA;
-        e->ring_pf_alloc[set] = true;
-    }
-    if (e->ring_read_recorded[set]) CU(e, cudaStreamWaitEvent(e->up_stream, e->ev_ring_read[set], 0));
-    cudaStream_t us = e->up_stream;
-    CU(e, cudaMemcpyAsync(r.off, ring_off, sizeof(uint32_t) * (C + 1), cudaMemcpyDefault, us));
-    if (n_entries) {
-        CU(e, cudaMemcpyAsync(r.arrival, arrival, sizeof(int64_t) * n_entries, cudaMemcpyDefault, us));
-        CU(e, cudaMemcpyAsync(r.sender, sender, sizeof(uint32_t) * n_entries, cudaMemcpyDefault, us));
-        CU(e, cudaMemcpyAsync(r.index, index, sizeof(uint64_t) * n_entries, cudaMemcpyDefault, us));
-    }
-    if (ch_msg_index) CU(e, cudaMemcpyAsync(r.cmi, ch_msg_index, sizeof(uint64_t) * C, cudaMemcpyDefault, us));
-    CU(e, cudaEventRecord(e->ev_upload_rings, us));
-    e->staged_rings = true;
-    e->staged_ring_set = set;
-    e->staged_ring_total = n_entries;
-    e->staged_ring_cmi = ch_msg_index != nullptr;
-    e->ring_next = set ^ 1;
-    return CHD_OK;
+    const uint64_t C = e->g.cells, R = e->lim.max_ring_entries;
+    if (!r.cmi && !(dalloc(e, &r.off, C + 1) && dalloc(e, &r.arrival, R) && dalloc(e, &r.sender, R) && dalloc(e, &r.index, R) && dalloc(e, &r.cmi, C)))
+        return CHD_ERR_CUDA;  // (cmi is allocated last)
+    st = copy_rings(e, e->up_stream, r, ring_off, n_entries, arrival, sender, index, ch_msg_index);
+    return st != CHD_OK ? st : chd_pf_end(e, e->pf_ring);
 }
 
 chd_status chd_adopt_prefetched(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
-    if (!e->staged && !e->staged_q && !e->staged_rings) {
+    if (e->pf_pos.staged < 0 && e->pf_q.staged < 0 && e->pf_ring.staged < 0) {
         e->fail("chd_adopt_prefetched without a preceding chd_prefetch_entities / chd_prefetch_queries / chd_prefetch_rings");
         return CHD_ERR_STATE;
     }
     CU(e, cudaSetDevice(e->device));
-    if (e->staged_q) {  // consumed by the next chd_begin_interest / chd_update_interest called with q == NULL
-        e->adopted_qd = e->staged_qd;
-        e->adopted_q_set = e->staged_q_set;
-        e->have_adopted_q = true;
-        e->wait_q = true;
-        e->staged_q = false;
-    }
-    if (e->staged_rings) {
-        const chd_engine::RStage& r = e->ring_pf[e->staged_ring_set];
-        e->ring_off_p = r.off; e->ring_arrival_p = r.arrival; e->ring_sender_p = r.sender; e->ring_index_p = r.index;
-        e->ch_msg_index_p = e->staged_ring_cmi ? r.cmi : nullptr;
-        e->have_ch_msg_index = e->staged_ring_cmi;
-        e->ring_set = e->staged_ring_set;
-        e->wait_rings = true;
-        e->staged_rings = false;
-        set_u32_kernel<<<1, 1, 0, e->stream>>>(e->d_ring_total, e->staged_ring_total);
+    chd_pf_adopt(e->pf_q);  // consumed by the next chd_begin_interest / chd_update_interest called with q == NULL
+    if (chd_pf_adopt(e->pf_ring)) {
+        const chd_engine::RStage& r = e->ring_pf[e->pf_ring.cur];
+        e->ring = staged_ring(e, r);
+        set_u32_kernel<<<1, 1, 0, e->stream>>>(e->d_ring_total, r.total);
         KCHECK(e);
     }
-    if (!e->staged) return CHD_OK;
-    CU(e, cudaStreamWaitEvent(e->stream, e->ev_upload, 0));
-    e->pos_buf ^= 1;
-    e->d_x = e->d_xb[e->pos_buf];
-    e->d_z = e->d_zb[e->pos_buf];
+    if (!chd_pf_adopt(e->pf_pos)) return CHD_OK;
+    chd_status st = chd_pf_wait(e, e->pf_pos, e->stream);
+    if (st != CHD_OK) return st;
+    e->d_x = e->d_xb[e->pf_pos.cur];
+    e->d_z = e->d_zb[e->pf_pos.cur];
     e->pos_x = e->d_x;
     e->pos_z = e->d_z;
-    if (e->staged_n != e->n_own) e->have_prev_key = false;
-    e->n_own = e->staged_n;
-    e->n_halo = 0;
-    e->halo_on_device = false;
-    e->assigned = false;
-    e->entities_dirty = true;
-    e->staged = false;
+    chd_entities_replaced(e, e->pos_n[e->pf_pos.cur]);
     return CHD_OK;
 }
 
@@ -424,7 +399,7 @@ static chd_status aux_chain_enqueue(chd_engine* e, cudaStream_t s, const chd_que
 
 chd_status chd_begin_interest(chd_engine* e, const chd_query_batch* q, int64_t t_ns, int with_fanout) {
     if (!e) return CHD_ERR_INVALID;
-    if (!q && !e->have_adopted_q) {
+    if (!q && e->pf_q.cur < 0) {
         e->fail("chd_begin_interest: q == NULL needs chd_prefetch_queries + chd_adopt_prefetched first");
         return CHD_ERR_STATE;
     }

@@ -114,39 +114,29 @@ class Engine:
         return out
 
     # ---- entities / build
-    def set_entities(self, x, z, n=None):
+    def _upload_positions(self, fn, keep, dtype, x, z, n):
+        # numpy arrays are converted to `dtype`; the H2D copy is asynchronous, so the arrays stay referenced in `keep` until
+        # the next upload of the same kind
         if isinstance(x, np.ndarray):
-            x = np.ascontiguousarray(x, np.float64)
-            z = np.ascontiguousarray(z, np.float64)
+            x = np.ascontiguousarray(x, dtype)
+            z = np.ascontiguousarray(z, dtype)
         n = len(x) if n is None else n
-        self._keep = [x, z]  # async H2D: keep alive until the next call
-        self._ck(self.L.chd_set_entities(self.h, ptr(x), ptr(z), int(n)))
+        setattr(self, keep, [x, z])
+        self._ck(fn(self.h, ptr(x), ptr(z), int(n)))
+
+    def set_entities(self, x, z, n=None):
+        self._upload_positions(self.L.chd_set_entities, "_keep", np.float64, x, z, n)
 
     def prefetch_entities(self, x, z, n=None):
         """Start the H2D upload of the NEXT tick's positions (overlaps the tick in flight); see chd_prefetch_entities."""
-        if isinstance(x, np.ndarray):
-            x = np.ascontiguousarray(x, np.float64)
-            z = np.ascontiguousarray(z, np.float64)
-        n = len(x) if n is None else n
-        self._keep_prefetch = [x, z]
-        self._ck(self.L.chd_prefetch_entities(self.h, ptr(x), ptr(z), int(n)))
+        self._upload_positions(self.L.chd_prefetch_entities, "_keep_prefetch", np.float64, x, z, n)
 
     def set_entities_f32(self, x, z, n=None):
         """Positions that are floats at the source (unrealpb.FVector): uploaded as floats, widened exactly on the device."""
-        if isinstance(x, np.ndarray):
-            x = np.ascontiguousarray(x, np.float32)
-            z = np.ascontiguousarray(z, np.float32)
-        n = len(x) if n is None else n
-        self._keep = [x, z]
-        self._ck(self.L.chd_set_entities_f32(self.h, ptr(x), ptr(z), int(n)))
+        self._upload_positions(self.L.chd_set_entities_f32, "_keep", np.float32, x, z, n)
 
     def prefetch_entities_f32(self, x, z, n=None):
-        if isinstance(x, np.ndarray):
-            x = np.ascontiguousarray(x, np.float32)
-            z = np.ascontiguousarray(z, np.float32)
-        n = len(x) if n is None else n
-        self._keep_prefetch = [x, z]
-        self._ck(self.L.chd_prefetch_entities_f32(self.h, ptr(x), ptr(z), int(n)))
+        self._upload_positions(self.L.chd_prefetch_entities_f32, "_keep_prefetch", np.float32, x, z, n)
 
     def adopt_prefetched(self):
         self._ck(self.L.chd_adopt_prefetched(self.h))
@@ -211,14 +201,18 @@ class Engine:
     def emit_visible(self):
         self._ck(self.L.chd_emit_visible(self.h))
 
-    def set_rings(self, ring_off, arrival, sender, index, channel_msg_index=None):
+    def _upload_rings(self, fn, keep, ring_off, arrival, sender, index, channel_msg_index):
+        # the arrays stay referenced in `keep` until the next upload of the same kind (asynchronous H2D)
         ring_off = np.ascontiguousarray(ring_off, np.uint32)
         arrival = np.ascontiguousarray(arrival, np.int64)
         sender = np.ascontiguousarray(sender, np.uint32)
         index = np.ascontiguousarray(index, np.uint64)
         cmi = None if channel_msg_index is None else np.ascontiguousarray(channel_msg_index, np.uint64)
-        self._keep_ring = [ring_off, arrival, sender, index, cmi]
-        self._ck(self.L.chd_set_rings(self.h, ptr(ring_off), int(ring_off[-1]), ptr(arrival), ptr(sender), ptr(index), ptr(cmi)))
+        setattr(self, keep, [ring_off, arrival, sender, index, cmi])
+        self._ck(fn(self.h, ptr(ring_off), int(ring_off[-1]), ptr(arrival), ptr(sender), ptr(index), ptr(cmi)))
+
+    def set_rings(self, ring_off, arrival, sender, index, channel_msg_index=None):
+        self._upload_rings(self.L.chd_set_rings, "_keep_ring", ring_off, arrival, sender, index, channel_msg_index)
 
     def fanout_tick(self, t_ns):
         self._ck(self.L.chd_fanout_tick(self.h, int(t_ns)))
@@ -237,13 +231,7 @@ class Engine:
         self._ck(self.L.chd_prefetch_queries(self.h, C.byref(batch)))
 
     def prefetch_rings(self, ring_off, arrival, sender, index, channel_msg_index=None):
-        ring_off = np.ascontiguousarray(ring_off, np.uint32)
-        arrival = np.ascontiguousarray(arrival, np.int64)
-        sender = np.ascontiguousarray(sender, np.uint32)
-        index = np.ascontiguousarray(index, np.uint64)
-        cmi = None if channel_msg_index is None else np.ascontiguousarray(channel_msg_index, np.uint64)
-        self._keep_pf_ring = [ring_off, arrival, sender, index, cmi]
-        self._ck(self.L.chd_prefetch_rings(self.h, ptr(ring_off), int(ring_off[-1]), ptr(arrival), ptr(sender), ptr(index), ptr(cmi)))
+        self._upload_rings(self.L.chd_prefetch_rings, "_keep_pf_ring", ring_off, arrival, sender, index, channel_msg_index)
 
     def tick(self, batch, t_ns, flags=capi.TICK_ALL, want_summary=True):
         s = TickSummary() if want_summary else None

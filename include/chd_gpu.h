@@ -210,9 +210,11 @@ chd_status chd_emit_visible(chd_engine* e);
 chd_status chd_set_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival_ns,
                          const uint32_t* sender_conn_id, const uint64_t* message_index, const uint64_t* channel_msg_index);
 /* The same for the other per-tick inputs: the query batch (consumed by the next chd_begin_interest / chd_update_interest
- * called with q == NULL) and the update rings (arguments as chd_set_rings).  Each kind has two staging sets; a set is
- * refilled only after the tick that read it.  chd_adopt_prefetched hands over everything prefetched since the last
- * adoption (any subset of positions / queries / rings). */
+ * called with q == NULL) and the update rings (arguments as chd_set_rings; CHD_ERR_STATE on device-owned rings, see
+ * chd_rings_init).  Each kind has two staging sets: a prefetch fills the one not adopted last, and only after the work that
+ * last read it, so a host that prefetches for tick k+1 while tick k runs alternates between them and never waits for tick k.
+ * A second prefetch of one kind before an adoption replaces the first.  chd_adopt_prefetched hands over everything
+ * prefetched since the last adoption (any subset of positions / queries / rings). */
 chd_status chd_prefetch_queries(chd_engine* e, const chd_query_batch* q);
 chd_status chd_prefetch_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
                               const uint64_t* index, const uint64_t* ch_msg_index);

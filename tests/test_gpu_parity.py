@@ -845,7 +845,8 @@ def test_zero_copy_device_inputs_match_host_inputs(chd):
 def test_prefetched_inputs_match_direct_upload(chd):
     """chd_prefetch_{entities,queries,rings} + chd_adopt_prefetched (double-buffered uploads that overlap the tick in
     flight) give the same pairs, visible lists, fan-out decisions and handover lists as chd_set_entities / chd_set_rings /
-    an explicit query batch, tick after tick."""
+    an explicit query batch, tick after tick.  "mixed" switches between the two (a direct tick between prefetched ones) and
+    prefetches one tick's inputs twice, the first time with other data: the second upload is the one adopted."""
     wc = chd.synth.scaled(chd.synth.CONFIGS["benchmark"], 60_000, 5_000)
     ex, ez = chd.synth.entities(wc)
     conn, _, _, _ = chd.synth.subscribers(wc, ex, ez)
@@ -856,33 +857,39 @@ def test_prefetched_inputs_match_direct_upload(chd):
         _, cx, cz, r = chd.synth.subscribers(wc, ex, ez)
         ring_state, off, arr, snd, idx, cmi = chd.synth.update_rings(wc, tick, t, 33_000_000, 4, len(conn), ring_len=16, state=ring_state)
         frames.append(dict(t=t, x=ex.copy(), z=ez.copy(), q=(cx, cz, r), rings=(off, arr, snd, idx, cmi)))
+    plans = {"direct": ["direct"] * 7, "prefetch": ["prefetch"] * 7,
+             "mixed": ["prefetch", "prefetch", "direct", "prefetch", "prefetch", "twice", "prefetch"]}
     out = {}
-    for mode in ("direct", "prefetch"):
+    for mode, plan in plans.items():
         e = chd.engine.Engine(wc.cfg(), wc.n_entities, wc.n_subscribers, max_visible=1 << 24)
         e.set_subscribers(conn)
         res = []
 
-        def prefetch(f):
+        def prefetch(f, n=None):
             batch, keep = chd.engine.make_batch(len(f["q"][0]), sub=None, sphere=f["q"])
             e.prefetch_rings(*f["rings"])
             e.prefetch_queries(batch, keep)
-            e.prefetch_entities(f["x"], f["z"])
+            e.prefetch_entities(f["x"], f["z"], n)
 
-        if mode == "prefetch":
-            prefetch(frames[0])
+        def stage(tick):  # uploads the inputs of a prefetched tick ahead of it
+            if tick < len(frames) and plan[tick] != "direct":
+                if plan[tick] == "twice":
+                    prefetch(frames[0], len(frames[0]["x"]) - 1000)  # other positions (and fewer), queries and rings
+                prefetch(frames[tick])
+
+        stage(0)
         for tick, f in enumerate(frames):
-            if mode == "prefetch":
-                e.adopt_prefetched()
-                e.begin_interest(None, f["t"])
-                e._ck(e.L.chd_tick(e.h, None, f["t"], chd.capi.TICK_ALL | chd.capi.TICK_EARLY_RESULTS, None))  # asynchronous
-                if tick + 1 < len(frames):
-                    prefetch(frames[tick + 1])  # goes up while the tick runs
-                s = e.summary()
-            else:
+            if plan[tick] == "direct":
                 e.set_rings(*f["rings"])
                 e.set_entities(f["x"], f["z"])
                 batch, keep = chd.engine.make_batch(len(f["q"][0]), sub=None, sphere=f["q"])
-                s = e.tick(batch, f["t"], chd.capi.TICK_ALL)
+                e.tick(batch, f["t"], chd.capi.TICK_ALL, want_summary=False)
+            else:
+                e.adopt_prefetched()
+                e.begin_interest(None, f["t"])
+                e.tick(None, f["t"], chd.capi.TICK_ALL | chd.capi.TICK_EARLY_RESULTS, want_summary=False)  # asynchronous
+            stage(tick + 1)  # goes up while the tick runs
+            s = e.summary()
             pairs = e.get_pairs(s.n_pairs)
             voff, vis = e.get_visible()
             due = e.get_due(s.n_due)
@@ -895,12 +902,13 @@ def test_prefetched_inputs_match_direct_upload(chd):
         with pytest.raises(Exception):
             e.begin_interest(None, 1)  # no adopted batch
         out[mode] = res
-    for a, b in zip(out["direct"], out["prefetch"]):
-        assert a[0] == b[0]
-        for k in a[1]:
-            np.testing.assert_array_equal(a[1][k], b[1][k])
-        for i in (2, 3, 4, 5):
-            np.testing.assert_array_equal(a[i], b[i])
+    for mode in ("prefetch", "mixed"):
+        for a, b in zip(out["direct"], out[mode]):
+            assert a[0] == b[0], mode
+            for k in a[1]:
+                np.testing.assert_array_equal(a[1][k], b[1][k])
+            for i in (2, 3, 4, 5):
+                np.testing.assert_array_equal(a[i], b[i])
     assert sum(r[0]["n_handover"] for r in out["direct"]) > 100 and sum(r[0]["n_due"] for r in out["direct"]) > 1000
 
 

@@ -366,6 +366,12 @@ def test_device_owned_rings_and_channel_time_origins(chd, oracle):
     start = rng.integers(0, 500, cells).astype(np.int64) * MS  # every channel was created at a different wall time
     assert e.L.chd_set_channel_start_times(e.h, capi.ptr(start)) == capi.OK
     assert e.L.chd_rings_init(e.h, 1024) == capi.OK
+    # host-owned rings cannot be prefetched over device-owned ones: a short set (one entry) is refused, so nothing is staged
+    # and the device-owned rings keep all their entries (checked against the oracle below)
+    short_off = np.array([0] + [1] * cells, np.uint32)
+    short_arr, short_snd, short_idx = np.array([1000 * MS], np.int64), np.array([7], np.uint32), np.array([1], np.uint64)
+    assert e.L.chd_prefetch_rings(e.h, capi.ptr(short_off), 1, capi.ptr(short_arr), capi.ptr(short_snd), capi.ptr(short_idx), None) == capi.ERR_STATE
+    assert e.L.chd_adopt_prefetched(e.h) == capi.ERR_STATE
     chans = [oracle.channel() for _ in range(cells)]
     cx, cz = rng.uniform(20, 280, S), rng.uniform(20, 180, S)
     rad = rng.choice([30.0, 80.0], S)
