@@ -13,9 +13,13 @@
 //   mp     = 0x08 channelId  0x20 msgType  0x2A len(cdu) cdu   (MessagePack; broadcast = stubId = 0 are omitted, data.go:301-308)
 //   cdu    = 0x0A len(any) any                                 (ChannelDataUpdateMessage.data; contextConnId = 0 omitted)
 //   any    = 0x0A len(url) url  0x12 len(value) value          (google.protobuf.Any)
-// Valid for channel data types merged by the default reflection merge without merge options (data.go:326-388); custom
-// MergeableChannelData types stay on the host.  Byte-level equality with Go's marshal is NOT defined (field order of a merged
-// message, map order): parity is at message level (tests decode these bytes with the protobuf runtime and compare with MergeFrom).
+// Like proto3 Marshal, a channelId / msgType of 0 and an empty type_url / value are omitted, so every entry has the size the
+// reference's send rules measure.  Valid for channel data types merged by the default reflection merge without merge options
+// (data.go:326-388); custom MergeableChannelData types stay on the host.  The wrapper layers are fixed proto3 encodings, so for
+// a given `value` the class entry is fully determined and the tests compare it byte for byte with the protobuf runtime's
+// serialization.  Only `value` itself (the concatenation of the selected entries) can differ in bytes from what Go would send
+// after merging (field order of a merged message, map order); it parses to the same message.  The framing is checked against
+// a plain restatement of connection.go's Send / flush rules (tests/_wire.py).
 #pragma once
 #include "chd_types.cuh"
 
@@ -48,12 +52,16 @@ __device__ __forceinline__ uint8_t* put_varint(uint8_t* p, uint64_t v) {
 struct MsgSizes {
     uint64_t value, any, cdu, mp, entry;
 };
+// proto3 Marshal omits a scalar field equal to 0 and a bytes / string field that is empty; a set message field (Any inside
+// ChannelDataUpdateMessage) is written even when empty
+__device__ __forceinline__ uint64_t scalar_field_len(uint64_t v) { return v ? 1 + varint_len(v) : 0; }
+__device__ __forceinline__ uint64_t bytes_field_len(uint64_t len) { return len ? 1 + varint_len(len) + len : 0; }
 __device__ __forceinline__ MsgSizes msg_sizes(uint64_t value_len, uint32_t url_len, uint32_t channel_id, uint32_t msg_type) {
     MsgSizes s;
     s.value = value_len;
-    s.any = 1 + varint_len(url_len) + url_len + 1 + varint_len(value_len) + value_len;
+    s.any = bytes_field_len(url_len) + bytes_field_len(value_len);
     s.cdu = 1 + varint_len(s.any) + s.any;
-    s.mp = 1 + varint_len(channel_id) + 1 + varint_len(msg_type) + 1 + varint_len(s.cdu) + s.cdu;
+    s.mp = scalar_field_len(channel_id) + scalar_field_len(msg_type) + 1 + varint_len(s.cdu) + s.cdu;
     s.entry = 1 + varint_len(s.mp) + s.mp;
     return s;
 }
@@ -120,28 +128,16 @@ __global__ void __launch_bounds__(128)
     uint64_t value = 0;
     if (d.kind == 0) value = in.full_off[cell + 1] - in.full_off[cell];
     else for_each_selected(ring, ring_total, cell, dk.lo, d.window_hi, skipped, me, [&](uint32_t e) { value += in.entry_off[e + 1] - in.entry_off[e]; });
+    // all lanes copy the url and the value; lane 0 then writes the field headers in front of them (zero / empty fields
+    // omitted like msg_sizes counts them).  The entry ends with the url bytes and the value field, so the sizes give the
+    // header lengths.
     const MsgSizes s = msg_sizes(value, in.url_len, d.channel_id, in.msg_type);
-    uint8_t* out = blob + cls_off[k];
-    uint8_t* p = out;
-    // every lane computes the header layout (cheap); lane 0 writes it
-    uint8_t hdr[64];
-    uint8_t* h = hdr;
-    *h++ = 0x0A; h = put_varint(h, s.mp);
-    *h++ = 0x08; h = put_varint(h, d.channel_id);
-    *h++ = 0x20; h = put_varint(h, in.msg_type);
-    *h++ = 0x2A; h = put_varint(h, s.cdu);
-    *h++ = 0x0A; h = put_varint(h, s.any);
-    *h++ = 0x0A; h = put_varint(h, in.url_len);
-    const uint32_t h1 = (uint32_t)(h - hdr);
-    for (uint32_t b = lane; b < h1; b += 32) p[b] = hdr[b];
-    p += h1;
+    const uint64_t value_field = bytes_field_len(s.value);
+    uint8_t* const out = blob + cls_off[k];
+    uint8_t* const url_at = out + (s.entry - in.url_len - value_field);
+    uint8_t* p = url_at;
     for (uint32_t b = lane; b < in.url_len; b += 32) p[b] = in.type_url[b];
-    p += in.url_len;
-    h = hdr;
-    *h++ = 0x12; h = put_varint(h, s.value);
-    const uint32_t h2 = (uint32_t)(h - hdr);
-    for (uint32_t b = lane; b < h2; b += 32) p[b] = hdr[b];
-    p += h2;
+    p += in.url_len + (value_field - s.value);
     if (d.kind == 0) {
         const uint8_t* src = in.full_bytes + in.full_off[cell];
         for (uint64_t b = lane; b < value; b += 32) p[b] = src[b];
@@ -152,6 +148,16 @@ __global__ void __launch_bounds__(128)
             for (uint64_t b = lane; b < len; b += 32) p[b] = src[b];
             p += len;
         });
+    }
+    if (lane == 0) {
+        uint8_t* h = out;
+        *h++ = 0x0A; h = put_varint(h, s.mp);
+        if (d.channel_id) { *h++ = 0x08; h = put_varint(h, d.channel_id); }
+        if (in.msg_type) { *h++ = 0x20; h = put_varint(h, in.msg_type); }
+        *h++ = 0x2A; h = put_varint(h, s.cdu);
+        *h++ = 0x0A; h = put_varint(h, s.any);
+        if (in.url_len) { *h++ = 0x0A; put_varint(h, in.url_len); }
+        if (s.value) { h = url_at + in.url_len; *h++ = 0x12; put_varint(h, s.value); }
     }
 }
 
@@ -177,10 +183,17 @@ __global__ void __launch_bounds__(256) frame_fill_kernel(const chd_due* __restri
 // snappy.MaxEncodedLen (golang/snappy encode.go): 32 + n + n/6
 __host__ __device__ __forceinline__ uint32_t snappy_max_len(uint32_t n) { return 32u + n + n / 6u; }
 
+// Send drops a message whose MessagePack is MaxPacketSize - PacketHeaderSize bytes or longer (connection.go:73-77).  A class
+// entry is 0x0A, the MessagePack's length varint and the MessagePack, so its length grows strictly with the MessagePack's:
+// the MessagePack reaches the limit exactly when the entry is at least as long as an entry holding a limit-sized MessagePack.
+// (Lengths clamped to 0xFFFFFFFF by payload_size_kernel are dropped too.)
+constexpr uint32_t MP_DROP = PKT_MAX - PKT_HDR;
+__device__ __forceinline__ bool send_drops(uint32_t entry_len) { return entry_len >= 1 + varint_len(MP_DROP) + MP_DROP; }
+
 // Per connection: order its decisions (ascending due index: a deterministic stand-in for the reference's send-queue order,
 // which is unspecified across channel goroutines), cut them into packets of at most MaxPacketSize bytes (connection.go:643-659: a
-// message that would overflow the packet opens the next one; a single message >= MaxPacketSize - 5 is dropped like
-// connection.go:73-77 does) and reserve the connection's output region (worst case for compressed connections).
+// message that would overflow the packet opens the next one; a message send_drops() refuses is skipped wherever it stands)
+// and reserve the connection's output region (worst case for compressed connections).
 __global__ void __launch_bounds__(128)
     frame_size_kernel(uint32_t n_slots, const uint32_t* __restrict__ off, uint32_t* __restrict__ idx, const uint32_t* __restrict__ class_of,
                       const uint32_t* __restrict__ cls_len, const uint8_t* __restrict__ compression, uint32_t* __restrict__ conn_cap,
@@ -198,7 +211,7 @@ __global__ void __launch_bounds__(128)
     uint32_t total = 0, cur = 0, dropped = 0;
     for (uint32_t a = b; a < e; a++) {
         const uint32_t L = cls_len[class_of[idx[a]]];
-        if (L >= PKT_MAX - PKT_HDR) { dropped++; continue; }
+        if (send_drops(L)) { dropped++; continue; }
         if (cur + L > PKT_MAX) {
             total += PKT_HDR + (comp ? snappy_max_len(cur) : cur);
             cur = 0;
@@ -284,7 +297,7 @@ __global__ void __launch_bounds__(128)
         uint32_t cur = 0, a2 = a;
         while (a2 < e) {
             const uint32_t L = cls_len[class_of[idx[a2]]];
-            if (L >= PKT_MAX - PKT_HDR) { a2++; if (cur == 0) a = a2; continue; }  // dropped message (skipped wherever it stands)
+            if (send_drops(L)) { a2++; if (cur == 0) a = a2; continue; }  // dropped message (skipped wherever it stands)
             if (cur + L > PKT_MAX) break;
             cur += L;
             a2++;
@@ -295,22 +308,29 @@ __global__ void __launch_bounds__(128)
         for (uint32_t k = a; k < a2; k++) {
             const uint32_t c = class_of[idx[k]];
             const uint32_t L = cls_len[c];
-            if (L >= PKT_MAX - PKT_HDR) continue;
+            if (send_drops(L)) continue;
             const uint8_t* src = blob + cls_off[c];
             for (uint32_t i = lane; i < L; i += 32) body[wpos + i] = src[i];
             wpos += L;
         }
         __syncwarp();
         uint32_t body_len = cur;
+        bool snappy = false;
         if (comp) {
             for (int i = lane; i < (1 << SNAPPY_HASH_BITS); i += 32) s_table[w][i] = 0;
             __syncwarp();
             if (lane == 0) body_len = snappy_encode(body, cur, region + pos + PKT_HDR, s_table[w]);
             body_len = __shfl_sync(0xffffffffu, body_len, 0);
+            snappy = body_len <= PKT_MAX;
+            if (!snappy) {  // encoded body overflows the 16-bit size field: send the packet raw (chd_gpu.h, chd_frame_packets)
+                __syncwarp();
+                for (uint32_t i = lane; i < cur; i += 32) region[pos + PKT_HDR + i] = body[i];
+                body_len = cur;
+            }
         }
         if (lane == 0) {  // 'C' 'H' size_hi size_lo compressionType (connection.go:684-688)
             uint8_t* t = region + pos;
-            t[0] = 67; t[1] = 72; t[2] = (uint8_t)((body_len >> 8) & 0xff); t[3] = (uint8_t)(body_len & 0xff); t[4] = comp ? 1 : 0;
+            t[0] = 67; t[1] = 72; t[2] = (uint8_t)((body_len >> 8) & 0xff); t[3] = (uint8_t)(body_len & 0xff); t[4] = snappy ? 1 : 0;
         }
         pos += PKT_HDR + body_len;
         frames++;

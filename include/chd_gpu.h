@@ -518,12 +518,19 @@ chd_status chd_due_classes(chd_engine* e, uint32_t* out_class_of, uint32_t* out_
  *                           blob[class_off[k] .. class_off[k+1]) = one Packet.messages entry (0x0A len MessagePack{channelId,
  *                           msgType, msgBody = ChannelDataUpdateMessage{data = Any{type_url, value}}}) where value = the
  *                           concatenation of the selected ring entries' bytes (= proto.Merge of them, by the protobuf encoding
- *                           rules) or the channel's full data for a FULL send.  Outputs may be NULL (results stay on the GPU).
+ *                           rules) or the channel's full data for a FULL send.  Fields equal to 0 or empty are omitted as proto3
+ *                           Marshal omits them, so the entry is byte for byte the protobuf serialization of that Packet.
+ *                           Outputs may be NULL (results stay on the GPU).
  *   chd_frame_packets       per connection (subscriber slot s): bytes out[conn_off[s] .. conn_off[s] + conn_len[s]) = its packets
- *                           back to back, each 5-byte tag + body; a packet holds as many of the connection's messages as fit
- *                           MaxPacketSize (0xffff), a single message >= MaxPacketSize - 5 is dropped (connection.go:73-77; counted
- *                           in *n_dropped); compression[s] = 1 -> snappy block format (decodes with any snappy decoder; the bytes
- *                           differ from Go's encoder).  conn_off is spaced for the worst case; conn_frames[s] = packets written.
+ *                           back to back, each 5-byte tag + body, messages in ascending due index; a packet holds as many of
+ *                           the connection's messages as fit MaxPacketSize (0xffff), a message whose MessagePack is
+ *                           >= MaxPacketSize - 5 bytes is dropped (connection.go:73-77; counted in *n_dropped); compression[s] = 1
+ *                           -> snappy block format (decodes with any snappy decoder; the bytes differ from Go's encoder).
+ *                           Deviation: a packet whose snappy encoding would exceed MaxPacketSize is sent uncompressed, with
+ *                           compressionType 0 in its tag (readers decide per packet from the tag: connection.go:497-513,
+ *                           client.go:208).  The reference writer refuses such a packet (connection.go:688-691) and its messages
+ *                           are lost; Go's encoder rarely produces one, this engine's simpler encoder can on incompressible
+ *                           bodies near 64 KB.  conn_off is spaced for the worst case; conn_frames[s] = packets written.
  * Valid for channel data types merged by the default reflection merge without ChannelDataMergeOptions (data.go:326-388);
  * types with a custom Merge stay on the host.  Synchronous; buffers of this stage grow on demand. */
 chd_status chd_set_payload_bytes(chd_engine* e, const uint64_t* entry_off, uint32_t n_entries, const uint8_t* entry_bytes, const uint64_t* full_off,

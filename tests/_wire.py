@@ -54,3 +54,44 @@ def _build():
 Packet, MessagePack, ChannelDataUpdateMessage, TestChannelDataMessage = _build()
 TYPE_URL = "type.googleapis.com/chdtest.TestChannelDataMessage"
 MSG_CHANNEL_DATA_UPDATE = 8  # channeld.proto:121
+
+# ---- connection.go's send rules, restated with the protobuf runtime measuring every size
+MAX_PACKET_SIZE = 0x00FFFF  # connection.go:27
+PACKET_HEADER_SIZE = 5      # connection.go:28
+
+
+def message_pack(channel_id, value, type_url=TYPE_URL, msg_type=MSG_CHANNEL_DATA_UPDATE):
+    """The MessagePack Send builds for a CHANNEL_DATA_UPDATE whose Any.value is `value` (data.go:293-318, connection.go:58-71)."""
+    body = ChannelDataUpdateMessage(data=any_pb2.Any(type_url=type_url, value=value)).SerializeToString()
+    return MessagePack(channelId=channel_id, msgType=msg_type, msgBody=body)
+
+
+def class_entry(channel_id, value, type_url=TYPE_URL, msg_type=MSG_CHANNEL_DATA_UPDATE):
+    """The bytes of that MessagePack as one Packet.messages entry: a Packet holding only it, serialized."""
+    return Packet(messages=[message_pack(channel_id, value, type_url, msg_type)]).SerializeToString()
+
+
+def flush(mps):
+    """One connection's MessagePacks in queue order -> (serialized packets, number dropped).
+    Send (connection.go:73-77) drops a MessagePack of proto.Size >= MaxPacketSize - PacketHeaderSize; flush (:640-660) appends
+    to the packet and, when proto.Size(packet) then exceeds MaxPacketSize, takes the message back out and opens the next
+    packet with it."""
+    packets, cur, dropped = [], Packet(), 0
+    for mp in mps:
+        if mp.ByteSize() >= MAX_PACKET_SIZE - PACKET_HEADER_SIZE:
+            dropped += 1
+            continue
+        cur.messages.append(mp)
+        if cur.ByteSize() > MAX_PACKET_SIZE:
+            del cur.messages[-1]
+            packets.append(cur.SerializeToString())
+            cur = Packet(messages=[mp])
+    if len(cur.messages):
+        packets.append(cur.SerializeToString())
+    return packets, dropped
+
+
+def frame(packet, compression_type=0):
+    """'C' 'H' size_hi size_lo compressionType + body (connection.go:684-688)."""
+    assert len(packet) <= MAX_PACKET_SIZE
+    return bytes([67, 72, len(packet) >> 8, len(packet) & 0xFF, compression_type]) + packet
