@@ -54,13 +54,10 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
     chd_status st = chd_epoch_tick(e, s, EP_DELTA);
     if (st != CHD_OK) return st;
     // sizes and the key / pair buffers in use are baked into the captured launches
-    uint64_t key = mix_key(mix_key(mix_key(mix_key(0x64656c7461ull, d.n), d.n_slots), D.n_out), (uint64_t)e->cur);
-    key = mix_key(mix_key(mix_key(key, (uint64_t)(uintptr_t)d.key), (uint64_t)(uintptr_t)d.enter), (uint64_t)(uintptr_t)d.leave);
-    key = mix_key(mix_key(key, d.enter_cap), d.leave_cap);
-    const int slot = (e->d_key == e->d_key_a ? 0 : 1) + 2 * e->cur;
+    const uint64_t key = stage_key(0x64656c7461ull, d.n, d.n_slots, D.n_out, e->cur, d.key, d.enter, d.leave, d.enter_cap, d.leave_cap);
     const unsigned grid = (unsigned)e->sm_count * 8;
     const unsigned slot_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(blocks_for((uint64_t)D.n_out * 32, DELTA_THREADS), (uint64_t)e->sm_count * 32));
-    return run_stage(e, s, D.g[slot], key, [&]() -> chd_status {
+    return run_stage(e, s, D.g, key, [&]() -> chd_status {
         bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_DELTA);
         KCHECK(e);
         SCAN(e, exclusive_scan_fn<DeltaArrivalFlag, uint32_t>(DeltaArrivalFlag{d.sorted, d.key, d.snap_key, d.snap_hdr, C}, D.arr_rank, N, D.site_arr, s,

@@ -298,7 +298,6 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
          chd_make_site(e, e->site_border, N + 1, EP_BORDER) &&
          dalloc(e, &e->d_ho_entity, N) && dalloc(e, &e->d_ho_src, N) && dalloc(e, &e->d_ho_dst, N) &&
          dalloc(e, &e->d_bflag, N + 1) && dalloc(e, &e->d_boff, N + 2);
-    e->d_key_a = e->d_key;
     ok = ok && dalloc(e, &e->d_conn, S) && dalloc(e, &e->d_slot_ctl, S) && dalloc(e, &e->d_slot_src, S) && dalloc(e, &e->d_lc_slot, S) &&
          dalloc(e, &e->d_lc_aux, S) && alloc_pairbuf(e, e->pairs[0]) && alloc_pairbuf(e, e->pairs[1]);
     ok = ok && alloc_qstage(e, e->dq);

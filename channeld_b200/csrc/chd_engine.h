@@ -60,11 +60,13 @@ struct chd_engine {
     int sm_count = 132;
     int l2_bytes = 50 << 20;  // both read from the device in chd_create
     uint64_t n_launch = 0;  // kernels launched by this engine (bench.py reports it as gpu_launches)
-    // CUDA graphs: the launch-bound small-kernel stages are captured once per (shape, parity) and replayed.
+    // CUDA graphs: the launch-bound small-kernel stages are captured per key and replayed (run_stage).  A slot holds one key:
+    // pending (exec == nullptr) or captured; key 0 marks a free slot.
     struct GraphSlot {
         cudaGraphExec_t exec = nullptr;
-        uint64_t key = 0, pending_key = 0;
+        uint64_t key = 0;
         uint64_t nodes = 0;
+        uint64_t used = 0;  // GraphSet::clock at this slot's last lookup
         GraphSlot() = default;
         GraphSlot(const GraphSlot&) = delete;
         GraphSlot& operator=(const GraphSlot&) = delete;
@@ -74,13 +76,16 @@ struct chd_engine {
             exec = nullptr;
         }
     };
+    struct GraphSet {  // the graphs of one run_stage call site
+        GraphSlot slot[8];
+        uint64_t clock = 0;
+    };
     bool use_graphs = true;
     cudaStream_t aux_stream = nullptr;
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_interest = nullptr, ev_pairs = nullptr;
     bool interest_pending = false, pending_fanout = false;  // chd_begin_interest issued, not yet joined by chd_tick
-    GraphSlot g_build[4], g_build_b[4], g_interest[4], g_interest_b[4], g_emit_prep[2], g_fanout[4], g_export[8], g_import[4];  // build / export: [key buffer][position buffer]
+    GraphSet g_build, g_build_b, g_interest, g_interest_b, g_emit_prep, g_fanout, g_export, g_import;
     uint64_t graph_launches = 0, graph_captures = 0;
-    uint32_t* d_key_a = nullptr;  // identity of the first key buffer (graph slot selection)
     int64_t* d_time = nullptr;      // [0] = now_ns of the last update_interest, [1] = t_ns of the last fanout_tick
     uint32_t* d_ring_total = nullptr;
     // optional per-stage CUDA-event timing (chd_profile_*): [stage][0=start,1=stop]
@@ -282,7 +287,7 @@ struct chd_engine {
         uint64_t enter_cap = 0, leave_cap = 0;
         uint32_t n_out = 0;  // slots the output CSRs cover: max(slots now, slots at any earlier delta) (never shrinks)
         ScanSite site_arr{}, site_dep{}, site_enter{}, site_leave{};
-        GraphSlot g[4];  // [key buffer][pair-buffer parity]
+        GraphSet g;
         cudaEvent_t ev_in = nullptr, ev_done = nullptr;  // two-stream tick: the build is done / the delta is done
         bool done_recorded = false;  // the last tick ran the delta off the engine stream: its end (and CHD_OVF_DELTA) is ev_done
     } dl;
@@ -449,36 +454,44 @@ static bool ensure_cap(chd_engine* e, T** p, uint64_t* cap, uint64_t need, uint6
 
 static inline unsigned blocks_for(uint64_t n, unsigned threads) { return (unsigned)((n + threads - 1) / threads); }
 
-// Replayable cell assignments (build, border export) are captured per [key buffer the new keys go to][front position pair]:
-// returns the graph slot and that key buffer.
-static inline int assign_graph_slot(const chd_engine* e, uint32_t** target) {
-    *target = e->have_prev_key ? e->d_prev_key : e->d_key;
-    return (*target == e->d_key_a ? 0 : 1) + 2 * e->pf_pos.cur;
-}
-
 static inline uint64_t mix_key(uint64_t h, uint64_t v) {
     h ^= v + 0x9E3779B97F4A7C15ull + (h << 6) + (h >> 2);
     return h;
 }
+static inline uint64_t key_word(uint64_t v) { return v; }
+static inline uint64_t key_word(const void* p) { return (uint64_t)(uintptr_t)p; }
+
+// A graph key: `tag` with each value mixed in turn (a pointer as its address).
+template <typename... V>
+static inline uint64_t stage_key(uint64_t tag, V... v) {
+    uint64_t h = tag;
+    ((h = mix_key(h, key_word(v))), ...);
+    return h;
+}
 
 // Runs `enqueue` (kernel launches + memsets on `s` only, no host sync) either directly or as a CUDA graph replayed on `s`.
-// A graph is captured only after the same key was seen twice in a row, so workloads whose batch shape changes
-// every tick simply run direct launches.
+// The key is a graph's only identity (it covers every pointer and size the launches bake in): each call site keeps up to 8
+// keys in its GraphSet, captures a key at its second sighting and replays it from then on, and gives a key it does not hold
+// the least recently used slot and direct launches, so a shape that changes every tick runs direct launches.
 template <typename F>
-static chd_status run_stage(chd_engine* e, cudaStream_t s, chd_engine::GraphSlot& slot, uint64_t key, F&& enqueue) {
+static chd_status run_stage(chd_engine* e, cudaStream_t s, chd_engine::GraphSet& set, uint64_t key, F&& enqueue) {
     key |= 1;  // never 0
     if (!e->use_graphs || s == nullptr) return enqueue();
-    if (slot.exec && slot.key == key) {
-        CU(e, cudaGraphLaunch(slot.exec, s));
-        e->n_launch += slot.nodes;
+    chd_engine::GraphSlot* slot = &set.slot[0];  // the slot holding this key, else the least recently used one
+    for (chd_engine::GraphSlot& g : set.slot)
+        if (g.key == key || (slot->key != key && g.used < slot->used)) slot = &g;
+    slot->used = ++set.clock;
+    if (slot->key != key) {  // first sighting: run direct, capture next time
+        slot->release();
+        slot->key = key;
+        return enqueue();
+    }
+    if (slot->exec) {
+        CU(e, cudaGraphLaunch(slot->exec, s));
+        e->n_launch += slot->nodes;
         e->graph_launches++;
         return CHD_OK;
     }
-    if (slot.pending_key != key) {  // first sighting: run direct, capture next time
-        slot.pending_key = key;
-        return enqueue();
-    }
-    slot.release();
     const uint64_t l0 = e->n_launch;
     // Stateless entry points (chd_cell_of, chd_query_channel_ids) may be called from other threads and launch into the engine
     // stream: they hold the engine mutex for their whole call, so taking it here keeps their work out of the capture.
@@ -498,21 +511,20 @@ static chd_status run_stage(chd_engine* e, cudaStream_t s, chd_engine::GraphSlot
         e->n_launch = l0;
         return st == CHD_OK ? enqueue() : st;
     }
-    r = cudaGraphInstantiate(&slot.exec, g, 0);
+    r = cudaGraphInstantiate(&slot->exec, g, 0);
     cudaGraphDestroy(g);
     if (r != cudaSuccess) {
-        slot.exec = nullptr;
+        slot->exec = nullptr;
         e->use_graphs = false;
         cudaGetLastError();
         e->n_launch = l0;
         return enqueue();
     }
-    slot.nodes = e->n_launch - l0;
+    slot->nodes = e->n_launch - l0;
     e->n_launch = l0;
-    slot.key = key;
     e->graph_captures++;
-    CU(e, cudaGraphLaunch(slot.exec, s));
-    e->n_launch += slot.nodes;
+    CU(e, cudaGraphLaunch(slot->exec, s));
+    e->n_launch += slot->nodes;
     e->graph_launches++;
     return CHD_OK;
 }

@@ -347,29 +347,26 @@ chd_status chd_build_on(chd_engine* e, cudaStream_t s) {
     if (st != CHD_OK) return st;
     bool counts_recorded = false;
     if (!e->assigned && !e->halo_on_device) {
-        // single-GPU flow: assign + sort as one replayable graph.  The key buffers swap every assignment
-        // (handover detection compares against the previous keys), so there are two graph variants.
-        uint32_t* target = nullptr;  // buffer the new keys will be written to
-        const int slot = assign_graph_slot(e, &target);
-        uint64_t key = mix_key(mix_key(mix_key(0x6275696c64ull, e->n_own), e->have_gid), e->have_prev_key);
-        key = mix_key(mix_key(key, (uint64_t)(uintptr_t)target), (uint64_t)(uintptr_t)e->pos_x ^ ((uint64_t)(uintptr_t)e->pos_z << 1));
+        // single-GPU flow: assign + sort as one replayable graph.  The key buffers swap every assignment (handover detection
+        // compares against the previous keys); the graph bakes in the sizes, the buffer the new keys go to and the positions.
+        const uint64_t key = stage_key(0x6275696c64ull, e->n_own, e->have_gid, e->have_prev_key, e->have_prev_key ? e->d_prev_key : e->d_key,
+                                       e->pos_x, e->pos_z);
         // single-pass builds (<= 1023 cells) run as two replayable halves with an event in between: the cell CSR offsets are
         // final after the first (assignment + histogram + scan), so the emit preparation overlaps the scatter
         const bool split = e->g.cells + 1 <= BUILD_MAX_BINS && e->n_own > 0;
-        st = run_stage(e, s, e->g_build[slot], key, [&]() { return build_enqueue(e, s, true, split ? 1 : 0); });
+        st = run_stage(e, s, e->g_build, key, [&]() { return build_enqueue(e, s, true, split ? 1 : 0); });
         if (st == CHD_OK && !e->assigned) chd_assign_host(e);  // replayed graph
         if (st == CHD_OK && split) {
             CU(e, cudaEventRecord(e->ev_counts, s));
             counts_recorded = true;
-            st = run_stage(e, s, e->g_build_b[slot], mix_key(key, 0x62), [&]() { return build_enqueue(e, s, false, 2); });
+            st = run_stage(e, s, e->g_build_b, stage_key(key, 0x62), [&]() { return build_enqueue(e, s, false, 2); });
         }
         if (st == CHD_OK) st = chd_note_pos_read(e, s);
     } else if (e->assigned && e->halo_on_device) {
         // multi-GPU flow: cells were assigned by chd_export_border and the halo appended on the device; the sort over
         // own + halo entities is sized by capacity (device-side length) and therefore replayable as well.
-        const int slot = e->d_key == e->d_key_a ? 0 : 1;
-        uint64_t key = mix_key(mix_key(mix_key(0x736f7274ull, e->lim.max_entities), e->have_gid), (uint64_t)(uintptr_t)e->d_key);
-        st = run_stage(e, s, e->g_build[slot], key, [&]() { return build_enqueue(e, s, false); });
+        const uint64_t key = stage_key(0x736f7274ull, e->lim.max_entities, e->have_gid, e->d_key);
+        st = run_stage(e, s, e->g_build, key, [&]() { return build_enqueue(e, s, false); });
     } else {
         const bool with_assign = !e->assigned;
         st = build_enqueue(e, s, with_assign);

@@ -336,22 +336,19 @@ chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query
         st = upload_queries(e, s, q, &d, true);  // H2D / D2D copies into the engine's SoA: outside the graph
         if (st != CHD_OK) return st;
     }
-    const int gslot = e->cur + (pf_set == 1 ? 2 : 0);
     // (outside the replayed graphs: the tick time is a launch argument) tick time, new scan epoch, zeroed counters
     // n_query_errors / n_sub_new / n_unsub / n_kept and window cursor
     chd_epoch_tick(e, s, EP_QUERY);
     stage_begin_kernel<<<1, 1, 0, s>>>(e->d_time, now_ns, e->d_epoch + EP_QUERY, &e->d_ctr->n_query_errors, 4, e->d_win_cursor);
     KCHECK(e);
     // the graph bakes in which staging arrays are live, the batch size and the pair-buffer parity
-    uint64_t key = mix_key(mix_key(mix_key(0x696e74ull, d.n), e->n_slots), (uint64_t)e->cur);
-    key = mix_key(mix_key(mix_key(key, e->lifecycle_used), (uint64_t)(uintptr_t)e->mig.base), e->have_cell_start);
-    const void* baked[] = {d.sub, d.kind, d.sph_cx, d.sph_cz, d.sph_r, d.box_cx, d.box_cz, d.box_ex, d.box_ez, d.cone_cx, d.cone_cz,
-                           d.cone_dx, d.cone_dz, d.cone_angle, d.cone_r, d.spot_off, d.spot_ndist, d.spot_x, d.spot_z, d.spot_dist};
-    for (const void* p : baked) key = mix_key(key, (uint64_t)(uintptr_t)p);  // pointers are baked into the captured launches
-    st = run_stage(e, s, e->g_interest[gslot], key, [&]() { return interest_enqueue(e, s, d, 0); });
+    const uint64_t key = stage_key(0x696e74ull, d.n, e->n_slots, e->cur, e->lifecycle_used, e->mig.base, e->have_cell_start, d.sub, d.kind, d.sph_cx,
+                                   d.sph_cz, d.sph_r, d.box_cx, d.box_cz, d.box_ex, d.box_ez, d.cone_cx, d.cone_cz, d.cone_dx, d.cone_dz, d.cone_angle,
+                                   d.cone_r, d.spot_off, d.spot_ndist, d.spot_x, d.spot_z, d.spot_dist);
+    st = run_stage(e, s, e->g_interest, key, [&]() { return interest_enqueue(e, s, d, 0); });
     if (st != CHD_OK) return st;
     CU(e, cudaEventRecord(e->ev_pairs, s));  // the new pairs exist: emit may start (chd_tick waits on this)
-    st = run_stage(e, s, e->g_interest_b[gslot], mix_key(key, 0xb), [&]() { return interest_enqueue(e, s, d, 1); });
+    st = run_stage(e, s, e->g_interest_b, stage_key(key, 0xb), [&]() { return interest_enqueue(e, s, d, 1); });
     if (st != CHD_OK) return st;
     st = chd_pf_note_read(e, e->pf_q, pf_set, s);  // the staging set may be refilled once these kernels have run
     if (st != CHD_OK) return st;

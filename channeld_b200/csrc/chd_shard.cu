@@ -107,15 +107,11 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
     chd_status st = chd_epoch_tick(e, s, EP_BORDER);
     if (st != CHD_OK) return st;
     if (!e->assigned) {
-        // replayable: cell assignment + border selection of one tick (two variants: the key buffers ping-pong)
-        uint32_t* target = nullptr;
-        const int slot = assign_graph_slot(e, &target);
-        uint64_t key = mix_key(mix_key(mix_key(0x6578706full, n), e->have_gid), e->have_prev_key);
-        key = mix_key(mix_key(key, (uint64_t)(uintptr_t)target), (uint64_t)(uintptr_t)e->pos_x ^ ((uint64_t)(uintptr_t)e->pos_z << 1));
-        key = mix_key(mix_key(key, (uint64_t)(uintptr_t)d_records), cap_records);
-        key = mix_key(mix_key(mix_key(key, e->g.col_lo), e->g.col_hi), e->g.halo);
-        key = mix_key(key, to_peers ? 1 : 0);
-        st = run_stage(e, s, e->g_export[slot + (to_peers ? 4 : 0)], key, enqueue);
+        // replayable: cell assignment + border selection of one tick.  The graph bakes in the sizes, the key buffer the new keys
+        // go to, the positions, the records, the slab and the exchange path.
+        const uint64_t key = stage_key(0x6578706full, n, e->have_gid, e->have_prev_key, e->have_prev_key ? e->d_prev_key : e->d_key, e->pos_x, e->pos_z,
+                                       d_records, cap_records, e->g.col_lo, e->g.col_hi, e->g.halo, to_peers);
+        st = run_stage(e, s, e->g_export, key, enqueue);
         if (st == CHD_OK && !e->assigned) chd_assign_host(e);  // replayed graph
         if (st == CHD_OK) st = chd_note_pos_read(e, s);
     } else {
@@ -152,16 +148,12 @@ chd_status chd_import_halo(chd_engine* e, const uint32_t* d_records, uint32_t n_
     {
         chd_status st0 = chd_epoch_tick(e, s, EP_BORDER);
         if (st0 != CHD_OK) return st0;
-        const int slot = e->d_key == e->d_key_a ? 0 : 1;  // the halo keys are appended to the current key buffer
         // peer exchange: the records sit in this tick's buffer of the own window, the live counts come from the flags
         const bool from_peers = e->peer_push && d_records >= e->d_peer_win && d_records < e->d_peer_win + 2ull * e->comm_world * e->rec_stride_words;
-        const int parity = from_peers && d_records != e->d_peer_win ? 1 : 0;
-        uint64_t key = mix_key(mix_key(mix_key(0x696d706full, n_records), skip_first), skip_count);
-        key = mix_key(mix_key(key, e->rec_per_rank), e->rec_stride_words);
-        key = mix_key(mix_key(mix_key(key, (uint64_t)(uintptr_t)d_records), e->n_own), (uint64_t)(uintptr_t)e->d_key);
-        key = mix_key(mix_key(mix_key(key, e->g.col_lo), e->g.col_hi), e->g.halo);
-        key = mix_key(key, from_peers ? 1 : 0);
-        chd_status st = run_stage(e, s, e->g_import[slot + 2 * parity], key, [&]() -> chd_status {
+        // the graph bakes in the sizes, the records, the key buffer the halo keys are appended to, the slab and the exchange path
+        const uint64_t key = stage_key(0x696d706full, n_records, skip_first, skip_count, e->rec_per_rank, e->rec_stride_words, d_records, e->n_own,
+                                       e->d_key, e->g.col_lo, e->g.col_hi, e->g.halo, from_peers);
+        chd_status st = run_stage(e, s, e->g_import, key, [&]() -> chd_status {
             const RecView rv{d_records, e->rec_per_rank ? e->rec_per_rank : (n_records ? n_records : 1u),
                              e->rec_per_rank ? e->rec_stride_words : 2ull * (n_records ? n_records : 1u)};
             if (from_peers) {  // (the push kernel of this tick has bumped the compaction site's epoch)

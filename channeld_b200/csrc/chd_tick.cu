@@ -28,10 +28,10 @@ static chd_status emit_prep_enqueue(chd_engine* e, cudaStream_t s, bool cta_tile
     const uint64_t P = e->lim.max_pairs;
     const unsigned grid = (unsigned)e->sm_count * 8;
     const uint32_t tile = cta_tiles ? (uint32_t)EMIT_TILE : (uint32_t)EMIT_WARP_TILE;
-    const uint64_t key = mix_key(mix_key(mix_key(mix_key(0x656d6974ull, S), (uint64_t)e->cur), cta_tiles), (uint64_t)(uintptr_t)s);
+    const uint64_t key = stage_key(0x656d6974ull, S, e->cur, cta_tiles, s);
     chd_status st = chd_epoch_tick(e, s, EP_EMIT);
     if (st != CHD_OK) return st;
-    return run_stage(e, s, e->g_emit_prep[e->cur], key, [&]() -> chd_status {
+    return run_stage(e, s, e->g_emit_prep, key, [&]() -> chd_status {
         // per-pair visible counts are computed by the scan itself; the partition pass opens the next epoch
         SCAN(e, exclusive_scan_fn<PairVcountIn, uint64_t>(PairVcountIn{pb.cell, e->d_cell_start}, e->d_voff, P, e->site_voff, s, pb.off + S));
         emit_partition_kernel<<<grid, 256, 0, s>>>(pb.off + S, P, e->d_voff, pb.cell, e->d_cell_start, e->d_first_pair, cta_tiles ? e->d_tile_desc : nullptr,
@@ -291,11 +291,10 @@ static chd_status fanout_enqueue(chd_engine* e, cudaStream_t s, int64_t t_ns) {
     KCHECK(e);
     const RingDev ring = chd_ring_view(e);
     const unsigned grid = (unsigned)e->sm_count * 16;
-    uint64_t key = mix_key(mix_key(mix_key(0x66616eull, S), (uint64_t)e->cur), ring.channel_msg_index != nullptr);
-    for (const void* p : {(const void*)ring.off, (const void*)ring.end, (const void*)ring.arrival, (const void*)ring.sender, (const void*)ring.index,
-                          (const void*)ring.channel_msg_index, (const void*)ring.start})
-        key = mix_key(key, (uint64_t)(uintptr_t)p);  // pointers are baked into the captured launch
-    st = run_stage(e, s, e->g_fanout[e->cur + (e->pf_ring.cur == 1 ? 2 : 0)], key, [&]() -> chd_status {
+    // the graph bakes in the slot count, the pair-buffer parity and the ring pointers
+    const uint64_t key = stage_key(0x66616eull, S, e->cur, ring.channel_msg_index != nullptr, ring.off, ring.end, ring.arrival, ring.sender, ring.index,
+                                   ring.channel_msg_index, ring.start);
+    st = run_stage(e, s, e->g_fanout, key, [&]() -> chd_status {
         const unsigned blocks = (unsigned)std::min<uint64_t>((P + 127) / 128, (uint64_t)e->sm_count * 16);
         fanout_kernel<<<blocks ? blocks : 1, 128, 0, s>>>(pb.off + S, P, pb, e->d_conn, ring, e->d_time + 1, e->g.id_start, e->d_by_cell, e->d_due,
                                                           e->d_due_key, e->lim.max_due, e->d_ctr);
