@@ -151,12 +151,12 @@ __device__ __forceinline__ void emit_tile_general(uint64_t t, uint64_t n_tiles, 
     }
 }
 
-// One CTA per 8 KB tile of the output (EMIT_TILE = 2048 entries: EMIT_ROWS rows of 256 x 16 bytes), dispatched by the
-// hardware block scheduler.  Streaming stores (st.global.cs) keep the write stream from evicting the L2-resident sources.
-// This kernel copies the SIMPLE tiles only (at most two segments: everything a thread needs is the 16-byte descriptor
-// {src0, src1, ends, p0}); tiles with more segments are listed by the partition pass and copied by
-// emit_visible_general_kernel.  The loop only runs more than once if the host under-estimated the tile count when it sized
-// the grid.
+// EMIT_TILES_PER_CTA 8 KB tiles of the output per CTA (EMIT_TILE = 2048 entries: EMIT_ROWS rows of 256 x 16 bytes), the CTAs
+// dispatched by the hardware block scheduler.  Streaming stores (st.global.cs) keep the write stream from evicting the
+// L2-resident sources.  This kernel copies the SIMPLE tiles only (at most two segments: everything a thread needs is the
+// 16-byte descriptor {src0, src1, ends, p0}); tiles with more segments are listed by the partition pass and copied by
+// emit_visible_general_kernel.  CTA b copies tiles b, b + grid, ...; the loop runs more often than EMIT_TILES_PER_CTA only if
+// the host under-estimated the tile count when it sized the grid.
 // A chunk that starts m = src & 3 entries into an aligned 16-byte chunk a takes the rest from chunk a + 1, which the next lane
 // loaded already (shuffle); lane 31, and a lane whose neighbour reads elsewhere, loads it itself.  (Keeping the sources at
 // 4 B x N is what keeps them in L2 next to the write stream: with 16 B x N the same kernel ran 25 % slower, DESIGN §8.)
@@ -176,6 +176,9 @@ __global__ void __launch_bounds__(EMIT_THREADS, CHD_EMIT_MIN_BLOCKS)
     const uint32_t tid4 = threadIdx.x * 4, lane = threadIdx.x & 31;
     for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
         if (t != blockIdx.x) dw = __ldg(reinterpret_cast<const uint4*>(desc + t));
+        // the next tile's descriptor is pulled into L1 while this tile is copied (no register held for it): a CTA that copies
+        // several tiles then waits for one round trip to L2 per tile instead of two dependent ones
+        if (t + gridDim.x < n_tiles) asm volatile("prefetch.global.L1 [%0];" ::"l"(desc + t + gridDim.x));
         if (dw.z & 0x80000000u) continue;  // CTA-uniform: a general tile
         const uint32_t end0 = dw.z & 0x7FFFu, end1 = (dw.z >> 16) & 0x7FFFu;  // a simple tile's second segment reaches the end of the tile / list
         uint32_t* __restrict__ out = vis_entity + (uint64_t)t * EMIT_TILE;

@@ -48,7 +48,7 @@ static chd_status emit_kernel_enqueue(chd_engine* e, cudaStream_t s, bool cta_ti
     const uint64_t P = e->lim.max_pairs;
     StageTimer kt(e, s, CHD_STAGE_EMIT_KERNEL);
     if (cta_tiles) {
-        // One CTA per tile, dispatched by the hardware block scheduler.  The tile count lives on the device; the grid is
+        // EMIT_TILES_PER_CTA tiles per CTA, dispatched by the hardware block scheduler.  The tile count lives on the device; the grid is
         // sized from the last visible count the host has seen (+3 %: the kernel loops if that was too few, surplus CTAs exit
         // at once), from the capacity before that.
         const uint64_t cap_tiles = (e->lim.max_visible + EMIT_TILE - 1) / EMIT_TILE;
