@@ -27,7 +27,9 @@ TICK_VISIBLE_DELTA = 16
 OVF_PAIRS, OVF_WINDOW, OVF_VISIBLE, OVF_DUE, OVF_BORDER, OVF_RING = 1, 2, 4, 8, 16, 32
 OVF_DELTA = 64
 (VIEW_CELL_START, VIEW_SORTED_ENTITY, VIEW_ENT_CELL, VIEW_PAIR_OFF, VIEW_PAIR_CHANNEL, VIEW_PAIR_DIST, VIEW_VIS_OFF, VIEW_VIS_ENTITY, VIEW_DUE,
- VIEW_DELTA_ENTER_OFF, VIEW_DELTA_ENTER, VIEW_DELTA_LEAVE_OFF, VIEW_DELTA_LEAVE) = range(13)
+ VIEW_DELTA_ENTER_OFF, VIEW_DELTA_ENTER, VIEW_DELTA_LEAVE_OFF, VIEW_DELTA_LEAVE, VIEW_ENTITY_ID) = range(14)
+# per-event statuses of chd_spawn_entities / chd_despawn_entities (entity-table mode)
+EV_OK, EV_DUPLICATE, EV_UNKNOWN_ID, EV_RESERVED_ID, EV_TABLE_FULL = 0, 1, 2, 3, 4
 PF_HAD_FIRST, PF_NEW, PF_SKIP_SELF = 1, 2, 4
 
 
@@ -112,6 +114,16 @@ class TickSummary(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_ if k != "reserved"}
 
 
+class EntityStats(C.Structure):
+    _fields_ = [
+        ("live", C.c_uint32), ("high_water", C.c_uint32), ("quarantined", C.c_uint32), ("free_slots", C.c_uint32),
+        ("moves_applied", C.c_uint64), ("moves_unknown", C.c_uint64), ("moves_superseded", C.c_uint64), ("rebuilds", C.c_uint64),
+    ]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 # every symbol include/chd_gpu.h declares (checked by tests/test_abi.py against the header text)
 SYMBOLS = [
     "chd_abi_version", "chd_default_limits", "chd_create", "chd_destroy", "chd_last_error", "chd_set_stream", "chd_sync",
@@ -124,8 +136,10 @@ SYMBOLS = [
     "chd_graph_launch_count",
     "chd_add_subscribers", "chd_remove_subscribers", "chd_fetch_results_async", "chd_fetch_wait", "chd_rings_init", "chd_rings_append", "chd_get_rings", "chd_set_channel_start_times", "chd_set_payload_bytes", "chd_assemble_payloads", "chd_frame_packets", "chd_comm_unique_id", "chd_comm_init", "chd_comm_info", "chd_comm_destroy", "chd_tick_sharded", "chd_collective_count", "chd_comm_exchange_mode", "chd_comm_use_collective", "chd_migrate_out", "chd_migrate_in", "chd_get_rehome",
     "chd_reserve_visible_delta", "chd_visible_delta", "chd_get_visible_delta",
+    "chd_entity_table_init", "chd_spawn_entities", "chd_spawn_entities_f32", "chd_despawn_entities", "chd_move_entities", "chd_move_entities_f32",
+    "chd_get_entity_stats",
 ]
-STAGE_BUILD, STAGE_INTEREST, STAGE_EMIT, STAGE_EMIT_KERNEL, STAGE_FANOUT, STAGE_TICK, STAGE_EXPORT, STAGE_EXCHANGE, STAGE_IMPORT, STAGE_READBACK, STAGE_VISIBLE_DELTA = range(11)
+STAGE_BUILD, STAGE_INTEREST, STAGE_EMIT, STAGE_EMIT_KERNEL, STAGE_FANOUT, STAGE_TICK, STAGE_EXPORT, STAGE_EXCHANGE, STAGE_IMPORT, STAGE_READBACK, STAGE_VISIBLE_DELTA, STAGE_ENTITY_EVENTS = range(12)
 
 _lib = None
 
@@ -305,6 +319,18 @@ def lib():
     L.chd_visible_delta.argtypes = [vp]
     L.chd_get_visible_delta.restype = C.c_int
     L.chd_get_visible_delta.argtypes = [vp, vp, vp, vp, vp, C.c_uint64, u64p, u64p, u32p]
+    L.chd_entity_table_init.restype = C.c_int
+    L.chd_entity_table_init.argtypes = [vp]
+    for f in (L.chd_spawn_entities, L.chd_spawn_entities_f32):
+        f.restype = C.c_int
+        f.argtypes = [vp, vp, vp, vp, C.c_uint32, vp]
+    L.chd_despawn_entities.restype = C.c_int
+    L.chd_despawn_entities.argtypes = [vp, vp, C.c_uint32, vp]
+    for f in (L.chd_move_entities, L.chd_move_entities_f32):
+        f.restype = C.c_int
+        f.argtypes = [vp, vp, vp, vp, C.c_uint32]
+    L.chd_get_entity_stats.restype = C.c_int
+    L.chd_get_entity_stats.argtypes = [vp, C.POINTER(EntityStats)]
     _lib = L
     return L
 

@@ -216,6 +216,26 @@ class GpuStaticGrid2DSpatialController:
         s = self.engine.summary()
         return self.engine.get_handover(int(s.n_handover))
 
+    # -- entities as the reference delivers them, keyed by NetGUID (entity-table mode, switched on by the first call):
+    # SpawnObjects = handleSpawnObject's GetChannelId + addSpatialEntity (pkg/unreal/message.go:20-150), DestroyObjects = the
+    # destroy handler (message.go:152-203), MoveEntities = ENTITY-channel updates whose Merge hook calls Notify for that entity only
+    # (examples/channeld-ue-tps/tpspb/data.go:227-256, spatial.go:612-626).  Spawns / destroys return a capi.EV_* status per id;
+    # results (cells, visible lists, handovers, deltas) name NetGUIDs.
+    def _table(self):
+        if not getattr(self, "_table_on", False):
+            self.engine.entity_table_init()
+            self._table_on = True
+        return self.engine
+
+    def SpawnObjects(self, net_ids, x, z) -> np.ndarray:
+        return self._table().spawn_entities(net_ids, x, z)
+
+    def DestroyObjects(self, net_ids) -> np.ndarray:
+        return self._table().despawn_entities(net_ids)
+
+    def MoveEntities(self, net_ids, x, z) -> None:
+        self._table().move_entities(net_ids, x, z)
+
     # -- Tick()   (channel.go:358-387 for all spatial channels at once)
     def Tick(self, batch, t_ns, flags=capi.TICK_ALL):
         return self.engine.tick(batch, t_ns, flags)

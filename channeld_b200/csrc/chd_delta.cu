@@ -41,6 +41,11 @@ chd_status chd_delta_check(chd_engine* e, bool will_build) {
         e->fail("visible delta needs a chd_build of the current cell assignment");
         return CHD_ERR_STATE;
     }
+    if (!will_build && e->tbl.on && e->entities_dirty) {
+        // entity-table mode: the ids the lists are translated with must be those of the build the delta measures
+        e->fail("visible delta needs a chd_build after the last spawn / move / despawn");
+        return CHD_ERR_STATE;
+    }
     return CHD_OK;
 }
 
@@ -54,7 +59,8 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
     chd_status st = chd_epoch_tick(e, s, EP_DELTA);
     if (st != CHD_OK) return st;
     // sizes and the key / pair buffers in use are baked into the captured launches
-    const uint64_t key = stage_key(0x64656c7461ull, d.n, d.n_slots, D.n_out, e->cur, d.key, d.enter, d.leave, d.enter_cap, d.leave_cap);
+    const uint64_t key = stage_key(0x64656c7461ull, d.n, d.n_slots, D.n_out, e->cur, d.key, d.enter, d.leave, d.enter_cap, d.leave_cap, e->tbl.on,
+                                   e->tbl.d_id_of_slot);
     const unsigned grid = (unsigned)e->sm_count * 8;
     const unsigned slot_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(blocks_for((uint64_t)D.n_out * 32, DELTA_THREADS), (uint64_t)e->sm_count * 32));
     return run_stage(e, s, D.g, key, [&]() -> chd_status {
@@ -72,6 +78,10 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
         SCAN(e, exclusive_scan_1p<uint32_t, uint64_t>(D.cnt_leave, D.leave_off, D.n_out, D.site_leave, s));
         delta_slots_kernel<true><<<slot_grid, DELTA_THREADS, 0, s>>>(d);
         KCHECK(e);
+        if (e->tbl.on) {  // entity-table mode: the lists name ids (here: a later spawn must not change lists already computed)
+            const chd_status ts = chd_table_delta_ids(e, s);
+            if (ts != CHD_OK) return ts;
+        }
         delta_advance_kernel<<<grid, DELTA_THREADS, 0, s>>>(d, (uint32_t)e->lim.max_pairs);
         KCHECK(e);
         return CHD_OK;

@@ -173,6 +173,8 @@ void chd_destroy(chd_engine* e) {
     if (e->h_ctr) cudaFreeHost(e->h_ctr);
     if (e->h_u32) cudaFreeHost(e->h_u32);
     if (e->h_get) cudaFreeHost(e->h_get);
+    for (uint8_t* h : e->tbl.h_stage)
+        if (h) cudaFreeHost(h);
     if (e->own_stream && e->stream) cudaStreamDestroy(e->stream);
     delete e;  // on e->device: the graph slots release their executables
 }

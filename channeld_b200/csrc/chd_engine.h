@@ -8,6 +8,7 @@
 //   chd_results.cu   getters, chd_fetch_results, device views
 //   chd_shard.cu     multi-GPU X-slabs: border export, halo import, the NCCL exchange
 //   chd_extras.cu    window classes, ADJACENT_CHANNELS broadcast sets, config-plane helpers
+//   chd_table.cu     entity-table mode: spawn / move / despawn by id, the id-valued results
 #pragma once
 #include <cuda_runtime.h>
 
@@ -18,9 +19,11 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <mutex>
 #include <new>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 #include "chd_scan.cuh"
@@ -292,6 +295,36 @@ struct chd_engine {
         bool done_recorded = false;  // the last tick ran the delta off the engine stream: its end (and CHD_OVF_DELTA) is ev_done
     } dl;
     bool delta_blocked = false;  // chd_set_slab / chd_set_entity_ids were used: halo indices are not stable, no deltas
+    // ---- entity-table mode (chd_table.cu): entities spawned / moved / despawned by id; everything is allocated by
+    // chd_entity_table_init.  Slots are position indices; n_own is the high-water mark.
+    struct Table {
+        bool on = false;
+        std::unordered_map<uint32_t, uint32_t> slot_of;  // live id -> slot
+        std::deque<uint32_t> free_fifo;                  // released slots, reused first in, first out
+        struct Held {
+            uint32_t slot;
+            uint64_t build;  // the first build that sees the slot empty: released by a successful delta of that build or a later one
+        };
+        std::deque<Held> quarantine;
+        uint32_t hw = 0;       // slots [0, hw) have been used
+        uint32_t bits = 0;     // the device table has 2^bits words
+        uint64_t used = 0;     // live entries + tombstones in the device table
+        uint64_t rebuilds = 0, builds = 0;  // builds: table-mode builds so far (the device counts them too: d_build_seq)
+        bool ho_raw = false;   // the handover list holds slots of a fresh cell assignment (chd_assign_host)
+        uint64_t* d_table = nullptr;
+        uint32_t *d_id_of_slot = nullptr, *d_snap_id = nullptr, *d_sorted_id = nullptr, *d_winner = nullptr, *d_mslot = nullptr;
+        uint32_t *d_ho_tmp = nullptr, *d_build_seq = nullptr;  // d_build_seq[0] = builds, [1] = stashed handover count
+        uint8_t* d_flag = nullptr;                             // slot spawned / despawned since the last cell assignment
+        unsigned long long* d_stats = nullptr;                 // moves applied, to unknown ids, superseded within a call
+        uint32_t* d_ev = nullptr;   // event staging: [N] ids, [N] slots
+        double* d_ev_pos = nullptr;  // [2N] x, z (moves: f64, or f32 in the first half)
+        // spawn / despawn uploads go through two pinned buffers, each reused once the copy made from it two calls ago is done
+        uint8_t* h_stage[2] = {nullptr, nullptr};
+        uint64_t h_stage_cap[2] = {0, 0};
+        cudaEvent_t ev_stage[2] = {nullptr, nullptr};
+        int next_stage = 0;
+        GraphSet g_post;
+    } tbl;
 
     bool fail(const char* fmt, ...) const {
         char buf[512];
@@ -437,7 +470,17 @@ chd_status chd_sort_pass_any(chd_engine* e, cudaStream_t s, uint32_t* hist, cons
 // visible-set delta (chd_delta.cu): whether one may run now (will_build: the caller builds first), and the stage itself on `s`
 chd_status chd_delta_check(chd_engine* e, bool will_build);
 chd_status chd_delta_on(chd_engine* e, cudaStream_t s);
+// entity-table mode (chd_table.cu): the call named `fn` is not available in it (CHD_ERR_STATE); the pass after every table-mode build
+// (sorted ids, handover list in ids); the delta's translation to ids, inside its stage; a decoded summary's last successful delta
+chd_status chd_table_refuse(chd_engine* e, const char* fn);
+chd_status chd_table_after_build(chd_engine* e, cudaStream_t s);
+chd_status chd_table_delta_ids(chd_engine* e, cudaStream_t s);
+void chd_table_observe(chd_engine* e, uint32_t delta_build);
 }
+
+// What the cell CSR's sorted_entity, the visible lists and the read-back report: entity indices, or ids in entity-table mode.  The
+// slot-valued d_sorted_ent stays what the delta reads.
+static inline const uint32_t* chd_sorted_out(const chd_engine* e) { return e->tbl.on ? e->tbl.d_sorted_id : e->d_sorted_ent; }
 
 // Grow-on-demand buffer: when `need` elements exceed `*cap`, the buffer is replaced (contents not kept) by one of `count`
 // elements, the caller's growth policy.  *cap is 0 exactly when there is no buffer.

@@ -130,6 +130,7 @@ void chd_entities_replaced(chd_engine* e, uint32_t n) {
 // up_stream (prefetch).  Device-resident doubles given to a set are read in place.
 static chd_status upload_positions(chd_engine* e, const char* fn, const void* x, const void* z, uint32_t n, bool f32, bool prefetch) {
     if (!e || (n && (!x || !z))) return CHD_ERR_INVALID;
+    if (e->tbl.on) return chd_table_refuse(e, fn);
     if (n > e->lim.max_entities) {
         e->fail("%s: %u > max_entities %u", fn, n, e->lim.max_entities);
         return CHD_ERR_CAPACITY;
@@ -181,6 +182,7 @@ chd_status chd_prefetch_entities_f32(chd_engine* e, const float* x, const float*
 
 chd_status chd_entity_buffers(chd_engine* e, double** d_x, double** d_z, uint32_t* n) {
     if (!e) return CHD_ERR_INVALID;
+    if (e->tbl.on) return chd_table_refuse(e, "chd_entity_buffers");
     if (d_x) *d_x = e->d_x;
     if (d_z) *d_z = e->d_z;
     if (n) *n = e->n_own;
@@ -193,12 +195,14 @@ chd_status chd_entity_buffers(chd_engine* e, double** d_x, double** d_z, uint32_
 
 chd_status chd_set_entity_count(chd_engine* e, uint32_t n) {
     if (!e || n > e->lim.max_entities) return CHD_ERR_INVALID;
+    if (e->tbl.on) return chd_table_refuse(e, "chd_set_entity_count");
     chd_entities_replaced(e, n);
     return CHD_OK;
 }
 
 chd_status chd_set_entity_ids(chd_engine* e, const uint32_t* gid, uint32_t n) {
     if (!e || n > e->lim.max_entities) return CHD_ERR_INVALID;
+    if (e->tbl.on) return chd_table_refuse(e, "chd_set_entity_ids");
     CU(e, cudaSetDevice(e->device));
     e->delta_blocked = true;  // global ids: the multi-GPU flow (chd_visible_delta is single-GPU only)
     if (!gid) {
@@ -238,6 +242,7 @@ uint32_t* chd_assign_host(chd_engine* e) {
     if (e->n_own) e->have_prev_key = true;
     e->n_halo = 0;
     e->assigned = true;
+    e->tbl.ho_raw = true;  // (entity-table mode: the handover list now names slots until chd_table_after_build)
     return prev;
 }
 
@@ -372,6 +377,8 @@ chd_status chd_build_on(chd_engine* e, cudaStream_t s) {
         st = build_enqueue(e, s, with_assign);
         if (st == CHD_OK && with_assign) st = chd_note_pos_read(e, s);
     }
+    if (st != CHD_OK) return st;
+    st = chd_table_after_build(e, s);  // (entity-table mode only)
     if (st != CHD_OK) return st;
     if (!counts_recorded) CU(e, cudaEventRecord(e->ev_counts, s));  // (cell counts final = build done)
     e->n_sorted = e->n_own + e->n_halo;

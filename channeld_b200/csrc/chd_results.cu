@@ -64,7 +64,7 @@ chd_status chd_get_cells(chd_engine* e, uint32_t* cell_start, uint32_t* sorted_e
         uint32_t nin = 0;
         chd_status st = chd_read_u32(e, e->d_cell_start + C, &nin);
         if (st != CHD_OK) return st;
-        CU(e, cudaMemcpyAsync(sorted_entity, e->d_sorted_ent, sizeof(uint32_t) * nin, cudaMemcpyDefault, e->stream));
+        CU(e, cudaMemcpyAsync(sorted_entity, chd_sorted_out(e), sizeof(uint32_t) * nin, cudaMemcpyDefault, e->stream));
     }
     CU(e, cudaStreamSynchronize(e->stream));
     return CHD_OK;
@@ -260,7 +260,7 @@ chd_status chd_fetch_results(chd_engine* e, const chd_result_buffers* b, chd_tic
     if (b->cell_start) CU(e, cudaMemcpyAsync(b->cell_start, e->d_cell_start, sizeof(uint32_t) * ((uint64_t)e->g.cells + 1), cudaMemcpyDefault, s));
     if (b->sorted_entity) {
         if (ca.n_entities_in_world > b->entity_cap) return drain(CHD_ERR_CAPACITY);
-        CU(e, cudaMemcpyAsync(b->sorted_entity, e->d_sorted_ent, sizeof(uint32_t) * (uint64_t)ca.n_entities_in_world, cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(b->sorted_entity, chd_sorted_out(e), sizeof(uint32_t) * (uint64_t)ca.n_entities_in_world, cudaMemcpyDefault, s));
     }
     cudaStream_t sa = s;  // stream carrying the phase-A copies
     if (early) {  // phase B, on its own stream: its counter read-back must not queue behind the phase-A copies
@@ -334,7 +334,7 @@ chd_status chd_fetch_results_async(chd_engine* e, const chd_result_buffers* b, v
     if (b->unsub_channel) A.seg[A.n++] = seg(e->d_gone_ch, b->unsub_channel, &ctr->n_unsub, 0, b->diff_cap, 1, 0);
     if (b->query_status) A.seg[A.n++] = seg(e->d_status, b->query_status, nullptr, std::min<uint64_t>(e->last_nq, b->status_cap), b->status_cap, 1, 0);
     if (b->cell_start) A.seg[A.n++] = seg(e->d_cell_start, b->cell_start, nullptr, (uint64_t)e->g.cells + 1, (uint64_t)e->g.cells + 1, 1, 0);
-    if (b->sorted_entity) A.seg[A.n++] = seg(e->d_sorted_ent, b->sorted_entity, &ctr->n_entities_in_world, 0, b->entity_cap, 1, 0);
+    if (b->sorted_entity) A.seg[A.n++] = seg(chd_sorted_out(e), b->sorted_entity, &ctr->n_entities_in_world, 0, b->entity_cap, 1, 0);
     PackArgs A2{};  // (the handover triple: a second launch keeps PackArgs small)
     A2.truncated = A.truncated;
     const uint64_t hcap = std::min<uint64_t>(b->handover_cap, e->ho_cap);
@@ -463,7 +463,7 @@ chd_status chd_device_view(chd_engine* e, int which, void** d_ptr, uint64_t* cou
     void* p = nullptr;
     switch (which) {
         case CHD_VIEW_CELL_START: p = e->d_cell_start; c = (uint64_t)e->g.cells + 2; break;
-        case CHD_VIEW_SORTED_ENTITY: p = e->d_sorted_ent; c = e->n_sorted; break;
+        case CHD_VIEW_SORTED_ENTITY: p = (void*)chd_sorted_out(e); c = e->n_sorted; break;
         case CHD_VIEW_ENT_CELL: p = e->d_key; c = e->n_own + e->n_halo; break;
         case CHD_VIEW_PAIR_OFF: p = pb.off; c = (uint64_t)e->n_slots + 1; break;
         case CHD_VIEW_PAIR_CHANNEL: p = pb.cell; c = e->lim.max_pairs; break;
@@ -475,9 +475,14 @@ chd_status chd_device_view(chd_engine* e, int which, void** d_ptr, uint64_t* cou
         case CHD_VIEW_DELTA_ENTER: p = e->dl.enter; c = e->dl.enter_cap; break;
         case CHD_VIEW_DELTA_LEAVE_OFF: p = e->dl.leave_off; c = (uint64_t)e->dl.n_out + 1; break;
         case CHD_VIEW_DELTA_LEAVE: p = e->dl.leave; c = e->dl.leave_cap; break;
+        case CHD_VIEW_ENTITY_ID: p = e->tbl.d_id_of_slot; c = e->tbl.hw; break;
         default: return CHD_ERR_INVALID;
     }
-    if (which >= CHD_VIEW_DELTA_ENTER_OFF && !e->dl.on) {
+    if (which == CHD_VIEW_ENTITY_ID && !e->tbl.on) {
+        e->fail("chd_device_view: CHD_VIEW_ENTITY_ID needs entity-table mode (chd_entity_table_init)");
+        return CHD_ERR_STATE;
+    }
+    if (which >= CHD_VIEW_DELTA_ENTER_OFF && which <= CHD_VIEW_DELTA_LEAVE && !e->dl.on) {
         e->fail("chd_device_view: no visible delta before chd_reserve_visible_delta");
         return CHD_ERR_STATE;
     }

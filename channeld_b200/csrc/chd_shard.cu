@@ -61,6 +61,7 @@ NcclApi* nccl_api() {
 extern "C" {
 
 chd_status chd_set_slab(chd_engine* e, uint32_t col_lo, uint32_t col_hi, uint32_t halo) {
+    if (e && e->tbl.on) return chd_table_refuse(e, "chd_set_slab");
     if (!e || col_lo >= col_hi || col_hi > e->g.cols) return CHD_ERR_INVALID;
     e->g.col_lo = col_lo;
     e->g.col_hi = col_hi;
@@ -71,6 +72,7 @@ chd_status chd_set_slab(chd_engine* e, uint32_t col_lo, uint32_t col_hi, uint32_
 }
 
 chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_records, uint32_t* out_count) {
+    if (e && e->tbl.on) return chd_table_refuse(e, "chd_export_border");
     if (!e || !d_records) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
     cudaStream_t s = e->stream;
@@ -130,6 +132,7 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
 }
 
 chd_status chd_import_halo(chd_engine* e, const uint32_t* d_records, uint32_t n_records, uint32_t skip_first, uint32_t skip_count) {
+    if (e && e->tbl.on) return chd_table_refuse(e, "chd_import_halo");
     if (!e || (n_records && !d_records)) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
     if (!e->assigned) {
@@ -190,6 +193,7 @@ chd_status chd_comm_unique_id(void* out_id) {
 
 chd_status chd_comm_init(chd_engine* e, const void* unique_id, int rank, int world, uint32_t halo_cols, uint32_t border_capacity,
                          uint32_t migrate_subscribers, uint32_t migrate_pairs) {
+    if (e && e->tbl.on) return chd_table_refuse(e, "chd_comm_init");
     if (!e || !unique_id || world < 1 || rank < 0 || rank >= world || border_capacity == 0) return CHD_ERR_INVALID;
     if (world >= 4096 || migrate_subscribers >= (1u << 20)) return CHD_ERR_INVALID;  // (slot_src packs rank:12 | record:20)
     if (e->comm) {
@@ -329,6 +333,7 @@ chd_status chd_comm_destroy(chd_engine* e) {
 // are selected, ONE all-gather moves every rank's records over NVLink, the records this slab needs are appended as halo
 // entities, then build + emit run over own + halo entities and the streams join.  Nothing synchronises with the host.
 chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_ns, uint32_t flags, chd_tick_summary* out) {
+    if (e && e->tbl.on) return chd_table_refuse(e, "chd_tick_sharded");
     if (!e) return CHD_ERR_INVALID;
     if (!e->comm) {
         e->fail("chd_tick_sharded before chd_comm_init");

@@ -1,0 +1,414 @@
+// chd_table.cu — entity-table mode: spawn, move and despawn entities by id (chd_table.cuh).  The host side owns everything that
+// must be answered synchronously or assigned deterministically (statuses, id -> slot, free FIFO, quarantine); moves, the
+// high-volume path, resolve their ids on the device.
+#include "chd_engine.h"
+
+#include "chd_table.cuh"
+
+#include <unordered_set>
+
+namespace {
+
+chd_status need_table(chd_engine* e, const char* fn) {
+    if (e->tbl.on) return CHD_OK;
+    e->fail("%s before chd_entity_table_init", fn);
+    return CHD_ERR_STATE;
+}
+
+// The positions changed: nothing is assigned or built for them yet.  Unlike chd_entities_replaced this keeps handover detection on
+// when the high-water mark grows: the new slots are flagged and left out of the handover list.
+void touched(chd_engine* e) {
+    e->n_own = e->tbl.hw;
+    e->n_halo = 0;
+    e->assigned = false;
+    e->entities_dirty = true;
+}
+
+unsigned grid_for(const chd_engine* e, uint64_t n) {
+    return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(blocks_for(n, TBL_THREADS), (uint64_t)e->sm_count * 8));
+}
+
+// A pinned staging buffer of at least `bytes` whose last upload has completed (two alternate: a host that spawns every tick waits
+// for the copy it made a call earlier, not for the one just enqueued).  The caller records ev_stage[*k] after its copies.
+chd_status take_stage(chd_engine* e, uint64_t bytes, int* k, uint8_t** out) {
+    chd_engine::Table& t = e->tbl;
+    *k = t.next_stage;
+    t.next_stage ^= 1;
+    CU(e, cudaEventSynchronize(t.ev_stage[*k]));
+    if (t.h_stage_cap[*k] < bytes) {
+        if (t.h_stage[*k]) CU(e, cudaFreeHost(t.h_stage[*k]));
+        t.h_stage[*k] = nullptr;
+        t.h_stage_cap[*k] = 0;
+        const uint64_t cap = std::max<uint64_t>(bytes, 4096);
+        CU(e, cudaHostAlloc((void**)&t.h_stage[*k], cap, cudaHostAllocDefault));
+        t.h_stage_cap[*k] = cap;
+    }
+    *out = t.h_stage[*k];
+    return CHD_OK;
+}
+
+// An event array on the host: host arrays are read where they are, device arrays are copied back (statuses are synchronous).
+template <typename T>
+chd_status host_view(chd_engine* e, const T* p, uint32_t n, std::vector<T>& keep, const T** out) {
+    *out = p;
+    if (!n || !chd_is_device_ptr(e, p)) return CHD_OK;
+    keep.resize(n);
+    CU(e, cudaMemcpy(keep.data(), p, sizeof(T) * n, cudaMemcpyDeviceToHost));
+    *out = keep.data();
+    return CHD_OK;
+}
+
+chd_status put_status(chd_engine* e, uint8_t* out, const std::vector<uint8_t>& st) {
+    if (!out || st.empty()) return CHD_OK;
+    if (chd_is_device_ptr(e, out)) {
+        CU(e, cudaMemcpy(out, st.data(), st.size(), cudaMemcpyHostToDevice));
+    } else {
+        memcpy(out, st.data(), st.size());
+    }
+    return CHD_OK;
+}
+
+// Uploads m (id, slot) pairs and, with positions, their x / z (as doubles) into the device event staging on the engine stream.
+chd_status upload_events(chd_engine* e, const std::vector<uint32_t>& id, const std::vector<uint32_t>& slot, const std::vector<double>* x,
+                         const std::vector<double>* z) {
+    chd_engine::Table& t = e->tbl;
+    const uint64_t m = id.size();
+    if (!m) return CHD_OK;
+    int k = 0;
+    uint8_t* h = nullptr;
+    chd_status st = take_stage(e, m * (x ? 24 : 8), &k, &h);
+    if (st != CHD_OK) return st;
+    uint32_t* hi = reinterpret_cast<uint32_t*>(h + (x ? 16 * m : 0));
+    memcpy(hi, id.data(), 4 * m);
+    memcpy(hi + m, slot.data(), 4 * m);
+    if (x) {
+        memcpy(h, x->data(), 8 * m);
+        memcpy(h + 8 * m, z->data(), 8 * m);
+        CU(e, cudaMemcpyAsync(t.d_ev_pos, h, 16 * m, cudaMemcpyHostToDevice, e->stream));
+    }
+    CU(e, cudaMemcpyAsync(t.d_ev, hi, 8 * m, cudaMemcpyHostToDevice, e->stream));
+    CU(e, cudaEventRecord(t.ev_stage[k], e->stream));
+    return CHD_OK;
+}
+
+// The device table from the host map (live entries only: the tombstones go), stream-ordered.
+chd_status rebuild_table(chd_engine* e) {
+    chd_engine::Table& t = e->tbl;
+    std::vector<uint32_t> id, slot;
+    id.reserve(t.slot_of.size());
+    slot.reserve(t.slot_of.size());
+    for (const auto& kv : t.slot_of) {
+        id.push_back(kv.first);
+        slot.push_back(kv.second);
+    }
+    CU(e, cudaMemsetAsync(t.d_table, 0, 8ull << t.bits, e->stream));
+    chd_status st = upload_events(e, id, slot, nullptr, nullptr);
+    if (st != CHD_OK) return st;
+    if (!id.empty()) {
+        const uint32_t m = (uint32_t)id.size();
+        tbl_spawn_kernel<<<grid_for(e, m), TBL_THREADS, 0, e->stream>>>(t.d_table, t.bits, t.d_ev, t.d_ev + m, nullptr, nullptr, m, nullptr, nullptr, nullptr,
+                                                                       nullptr);
+        KCHECK(e);
+    }
+    t.used = id.size();
+    t.rebuilds++;
+    return CHD_OK;
+}
+
+bool reserved_id(uint32_t id) { return id == 0u || id == 0xFFFFFFFFu; }
+
+chd_status spawn(chd_engine* e, const char* fn, const uint32_t* id_in, const void* x_in, const void* z_in, bool f32, uint32_t n, uint8_t* out_status) {
+    if (!e || (n && (!id_in || !x_in || !z_in))) return CHD_ERR_INVALID;
+    chd_status st = need_table(e, fn);
+    if (st != CHD_OK) return st;
+    CU(e, cudaSetDevice(e->device));
+    chd_engine::Table& t = e->tbl;
+    std::vector<uint32_t> kid;
+    const uint32_t* ids = nullptr;
+    st = host_view(e, id_in, n, kid, &ids);
+    if (st != CHD_OK) return st;
+    // positions as doubles: the float form widens exactly, as chd_set_entities_f32 does
+    std::vector<double> px(n), pz(n);
+    if (f32) {
+        std::vector<float> kx, kz;
+        const float *fx = nullptr, *fz = nullptr;
+        if ((st = host_view(e, (const float*)x_in, n, kx, &fx)) != CHD_OK || (st = host_view(e, (const float*)z_in, n, kz, &fz)) != CHD_OK) return st;
+        for (uint32_t i = 0; i < n; i++) {
+            px[i] = (double)fx[i];
+            pz[i] = (double)fz[i];
+        }
+    } else {
+        std::vector<double> kx, kz;
+        const double *dx = nullptr, *dz = nullptr;
+        if ((st = host_view(e, (const double*)x_in, n, kx, &dx)) != CHD_OK || (st = host_view(e, (const double*)z_in, n, kz, &dz)) != CHD_OK) return st;
+        std::copy(dx, dx + n, px.begin());
+        std::copy(dz, dz + n, pz.begin());
+    }
+    std::vector<uint8_t> status(n, (uint8_t)CHD_EV_OK);
+    std::vector<uint32_t> aid, aslot;
+    std::vector<double> ax, az;
+    std::unordered_set<uint32_t> seen;
+    seen.reserve(n);
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t id = ids[i];
+        uint32_t slot = 0;
+        if (reserved_id(id)) {
+            status[i] = CHD_EV_RESERVED_ID;
+        } else if (!seen.insert(id).second || t.slot_of.count(id)) {
+            status[i] = CHD_EV_DUPLICATE;
+        } else if (!t.free_fifo.empty()) {
+            slot = t.free_fifo.front();
+            t.free_fifo.pop_front();
+        } else if (t.hw < e->lim.max_entities) {
+            slot = t.hw++;
+        } else {
+            status[i] = CHD_EV_TABLE_FULL;
+        }
+        if (status[i] != CHD_EV_OK) continue;
+        aid.push_back(id);
+        aslot.push_back(slot);
+        ax.push_back(px[i]);
+        az.push_back(pz[i]);
+    }
+    const uint64_t m = aid.size();
+    if (m) {
+        StageTimer timer(e, e->stream, CHD_STAGE_ENTITY_EVENTS);
+        if ((t.used + m) * 4 > (3ull << t.bits)) {  // live + tombstones would pass 3/4 of the table
+            st = rebuild_table(e);
+            if (st != CHD_OK) return st;
+        }
+        for (uint64_t j = 0; j < m; j++) t.slot_of[aid[j]] = aslot[j];
+        t.used += m;
+        st = upload_events(e, aid, aslot, &ax, &az);
+        if (st != CHD_OK) return st;
+        tbl_spawn_kernel<<<grid_for(e, m), TBL_THREADS, 0, e->stream>>>(t.d_table, t.bits, t.d_ev, t.d_ev + m, t.d_ev_pos, t.d_ev_pos + m, (uint32_t)m,
+                                                                       t.d_id_of_slot, e->d_x, e->d_z, t.d_flag);
+        KCHECK(e);
+        touched(e);
+    }
+    return put_status(e, out_status, status);
+}
+
+chd_status move(chd_engine* e, const char* fn, const uint32_t* id, const void* x, const void* z, bool f32, uint32_t n) {
+    if (!e || (n && (!id || !x || !z))) return CHD_ERR_INVALID;
+    chd_status st = need_table(e, fn);
+    if (st != CHD_OK) return st;
+    const uint64_t N = e->lim.max_entities;
+    if (n > N) {
+        e->fail("%s: %u moves in one call > max_entities %llu", fn, n, (unsigned long long)N);
+        return CHD_ERR_CAPACITY;
+    }
+    if (!n) return CHD_OK;
+    CU(e, cudaSetDevice(e->device));
+    chd_engine::Table& t = e->tbl;
+    cudaStream_t s = e->stream;
+    StageTimer timer(e, s, CHD_STAGE_ENTITY_EVENTS);
+    // host inputs are copied into the event staging, device inputs read in place
+    const uint32_t* did = id;
+    if (!chd_is_device_ptr(e, id)) {
+        CU(e, cudaMemcpyAsync(t.d_ev, id, 4ull * n, cudaMemcpyDefault, s));
+        did = t.d_ev;
+    }
+    const size_t w = f32 ? sizeof(float) : sizeof(double);
+    const void *dx = x, *dz = z;
+    if (!(chd_is_device_ptr(e, x) && chd_is_device_ptr(e, z))) {
+        uint8_t* base = reinterpret_cast<uint8_t*>(t.d_ev_pos);
+        CU(e, cudaMemcpyAsync(base, x, w * n, cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(base + w * N, z, w * n, cudaMemcpyDefault, s));
+        dx = base;
+        dz = base + w * N;
+    }
+    const unsigned grid = grid_for(e, n);
+    tbl_move_resolve_kernel<<<grid, TBL_THREADS, 0, s>>>(t.d_table, t.bits, did, n, t.d_mslot, t.d_winner, t.d_stats);
+    KCHECK(e);
+    if (f32)
+        tbl_move_apply_kernel<float><<<grid, TBL_THREADS, 0, s>>>(t.d_mslot, t.d_winner, (const float*)dx, (const float*)dz, n, e->d_x, e->d_z, t.d_stats);
+    else
+        tbl_move_apply_kernel<double><<<grid, TBL_THREADS, 0, s>>>(t.d_mslot, t.d_winner, (const double*)dx, (const double*)dz, n, e->d_x, e->d_z, t.d_stats);
+    KCHECK(e);
+    touched(e);
+    return CHD_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+chd_status chd_table_refuse(chd_engine* e, const char* fn) {
+    e->fail("%s is not available in entity-table mode (chd_entity_table_init): use chd_spawn_entities / chd_move_entities / chd_despawn_entities", fn);
+    return CHD_ERR_STATE;
+}
+
+chd_status chd_entity_table_init(chd_engine* e) {
+    if (!e) return CHD_ERR_INVALID;
+    chd_engine::Table& t = e->tbl;
+    if (t.on || e->built || e->n_own || e->pf_pos.staged >= 0 || e->delta_blocked || e->comm) {
+        e->fail("chd_entity_table_init needs a fresh engine (no entities set or built, no chd_set_slab / chd_set_entity_ids / chd_comm_init)");
+        return CHD_ERR_STATE;
+    }
+    CU(e, cudaSetDevice(e->device));
+    const uint64_t N = e->lim.max_entities;
+    uint32_t bits = 4;
+    while ((1ull << bits) < 2 * N) bits++;
+    const bool ok = dalloc(e, &t.d_table, 1ull << bits) && dalloc(e, &t.d_id_of_slot, N) && dalloc(e, &t.d_snap_id, N) &&
+                    dalloc(e, &t.d_sorted_id, ((N + 3) / 4) * 4 + 8) &&  // the padding and alignment of d_sorted_ent (the emit kernels read it)
+                    dalloc(e, &t.d_winner, N) && dalloc(e, &t.d_mslot, N) && dalloc(e, &t.d_ho_tmp, 3 * N) && dalloc(e, &t.d_build_seq, 2) &&
+                    dalloc(e, &t.d_flag, N) && dalloc(e, &t.d_stats, 3) && dalloc(e, &t.d_ev, 2 * N) && dalloc(e, &t.d_ev_pos, 2 * N) &&
+                    chd_make_event(e, &t.ev_stage[0]) && chd_make_event(e, &t.ev_stage[1]);
+    if (!ok) return CHD_ERR_CUDA;
+    cudaStream_t s = e->stream;
+    CU(e, cudaMemsetAsync(t.d_table, 0, 8ull << bits, s));
+    CU(e, cudaMemsetAsync(t.d_id_of_slot, 0, 4 * N, s));
+    CU(e, cudaMemsetAsync(t.d_snap_id, 0, 4 * N, s));
+    CU(e, cudaMemsetAsync(t.d_winner, 0, 4 * N, s));
+    CU(e, cudaMemsetAsync(t.d_flag, 0, N, s));
+    CU(e, cudaMemsetAsync(t.d_stats, 0, 24, s));
+    CU(e, cudaMemsetAsync(t.d_build_seq, 0, 8, s));
+    CU(e, cudaMemsetAsync(&e->d_ctr->delta_build, 0, 4, s));
+    tbl_park_kernel<<<grid_for(e, N), TBL_THREADS, 0, s>>>(e->d_x, e->d_z, (uint32_t)N);  // every slot starts outside the world
+    KCHECK(e);
+    CU(e, cudaStreamSynchronize(s));
+    e->pos_x = e->d_x;
+    e->pos_z = e->d_z;
+    t.bits = bits;
+    t.on = true;
+    return CHD_OK;
+}
+
+chd_status chd_spawn_entities(chd_engine* e, const uint32_t* id, const double* x, const double* z, uint32_t n, uint8_t* out_status) {
+    return spawn(e, "chd_spawn_entities", id, x, z, false, n, out_status);
+}
+chd_status chd_spawn_entities_f32(chd_engine* e, const uint32_t* id, const float* x, const float* z, uint32_t n, uint8_t* out_status) {
+    return spawn(e, "chd_spawn_entities_f32", id, x, z, true, n, out_status);
+}
+
+chd_status chd_despawn_entities(chd_engine* e, const uint32_t* id_in, uint32_t n, uint8_t* out_status) {
+    if (!e || (n && !id_in)) return CHD_ERR_INVALID;
+    chd_status st = need_table(e, "chd_despawn_entities");
+    if (st != CHD_OK) return st;
+    CU(e, cudaSetDevice(e->device));
+    chd_engine::Table& t = e->tbl;
+    std::vector<uint32_t> kid;
+    const uint32_t* ids = nullptr;
+    st = host_view(e, id_in, n, kid, &ids);
+    if (st != CHD_OK) return st;
+    std::vector<uint8_t> status(n, (uint8_t)CHD_EV_OK);
+    std::vector<uint32_t> aid, aslot;
+    std::unordered_set<uint32_t> seen;
+    seen.reserve(n);
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t id = ids[i];
+        if (reserved_id(id)) {
+            status[i] = CHD_EV_RESERVED_ID;
+            continue;
+        }
+        if (!seen.insert(id).second) {
+            status[i] = CHD_EV_DUPLICATE;
+            continue;
+        }
+        auto it = t.slot_of.find(id);
+        if (it == t.slot_of.end()) {
+            status[i] = CHD_EV_UNKNOWN_ID;
+            continue;
+        }
+        const uint32_t slot = it->second;
+        t.slot_of.erase(it);
+        aid.push_back(id);
+        aslot.push_back(slot);
+        // With visible deltas on, the slot waits until a delta that measured a build without it has succeeded: reused earlier, the
+        // snapshot would still hold the old instance there and the delta could not tell the two apart.
+        if (e->dl.on)
+            t.quarantine.push_back(chd_engine::Table::Held{slot, t.builds + 1});
+        else
+            t.free_fifo.push_back(slot);
+    }
+    const uint32_t m = (uint32_t)aid.size();
+    if (m) {
+        StageTimer timer(e, e->stream, CHD_STAGE_ENTITY_EVENTS);
+        st = upload_events(e, aid, aslot, nullptr, nullptr);
+        if (st != CHD_OK) return st;
+        tbl_despawn_kernel<<<grid_for(e, m), TBL_THREADS, 0, e->stream>>>(t.d_table, t.bits, t.d_ev, t.d_ev + m, m, t.d_id_of_slot, e->d_x, e->d_z, t.d_flag);
+        KCHECK(e);
+        touched(e);
+    }
+    return put_status(e, out_status, status);
+}
+
+chd_status chd_move_entities(chd_engine* e, const uint32_t* id, const double* x, const double* z, uint32_t n) {
+    return move(e, "chd_move_entities", id, x, z, false, n);
+}
+chd_status chd_move_entities_f32(chd_engine* e, const uint32_t* id, const float* x, const float* z, uint32_t n) {
+    return move(e, "chd_move_entities_f32", id, x, z, true, n);
+}
+
+chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out) {
+    if (!e || !out) return CHD_ERR_INVALID;
+    chd_status st = need_table(e, "chd_get_entity_stats");
+    if (st != CHD_OK) return st;
+    CU(e, cudaSetDevice(e->device));
+    const chd_engine::Table& t = e->tbl;
+    uint64_t* h64 = reinterpret_cast<uint64_t*>(e->h_get);
+    CU(e, cudaMemcpyAsync(h64, t.d_stats, 24, cudaMemcpyDeviceToHost, e->stream));
+    CU(e, cudaStreamSynchronize(e->stream));
+    out->live = (uint32_t)t.slot_of.size();
+    out->high_water = t.hw;
+    out->quarantined = (uint32_t)t.quarantine.size();
+    out->free_slots = (uint32_t)t.free_fifo.size() + (e->lim.max_entities - t.hw);
+    out->moves_applied = h64[0];
+    out->moves_unknown = h64[1];
+    out->moves_superseded = h64[2];
+    out->rebuilds = t.rebuilds;
+    return CHD_OK;
+}
+
+// After every table-mode build, on the build's stream: the id-valued copy of the sorted entity array and, after a fresh cell
+// assignment, the handover list in ids without the slots spawned or despawned since the previous one (then the flags clear).
+chd_status chd_table_after_build(chd_engine* e, cudaStream_t s) {
+    chd_engine::Table& t = e->tbl;
+    if (!t.on) return CHD_OK;
+    const uint32_t n = e->n_own + e->n_halo;
+    const bool raw = t.ho_raw;
+    const uint64_t key = stage_key(0x7461626c65ull, n, raw, e->d_sorted_ent, t.d_sorted_id, t.d_id_of_slot, e->ho_cap);
+    const unsigned grid = (unsigned)e->sm_count * 4;
+    chd_status st = run_stage(e, s, t.g_post, key, [&]() -> chd_status {
+        tbl_gather_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(e->d_sorted_ent, t.d_id_of_slot, n, t.d_sorted_id, t.d_build_seq);
+        KCHECK(e);
+        if (!raw) return CHD_OK;
+        const HandoverOut ho{e->d_ho_entity, e->d_ho_src, e->d_ho_dst, &e->d_ctr->n_handover, e->ho_cap};
+        tbl_handover_stash_kernel<<<grid, TBL_THREADS, 0, s>>>(ho, t.d_ho_tmp, t.d_build_seq + 1);
+        KCHECK(e);
+        CU(e, cudaMemsetAsync(&e->d_ctr->n_handover, 0, 4, s));
+        tbl_handover_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(ho, t.d_ho_tmp, t.d_build_seq + 1, t.d_flag, t.d_id_of_slot);
+        KCHECK(e);
+        if (n) CU(e, cudaMemsetAsync(t.d_flag, 0, n, s));
+        return CHD_OK;
+    });
+    if (st != CHD_OK) return st;
+    t.builds++;
+    t.ho_raw = false;
+    return CHD_OK;
+}
+
+// Inside the visible-delta stage, after the write pass: enter / leave lists from slots to ids, then the snapshot's ids advance.
+chd_status chd_table_delta_ids(chd_engine* e, cudaStream_t s) {
+    chd_engine::Table& t = e->tbl;
+    const chd_engine::Delta& D = e->dl;
+    const unsigned grid = (unsigned)e->sm_count * 8;
+    tbl_delta_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(D.enter_off, D.leave_off, D.n_out, D.enter_cap, D.leave_cap, D.enter, D.leave, t.d_id_of_slot, t.d_snap_id,
+                                                      t.d_build_seq, &e->d_ctr->delta_build);
+    KCHECK(e);
+    tbl_delta_commit_kernel<<<grid, TBL_THREADS, 0, s>>>(D.enter_off, D.leave_off, D.n_out, D.enter_cap, D.leave_cap, t.d_id_of_slot, e->n_sorted, t.d_snap_id);
+    KCHECK(e);
+    return CHD_OK;
+}
+
+// A summary the host decoded says that the last successful delta measured build `delta_build`: the slots despawned before that
+// build are out of every snapshot a later delta compares against, so they may be reused.
+void chd_table_observe(chd_engine* e, uint32_t delta_build) {
+    chd_engine::Table& t = e->tbl;
+    while (!t.quarantine.empty() && t.quarantine.front().build <= delta_build) {
+        t.free_fifo.push_back(t.quarantine.front().slot);
+        t.quarantine.pop_front();
+    }
+}
+}  // extern "C"

@@ -56,13 +56,13 @@ static chd_status emit_kernel_enqueue(chd_engine* e, cudaStream_t s, bool cta_ti
         if (tiles == 0) tiles = 1;
         if (tiles > 0x7fffffffull) tiles = 0x7fffffffull;
         tiles = (tiles + EMIT_TILES_PER_CTA - 1) / EMIT_TILES_PER_CTA;
-        emit_visible_kernel<<<(unsigned)tiles, EMIT_THREADS, CHD_EMIT_DYN_SMEM, s>>>(&e->d_ctr->n_visible, e->d_sorted_ent, e->d_tile_desc, e->d_vis, e->lim.max_visible);
+        emit_visible_kernel<<<(unsigned)tiles, EMIT_THREADS, CHD_EMIT_DYN_SMEM, s>>>(&e->d_ctr->n_visible, chd_sorted_out(e), e->d_tile_desc, e->d_vis, e->lim.max_visible);
         KCHECK(e);
         emit_visible_general_kernel<<<(unsigned)e->sm_count * 2, EMIT_THREADS, 0, s>>>(e->d_general_tiles, e->d_n_general, pb.off + S, P, &e->d_ctr->n_visible,
-                                                                                       e->d_voff, pb.cell, e->d_cell_start, e->d_sorted_ent,
+                                                                                       e->d_voff, pb.cell, e->d_cell_start, chd_sorted_out(e),
                                                                                        e->d_first_pair, e->d_vis, e->lim.max_visible);
     } else {
-        emit_visible_warp_kernel<<<(unsigned)e->sm_count * 4, EMIT_THREADS, 0, s>>>(pb.off + S, P, e->d_voff, pb.cell, e->d_cell_start, e->d_sorted_ent,
+        emit_visible_warp_kernel<<<(unsigned)e->sm_count * 4, EMIT_THREADS, 0, s>>>(pb.off + S, P, e->d_voff, pb.cell, e->d_cell_start, chd_sorted_out(e),
                                                                                     e->d_first_pair, e->d_vis, e->lim.max_visible);
     }
     KCHECK(e);
@@ -362,6 +362,7 @@ chd_status chd_summary(chd_engine* e, chd_tick_summary* out) {
 
 chd_status chd_decode_summary(chd_engine* e, chd_tick_summary* out) {
     const Counters& c = *e->h_ctr;
+    if (e->tbl.on) chd_table_observe(e, c.delta_build);
     out->n_pairs = c.n_pairs; out->n_visible = c.n_visible; out->n_entities_in_world = c.n_entities_in_world;
     out->n_query_errors = c.n_query_errors; out->n_sub_new = c.n_sub_new; out->n_unsub = c.n_unsub; out->n_kept = c.n_kept;
     out->n_due = c.n_due; out->n_handover = c.n_handover; out->overflow = c.overflow; out->required_pairs = c.required_pairs;

@@ -88,7 +88,8 @@ struct Counters {  // device mirror of chd_tick_summary's counters
     unsigned long long n_pairs, n_visible;
     uint32_t n_entities_in_world, n_query_errors, n_sub_new, n_unsub, n_kept, n_due, n_handover, overflow;
     unsigned long long required_pairs, required_window_cells, required_visible;
-    uint32_t required_due, reserved;
+    uint32_t required_due;
+    uint32_t delta_build;  // entity-table mode: the build number the last successful visible delta measured (chd_table.cuh)
 };
 
 // Pending lifecycle change of a subscriber slot, applied by the next interest update (chd_interest.cuh):

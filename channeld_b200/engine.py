@@ -349,6 +349,48 @@ class Engine:
         self._ck(self.L.chd_get_visible_delta(self.h, ptr(eo), ptr(en), ptr(lo), ptr(le), max(ne, nl, 1), None, None, None))
         return eo, en[:ne], lo, le[:nl]
 
+    # ---- entity-table mode: entities spawned, moved and despawned by id; every result names ids
+    def entity_table_init(self):
+        self._ck(self.L.chd_entity_table_init(self.h))
+
+    def _events(self, fn, ids, x=None, z=None, dtype=np.float64, status=True):
+        # numpy arrays and sequences are converted; torch tensors (pinned host or CUDA) are passed as they are
+        if not hasattr(ids, "data_ptr"):
+            ids = np.ascontiguousarray(ids, np.uint32)
+        if x is not None and not hasattr(x, "data_ptr"):
+            x = np.ascontiguousarray(x, dtype)
+            z = np.ascontiguousarray(z, dtype)
+        n = len(ids)
+        args = [self.h, ptr(ids)] + ([] if x is None else [ptr(x), ptr(z)]) + [n]
+        if not status:
+            self._keep_moves = [ids, x, z]  # the H2D copy is asynchronous: referenced until the next move
+            self._ck(fn(*args))
+            return None
+        st = np.zeros(n, np.uint8)
+        self._ck(fn(*(args + [ptr(st)])))
+        return st
+
+    def spawn_entities(self, ids, x, z):
+        """-> per-event status (capi.EV_*)."""
+        return self._events(self.L.chd_spawn_entities, ids, x, z)
+
+    def spawn_entities_f32(self, ids, x, z):
+        return self._events(self.L.chd_spawn_entities_f32, ids, x, z, np.float32)
+
+    def despawn_entities(self, ids):
+        return self._events(self.L.chd_despawn_entities, ids)
+
+    def move_entities(self, ids, x, z):
+        self._events(self.L.chd_move_entities, ids, x, z, status=False)
+
+    def move_entities_f32(self, ids, x, z):
+        self._events(self.L.chd_move_entities_f32, ids, x, z, np.float32, status=False)
+
+    def entity_stats(self):
+        s = capi.EntityStats()
+        self._ck(self.L.chd_get_entity_stats(self.h, C.byref(s)))
+        return s.as_dict()
+
     def device_view(self, which):
         p, n = C.c_void_p(), C.c_uint64()
         self._ck(self.L.chd_device_view(self.h, which, C.byref(p), C.byref(n)))

@@ -281,14 +281,47 @@ class GpuStaticGrid2DSpatialController {
         return r;
     }
 
+    // Entities keyed by NetGUID (entity-table mode, include/chd_gpu.h): SpawnObjects = handleSpawnObject's GetChannelId +
+    // addSpatialEntity (pkg/unreal/message.go:20-150), DestroyObjects = the destroy handler (message.go:152-203), MoveEntities =
+    // ENTITY-channel updates whose Merge hook calls Notify for that entity alone (spatial.go:612-626).  The first call switches the
+    // engine into the mode; from then on every result names NetGUIDs.  Spawn / destroy return a CHD_EV_* status per id.
+    std::vector<uint8_t> SpawnObjects(const std::vector<uint32_t>& net_id, const std::vector<double>& x, const std::vector<double>& z) {
+        if (x.size() != net_id.size() || z.size() != net_id.size()) throw SpatialError("SpawnObjects: array sizes differ");
+        Table();
+        std::vector<uint8_t> st(net_id.size());
+        check(chd_spawn_entities(engine_, net_id.data(), x.data(), z.data(), (uint32_t)net_id.size(), st.data()));
+        return st;
+    }
+    std::vector<uint8_t> DestroyObjects(const std::vector<uint32_t>& net_id) {
+        Table();
+        std::vector<uint8_t> st(net_id.size());
+        check(chd_despawn_entities(engine_, net_id.data(), (uint32_t)net_id.size(), st.data()));
+        return st;
+    }
+    // stream-ordered: the arrays are read after the call returns (keep them until the next Summary / FetchResults)
+    void MoveEntities(const uint32_t* net_id, const float* x, const float* z, uint32_t n) {
+        Table();
+        check(chd_move_entities_f32(engine_, net_id, x, z, n));
+    }
+    chd_entity_stats GetEntityStats() {
+        chd_entity_stats s{};
+        check(chd_get_entity_stats(engine_, &s));
+        return s;
+    }
+
     chd_engine* engine() { return engine_; }
 
    private:
+    void Table() {
+        if (!table_) check(chd_entity_table_init(engine_));
+        table_ = true;
+    }
     void check(chd_status st) const {
         if (st != CHD_OK) throw SpatialError(chd_last_error(engine_));
     }
     chd_grid_cfg cfg_{};
     chd_engine* engine_ = nullptr;
+    bool table_ = false;
 };
 
 }  // namespace channeld

@@ -32,8 +32,9 @@ import (
 type GpuStaticGrid2DSpatialController struct {
 	StaticGrid2DSpatialController // LoadConfig fields, GetRegions, CreateChannels, Tick, Notify orchestration
 
-	engine *C.chd_engine
-	mu     sync.Mutex // chd_cell_of / chd_query_channel_ids are internally locked; this guards engine lifetime
+	engine  *C.chd_engine
+	mu      sync.Mutex // chd_cell_of / chd_query_channel_ids are internally locked; this guards engine lifetime
+	tableOn bool       // entity-table mode (SpawnObjects / DestroyObjects / MoveEntities)
 }
 
 // LoadConfig (spatial.go:141-159) + engine creation.  ServerInterestBorderSize == 0 is tolerated like
@@ -434,11 +435,82 @@ func (ctl *GpuStaticGrid2DSpatialController) VisibleDelta() (enterOff []uint64, 
 	return enterOff, enter[:ne], leaveOff, leave[:nl], nil
 }
 
+// SpawnObjects / DestroyObjects / MoveEntities deliver entities the way channeld does, keyed by NetGUID (entity-table mode,
+// chd_entity_table_init, switched on by the first call): SpawnObjects = handleSpawnObject's GetChannelId + addSpatialEntity
+// (pkg/unreal/message.go:20-150), DestroyObjects = the destroy handler (message.go:152-203), MoveEntities = ENTITY-channel updates
+// whose Merge hook calls Notify for that entity alone (spatial.go:612-626).  Every result then names NetGUIDs (cells, visible
+// lists, handovers, deltas).  Spawn / destroy statuses (CHD_EV_*) come back before the call returns, so Go slices are fine there;
+// MoveEntities is stream-ordered and its arrays must be C memory (PinnedUint32s / PinnedFloat32s).  UN-RUN like the rest of this file.
+func (ctl *GpuStaticGrid2DSpatialController) entityTable() error {
+	if ctl.tableOn {
+		return nil
+	}
+	if st := C.chd_entity_table_init(ctl.engine); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	ctl.tableOn = true
+	return nil
+}
+
+func (ctl *GpuStaticGrid2DSpatialController) SpawnObjects(netIds []uint32, x, z []float64) ([]uint8, error) {
+	if len(x) != len(netIds) || len(z) != len(netIds) {
+		return nil, errors.New("SpawnObjects: array sizes differ")
+	}
+	if err := ctl.entityTable(); err != nil || len(netIds) == 0 {
+		return nil, err
+	}
+	status := make([]uint8, len(netIds))
+	if st := C.chd_spawn_entities(ctl.engine, (*C.uint32_t)(unsafe.Pointer(&netIds[0])), (*C.double)(unsafe.Pointer(&x[0])),
+		(*C.double)(unsafe.Pointer(&z[0])), C.uint32_t(len(netIds)), (*C.uint8_t)(unsafe.Pointer(&status[0]))); st != C.CHD_OK {
+		return nil, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return status, nil
+}
+
+func (ctl *GpuStaticGrid2DSpatialController) DestroyObjects(netIds []uint32) ([]uint8, error) {
+	if err := ctl.entityTable(); err != nil || len(netIds) == 0 {
+		return nil, err
+	}
+	status := make([]uint8, len(netIds))
+	if st := C.chd_despawn_entities(ctl.engine, (*C.uint32_t)(unsafe.Pointer(&netIds[0])), C.uint32_t(len(netIds)),
+		(*C.uint8_t)(unsafe.Pointer(&status[0]))); st != C.CHD_OK {
+		return nil, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return status, nil
+}
+
+// MoveEntities: netIds / x / z in C memory, valid until the next Summary / FetchResults.  The last move of an id in one call wins;
+// moves of ids that are not live are ignored (counted in EntityStats).
+func (ctl *GpuStaticGrid2DSpatialController) MoveEntities(netIds []uint32, x, z []float32) error {
+	if len(x) != len(netIds) || len(z) != len(netIds) {
+		return errors.New("MoveEntities: array sizes differ")
+	}
+	if err := ctl.entityTable(); err != nil || len(netIds) == 0 {
+		return err
+	}
+	if st := C.chd_move_entities_f32(ctl.engine, (*C.uint32_t)(unsafe.Pointer(&netIds[0])), (*C.float)(unsafe.Pointer(&x[0])),
+		(*C.float)(unsafe.Pointer(&z[0])), C.uint32_t(len(netIds))); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
+func (ctl *GpuStaticGrid2DSpatialController) EntityStats() (C.chd_entity_stats, error) {
+	var s C.chd_entity_stats
+	if st := C.chd_get_entity_stats(ctl.engine, &s); st != C.CHD_OK {
+		return s, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return s, nil
+}
+
 // PinnedFloat64s / PinnedUint32s / PinnedInt64s / PinnedUint64s carve staging slices out of page-locked C memory
 // (chd_alloc_pinned): uploads from them are truly asynchronous and, being C memory, they may be referenced by the
 // engine after a cgo call has returned (PrefetchTick).  Release with FreePinned(unsafe.Pointer(&s[0])).
 func PinnedFloat64s(n int) []float64 {
 	return unsafe.Slice((*float64)(C.chd_alloc_pinned(C.uint64_t(8*n))), n)
+}
+func PinnedFloat32s(n int) []float32 {
+	return unsafe.Slice((*float32)(C.chd_alloc_pinned(C.uint64_t(4*n))), n)
 }
 func PinnedUint32s(n int) []uint32 {
 	return unsafe.Slice((*uint32)(C.chd_alloc_pinned(C.uint64_t(4*n))), n)

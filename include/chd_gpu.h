@@ -101,7 +101,8 @@ chd_status chd_cell_of_valid(chd_engine* e, const double* x, const double* z, ui
 
 /* ---- entity positions (SoA).  Replaces the per-cell entity maps the reference keeps in
  * SpatialChannelData.Entities (pkg/unrealpb/extension.go:38-62) fed by AddEntity/RemoveEntity
- * (spatial.go:606-609,702-736).  Entity i has id i (the host maps it to EntityChannelIdStart + i). */
+ * (spatial.go:606-609,702-736).  Entity i has id i (the host maps it to EntityChannelIdStart + i).  Entity-table mode
+ * (chd_entity_table_init, below) replaces these snapshots with spawn / move / despawn events keyed by id. */
 chd_status chd_set_entities(chd_engine* e, const double* x, const double* z, uint32_t n);
 /* Double-buffered upload for pipelined hosts: chd_prefetch_entities starts copying the NEXT tick's host positions
  * into the engine's second pair of position buffers on a dedicated upload stream and returns immediately; it may be
@@ -374,6 +375,64 @@ chd_status chd_visible_delta(chd_engine* e);
 chd_status chd_get_visible_delta(chd_engine* e, uint64_t* enter_off, uint32_t* enter_entity, uint64_t* leave_off, uint32_t* leave_entity,
                                  uint64_t cap, uint64_t* n_entered, uint64_t* n_left, uint32_t* n_slots);
 
+/* ---- entity-table mode: entities as events keyed by id, as channeld delivers them (SpawnObjectMessage / DestroyObjectMessage,
+ * pkg/unreal/message.go:20-203; a move is an ENTITY-channel update whose Merge hook calls Notify for that entity alone,
+ * spatial.go:612-626).  The engine keeps the id -> slot map and assigns position slots itself; the host never sees a slot.
+ *   chd_entity_table_init  switches a FRESH engine into table mode (CHD_ERR_STATE after any chd_set_entities* / chd_prefetch_entities*
+ *                          / chd_build, or after chd_set_slab / chd_set_entity_ids / chd_comm_init).  Allocates the device id table
+ *                          (2^k >= 2 x max_entities words) and the slot -> id array, and parks every position slot (NaN: outside
+ *                          the world).  From then on chd_set_entities*, chd_prefetch_entities*, chd_entity_buffers,
+ *                          chd_set_entity_count, chd_set_entity_ids and the multi-GPU calls (chd_set_slab, chd_export_border,
+ *                          chd_import_halo, chd_comm_init, chd_tick_sharded) return CHD_ERR_STATE: the mode is single-GPU.
+ *   chd_spawn_entities     AddEntity for each (id[i], x[i], z[i]); _f32: FVector positions, widened exactly as chd_set_entities_f32
+ *                          widens them.  out_status[i] (may be NULL) is one CHD_EV_* per event, written before the call returns.
+ *   chd_despawn_entities   RemoveEntity for each id[i]; out_status as for spawns.
+ *   chd_move_entities      new positions of live ids (_f32: FVector positions).  If one call moves an id several times the LAST one
+ *                          in array order wins (the reference applies updates in arrival order).  A move of an id that is not live
+ *                          (reserved ids included) is ignored and counted.  Ids are resolved on the device.
+ *   chd_get_entity_stats   synchronous counters (below).
+ * Events are stream-ordered and apply in call order; pointer rules are those of chd_set_entities (host inputs are copied, device
+ * inputs of a move are read in place; the ids and positions of a spawn / despawn are read on the host, a device array is copied back
+ * first).  Statuses:
+ *   reserved ids  0 and 0xFFFFFFFF are rejected (CHD_EV_RESERVED_ID; a NetGUID of 0 is invalid in the reference, message.go:40-43);
+ *   duplicate     a spawn of a live id, or an id repeated in one spawn / despawn call (the first occurrence is applied);
+ *   unknown id    a despawn of an id that is not live;
+ *   table full    no slot is free (see the quarantine below).
+ * A rejected event changes nothing.  A spawn outside the world is live but in no cell (the reference logs it and does not add it);
+ * a later move into the world is reported as a handover from 0.
+ * Results in table mode name IDS: the cell CSR's sorted_entity (chd_get_cells, chd_fetch_results*, CHD_VIEW_SORTED_ENTITY), the
+ * visible lists, the handover list (chd_get_handover, the fetch paths, summary.n_handover) and the visible-set deltas.  Inside a
+ * cell, entries are in slot order; slots are assigned deterministically (a released slot first in first out, then the next fresh
+ * one), so the same event sequence gives identical arrays, with or without CUDA graphs.  The handover list holds the moved entities
+ * whose cell changed since the previous build, including dst = 0 for leaving the world; entities spawned or despawned since then are
+ * not in it (those are AddEntity / RemoveEntity, not Notify); after a standalone chd_assign_cells it names ids once the following
+ * chd_build has run.  CHD_VIEW_ENTITY_ID gives the id of each slot (0 = empty) for
+ * consumers that stay on the device.
+ * Visible-set deltas work in table mode: a despawned id that is spawned again is a new instance, in `leave` (the old one) and in
+ * `enter` (the new one).  Slot quarantine keeps that exact: without chd_reserve_visible_delta a despawned slot may be reused by the
+ * next spawn call; with it, only after a delta that ran after the despawn has SUCCEEDED, as observed by the library in a summary it
+ * read (chd_summary, chd_tick with `out`, chd_fetch_results, chd_fetch_wait); after CHD_OVF_DELTA the slot stays quarantined.
+ * Until a slot is released spawns take fresh ones, and when none is left the status is CHD_EV_TABLE_FULL.  A standalone
+ * chd_visible_delta needs a chd_build after the last event (CHD_ERR_STATE otherwise; chd_tick builds first). */
+enum { CHD_EV_OK = 0, CHD_EV_DUPLICATE = 1, CHD_EV_UNKNOWN_ID = 2, CHD_EV_RESERVED_ID = 3, CHD_EV_TABLE_FULL = 4 };
+typedef struct chd_entity_stats {
+    uint32_t live;              /* ids spawned and not despawned */
+    uint32_t high_water;        /* slots ever used (the entity count every build covers) */
+    uint32_t quarantined;       /* despawned slots waiting for a successful visible delta */
+    uint32_t free_slots;        /* slots a spawn could take now: released ones + max_entities - high_water */
+    uint64_t moves_applied;     /* since chd_entity_table_init */
+    uint64_t moves_unknown;     /* moves of ids that were not live */
+    uint64_t moves_superseded;  /* moves overridden by a later move of the same id in the same call */
+    uint64_t rebuilds;          /* device id-table rebuilds (live entries + tombstones passed 3/4 of the table) */
+} chd_entity_stats;
+chd_status chd_entity_table_init(chd_engine* e);
+chd_status chd_spawn_entities(chd_engine* e, const uint32_t* id, const double* x, const double* z, uint32_t n, uint8_t* out_status);
+chd_status chd_spawn_entities_f32(chd_engine* e, const uint32_t* id, const float* x, const float* z, uint32_t n, uint8_t* out_status);
+chd_status chd_despawn_entities(chd_engine* e, const uint32_t* id, uint32_t n, uint8_t* out_status);
+chd_status chd_move_entities(chd_engine* e, const uint32_t* id, const double* x, const double* z, uint32_t n);
+chd_status chd_move_entities_f32(chd_engine* e, const uint32_t* id, const float* x, const float* z, uint32_t n);
+chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out);
+
 /* ---- all host-facing results of a tick in ONE call instead of one or two synchronisations per getter.  After a
  * two-stream tick (chd_tick with emit, or chd_begin_interest + chd_tick) the lists are copied in the order they become
  * final, on the engine's read-back streams, while the expanded-list kernel may still be running: first the pairs /
@@ -421,7 +480,9 @@ enum {
     CHD_VIEW_CELL_START = 0, CHD_VIEW_SORTED_ENTITY, CHD_VIEW_ENT_CELL, CHD_VIEW_PAIR_OFF, CHD_VIEW_PAIR_CHANNEL,
     CHD_VIEW_PAIR_DIST, CHD_VIEW_VIS_OFF, CHD_VIEW_VIS_ENTITY, CHD_VIEW_DUE,
     /* the visible-set delta (chd_visible_delta): u64 offsets [slots + 1] and u32 entities [capacity] of each list */
-    CHD_VIEW_DELTA_ENTER_OFF, CHD_VIEW_DELTA_ENTER, CHD_VIEW_DELTA_LEAVE_OFF, CHD_VIEW_DELTA_LEAVE
+    CHD_VIEW_DELTA_ENTER_OFF, CHD_VIEW_DELTA_ENTER, CHD_VIEW_DELTA_LEAVE_OFF, CHD_VIEW_DELTA_LEAVE,
+    /* entity-table mode: u32 id of each slot [high-water mark], 0 = empty */
+    CHD_VIEW_ENTITY_ID
 };
 chd_status chd_device_view(chd_engine* e, int which, void** d_ptr, uint64_t* count);
 
@@ -583,6 +644,7 @@ enum { CHD_STAGE_BUILD = 0, CHD_STAGE_INTEREST, CHD_STAGE_EMIT, CHD_STAGE_EMIT_K
        CHD_STAGE_EXPORT, CHD_STAGE_EXCHANGE, CHD_STAGE_IMPORT, /* the three steps of chd_tick_sharded before the tick proper */
        CHD_STAGE_READBACK,                                     /* chd_fetch_results_async: the PCIe hop (snapshot -> pinned host) */
        CHD_STAGE_VISIBLE_DELTA,                                /* chd_visible_delta / CHD_TICK_VISIBLE_DELTA */
+       CHD_STAGE_ENTITY_EVENTS,                                /* chd_spawn_entities* / chd_move_entities* / chd_despawn_entities */
        CHD_STAGE_COUNT };
 uint64_t chd_launch_count(const chd_engine* e);
 /* The launch-bound stages (build, interest update, emit preparation, fan-out) are replayed as CUDA graphs once
