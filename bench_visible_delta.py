@@ -1,9 +1,10 @@
 """Cost and size of the visible-set delta (chd_visible_delta) at the benchmark configuration (1 M entities, 100 K subscribers,
 r = 50, 15 x 15 cells), with every entity moving every tick (synth.move_entities, max step 60) and every subscriber standing on
-its entity.  Three tick forms run on three engines with identical inputs, in alternating blocks of ticks:
+its entity.  Four tick forms run on four engines with identical inputs, in alternating blocks of ticks:
     all        CHD_TICK_ALL
     all+delta  CHD_TICK_ALL | CHD_TICK_VISIBLE_DELTA
     delta      CHD_TICK_BUILD | CHD_TICK_FANOUT | CHD_TICK_VISIBLE_DELTA  (no expanded lists)
+    delta ids  the same in id mode (chd_reserve_visible_delta_ids): the entities carry a fixed permutation as global ids
 Prints one JSON line: the card and its power limit, device ms per tick of each form (CHD_STAGE_TICK: the engine stream's span of
 the tick, per-stage profiling on), the delta stage's own time (CHD_STAGE_VISIBLE_DELTA) and entered + left entries per tick
 against the visible-list size V.  Reads nothing outside the repository and writes nothing.
@@ -47,14 +48,18 @@ def main():
     idx = (np.arange(S, dtype=np.int64) * (N // S)) % N
     r = np.full(S, wc.radius)
     forms = {"all": capi.TICK_ALL, "all+delta": capi.TICK_ALL | capi.TICK_VISIBLE_DELTA,
-             "delta": capi.TICK_BUILD | capi.TICK_FANOUT | capi.TICK_VISIBLE_DELTA}
+             "delta": capi.TICK_BUILD | capi.TICK_FANOUT | capi.TICK_VISIBLE_DELTA,
+             "delta ids": capi.TICK_BUILD | capi.TICK_FANOUT | capi.TICK_VISIBLE_DELTA}
     _, off, arr, snd, ridx, cmi = synth.update_rings(wc, 0, 0, 33_000_000, 4, S, ring_len=64)
     runs = {}
     for name, flags in forms.items():
         e = engine.Engine(wc.cfg(), N, S)
         e.set_subscribers(np.arange(1, S + 1, dtype=np.uint32))
         e.set_rings(off, arr, snd, ridx, cmi)
-        if flags & capi.TICK_VISIBLE_DELTA:
+        if name == "delta ids":
+            e.set_entity_ids(np.random.default_rng(1).permutation(N).astype(np.uint32))
+            e.reserve_visible_delta_ids(600_000_000, N)
+        elif flags & capi.TICK_VISIBLE_DELTA:
             e.reserve_visible_delta(600_000_000)  # the first delta enters every visible list (V = 4.9e8)
         runs[name] = dict(e=e, flags=flags, x=x0.copy(), z=z0.copy(), t=0, tick_ms=[], delta_ms=[], changes=[], visible=[])
 

@@ -26,6 +26,7 @@ TICK_EARLY_RESULTS = 8
 TICK_VISIBLE_DELTA = 16
 OVF_PAIRS, OVF_WINDOW, OVF_VISIBLE, OVF_DUE, OVF_BORDER, OVF_RING = 1, 2, 4, 8, 16, 32
 OVF_DELTA = 64
+OVF_DELTA_IDS = 128
 (VIEW_CELL_START, VIEW_SORTED_ENTITY, VIEW_ENT_CELL, VIEW_PAIR_OFF, VIEW_PAIR_CHANNEL, VIEW_PAIR_DIST, VIEW_VIS_OFF, VIEW_VIS_ENTITY, VIEW_DUE,
  VIEW_DELTA_ENTER_OFF, VIEW_DELTA_ENTER, VIEW_DELTA_LEAVE_OFF, VIEW_DELTA_LEAVE, VIEW_ENTITY_ID) = range(14)
 # per-event statuses of chd_spawn_entities / chd_despawn_entities (entity-table mode)
@@ -135,7 +136,7 @@ SYMBOLS = [
     "chd_get_regions", "chd_damping_interval_ms", "chd_launch_count", "chd_profile_enable", "chd_profile_get", "chd_profile_timeline", "chd_enable_graphs",
     "chd_graph_launch_count",
     "chd_add_subscribers", "chd_remove_subscribers", "chd_fetch_results_async", "chd_fetch_wait", "chd_rings_init", "chd_rings_append", "chd_get_rings", "chd_set_channel_start_times", "chd_set_payload_bytes", "chd_assemble_payloads", "chd_frame_packets", "chd_comm_unique_id", "chd_comm_init", "chd_comm_info", "chd_comm_destroy", "chd_tick_sharded", "chd_collective_count", "chd_comm_exchange_mode", "chd_comm_use_collective", "chd_migrate_out", "chd_migrate_in", "chd_get_rehome",
-    "chd_reserve_visible_delta", "chd_visible_delta", "chd_get_visible_delta",
+    "chd_reserve_visible_delta", "chd_reserve_visible_delta_ids", "chd_visible_delta", "chd_get_visible_delta",
     "chd_entity_table_init", "chd_spawn_entities", "chd_spawn_entities_f32", "chd_despawn_entities", "chd_move_entities", "chd_move_entities_f32",
     "chd_get_entity_stats",
 ]
@@ -315,6 +316,8 @@ def lib():
     L.chd_comm_use_collective.argtypes = [vp, C.c_int]
     L.chd_reserve_visible_delta.restype = C.c_int
     L.chd_reserve_visible_delta.argtypes = [vp, C.c_uint64]
+    L.chd_reserve_visible_delta_ids.restype = C.c_int
+    L.chd_reserve_visible_delta_ids.argtypes = [vp, C.c_uint64, C.c_uint32]
     L.chd_visible_delta.restype = C.c_int
     L.chd_visible_delta.argtypes = [vp]
     L.chd_get_visible_delta.restype = C.c_int

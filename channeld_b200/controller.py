@@ -247,6 +247,11 @@ class GpuStaticGrid2DSpatialController:
     def ReserveVisibleDelta(self, cap_entries):
         self.engine.reserve_visible_delta(cap_entries)
 
-    # -> (enter_off, enter, leave_off, leave): CSR by subscriber slot of entity indices.
+    # The same with entities named by global id in [0, id_space) (engine.set_entity_ids / the halo records): the mode for
+    # sharded engines.  Migrated connections are netted on the host (sharding.net_migrant_delta).
+    def ReserveVisibleDeltaIds(self, cap_entries, id_space):
+        self.engine.reserve_visible_delta_ids(cap_entries, id_space)
+
+    # -> (enter_off, enter, leave_off, leave): CSR by subscriber slot of entity indices (global ids in id mode).
     def GetVisibleDelta(self):
         return self.engine.get_visible_delta()

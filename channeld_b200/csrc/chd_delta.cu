@@ -22,18 +22,41 @@ static DeltaDev delta_view(chd_engine* e) {
     d.enter = D.enter; d.leave = D.leave; d.enter_cap = D.enter_cap; d.leave_cap = D.leave_cap;
     d.n_out = D.n_out;
     d.overflow = &e->d_ctr->overflow;
+    d.bad_ids = nullptr;
+    if (D.ids) {
+        // Id mode: the cell CSRs (now: the build's d_sorted_ent, sorted with d_gid as values; snapshot: its copy) hold global ids, so
+        // the kernels must look an entity's cell up by global id.  now_gkey is that lookup for the current state and snap_key, copied
+        // from it by the advance, for the snapshot; snap_hdr[0] = n = id_space once a delta has succeeded (0 before: nothing).
+        // The kernels treat `e < n ? key[e] : cells` and `ent >= other_n` as "absent"; that stays right because
+        //   - every id of a state whose lists are written is < id_space (the scatter checks it, else CHD_OVF_DELTA_IDS);
+        //   - an id < id_space that is absent from a state reads 0xFFFFFFFF there, which, like `cells`, no cell list holds;
+        //   - an id is in at most one cell (duplicates are refused), as an index is in index mode.
+        d.key = D.now_gkey;
+        d.n = D.id_space;
+        d.bad_ids = D.bad_ids;
+    }
     return d;
 }
 
 extern "C" {
 
 chd_status chd_delta_check(chd_engine* e, bool will_build) {
-    if (e->delta_blocked) {
-        e->fail("visible deltas are single-GPU only: this engine used chd_set_slab / chd_set_entity_ids / chd_comm_init");
+    if (e->delta_blocked && !e->dl.ids) {
+        e->fail("index-mode visible deltas are single-GPU only: this engine used chd_set_slab / chd_set_entity_ids / chd_comm_init "
+                "(chd_reserve_visible_delta_ids names entities by global id instead)");
         return CHD_ERR_STATE;
     }
     if (!e->dl.on) {
         e->fail("visible delta before chd_reserve_visible_delta");
+        return CHD_ERR_STATE;
+    }
+    if (e->dl.ids && !e->have_gid) {
+        e->fail("id-mode visible delta on an engine without global ids (chd_set_entity_ids)");
+        return CHD_ERR_STATE;
+    }
+    if (!will_build && e->dl.ids && e->entities_dirty) {
+        // id mode: the ids scattered by the delta must be those the build sorted
+        e->fail("id-mode visible delta needs a chd_build after the last chd_set_entities / chd_set_entity_ids / chd_import_halo");
         return CHD_ERR_STATE;
     }
     if (!will_build && (!e->built || (e->assigned && e->entities_dirty))) {
@@ -59,14 +82,29 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
     chd_status st = chd_epoch_tick(e, s, EP_DELTA);
     if (st != CHD_OK) return st;
     // sizes and the key / pair buffers in use are baked into the captured launches
-    const uint64_t key = stage_key(0x64656c7461ull, d.n, d.n_slots, D.n_out, e->cur, d.key, d.enter, d.leave, d.enter_cap, d.leave_cap, e->tbl.on,
-                                   e->tbl.d_id_of_slot);
+    uint64_t key = stage_key(0x64656c7461ull, d.n, d.n_slots, D.n_out, e->cur, d.key, d.enter, d.leave, d.enter_cap, d.leave_cap, e->tbl.on,
+                             e->tbl.d_id_of_slot);
+    // id mode: the scatter bakes in the build's length (host count or d_n_build) and the key / id buffers it reads
+    const uint32_t* n_ptr = e->sorted_dev_n ? e->d_n_build : nullptr;
+    const uint32_t n_scatter = e->sorted_dev_n ? e->lim.max_entities : e->n_sorted;
+    if (D.ids) key = stage_key(key, 0x696473ull, D.id_space, n_scatter, n_ptr, e->d_key, e->d_gid, e->d_n_build);
     const unsigned grid = (unsigned)e->sm_count * 8;
     const unsigned slot_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(blocks_for((uint64_t)D.n_out * 32, DELTA_THREADS), (uint64_t)e->sm_count * 32));
     return run_stage(e, s, D.g, key, [&]() -> chd_status {
         bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_DELTA);
         KCHECK(e);
-        SCAN(e, exclusive_scan_fn<DeltaArrivalFlag, uint32_t>(DeltaArrivalFlag{d.sorted, d.key, d.snap_key, d.snap_hdr, C}, D.arr_rank, N, D.site_arr, s,
+        if (D.ids) {
+            // The halo import (it writes d_key / d_gid / d_n_build past the own entities) and the build run on the engine stream:
+            // a standalone delta follows them there, and a tick's delta (chd_tick_sharded ends in chd_tick) runs on the engine stream
+            // after its build or on prep_stream after dl.ev_in, recorded on the engine stream after the build.  Either way the
+            // scatter reads this tick's imported halo.
+            CU(e, cudaMemsetAsync(D.now_gkey, 0xFF, 4ull * D.id_space, s));
+            CU(e, cudaMemsetAsync(D.bad_ids, 0, 4, s));
+            delta_id_scatter_kernel<<<grid, DELTA_THREADS, 0, s>>>(e->d_gid, e->d_key, n_scatter, n_ptr, C, D.now_gkey, D.id_space, D.bad_ids,
+                                                                   d.overflow);
+            KCHECK(e);
+        }
+        SCAN(e, exclusive_scan_fn<DeltaArrivalFlag, uint32_t>(DeltaArrivalFlag{d.sorted, d.key, d.snap_key, d.snap_hdr, d.n, C}, D.arr_rank, N, D.site_arr, s,
                                                               d.cell_start + C));
         SCAN(e, exclusive_scan_fn<DeltaDepartureFlag, uint32_t>(DeltaDepartureFlag{d.snap_sorted, d.snap_key, d.key, d.n, C}, D.dep_rank, N, D.site_dep, s,
                                                                 d.snap_cell_start + C));
@@ -88,9 +126,8 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
     });
 }
 
-chd_status chd_reserve_visible_delta(chd_engine* e, uint64_t cap_entries) {
-    if (!e) return CHD_ERR_INVALID;
-    if (e->delta_blocked) return chd_delta_check(e, true);
+// The first reserve picks the mode (ids: id mode over [0, id_space)) and allocates; every later one only grows the lists.
+static chd_status delta_reserve(chd_engine* e, uint64_t cap_entries, bool ids, uint32_t id_space) {
     CU(e, cudaSetDevice(e->device));
     // a delta of an earlier tick may still be running (on the engine stream or, inside a tick, on prep_stream)
     CU(e, cudaStreamSynchronize(e->stream));
@@ -98,7 +135,10 @@ chd_status chd_reserve_visible_delta(chd_engine* e, uint64_t cap_entries) {
     chd_engine::Delta& D = e->dl;
     const uint64_t N = e->lim.max_entities, S = e->lim.max_subscribers, P = e->lim.max_pairs, C = e->g.cells;
     if (!D.on) {
-        const bool ok = dalloc(e, &D.snap_key, N) && dalloc(e, &D.snap_cell_start, C + 2) && dalloc(e, &D.snap_sorted, N) &&
+        // id mode: snap_key and now_gkey are indexed by global id
+        const bool ok = dalloc(e, &D.snap_key, ids ? (uint64_t)id_space : N) &&
+                        (!ids || (dalloc(e, &D.now_gkey, id_space) && dalloc(e, &D.bad_ids, 1))) && dalloc(e, &D.snap_cell_start, C + 2) &&
+                        dalloc(e, &D.snap_sorted, N) &&
                         dalloc(e, &D.snap_pair_off, S + 1) && dalloc(e, &D.snap_pair_cell, P) && dalloc(e, &D.snap_hdr, 2) &&
                         dalloc(e, &D.arr_rank, N + 1) && dalloc(e, &D.dep_rank, N + 1) && dalloc(e, &D.arr, N) && dalloc(e, &D.dep, N) &&
                         dalloc(e, &D.arr_start, C + 1) && dalloc(e, &D.dep_start, C + 1) && dalloc(e, &D.cnt_enter, S) &&
@@ -114,14 +154,38 @@ chd_status chd_reserve_visible_delta(chd_engine* e, uint64_t cap_entries) {
         CU(e, cudaMemsetAsync(D.snap_pair_off, 0, (S + 1) * 4, e->stream));
         CU(e, cudaStreamSynchronize(0));  // (chd_make_site clears its descriptors on the default stream)
         D.on = true;
+        D.ids = ids;
+        D.id_space = ids ? id_space : 0;
     }
     if (!ensure_cap(e, &D.enter, &D.enter_cap, cap_entries, cap_entries) || !ensure_cap(e, &D.leave, &D.leave_cap, cap_entries, cap_entries))
         return CHD_ERR_CUDA;
     // the lists of the last delta are gone (a grown buffer starts empty): report an empty delta until the next one
     CU(e, cudaMemsetAsync(D.enter_off, 0, (S + 1) * 8, e->stream));
     CU(e, cudaMemsetAsync(D.leave_off, 0, (S + 1) * 8, e->stream));
+    if (D.ids) CU(e, cudaMemsetAsync(D.bad_ids, 0, 4, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
     return CHD_OK;
+}
+
+chd_status chd_reserve_visible_delta(chd_engine* e, uint64_t cap_entries) {
+    if (!e) return CHD_ERR_INVALID;
+    if (e->dl.ids) return delta_reserve(e, cap_entries, true, e->dl.id_space);  // id mode: grows the lists only
+    if (e->delta_blocked) return chd_delta_check(e, true);
+    return delta_reserve(e, cap_entries, false, 0);
+}
+
+chd_status chd_reserve_visible_delta_ids(chd_engine* e, uint64_t cap_entries, uint32_t id_space) {
+    if (!e || id_space == 0) return CHD_ERR_INVALID;
+    if (e->tbl.on) return chd_table_refuse(e, "chd_reserve_visible_delta_ids");
+    if (e->dl.on && !e->dl.ids) {
+        e->fail("chd_reserve_visible_delta_ids: this engine's visible deltas are in index mode (chd_reserve_visible_delta came first)");
+        return CHD_ERR_STATE;
+    }
+    if (e->dl.on && id_space != e->dl.id_space) {
+        e->fail("chd_reserve_visible_delta_ids: id_space %u differs from the %u the mode was set up with", id_space, e->dl.id_space);
+        return CHD_ERR_INVALID;
+    }
+    return delta_reserve(e, cap_entries, true, id_space);
 }
 
 chd_status chd_visible_delta(chd_engine* e) {
@@ -147,14 +211,21 @@ chd_status chd_get_visible_delta(chd_engine* e, uint64_t* enter_off, uint32_t* e
     uint64_t* h64 = (uint64_t*)e->h_get;
     CU(e, cudaMemcpyAsync(h64, D.enter_off + S, 8, cudaMemcpyDeviceToHost, s));
     CU(e, cudaMemcpyAsync(h64 + 1, D.leave_off + S, 8, cudaMemcpyDeviceToHost, s));
+    if (D.ids) CU(e, cudaMemcpyAsync(h64 + 2, D.bad_ids, 4, cudaMemcpyDeviceToHost, s));
     CU(e, cudaStreamSynchronize(s));
     const uint64_t ne = h64[0], nl = h64[1];
+    const bool bad_ids = D.ids && (uint32_t)h64[2] != 0;
     if (n_entered) *n_entered = ne;
     if (n_left) *n_left = nl;
     if (n_slots) *n_slots = S;
     if (enter_off) CU(e, cudaMemcpyAsync(enter_off, D.enter_off, 8ull * (S + 1ull), cudaMemcpyDefault, s));
     if (leave_off) CU(e, cudaMemcpyAsync(leave_off, D.leave_off, 8ull * (S + 1ull), cudaMemcpyDefault, s));
     if (enter_entity || leave_entity) {
+        if (bad_ids) {
+            CU(e, cudaStreamSynchronize(s));
+            e->fail("the last visible delta met an id >= id_space %u or an id held twice (CHD_OVF_DELTA_IDS): no lists", D.id_space);
+            return CHD_ERR_INVALID;
+        }
         if (ne > D.enter_cap || nl > D.leave_cap) {
             CU(e, cudaStreamSynchronize(s));
             e->fail("the last visible delta overflowed (CHD_OVF_DELTA): %llu entered / %llu left > capacity %llu",

@@ -13,6 +13,10 @@
 //    Every entity comes out once, cells ascending and entities ascending inside a cell: the order of the visible lists, no sort.
 //    A count pass, two scans into u64 offsets and a write pass (one warp per slot).
 // 3. The snapshot advances (device-side copies) only if both lists fitted.
+//
+// Id mode (chd_reserve_visible_delta_ids) runs the same kernels with the entity identity moved from the index to the GLOBAL id:
+// the cell CSRs hold global ids there (the build sorts d_gid as its values), so the stage first scatters every in-world entity's
+// cell into a key array indexed by global id (delta_id_scatter_kernel) and hands that array to the kernels below as `key`.
 #pragma once
 #include "chd_scan.cuh"
 #include "chd_types.cuh"
@@ -41,18 +45,40 @@ struct DeltaDev {
     uint64_t enter_cap, leave_cap;
     uint32_t n_out;  // slots the output CSRs cover (>= n_slots and >= the snapshot's slot count)
     uint32_t* overflow;
+    const uint32_t* bad_ids;  // id mode: nonzero when this state's ids are unusable (CHD_OVF_DELTA_IDS); nullptr in index mode
 };
 
-// position j of the current cell CSR holds an entity that was elsewhere (or absent) at the snapshot
+// position j of the current cell CSR holds an entity that was elsewhere (or absent) at the snapshot.  Every entity of the
+// current CSR is below n, except an out-of-range id of an id-mode state that the stage discards (CHD_OVF_DELTA_IDS).
 struct DeltaArrivalFlag {
     const uint32_t *sorted, *key, *snap_key, *snap_hdr;
-    uint32_t cells;
+    uint32_t n, cells;
     __device__ __forceinline__ uint64_t operator()(uint64_t j) const {
         const uint32_t e = sorted[j];
         const uint32_t was = e < snap_hdr[0] ? snap_key[e] : cells;
-        return was != key[e] ? 1u : 0u;
+        const uint32_t now = e < n ? key[e] : cells;
+        return was != now ? 1u : 0u;
     }
 };
+
+// Id mode: gkey[id] = cell of every in-world entity of the last build (own and halo, i < the build's length), gkey cleared to
+// 0xFFFFFFFF (absent) before.  An id >= id_space, or an id that two in-world entities hold, sets *bad and CHD_OVF_DELTA_IDS.
+__global__ void __launch_bounds__(DELTA_THREADS) delta_id_scatter_kernel(const uint32_t* gid, const uint32_t* key, uint32_t n, const uint32_t* n_ptr,
+                                                                         uint32_t cells, uint32_t* gkey, uint32_t id_space, uint32_t* bad,
+                                                                         uint32_t* overflow) {
+    const uint32_t m = n_ptr ? min(*n_ptr, n) : n;
+    bool err = false;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
+        const uint32_t k = key[i];
+        if (k >= cells) continue;  // an own entity outside the world: absent, never a duplicate
+        const uint32_t g = gid[i];
+        if (g >= id_space || atomicExch(&gkey[g], k) != 0xFFFFFFFFu) err = true;
+    }
+    if (err) {
+        atomicOr(bad, 1u);
+        atomicOr(overflow, (uint32_t)CHD_OVF_DELTA_IDS);
+    }
+}
 
 // position j of the snapshot's cell CSR holds an entity that is elsewhere (or absent) now
 struct DeltaDepartureFlag {
@@ -120,12 +146,14 @@ __device__ __forceinline__ uint32_t delta_side(const uint32_t* from, uint32_t fb
 }
 
 // WRITE = false: per-slot counts; WRITE = true: the lists at the scanned offsets, if both fit (else CHD_OVF_DELTA, nothing written)
+// and the state's ids were usable (else nothing written: the scatter raised CHD_OVF_DELTA_IDS)
 template <bool WRITE>
 __global__ void __launch_bounds__(DELTA_THREADS) delta_slots_kernel(DeltaDev d) {
     if (WRITE && (d.enter_off[d.n_out] > d.enter_cap || d.leave_off[d.n_out] > d.leave_cap)) {
         if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(d.overflow, (uint32_t)CHD_OVF_DELTA);
         return;
     }
+    if (WRITE && d.bad_ids && *d.bad_ids) return;
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
     const uint32_t snap_n = d.snap_hdr[0], snap_slots = d.snap_hdr[1];
@@ -143,9 +171,10 @@ __global__ void __launch_bounds__(DELTA_THREADS) delta_slots_kernel(DeltaDev d) 
     }
 }
 
-// the current state becomes the snapshot, unless a list overflowed
+// the current state becomes the snapshot, unless a list overflowed or its ids were unusable
 __global__ void __launch_bounds__(DELTA_THREADS) delta_advance_kernel(DeltaDev d, uint32_t pairs_max) {
     if (d.enter_off[d.n_out] > d.enter_cap || d.leave_off[d.n_out] > d.leave_cap) return;
+    if (d.bad_ids && *d.bad_ids) return;
     const uint32_t n_in = d.cell_start[d.cells], n_pairs = d.pair_off[d.n_slots];
     const uint32_t span = max(max(d.n, pairs_max), max(d.cells + 2, d.n_slots + 1));
     const uint32_t first = blockIdx.x * blockDim.x + threadIdx.x;

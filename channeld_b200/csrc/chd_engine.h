@@ -126,6 +126,7 @@ struct chd_engine {
     uint32_t build_blocks = 0;
     bool assigned = false, built = false, have_prev_key = false, entities_dirty = false;
     uint32_t n_sorted = 0;
+    bool sorted_dev_n = false;  // the last build's length was d_n_build (own + halo on the device), not n_sorted
     // handover
     uint32_t *d_ho_entity = nullptr, *d_ho_src = nullptr, *d_ho_dst = nullptr;
     uint32_t ho_cap = 0;
@@ -278,9 +279,14 @@ struct chd_engine {
     // scratch of the tick driver's getters (chd_get_visible*, export counts): separate from h_u32, which the stateless entry
     // points use under the engine mutex from other threads
     uint32_t* h_get = nullptr;
-    // ---- visible-set deltas (chd_delta.cu): everything is allocated by the first chd_reserve_visible_delta
+    // ---- visible-set deltas (chd_delta.cu): everything is allocated by the first chd_reserve_visible_delta(_ids)
     struct Delta {
         bool on = false;
+        // id mode (chd_reserve_visible_delta_ids): entities are named by global id; snap_key and now_gkey are indexed by it
+        bool ids = false;
+        uint32_t id_space = 0;
+        uint32_t* now_gkey = nullptr;  // [id_space] cell of each id in the last build, 0xFFFFFFFF = absent
+        uint32_t* bad_ids = nullptr;   // [1] the last id-mode delta met an id >= id_space or a duplicate (CHD_OVF_DELTA_IDS)
         uint32_t *snap_key = nullptr, *snap_cell_start = nullptr, *snap_sorted = nullptr, *snap_pair_off = nullptr, *snap_pair_cell = nullptr;
         uint32_t* snap_hdr = nullptr;  // [0] entity count, [1] slot count of the snapshot
         uint32_t *arr_rank = nullptr, *dep_rank = nullptr, *arr = nullptr, *dep = nullptr, *arr_start = nullptr, *dep_start = nullptr;
@@ -294,7 +300,9 @@ struct chd_engine {
         cudaEvent_t ev_in = nullptr, ev_done = nullptr;  // two-stream tick: the build is done / the delta is done
         bool done_recorded = false;  // the last tick ran the delta off the engine stream: its end (and CHD_OVF_DELTA) is ev_done
     } dl;
-    bool delta_blocked = false;  // chd_set_slab / chd_set_entity_ids were used: halo indices are not stable, no deltas
+    // chd_set_slab / chd_set_entity_ids / chd_comm_init were used: halo indices are not stable, no index-mode deltas (id mode is
+    // not affected)
+    bool delta_blocked = false;
     // ---- entity-table mode (chd_table.cu): entities spawned / moved / despawned by id; everything is allocated by
     // chd_entity_table_init.  Slots are position indices; n_own is the high-water mark.
     struct Table {

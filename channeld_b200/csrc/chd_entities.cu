@@ -204,7 +204,7 @@ chd_status chd_set_entity_ids(chd_engine* e, const uint32_t* gid, uint32_t n) {
     if (!e || n > e->lim.max_entities) return CHD_ERR_INVALID;
     if (e->tbl.on) return chd_table_refuse(e, "chd_set_entity_ids");
     CU(e, cudaSetDevice(e->device));
-    e->delta_blocked = true;  // global ids: the multi-GPU flow (chd_visible_delta is single-GPU only)
+    e->delta_blocked = true;  // global ids: the multi-GPU flow (index-mode visible deltas are single-GPU only)
     if (!gid) {
         e->have_gid = false;
         return CHD_OK;
@@ -382,6 +382,7 @@ chd_status chd_build_on(chd_engine* e, cudaStream_t s) {
     if (st != CHD_OK) return st;
     if (!counts_recorded) CU(e, cudaEventRecord(e->ev_counts, s));  // (cell counts final = build done)
     e->n_sorted = e->n_own + e->n_halo;
+    e->sorted_dev_n = e->halo_on_device;
     e->built = true;
     e->entities_dirty = false;
     return CHD_OK;

@@ -242,8 +242,9 @@ chd_status chd_table_refuse(chd_engine* e, const char* fn) {
 chd_status chd_entity_table_init(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     chd_engine::Table& t = e->tbl;
-    if (t.on || e->built || e->n_own || e->pf_pos.staged >= 0 || e->delta_blocked || e->comm) {
-        e->fail("chd_entity_table_init needs a fresh engine (no entities set or built, no chd_set_slab / chd_set_entity_ids / chd_comm_init)");
+    if (t.on || e->built || e->n_own || e->pf_pos.staged >= 0 || e->delta_blocked || e->comm || e->dl.ids) {
+        e->fail("chd_entity_table_init needs a fresh engine (no entities set or built, no chd_set_slab / chd_set_entity_ids / chd_comm_init / "
+                "chd_reserve_visible_delta_ids)");
         return CHD_ERR_STATE;
     }
     CU(e, cudaSetDevice(e->device));

@@ -332,6 +332,10 @@ class Engine:
     def reserve_visible_delta(self, cap_entries):
         self._ck(self.L.chd_reserve_visible_delta(self.h, int(cap_entries)))
 
+    def reserve_visible_delta_ids(self, cap_entries, id_space):
+        """Id mode: the deltas name global ids in [0, id_space) (chd_set_entity_ids, halo records); works on slabs too."""
+        self._ck(self.L.chd_reserve_visible_delta_ids(self.h, int(cap_entries), int(id_space)))
+
     def visible_delta(self):
         self._ck(self.L.chd_visible_delta(self.h))
 

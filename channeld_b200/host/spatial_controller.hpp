@@ -265,6 +265,9 @@ class GpuStaticGrid2DSpatialController {
     };
     // once before the first tick with CHD_TICK_VISIBLE_DELTA, and again (larger) after CHD_OVF_DELTA
     void ReserveVisibleDelta(uint64_t cap_entries) { check(chd_reserve_visible_delta(engine_, cap_entries)); }
+    // id mode instead (chosen by whichever reserve comes first): the deltas name global ids in [0, id_space), also on sharded
+    // engines; the host nets a migrated connection's leave list on the old rank against its enter list on the new one
+    void ReserveVisibleDeltaIds(uint64_t cap_entries, uint32_t id_space) { check(chd_reserve_visible_delta_ids(engine_, cap_entries, id_space)); }
     VisibleDelta GetVisibleDelta() {
         VisibleDelta r;
         uint64_t ne = 0, nl = 0;

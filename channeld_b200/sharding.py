@@ -101,3 +101,15 @@ def plan_migrations(table: SlotTable, new_owner):
         call[3] = [(j, table.place(j, call[0])) for j in call[3]]
     arrivals = [[(j, table.place(j, r)) for j in arrivals[r]] for r in range(world)]
     return arrivals, out_lists, [tuple(c) for c in in_calls], vacated
+
+
+def net_migrant_delta(leave_src, enter_dst):
+    """A connection migrated from rank A to rank B (plan_migrations' in_calls), as id-mode visible deltas see it: A's delta
+    reports its old slot leaving everything A's snapshot held, B's reports its new slot entering everything it sees now.  The
+    connection's own delta is their net:
+        enter = enter_B \\ leave_A        leave = leave_A \\ enter_B
+    exact when leave_src is A's delta of the tick that ran chd_migrate_out and enter_dst is B's first successful delta for the
+    connection.  Global ids in, (enter, leave) out as u32 arrays in the order of the lists they come from."""
+    leave_src = np.asarray(leave_src, np.uint32)
+    enter_dst = np.asarray(enter_dst, np.uint32)
+    return enter_dst[~np.isin(enter_dst, leave_src)], leave_src[~np.isin(leave_src, enter_dst)]

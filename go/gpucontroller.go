@@ -416,6 +416,16 @@ func (ctl *GpuStaticGrid2DSpatialController) ReserveVisibleDelta(capEntries uint
 	return nil
 }
 
+// ReserveVisibleDeltaIds picks id mode instead: the deltas name global ids in [0, idSpace) (SetEntityIds, the halo records),
+// which also works on sharded engines.  A connection migrated from rank A to rank B is netted by the host: enter = enter_B \
+// leave_A, leave = leave_A \ enter_B.
+func (ctl *GpuStaticGrid2DSpatialController) ReserveVisibleDeltaIds(capEntries uint64, idSpace uint32) error {
+	if st := C.chd_reserve_visible_delta_ids(ctl.engine, C.uint64_t(capEntries), C.uint32_t(idSpace)); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
 func (ctl *GpuStaticGrid2DSpatialController) VisibleDelta() (enterOff []uint64, enter []uint32, leaveOff []uint64, leave []uint32, err error) {
 	var ne, nl C.uint64_t
 	var slots C.uint32_t

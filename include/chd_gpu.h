@@ -286,7 +286,9 @@ typedef struct chd_tick_summary {
  *   CHD_OVF_BORDER  multi-GPU border / halo capacity exceeded: this tick's halo is incomplete */
 enum { CHD_OVF_PAIRS = 1, CHD_OVF_WINDOW = 2, CHD_OVF_VISIBLE = 4, CHD_OVF_DUE = 8, CHD_OVF_BORDER = 16,
        CHD_OVF_RING = 32, /* a device-owned ring slab was full of live entries: its oldest entry was dropped */
-       CHD_OVF_DELTA = 64 /* the visible-set delta did not fit chd_reserve_visible_delta's capacity: see chd_visible_delta */ };
+       CHD_OVF_DELTA = 64, /* the visible-set delta did not fit chd_reserve_visible_delta's capacity: see chd_visible_delta */
+       CHD_OVF_DELTA_IDS = 128 /* id-mode delta: an id >= id_space, or one id twice among one state's in-world entities; handled
+                                  like CHD_OVF_DELTA (no lists, snapshot kept): see chd_reserve_visible_delta_ids */ };
 /* bit 31: a device-side wait timed out (results invalid, please report).  A macro, not an enumerator: ISO C enumerators
  * must fit an int. */
 #define CHD_OVF_INTERNAL 0x80000000u
@@ -351,7 +353,8 @@ chd_status chd_get_handover(chd_engine* e, uint32_t* entity, uint32_t* src_chann
  * into the next delta.  So a removed slot (chd_remove_subscribers, chd_set_subscribers) leaves everything it saw, an added slot
  * enters what its first query makes visible, and a failed query (CHD_Q_ERR_*) changes nothing for its slot.
  * "now" is the state of the last chd_build and the current subscriptions; CHD_ERR_STATE if chd_assign_cells ran after that build.
- * Entity identity is the entity index.  An index at or above the entity count of a state, or outside the world in it (NaN-parked
+ * Entity identity depends on the mode, which the first reserve call picks (index mode: chd_reserve_visible_delta, id mode:
+ * chd_reserve_visible_delta_ids, below).  In index mode it is the entity index.  An index at or above the entity count of a state, or outside the world in it (NaN-parked
  * slots included), is absent from that state: appended spawns, a shrunk array and parked slots come out as enter / leave.  An
  * index reused for a different entity between two deltas is invisible to the engine: the host despawns / spawns it itself.
  * Order: entered(s) by (current cell asc, entity asc), left(s) by (snapshot cell asc, entity asc): the order of the visible
@@ -368,9 +371,28 @@ chd_status chd_get_handover(chd_engine* e, uint32_t* entity, uint32_t* src_chann
  *                              *n_slots = max(slots now, slots at any earlier delta): slots dropped by chd_set_subscribers still
  *                              report what they left.  Synchronous; any pointer may be NULL; CHD_ERR_CAPACITY if a requested list
  *                              does not fit cap or the last delta overflowed.
- * Single-GPU only: CHD_ERR_STATE on an engine that has used chd_set_slab, chd_set_entity_ids or chd_comm_init (halo entity indices
- * are not stable from tick to tick there). */
+ * Index mode is single-GPU only: CHD_ERR_STATE on an engine that has used chd_set_slab, chd_set_entity_ids or chd_comm_init (halo
+ * entity indices are not stable from tick to tick there).
+ *
+ * Id mode: entity identity is the GLOBAL id (chd_set_entity_ids for own entities, the halo records of chd_import_halo /
+ * chd_tick_sharded for the rest), not the entity index.  Works on single engines with ids, on slabs driven through the building
+ * blocks and in chd_tick_sharded, and survives halo reordering, re-homing (own on one rank, halo on another, then own there) and a
+ * host that permutes its entity array between deltas.  The lists name global ids; inside a cell they follow the cell CSR (own
+ * entities in array order, then halo entities in import order), so, as for the multi-GPU visible lists, read each cell's part as a set.
+ *   chd_reserve_visible_delta_ids  as chd_reserve_visible_delta, and picks id mode over the ids [0, id_space) (the snapshot takes
+ *                                  8 bytes per id of id_space).  CHD_ERR_STATE after index mode was picked or in entity-table mode;
+ *                                  later calls of either reserve function on an id-mode engine only grow the lists (a different
+ *                                  id_space: CHD_ERR_INVALID).
+ * An id-mode delta needs ids for the own entities (CHD_ERR_STATE otherwise) and, standalone, a chd_build after the last change of
+ * positions, ids or halo.  If an in-world entity of the current state has an id >= id_space, or two in-world entities share an id
+ * (the host routed one entity to two places), CHD_OVF_DELTA_IDS is raised: no lists are written and the snapshot is not advanced,
+ * so the next clean delta covers everything (chd_get_visible_delta then returns CHD_ERR_INVALID for the lists).  Entities outside
+ * the world are absent and never count as duplicates.
+ * Subscriber migration (chd_migrate_out / chd_migrate_in): the source rank's next delta reports the emigrant leaving everything its
+ * snapshot held, the destination's reports the immigrant entering everything it sees; the host nets the two (enter = enter_B \
+ * leave_A, leave = leave_A \ enter_B), exact when A's leave list is paired with B's first successful delta for that connection. */
 chd_status chd_reserve_visible_delta(chd_engine* e, uint64_t cap_entries);
+chd_status chd_reserve_visible_delta_ids(chd_engine* e, uint64_t cap_entries, uint32_t id_space);
 chd_status chd_visible_delta(chd_engine* e);
 chd_status chd_get_visible_delta(chd_engine* e, uint64_t* enter_off, uint32_t* enter_entity, uint64_t* leave_off, uint32_t* leave_entity,
                                  uint64_t cap, uint64_t* n_entered, uint64_t* n_left, uint32_t* n_slots);
