@@ -138,7 +138,7 @@ SYMBOLS = [
     "chd_add_subscribers", "chd_remove_subscribers", "chd_fetch_results_async", "chd_fetch_wait", "chd_rings_init", "chd_rings_append", "chd_get_rings", "chd_set_channel_start_times", "chd_set_payload_bytes", "chd_assemble_payloads", "chd_frame_packets", "chd_comm_unique_id", "chd_comm_init", "chd_comm_info", "chd_comm_destroy", "chd_tick_sharded", "chd_collective_count", "chd_comm_exchange_mode", "chd_comm_use_collective", "chd_migrate_out", "chd_migrate_in", "chd_get_rehome",
     "chd_reserve_visible_delta", "chd_reserve_visible_delta_ids", "chd_visible_delta", "chd_get_visible_delta",
     "chd_entity_table_init", "chd_spawn_entities", "chd_spawn_entities_f32", "chd_despawn_entities", "chd_move_entities", "chd_move_entities_f32",
-    "chd_get_entity_stats",
+    "chd_get_entity_stats", "chd_handoff_entities",
 ]
 STAGE_BUILD, STAGE_INTEREST, STAGE_EMIT, STAGE_EMIT_KERNEL, STAGE_FANOUT, STAGE_TICK, STAGE_EXPORT, STAGE_EXCHANGE, STAGE_IMPORT, STAGE_READBACK, STAGE_VISIBLE_DELTA, STAGE_ENTITY_EVENTS = range(12)
 
@@ -334,6 +334,8 @@ def lib():
         f.argtypes = [vp, vp, vp, vp, C.c_uint32]
     L.chd_get_entity_stats.restype = C.c_int
     L.chd_get_entity_stats.argtypes = [vp, C.POINTER(EntityStats)]
+    L.chd_handoff_entities.restype = C.c_int
+    L.chd_handoff_entities.argtypes = [vp, vp, vp, vp, vp, C.c_uint32, u32p]
     _lib = L
     return L
 

@@ -34,6 +34,8 @@ static DeltaDev delta_view(chd_engine* e) {
         d.key = D.now_gkey;
         d.n = D.id_space;
         d.bad_ids = D.bad_ids;
+        // entity-table mode: d_sorted_ent holds build positions (slots, then halo records); the id-valued copy is the CSR by id
+        if (e->tbl.on) d.sorted = e->tbl.d_sorted_id;
     }
     return d;
 }
@@ -50,7 +52,7 @@ chd_status chd_delta_check(chd_engine* e, bool will_build) {
         e->fail("visible delta before chd_reserve_visible_delta");
         return CHD_ERR_STATE;
     }
-    if (e->dl.ids && !e->have_gid) {
+    if (e->dl.ids && !e->have_gid && !e->tbl.on) {
         e->fail("id-mode visible delta on an engine without global ids (chd_set_entity_ids)");
         return CHD_ERR_STATE;
     }
@@ -87,7 +89,9 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
     // id mode: the scatter bakes in the build's length (host count or d_n_build) and the key / id buffers it reads
     const uint32_t* n_ptr = e->sorted_dev_n ? e->d_n_build : nullptr;
     const uint32_t n_scatter = e->sorted_dev_n ? e->lim.max_entities : e->n_sorted;
-    if (D.ids) key = stage_key(key, 0x696473ull, D.id_space, n_scatter, n_ptr, e->d_key, e->d_gid, e->d_n_build);
+    // (entity-table mode: the slots below the high-water mark are named by the table's slot -> id array, read in place)
+    const uint32_t own = e->tbl.on ? e->n_own : 0;
+    if (D.ids) key = stage_key(key, 0x696473ull, D.id_space, n_scatter, n_ptr, e->d_key, e->d_gid, e->d_n_build, own, d.sorted);
     const unsigned grid = (unsigned)e->sm_count * 8;
     const unsigned slot_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(blocks_for((uint64_t)D.n_out * 32, DELTA_THREADS), (uint64_t)e->sm_count * 32));
     return run_stage(e, s, D.g, key, [&]() -> chd_status {
@@ -100,8 +104,8 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
             // scatter reads this tick's imported halo.
             CU(e, cudaMemsetAsync(D.now_gkey, 0xFF, 4ull * D.id_space, s));
             CU(e, cudaMemsetAsync(D.bad_ids, 0, 4, s));
-            delta_id_scatter_kernel<<<grid, DELTA_THREADS, 0, s>>>(e->d_gid, e->d_key, n_scatter, n_ptr, C, D.now_gkey, D.id_space, D.bad_ids,
-                                                                   d.overflow);
+            delta_id_scatter_kernel<<<grid, DELTA_THREADS, 0, s>>>(e->d_gid, e->tbl.d_id_of_slot, own, e->d_key, n_scatter, n_ptr, C, D.now_gkey,
+                                                                   D.id_space, D.bad_ids, d.overflow);
             KCHECK(e);
         }
         SCAN(e, exclusive_scan_fn<DeltaArrivalFlag, uint32_t>(DeltaArrivalFlag{d.sorted, d.key, d.snap_key, d.snap_hdr, d.n, C}, D.arr_rank, N, D.site_arr, s,
@@ -116,7 +120,7 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
         SCAN(e, exclusive_scan_1p<uint32_t, uint64_t>(D.cnt_leave, D.leave_off, D.n_out, D.site_leave, s));
         delta_slots_kernel<true><<<slot_grid, DELTA_THREADS, 0, s>>>(d);
         KCHECK(e);
-        if (e->tbl.on) {  // entity-table mode: the lists name ids (here: a later spawn must not change lists already computed)
+        if (e->tbl.on && !D.ids) {  // entity-table index mode: the lists name ids (here: a later spawn must not change lists already computed)
             const chd_status ts = chd_table_delta_ids(e, s);
             if (ts != CHD_OK) return ts;
         }
@@ -176,7 +180,8 @@ chd_status chd_reserve_visible_delta(chd_engine* e, uint64_t cap_entries) {
 
 chd_status chd_reserve_visible_delta_ids(chd_engine* e, uint64_t cap_entries, uint32_t id_space) {
     if (!e || id_space == 0) return CHD_ERR_INVALID;
-    if (e->tbl.on) return chd_table_refuse(e, "chd_reserve_visible_delta_ids");
+    // entity-table mode: id mode is the delta mode of slab engines; on one GPU the index-mode deltas already name ids
+    if (e->tbl.on && !e->slab) return chd_table_refuse(e, "chd_reserve_visible_delta_ids on an engine that is not a slab");
     if (e->dl.on && !e->dl.ids) {
         e->fail("chd_reserve_visible_delta_ids: this engine's visible deltas are in index mode (chd_reserve_visible_delta came first)");
         return CHD_ERR_STATE;

@@ -31,6 +31,12 @@ struct GridDev {
     int32_t default_delay_ms;
 };
 
+// The rank owning grid column `col` when `world` ranks split the columns into X-slabs (chd_comm_init): the largest rank r with
+// floor(r * cols / world) <= col.
+__device__ __forceinline__ uint32_t slab_owner(uint32_t col, uint32_t cols, uint32_t world) {
+    return min((uint32_t)((((uint64_t)col + 1) * world - 1) / cols), world - 1);
+}
+
 __device__ __forceinline__ double f64sub(double a, double b) { return __dsub_rn(a, b); }
 __device__ __forceinline__ double f64add(double a, double b) { return __dadd_rn(a, b); }
 __device__ __forceinline__ double f64mul(double a, double b) { return __dmul_rn(a, b); }

@@ -303,6 +303,9 @@ struct chd_engine {
     // chd_set_slab / chd_set_entity_ids / chd_comm_init were used: halo indices are not stable, no index-mode deltas (id mode is
     // not affected)
     bool delta_blocked = false;
+    // chd_set_slab (directly or through chd_comm_init) made this engine an X-slab: the multi-GPU calls work in entity-table mode
+    // only on such an engine, made a slab before chd_entity_table_init
+    bool slab = false;
     // ---- entity-table mode (chd_table.cu): entities spawned / moved / despawned by id; everything is allocated by
     // chd_entity_table_init.  Slots are position indices; n_own is the high-water mark.
     struct Table {
@@ -481,6 +484,8 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s);
 // entity-table mode (chd_table.cu): the call named `fn` is not available in it (CHD_ERR_STATE); the pass after every table-mode build
 // (sorted ids, handover list in ids); the delta's translation to ids, inside its stage; a decoded summary's last successful delta
 chd_status chd_table_refuse(chd_engine* e, const char* fn);
+// CHD_OK unless the engine is in entity-table mode without having been made a slab first (then CHD_ERR_STATE for the call `fn`)
+chd_status chd_table_slab_check(chd_engine* e, const char* fn);
 chd_status chd_table_after_build(chd_engine* e, cudaStream_t s);
 chd_status chd_table_delta_ids(chd_engine* e, cudaStream_t s);
 void chd_table_observe(chd_engine* e, uint32_t delta_build);

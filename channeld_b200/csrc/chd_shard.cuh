@@ -192,8 +192,7 @@ __global__ void __launch_bounds__(256) rehome_kernel(GridDev g, const uint32_t* 
     __syncthreads();
     if (away && s_base + my < cap) {
         out_gid[s_base + my] = gid ? gid[i] : i;
-        // owner of a column = the largest rank r with floor(r * cols / world) <= col
-        out_rank[s_base + my] = min((uint32_t)((((uint64_t)col + 1) * world - 1) / g.cols), world - 1);
+        out_rank[s_base + my] = slab_owner(col, g.cols, world);
     }
 }
 

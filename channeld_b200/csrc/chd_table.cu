@@ -15,11 +15,13 @@ chd_status need_table(chd_engine* e, const char* fn) {
     return CHD_ERR_STATE;
 }
 
-// The positions changed: nothing is assigned or built for them yet.  Unlike chd_entities_replaced this keeps handover detection on
-// when the high-water mark grows: the new slots are flagged and left out of the handover list.
+// The positions changed: nothing is assigned or built for them yet, and a halo imported before may sit where the high-water mark
+// now reaches.  Unlike chd_entities_replaced this keeps handover detection on when the high-water mark grows: the new slots are
+// flagged and left out of the handover list.
 void touched(chd_engine* e) {
     e->n_own = e->tbl.hw;
     e->n_halo = 0;
+    e->halo_on_device = false;
     e->assigned = false;
     e->entities_dirty = true;
 }
@@ -239,12 +241,19 @@ chd_status chd_table_refuse(chd_engine* e, const char* fn) {
     return CHD_ERR_STATE;
 }
 
+chd_status chd_table_slab_check(chd_engine* e, const char* fn) {
+    if (!e->tbl.on || e->slab) return CHD_OK;
+    e->fail("%s in entity-table mode needs an engine made a slab (chd_set_slab / chd_comm_init) before chd_entity_table_init", fn);
+    return CHD_ERR_STATE;
+}
+
 chd_status chd_entity_table_init(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     chd_engine::Table& t = e->tbl;
-    if (t.on || e->built || e->n_own || e->pf_pos.staged >= 0 || e->delta_blocked || e->comm || e->dl.ids) {
-        e->fail("chd_entity_table_init needs a fresh engine (no entities set or built, no chd_set_slab / chd_set_entity_ids / chd_comm_init / "
-                "chd_reserve_visible_delta_ids)");
+    // a slab (chd_set_slab / chd_comm_init) may come first: that is how a table engine becomes a rank of a sharded world
+    if (t.on || e->built || e->assigned || e->n_own || e->pf_pos.staged >= 0 || e->have_gid || (e->delta_blocked && !e->slab) || e->dl.ids) {
+        e->fail("chd_entity_table_init needs a fresh engine (no entities set, assigned or built, no chd_set_entity_ids / chd_export_border / "
+                "chd_reserve_visible_delta_ids; chd_set_slab / chd_comm_init may come first)");
         return CHD_ERR_STATE;
     }
     CU(e, cudaSetDevice(e->device));
@@ -316,9 +325,10 @@ chd_status chd_despawn_entities(chd_engine* e, const uint32_t* id_in, uint32_t n
         t.slot_of.erase(it);
         aid.push_back(id);
         aslot.push_back(slot);
-        // With visible deltas on, the slot waits until a delta that measured a build without it has succeeded: reused earlier, the
-        // snapshot would still hold the old instance there and the delta could not tell the two apart.
-        if (e->dl.on)
+        // With index-mode visible deltas on, the slot waits until a delta that measured a build without it has succeeded: reused
+        // earlier, the snapshot would still hold the old instance there and the delta could not tell the two apart.  Id-mode
+        // deltas name ids, not slots: no quarantine.
+        if (e->dl.on && !e->dl.ids)
             t.quarantine.push_back(chd_engine::Table::Held{slot, t.builds + 1});
         else
             t.free_fifo.push_back(slot);
@@ -362,17 +372,73 @@ chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out) {
     return CHD_OK;
 }
 
+chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank, double* x, double* z, uint32_t cap, uint32_t* count) {
+    if (!e || !count || (cap && (!id || !dst_rank || !x || !z))) return CHD_ERR_INVALID;
+    chd_status st = need_table(e, "chd_handoff_entities");
+    if (st != CHD_OK) return st;
+    if (!e->assigned) {
+        // the keys must describe the current positions: a spawn, move, despawn or hand-off since the last assignment changed them
+        e->fail("chd_handoff_entities needs a cell assignment after the last spawn / move / despawn / hand-off (chd_export_border, "
+                "chd_assign_cells, chd_build or a tick)");
+        return CHD_ERR_STATE;
+    }
+    CU(e, cudaSetDevice(e->device));
+    chd_engine::Table& t = e->tbl;
+    cudaStream_t s = e->stream;
+    const uint64_t N = e->lim.max_entities;
+    const uint32_t world = e->comm ? (uint32_t)e->comm_world : 1u;
+    // the list goes to the event staging (free between calls: every user is on this stream) and the radix sort's temporaries
+    uint32_t *d_id = t.d_ev, *d_slot = t.d_ev + N, *d_dst = e->d_tmp_val;
+    double *d_hx = t.d_ev_pos, *d_hz = t.d_ev_pos + N;
+    st = chd_epoch_tick(e, s, EP_BORDER);
+    if (st != CHD_OK) return st;
+    bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_BORDER);
+    KCHECK(e);
+    SCAN(e, compact_1p(HandoffFlag{e->g, e->d_key},
+                       HandoffSink{e->g, world, e->d_key, t.d_id_of_slot, e->d_x, e->d_z, d_id, d_slot, d_dst, d_hx, d_hz, e->d_boff}, e->n_own,
+                       e->site_border, s));
+    st = chd_read_u32(e, e->d_boff, count);
+    if (st != CHD_OK) return st;
+    const uint32_t m = *count;
+    if (m > cap) {  // transactional: nothing removed, a repeat call with a larger buffer lists the same entities
+        e->fail("chd_handoff_entities: %u entities to hand off > cap %u", m, cap);
+        return CHD_ERR_CAPACITY;
+    }
+    if (!m) return CHD_OK;
+    CU(e, cudaMemcpyAsync(id, d_id, 4ull * m, cudaMemcpyDefault, s));
+    CU(e, cudaMemcpyAsync(dst_rank, d_dst, 4ull * m, cudaMemcpyDefault, s));
+    CU(e, cudaMemcpyAsync(x, d_hx, 8ull * m, cudaMemcpyDefault, s));
+    CU(e, cudaMemcpyAsync(z, d_hz, 8ull * m, cudaMemcpyDefault, s));
+    std::vector<uint32_t> hid(m), hslot(m);
+    CU(e, cudaMemcpyAsync(hid.data(), d_id, 4ull * m, cudaMemcpyDeviceToHost, s));
+    CU(e, cudaMemcpyAsync(hslot.data(), d_slot, 4ull * m, cudaMemcpyDeviceToHost, s));
+    CU(e, cudaStreamSynchronize(s));
+    // The ids live on at their new owner: the slots are free at once (no quarantine), in slot order.  The apply pass is a
+    // despawn's (tombstone, slot -> id cleared, slot parked and flagged), so neither rank reports the hand-off as a handover.
+    for (uint32_t j = 0; j < m; j++) {
+        t.slot_of.erase(hid[j]);
+        t.free_fifo.push_back(hslot[j]);
+    }
+    StageTimer timer(e, s, CHD_STAGE_ENTITY_EVENTS);
+    tbl_despawn_kernel<<<grid_for(e, m), TBL_THREADS, 0, s>>>(t.d_table, t.bits, d_id, d_slot, m, t.d_id_of_slot, e->d_x, e->d_z, t.d_flag);
+    KCHECK(e);
+    touched(e);
+    return CHD_OK;
+}
+
 // After every table-mode build, on the build's stream: the id-valued copy of the sorted entity array and, after a fresh cell
 // assignment, the handover list in ids without the slots spawned or despawned since the previous one (then the flags clear).
 chd_status chd_table_after_build(chd_engine* e, cudaStream_t s) {
     chd_engine::Table& t = e->tbl;
     if (!t.on) return CHD_OK;
-    const uint32_t n = e->n_own + e->n_halo;
+    // on slabs the build's length (own slots + halo records) lives on the device
+    const uint32_t* n_ptr = e->halo_on_device ? e->d_n_build : nullptr;
+    const uint32_t n = e->halo_on_device ? e->lim.max_entities : e->n_own + e->n_halo, own = e->n_own;
     const bool raw = t.ho_raw;
-    const uint64_t key = stage_key(0x7461626c65ull, n, raw, e->d_sorted_ent, t.d_sorted_id, t.d_id_of_slot, e->ho_cap);
+    const uint64_t key = stage_key(0x7461626c65ull, n, n_ptr, own, e->d_gid, raw, e->d_sorted_ent, t.d_sorted_id, t.d_id_of_slot, e->ho_cap);
     const unsigned grid = (unsigned)e->sm_count * 4;
     chd_status st = run_stage(e, s, t.g_post, key, [&]() -> chd_status {
-        tbl_gather_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(e->d_sorted_ent, t.d_id_of_slot, n, t.d_sorted_id, t.d_build_seq);
+        tbl_gather_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(e->d_sorted_ent, t.d_id_of_slot, e->d_gid, own, n, n_ptr, t.d_sorted_id, t.d_build_seq);
         KCHECK(e);
         if (!raw) return CHD_OK;
         const HandoverOut ho{e->d_ho_entity, e->d_ho_src, e->d_ho_dst, &e->d_ctr->n_handover, e->ho_cap};
@@ -381,7 +447,7 @@ chd_status chd_table_after_build(chd_engine* e, cudaStream_t s) {
         CU(e, cudaMemsetAsync(&e->d_ctr->n_handover, 0, 4, s));
         tbl_handover_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(ho, t.d_ho_tmp, t.d_build_seq + 1, t.d_flag, t.d_id_of_slot);
         KCHECK(e);
-        if (n) CU(e, cudaMemsetAsync(t.d_flag, 0, n, s));
+        if (own) CU(e, cudaMemsetAsync(t.d_flag, 0, own, s));
         return CHD_OK;
     });
     if (st != CHD_OK) return st;

@@ -105,12 +105,52 @@ __global__ void __launch_bounds__(TBL_THREADS) tbl_move_apply_kernel(const uint3
     tbl_block_count(stats + 2, superseded);
 }
 
-// After a build: sorted_id[i] = id of sorted slot i (what the emit kernels and the read-back see); advances the device build number.
-__global__ void __launch_bounds__(TBL_THREADS) tbl_gather_ids_kernel(const uint32_t* __restrict__ sorted_slot, const uint32_t* __restrict__ id_of_slot, uint32_t n,
+// The id of build position p: a slot's table id below `own` (the high-water mark), a halo record's id (gid, written by the
+// import) from there on.  Halo ids never enter id_of_slot: a later spawn into such a position must not inherit one.
+__device__ __forceinline__ uint32_t tbl_id_at(const uint32_t* __restrict__ id_of_slot, const uint32_t* __restrict__ gid, uint32_t own, uint32_t p) {
+    return p < own ? id_of_slot[p] : gid[p];
+}
+
+// After a build: sorted_id[i] = id of sorted position i (what the emit kernels and the read-back see); advances the device build
+// number.  n_ptr: the build's length lives on the device (own + halo), n is then the capacity.
+__global__ void __launch_bounds__(TBL_THREADS) tbl_gather_ids_kernel(const uint32_t* __restrict__ sorted_slot, const uint32_t* __restrict__ id_of_slot,
+                                                                     const uint32_t* __restrict__ gid, uint32_t own, uint32_t n, const uint32_t* __restrict__ n_ptr,
                                                                      uint32_t* __restrict__ sorted_id, uint32_t* build_seq) {
     if (blockIdx.x == 0 && threadIdx.x == 0) *build_seq += 1;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) sorted_id[i] = id_of_slot[sorted_slot[i]];
+    const uint32_t m = n_ptr ? min(*n_ptr, n) : n;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) sorted_id[i] = tbl_id_at(id_of_slot, gid, own, sorted_slot[i]);
 }
+
+// chd_handoff_entities, one compaction (compact_1p): the own in-world slots whose column lies outside this rank's slab, with their
+// id, the rank owning that column, their slot and their position.
+struct HandoffFlag {
+    GridDev g;
+    const uint32_t* __restrict__ key;
+    __device__ __forceinline__ bool operator()(uint64_t i) const {
+        const uint32_t k = key[i];
+        if (k >= g.cells) return false;  // (free and despawned slots are parked outside the world)
+        const uint32_t col = k % g.cols;
+        return col < g.col_lo || col >= g.col_hi;
+    }
+};
+struct HandoffSink {
+    GridDev g;
+    uint32_t world;
+    const uint32_t* __restrict__ key;
+    const uint32_t* __restrict__ id_of_slot;
+    const double *__restrict__ px, *__restrict__ pz;
+    uint32_t *__restrict__ id, *__restrict__ slot, *__restrict__ dst;
+    double *__restrict__ x, *__restrict__ z;
+    uint32_t* __restrict__ count;
+    __device__ __forceinline__ void operator()(uint64_t i, uint32_t k) const {
+        id[k] = id_of_slot[i];
+        slot[k] = (uint32_t)i;
+        dst[k] = slab_owner(key[i] % g.cols, g.cols, world);
+        x[k] = px[i];
+        z[k] = pz[i];
+    }
+    __device__ __forceinline__ void total(uint32_t c) const { *count = c; }
+};
 
 // Handover list, pass 1: move the slot-valued list aside (tmp = entity | src | dst, each `cap` long) with its length.
 __global__ void __launch_bounds__(TBL_THREADS) tbl_handover_stash_kernel(HandoverOut ho, uint32_t* __restrict__ tmp, uint32_t* __restrict__ tmp_n) {

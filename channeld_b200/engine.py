@@ -455,6 +455,20 @@ class Engine:
         k = min(n.value, cap)
         return gid[:k].copy(), dst[:k].copy(), n.value
 
+    def handoff_entities(self, cap=1 << 16):
+        """Entity-table mode on slabs: lists the own entities whose column another rank owns and removes them from this table
+        -> (id u32, dst_rank u32, x f64, z f64); the receiving rank adopts them with spawn_entities(id, x, z)."""
+        n = C.c_uint32()
+        while True:
+            ids, dst, x, z = np.zeros(cap, np.uint32), np.zeros(cap, np.uint32), np.zeros(cap), np.zeros(cap)
+            st = self.L.chd_handoff_entities(self.h, ptr(ids), ptr(dst), ptr(x), ptr(z), int(cap), C.byref(n))
+            if st != capi.ERR_CAPACITY or n.value <= cap:
+                break
+            cap = n.value  # nothing was removed: the same list again, with room for it
+        self._ck(st)
+        k = n.value
+        return ids[:k].copy(), dst[:k].copy(), x[:k].copy(), z[:k].copy()
+
     def comm_info(self):
         r, w, ver = C.c_int(), C.c_int(), C.c_int()
         lo, hi, halo = C.c_uint32(), C.c_uint32(), C.c_uint32()

@@ -219,6 +219,27 @@ class GpuStaticGrid2DSpatialController {
         for (uint32_t i = 0; i < n && i < cap; i++) r.emplace_back(id[i], dst[i]);
         return r;
     }
+    // Entity-table mode on slabs, after the tick: the own entities whose column another rank owns, removed from this rank's table
+    // with their exact positions; the destination adopts each one with SpawnObjects({id}, {x}, {z}).
+    struct Handoff {
+        std::vector<uint32_t> net_id, dst_rank;
+        std::vector<double> x, z;
+    };
+    Handoff HandoffEntities(uint32_t cap = 1024) {
+        for (;;) {
+            Handoff h{std::vector<uint32_t>(cap ? cap : 1), std::vector<uint32_t>(cap ? cap : 1), std::vector<double>(cap ? cap : 1),
+                      std::vector<double>(cap ? cap : 1)};
+            uint32_t n = 0;
+            const chd_status st = chd_handoff_entities(engine_, h.net_id.data(), h.dst_rank.data(), h.x.data(), h.z.data(), cap, &n);
+            if (st == CHD_ERR_CAPACITY && n > cap) {  // nothing was removed: ask again with room for the whole list
+                cap = n;
+                continue;
+            }
+            check(st);
+            h.net_id.resize(n), h.dst_rank.resize(n), h.x.resize(n), h.z.resize(n);
+            return h;
+        }
+    }
 
     // Recipients of BroadcastType_ADJACENT_CHANNELS messages (message.go:188-239), batched: CSR of subscriber slots.
     struct BroadcastSets {

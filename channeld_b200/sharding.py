@@ -113,3 +113,63 @@ def net_migrant_delta(leave_src, enter_dst):
     leave_src = np.asarray(leave_src, np.uint32)
     enter_dst = np.asarray(enter_dst, np.uint32)
     return enter_dst[~np.isin(enter_dst, leave_src)], leave_src[~np.isin(leave_src, enter_dst)]
+
+
+class EntityRouter:
+    """Host router of a sharded entity-table host (chd_entity_table_init on X-slabs): every rank's table holds the entities it
+    owns, and the router keeps id -> owning rank.  A spawn goes to the owner of its position's column (a spawn outside the world to
+    the owner of the clamped column); moves and despawns go to the id's current owner; after each tick the ranks' hand-off lists
+    (chd_handoff_entities) become adoption batches (spawns) for their destinations and the map follows.  Ids the router does not
+    know are routed nowhere.  Every method returns one batch per rank."""
+
+    def __init__(self, world: int, cols: int, offx: float, w: float):
+        self.world, self.cols, self.offx, self.w = int(world), int(cols), float(offx), float(w)
+        self.owner = {}  # id -> rank
+
+    def owner_of_x(self, x):
+        """Owning rank of the (clamped) column of each x."""
+        with np.errstate(invalid="ignore"):
+            c = np.floor((np.asarray(x, np.float64) - self.offx) / self.w)
+        c = np.where(np.isnan(c), 0, np.clip(c, 0, self.cols - 1)).astype(np.int64)
+        return owner_of_column(c, self.cols, self.world)
+
+    def _split(self, rank, *arrays):
+        return [tuple(np.asarray(a)[rank == r] for a in arrays) for r in range(self.world)]
+
+    def _rank_of_ids(self, ids):
+        return np.array([self.owner.get(int(i), -1) for i in ids], np.int64)
+
+    def spawn(self, ids, x, z):
+        """-> per rank (ids u32, x, z).  An id that is already live goes to its owner (which reports it as a duplicate)."""
+        ids = np.asarray(ids, np.uint32)
+        rank = self.owner_of_x(x)
+        known = self._rank_of_ids(ids)
+        rank = np.where(known >= 0, known, rank)
+        for i, r in zip(ids.tolist(), rank.tolist()):
+            self.owner.setdefault(i, r)
+        return self._split(rank, ids, np.asarray(x, np.float64), np.asarray(z, np.float64))
+
+    def move(self, ids, x, z):
+        """-> per rank (ids u32, x, z) for chd_move_entities."""
+        ids = np.asarray(ids, np.uint32)
+        return self._split(self._rank_of_ids(ids), ids, np.asarray(x), np.asarray(z))
+
+    def despawn(self, ids):
+        """-> per rank ids u32; the ids leave the map."""
+        ids = np.asarray(ids, np.uint32)
+        rank = self._rank_of_ids(ids)
+        for i in ids.tolist():
+            self.owner.pop(i, None)
+        return [b[0] for b in self._split(rank, ids)]
+
+    def handoff(self, lists):
+        """lists[r] = rank r's chd_handoff_entities result (id, dst_rank, x, z) -> per rank (ids u32, x, z) to adopt with
+        chd_spawn_entities; every listed id is owned by its destination from now on."""
+        out = [([], [], []) for _ in range(self.world)]
+        for ids, dst, x, z in lists:
+            for i, d, xi, zi in zip(np.asarray(ids).tolist(), np.asarray(dst).tolist(), np.asarray(x), np.asarray(z)):
+                self.owner[i] = d
+                out[d][0].append(i)
+                out[d][1].append(xi)
+                out[d][2].append(zi)
+        return [(np.asarray(a, np.uint32), np.asarray(b, np.float64), np.asarray(c, np.float64)) for a, b, c in out]

@@ -643,6 +643,28 @@ func (ctl *GpuStaticGrid2DSpatialController) Rehome(capEntities int) (gid, dstRa
 	return gid[:k], dstRank[:k], nil
 }
 
+// HandoffEntities (entity-table mode on slabs, after the tick): the own entities whose column another rank owns, removed from
+// this rank's table with their exact positions; the destination rank adopts each one with SpawnObjects.  A list longer than
+// capEntities is asked for again with room for it (nothing is removed by the refused call).
+func (ctl *GpuStaticGrid2DSpatialController) HandoffEntities(capEntities int) (netIds, dstRank []uint32, x, z []float64, err error) {
+	for {
+		netIds, dstRank = make([]uint32, capEntities+1), make([]uint32, capEntities+1)
+		x, z = make([]float64, capEntities+1), make([]float64, capEntities+1)
+		var n C.uint32_t
+		st := C.chd_handoff_entities(ctl.engine, (*C.uint32_t)(unsafe.Pointer(&netIds[0])), (*C.uint32_t)(unsafe.Pointer(&dstRank[0])),
+			(*C.double)(unsafe.Pointer(&x[0])), (*C.double)(unsafe.Pointer(&z[0])), C.uint32_t(capEntities), &n)
+		if st == C.CHD_ERR_CAPACITY && int(n) > capEntities {
+			capEntities = int(n)
+			continue
+		}
+		if st != C.CHD_OK {
+			return nil, nil, nil, nil, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+		}
+		k := int(n)
+		return netIds[:k], dstRank[:k], x[:k], z[:k], nil
+	}
+}
+
 // RingsInit / RingsAppend: ChannelData.OnUpdate's buffer on the GPU (data.go:149-173); updOff is the CSR by cell of this tick's
 // updates (arrival order per cell), arrival / sender in C memory when the call is used on the tick path.
 func (ctl *GpuStaticGrid2DSpatialController) RingsInit(capacityPerCell uint32) error {

@@ -380,11 +380,14 @@ chd_status chd_get_handover(chd_engine* e, uint32_t* entity, uint32_t* src_chann
  * host that permutes its entity array between deltas.  The lists name global ids; inside a cell they follow the cell CSR (own
  * entities in array order, then halo entities in import order), so, as for the multi-GPU visible lists, read each cell's part as a set.
  *   chd_reserve_visible_delta_ids  as chd_reserve_visible_delta, and picks id mode over the ids [0, id_space) (the snapshot takes
- *                                  8 bytes per id of id_space).  CHD_ERR_STATE after index mode was picked or in entity-table mode;
- *                                  later calls of either reserve function on an id-mode engine only grow the lists (a different
- *                                  id_space: CHD_ERR_INVALID).
- * An id-mode delta needs ids for the own entities (CHD_ERR_STATE otherwise) and, standalone, a chd_build after the last change of
- * positions, ids or halo.  If an in-world entity of the current state has an id >= id_space, or two in-world entities share an id
+ *                                  8 bytes per id of id_space).  CHD_ERR_STATE after index mode was picked; later calls of either
+ *                                  reserve function on an id-mode engine only grow the lists (a different id_space: CHD_ERR_INVALID).
+ *                                  In entity-table mode it is the delta mode of an engine made a slab (chd_set_slab / chd_comm_init,
+ *                                  a one-slab world included) before chd_entity_table_init: the table ids are the global ids, so
+ *                                  every table id must be below id_space.  On a table engine that is not a slab: CHD_ERR_STATE (its
+ *                                  index-mode deltas already name ids).
+ * An id-mode delta needs ids for the own entities (chd_set_entity_ids or entity-table mode; CHD_ERR_STATE otherwise) and,
+ * standalone, a chd_build after the last change of positions, ids, table or halo.  If an in-world entity of the current state has an id >= id_space, or two in-world entities share an id
  * (the host routed one entity to two places), CHD_OVF_DELTA_IDS is raised: no lists are written and the snapshot is not advanced,
  * so the next clean delta covers everything (chd_get_visible_delta then returns CHD_ERR_INVALID for the lists).  Entities outside
  * the world are absent and never count as duplicates.
@@ -401,11 +404,15 @@ chd_status chd_get_visible_delta(chd_engine* e, uint64_t* enter_off, uint32_t* e
  * pkg/unreal/message.go:20-203; a move is an ENTITY-channel update whose Merge hook calls Notify for that entity alone,
  * spatial.go:612-626).  The engine keeps the id -> slot map and assigns position slots itself; the host never sees a slot.
  *   chd_entity_table_init  switches a FRESH engine into table mode (CHD_ERR_STATE after any chd_set_entities* / chd_prefetch_entities*
- *                          / chd_build, or after chd_set_slab / chd_set_entity_ids / chd_comm_init).  Allocates the device id table
- *                          (2^k >= 2 x max_entities words) and the slot -> id array, and parks every position slot (NaN: outside
- *                          the world).  From then on chd_set_entities*, chd_prefetch_entities*, chd_entity_buffers,
- *                          chd_set_entity_count, chd_set_entity_ids and the multi-GPU calls (chd_set_slab, chd_export_border,
- *                          chd_import_halo, chd_comm_init, chd_tick_sharded) return CHD_ERR_STATE: the mode is single-GPU.
+ *                          / chd_assign_cells / chd_build, or after chd_set_entity_ids / chd_export_border /
+ *                          chd_reserve_visible_delta_ids).  chd_set_slab / chd_comm_init may come first: that makes it a table
+ *                          engine on slabs (below).  Allocates the device id table (2^k >= 2 x max_entities words) and the slot
+ *                          -> id array, and parks every position slot (NaN: outside the world).  From then on these return
+ *                          CHD_ERR_STATE: the calls that bypass the table (chd_set_entities*, chd_prefetch_entities*,
+ *                          chd_entity_buffers, chd_set_entity_count, chd_set_entity_ids: the table ids ARE the global ids), and
+ *                          chd_set_slab / chd_comm_init (the slab is fixed once the table exists).  chd_export_border,
+ *                          chd_import_halo and chd_tick_sharded work on a table engine made a slab first, and return
+ *                          CHD_ERR_STATE on one that was not: such an engine is single-GPU.
  *   chd_spawn_entities     AddEntity for each (id[i], x[i], z[i]); _f32: FVector positions, widened exactly as chd_set_entities_f32
  *                          widens them.  out_status[i] (may be NULL) is one CHD_EV_* per event, written before the call returns.
  *   chd_despawn_entities   RemoveEntity for each id[i]; out_status as for spawns.
@@ -430,12 +437,23 @@ chd_status chd_get_visible_delta(chd_engine* e, uint64_t* enter_off, uint32_t* e
  * not in it (those are AddEntity / RemoveEntity, not Notify); after a standalone chd_assign_cells it names ids once the following
  * chd_build has run.  CHD_VIEW_ENTITY_ID gives the id of each slot (0 = empty) for
  * consumers that stay on the device.
- * Visible-set deltas work in table mode: a despawned id that is spawned again is a new instance, in `leave` (the old one) and in
- * `enter` (the new one).  Slot quarantine keeps that exact: without chd_reserve_visible_delta a despawned slot may be reused by the
+ * Visible-set deltas work in table mode.  In index mode (chd_reserve_visible_delta, single-GPU) a despawned id that is spawned
+ * again is a new instance, in `leave` (the old one) and in `enter` (the new one).  In id mode (chd_reserve_visible_delta_ids)
+ * identity is the id: a despawn followed by a spawn of the same id between two deltas is NOT reported where a slot sees the id in
+ * both states, and no slot is quarantined.  Index-mode slot quarantine keeps index mode exact: without chd_reserve_visible_delta a despawned slot may be reused by the
  * next spawn call; with it, only after a delta that ran after the despawn has SUCCEEDED, as observed by the library in a summary it
  * read (chd_summary, chd_tick with `out`, chd_fetch_results, chd_fetch_wait); after CHD_OVF_DELTA the slot stays quarantined.
  * Until a slot is released spawns take fresh ones, and when none is left the status is CHD_EV_TABLE_FULL.  A standalone
- * chd_visible_delta needs a chd_build after the last event (CHD_ERR_STATE otherwise; chd_tick builds first). */
+ * chd_visible_delta needs a chd_build after the last event (CHD_ERR_STATE otherwise; chd_tick builds first).
+ * Table mode on slabs (chd_set_slab or chd_comm_init, then chd_entity_table_init): each rank's table holds the entities it OWNS;
+ * every id is live on at most one rank.  Per tick: events -> chd_export_border (border records carry table ids) -> exchange ->
+ * chd_import_halo -> chd_build / chd_tick, or events -> chd_tick_sharded; the events are stream-ordered before the tick and the
+ * tick adds no host synchronisation.  Results name ids, own and halo alike.  The handover list reports each cell change once, by
+ * the rank that owned the entity when it happened (the destination may be a cell of another slab); handover detection stays on
+ * when ownership changes, because slots handed off (chd_handoff_entities) or adopted (a spawn) are flagged like despawns and
+ * spawns: neither rank reports the hand-off itself, and a cell change of an adopted entity before its new owner's next cell
+ * assignment is not reported either (it counts as the spawn's).  Id-mode deltas are the only delta mode on slabs; an id that goes
+ * from halo to own (or back) while a slot sees it is in neither list. */
 enum { CHD_EV_OK = 0, CHD_EV_DUPLICATE = 1, CHD_EV_UNKNOWN_ID = 2, CHD_EV_RESERVED_ID = 3, CHD_EV_TABLE_FULL = 4 };
 typedef struct chd_entity_stats {
     uint32_t live;              /* ids spawned and not despawned */
@@ -516,7 +534,8 @@ chd_status chd_device_view(chd_engine* e, int which, void** d_ptr, uint64_t* cou
  * rank's own and ignored), keeps those whose column lies in [col_lo-halo, col_hi+halo) and appends them as
  * position-less halo entities; the following chd_build sorts own + halo entities into the cell CSR.
  * Call order per tick: chd_set_entities -> chd_export_border (runs chd_assign_cells) -> all-gather ->
- * chd_import_halo -> chd_build.  Entity ids are global: set with chd_set_entity_ids. */
+ * chd_import_halo -> chd_build.  Entity ids are global: set with chd_set_entity_ids, or the table ids in entity-table mode
+ * (spawn / move / despawn events take the place of chd_set_entities there). */
 chd_status chd_set_slab(chd_engine* e, uint32_t col_lo, uint32_t col_hi, uint32_t halo);
 chd_status chd_set_entity_ids(chd_engine* e, const uint32_t* global_id, uint32_t n);
 /* out_count may be NULL: then nothing synchronises with the host (an overflow of cap_records or of the entity capacity
@@ -558,7 +577,9 @@ chd_status chd_comm_use_collective(chd_engine* e, int on);
  * every rank that needs it (visibility stays exact whatever the ownership); chd_get_rehome lists the own entities whose column
  * now belongs to another rank (global id, destination rank) so the host can re-route their position feed — the sender drops
  * them from its next chd_set_entities, the receiver includes them (the reference moves an entity between spatial channels the
- * same way, spatial.go:683-736).
+ * same way, spatial.go:683-736).  In entity-table mode the host holds no positions: after the tick, chd_handoff_entities lists
+ * those entities with their positions and removes them from the sender's table, and the receiver adopts them with
+ * chd_spawn_entities before its next tick; moves and despawns of an id go to its current owner from then on.
  * SUBSCRIBERS live on the rank that owns their centre's column (the host routes each query there).  When that owner changes
  * from rank A to rank B the subscriber's subscriptions and fan-out state (lastFanOutTime, hadFirstFanOut, lastMessageIndex per
  * channel) travel INSIDE the tick's all-gather, so nothing is reset and nobody is re-sent FULL channel data:
@@ -572,9 +593,19 @@ chd_status chd_comm_use_collective(chd_engine* e, int on);
  * without state).  slot / conn_id are HOST arrays. */
 chd_status chd_migrate_out(chd_engine* e, const uint32_t* slot, uint32_t n);
 chd_status chd_migrate_in(chd_engine* e, uint32_t src_rank, uint32_t first_index, const uint32_t* slot, const uint32_t* conn_id, uint32_t n);
-/* own entities (of the last cell assignment) whose column lies outside this rank's slab: global id + the rank that owns the
- * column now.  Synchronous.  *count = how many there are (copies min(count, cap)). */
+/* own entities (of the last cell assignment) whose column lies outside this rank's slab: global id (entity-table mode: table id) +
+ * the rank that owns the column now.  Synchronous and read-only.  *count = how many there are (copies min(count, cap)). */
 chd_status chd_get_rehome(chd_engine* e, uint32_t* global_id, uint32_t* dst_rank, uint32_t cap, uint32_t* count);
+/* Entity-table mode on slabs: hands the entities chd_get_rehome would list to their new owners.  Lists the own live in-world
+ * entities of the last cell assignment whose column lies outside [col_lo, col_hi): id[i], dst_rank[i] (as chd_get_rehome computes
+ * it) and the exact f64 position x[i], z[i]; and removes them from this rank's table (tombstone, slot -> id cleared, the slot
+ * parked, flagged and released at once to the free-slot FIFO: the id lives on elsewhere, so no quarantine; `live` drops).  This
+ * is not a despawn: the receiving rank adopts each entity with chd_spawn_entities(id, x, z), and the position arrives bit-exact.
+ * Synchronous and transactional: *count = the number of entities eligible; if *count > cap, CHD_ERR_CAPACITY and nothing is
+ * removed (a repeat call with a larger buffer lists the same set).  The output arrays may be host or device memory; they may be
+ * NULL only with cap = 0.  CHD_ERR_STATE outside table mode, before any cell assignment, and after a spawn / move / despawn /
+ * hand-off since the last assignment (the positions could be stale).  Call it once per tick, after the tick. */
+chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank, double* x, double* z, uint32_t cap, uint32_t* count);
 
 /* ---- window classes of the last fan-out pass (SURVEY.md §8f rank 1: payload assembly).  The reference merges the selected
  * update window afresh for every subscriber (data.go:248-252); decisions of one channel whose merged payload is
