@@ -483,6 +483,42 @@ int orc_channel_get_state(const orc_channel* ch, uint32_t conn_id, int64_t* last
     return 0;
 }
 
+void orc_channels_subscribe(orc_channel* const* ch, const uint32_t* chan, const uint32_t* conn_id, const uint32_t* interval_ms,
+                            uint64_t n, int64_t now_ns, int32_t delay_ms, int skip_self, int skip_first) {
+    for (uint64_t i = 0; i < n; i++) orc_channel_subscribe(ch[chan[i]], conn_id[i], now_ns, interval_ms[i], delay_ms, skip_self, skip_first);
+}
+
+void orc_channels_unsubscribe(orc_channel* const* ch, const uint32_t* chan, const uint32_t* conn_id, uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) orc_channel_unsubscribe(ch[chan[i]], conn_id[i]);
+}
+
+void orc_channels_on_update(orc_channel* const* ch, const uint32_t* chan, const int64_t* arrival_ns, const uint32_t* sender_conn_id,
+                            uint64_t n) {
+    for (uint64_t i = 0; i < n; i++) orc_channel_on_update(ch[chan[i]], arrival_ns[i], sender_conn_id[i]);
+}
+
+uint64_t orc_channels_tick_data(orc_channel* const* ch, uint32_t n_ch, int64_t t_ns, orc_send* out, uint64_t cap, uint64_t* out_off) {
+    uint64_t total = 0;
+    out_off[0] = 0;
+    for (uint32_t c = 0; c < n_ch; c++) {
+        const uint64_t room = cap - total;
+        const uint32_t k = orc_channel_tick_data(ch[c], t_ns, out + total, room > 0xFFFFFFFEull ? 0xFFFFFFFEu : uint32_t(room));
+        if (k == uint32_t(-1)) return uint64_t(-1);
+        total += k;
+        out_off[c + 1] = total;
+    }
+    return total;
+}
+
+void orc_channels_get_state(orc_channel* const* ch, const uint32_t* chan, const uint32_t* conn_id, uint64_t n, int64_t* last_fanout,
+                            uint8_t* had_first, uint64_t* last_msg_index, uint8_t* found) {
+    for (uint64_t i = 0; i < n; i++) {
+        int had = 0;
+        found[i] = orc_channel_get_state(ch[chan[i]], conn_id[i], &last_fanout[i], &had, &last_msg_index[i]) == 0;
+        had_first[i] = uint8_t(had);
+    }
+}
+
 /* ------------------------------------------------------------------ visible sets ------ */
 namespace {
 struct CellLists {

@@ -149,6 +149,20 @@ uint32_t orc_channel_tick_data_ex(orc_channel*, int64_t t_ns, orc_send* out, uin
 int orc_channel_get_state(const orc_channel*, uint32_t conn_id, int64_t* last_fanout, int* had_first,
                           uint64_t* last_msg_index);
 
+/* ---- the same per-channel calls over many channels at once (tests at hundreds of thousands of subscriptions).  Each loops
+ * over the functions above in array order; `ch` is an array of channel handles and chan[i] selects one of them. ---- */
+void orc_channels_subscribe(orc_channel* const* ch, const uint32_t* chan, const uint32_t* conn_id, const uint32_t* interval_ms,
+                            uint64_t n, int64_t now_ns, int32_t delay_ms, int skip_self, int skip_first);
+void orc_channels_unsubscribe(orc_channel* const* ch, const uint32_t* chan, const uint32_t* conn_id, uint64_t n);
+void orc_channels_on_update(orc_channel* const* ch, const uint32_t* chan, const int64_t* arrival_ns, const uint32_t* sender_conn_id,
+                            uint64_t n);
+/* tick_data of channels 0 .. n_ch-1 in turn; the sends of channel c are out[out_off[c] .. out_off[c+1]).  Returns the total,
+ * or (uint64_t)-1 when `cap` is too small or a channel's iteration bound trips. */
+uint64_t orc_channels_tick_data(orc_channel* const* ch, uint32_t n_ch, int64_t t_ns, orc_send* out, uint64_t cap, uint64_t* out_off);
+/* found[i] = 0 when conn_id[i] is not subscribed to chan[i] (the state outputs are then left as they were) */
+void orc_channels_get_state(orc_channel* const* ch, const uint32_t* chan, const uint32_t* conn_id, uint64_t n, int64_t* last_fanout,
+                            uint8_t* had_first, uint64_t* last_msg_index, uint8_t* found);
+
 /* ---- derived: per-subscriber visible-entity lists (SURVEY.md §8 a14) ----
  * visible(s) = { e : cell(pos_e) in keys(QueryChannelIds(query_s)) }, canonical order (cell asc, entity idx asc).
  * Sphere-only batch (the benchmark shape).  pair_off[nq+1], vis_off[nq+1] (u64).  status[nq].

@@ -94,6 +94,18 @@ class Oracle:
         L.orc_channel_tick_data.argtypes = [C.c_void_p, C.c_int64, C.POINTER(Send), C.c_uint32]
         L.orc_channel_get_state.restype = C.c_int
         L.orc_channel_get_state.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_int64), C.POINTER(C.c_int), u64p]
+        vp = C.c_void_p
+        L.orc_channels_subscribe.restype = None
+        L.orc_channels_subscribe.argtypes = [vp, u32p, u32p, u32p, C.c_uint64, C.c_int64, C.c_int32, C.c_int, C.c_int]
+        L.orc_channels_unsubscribe.restype = None
+        L.orc_channels_unsubscribe.argtypes = [vp, u32p, u32p, C.c_uint64]
+        L.orc_channels_on_update.restype = None
+        L.orc_channels_on_update.argtypes = [vp, u32p, C.POINTER(C.c_int64), u32p, C.c_uint64]
+        L.orc_channels_tick_data.restype = C.c_uint64
+        L.orc_channels_tick_data.argtypes = [vp, C.c_uint32, C.c_int64, C.POINTER(Send), C.c_uint64, u64p]
+        L.orc_channels_get_state.restype = None
+        L.orc_channels_get_state.argtypes = [vp, u32p, u32p, C.c_uint64, C.POINTER(C.c_int64), C.POINTER(C.c_uint8), u64p,
+                                             C.POINTER(C.c_uint8)]
         L.orc_sphere_tick.restype = C.c_int
         L.orc_sphere_tick.argtypes = [C.POINTER(Grid), f64p, f64p, C.c_uint32, f64p, f64p, f64p, C.c_uint32,
                                       u32p, u64p, u32p, u32p, C.c_uint64, u64p, u32p, C.c_uint64, C.c_int]
@@ -193,6 +205,9 @@ class Oracle:
     def channel(self):
         return OracleChannel(self)
 
+    def channels(self, n):
+        return OracleChannels(self, n)
+
     # ---- derived ----
     def sphere_tick(self, g, ex, ez, cx, cz, r):
         ex = np.ascontiguousarray(ex, np.float64); ez = np.ascontiguousarray(ez, np.float64)
@@ -267,6 +282,64 @@ class OracleChannel:
         a, b, c = C.c_int64(0), C.c_int(0), C.c_uint64(0)
         rc = self.L.orc_channel_get_state(self.h, conn, C.byref(a), C.byref(b), C.byref(c))
         return None if rc else (a.value, bool(b.value), c.value)
+
+
+SEND_DTYPE = np.dtype([("conn_id", np.uint32), ("kind", np.uint32), ("n_selected", np.uint32), ("first_sel", np.uint32),
+                       ("last_sel", np.uint32), ("sel_hash", np.uint64), ("last_message_index", np.uint64), ("window_hi", np.int64)],
+                      align=True)
+assert SEND_DTYPE.itemsize == C.sizeof(Send)
+
+
+class OracleChannels:
+    """n oracle channels (one per cell) driven with arrays: the batched orc_channels_* calls, each a loop over the per-channel
+    functions OracleChannel wraps."""
+
+    def __init__(self, orc, n):
+        self.L = orc.lib
+        self.n = n
+        self.h = np.array([self.L.orc_channel_new() for _ in range(n)], np.uint64)
+
+    def __del__(self):
+        try:
+            for h in self.h:
+                self.L.orc_channel_free(C.c_void_p(int(h)))
+        except Exception:
+            pass
+
+    def _hp(self):
+        return C.c_void_p(self.h.ctypes.data)
+
+    def subscribe(self, chan, conn, now_ns, interval_ms, delay_ms=0, skip_self=True, skip_first=False):
+        chan, conn, iv = (np.ascontiguousarray(a, np.uint32) for a in (chan, conn, interval_ms))
+        self.L.orc_channels_subscribe(self._hp(), _p(chan, u32p), _p(conn, u32p), _p(iv, u32p), len(chan), int(now_ns), delay_ms,
+                                      int(skip_self), int(skip_first))
+
+    def unsubscribe(self, chan, conn):
+        chan, conn = (np.ascontiguousarray(a, np.uint32) for a in (chan, conn))
+        self.L.orc_channels_unsubscribe(self._hp(), _p(chan, u32p), _p(conn, u32p), len(chan))
+
+    def on_update(self, chan, arrival_ns, sender):
+        chan, sender = (np.ascontiguousarray(a, np.uint32) for a in (chan, sender))
+        arrival_ns = np.ascontiguousarray(arrival_ns, np.int64)
+        self.L.orc_channels_on_update(self._hp(), _p(chan, u32p), arrival_ns.ctypes.data_as(C.POINTER(C.c_int64)), _p(sender, u32p),
+                                      len(chan))
+
+    def tick_data(self, t_ns, cap):
+        """-> (sends[SEND_DTYPE], off[n+1]): the sends of channel c are sends[off[c]:off[c+1]]"""
+        out = np.zeros(max(int(cap), 1), SEND_DTYPE)
+        off = np.zeros(self.n + 1, np.uint64)
+        k = self.L.orc_channels_tick_data(self._hp(), self.n, int(t_ns), out.ctypes.data_as(C.POINTER(Send)), int(cap), _p(off, u64p))
+        assert k != 2 ** 64 - 1, "oracle tick_data: capacity/iteration bound"
+        return out[:k], off
+
+    def state(self, chan, conn):
+        """-> (last[n], had_first[n], last_index[n], found[n])"""
+        chan, conn = (np.ascontiguousarray(a, np.uint32) for a in (chan, conn))
+        n = len(chan)
+        last = np.zeros(n, np.int64); had = np.zeros(n, np.uint8); li = np.zeros(n, np.uint64); found = np.zeros(n, np.uint8)
+        self.L.orc_channels_get_state(self._hp(), _p(chan, u32p), _p(conn, u32p), n, last.ctypes.data_as(C.POINTER(C.c_int64)),
+                                      had.ctypes.data_as(C.POINTER(C.c_uint8)), _p(li, u64p), found.ctypes.data_as(C.POINTER(C.c_uint8)))
+        return last, had.astype(bool), li, found.astype(bool)
 
 
 def build():
