@@ -34,45 +34,13 @@ static DeltaDev delta_view(chd_engine* e) {
         d.key = D.now_gkey;
         d.n = D.id_space;
         d.bad_ids = D.bad_ids;
-        // entity-table mode: d_sorted_ent holds build positions (slots, then halo records); the id-valued copy is the CSR by id
-        if (e->tbl.on) d.sorted = e->tbl.d_sorted_id;
+        // the CSR by id: d_sorted_ent, or in entity-table mode (where it holds build positions) the table pass's id-valued copy
+        d.sorted = chd_sorted_out(e);
     }
     return d;
 }
 
 extern "C" {
-
-chd_status chd_delta_check(chd_engine* e, bool will_build) {
-    if (e->delta_blocked && !e->dl.ids) {
-        e->fail("index-mode visible deltas are single-GPU only: this engine used chd_set_slab / chd_set_entity_ids / chd_comm_init "
-                "(chd_reserve_visible_delta_ids names entities by global id instead)");
-        return CHD_ERR_STATE;
-    }
-    if (!e->dl.on) {
-        e->fail("visible delta before chd_reserve_visible_delta");
-        return CHD_ERR_STATE;
-    }
-    if (e->dl.ids && !e->have_gid && !e->tbl.on) {
-        e->fail("id-mode visible delta on an engine without global ids (chd_set_entity_ids)");
-        return CHD_ERR_STATE;
-    }
-    if (!will_build && e->dl.ids && e->entities_dirty) {
-        // id mode: the ids scattered by the delta must be those the build sorted
-        e->fail("id-mode visible delta needs a chd_build after the last chd_set_entities / chd_set_entity_ids / chd_import_halo");
-        return CHD_ERR_STATE;
-    }
-    if (!will_build && (!e->built || (e->assigned && e->entities_dirty))) {
-        // chd_assign_cells rewrote the keys since the last build: keys and cell CSR no longer describe one state
-        e->fail("visible delta needs a chd_build of the current cell assignment");
-        return CHD_ERR_STATE;
-    }
-    if (!will_build && e->tbl.on && e->entities_dirty) {
-        // entity-table mode: the ids the lists are translated with must be those of the build the delta measures
-        e->fail("visible delta needs a chd_build after the last spawn / move / despawn");
-        return CHD_ERR_STATE;
-    }
-    return CHD_OK;
-}
 
 chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
     chd_engine::Delta& D = e->dl;
@@ -83,15 +51,14 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
     const uint64_t N = e->lim.max_entities;
     chd_status st = chd_epoch_tick(e, s, EP_DELTA);
     if (st != CHD_OK) return st;
-    // sizes and the key / pair buffers in use are baked into the captured launches
+    // sizes, the key / pair buffers in use and the ids (the id scatter's, the table lists') are baked into the captured launches
+    const EntityIds ids = chd_entity_ids(e);
     uint64_t key = stage_key(0x64656c7461ull, d.n, d.n_slots, D.n_out, e->cur, d.key, d.enter, d.leave, d.enter_cap, d.leave_cap, e->tbl.on,
-                             e->tbl.d_id_of_slot);
-    // id mode: the scatter bakes in the build's length (host count or d_n_build) and the key / id buffers it reads
+                             ids.own_ids, ids.gid, ids.own);
+    // id mode: the scatter bakes in the build's length (host count or d_n_build) and the key buffer it reads
     const uint32_t* n_ptr = e->sorted_dev_n ? e->d_n_build : nullptr;
     const uint32_t n_scatter = e->sorted_dev_n ? e->lim.max_entities : e->n_sorted;
-    // (entity-table mode: the slots below the high-water mark are named by the table's slot -> id array, read in place)
-    const uint32_t own = e->tbl.on ? e->n_own : 0;
-    if (D.ids) key = stage_key(key, 0x696473ull, D.id_space, n_scatter, n_ptr, e->d_key, e->d_gid, e->d_n_build, own, d.sorted);
+    if (D.ids) key = stage_key(key, 0x696473ull, D.id_space, n_scatter, n_ptr, e->d_key, e->d_n_build, d.sorted);
     const unsigned grid = (unsigned)e->sm_count * 8;
     const unsigned slot_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(blocks_for((uint64_t)D.n_out * 32, DELTA_THREADS), (uint64_t)e->sm_count * 32));
     return run_stage(e, s, D.g, key, [&]() -> chd_status {
@@ -104,8 +71,7 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
             // scatter reads this tick's imported halo.
             CU(e, cudaMemsetAsync(D.now_gkey, 0xFF, 4ull * D.id_space, s));
             CU(e, cudaMemsetAsync(D.bad_ids, 0, 4, s));
-            delta_id_scatter_kernel<<<grid, DELTA_THREADS, 0, s>>>(e->d_gid, e->tbl.d_id_of_slot, own, e->d_key, n_scatter, n_ptr, C, D.now_gkey,
-                                                                   D.id_space, D.bad_ids, d.overflow);
+            delta_id_scatter_kernel<<<grid, DELTA_THREADS, 0, s>>>(ids, e->d_key, n_scatter, n_ptr, C, D.now_gkey, D.id_space, D.bad_ids, d.overflow);
             KCHECK(e);
         }
         SCAN(e, exclusive_scan_fn<DeltaArrivalFlag, uint32_t>(DeltaArrivalFlag{d.sorted, d.key, d.snap_key, d.snap_hdr, d.n, C}, D.arr_rank, N, D.site_arr, s,
@@ -173,32 +139,21 @@ static chd_status delta_reserve(chd_engine* e, uint64_t cap_entries, bool ids, u
 
 chd_status chd_reserve_visible_delta(chd_engine* e, uint64_t cap_entries) {
     if (!e) return CHD_ERR_INVALID;
-    if (e->dl.ids) return delta_reserve(e, cap_entries, true, e->dl.id_space);  // id mode: grows the lists only
-    if (e->delta_blocked) return chd_delta_check(e, true);
-    return delta_reserve(e, cap_entries, false, 0);
+    if (chd_rule_index_delta(e) != CHD_OK) return CHD_ERR_STATE;
+    return delta_reserve(e, cap_entries, e->dl.ids, e->dl.id_space);  // (id mode: grows the lists only)
 }
 
 chd_status chd_reserve_visible_delta_ids(chd_engine* e, uint64_t cap_entries, uint32_t id_space) {
     if (!e || id_space == 0) return CHD_ERR_INVALID;
-    // entity-table mode: id mode is the delta mode of slab engines; on one GPU the index-mode deltas already name ids
-    if (e->tbl.on && !e->slab) return chd_table_refuse(e, "chd_reserve_visible_delta_ids on an engine that is not a slab");
-    if (e->dl.on && !e->dl.ids) {
-        e->fail("chd_reserve_visible_delta_ids: this engine's visible deltas are in index mode (chd_reserve_visible_delta came first)");
-        return CHD_ERR_STATE;
-    }
-    if (e->dl.on && id_space != e->dl.id_space) {
-        e->fail("chd_reserve_visible_delta_ids: id_space %u differs from the %u the mode was set up with", id_space, e->dl.id_space);
-        return CHD_ERR_INVALID;
-    }
-    return delta_reserve(e, cap_entries, true, id_space);
+    const chd_status st = chd_rule_id_delta(e, id_space);
+    return st != CHD_OK ? st : delta_reserve(e, cap_entries, true, id_space);
 }
 
 chd_status chd_visible_delta(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
-    chd_status st = chd_delta_check(e, false);
-    if (st != CHD_OK) return st;
+    if (chd_delta_check(e, false) != CHD_OK) return CHD_ERR_STATE;
     CU(e, cudaSetDevice(e->device));
-    st = chd_fetch_guard(e, e->stream);
+    const chd_status st = chd_fetch_guard(e, e->stream);
     return st != CHD_OK ? st : chd_delta_on(e, e->stream);
 }
 

@@ -63,17 +63,14 @@ struct DeltaArrivalFlag {
 
 // Id mode: gkey[id] = cell of every in-world entity of the last build (own and halo, i < the build's length), gkey cleared to
 // 0xFFFFFFFF (absent) before.  An id >= id_space, or an id that two in-world entities hold, sets *bad and CHD_OVF_DELTA_IDS.
-// Entity-table mode: positions below `own` (the table's high-water mark) are slots named by id_of_slot, the halo records after
-// them by gid; elsewhere own = 0 and gid names every position.
-__global__ void __launch_bounds__(DELTA_THREADS) delta_id_scatter_kernel(const uint32_t* gid, const uint32_t* id_of_slot, uint32_t own, const uint32_t* key,
-                                                                         uint32_t n, const uint32_t* n_ptr, uint32_t cells, uint32_t* gkey, uint32_t id_space,
-                                                                         uint32_t* bad, uint32_t* overflow) {
+__global__ void __launch_bounds__(DELTA_THREADS) delta_id_scatter_kernel(EntityIds ids, const uint32_t* key, uint32_t n, const uint32_t* n_ptr,
+                                                                         uint32_t cells, uint32_t* gkey, uint32_t id_space, uint32_t* bad, uint32_t* overflow) {
     const uint32_t m = n_ptr ? min(*n_ptr, n) : n;
     bool err = false;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) {
         const uint32_t k = key[i];
         if (k >= cells) continue;  // an own entity outside the world: absent, never a duplicate
-        const uint32_t g = i < own ? id_of_slot[i] : gid[i];
+        const uint32_t g = ids.at(i);
         if (g >= id_space || atomicExch(&gkey[g], k) != 0xFFFFFFFFu) err = true;
     }
     if (err) {

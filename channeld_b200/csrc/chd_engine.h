@@ -8,7 +8,7 @@
 //   chd_results.cu   getters, chd_fetch_results, device views
 //   chd_shard.cu     multi-GPU X-slabs: border export, halo import, the NCCL exchange
 //   chd_extras.cu    window classes, ADJACENT_CHANNELS broadcast sets, config-plane helpers
-//   chd_table.cu     entity-table mode: spawn / move / despawn by id, the id-valued results
+//   chd_table.cu     the mode rules; entity-table mode: spawn / move / despawn by id, the id-valued results
 #pragma once
 #include <cuda_runtime.h>
 
@@ -301,7 +301,7 @@ struct chd_engine {
         bool done_recorded = false;  // the last tick ran the delta off the engine stream: its end (and CHD_OVF_DELTA) is ev_done
     } dl;
     // chd_set_slab / chd_set_entity_ids / chd_comm_init were used: halo indices are not stable, no index-mode deltas (id mode is
-    // not affected)
+    // not affected).  Sticky: chd_set_entity_ids(NULL) leaves no other trace, so this cannot be derived from have_gid / slab.
     bool delta_blocked = false;
     // chd_set_slab (directly or through chd_comm_init) made this engine an X-slab: the multi-GPU calls work in entity-table mode
     // only on such an engine, made a slab before chd_entity_table_init
@@ -478,14 +478,18 @@ RingDev chd_ring_view(const chd_engine* e);
 chd_status chd_sort_pass_any(chd_engine* e, cudaStream_t s, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in, uint32_t n,
                              const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits, uint32_t* key_out,
                              uint32_t* val_out, ScatterExtras ex = ScatterExtras{nullptr, 0, nullptr}, unsigned long long* bump = nullptr);
-// visible-set delta (chd_delta.cu): whether one may run now (will_build: the caller builds first), and the stage itself on `s`
-chd_status chd_delta_check(chd_engine* e, bool will_build);
+// the visible-set delta stage on `s` (chd_delta.cu)
 chd_status chd_delta_on(chd_engine* e, cudaStream_t s);
-// entity-table mode (chd_table.cu): the call named `fn` is not available in it (CHD_ERR_STATE); the pass after every table-mode build
-// (sorted ids, handover list in ids); the delta's translation to ids, inside its stage; a decoded summary's last successful delta
-chd_status chd_table_refuse(chd_engine* e, const char* fn);
-// CHD_OK unless the engine is in entity-table mode without having been made a slab first (then CHD_ERR_STATE for the call `fn`)
-chd_status chd_table_slab_check(chd_engine* e, const char* fn);
+// the mode rules (chd_table.cu, numbered as in DESIGN.md §5): CHD_OK, or the error set and CHD_ERR_STATE (6: or CHD_ERR_INVALID)
+chd_status chd_rule_not_table(chd_engine* e, const char* fn);
+chd_status chd_rule_table_on_slab(chd_engine* e, const char* fn);
+chd_status chd_rule_table(chd_engine* e, const char* fn);
+chd_status chd_rule_index_delta(chd_engine* e);
+chd_status chd_rule_id_delta(chd_engine* e, uint32_t id_space);
+chd_status chd_delta_check(chd_engine* e, bool will_build);
+chd_status chd_rule_halo_import(chd_engine* e);
+// entity-table mode (chd_table.cu): the pass after every table-mode build (sorted ids, handover list in ids); the delta's
+// translation to ids, inside its stage; a decoded summary's last successful delta
 chd_status chd_table_after_build(chd_engine* e, cudaStream_t s);
 chd_status chd_table_delta_ids(chd_engine* e, cudaStream_t s);
 void chd_table_observe(chd_engine* e, uint32_t delta_build);
@@ -494,6 +498,11 @@ void chd_table_observe(chd_engine* e, uint32_t delta_build);
 // What the cell CSR's sorted_entity, the visible lists and the read-back report: entity indices, or ids in entity-table mode.  The
 // slot-valued d_sorted_ent stays what the delta reads.
 static inline const uint32_t* chd_sorted_out(const chd_engine* e) { return e->tbl.on ? e->tbl.d_sorted_id : e->d_sorted_ent; }
+
+// The ids build positions carry: entity-table slots by the table and the halo after them by d_gid, else d_gid or the index.
+static inline EntityIds chd_entity_ids(const chd_engine* e) {
+    return e->tbl.on ? EntityIds{e->tbl.d_id_of_slot, e->d_gid, e->n_own} : EntityIds{nullptr, e->have_gid ? e->d_gid : nullptr, 0};
+}
 
 // Grow-on-demand buffer: when `need` elements exceed `*cap`, the buffer is replaced (contents not kept) by one of `count`
 // elements, the caller's growth policy.  *cap is 0 exactly when there is no buffer.

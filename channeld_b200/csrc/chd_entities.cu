@@ -130,7 +130,7 @@ void chd_entities_replaced(chd_engine* e, uint32_t n) {
 // up_stream (prefetch).  Device-resident doubles given to a set are read in place.
 static chd_status upload_positions(chd_engine* e, const char* fn, const void* x, const void* z, uint32_t n, bool f32, bool prefetch) {
     if (!e || (n && (!x || !z))) return CHD_ERR_INVALID;
-    if (e->tbl.on) return chd_table_refuse(e, fn);
+    if (chd_rule_not_table(e, fn) != CHD_OK) return CHD_ERR_STATE;
     if (n > e->lim.max_entities) {
         e->fail("%s: %u > max_entities %u", fn, n, e->lim.max_entities);
         return CHD_ERR_CAPACITY;
@@ -182,7 +182,7 @@ chd_status chd_prefetch_entities_f32(chd_engine* e, const float* x, const float*
 
 chd_status chd_entity_buffers(chd_engine* e, double** d_x, double** d_z, uint32_t* n) {
     if (!e) return CHD_ERR_INVALID;
-    if (e->tbl.on) return chd_table_refuse(e, "chd_entity_buffers");
+    if (chd_rule_not_table(e, "chd_entity_buffers") != CHD_OK) return CHD_ERR_STATE;
     if (d_x) *d_x = e->d_x;
     if (d_z) *d_z = e->d_z;
     if (n) *n = e->n_own;
@@ -195,14 +195,14 @@ chd_status chd_entity_buffers(chd_engine* e, double** d_x, double** d_z, uint32_
 
 chd_status chd_set_entity_count(chd_engine* e, uint32_t n) {
     if (!e || n > e->lim.max_entities) return CHD_ERR_INVALID;
-    if (e->tbl.on) return chd_table_refuse(e, "chd_set_entity_count");
+    if (chd_rule_not_table(e, "chd_set_entity_count") != CHD_OK) return CHD_ERR_STATE;
     chd_entities_replaced(e, n);
     return CHD_OK;
 }
 
 chd_status chd_set_entity_ids(chd_engine* e, const uint32_t* gid, uint32_t n) {
     if (!e || n > e->lim.max_entities) return CHD_ERR_INVALID;
-    if (e->tbl.on) return chd_table_refuse(e, "chd_set_entity_ids");
+    if (chd_rule_not_table(e, "chd_set_entity_ids") != CHD_OK) return CHD_ERR_STATE;
     CU(e, cudaSetDevice(e->device));
     e->delta_blocked = true;  // global ids: the multi-GPU flow (index-mode visible deltas are single-GPU only)
     if (!gid) {

@@ -62,7 +62,7 @@ extern "C" {
 
 chd_status chd_set_slab(chd_engine* e, uint32_t col_lo, uint32_t col_hi, uint32_t halo) {
     // (entity-table mode on slabs: the slab comes first, then chd_entity_table_init; the table's slots do not move with the slab)
-    if (e && e->tbl.on) return chd_table_refuse(e, "chd_set_slab");
+    if (e && chd_rule_not_table(e, "chd_set_slab") != CHD_OK) return CHD_ERR_STATE;
     if (!e || col_lo >= col_hi || col_hi > e->g.cols) return CHD_ERR_INVALID;
     e->slab = true;
     e->g.col_lo = col_lo;
@@ -74,7 +74,7 @@ chd_status chd_set_slab(chd_engine* e, uint32_t col_lo, uint32_t col_hi, uint32_
 }
 
 chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_records, uint32_t* out_count) {
-    if (e && chd_table_slab_check(e, "chd_export_border") != CHD_OK) return CHD_ERR_STATE;
+    if (e && chd_rule_table_on_slab(e, "chd_export_border") != CHD_OK) return CHD_ERR_STATE;
     if (!e || !d_records) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
     cudaStream_t s = e->stream;
@@ -85,9 +85,9 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
     const uint32_t n = e->n_own;
     // inside chd_tick_sharded with the peer exchange the records go straight into the peers' windows afterwards: no padding needed
     const bool to_peers = e->peer_push && d_records == e->d_rec_local;
-    // a record names its entity by global id: the table id of the slot in entity-table mode (free and despawned slots are parked
-    // outside the world, so BorderFlag skips them)
-    const uint32_t* gid = e->tbl.on ? e->tbl.d_id_of_slot : (e->have_gid ? e->d_gid : nullptr);
+    // a record names its entity by global id.  Only own entities are exported: in entity-table mode (own = n_own) each record
+    // carries the table id of its slot (free and despawned slots are parked outside the world, so BorderFlag skips them).
+    const EntityIds ids = chd_entity_ids(e);
     auto enqueue = [&]() -> chd_status {
         const bool bump_in_assign = !e->assigned && n;
         if (bump_in_assign) e->assign_bump = e->d_epoch + EP_BORDER;
@@ -98,7 +98,7 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
             KCHECK(e);
         }
         if (!to_peers) CU(e, cudaMemsetAsync(d_records, 0xFF, 8ull * cap_records, s));  // unused records read as "no cell"
-        SCAN(e, compact_1p(BorderFlag{e->g, e->d_key}, BorderSink{e->d_key, gid, d_records, cap_records, e->d_boff + n, e->d_ctr},
+        SCAN(e, compact_1p(BorderFlag{e->g, e->d_key}, BorderSink{e->d_key, ids, d_records, cap_records, e->d_boff + n, e->d_ctr},
                            n, e->site_border, s));
         if (to_peers) {
             PeerWindows pw{};
@@ -117,7 +117,7 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
         // replayable: cell assignment + border selection of one tick.  The graph bakes in the sizes, the key buffer the new keys
         // go to, the positions, the ids the records carry, the records, the slab and the exchange path.
         const uint64_t key = stage_key(0x6578706full, n, e->have_gid, e->have_prev_key, e->have_prev_key ? e->d_prev_key : e->d_key, e->pos_x, e->pos_z,
-                                       gid, d_records, cap_records, e->g.col_lo, e->g.col_hi, e->g.halo, to_peers);
+                                       ids.own_ids, ids.gid, ids.own, d_records, cap_records, e->g.col_lo, e->g.col_hi, e->g.halo, to_peers);
         st = run_stage(e, s, e->g_export, key, enqueue);
         if (st == CHD_OK && !e->assigned) chd_assign_host(e);  // replayed graph
         if (st == CHD_OK) st = chd_note_pos_read(e, s);
@@ -137,17 +137,10 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
 }
 
 chd_status chd_import_halo(chd_engine* e, const uint32_t* d_records, uint32_t n_records, uint32_t skip_first, uint32_t skip_count) {
-    if (e && chd_table_slab_check(e, "chd_import_halo") != CHD_OK) return CHD_ERR_STATE;
+    if (e && chd_rule_table_on_slab(e, "chd_import_halo") != CHD_OK) return CHD_ERR_STATE;
     if (!e || (n_records && !d_records)) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
-    if (!e->assigned) {
-        e->fail("chd_import_halo before chd_export_border / chd_assign_cells");
-        return CHD_ERR_STATE;
-    }
-    if (!e->have_gid && !e->tbl.on) {  // (entity-table mode: the table ids are the global ids)
-        e->fail("chd_import_halo requires global entity ids (chd_set_entity_ids or entity-table mode)");
-        return CHD_ERR_STATE;
-    }
+    if (chd_rule_halo_import(e) != CHD_OK) return CHD_ERR_STATE;
     cudaStream_t s = e->stream;
     if (n_records > e->lim.max_entities) {
         e->fail("halo import of %u records > max_entities scratch %u", n_records, e->lim.max_entities);
@@ -198,7 +191,7 @@ chd_status chd_comm_unique_id(void* out_id) {
 
 chd_status chd_comm_init(chd_engine* e, const void* unique_id, int rank, int world, uint32_t halo_cols, uint32_t border_capacity,
                          uint32_t migrate_subscribers, uint32_t migrate_pairs) {
-    if (e && e->tbl.on) return chd_table_refuse(e, "chd_comm_init");
+    if (e && chd_rule_not_table(e, "chd_comm_init") != CHD_OK) return CHD_ERR_STATE;
     if (!e || !unique_id || world < 1 || rank < 0 || rank >= world || border_capacity == 0) return CHD_ERR_INVALID;
     if (world >= 4096 || migrate_subscribers >= (1u << 20)) return CHD_ERR_INVALID;  // (slot_src packs rank:12 | record:20)
     if (e->comm) {
@@ -339,7 +332,7 @@ chd_status chd_comm_destroy(chd_engine* e) {
 // entities, then build + emit run over own + halo entities and the streams join.  Nothing synchronises with the host.
 chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_ns, uint32_t flags, chd_tick_summary* out) {
     if (!e) return CHD_ERR_INVALID;
-    if (chd_table_slab_check(e, "chd_tick_sharded") != CHD_OK) return CHD_ERR_STATE;
+    if (chd_rule_table_on_slab(e, "chd_tick_sharded") != CHD_OK) return CHD_ERR_STATE;
     if (!e->comm) {
         e->fail("chd_tick_sharded before chd_comm_init");
         return CHD_ERR_STATE;
@@ -469,8 +462,8 @@ chd_status chd_get_rehome(chd_engine* e, uint32_t* global_id, uint32_t* dst_rank
     // scratch: the radix sort's temporaries are free between builds
     CU(e, cudaMemsetAsync(e->d_boff, 0, 4, s));
     if (n) {
-        const uint32_t* gid = e->tbl.on ? e->tbl.d_id_of_slot : (e->have_gid ? e->d_gid : nullptr);
-        rehome_kernel<<<blocks_for(n, 256), 256, 0, s>>>(e->g, e->d_key, gid, n, world, e->d_tmp_key, e->d_tmp_val,
+        // (own entities only: in entity-table mode each carries the table id of its slot)
+        rehome_kernel<<<blocks_for(n, 256), 256, 0, s>>>(e->g, e->d_key, chd_entity_ids(e), n, world, e->d_tmp_key, e->d_tmp_val,
                                                          e->lim.max_entities, e->d_boff);
         KCHECK(e);
     }

@@ -25,14 +25,14 @@ struct BorderFlag {
 };
 struct BorderSink {
     const uint32_t* __restrict__ key;
-    const uint32_t* __restrict__ gid;  // nullptr: entity index = global id
+    EntityIds ids;
     uint32_t* __restrict__ out;
     uint32_t cap;
     uint32_t* __restrict__ count_out;
     Counters* __restrict__ ctr;
     __device__ __forceinline__ void operator()(uint64_t i, uint32_t k) const {
         if (k < cap) {
-            out[2 * k] = gid ? gid[i] : (uint32_t)i;
+            out[2 * k] = ids.at((uint32_t)i);
             out[2 * k + 1] = key[i];
         }
     }
@@ -173,7 +173,7 @@ __global__ void peer_wait_kernel(uint32_t* own_win, uint64_t stride_words, uint3
 }
 
 // chd_get_rehome: own entities whose column now belongs to another rank (a set: block-aggregated append)
-__global__ void __launch_bounds__(256) rehome_kernel(GridDev g, const uint32_t* __restrict__ key, const uint32_t* __restrict__ gid, uint32_t n,
+__global__ void __launch_bounds__(256) rehome_kernel(GridDev g, const uint32_t* __restrict__ key, EntityIds ids, uint32_t n,
                                                      uint32_t world, uint32_t* __restrict__ out_gid, uint32_t* __restrict__ out_rank,
                                                      uint32_t cap, uint32_t* __restrict__ count) {
     __shared__ uint32_t s_cnt, s_base;
@@ -191,7 +191,7 @@ __global__ void __launch_bounds__(256) rehome_kernel(GridDev g, const uint32_t* 
     if (threadIdx.x == 0 && s_cnt) s_base = atomicAdd(count, s_cnt);
     __syncthreads();
     if (away && s_base + my < cap) {
-        out_gid[s_base + my] = gid ? gid[i] : i;
+        out_gid[s_base + my] = ids.at(i);
         out_rank[s_base + my] = slab_owner(col, g.cols, world);
     }
 }

@@ -9,12 +9,6 @@
 
 namespace {
 
-chd_status need_table(chd_engine* e, const char* fn) {
-    if (e->tbl.on) return CHD_OK;
-    e->fail("%s before chd_entity_table_init", fn);
-    return CHD_ERR_STATE;
-}
-
 // The positions changed: nothing is assigned or built for them yet, and a halo imported before may sit where the high-water mark
 // now reaches.  Unlike chd_entities_replaced this keeps handover detection on when the high-water mark grows: the new slots are
 // flagged and left out of the handover list.
@@ -121,13 +115,12 @@ bool reserved_id(uint32_t id) { return id == 0u || id == 0xFFFFFFFFu; }
 
 chd_status spawn(chd_engine* e, const char* fn, const uint32_t* id_in, const void* x_in, const void* z_in, bool f32, uint32_t n, uint8_t* out_status) {
     if (!e || (n && (!id_in || !x_in || !z_in))) return CHD_ERR_INVALID;
-    chd_status st = need_table(e, fn);
-    if (st != CHD_OK) return st;
+    if (chd_rule_table(e, fn) != CHD_OK) return CHD_ERR_STATE;
     CU(e, cudaSetDevice(e->device));
     chd_engine::Table& t = e->tbl;
     std::vector<uint32_t> kid;
     const uint32_t* ids = nullptr;
-    st = host_view(e, id_in, n, kid, &ids);
+    chd_status st = host_view(e, id_in, n, kid, &ids);
     if (st != CHD_OK) return st;
     // positions as doubles: the float form widens exactly, as chd_set_entities_f32 does
     std::vector<double> px(n), pz(n);
@@ -193,8 +186,7 @@ chd_status spawn(chd_engine* e, const char* fn, const uint32_t* id_in, const voi
 
 chd_status move(chd_engine* e, const char* fn, const uint32_t* id, const void* x, const void* z, bool f32, uint32_t n) {
     if (!e || (n && (!id || !x || !z))) return CHD_ERR_INVALID;
-    chd_status st = need_table(e, fn);
-    if (st != CHD_OK) return st;
+    if (chd_rule_table(e, fn) != CHD_OK) return CHD_ERR_STATE;
     const uint64_t N = e->lim.max_entities;
     if (n > N) {
         e->fail("%s: %u moves in one call > max_entities %llu", fn, n, (unsigned long long)N);
@@ -232,30 +224,87 @@ chd_status move(chd_engine* e, const char* fn, const uint32_t* id, const void* x
     return CHD_OK;
 }
 
+template <typename... A>
+chd_status refuse(const chd_engine* e, const char* fmt, A... a) {
+    e->fail(fmt, a...);
+    return CHD_ERR_STATE;
+}
+
 }  // namespace
 
 extern "C" {
 
-chd_status chd_table_refuse(chd_engine* e, const char* fn) {
-    e->fail("%s is not available in entity-table mode (chd_entity_table_init): use chd_spawn_entities / chd_move_entities / chd_despawn_entities", fn);
-    return CHD_ERR_STATE;
+// ---- The mode rules (DESIGN.md §5, same numbers): entities are named by index, by global id (chd_set_entity_ids) or by table id
+// (entity-table mode), visible deltas by index or by global id (id mode).  Entry points call their rule after the argument checks.
+
+// 1. Refused in entity-table mode: the calls that bypass the table (positions, counts, global ids, a slab).
+chd_status chd_rule_not_table(chd_engine* e, const char* fn) {
+    if (!e->tbl.on) return CHD_OK;
+    return refuse(e, "%s is not available in entity-table mode (chd_entity_table_init): use chd_spawn_entities / chd_move_entities / chd_despawn_entities", fn);
 }
 
-chd_status chd_table_slab_check(chd_engine* e, const char* fn) {
+// 2. The multi-GPU calls take entity-table mode only on an engine made a slab before chd_entity_table_init.
+chd_status chd_rule_table_on_slab(chd_engine* e, const char* fn) {
     if (!e->tbl.on || e->slab) return CHD_OK;
-    e->fail("%s in entity-table mode needs an engine made a slab (chd_set_slab / chd_comm_init) before chd_entity_table_init", fn);
-    return CHD_ERR_STATE;
+    return refuse(e, "%s in entity-table mode needs an engine made a slab (chd_set_slab / chd_comm_init) before chd_entity_table_init", fn);
+}
+
+// 3. The calls by id need entity-table mode.
+chd_status chd_rule_table(chd_engine* e, const char* fn) { return e->tbl.on ? CHD_OK : refuse(e, "%s before chd_entity_table_init", fn); }
+
+// 4. Entity-table mode starts on a fresh engine; a slab may come first (that is how a table engine becomes a rank of a sharded
+// world).  delta_blocked without a slab: chd_set_entity_ids was called, perhaps with NULL.
+chd_status chd_rule_fresh_engine(chd_engine* e) {
+    if (e->tbl.on || e->built || e->assigned || e->n_own || e->pf_pos.staged >= 0 || e->have_gid || (e->delta_blocked && !e->slab) || e->dl.ids)
+        return refuse(e, "chd_entity_table_init needs a fresh engine (no entities set, assigned or built, no chd_set_entity_ids / chd_export_border / "
+                         "chd_reserve_visible_delta_ids; chd_set_slab / chd_comm_init may come first)");
+    return CHD_OK;
+}
+
+// 5. Index-mode deltas are single-GPU only (halo indices are not stable): refused after delta_blocked unless id mode is on.
+chd_status chd_rule_index_delta(chd_engine* e) {
+    if (!e->delta_blocked || e->dl.ids) return CHD_OK;
+    return refuse(e, "index-mode visible deltas are single-GPU only: this engine used chd_set_slab / chd_set_entity_ids / chd_comm_init "
+                     "(chd_reserve_visible_delta_ids names entities by global id instead)");
+}
+
+// 6. Id mode never follows index mode and keeps its id_space.  In entity-table mode it is the delta mode of slab engines: on one
+// GPU the index-mode deltas already name ids.
+chd_status chd_rule_id_delta(chd_engine* e, uint32_t id_space) {
+    if (e->tbl.on && !e->slab) return chd_rule_not_table(e, "chd_reserve_visible_delta_ids on an engine that is not a slab");
+    if (e->dl.on && !e->dl.ids)
+        return refuse(e, "chd_reserve_visible_delta_ids: this engine's visible deltas are in index mode (chd_reserve_visible_delta came first)");
+    if (!e->dl.on || id_space == e->dl.id_space) return CHD_OK;
+    e->fail("chd_reserve_visible_delta_ids: id_space %u differs from the %u the mode was set up with", id_space, e->dl.id_space);
+    return CHD_ERR_INVALID;
+}
+
+// 7 (after 5). A delta runs after a reserve, in id mode with global ids, on a build of the current state (will_build: built first).
+chd_status chd_delta_check(chd_engine* e, bool will_build) {
+    if (chd_rule_index_delta(e) != CHD_OK) return CHD_ERR_STATE;
+    if (!e->dl.on) return refuse(e, "visible delta before chd_reserve_visible_delta");
+    if (e->dl.ids && !e->have_gid && !e->tbl.on) return refuse(e, "id-mode visible delta on an engine without global ids (chd_set_entity_ids)");
+    if (will_build) return CHD_OK;
+    // id mode: the ids scattered by the delta must be those the build sorted
+    if (e->dl.ids && e->entities_dirty)
+        return refuse(e, "id-mode visible delta needs a chd_build after the last chd_set_entities / chd_set_entity_ids / chd_import_halo");
+    // chd_assign_cells rewrote the keys since the last build: keys and cell CSR no longer describe one state
+    if (!e->built || (e->assigned && e->entities_dirty)) return refuse(e, "visible delta needs a chd_build of the current cell assignment");
+    // entity-table mode: the ids the lists are translated with must be those of the build the delta measures
+    if (e->tbl.on && e->entities_dirty) return refuse(e, "visible delta needs a chd_build after the last spawn / move / despawn");
+    return CHD_OK;
+}
+
+// 8. The halo import appends to a cell assignment, and its records name entities by global id.
+chd_status chd_rule_halo_import(chd_engine* e) {
+    if (!e->assigned) return refuse(e, "chd_import_halo before chd_export_border / chd_assign_cells");
+    return e->have_gid || e->tbl.on ? CHD_OK : refuse(e, "chd_import_halo requires global entity ids (chd_set_entity_ids or entity-table mode)");
 }
 
 chd_status chd_entity_table_init(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
+    if (chd_rule_fresh_engine(e) != CHD_OK) return CHD_ERR_STATE;
     chd_engine::Table& t = e->tbl;
-    // a slab (chd_set_slab / chd_comm_init) may come first: that is how a table engine becomes a rank of a sharded world
-    if (t.on || e->built || e->assigned || e->n_own || e->pf_pos.staged >= 0 || e->have_gid || (e->delta_blocked && !e->slab) || e->dl.ids) {
-        e->fail("chd_entity_table_init needs a fresh engine (no entities set, assigned or built, no chd_set_entity_ids / chd_export_border / "
-                "chd_reserve_visible_delta_ids; chd_set_slab / chd_comm_init may come first)");
-        return CHD_ERR_STATE;
-    }
     CU(e, cudaSetDevice(e->device));
     const uint64_t N = e->lim.max_entities;
     uint32_t bits = 4;
@@ -294,13 +343,12 @@ chd_status chd_spawn_entities_f32(chd_engine* e, const uint32_t* id, const float
 
 chd_status chd_despawn_entities(chd_engine* e, const uint32_t* id_in, uint32_t n, uint8_t* out_status) {
     if (!e || (n && !id_in)) return CHD_ERR_INVALID;
-    chd_status st = need_table(e, "chd_despawn_entities");
-    if (st != CHD_OK) return st;
+    if (chd_rule_table(e, "chd_despawn_entities") != CHD_OK) return CHD_ERR_STATE;
     CU(e, cudaSetDevice(e->device));
     chd_engine::Table& t = e->tbl;
     std::vector<uint32_t> kid;
     const uint32_t* ids = nullptr;
-    st = host_view(e, id_in, n, kid, &ids);
+    chd_status st = host_view(e, id_in, n, kid, &ids);
     if (st != CHD_OK) return st;
     std::vector<uint8_t> status(n, (uint8_t)CHD_EV_OK);
     std::vector<uint32_t> aid, aslot;
@@ -354,8 +402,7 @@ chd_status chd_move_entities_f32(chd_engine* e, const uint32_t* id, const float*
 
 chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out) {
     if (!e || !out) return CHD_ERR_INVALID;
-    chd_status st = need_table(e, "chd_get_entity_stats");
-    if (st != CHD_OK) return st;
+    if (chd_rule_table(e, "chd_get_entity_stats") != CHD_OK) return CHD_ERR_STATE;
     CU(e, cudaSetDevice(e->device));
     const chd_engine::Table& t = e->tbl;
     uint64_t* h64 = reinterpret_cast<uint64_t*>(e->h_get);
@@ -374,8 +421,7 @@ chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out) {
 
 chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank, double* x, double* z, uint32_t cap, uint32_t* count) {
     if (!e || !count || (cap && (!id || !dst_rank || !x || !z))) return CHD_ERR_INVALID;
-    chd_status st = need_table(e, "chd_handoff_entities");
-    if (st != CHD_OK) return st;
+    if (chd_rule_table(e, "chd_handoff_entities") != CHD_OK) return CHD_ERR_STATE;
     if (!e->assigned) {
         // the keys must describe the current positions: a spawn, move, despawn or hand-off since the last assignment changed them
         e->fail("chd_handoff_entities needs a cell assignment after the last spawn / move / despawn / hand-off (chd_export_border, "
@@ -390,12 +436,12 @@ chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank,
     // the list goes to the event staging (free between calls: every user is on this stream) and the radix sort's temporaries
     uint32_t *d_id = t.d_ev, *d_slot = t.d_ev + N, *d_dst = e->d_tmp_val;
     double *d_hx = t.d_ev_pos, *d_hz = t.d_ev_pos + N;
-    st = chd_epoch_tick(e, s, EP_BORDER);
+    chd_status st = chd_epoch_tick(e, s, EP_BORDER);
     if (st != CHD_OK) return st;
     bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_BORDER);
     KCHECK(e);
     SCAN(e, compact_1p(HandoffFlag{e->g, e->d_key},
-                       HandoffSink{e->g, world, e->d_key, t.d_id_of_slot, e->d_x, e->d_z, d_id, d_slot, d_dst, d_hx, d_hz, e->d_boff}, e->n_own,
+                       HandoffSink{e->g, world, e->d_key, chd_entity_ids(e), e->d_x, e->d_z, d_id, d_slot, d_dst, d_hx, d_hz, e->d_boff}, e->n_own,
                        e->site_border, s));
     st = chd_read_u32(e, e->d_boff, count);
     if (st != CHD_OK) return st;
@@ -433,21 +479,22 @@ chd_status chd_table_after_build(chd_engine* e, cudaStream_t s) {
     if (!t.on) return CHD_OK;
     // on slabs the build's length (own slots + halo records) lives on the device
     const uint32_t* n_ptr = e->halo_on_device ? e->d_n_build : nullptr;
-    const uint32_t n = e->halo_on_device ? e->lim.max_entities : e->n_own + e->n_halo, own = e->n_own;
+    const uint32_t n = e->halo_on_device ? e->lim.max_entities : e->n_own + e->n_halo;
+    const EntityIds ids = chd_entity_ids(e);
     const bool raw = t.ho_raw;
-    const uint64_t key = stage_key(0x7461626c65ull, n, n_ptr, own, e->d_gid, raw, e->d_sorted_ent, t.d_sorted_id, t.d_id_of_slot, e->ho_cap);
+    const uint64_t key = stage_key(0x7461626c65ull, n, n_ptr, ids.own, ids.gid, raw, e->d_sorted_ent, t.d_sorted_id, ids.own_ids, e->ho_cap);
     const unsigned grid = (unsigned)e->sm_count * 4;
     chd_status st = run_stage(e, s, t.g_post, key, [&]() -> chd_status {
-        tbl_gather_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(e->d_sorted_ent, t.d_id_of_slot, e->d_gid, own, n, n_ptr, t.d_sorted_id, t.d_build_seq);
+        tbl_gather_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(e->d_sorted_ent, ids, n, n_ptr, t.d_sorted_id, t.d_build_seq);
         KCHECK(e);
         if (!raw) return CHD_OK;
         const HandoverOut ho{e->d_ho_entity, e->d_ho_src, e->d_ho_dst, &e->d_ctr->n_handover, e->ho_cap};
         tbl_handover_stash_kernel<<<grid, TBL_THREADS, 0, s>>>(ho, t.d_ho_tmp, t.d_build_seq + 1);
         KCHECK(e);
         CU(e, cudaMemsetAsync(&e->d_ctr->n_handover, 0, 4, s));
-        tbl_handover_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(ho, t.d_ho_tmp, t.d_build_seq + 1, t.d_flag, t.d_id_of_slot);
+        tbl_handover_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(ho, t.d_ho_tmp, t.d_build_seq + 1, t.d_flag, ids);
         KCHECK(e);
-        if (own) CU(e, cudaMemsetAsync(t.d_flag, 0, own, s));
+        if (e->n_own) CU(e, cudaMemsetAsync(t.d_flag, 0, e->n_own, s));
         return CHD_OK;
     });
     if (st != CHD_OK) return st;
@@ -461,10 +508,11 @@ chd_status chd_table_delta_ids(chd_engine* e, cudaStream_t s) {
     chd_engine::Table& t = e->tbl;
     const chd_engine::Delta& D = e->dl;
     const unsigned grid = (unsigned)e->sm_count * 8;
-    tbl_delta_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(D.enter_off, D.leave_off, D.n_out, D.enter_cap, D.leave_cap, D.enter, D.leave, t.d_id_of_slot, t.d_snap_id,
+    const EntityIds ids = chd_entity_ids(e);  // (index mode runs on one GPU: every position is a slot below the high-water mark)
+    tbl_delta_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(D.enter_off, D.leave_off, D.n_out, D.enter_cap, D.leave_cap, D.enter, D.leave, ids, t.d_snap_id,
                                                       t.d_build_seq, &e->d_ctr->delta_build);
     KCHECK(e);
-    tbl_delta_commit_kernel<<<grid, TBL_THREADS, 0, s>>>(D.enter_off, D.leave_off, D.n_out, D.enter_cap, D.leave_cap, t.d_id_of_slot, e->n_sorted, t.d_snap_id);
+    tbl_delta_commit_kernel<<<grid, TBL_THREADS, 0, s>>>(D.enter_off, D.leave_off, D.n_out, D.enter_cap, D.leave_cap, ids, e->n_sorted, t.d_snap_id);
     KCHECK(e);
     return CHD_OK;
 }

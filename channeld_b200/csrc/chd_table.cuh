@@ -105,20 +105,13 @@ __global__ void __launch_bounds__(TBL_THREADS) tbl_move_apply_kernel(const uint3
     tbl_block_count(stats + 2, superseded);
 }
 
-// The id of build position p: a slot's table id below `own` (the high-water mark), a halo record's id (gid, written by the
-// import) from there on.  Halo ids never enter id_of_slot: a later spawn into such a position must not inherit one.
-__device__ __forceinline__ uint32_t tbl_id_at(const uint32_t* __restrict__ id_of_slot, const uint32_t* __restrict__ gid, uint32_t own, uint32_t p) {
-    return p < own ? id_of_slot[p] : gid[p];
-}
-
 // After a build: sorted_id[i] = id of sorted position i (what the emit kernels and the read-back see); advances the device build
 // number.  n_ptr: the build's length lives on the device (own + halo), n is then the capacity.
-__global__ void __launch_bounds__(TBL_THREADS) tbl_gather_ids_kernel(const uint32_t* __restrict__ sorted_slot, const uint32_t* __restrict__ id_of_slot,
-                                                                     const uint32_t* __restrict__ gid, uint32_t own, uint32_t n, const uint32_t* __restrict__ n_ptr,
-                                                                     uint32_t* __restrict__ sorted_id, uint32_t* build_seq) {
+__global__ void __launch_bounds__(TBL_THREADS) tbl_gather_ids_kernel(const uint32_t* __restrict__ sorted_slot, EntityIds ids, uint32_t n,
+                                                                     const uint32_t* __restrict__ n_ptr, uint32_t* __restrict__ sorted_id, uint32_t* build_seq) {
     if (blockIdx.x == 0 && threadIdx.x == 0) *build_seq += 1;
     const uint32_t m = n_ptr ? min(*n_ptr, n) : n;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) sorted_id[i] = tbl_id_at(id_of_slot, gid, own, sorted_slot[i]);
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < m; i += gridDim.x * blockDim.x) sorted_id[i] = ids.at(sorted_slot[i]);
 }
 
 // chd_handoff_entities, one compaction (compact_1p): the own in-world slots whose column lies outside this rank's slab, with their
@@ -137,13 +130,13 @@ struct HandoffSink {
     GridDev g;
     uint32_t world;
     const uint32_t* __restrict__ key;
-    const uint32_t* __restrict__ id_of_slot;
+    EntityIds ids;
     const double *__restrict__ px, *__restrict__ pz;
     uint32_t *__restrict__ id, *__restrict__ slot, *__restrict__ dst;
     double *__restrict__ x, *__restrict__ z;
     uint32_t* __restrict__ count;
     __device__ __forceinline__ void operator()(uint64_t i, uint32_t k) const {
-        id[k] = id_of_slot[i];
+        id[k] = ids.at((uint32_t)i);
         slot[k] = (uint32_t)i;
         dst[k] = slab_owner(key[i] % g.cols, g.cols, world);
         x[k] = px[i];
@@ -166,7 +159,7 @@ __global__ void __launch_bounds__(TBL_THREADS) tbl_handover_stash_kernel(Handove
 // Handover list, pass 2 (count zeroed in between): keep the moved entities that were neither spawned nor despawned since the
 // previous assignment, named by id.
 __global__ void __launch_bounds__(TBL_THREADS) tbl_handover_ids_kernel(HandoverOut ho, const uint32_t* __restrict__ tmp, const uint32_t* __restrict__ tmp_n,
-                                                                       const uint8_t* __restrict__ flag, const uint32_t* __restrict__ id_of_slot) {
+                                                                       const uint8_t* __restrict__ flag, EntityIds ids) {
     const uint32_t n = *tmp_n, lane = threadIdx.x & 31;
     for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {  // (warp-uniform trip count)
         const uint32_t i = base + threadIdx.x;
@@ -177,7 +170,7 @@ __global__ void __launch_bounds__(TBL_THREADS) tbl_handover_ids_kernel(HandoverO
         if (lane == 0 && m) at = atomicAdd(ho.count, (uint32_t)__popc(m));
         at = __shfl_sync(0xffffffffu, at, 0) + __popc(m & ((1u << lane) - 1u));
         if (keep) {
-            ho.entity[at] = id_of_slot[s];
+            ho.entity[at] = ids.at(s);
             ho.src_cell[at] = tmp[ho.cap + i];
             ho.dst_cell[at] = tmp[2ull * ho.cap + i];
         }
@@ -188,23 +181,21 @@ __global__ void __launch_bounds__(TBL_THREADS) tbl_handover_ids_kernel(HandoverO
 // ids (snapshot ids for leave: a despawned slot's id is gone from id_of_slot).  Only if both lists fitted; then the build number
 // the delta measured is published in the counters (a quarantined slot is released once the host has read it).
 __global__ void __launch_bounds__(TBL_THREADS) tbl_delta_ids_kernel(const uint64_t* __restrict__ enter_off, const uint64_t* __restrict__ leave_off, uint32_t n_out,
-                                                                    uint64_t enter_cap, uint64_t leave_cap, uint32_t* enter, uint32_t* leave,
-                                                                    const uint32_t* __restrict__ id_of_slot, const uint32_t* __restrict__ snap_id,
-                                                                    const uint32_t* __restrict__ build_seq, uint32_t* ok_build) {
+                                                                    uint64_t enter_cap, uint64_t leave_cap, uint32_t* enter, uint32_t* leave, EntityIds ids,
+                                                                    const uint32_t* __restrict__ snap_id, const uint32_t* __restrict__ build_seq, uint32_t* ok_build) {
     const uint64_t ne = enter_off[n_out], nl = leave_off[n_out];
     if (ne > enter_cap || nl > leave_cap) return;
     const uint64_t first = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (uint64_t)gridDim.x * blockDim.x;
     if (first == 0) *ok_build = *build_seq;
-    for (uint64_t j = first; j < ne; j += stride) enter[j] = id_of_slot[enter[j]];
+    for (uint64_t j = first; j < ne; j += stride) enter[j] = ids.at(enter[j]);
     for (uint64_t j = first; j < nl; j += stride) leave[j] = snap_id[leave[j]];
 }
 
 // ... and, after the translation, the snapshot's ids advance with the snapshot (same condition as delta_advance_kernel)
 __global__ void __launch_bounds__(TBL_THREADS) tbl_delta_commit_kernel(const uint64_t* __restrict__ enter_off, const uint64_t* __restrict__ leave_off, uint32_t n_out,
-                                                                       uint64_t enter_cap, uint64_t leave_cap, const uint32_t* __restrict__ id_of_slot, uint32_t n,
-                                                                       uint32_t* __restrict__ snap_id) {
+                                                                       uint64_t enter_cap, uint64_t leave_cap, EntityIds ids, uint32_t n, uint32_t* __restrict__ snap_id) {
     if (enter_off[n_out] > enter_cap || leave_off[n_out] > leave_cap) return;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) snap_id[i] = id_of_slot[i];
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) snap_id[i] = ids.at(i);
 }
 
 __global__ void __launch_bounds__(TBL_THREADS) tbl_park_kernel(double* px, double* pz, uint32_t n) {

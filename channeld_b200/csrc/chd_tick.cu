@@ -448,10 +448,7 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
         e->fail("chd_tick: a query batch was given while chd_begin_interest is pending");
         return CHD_ERR_STATE;
     }
-    if (do_delta) {
-        st = chd_delta_check(e, need_build);
-        if (st != CHD_OK) return st;
-    }
+    if (do_delta && chd_delta_check(e, need_build) != CHD_OK) return CHD_ERR_STATE;
     if (!started && !((q || do_fanout) && (need_build || do_emit))) {
         if (need_build) {
             st = chd_build_on(e, s);

@@ -160,6 +160,14 @@ struct ScatterExtras {
     uint32_t* n_in_world;
 };
 
+// The id build position p carries (chd_entity_ids): below `own` an entity-table slot's, else gid's (global ids, and the halo ids
+// the import writes) or p without gid.  Halo ids never enter own_ids: a later spawn into such a position must not inherit one.
+struct EntityIds {
+    const uint32_t *__restrict__ own_ids, *__restrict__ gid;
+    uint32_t own;
+    __device__ __forceinline__ uint32_t at(uint32_t p) const { return p < own ? own_ids[p] : (gid ? gid[p] : p); }
+};
+
 struct BcastDev {
     uint32_t n;
     const uint32_t *channel, *flags, *sender, *client;

@@ -392,53 +392,6 @@ def test_statuses_and_counters(chd):
     assert c.engine.get_cells()[1].tolist() == [43]
 
 
-@gpu
-def test_mode_rules(chd):
-    """In table mode every snapshot and multi-GPU entry point returns CHD_ERR_STATE; chd_entity_table_init does after a build."""
-    cap = chd.capi
-    L = cap.lib()
-    wc = chd.synth.CONFIGS["2x2"]
-    e = chd.engine.Engine(wc.cfg(), 16, 2)
-    assert L.chd_get_entity_stats(e.h, C.byref(cap.EntityStats())) == cap.ERR_STATE
-    assert L.chd_spawn_entities(e.h, None, None, None, 0, None) == cap.ERR_STATE
-    p, n = C.c_void_p(), C.c_uint64()
-    assert L.chd_device_view(e.h, cap.VIEW_ENTITY_ID, C.byref(p), C.byref(n)) == cap.ERR_STATE
-    e.entity_table_init()
-    assert L.chd_entity_table_init(e.h) == cap.ERR_STATE
-    x, z = np.zeros(4), np.zeros(4)
-    xf, zf = np.zeros(4, np.float32), np.zeros(4, np.float32)
-    gid = np.arange(4, dtype=np.uint32)
-    uid = (C.c_uint8 * 128)()
-    b, keep = chd.engine.make_batch(0)
-    calls = {
-        "chd_set_entities": lambda: L.chd_set_entities(e.h, cap.ptr(x), cap.ptr(z), 4),
-        "chd_prefetch_entities": lambda: L.chd_prefetch_entities(e.h, cap.ptr(x), cap.ptr(z), 4),
-        "chd_set_entities_f32": lambda: L.chd_set_entities_f32(e.h, cap.ptr(xf), cap.ptr(zf), 4),
-        "chd_prefetch_entities_f32": lambda: L.chd_prefetch_entities_f32(e.h, cap.ptr(xf), cap.ptr(zf), 4),
-        "chd_entity_buffers": lambda: L.chd_entity_buffers(e.h, None, None, None),
-        "chd_set_entity_count": lambda: L.chd_set_entity_count(e.h, 4),
-        "chd_set_entity_ids": lambda: L.chd_set_entity_ids(e.h, cap.ptr(gid), 4),
-        "chd_set_slab": lambda: L.chd_set_slab(e.h, 0, 1, 1),
-        "chd_comm_init": lambda: L.chd_comm_init(e.h, uid, 0, 1, 1, 16, 0, 0),
-        "chd_export_border": lambda: L.chd_export_border(e.h, None, 0, None),
-        "chd_import_halo": lambda: L.chd_import_halo(e.h, None, 0, 0, 0),
-        "chd_tick_sharded": lambda: L.chd_tick_sharded(e.h, C.byref(b), 0, cap.TICK_ALL, None),
-    }
-    for name, f in calls.items():
-        assert f() == cap.ERR_STATE, name
-    # a standalone delta needs a build after the last event
-    e.reserve_visible_delta(64)
-    e.spawn_entities([1], [0.0], [0.0])
-    assert L.chd_visible_delta(e.h) == cap.ERR_STATE
-    e.build()
-    assert L.chd_visible_delta(e.h) == cap.OK
-    assert L.chd_device_view(e.h, cap.VIEW_ENTITY_ID, C.byref(p), C.byref(n)) == cap.OK and n.value == 1
-    f = chd.engine.Engine(wc.cfg(), 16, 2)
-    f.set_entities(x, z)
-    f.build()
-    assert L.chd_entity_table_init(f.h) == cap.ERR_STATE
-
-
 def _run_arrays(chd, oracle, w, graphs, ticks=8):
     e = table_engine(chd, w, graphs)
     m = Model(w.N, deltas=True)

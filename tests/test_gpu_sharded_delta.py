@@ -364,50 +364,3 @@ def test_ovf_delta_then_reserve_recovers_in_id_mode(chd):
     assert st == chd.capi.OK and s.overflow == 0
     _check_delta(e.get_visible_delta(), EMPTY, e.get_visible())
     e.close()
-
-
-def test_id_mode_state_errors(chd):
-    wc, x, z, idx = _world(chd, 2_000, 200)
-    N, S = wc.n_entities, wc.n_subscribers
-    L = chd.capi.lib()
-
-    def status(call):
-        with pytest.raises(chd.capi.ChdError) as ei:
-            call()
-        return ei.value.status
-
-    # id mode after index mode
-    e = chd.engine.Engine(wc.cfg(), N, S)
-    e.reserve_visible_delta(64)
-    assert status(lambda: e.reserve_visible_delta_ids(64, N)) == chd.capi.ERR_STATE
-    e.close()
-    # in entity-table mode, and entity-table mode after id mode
-    e = chd.engine.Engine(wc.cfg(), N, S)
-    e.entity_table_init()
-    assert status(lambda: e.reserve_visible_delta_ids(64, N)) == chd.capi.ERR_STATE
-    e.close()
-    e = chd.engine.Engine(wc.cfg(), N, S)
-    e.reserve_visible_delta_ids(64, N)
-    assert status(e.entity_table_init) == chd.capi.ERR_STATE
-    e.close()
-    # without ids for the own entities
-    e = chd.engine.Engine(wc.cfg(), N, S)
-    e.set_subscribers(np.arange(1, S + 1, dtype=np.uint32))
-    e.reserve_visible_delta_ids(1 << 16, N)
-    e.set_entities(x, z)
-    batch, keep = _batch(chd, np.arange(S), x[idx], z[idx], np.full(S, wc.radius))
-    assert status(lambda: e.tick(batch, 0, DELTA_FLAGS)) == chd.capi.ERR_STATE
-    e.build()
-    assert status(e.visible_delta) == chd.capi.ERR_STATE
-    # with ids, but set after the last build: a standalone delta needs a build first
-    e.set_entity_ids(np.arange(N, dtype=np.uint32))
-    assert status(e.visible_delta) == chd.capi.ERR_STATE
-    e.build()
-    e.update_interest(batch, 0)
-    e.visible_delta()
-    assert e.visible_delta_counts()[0] > 0
-    e.close()
-    # argument checks
-    e = chd.engine.Engine(wc.cfg(), N, S)
-    assert L.chd_reserve_visible_delta_ids(e.h, 64, 0) == chd.capi.ERR_INVALID
-    e.close()

@@ -429,22 +429,3 @@ def test_delta_through_the_controller(chd):
         _assert_delta(c.GetVisibleDelta(), want)
         _assert_delta(c.GetVisibleDelta(), want)  # a second read returns the same delta
         prev = now
-
-
-def test_delta_is_single_gpu_only(chd):
-    wc, x, z, idx, r = _world(chd, "benchmark", 30_000, 3_000)
-    S = wc.n_subscribers
-    for block in ("slab", "ids"):
-        e = chd.engine.Engine(wc.cfg(), wc.n_entities, S)
-        e.set_subscribers(np.arange(1, S + 1, dtype=np.uint32))
-        e.reserve_visible_delta(1024)
-        if block == "slab":
-            e.set_slab(0, wc.cols, 0)
-        else:
-            e.set_entity_ids(np.arange(len(x), dtype=np.uint32))
-        e.set_entities(x, z)
-        for call in (lambda: e.reserve_visible_delta(1024), e.visible_delta,
-                     lambda: e.tick(_batch(chd, idx, x, z, r)[0], 0, chd.capi.TICK_BUILD | chd.capi.TICK_VISIBLE_DELTA)):
-            with pytest.raises(chd.capi.ChdError) as ei:
-                call()
-            assert ei.value.status == chd.capi.ERR_STATE
