@@ -746,4 +746,96 @@ uint64_t orc_baseline_run(const orc_grid* g, const double* ex, const double* ez,
     return total;
 }
 
+/* ------------------------------------------------------------------ visible-set deltas ------ */
+namespace {
+struct DeltaState {
+    const uint32_t* cell;
+    uint32_t n;
+    const uint64_t* pair_off;
+    const uint32_t* pair_cell;
+    uint32_t slots;
+    std::vector<uint32_t> start, members;  // the state's entities by cell (cell asc, entity asc)
+
+    uint32_t cell_of(uint32_t e, uint32_t cells) const { return e < n && cell[e] < cells ? cell[e] : cells; }
+    void build(uint32_t cells) {
+        start.assign(size_t(cells) + 1, 0);
+        for (uint32_t e = 0; e < n; e++)
+            if (cell[e] < cells) start[cell[e] + 1]++;
+        for (uint32_t c = 0; c < cells; c++) start[c + 1] += start[c];
+        members.resize(start[cells]);
+        std::vector<uint32_t> cur(start.begin(), start.end() - 1);
+        for (uint32_t e = 0; e < n; e++)
+            if (cell[e] < cells) members[cur[cell[e]]++] = e;
+    }
+    // slot s's cells, ascending (a slot at or above the state's slot count has none)
+    void slot_cells(uint32_t s, uint32_t cells, std::vector<uint32_t>& out) const {
+        out.clear();
+        if (s < slots)
+            for (uint64_t k = pair_off[s]; k < pair_off[s + 1]; k++)
+                if (pair_cell[k] < cells) out.push_back(pair_cell[k]);
+        std::sort(out.begin(), out.end());
+        out.erase(std::unique(out.begin(), out.end()), out.end());
+    }
+};
+
+// the members of the cells `from` in state a whose cell in state b is not marked; counts them, and stores them from out on
+uint64_t delta_side(const DeltaState& a, const std::vector<uint32_t>& from, const DeltaState& b, const std::vector<uint8_t>& mark_b,
+                    uint32_t cells, uint32_t* out) {
+    uint64_t k = 0;
+    for (uint32_t c : from)
+        for (uint32_t j = a.start[c]; j < a.start[c + 1]; j++) {
+            const uint32_t e = a.members[j];
+            const uint32_t cb = b.cell_of(e, cells);
+            if (cb < cells && mark_b[cb]) continue;
+            if (out) out[k] = e;
+            k++;
+        }
+    return k;
+}
+}  // namespace
+
+int orc_visible_delta(uint32_t cells, const uint32_t* prev_cell, uint32_t prev_n, const uint64_t* prev_pair_off, const uint32_t* prev_pair_cell,
+                      uint32_t prev_slots, const uint32_t* now_cell, uint32_t now_n, const uint64_t* now_pair_off, const uint32_t* now_pair_cell,
+                      uint32_t now_slots, uint64_t* enter_off, uint32_t* enter, uint64_t enter_cap, uint64_t* leave_off, uint32_t* leave,
+                      uint64_t leave_cap, int n_threads) {
+    if (n_threads < 1) n_threads = 1;
+    DeltaState prev{prev_cell, prev_n, prev_pair_off, prev_pair_cell, prev_slots, {}, {}};
+    DeltaState now{now_cell, now_n, now_pair_off, now_pair_cell, now_slots, {}, {}};
+    prev.build(cells);
+    now.build(cells);
+    const uint32_t n_out = std::max(prev_slots, now_slots);
+    // pass 1 counts (into the offsets, shifted by one); pass 2 writes at the scanned offsets
+    auto pass = [&](bool write) {
+        Pool::get().run(n_threads, [&](int t) {
+            const uint32_t lo = uint32_t(uint64_t(n_out) * uint64_t(t) / uint64_t(n_threads));
+            const uint32_t hi = uint32_t(uint64_t(n_out) * uint64_t(t + 1) / uint64_t(n_threads));
+            std::vector<uint8_t> mark_p(cells, 0), mark_q(cells, 0);
+            std::vector<uint32_t> P, Q;
+            for (uint32_t s = lo; s < hi; s++) {
+                prev.slot_cells(s, cells, P);
+                now.slot_cells(s, cells, Q);
+                for (uint32_t c : P) mark_p[c] = 1;
+                for (uint32_t c : Q) mark_q[c] = 1;
+                const uint64_t ne = delta_side(now, Q, prev, mark_p, cells, write && enter ? enter + enter_off[s] : nullptr);
+                const uint64_t nl = delta_side(prev, P, now, mark_q, cells, write && leave ? leave + leave_off[s] : nullptr);
+                if (!write) {
+                    enter_off[s + 1] = ne;
+                    leave_off[s + 1] = nl;
+                }
+                for (uint32_t c : P) mark_p[c] = 0;
+                for (uint32_t c : Q) mark_q[c] = 0;
+            }
+        });
+    };
+    pass(false);
+    enter_off[0] = leave_off[0] = 0;
+    for (uint32_t s = 0; s < n_out; s++) {
+        enter_off[s + 1] += enter_off[s];
+        leave_off[s + 1] += leave_off[s];
+    }
+    if ((enter && enter_off[n_out] > enter_cap) || (leave && leave_off[n_out] > leave_cap)) return ORC_ERR_CAPACITY;
+    if (enter || leave) pass(true);
+    return ORC_OK;
+}
+
 }  // extern "C"

@@ -172,6 +172,20 @@ int orc_sphere_tick(const orc_grid* g, const double* ex, const double* ez, uint3
                     uint32_t* status, uint64_t* pair_off, uint32_t* pair_cell, uint32_t* pair_dist, uint64_t pair_cap,
                     uint64_t* vis_off, uint32_t* vis_entity, uint64_t vis_cap, int n_threads);
 
+/* ---- derived: visible-set deltas between two states (the definition, not the CUDA path's arrival / departure method) ----
+ * A state is a cell per entity (cell[e] >= cells: out of the world) over n entities and its pairs as a CSR by slot of cell INDICES
+ * (pair_off[n_slots+1], pair_cell[]).  With P_s, Q_s = slot s's cells at `prev` and `now`:
+ *   entered(s) = { e : cell_now(e) in Q_s and cell_prev(e) not in P_s }
+ *   left(s)    = { e : cell_prev(e) in P_s and cell_now(e) not in Q_s }
+ * An entity with no cell in a state, or at or above that state's entity count, is in no set of it.  Output: CSRs by slot over
+ * max(prev_slots, now_slots) slots (u64 offsets), each list cell ascending, then entity ascending.  enter / leave may be NULL to only
+ * count (the offsets are written either way).  Returns 0, or ORC_ERR_CAPACITY (nothing written past enter_cap / leave_cap).
+ * The slots are split over n_threads threads of the pool. */
+int orc_visible_delta(uint32_t cells, const uint32_t* prev_cell, uint32_t prev_n, const uint64_t* prev_pair_off, const uint32_t* prev_pair_cell,
+                      uint32_t prev_slots, const uint32_t* now_cell, uint32_t now_n, const uint64_t* now_pair_off, const uint32_t* now_pair_cell,
+                      uint32_t now_slots, uint64_t* enter_off, uint32_t* enter, uint64_t enter_cap, uint64_t* leave_off, uint32_t* leave,
+                      uint64_t leave_cap, int n_threads);
+
 /* Timed CPU baseline: for queries [q_begin,q_end) run the per-query map-building QueryChannelIds and
  * copy every visible entity index into a per-thread scratch list (the work the reference's fan-out
  * implies), using cell lists built from all n_ent entities (build != 0: rebuilt inside the call, in parallel over n_threads;

@@ -109,6 +109,9 @@ class Oracle:
         L.orc_sphere_tick.restype = C.c_int
         L.orc_sphere_tick.argtypes = [C.POINTER(Grid), f64p, f64p, C.c_uint32, f64p, f64p, f64p, C.c_uint32,
                                       u32p, u64p, u32p, u32p, C.c_uint64, u64p, u32p, C.c_uint64, C.c_int]
+        L.orc_visible_delta.restype = C.c_int
+        L.orc_visible_delta.argtypes = [C.c_uint32, u32p, C.c_uint32, u64p, u32p, C.c_uint32, u32p, C.c_uint32, u64p, u32p, C.c_uint32,
+                                        u64p, u32p, C.c_uint64, u64p, u32p, C.c_uint64, C.c_int]
         L.orc_baseline_run.restype = C.c_uint64
         L.orc_baseline_run.argtypes = [C.POINTER(Grid), f64p, f64p, C.c_uint32, f64p, f64p, f64p,
                                        C.c_uint32, C.c_uint32, C.c_int, C.c_int]
@@ -229,6 +232,43 @@ class Oracle:
         assert rc == 0
         return dict(status=status, pair_off=poff, pair_cell=pc[:P], pair_dist=pd[:P], vis_off=voff, vis_entity=ve[:V])
 
+    def sphere_pairs(self, g, ex, ez, cx, cz, r):
+        """sphere_tick without the visible lists (only their offsets): -> dict(status, pair_off u64, pair_cell channel ids, pair_dist,
+        vis_off)"""
+        ex = np.ascontiguousarray(ex, np.float64); ez = np.ascontiguousarray(ez, np.float64)
+        cx = np.ascontiguousarray(cx, np.float64); cz = np.ascontiguousarray(cz, np.float64)
+        r = np.ascontiguousarray(r, np.float64)
+        nq = len(cx)
+        status = np.zeros(nq, np.uint32)
+        poff = np.zeros(nq + 1, np.uint64)
+        voff = np.zeros(nq + 1, np.uint64)
+        args = (C.byref(g), _p(ex, f64p), _p(ez, f64p), len(ex), _p(cx, f64p), _p(cz, f64p), _p(r, f64p), nq, _p(status, u32p), _p(poff, u64p))
+        self.lib.orc_sphere_tick(*args, None, None, 0, _p(voff, u64p), None, 0, 1)
+        P = int(poff[nq])
+        pc = np.zeros(max(P, 1), np.uint32); pd = np.zeros(max(P, 1), np.uint32)
+        rc = self.lib.orc_sphere_tick(*args, _p(pc, u32p), _p(pd, u32p), P, _p(voff, u64p), None, 0, 1)
+        assert rc == 0
+        return dict(status=status, pair_off=poff, pair_cell=pc[:P], pair_dist=pd[:P], vis_off=voff)
+
+    def visible_delta(self, cells, prev, now, n_threads=None):
+        """orc_visible_delta.  prev / now = (cell per entity, pair_off, pair_cell): cells >= `cells` are out of the world, pair cells
+        are cell indices.  -> (enter_off u64, enter u32, leave_off u64, leave u32) over max(slots before, slots now) slots."""
+        def state(s):
+            cell, off, pc = s
+            return (np.ascontiguousarray(cell, np.uint32), np.ascontiguousarray(off, np.uint64), np.ascontiguousarray(pc, np.uint32))
+
+        (pcl, poff, ppc), (ncl, noff, npc) = state(prev), state(now)
+        n_out = max(len(poff), len(noff)) - 1
+        eo, lo = np.zeros(n_out + 1, np.uint64), np.zeros(n_out + 1, np.uint64)
+        nt = int(n_threads or os.cpu_count() or 1)
+        args = (int(cells), _p(pcl, u32p), len(pcl), _p(poff, u64p), _p(ppc, u32p), len(poff) - 1, _p(ncl, u32p), len(ncl), _p(noff, u64p),
+                _p(npc, u32p), len(noff) - 1)
+        assert self.lib.orc_visible_delta(*args, _p(eo, u64p), None, 0, _p(lo, u64p), None, 0, nt) == OK
+        ne, nl = int(eo[-1]), int(lo[-1])
+        en, le = np.zeros(max(ne, 1), np.uint32), np.zeros(max(nl, 1), np.uint32)
+        assert self.lib.orc_visible_delta(*args, _p(eo, u64p), _p(en, u32p), ne, _p(lo, u64p), _p(le, u32p), nl, nt) == OK
+        return eo, en[:ne], lo, le[:nl]
+
     def baseline_run(self, g, ex, ez, cx, cz, r, q_begin, q_end, n_threads, build):
         return self.lib.orc_baseline_run(C.byref(g), _p(ex, f64p), _p(ez, f64p), len(ex), _p(cx, f64p), _p(cz, f64p),
                                          _p(r, f64p), q_begin, q_end, n_threads, int(build))
@@ -340,6 +380,23 @@ class OracleChannels:
         self.L.orc_channels_get_state(self._hp(), _p(chan, u32p), _p(conn, u32p), n, last.ctypes.data_as(C.POINTER(C.c_int64)),
                                       had.ctypes.data_as(C.POINTER(C.c_uint8)), _p(li, u64p), found.ctypes.data_as(C.POINTER(C.c_uint8)))
         return last, had.astype(bool), li, found.astype(bool)
+
+
+def update_pairs(prev_off, prev_cell, n_slots, slots, status, q_off, q_cell):
+    """The pairs after an interest update, as the engine keeps them: slot slots[k] takes query k's cells (q_off / q_cell, a CSR by
+    query) when status[k] == 0; a slot whose query failed, and every slot without a query, keeps its cells.  prev_off may cover fewer
+    than n_slots slots (the others had none).  -> (pair_off u64[n_slots + 1], pair_cell)"""
+    prev_off = np.asarray(prev_off, np.int64)
+    prev_off = np.concatenate([prev_off, np.full(n_slots + 1 - len(prev_off), prev_off[-1])])
+    q_off = np.asarray(q_off, np.int64)
+    lens, src = np.diff(prev_off), prev_off[:-1].copy()
+    ok = np.asarray(status) == 0
+    s_ok = np.asarray(slots, np.int64)[ok]
+    lens[s_ok] = np.diff(q_off)[ok]
+    src[s_ok] = q_off[:-1][ok] + len(prev_cell)  # in the concatenation of both cell arrays
+    buf = np.concatenate([np.asarray(prev_cell, np.uint32), np.asarray(q_cell, np.uint32)])
+    off = np.concatenate([[0], np.cumsum(lens)])
+    return off.astype(np.uint64), buf[np.repeat(src - off[:-1], lens) + np.arange(off[-1])]
 
 
 def build():
