@@ -102,6 +102,15 @@ class ResultBuffers(C.Structure):
     ]
 
 
+class DeltaBuffers(C.Structure):
+    _fields_ = [("enter_off", C.c_void_p), ("leave_off", C.c_void_p), ("enter_entity", C.c_void_p), ("leave_entity", C.c_void_p),
+                ("slot_cap", C.c_uint64), ("entity_cap", C.c_uint64)]
+
+
+class DeltaCounts(C.Structure):
+    _fields_ = [("n_entered", C.c_uint64), ("n_left", C.c_uint64), ("n_slots", C.c_uint32), ("deltas", C.c_uint32)]
+
+
 class TickSummary(C.Structure):
     _fields_ = [
         ("n_pairs", C.c_uint64), ("n_visible", C.c_uint64), ("n_entities_in_world", C.c_uint32),
@@ -137,6 +146,7 @@ SYMBOLS = [
     "chd_graph_launch_count",
     "chd_add_subscribers", "chd_remove_subscribers", "chd_fetch_results_async", "chd_fetch_wait", "chd_rings_init", "chd_rings_append", "chd_get_rings", "chd_set_channel_start_times", "chd_set_payload_bytes", "chd_assemble_payloads", "chd_frame_packets", "chd_comm_unique_id", "chd_comm_init", "chd_comm_info", "chd_comm_destroy", "chd_tick_sharded", "chd_collective_count", "chd_comm_exchange_mode", "chd_comm_use_collective", "chd_migrate_out", "chd_migrate_in", "chd_get_rehome",
     "chd_reserve_visible_delta", "chd_reserve_visible_delta_ids", "chd_visible_delta", "chd_get_visible_delta",
+    "chd_fetch_results_delta", "chd_fetch_results_async_delta", "chd_fetch_wait_delta",
     "chd_entity_table_init", "chd_spawn_entities", "chd_spawn_entities_f32", "chd_despawn_entities", "chd_move_entities", "chd_move_entities_f32",
     "chd_get_entity_stats", "chd_handoff_entities",
 ]
@@ -274,6 +284,12 @@ def lib():
     L.chd_fetch_results_async.argtypes = [vp, C.POINTER(ResultBuffers), vp]
     L.chd_fetch_wait.restype = C.c_int
     L.chd_fetch_wait.argtypes = [vp, C.POINTER(TickSummary)]
+    L.chd_fetch_results_delta.restype = C.c_int
+    L.chd_fetch_results_delta.argtypes = [vp, C.POINTER(ResultBuffers), C.POINTER(DeltaBuffers), C.POINTER(TickSummary), C.POINTER(DeltaCounts)]
+    L.chd_fetch_results_async_delta.restype = C.c_int
+    L.chd_fetch_results_async_delta.argtypes = [vp, C.POINTER(ResultBuffers), C.POINTER(DeltaBuffers), vp]
+    L.chd_fetch_wait_delta.restype = C.c_int
+    L.chd_fetch_wait_delta.argtypes = [vp, C.POINTER(TickSummary), C.POINTER(DeltaCounts)]
     L.chd_rings_init.restype = C.c_int
     L.chd_rings_init.argtypes = [vp, C.c_uint32]
     L.chd_rings_append.restype = C.c_int

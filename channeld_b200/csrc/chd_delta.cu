@@ -61,7 +61,11 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
     if (D.ids) key = stage_key(key, 0x696473ull, D.id_space, n_scatter, n_ptr, e->d_key, e->d_n_build, d.sorted);
     const unsigned grid = (unsigned)e->sm_count * 8;
     const unsigned slot_grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(blocks_for((uint64_t)D.n_out * 32, DELTA_THREADS), (uint64_t)e->sm_count * 32));
-    return run_stage(e, s, D.g, key, [&]() -> chd_status {
+    if (D.read_guard) {  // an asynchronous fetch may still be snapshotting the lists and offsets this delta rewrites
+        CU(e, cudaStreamWaitEvent(s, D.ev_read[D.read_fi], 0));
+        D.read_guard = false;
+    }
+    st = run_stage(e, s, D.g, key, [&]() -> chd_status {
         bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_DELTA);
         KCHECK(e);
         if (D.ids) {
@@ -94,6 +98,10 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
         KCHECK(e);
         return CHD_OK;
     });
+    if (st != CHD_OK) return st;
+    CU(e, cudaEventRecord(D.ev_end, s));
+    D.seq++;
+    return CHD_OK;
 }
 
 // The first reserve picks the mode (ids: id mode over [0, id_space)) and allocates; every later one only grows the lists.
@@ -102,6 +110,8 @@ static chd_status delta_reserve(chd_engine* e, uint64_t cap_entries, bool ids, u
     // a delta of an earlier tick may still be running (on the engine stream or, inside a tick, on prep_stream)
     CU(e, cudaStreamSynchronize(e->stream));
     CU(e, cudaStreamSynchronize(e->prep_stream));
+    // an asynchronous fetch may still be snapshotting the lists that ensure_cap frees
+    if (e->dl_stream_d) CU(e, cudaStreamSynchronize(e->dl_stream_d));
     chd_engine::Delta& D = e->dl;
     const uint64_t N = e->lim.max_entities, S = e->lim.max_subscribers, P = e->lim.max_pairs, C = e->g.cells;
     if (!D.on) {
@@ -115,7 +125,8 @@ static chd_status delta_reserve(chd_engine* e, uint64_t cap_entries, bool ids, u
                         dalloc(e, &D.cnt_leave, S) && dalloc(e, &D.enter_off, S + 1) && dalloc(e, &D.leave_off, S + 1) &&
                         chd_make_site(e, D.site_arr, N + 1, EP_DELTA) && chd_make_site(e, D.site_dep, N + 1, EP_DELTA) &&
                         chd_make_site(e, D.site_enter, S + 1, EP_DELTA) && chd_make_site(e, D.site_leave, S + 1, EP_DELTA) &&
-                        chd_make_event(e, &D.ev_in) && chd_make_event(e, &D.ev_done);
+                        chd_make_event(e, &D.ev_in) && chd_make_event(e, &D.ev_done) && chd_make_event(e, &D.ev_end) &&
+                        chd_make_event(e, &D.ev_read[0]) && chd_make_event(e, &D.ev_read[1]);
         if (!ok) return CHD_ERR_CUDA;
         for (ScanSite* site : {&D.site_arr, &D.site_dep, &D.site_enter, &D.site_leave}) site->error = &e->d_ctr->overflow;
         // the empty snapshot: no entities, no cells populated, no slots

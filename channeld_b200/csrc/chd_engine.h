@@ -223,6 +223,9 @@ struct chd_engine {
     uint8_t* d_fetch_stage[2] = {nullptr, nullptr};
     uint64_t fetch_stage_bytes[2] = {0, 0};
     void* fetch_header[2] = {nullptr, nullptr};
+    // the visible delta of fetch set fi: deltas it carries (0: none or no delta buffers) and n_slots; dl_stream_d: its snapshot hop
+    uint32_t fetch_deltas[2] = {0, 0}, fetch_delta_slots[2] = {0, 0};
+    cudaStream_t dl_stream_d = nullptr;
     uint64_t fetch_issued = 0, fetch_waited = 0;
     bool fetch_guard = false;
     bool early_ready = false;  // ev_join + ev_prep_done of the last tick are recorded
@@ -299,6 +302,12 @@ struct chd_engine {
         GraphSet g;
         cudaEvent_t ev_in = nullptr, ev_done = nullptr;  // two-stream tick: the build is done / the delta is done
         bool done_recorded = false;  // the last tick ran the delta off the engine stream: its end (and CHD_OVF_DELTA) is ev_done
+        // read-back (chd_fetch_results*_delta): deltas enqueued (seq) and seq at the last fetch; ev_end: recorded after every delta on
+        // its stream.  ev_read[fi]: fetch set fi's snapshot of the lists is done; the next delta waits for the latest (read_guard).
+        uint64_t seq = 0, fetched = 0;
+        cudaEvent_t ev_end = nullptr, ev_read[2] = {nullptr, nullptr};
+        bool read_guard = false;
+        int read_fi = 0;
     } dl;
     // chd_set_slab / chd_set_entity_ids / chd_comm_init were used: halo indices are not stable, no index-mode deltas (id mode is
     // not affected).  Sticky: chd_set_entity_ids(NULL) leaves no other trace, so this cannot be derived from have_gid / slab.

@@ -1,7 +1,7 @@
 /* tick_loop.c — the C ABI as a host sees it (plain C99; what the cgo shim in go/gpucontroller.go does, minus Go).
  * One engine, the pipelined tick loop of INTEGRATION.md §2: while tick k runs on the GPU the inputs of tick k+1 are
- * uploaded, and the results of tick k-1 are consumed (chd_fetch_results_async / chd_fetch_wait: the host never waits for a tick
- * before it has enqueued the next one).
+ * uploaded, and the results of tick k-1 are consumed (chd_fetch_results_async_delta / chd_fetch_wait_delta: the host never waits
+ * for a tick before it has enqueued the next one), the visible-set delta (entities each subscriber spawns / despawns) among them.
  *
  *   gcc -std=c99 -Iinclude examples/tick_loop.c -Lchanneld_b200 -lchd_b200 -Wl,-rpath,$PWD/channeld_b200 -lm -o tick_loop
  *
@@ -112,6 +112,18 @@ int main(void) {
         rb[k].sorted_entity = chd_alloc_pinned(4ull * n_entities);
         hdr[k] = chd_alloc_pinned(CHD_FETCH_HEADER_BYTES);
     }
+    /* the visible-set delta of each tick rides in the same fetch: per subscriber slot the entities entered and left */
+    const uint64_t delta_cap = 8000000; /* entries per list and tick: the first delta enters every visible entry (about 5e6 here) */
+    CHECK(chd_reserve_visible_delta(e, delta_cap));
+    chd_delta_buffers db[2];
+    for (int k = 0; k < 2; k++) {
+        db[k].slot_cap = n_subs + 1ull;
+        db[k].entity_cap = delta_cap;
+        db[k].enter_off = chd_alloc_pinned(8ull * db[k].slot_cap);
+        db[k].leave_off = chd_alloc_pinned(8ull * db[k].slot_cap);
+        db[k].enter_entity = chd_alloc_pinned(4ull * delta_cap);
+        db[k].leave_entity = chd_alloc_pinned(4ull * delta_cap);
+    }
 
 #define PREFETCH(s)                                                                                                       \
     do {                                                                                                                  \
@@ -127,25 +139,30 @@ int main(void) {
     fill_inputs(&st[0], n_entities, n_subs, cells, 0);
     PREFETCH(&st[0]);
     chd_tick_summary sum;
+    chd_delta_counts dc;
     for (int tick = 0; tick < 100; tick++) {
         const int64_t now = (int64_t)(tick + 1) * tick_ns;
         CHECK(chd_adopt_prefetched(e));            /* inputs of this tick were uploaded during the previous one */
         CHECK(chd_begin_interest(e, NULL, now, 1)); /* interest diff + fan-out pass start on the second stream */
-        CHECK(chd_tick(e, NULL, now, CHD_TICK_ALL, NULL)); /* asynchronous */
+        CHECK(chd_tick(e, NULL, now, CHD_TICK_ALL | CHD_TICK_VISIBLE_DELTA, NULL)); /* asynchronous */
         staging* next = &st[(tick + 1) & 1];
         fill_inputs(next, n_entities, n_subs, cells, tick + 1); /* the host collects tick k+1 while tick k runs */
         PREFETCH(next);
-        CHECK(chd_fetch_results_async(e, &rb[tick & 1], hdr[tick & 1])); /* returns at once: device-side sizes, pinned targets */
+        /* returns at once: device-side sizes, pinned targets */
+        CHECK(chd_fetch_results_async_delta(e, &rb[tick & 1], &db[tick & 1], hdr[tick & 1]));
         if (tick == 0) continue;
         /* results of tick - 1, while tick runs on the GPU */
-        CHECK(chd_fetch_wait(e, &sum));
+        CHECK(chd_fetch_wait_delta(e, &sum, &dc));
         /* apply from rb[(tick - 1) & 1]: sum.n_sub_new x handleSubToChannel(new_sub[i], new_channel[i]), sum.n_unsub x
-         * handleUnsubFromChannel, sum.n_due x fanOutDataUpdate(due[i]), sum.n_handover x the orchestration half of Notify */
+         * handleUnsubFromChannel, sum.n_due x fanOutDataUpdate(due[i]), sum.n_handover x the orchestration half of Notify;
+         * from db[(tick - 1) & 1]: for each slot s < dc.n_slots spawn enter_entity[enter_off[s] .. enter_off[s + 1]) and despawn
+         * leave_entity[leave_off[s] .. leave_off[s + 1]) (dc.deltas == 1: exactly this tick's delta) */
         if ((tick - 1) % 25 == 0)
-            printf("tick %d: %llu pairs, %llu visible entries, +%u/-%u subscriptions, %u sends, %u handovers\n", tick - 1,
-                   (unsigned long long)sum.n_pairs, (unsigned long long)sum.n_visible, sum.n_sub_new, sum.n_unsub, sum.n_due, sum.n_handover);
+            printf("tick %d: %llu pairs, %llu visible entries, +%u/-%u subscriptions, %u sends, %u handovers, %llu entered / %llu left\n",
+                   tick - 1, (unsigned long long)sum.n_pairs, (unsigned long long)sum.n_visible, sum.n_sub_new, sum.n_unsub, sum.n_due,
+                   sum.n_handover, (unsigned long long)dc.n_entered, (unsigned long long)dc.n_left);
     }
-    CHECK(chd_fetch_wait(e, &sum)); /* the last tick */
+    CHECK(chd_fetch_wait_delta(e, &sum, &dc)); /* the last tick */
     chd_destroy(e);
     free(conn);
     return 0;

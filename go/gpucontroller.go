@@ -407,7 +407,9 @@ func (ctl *GpuStaticGrid2DSpatialController) DueClasses(nDue int) (classOf, rep,
 
 // VisibleDelta returns, per subscriber slot, the entity indices to spawn (enter) and despawn (leave) since the last visible
 // delta: the net effect of the FULL data a new subscription sends, the despawns of an unsubscription and the handovers between
-// cells (spatial.go:612-858).  Call ReserveVisibleDelta once, then tick with CHD_TICK_VISIBLE_DELTA.  UN-RUN like the rest
+// cells (spatial.go:612-858).  Call ReserveVisibleDelta once, then tick with CHD_TICK_VISIBLE_DELTA.  VisibleDelta makes two
+// blocking calls on the engine stream: in the pipelined loop it waits for the tick in flight and returns ITS lists.  A pipelined
+// host reads the lists with the tick's other results instead: FetchResultsAsyncDelta / FetchWaitDelta.  UN-RUN like the rest
 // of this file.
 func (ctl *GpuStaticGrid2DSpatialController) ReserveVisibleDelta(capEntries uint64) error {
 	if st := C.chd_reserve_visible_delta(ctl.engine, C.uint64_t(capEntries)); st != C.CHD_OK {
@@ -550,6 +552,25 @@ func (ctl *GpuStaticGrid2DSpatialController) FetchWait() (C.chd_tick_summary, er
 		return s, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
 	}
 	return s, nil
+}
+
+// FetchResultsAsyncDelta / FetchWaitDelta: the same read-back carrying the visible-set delta of the tick (delta buffers in C
+// pinned memory as well).  counts.deltas: 0 = the tick ran no delta, 1 = these are its lists, > 1 = earlier deltas were never
+// fetched.  After CHD_OVF_DELTA the wait returns an error and counts holds the required sizes (grow with ReserveVisibleDelta).
+func (ctl *GpuStaticGrid2DSpatialController) FetchResultsAsyncDelta(buffers *C.chd_result_buffers, delta *C.chd_delta_buffers, pinnedHeader unsafe.Pointer) error {
+	if st := C.chd_fetch_results_async_delta(ctl.engine, buffers, delta, pinnedHeader); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
+func (ctl *GpuStaticGrid2DSpatialController) FetchWaitDelta() (C.chd_tick_summary, C.chd_delta_counts, error) {
+	var s C.chd_tick_summary
+	var c C.chd_delta_counts
+	if st := C.chd_fetch_wait_delta(ctl.engine, &s, &c); st != C.CHD_OK {
+		return s, c, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return s, c, nil
 }
 
 // AddSubscribers / RemoveSubscribers: connection lifecycle (subscription.go:104-125, channel.go:414-475).  The host owns the

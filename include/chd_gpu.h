@@ -515,6 +515,38 @@ chd_status chd_fetch_results(chd_engine* e, const chd_result_buffers* bufs, chd_
 chd_status chd_fetch_results_async(chd_engine* e, const chd_result_buffers* bufs, void* pinned_header);
 chd_status chd_fetch_wait(chd_engine* e, chd_tick_summary* summary);
 
+/* ---- the visible-set delta read back with the tick's other results (the three calls above are these with delta == NULL).
+ * Which delta: a fetch (sync or async) carries the most recent delta enqueued since the previous fetch on this engine, by
+ * CHD_TICK_VISIBLE_DELTA (chd_tick, chd_tick_sharded) or by a standalone chd_visible_delta.  counts->deltas says how many were
+ * enqueued: 0 = none (the counts are 0 and no delta buffer is written), 1 = these are its lists, > 1 = these are the last one's
+ * lists and the earlier ones were never fetched (the host lost them).  With deltas >= 1 the offsets and lists equal what
+ * chd_get_visible_delta returns right after that delta, in index, id and entity-table mode.
+ * Overflow: after CHD_OVF_DELTA or CHD_OVF_DELTA_IDS the counts are the required sizes and no offsets or entries are copied; the
+ * summary carries the bit and the call (sync) or chd_fetch_wait_delta (async) returns CHD_ERR_CAPACITY.
+ * Caller capacity: slot_cap counts offsets (n_slots + 1 are needed for each CSR), entity_cap entries of each list.  If a requested
+ * buffer is too small, the sync form copies no delta buffer and returns CHD_ERR_CAPACITY; the async form truncates to the capacity
+ * and chd_fetch_wait_delta returns CHD_ERR_CAPACITY.
+ * Any pointer may be NULL (delta == NULL: no delta read-back).  The async form needs pinned memory for every non-NULL buffer.
+ * Delta buffers before any chd_reserve_visible_delta*: CHD_ERR_STATE.  chd_fetch_wait_delta may wait on any fetch (counts may be
+ * NULL); a fetch issued without delta buffers reports deltas = 0.  The async counts ride in the pinned header.
+ * Device memory: the async form snapshots the delta into the same HBM staging as the other lists, so each of its two staging sets
+ * grows to up to 8 x entity_cap + 16 x slot_cap bytes more.  The snapshot starts when the delta is done, beside the expanded-list
+ * kernel; only the next delta (and chd_reserve_visible_delta*) waits for it, the next tick's other stages do not. */
+typedef struct chd_delta_buffers {
+    uint64_t *enter_off, *leave_off;        /* [slot_cap] each: n_slots + 1 offsets */
+    uint32_t *enter_entity, *leave_entity;  /* [entity_cap] each */
+    uint64_t slot_cap, entity_cap;
+} chd_delta_buffers;
+typedef struct chd_delta_counts {
+    uint64_t n_entered, n_left; /* list lengths; after CHD_OVF_DELTA(_IDS), the required sizes */
+    uint32_t n_slots;           /* as chd_get_visible_delta's *n_slots */
+    uint32_t deltas;            /* deltas enqueued since the previous fetch (see above) */
+} chd_delta_counts;
+chd_status chd_fetch_results_delta(chd_engine* e, const chd_result_buffers* bufs, const chd_delta_buffers* delta, chd_tick_summary* summary,
+                                   chd_delta_counts* counts);
+chd_status chd_fetch_results_async_delta(chd_engine* e, const chd_result_buffers* bufs, const chd_delta_buffers* delta, void* pinned_header);
+chd_status chd_fetch_wait_delta(chd_engine* e, chd_tick_summary* summary, chd_delta_counts* counts);
+
 /* Device-resident views (valid until the next call that rewrites them) for consumers that stay on the GPU. */
 enum {
     CHD_VIEW_CELL_START = 0, CHD_VIEW_SORTED_ENTITY, CHD_VIEW_ENT_CELL, CHD_VIEW_PAIR_OFF, CHD_VIEW_PAIR_CHANNEL,
