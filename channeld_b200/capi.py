@@ -24,6 +24,9 @@ DUE_VOID = 0xFFFFFFFF
 TICK_BUILD, TICK_EMIT, TICK_FANOUT, TICK_ALL = 1, 2, 4, 7
 TICK_EARLY_RESULTS = 8
 TICK_VISIBLE_DELTA = 16
+TICK_FOLLOW = 32  # the tick's batch is the one chd_follow_queries generated (batch None)
+FOLLOW_ALL, FOLLOW_MOVED = 0, 1
+FOLLOW_NOT_SELECTED, FOLLOW_NO_ENTITY = 16, 17  # beside Q_* in chd_get_follow's status
 OVF_PAIRS, OVF_WINDOW, OVF_VISIBLE, OVF_DUE, OVF_BORDER, OVF_RING = 1, 2, 4, 8, 16, 32
 OVF_DELTA = 64
 OVF_DELTA_IDS = 128
@@ -111,6 +114,12 @@ class DeltaCounts(C.Structure):
     _fields_ = [("n_entered", C.c_uint64), ("n_left", C.c_uint64), ("n_slots", C.c_uint32), ("deltas", C.c_uint32)]
 
 
+class FollowBatch(C.Structure):
+    _fields_ = [("n", C.c_uint32), ("slot", C.c_void_p), ("entity", C.c_void_p), ("kind", C.c_void_p),
+                ("sph_r", C.c_void_p), ("box_ex", C.c_void_p), ("box_ez", C.c_void_p),
+                ("cone_dx", C.c_void_p), ("cone_dz", C.c_void_p), ("cone_angle", C.c_void_p), ("cone_r", C.c_void_p)]
+
+
 class TickSummary(C.Structure):
     _fields_ = [
         ("n_pairs", C.c_uint64), ("n_visible", C.c_uint64), ("n_entities_in_world", C.c_uint32),
@@ -149,8 +158,9 @@ SYMBOLS = [
     "chd_fetch_results_delta", "chd_fetch_results_async_delta", "chd_fetch_wait_delta",
     "chd_entity_table_init", "chd_spawn_entities", "chd_spawn_entities_f32", "chd_despawn_entities", "chd_move_entities", "chd_move_entities_f32",
     "chd_get_entity_stats", "chd_handoff_entities",
+    "chd_follow_bind", "chd_follow_unbind", "chd_follow_queries", "chd_get_follow",
 ]
-STAGE_BUILD, STAGE_INTEREST, STAGE_EMIT, STAGE_EMIT_KERNEL, STAGE_FANOUT, STAGE_TICK, STAGE_EXPORT, STAGE_EXCHANGE, STAGE_IMPORT, STAGE_READBACK, STAGE_VISIBLE_DELTA, STAGE_ENTITY_EVENTS = range(12)
+STAGE_BUILD, STAGE_INTEREST, STAGE_EMIT, STAGE_EMIT_KERNEL, STAGE_FANOUT, STAGE_TICK, STAGE_EXPORT, STAGE_EXCHANGE, STAGE_IMPORT, STAGE_READBACK, STAGE_VISIBLE_DELTA, STAGE_ENTITY_EVENTS, STAGE_FOLLOW = range(13)
 
 _lib = None
 
@@ -352,6 +362,14 @@ def lib():
     L.chd_get_entity_stats.argtypes = [vp, C.POINTER(EntityStats)]
     L.chd_handoff_entities.restype = C.c_int
     L.chd_handoff_entities.argtypes = [vp, vp, vp, vp, vp, C.c_uint32, u32p]
+    L.chd_follow_bind.restype = C.c_int
+    L.chd_follow_bind.argtypes = [vp, C.POINTER(FollowBatch)]
+    L.chd_follow_unbind.restype = C.c_int
+    L.chd_follow_unbind.argtypes = [vp, vp, C.c_uint32]
+    L.chd_follow_queries.restype = C.c_int
+    L.chd_follow_queries.argtypes = [vp, C.c_uint32]
+    L.chd_get_follow.restype = C.c_int
+    L.chd_get_follow.argtypes = [vp, vp, vp, vp, vp, vp, C.c_uint32, u32p, u32p]
     _lib = L
     return L
 

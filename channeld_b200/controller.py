@@ -236,8 +236,50 @@ class GpuStaticGrid2DSpatialController:
     def MoveEntities(self, net_ids, x, z) -> None:
         self._table().move_entities(net_ids, x, z)
 
-    # -- Tick()   (channel.go:358-387 for all spatial channels at once)
-    def Tick(self, batch, t_ns, flags=capi.TICK_ALL):
+    # -- connections whose interest follows their pawn (a client "stands on its pawn"): bound once, then every Tick(None, ...,
+    # follow=...) builds the UPDATE_SPATIAL_INTEREST batch (message_spatial.go:41-129) on the device from the entities' positions.
+    # queries[i] gives the AOI SHAPE of connection slot i (SphereAOI / BoxAOI / ConeAOI, any combination); its Center is ignored,
+    # the centre is entity net_ids[i] (entity index without SpawnObjects).  SpotsAOI is absolute and cannot follow an entity.
+    def FollowEntities(self, conn_slots, net_ids, queries: Sequence[SpatialInterestQuery]) -> None:
+        n = len(queries)
+        kind = np.zeros(n, np.uint8)
+        sph_r = np.zeros(n)
+        box = [np.zeros(n) for _ in range(2)]
+        cone = [np.zeros(n) for _ in range(4)]
+        for i, q in enumerate(queries):
+            if q is None:
+                raise SpatialError("query is nil")
+            if q.SpotsAOI is not None:
+                raise SpatialError("SpotsAOI has absolute positions and cannot follow an entity")
+            if q.SphereAOI is not None:
+                kind[i] |= capi.AOI_SPHERE
+                sph_r[i] = q.SphereAOI.Radius
+            if q.BoxAOI is not None:
+                if q.BoxAOI.Extent is None:
+                    raise SpatialError("BoxAOI with nil Extent")
+                kind[i] |= capi.AOI_BOX
+                box[0][i], box[1][i] = q.BoxAOI.Extent.X, q.BoxAOI.Extent.Z
+            if q.ConeAOI is not None:
+                if q.ConeAOI.Direction is None:
+                    raise SpatialError("ConeAOI with nil Direction")
+                kind[i] |= capi.AOI_CONE
+                c = q.ConeAOI
+                cone[0][i], cone[1][i], cone[2][i], cone[3][i] = c.Direction.X, c.Direction.Z, c.Angle, c.Radius
+            if not kind[i]:
+                raise SpatialError("query without an AOI")
+        self.engine.follow_bind(conn_slots, net_ids, kind=kind, sph_r=sph_r, box=box, cone=cone)
+
+    def UnfollowEntities(self, conn_slots) -> None:
+        self.engine.follow_unbind(conn_slots)
+
+    # -- Tick()   (channel.go:358-387 for all spatial channels at once).  follow = capi.FOLLOW_ALL / FOLLOW_MOVED with batch None:
+    # the batch is generated from the FollowEntities bindings.
+    def Tick(self, batch, t_ns, flags=capi.TICK_ALL, follow=None):
+        if follow is not None:
+            if batch is not None:
+                raise SpatialError("a followed tick generates its own batch")
+            self.engine.follow_queries(follow)
+            flags |= capi.TICK_FOLLOW
         return self.engine.tick(batch, t_ns, flags)
 
     # -- per client, the entities to spawn / despawn since the last delta: the net effect of the FULL data a new subscription

@@ -9,6 +9,7 @@
 //   chd_shard.cu     multi-GPU X-slabs: border export, halo import, the NCCL exchange
 //   chd_extras.cu    window classes, ADJACENT_CHANNELS broadcast sets, config-plane helpers
 //   chd_table.cu     the mode rules; entity-table mode: spawn / move / despawn by id, the id-valued results
+//   chd_follow.cu    followers: slot -> entity bindings and the query batch generated from them
 #pragma once
 #include <cuda_runtime.h>
 
@@ -121,7 +122,7 @@ struct chd_engine {
     // one look-back scan site per call site: stages run concurrently on two streams and must not share scan state
     unsigned long long* d_epoch = nullptr;  // [EP_COUNT] stage epochs for the look-back scans
     ScanSite site_hist_b{}, site_pchist_b{}, site_hist{}, site_qoff{}, site_slot{}, site_pchist{}, site_voff{}, site_border{};
-    uint64_t stage_execs[9] = {};  // [EP_COUNT]
+    uint64_t stage_execs[10] = {};  // [EP_COUNT]
     std::vector<ScanSite*> sites;  // every scan site (chd_make_site registers them)
     uint32_t build_blocks = 0;
     bool assigned = false, built = false, have_prev_key = false, entities_dirty = false;
@@ -345,6 +346,22 @@ struct chd_engine {
         int next_stage = 0;
         GraphSet g_post;
     } tbl;
+    // ---- followers (chd_follow.cu): everything is allocated by the first chd_follow_bind
+    struct Follow {
+        bool on = false;
+        std::vector<uint8_t> h_kind;  // host mirror of st.kind (0: the slot follows nothing): argument checks, counts
+        uint32_t n_bound = 0;
+        FollowDev st{};     // per-slot bindings, [max_subscribers]
+        FollowBatch q{};    // the generated batch, [max_queries]; q.n_selected: queries in it
+        QueryDev view{};    // the generated batch as the interest stage reads it
+        bool ready = false;     // a generated batch waits for the interest update that consumes it
+        uint8_t* d_stage = nullptr;  // chd_follow_bind / chd_follow_unbind: staged arguments
+        uint64_t stage_cap = 0;
+        uint32_t *g_slot = nullptr, *g_entity = nullptr, *g_status = nullptr, *g_count = nullptr;  // chd_get_follow's lists, [max_queries]
+        double *g_cx = nullptr, *g_cz = nullptr;
+        ScanSite site{};
+        GraphSet g;
+    } fw;
 
     bool fail(const char* fmt, ...) const {
         char buf[512];
@@ -438,7 +455,7 @@ static inline bool alloc_qstage(chd_engine* e, chd_engine::QStage& qs) {
            dalloc(e, &qs.spot_x, SP) && dalloc(e, &qs.spot_z, SP) && dalloc(e, &qs.spot_dist, SP);
 }
 
-enum { EP_BUILD = 0, EP_QUERY, EP_EMIT, EP_FANOUT, EP_BORDER, EP_BCAST, EP_CLASS, EP_PAYLOAD, EP_DELTA, EP_COUNT };  // d_epoch has EP_COUNT slots
+enum { EP_BUILD = 0, EP_QUERY, EP_EMIT, EP_FANOUT, EP_BORDER, EP_BCAST, EP_CLASS, EP_PAYLOAD, EP_DELTA, EP_FOLLOW, EP_COUNT };  // d_epoch has EP_COUNT slots
 static_assert(EP_COUNT == sizeof(chd_engine::stage_execs) / sizeof(uint64_t), "one execution counter per stage epoch");
 
 // ---- helpers shared by the translation units (C linkage only so that definitions may sit inside their extern "C" blocks)
@@ -497,6 +514,12 @@ chd_status chd_rule_index_delta(chd_engine* e);
 chd_status chd_rule_id_delta(chd_engine* e, uint32_t id_space);
 chd_status chd_delta_check(chd_engine* e, bool will_build);
 chd_status chd_rule_halo_import(chd_engine* e);
+chd_status chd_rule_follow(chd_engine* e, const char* fn);
+chd_status chd_rule_no_followers(chd_engine* e, const char* fn);
+chd_status chd_rule_one_batch(chd_engine* e, const char* fn);
+// followers (chd_follow.cu): the listed slots (n == 0 with slot == nullptr: every slot) follow nothing from now on; d_slot: the
+// same list on the device if the caller uploaded it already
+chd_status chd_follow_drop(chd_engine* e, const uint32_t* slot, const uint32_t* d_slot, uint32_t n);
 // entity-table mode (chd_table.cu): the pass after every table-mode build (sorted ids, handover list in ids); the delta's
 // translation to ids, inside its stage; a decoded summary's last successful delta
 chd_status chd_table_after_build(chd_engine* e, cudaStream_t s);

@@ -1,0 +1,253 @@
+// chd_follow.cu — followers: subscriber slots bound to an entity and an AOI shape, and the tick's query batch generated from the
+// bindings on the device (chd_follow.cuh).
+//
+// One generated batch is enough (chd_prefetch_queries needs two staging sets because its uploads run on another stream while a
+// tick is in flight): the generation runs on the engine stream, and the interest update that reads the batch is either on the
+// engine stream too or on the second stream between the tick's fork and its join, which the engine stream waits for before the
+// tick ends.  A generation enqueued after that tick is therefore ordered after the last read of the batch; while a
+// chd_begin_interest is pending (forked, not joined yet) chd_follow_queries is refused.  The generation writes follower-owned
+// arrays only, none of which an asynchronous read-back copies, so it needs no chd_fetch_guard.
+#include "chd_engine.h"
+
+#include "chd_follow.cuh"
+
+namespace {
+
+constexpr uint32_t SHAPE_KINDS = CHD_AOI_SPHERE | CHD_AOI_BOX | CHD_AOI_CONE;
+
+bool follow_alloc(chd_engine* e) {
+    chd_engine::Follow& F = e->fw;
+    if (F.on) return true;
+    const uint64_t S = e->lim.max_subscribers, Q = e->lim.max_queries;
+    FollowDev& d = F.st;
+    FollowBatch& q = F.q;
+    bool ok = dalloc(e, &d.entity, S) && dalloc(e, &d.kind, S) && dalloc(e, &d.dirty, S) && dalloc(e, &d.tslot, S) && dalloc(e, &d.res, S);
+    for (double** p : {&d.sph_r, &d.box_ex, &d.box_ez, &d.cone_dx, &d.cone_dz, &d.cone_angle, &d.cone_r, &d.last_x, &d.last_z}) ok = ok && dalloc(e, p, S);
+    ok = ok && dalloc(e, &q.sub, Q) && dalloc(e, &q.kind, Q) && dalloc(e, &q.n_selected, 1);
+    for (double** p : {&q.sph_cx, &q.sph_cz, &q.sph_r, &q.box_cx, &q.box_cz, &q.box_ex, &q.box_ez, &q.cone_cx, &q.cone_cz, &q.cone_dx, &q.cone_dz,
+                       &q.cone_angle, &q.cone_r})
+        ok = ok && dalloc(e, p, Q);
+    ok = ok && chd_make_site(e, F.site, S + 1, EP_FOLLOW);
+    if (!ok) return false;
+    if (cudaMemsetAsync(d.kind, 0, S, e->stream) != cudaSuccess || cudaMemsetAsync(q.n_selected, 0, 4, e->stream) != cudaSuccess)
+        return e->fail("cudaMemsetAsync failed in chd_follow_bind");
+    F.h_kind.assign(S, 0);
+    F.on = true;
+    return true;
+}
+
+// `bytes` of host data into the follower staging buffer, before the call returns (the caller's arrays are plain host memory)
+chd_status stage_upload(chd_engine* e, const void* h, uint64_t bytes) {
+    chd_engine::Follow& F = e->fw;
+    if (!ensure_cap(e, &F.d_stage, &F.stage_cap, bytes, bytes + bytes / 2 + 4096)) return CHD_ERR_CUDA;
+    CU(e, cudaMemcpyAsync(F.d_stage, h, bytes, cudaMemcpyHostToDevice, e->stream));
+    CU(e, cudaStreamSynchronize(e->stream));
+    return CHD_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+chd_status chd_follow_bind(chd_engine* e, const chd_follow_batch* b) {
+    if (!e || !b || (b->n && (!b->slot || !b->entity))) return CHD_ERR_INVALID;
+    if (chd_rule_follow(e, "chd_follow_bind") != CHD_OK) return CHD_ERR_STATE;
+    const uint32_t n = b->n;
+    if (!n) return CHD_OK;
+    std::lock_guard<std::recursive_mutex> lk(e->mu);
+    CU(e, cudaSetDevice(e->device));
+    // argument checks first: a refused call binds nothing
+    std::unordered_map<uint32_t, uint32_t> last;  // slot -> its last binding in the call
+    last.reserve(n);
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t s = b->slot[i], kind = b->kind ? b->kind[i] : (uint32_t)CHD_AOI_SPHERE;
+        if (s >= e->lim.max_subscribers || s >= e->n_slots) {
+            e->fail("chd_follow_bind: slot %u was never added (%u slots, max_subscribers %u)", s, e->n_slots, e->lim.max_subscribers);
+            return CHD_ERR_INVALID;
+        }
+        if (kind & CHD_AOI_SPOTS) {
+            e->fail("chd_follow_bind: CHD_AOI_SPOTS has absolute positions and cannot follow an entity (binding %u)", i);
+            return CHD_ERR_INVALID;
+        }
+        if (!kind || (kind & ~SHAPE_KINDS)) {
+            e->fail("chd_follow_bind: kind 0x%x of binding %u is not a mask of CHD_AOI_SPHERE | CHD_AOI_BOX | CHD_AOI_CONE", kind, i);
+            return CHD_ERR_INVALID;
+        }
+        if (((kind & CHD_AOI_SPHERE) && !b->sph_r) || ((kind & CHD_AOI_BOX) && (!b->box_ex || !b->box_ez)) ||
+            ((kind & CHD_AOI_CONE) && (!b->cone_dx || !b->cone_dz || !b->cone_angle || !b->cone_r))) {
+            e->fail("chd_follow_bind: binding %u has kind 0x%x but a shape array of that kind is NULL", i, kind);
+            return CHD_ERR_INVALID;
+        }
+        last[s] = i;
+    }
+    chd_engine::Follow& F = e->fw;
+    uint64_t fresh = 0;
+    for (const auto& kv : last) fresh += !(F.on && F.h_kind[kv.first]);
+    if (F.n_bound + fresh > e->lim.max_queries) {
+        e->fail("chd_follow_bind: %llu followers > max_queries %u", (unsigned long long)(F.n_bound + fresh), e->lim.max_queries);
+        return CHD_ERR_CAPACITY;
+    }
+    if (!follow_alloc(e)) return CHD_ERR_CUDA;
+    // staged SoA of the m winners: shape [7][m] doubles | slot [m] | entity [m] | kind [m]
+    const uint64_t m = last.size();
+    std::vector<uint8_t> h(m * (7 * 8 + 4 + 4 + 1));
+    double* shape = reinterpret_cast<double*>(h.data());
+    uint32_t* hs = reinterpret_cast<uint32_t*>(h.data() + 56 * m);
+    uint32_t* he = hs + m;
+    uint8_t* hk = reinterpret_cast<uint8_t*>(he + m);
+    const double* src[7] = {b->sph_r, b->box_ex, b->box_ez, b->cone_dx, b->cone_dz, b->cone_angle, b->cone_r};
+    uint64_t j = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        if (last[b->slot[i]] != i) continue;
+        hs[j] = b->slot[i];
+        he[j] = b->entity[i];
+        hk[j] = b->kind ? b->kind[i] : (uint8_t)CHD_AOI_SPHERE;
+        for (int a = 0; a < 7; a++) shape[a * m + j] = src[a] ? src[a][i] : 0.0;
+        j++;
+    }
+    chd_status st = stage_upload(e, h.data(), h.size());
+    if (st != CHD_OK) return st;
+    const uint8_t* d = F.d_stage;
+    const FollowStage stage{reinterpret_cast<const uint32_t*>(d + 56 * m), reinterpret_cast<const uint32_t*>(d + 60 * m), d + 64 * m,
+                            reinterpret_cast<const double*>(d)};
+    follow_bind_kernel<<<blocks_for(m, FOLLOW_THREADS), FOLLOW_THREADS, 0, e->stream>>>(stage, (uint32_t)m, F.st);
+    KCHECK(e);
+    for (uint64_t k = 0; k < m; k++) {
+        F.n_bound += !F.h_kind[hs[k]];
+        F.h_kind[hs[k]] = hk[k];
+    }
+    return CHD_OK;
+}
+
+chd_status chd_follow_drop(chd_engine* e, const uint32_t* slot, const uint32_t* d_slot, uint32_t n) {
+    chd_engine::Follow& F = e->fw;
+    if (!F.on || !F.n_bound) return CHD_OK;
+    const uint32_t S = e->lim.max_subscribers;
+    if (!slot) {  // every slot
+        CU(e, cudaMemsetAsync(F.st.kind, 0, S, e->stream));
+        std::fill(F.h_kind.begin(), F.h_kind.end(), (uint8_t)0);
+        F.n_bound = 0;
+        return CHD_OK;
+    }
+    uint32_t hit = 0;
+    for (uint32_t i = 0; i < n; i++)
+        if (slot[i] < S && F.h_kind[slot[i]]) {
+            F.h_kind[slot[i]] = 0;
+            hit++;
+        }
+    if (!hit) return CHD_OK;
+    F.n_bound -= hit;
+    if (!d_slot) {
+        chd_status st = stage_upload(e, slot, 4ull * n);
+        if (st != CHD_OK) return st;
+        d_slot = reinterpret_cast<const uint32_t*>(F.d_stage);
+    }
+    follow_unbind_kernel<<<blocks_for(n, FOLLOW_THREADS), FOLLOW_THREADS, 0, e->stream>>>(d_slot, n, S, F.st.kind);
+    KCHECK(e);
+    return CHD_OK;
+}
+
+chd_status chd_follow_unbind(chd_engine* e, const uint32_t* slot, uint32_t n) {
+    if (!e || (n && !slot)) return CHD_ERR_INVALID;
+    if (chd_rule_follow(e, "chd_follow_unbind") != CHD_OK) return CHD_ERR_STATE;
+    if (!n) return CHD_OK;
+    std::lock_guard<std::recursive_mutex> lk(e->mu);
+    CU(e, cudaSetDevice(e->device));
+    for (uint32_t i = 0; i < n; i++)
+        if (slot[i] >= e->lim.max_subscribers) {
+            e->fail("chd_follow_unbind: slot %u >= max_subscribers %u", slot[i], e->lim.max_subscribers);
+            return CHD_ERR_INVALID;
+        }
+    return chd_follow_drop(e, slot, nullptr, n);
+}
+
+chd_status chd_follow_queries(chd_engine* e, uint32_t mode) {
+    if (!e || (mode != CHD_FOLLOW_ALL && mode != CHD_FOLLOW_MOVED)) return CHD_ERR_INVALID;
+    if (chd_rule_follow(e, "chd_follow_queries") != CHD_OK || chd_rule_one_batch(e, "chd_follow_queries") != CHD_OK) return CHD_ERR_STATE;
+    std::lock_guard<std::recursive_mutex> lk(e->mu);
+    CU(e, cudaSetDevice(e->device));
+    chd_engine::Follow& F = e->fw;
+    if (!F.on || !F.n_bound) {  // nothing follows: an empty batch (it still applies pending lifecycle changes)
+        F.view = QueryDev{};
+        F.ready = true;
+        return CHD_OK;
+    }
+    cudaStream_t s = e->stream;
+    StageTimer timer(e, s, CHD_STAGE_FOLLOW);
+    const uint32_t S = e->n_slots, B = F.n_bound;
+    const FollowEntities ent = e->tbl.on ? FollowEntities{e->d_x, e->d_z, e->lim.max_entities, e->tbl.d_table, e->tbl.bits, e->tbl.d_id_of_slot}
+                                         : FollowEntities{e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z, e->n_own, nullptr, 0, nullptr};
+    chd_status st = chd_epoch_tick(e, s, EP_FOLLOW);
+    if (st != CHD_OK) return st;
+    const FollowBatch& q = F.q;
+    // the graph bakes in the slot and follower counts, the mode and where the positions live (the state arrays never move)
+    const uint64_t key = stage_key(0x666f6c6cull, S, B, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub);
+    st = run_stage(e, s, F.g, key, [&]() -> chd_status {
+        // the skip tail: entries behind the selected count name no slot and no kind
+        CU(e, cudaMemsetAsync(q.sub, 0xFF, 4ull * B, s));
+        CU(e, cudaMemsetAsync(q.kind, 0, B, s));
+        bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_FOLLOW);
+        KCHECK(e);
+        SCAN(e, compact_1p(FollowFlag{F.st, ent, mode}, FollowSink{F.st, q}, S, F.site, s));
+        return CHD_OK;
+    });
+    if (st != CHD_OK) return st;
+    if (!e->tbl.on) {  // the positions were read: a prefetch may refill their buffers after this
+        st = chd_note_pos_read(e, s);
+        if (st != CHD_OK) return st;
+    }
+    QueryDev v{};
+    v.n = B;
+    v.sub = q.sub; v.kind = q.kind;
+    v.sph_cx = q.sph_cx; v.sph_cz = q.sph_cz; v.sph_r = q.sph_r;
+    v.box_cx = q.box_cx; v.box_cz = q.box_cz; v.box_ex = q.box_ex; v.box_ez = q.box_ez;
+    v.cone_cx = q.cone_cx; v.cone_cz = q.cone_cz; v.cone_dx = q.cone_dx; v.cone_dz = q.cone_dz; v.cone_angle = q.cone_angle; v.cone_r = q.cone_r;
+    F.view = v;
+    F.ready = true;
+    return CHD_OK;
+}
+
+chd_status chd_get_follow(chd_engine* e, uint32_t* slot, uint32_t* entity, uint32_t* status, double* cx, double* cz, uint32_t cap, uint32_t* count,
+                          uint32_t* n_selected) {
+    if (!e) return CHD_ERR_INVALID;
+    if (chd_rule_follow(e, "chd_get_follow") != CHD_OK) return CHD_ERR_STATE;
+    chd_engine::Follow& F = e->fw;
+    if (F.ready || e->interest_pending) {
+        e->fail("chd_get_follow: the generated batch has not been consumed by an interest update yet (or chd_begin_interest is not joined)");
+        return CHD_ERR_STATE;
+    }
+    if (count) *count = 0;
+    if (n_selected) *n_selected = 0;
+    if (!F.on || !F.n_bound) return CHD_OK;
+    std::lock_guard<std::recursive_mutex> lk(e->mu);
+    CU(e, cudaSetDevice(e->device));
+    cudaStream_t s = e->stream;
+    const uint64_t Q = e->lim.max_queries;
+    if (!F.g_count && !(dalloc(e, &F.g_slot, Q) && dalloc(e, &F.g_entity, Q) && dalloc(e, &F.g_status, Q) && dalloc(e, &F.g_cx, Q) && dalloc(e, &F.g_cz, Q) &&
+                        dalloc(e, &F.g_count, 1)))
+        return CHD_ERR_CUDA;  // (g_count is allocated last)
+    chd_status st = chd_epoch_tick(e, s, EP_FOLLOW);
+    if (st != CHD_OK) return st;
+    bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_FOLLOW);
+    KCHECK(e);
+    SCAN(e, compact_1p(FollowBoundFlag{F.st.kind}, FollowReportSink{F.st, e->d_status, F.g_slot, F.g_entity, F.g_status, F.g_cx, F.g_cz, F.g_count}, e->n_slots,
+                       F.site, s));
+    uint32_t m = 0;
+    st = chd_read_u32(e, F.g_count, &m);
+    if (st != CHD_OK) return st;
+    if (count) *count = m;
+    if (n_selected) {
+        st = chd_read_u32(e, F.q.n_selected, n_selected);
+        if (st != CHD_OK) return st;
+    }
+    const uint64_t k = std::min(m, cap);
+    if (!k) return CHD_OK;
+    if (slot) CU(e, cudaMemcpyAsync(slot, F.g_slot, 4 * k, cudaMemcpyDefault, s));
+    if (entity) CU(e, cudaMemcpyAsync(entity, F.g_entity, 4 * k, cudaMemcpyDefault, s));
+    if (status) CU(e, cudaMemcpyAsync(status, F.g_status, 4 * k, cudaMemcpyDefault, s));
+    if (cx) CU(e, cudaMemcpyAsync(cx, F.g_cx, 8 * k, cudaMemcpyDefault, s));
+    if (cz) CU(e, cudaMemcpyAsync(cz, F.g_cz, 8 * k, cudaMemcpyDefault, s));
+    CU(e, cudaStreamSynchronize(s));
+    return CHD_OK;
+}
+}  // extern "C"

@@ -1,0 +1,141 @@
+// chd_follow.cuh — followers: subscriber slots whose area of interest is centred on an entity (chd_follow_bind).  The device keeps
+// one binding per slot and turns the bindings into the tick's query batch (chd_follow_queries) from the positions the build reads,
+// so the host neither mirrors positions nor packs and uploads queries.
+//
+// Generation is ONE single-pass compaction over the slots (compact_lookback_kernel, chd_scan.cuh): the flag functor resolves the
+// slot's entity, reads its position, decides selected / not selected / no entity and records that per slot; the sink writes the
+// query entry at the follower's rank among the selected ones, so the batch is in ascending slot order.  Reading a position by
+// entity is a gather of 16 bytes per follower: latency-bound (not measured in isolation).
+#pragma once
+#include "chd_scan.cuh"
+#include "chd_types.cuh"
+
+namespace chd {
+
+constexpr int FOLLOW_THREADS = 256;
+// res[] of a slot that is bound but has no query in the generated batch: FOLLOW_NO_QUERY | CHD_FOLLOW_NOT_SELECTED / _NO_ENTITY
+// (a selected follower's res is its batch entry, below 2^31)
+constexpr uint32_t FOLLOW_NO_QUERY = 0x80000000u;
+
+// Where a followed entity's position comes from: the arrays the build reads; in entity-table mode through the id table.
+struct FollowEntities {
+    const double *__restrict__ px, *__restrict__ pz;
+    uint32_t n;  // positions that exist: the entity count, or the table's slot capacity
+    const uint64_t* __restrict__ table;  // nullptr: index mode
+    uint32_t bits;
+    const uint32_t* __restrict__ id_of_slot;
+};
+
+struct FollowFlag {
+    FollowDev f;
+    FollowEntities ent;
+    uint32_t mode;
+    __device__ __forceinline__ bool operator()(uint64_t s) const {
+        if (!f.kind[s]) return false;
+        uint32_t p = f.entity[s];
+        if (ent.table) {
+            // a despawned slot is parked and may be reused by another id: the cached slot counts only while it still holds this id
+            const uint32_t id = p;
+            p = f.tslot[s];
+            if (p >= ent.n || id == 0u || ent.id_of_slot[p] != id) {
+                p = tbl_find(ent.table, ent.bits, id, nullptr);
+                f.tslot[s] = p;
+            }
+        }
+        if (p >= ent.n) {  // no such entity: no query, and a respawn counts as moved
+            f.res[s] = FOLLOW_NO_QUERY | (uint32_t)CHD_FOLLOW_NO_ENTITY;
+            f.dirty[s] = 1;
+            return false;
+        }
+        const double x = ent.px[p], z = ent.pz[p];
+        const bool moved = __double_as_longlong(x) != __double_as_longlong(f.last_x[s]) || __double_as_longlong(z) != __double_as_longlong(f.last_z[s]);
+        if (mode == (uint32_t)CHD_FOLLOW_MOVED && !f.dirty[s] && !moved) {
+            f.res[s] = FOLLOW_NO_QUERY | (uint32_t)CHD_FOLLOW_NOT_SELECTED;
+            return false;
+        }
+        f.last_x[s] = x;
+        f.last_z[s] = z;
+        f.dirty[s] = 0;
+        return true;
+    }
+};
+
+struct FollowSink {
+    FollowDev f;
+    FollowBatch q;
+    __device__ __forceinline__ void operator()(uint64_t s, uint32_t k) const {
+        const uint32_t kind = f.kind[s];
+        const double x = f.last_x[s], z = f.last_z[s];  // (written by this thread's flag call)
+        q.sub[k] = (uint32_t)s;
+        q.kind[k] = (uint8_t)kind;
+        if (kind & CHD_AOI_SPHERE) {
+            q.sph_cx[k] = x; q.sph_cz[k] = z; q.sph_r[k] = f.sph_r[s];
+        }
+        if (kind & CHD_AOI_BOX) {
+            q.box_cx[k] = x; q.box_cz[k] = z; q.box_ex[k] = f.box_ex[s]; q.box_ez[k] = f.box_ez[s];
+        }
+        if (kind & CHD_AOI_CONE) {
+            q.cone_cx[k] = x; q.cone_cz[k] = z; q.cone_dx[k] = f.cone_dx[s]; q.cone_dz[k] = f.cone_dz[s];
+            q.cone_angle[k] = f.cone_angle[s]; q.cone_r[k] = f.cone_r[s];
+        }
+        f.res[s] = k;
+    }
+    __device__ __forceinline__ void total(uint32_t c) const { *q.n_selected = c; }
+};
+
+// chd_get_follow: the bound slots in ascending order with what the last generation did with each of them.
+struct FollowBoundFlag {
+    const uint8_t* __restrict__ kind;
+    __device__ __forceinline__ bool operator()(uint64_t s) const { return kind[s] != 0; }
+};
+struct FollowReportSink {
+    FollowDev f;
+    const uint32_t* __restrict__ qstatus;  // statuses of the interest update that consumed the batch
+    uint32_t *__restrict__ slot, *__restrict__ entity, *__restrict__ status;
+    double *__restrict__ cx, *__restrict__ cz;
+    uint32_t* __restrict__ count;
+    __device__ __forceinline__ void operator()(uint64_t s, uint32_t k) const {
+        const uint32_t r = f.res[s];
+        slot[k] = (uint32_t)s;
+        entity[k] = f.entity[s];
+        status[k] = (r & FOLLOW_NO_QUERY) ? (r & ~FOLLOW_NO_QUERY) : qstatus[r];
+        cx[k] = f.last_x[s];
+        cz[k] = f.last_z[s];
+    }
+    __device__ __forceinline__ void total(uint32_t c) const { *count = c; }
+};
+
+// chd_follow_bind: scatter m staged bindings (one per slot: the host keeps the last of a slot named twice) into the per-slot state.
+// A bound slot starts dirty, with no query generated yet.
+struct FollowStage {
+    const uint32_t *__restrict__ slot, *__restrict__ entity;
+    const uint8_t* __restrict__ kind;
+    const double* __restrict__ shape;  // [7][m]: sph_r, box_ex, box_ez, cone_dx, cone_dz, cone_angle, cone_r
+};
+__global__ void __launch_bounds__(FOLLOW_THREADS) follow_bind_kernel(FollowStage st, uint32_t m, FollowDev f) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const uint32_t s = st.slot[i];
+    f.entity[s] = st.entity[i];
+    f.kind[s] = st.kind[i];
+    f.sph_r[s] = st.shape[i];
+    f.box_ex[s] = st.shape[(uint64_t)m + i];
+    f.box_ez[s] = st.shape[2ull * m + i];
+    f.cone_dx[s] = st.shape[3ull * m + i];
+    f.cone_dz[s] = st.shape[4ull * m + i];
+    f.cone_angle[s] = st.shape[5ull * m + i];
+    f.cone_r[s] = st.shape[6ull * m + i];
+    f.last_x[s] = 0.0;
+    f.last_z[s] = 0.0;
+    f.dirty[s] = 1;
+    f.tslot[s] = TBL_NONE;
+    f.res[s] = FOLLOW_NO_QUERY | (uint32_t)CHD_FOLLOW_NOT_SELECTED;
+}
+
+// chd_follow_unbind / chd_remove_subscribers: the listed slots follow nothing (slots beyond the state are ignored)
+__global__ void __launch_bounds__(FOLLOW_THREADS) follow_unbind_kernel(const uint32_t* __restrict__ slot, uint32_t n, uint32_t n_state, uint8_t* __restrict__ kind) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && slot[i] < n_state) kind[slot[i]] = 0;
+}
+
+}  // namespace chd

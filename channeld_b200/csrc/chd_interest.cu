@@ -40,7 +40,7 @@ chd_status chd_set_subscribers(chd_engine* e, const uint32_t* conn_id, uint32_t 
     if (n < e->lim.max_subscribers) CU(e, cudaMemsetAsync(e->d_conn + n, 0, sizeof(uint32_t) * (e->lim.max_subscribers - n), e->stream));
     e->n_slots = n;
     e->cur = 0;
-    return CHD_OK;
+    return chd_follow_drop(e, nullptr, nullptr, 0);  // no slot follows an entity any more
 }
 
 // slots (+ an optional per-slot value) of a lifecycle call -> device staging; slot lists are control-plane sized
@@ -105,7 +105,7 @@ chd_status chd_remove_subscribers(chd_engine* e, const uint32_t* slot, uint32_t 
     slot_ctl_set_kernel<<<blocks_for(n, 256), 256, 0, e->stream>>>(e->d_lc_slot, nullptr, n, (uint8_t)SLOT_REMOVE, 0u, e->d_slot_ctl, e->d_slot_src, nullptr);
     KCHECK(e);
     e->lifecycle_used = true;
-    return CHD_OK;
+    return chd_follow_drop(e, slot, e->d_lc_slot, n);  // a removed slot follows nothing
 }
 
 // copies the batch into the engine's device SoA (or a prefetch staging set) on `s` and returns the device view
@@ -318,9 +318,12 @@ chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query
     QueryDev d;
     chd_status st;
     int pf_set = -1;  // prefetch staging set this batch lives in
-    if (!q) {  // the batch uploaded by chd_prefetch_queries and handed over by chd_adopt_prefetched
+    if (!q && e->fw.ready) {  // the batch generated by chd_follow_queries: device-resident, ordered before this on the engine stream
+        d = e->fw.view;
+        e->fw.ready = false;  // consumed
+    } else if (!q) {  // the batch uploaded by chd_prefetch_queries and handed over by chd_adopt_prefetched
         if (e->pf_q.cur < 0) {
-            e->fail("interest update without a batch: q == NULL needs chd_prefetch_queries + chd_adopt_prefetched first");
+            e->fail("interest update without a batch: q == NULL needs chd_prefetch_queries + chd_adopt_prefetched, or chd_follow_queries, first");
             return CHD_ERR_STATE;
         }
         pf_set = e->pf_q.cur;

@@ -62,7 +62,7 @@ extern "C" {
 
 chd_status chd_set_slab(chd_engine* e, uint32_t col_lo, uint32_t col_hi, uint32_t halo) {
     // (entity-table mode on slabs: the slab comes first, then chd_entity_table_init; the table's slots do not move with the slab)
-    if (e && chd_rule_not_table(e, "chd_set_slab") != CHD_OK) return CHD_ERR_STATE;
+    if (e && (chd_rule_not_table(e, "chd_set_slab") != CHD_OK || chd_rule_no_followers(e, "chd_set_slab") != CHD_OK)) return CHD_ERR_STATE;
     if (!e || col_lo >= col_hi || col_hi > e->g.cols) return CHD_ERR_INVALID;
     e->slab = true;
     e->g.col_lo = col_lo;
@@ -191,7 +191,7 @@ chd_status chd_comm_unique_id(void* out_id) {
 
 chd_status chd_comm_init(chd_engine* e, const void* unique_id, int rank, int world, uint32_t halo_cols, uint32_t border_capacity,
                          uint32_t migrate_subscribers, uint32_t migrate_pairs) {
-    if (e && chd_rule_not_table(e, "chd_comm_init") != CHD_OK) return CHD_ERR_STATE;
+    if (e && (chd_rule_not_table(e, "chd_comm_init") != CHD_OK || chd_rule_no_followers(e, "chd_comm_init") != CHD_OK)) return CHD_ERR_STATE;
     if (!e || !unique_id || world < 1 || rank < 0 || rank >= world || border_capacity == 0) return CHD_ERR_INVALID;
     if (world >= 4096 || migrate_subscribers >= (1u << 20)) return CHD_ERR_INVALID;  // (slot_src packs rank:12 | record:20)
     if (e->comm) {

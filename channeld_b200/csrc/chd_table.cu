@@ -301,6 +301,25 @@ chd_status chd_rule_halo_import(chd_engine* e) {
     return e->have_gid || e->tbl.on ? CHD_OK : refuse(e, "chd_import_halo requires global entity ids (chd_set_entity_ids or entity-table mode)");
 }
 
+// 9. Followers (chd_follow_*) are single-GPU: a follower's entity may live on another rank, and border records carry no
+// positions.  So they are refused on a slab, and an engine with followers cannot become one.  `entity` of a binding is the table
+// id in entity-table mode and the entity index otherwise (chd_set_entity_ids does not change that).
+chd_status chd_rule_follow(chd_engine* e, const char* fn) {
+    return e->slab ? refuse(e, "%s: followers are not available on an engine made a slab (chd_set_slab / chd_comm_init)", fn) : CHD_OK;
+}
+chd_status chd_rule_no_followers(chd_engine* e, const char* fn) {
+    return e->fw.n_bound ? refuse(e, "%s: %u subscriber slots follow entities (chd_follow_bind); followers are single-GPU", fn, e->fw.n_bound) : CHD_OK;
+}
+
+// ... and one query batch per interest update: a generated batch (chd_follow_queries) and an adopted prefetched one
+// (chd_prefetch_queries + chd_adopt_prefetched) exclude each other until the update that consumes the first has been enqueued.
+chd_status chd_rule_one_batch(chd_engine* e, const char* fn) {
+    if (e->fw.ready) return refuse(e, "%s: the batch generated by chd_follow_queries has not been consumed by an interest update yet", fn);
+    if (e->pf_q.cur >= 0) return refuse(e, "%s: the adopted prefetched query batch has not been consumed by an interest update yet", fn);
+    if (e->interest_pending) return refuse(e, "%s: chd_begin_interest is pending (not joined by chd_tick yet)", fn);
+    return CHD_OK;
+}
+
 chd_status chd_entity_table_init(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_fresh_engine(e) != CHD_OK) return CHD_ERR_STATE;

@@ -11,25 +11,7 @@
 
 namespace chd {
 
-constexpr uint64_t TBL_EMPTY = 0;
-constexpr uint64_t TBL_TOMB = 0xFFFFFFFFull << 32;
-constexpr uint32_t TBL_NONE = 0xFFFFFFFFu;
 constexpr int TBL_THREADS = 256;
-
-__host__ __device__ __forceinline__ uint64_t tbl_home(uint32_t id, uint32_t bits) { return ((uint64_t)id * 0x9E3779B97F4A7C15ull) >> (64 - bits); }
-
-__device__ __forceinline__ uint32_t tbl_find(const uint64_t* __restrict__ table, uint32_t bits, uint32_t id, uint64_t* where) {
-    const uint64_t mask = (1ull << bits) - 1ull;
-    if (id == 0u || id == TBL_NONE) return TBL_NONE;
-    for (uint64_t h = tbl_home(id, bits);; h = (h + 1) & mask) {
-        const uint64_t w = table[h];
-        if (w == TBL_EMPTY) return TBL_NONE;
-        if ((uint32_t)(w >> 32) == id) {
-            if (where) *where = h;
-            return (uint32_t)w;
-        }
-    }
-}
 
 // Spawn apply (x != nullptr): insert (id, slot), slot -> id, the position, flag the slot.  Rebuild (x == nullptr): insert only.
 __global__ void __launch_bounds__(TBL_THREADS) tbl_spawn_kernel(uint64_t* table, uint32_t bits, const uint32_t* __restrict__ id, const uint32_t* __restrict__ slot,

@@ -333,6 +333,11 @@ chd_status chd_adopt_prefetched(chd_engine* e) {
         e->fail("chd_adopt_prefetched without a preceding chd_prefetch_entities / chd_prefetch_queries / chd_prefetch_rings");
         return CHD_ERR_STATE;
     }
+    if (e->pf_q.staged >= 0 && e->fw.ready) {
+        e->fail("chd_adopt_prefetched: a query batch was prefetched, but the batch generated by chd_follow_queries has not been consumed by an "
+                "interest update yet (one batch per update)");
+        return CHD_ERR_STATE;
+    }
     CU(e, cudaSetDevice(e->device));
     chd_pf_adopt(e->pf_q);  // consumed by the next chd_begin_interest / chd_update_interest called with q == NULL
     if (chd_pf_adopt(e->pf_ring)) {
@@ -399,8 +404,8 @@ static chd_status aux_chain_enqueue(chd_engine* e, cudaStream_t s, const chd_que
 
 chd_status chd_begin_interest(chd_engine* e, const chd_query_batch* q, int64_t t_ns, int with_fanout) {
     if (!e) return CHD_ERR_INVALID;
-    if (!q && e->pf_q.cur < 0) {
-        e->fail("chd_begin_interest: q == NULL needs chd_prefetch_queries + chd_adopt_prefetched first");
+    if (!q && e->pf_q.cur < 0 && !e->fw.ready) {
+        e->fail("chd_begin_interest: q == NULL needs chd_prefetch_queries + chd_adopt_prefetched, or chd_follow_queries, first");
         return CHD_ERR_STATE;
     }
     if (e->interest_pending) {
@@ -441,20 +446,27 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
     const bool do_fanout = flags & CHD_TICK_FANOUT;
     const bool do_delta = flags & CHD_TICK_VISIBLE_DELTA;
     const bool started = e->interest_pending;  // the aux chain of this tick was started by chd_begin_interest
+    const bool follow = flags & CHD_TICK_FOLLOW;  // the batch is the generated one (q == NULL)
+    if (follow && q) return CHD_ERR_INVALID;
+    if (follow && !started && !e->fw.ready) {
+        e->fail("chd_tick: CHD_TICK_FOLLOW without a batch generated by chd_follow_queries");
+        return CHD_ERR_STATE;
+    }
+    const bool interest = q || follow;  // this tick has an interest update of its own
     e->early_ready = false;
     e->build_done_recorded = false;
     e->dl.done_recorded = false;
-    if (started && q) {
+    if (started && interest) {
         e->fail("chd_tick: a query batch was given while chd_begin_interest is pending");
         return CHD_ERR_STATE;
     }
     if (do_delta && chd_delta_check(e, need_build) != CHD_OK) return CHD_ERR_STATE;
-    if (!started && !((q || do_fanout) && (need_build || do_emit))) {
+    if (!started && !((interest || do_fanout) && (need_build || do_emit))) {
         if (need_build) {
             st = chd_build_on(e, s);
             if (st != CHD_OK) return st;
         }
-        if (q) {
+        if (interest) {
             st = chd_update_interest_on(e, s, q, t_ns);
             if (st != CHD_OK) return st;
         }
@@ -469,7 +481,7 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
         return do_delta ? chd_delta_on(e, s) : CHD_OK;
     }
     if (!started) {
-        st = aux_chain_enqueue(e, s, q, q != nullptr, t_ns, do_fanout);
+        st = aux_chain_enqueue(e, s, q, interest, t_ns, do_fanout);
         if (st != CHD_OK) return st;
     }
     const bool fanout_done = started ? e->pending_fanout : do_fanout;
@@ -484,7 +496,7 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
     if (do_emit) {
         // the preparation waits for the new pairs (for the fork when this tick updates no interest); CHD_TICK_EARLY_RESULTS: the
         // copy kernel starts after the whole aux chain, so every host-facing result is final while it is still streaming
-        st = emit_enqueue(e, s, (started || q) ? e->ev_pairs : e->ev_interest, (flags & CHD_TICK_EARLY_RESULTS) ? e->ev_join : nullptr);
+        st = emit_enqueue(e, s, (started || interest) ? e->ev_pairs : e->ev_interest, (flags & CHD_TICK_EARLY_RESULTS) ? e->ev_join : nullptr);
         if (st != CHD_OK) return st;
     }
     if (do_delta) {
@@ -492,7 +504,7 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
         // the build and the new pairs, and the engine stream waits for it
         const cudaStream_t ds = e->prep_stream;
         CU(e, cudaStreamWaitEvent(ds, e->dl.ev_in, 0));
-        if (started || q) CU(e, cudaStreamWaitEvent(ds, e->ev_pairs, 0));
+        if (started || interest) CU(e, cudaStreamWaitEvent(ds, e->ev_pairs, 0));
         st = chd_delta_on(e, ds);
         if (st != CHD_OK) return st;
         CU(e, cudaEventRecord(e->dl.ev_done, ds));

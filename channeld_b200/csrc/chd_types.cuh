@@ -168,6 +168,46 @@ struct EntityIds {
     __device__ __forceinline__ uint32_t at(uint32_t p) const { return p < own ? own_ids[p] : (gid ? gid[p] : p); }
 };
 
+// ---- the entity table's id -> slot words and their lookup (layout: chd_table.cuh), shared with the followers' entity lookup
+constexpr uint64_t TBL_EMPTY = 0;
+constexpr uint64_t TBL_TOMB = 0xFFFFFFFFull << 32;
+constexpr uint32_t TBL_NONE = 0xFFFFFFFFu;
+
+__host__ __device__ __forceinline__ uint64_t tbl_home(uint32_t id, uint32_t bits) { return ((uint64_t)id * 0x9E3779B97F4A7C15ull) >> (64 - bits); }
+
+__device__ __forceinline__ uint32_t tbl_find(const uint64_t* __restrict__ table, uint32_t bits, uint32_t id, uint64_t* where) {
+    const uint64_t mask = (1ull << bits) - 1ull;
+    if (id == 0u || id == TBL_NONE) return TBL_NONE;
+    for (uint64_t h = tbl_home(id, bits);; h = (h + 1) & mask) {
+        const uint64_t w = table[h];
+        if (w == TBL_EMPTY) return TBL_NONE;
+        if ((uint32_t)(w >> 32) == id) {
+            if (where) *where = h;
+            return (uint32_t)w;
+        }
+    }
+}
+
+// ---- followers (chd_follow.cuh)
+// Per-slot binding state, [max_subscribers] each.  kind == 0: the slot follows nothing.
+struct FollowDev {
+    uint32_t* entity;  // entity index, or table id in entity-table mode
+    uint8_t* kind;     // CHD_AOI_SPHERE | BOX | CONE mask
+    double *sph_r, *box_ex, *box_ez, *cone_dx, *cone_dz, *cone_angle, *cone_r;
+    double *last_x, *last_z;  // centre of the last query generated for the slot
+    uint8_t* dirty;           // bound or re-bound since the last batch that selected the slot, or its entity was missing then
+    uint32_t* tslot;          // entity-table mode: the table slot the id was last found in (validated against slot -> id on use)
+    uint32_t* res;            // what the last generation did with the slot: batch entry, or FOLLOW_NO_QUERY | reason
+};
+
+// The generated batch: a query batch's SoA (chd_query_batch without spots) in device memory.
+struct FollowBatch {
+    uint32_t* sub;
+    uint8_t* kind;
+    double *sph_cx, *sph_cz, *sph_r, *box_cx, *box_cz, *box_ex, *box_ez, *cone_cx, *cone_cz, *cone_dx, *cone_dz, *cone_angle, *cone_r;
+    uint32_t* n_selected;
+};
+
 struct BcastDev {
     uint32_t n;
     const uint32_t *channel, *flags, *sender, *client;

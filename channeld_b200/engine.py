@@ -395,6 +395,49 @@ class Engine:
         self._ck(self.L.chd_get_entity_stats(self.h, C.byref(s)))
         return s.as_dict()
 
+    # ---- followers: subscriber slots whose AOI is centred on an entity; the device generates the tick's query batch
+    def follow_bind(self, slots, entities, kind=None, sph_r=None, box=None, cone=None):
+        """Binds slot[i] to entity[i] (entity index; table id in entity-table mode).  kind: AOI_SPHERE | AOI_BOX | AOI_CONE masks
+        (None = all sphere); sph_r, box=(ex, ez), cone=(dx, dz, angle, r): per-binding shape arrays of the kinds in use."""
+        slots = np.ascontiguousarray(slots, np.uint32)
+        entities = np.ascontiguousarray(entities, np.uint32)
+        keep = [slots, entities]
+
+        def arr(a, dtype=np.float64):
+            if a is None:
+                return None
+            a = np.ascontiguousarray(a, dtype)
+            keep.append(a)
+            return ptr(a)
+
+        b = capi.FollowBatch()
+        b.n, b.slot, b.entity, b.kind, b.sph_r = len(slots), ptr(slots), ptr(entities), arr(kind, np.uint8), arr(sph_r)
+        if box is not None:
+            b.box_ex, b.box_ez = (arr(a) for a in box)
+        if cone is not None:
+            b.cone_dx, b.cone_dz, b.cone_angle, b.cone_r = (arr(a) for a in cone)
+        self._ck(self.L.chd_follow_bind(self.h, C.byref(b)))
+
+    def follow_unbind(self, slots):
+        slots = np.ascontiguousarray(slots, np.uint32)
+        self._ck(self.L.chd_follow_unbind(self.h, ptr(slots), len(slots)))
+
+    def follow_queries(self, mode=capi.FOLLOW_ALL):
+        """Generates the tick's query batch from the bindings (asynchronous); the next begin_interest(None) /
+        update_interest(None) or tick(None, flags | TICK_FOLLOW) consumes it."""
+        self._ck(self.L.chd_follow_queries(self.h, int(mode)))
+
+    def get_follow(self):
+        """-> dict(slot, entity, status, cx, cz: one entry per follower in slot order; n_selected)."""
+        n, sel = C.c_uint32(), C.c_uint32()
+        self._ck(self.L.chd_get_follow(self.h, None, None, None, None, None, 0, C.byref(n), C.byref(sel)))
+        k = n.value
+        slot, ent, st = np.zeros(k, np.uint32), np.zeros(k, np.uint32), np.zeros(k, np.uint32)
+        cx, cz = np.zeros(k), np.zeros(k)
+        if k:
+            self._ck(self.L.chd_get_follow(self.h, ptr(slot), ptr(ent), ptr(st), ptr(cx), ptr(cz), k, None, None))
+        return dict(slot=slot, entity=ent, status=st, cx=cx, cz=cz, n_selected=sel.value)
+
     def device_view(self, which):
         p, n = C.c_void_p(), C.c_uint64()
         self._ck(self.L.chd_device_view(self.h, which, C.byref(p), C.byref(n)))

@@ -327,6 +327,12 @@ class GpuStaticGrid2DSpatialController {
         Table();
         check(chd_move_entities_f32(engine_, net_id, x, z, n));
     }
+    // Connections whose interest follows their pawn: bound once (FollowEntities; kind == nullptr: all sphere, shape arrays of unused
+    // kinds nullptr), then FollowQueries builds each tick's UPDATE_SPATIAL_INTEREST batch on the device; BeginInterest(nullptr, ..)
+    // or Tick(nullptr, .., flags | CHD_TICK_FOLLOW) consumes it.  net_id: the entity index outside entity-table mode.
+    void FollowEntities(const chd_follow_batch& b) { check(chd_follow_bind(engine_, &b)); }
+    void UnfollowEntities(const std::vector<uint32_t>& slot) { check(chd_follow_unbind(engine_, slot.data(), (uint32_t)slot.size())); }
+    void FollowQueries(uint32_t mode = CHD_FOLLOW_MOVED) { check(chd_follow_queries(engine_, mode)); }
     chd_entity_stats GetEntityStats() {
         chd_entity_stats s{};
         check(chd_get_entity_stats(engine_, &s));

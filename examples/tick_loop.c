@@ -164,6 +164,46 @@ int main(void) {
     }
     CHECK(chd_fetch_wait_delta(e, &sum, &dc)); /* the last tick */
     chd_destroy(e);
+
+    /* The same world without a position mirror on the host: entities are events keyed by id (entity-table mode) and every
+     * subscriber follows its pawn, so each tick is  move -> chd_follow_queries(MOVED) -> chd_begin_interest(NULL) -> chd_tick.
+     * Only the moved entities go up; the queries are generated on the device for the followers whose pawn moved. */
+    CHECK(chd_create(&cfg, &lim, 0, &e));
+    CHECK(chd_set_subscribers(e, conn, n_subs));
+    CHECK(chd_entity_table_init(e));
+    {
+        uint32_t* id = malloc(4ull * n_entities);
+        uint32_t* slot = malloc(4ull * n_subs);
+        uint32_t* pawn = malloc(4ull * n_subs);
+        for (uint32_t i = 0; i < n_entities; i++) id[i] = 3 * i + 1; /* NetGUID-like ids; 0 and 0xFFFFFFFF are reserved */
+        for (uint32_t j = 0; j < n_subs; j++) {
+            slot[j] = j;
+            pawn[j] = id[(uint64_t)j * (n_entities / n_subs)];
+        }
+        CHECK(chd_spawn_entities(e, id, st[0].x, st[0].z, n_entities, NULL));
+        chd_follow_batch fb;
+        memset(&fb, 0, sizeof fb);
+        fb.n = n_subs; /* kind == NULL: all sphere */
+        fb.slot = slot; fb.entity = pawn; fb.sph_r = st[0].r;
+        CHECK(chd_follow_bind(e, &fb));
+        const uint32_t n_moved = n_entities / 100;
+        uint32_t* mid = chd_alloc_pinned(4ull * n_moved);
+        for (int tick = 0; tick < 20; tick++) {
+            const int64_t now = (int64_t)(tick + 1) * tick_ns;
+            for (uint32_t i = 0; i < n_moved; i++) mid[i] = id[((uint64_t)i * 100 + (uint32_t)tick) % n_entities];
+            if (tick) CHECK(chd_move_entities(e, mid, st[tick & 1].x, st[tick & 1].z, n_moved)); /* stand-in positions */
+            CHECK(chd_follow_queries(e, tick ? CHD_FOLLOW_MOVED : CHD_FOLLOW_ALL));
+            CHECK(chd_begin_interest(e, NULL, now, 0));
+            CHECK(chd_tick(e, NULL, now, CHD_TICK_BUILD | CHD_TICK_EMIT, &sum));
+            /* after CHD_OVF_PAIRS / CHD_OVF_WINDOW in sum.overflow: generate the next batch with CHD_FOLLOW_ALL */
+        }
+        uint32_t followers = 0, selected = 0;
+        CHECK(chd_get_follow(e, NULL, NULL, NULL, NULL, NULL, 0, &followers, &selected));
+        printf("followers: %u bound, %u queries generated for the last tick, %llu pairs\n", followers, selected, (unsigned long long)sum.n_pairs);
+        chd_free_pinned(mid);
+        free(id); free(slot); free(pawn);
+    }
+    chd_destroy(e);
     free(conn);
     return 0;
 }

@@ -491,6 +491,52 @@ func (ctl *GpuStaticGrid2DSpatialController) DestroyObjects(netIds []uint32) ([]
 	return status, nil
 }
 
+// FollowEntities binds connection slots to the entities they stand on (chd_follow_bind); kind[i] is a CHD_AOI_SPHERE | BOX | CONE
+// mask (nil: all sphere) and shape the per-binding parameters in the order sph_r, box_ex, box_ez, cone_dx, cone_dz, cone_angle,
+// cone_r (a nil entry: no binding uses that kind).  The arrays are copied before the call returns, so Go slices are fine.
+// FollowQueries then generates each tick's interest batch on the device (mode CHD_FOLLOW_ALL / CHD_FOLLOW_MOVED); BeginInterest(nil)
+// or a Tick with CHD_TICK_FOLLOW consumes it.  Clients with a pawn are bound; server connections keep sending explicit queries.
+// UN-RUN like the rest of this file.
+func (ctl *GpuStaticGrid2DSpatialController) FollowEntities(slots, netIds []uint32, kind []uint8, shape [7][]float64) error {
+	if len(netIds) != len(slots) || len(slots) == 0 {
+		return errors.New("FollowEntities: array sizes differ or are empty")
+	}
+	var b C.chd_follow_batch
+	b.n = C.uint32_t(len(slots))
+	b.slot = (*C.uint32_t)(unsafe.Pointer(&slots[0]))
+	b.entity = (*C.uint32_t)(unsafe.Pointer(&netIds[0]))
+	if kind != nil {
+		b.kind = (*C.uint8_t)(unsafe.Pointer(&kind[0]))
+	}
+	dst := [7]**C.double{&b.sph_r, &b.box_ex, &b.box_ez, &b.cone_dx, &b.cone_dz, &b.cone_angle, &b.cone_r}
+	for i, a := range shape {
+		if a != nil {
+			*dst[i] = (*C.double)(unsafe.Pointer(&a[0]))
+		}
+	}
+	if st := C.chd_follow_bind(ctl.engine, &b); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
+func (ctl *GpuStaticGrid2DSpatialController) UnfollowEntities(slots []uint32) error {
+	if len(slots) == 0 {
+		return nil
+	}
+	if st := C.chd_follow_unbind(ctl.engine, (*C.uint32_t)(unsafe.Pointer(&slots[0])), C.uint32_t(len(slots))); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
+func (ctl *GpuStaticGrid2DSpatialController) FollowQueries(mode uint32) error {
+	if st := C.chd_follow_queries(ctl.engine, C.uint32_t(mode)); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
 // MoveEntities: netIds / x / z in C memory, valid until the next Summary / FetchResults.  The last move of an id in one call wins;
 // moves of ids that are not live are ignored (counted in EntityStats).
 func (ctl *GpuStaticGrid2DSpatialController) MoveEntities(netIds []uint32, x, z []float32) error {

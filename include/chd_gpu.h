@@ -280,6 +280,9 @@ typedef struct chd_tick_summary {
  *                   the diff lists are empty; required_pairs = the total the update would have needed
  *   CHD_OVF_WINDOW  the queries whose cell windows did not fit got CHD_Q_ERR_CAPACITY and, like any failed query, left their
  *                   subscribers untouched; the rest of the batch was applied; required_window_cells = scratch needed
+ *                   (either of these two on a tick whose batch came from chd_follow_queries(CHD_FOLLOW_MOVED): the followers'
+ *                   stored centres advanced when the batch was generated, not when it was applied, so re-issue the tick's queries
+ *                   with chd_follow_queries(CHD_FOLLOW_ALL))
  *   CHD_OVF_VISIBLE the expanded visible list was not written (offsets are valid); required_visible = entries needed
  *   CHD_OVF_DUE     the pairs whose decisions did not fit were left untouched (still due: they catch up at the next
  *                   chd_fanout_tick); the list holds the decisions that did fit plus CHD_DUE_VOID holes; required_due
@@ -310,14 +313,17 @@ enum {
     CHD_TICK_EARLY_RESULTS = 8,
     /* Run chd_visible_delta after the build and the interest update (with or without CHD_TICK_EMIT).  In a two-stream tick it
      * runs on a third stream next to the expanded-list kernel and the fan-out pass; the engine stream waits for it. */
-    CHD_TICK_VISIBLE_DELTA = 16
+    CHD_TICK_VISIBLE_DELTA = 16,
+    /* The tick's query batch is the one chd_follow_queries generated (pass q == NULL): the interest update consumes it as it
+     * consumes a batch given in q.  CHD_ERR_STATE if no generated batch is waiting, CHD_ERR_INVALID together with q != NULL. */
+    CHD_TICK_FOLLOW = 32
 };
 /* Optional early start: the interest update (and the fan-out pass when with_fanout != 0) do not depend on the entity
  * positions, so a host can start them as soon as the tick's queries and rings are known — on the engine's second
  * stream — and then upload / exchange positions; the following chd_tick(e, NULL, t_ns, flags, ..) runs build + emit
  * and joins.  Used by the multi-GPU driver to overlap the border exchange with the interest stage.
  * q == NULL (here and in chd_update_interest) = the batch uploaded by chd_prefetch_queries and handed over by
- * chd_adopt_prefetched; CHD_ERR_STATE if there is none. */
+ * chd_adopt_prefetched, or the batch generated by chd_follow_queries; CHD_ERR_STATE if there is none. */
 chd_status chd_begin_interest(chd_engine* e, const chd_query_batch* q, int64_t t_ns, int with_fanout);
 chd_status chd_tick(chd_engine* e, const chd_query_batch* q, int64_t t_ns, uint32_t flags, chd_tick_summary* out);
 
@@ -472,6 +478,66 @@ chd_status chd_despawn_entities(chd_engine* e, const uint32_t* id, uint32_t n, u
 chd_status chd_move_entities(chd_engine* e, const uint32_t* id, const double* x, const double* z, uint32_t n);
 chd_status chd_move_entities_f32(chd_engine* e, const uint32_t* id, const float* x, const float* z, uint32_t n);
 chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out);
+
+/* ---- followers: subscriber slots whose area of interest is centred on an entity ("a player stands on its pawn").  The engine
+ * holds the positions already (after the tick's entity events or position upload), so it can build the tick's query batch itself:
+ * the host binds slot -> (entity, AOI shape) once and then asks for the batch each tick, instead of mirroring every followed
+ * entity's position and packing and uploading 28-33 bytes per subscriber per tick.
+ *   chd_follow_bind     binds (or re-binds: that is how a shape or direction changes) slot[i] to entity[i] with the shape given by
+ *                       kind[i], a mask out of CHD_AOI_SPHERE | CHD_AOI_BOX | CHD_AOI_CONE; every kind of one follower is centred
+ *                       on the entity.  CHD_AOI_SPOTS has absolute positions and is refused.  entity[i] is the entity index; in
+ *                       entity-table mode it is the table id (with chd_set_entity_ids, ids without a table, it stays the index).
+ *                       A slot named twice in one call: the last one wins.  Arrays are HOST memory, copied before the call returns.
+ *                       CHD_ERR_INVALID (nothing is bound): a slot that was never added (>= the slot count), a kind of 0 or with
+ *                       other bits, a kind whose shape arrays are NULL; CHD_ERR_CAPACITY: more followers than
+ *                       chd_limits.max_queries.  The per-slot state is allocated by the first call.
+ *   chd_follow_unbind   the slots follow nothing from now on; their subscriptions stay as they are.  chd_remove_subscribers
+ *                       unbinds the removed slots, chd_set_subscribers unbinds every slot.
+ *   chd_follow_queries  generates the batch on the engine stream, ordered after every entity event / position upload or adoption
+ *                       enqueued before it; asynchronous, no host synchronisation.  The batch is the one a host would have packed:
+ *                       one query per selected follower, sub = its slot, centre = the f64 position the build reads for its entity
+ *                       (after f32 widening, after the last-wins election of moves), shape from the binding, selected followers
+ *                       in ascending slot order.  CHD_FOLLOW_ALL selects every follower whose entity exists.  CHD_FOLLOW_MOVED
+ *                       selects a follower whose entity exists and whose binding is new or changed since the last batch that
+ *                       selected it, or whose entity's position differs BITWISE from the centre of the last query generated for
+ *                       it; skipping the others is sound, an identical query gives identical subscriptions (kept pairs keep their
+ *                       fan-out state and interval, subscription.go:44-57).  A follower whose entity does not exist (index >= the
+ *                       entity count; id not live in the table — a slot reused by another id is not followed) gets no query and
+ *                       keeps its subscriptions, like a connection that sent no update; when the id is spawned again the follower
+ *                       resumes and counts as moved.  An entity outside the world gives CHD_Q_ERR_OUT_OF_WORLD from the query
+ *                       path as for any batch.  The batch has one entry per FOLLOWER (B): entries behind the selected ones are
+ *                       skip entries (sub = 0xFFFFFFFF, kind = 0, status CHD_Q_OK), so the batch length the interest stage and
+ *                       chd_get_query_status / the status list of chd_fetch_results* see is B, and entry i below the selected
+ *                       count is the i-th selected follower in slot order.  No followers: an empty batch (which still applies
+ *                       pending lifecycle changes).
+ *                       The batch is handed over like an adopted prefetched batch: the next chd_begin_interest /
+ *                       chd_update_interest with q == NULL, or chd_tick with CHD_TICK_FOLLOW, consumes it.  One batch per interest
+ *                       update: CHD_ERR_STATE while an adopted prefetched batch or an earlier generated one is unconsumed, and
+ *                       while a chd_begin_interest is pending; chd_adopt_prefetched of a query batch is refused while a generated
+ *                       one is unconsumed.  Queries of subscribers that follow nothing go through chd_update_interest in an
+ *                       update of their own.
+ *   chd_get_follow      after the interest update that consumed the batch (and before the next one): per follower, in ascending
+ *                       slot order, its slot, entity, the centre of the last query generated for it, and status = the CHD_Q_*
+ *                       status of its query, or CHD_FOLLOW_NOT_SELECTED / CHD_FOLLOW_NO_ENTITY.  *count = followers (copies
+ *                       min(count, cap)), *n_selected = queries in the last generated batch; this call is where the selected count
+ *                       is reported (chd_tick_summary is unchanged).  Synchronous; any pointer may be NULL.
+ * Followers are single-GPU: CHD_ERR_STATE on an engine made a slab (chd_set_slab / chd_comm_init; a follower's entity may live on
+ * another rank, and border records carry no positions), and those two calls are refused once a slot follows.  Not supported:
+ * centre offsets, cone directions taken from an entity's rotation, spots relative to an entity. */
+typedef struct chd_follow_batch {          /* SoA, HOST arrays */
+    uint32_t n;
+    const uint32_t* slot;                  /* [n] subscriber slot */
+    const uint32_t* entity;                /* [n] entity index, or table id in entity-table mode */
+    const uint8_t*  kind;                  /* [n] CHD_AOI_SPHERE | BOX | CONE mask, NULL = all CHD_AOI_SPHERE */
+    const double *sph_r, *box_ex, *box_ez, *cone_dx, *cone_dz, *cone_angle, *cone_r; /* [n] each; NULL if no binding uses the kind */
+} chd_follow_batch;
+enum { CHD_FOLLOW_ALL = 0, CHD_FOLLOW_MOVED = 1 };
+enum { CHD_FOLLOW_NOT_SELECTED = 16, CHD_FOLLOW_NO_ENTITY = 17 }; /* beside CHD_Q_* in chd_get_follow's status */
+chd_status chd_follow_bind(chd_engine* e, const chd_follow_batch* b);
+chd_status chd_follow_unbind(chd_engine* e, const uint32_t* slot, uint32_t n);
+chd_status chd_follow_queries(chd_engine* e, uint32_t mode);
+chd_status chd_get_follow(chd_engine* e, uint32_t* slot, uint32_t* entity, uint32_t* status, double* cx, double* cz, uint32_t cap,
+                          uint32_t* count, uint32_t* n_selected);
 
 /* ---- all host-facing results of a tick in ONE call instead of one or two synchronisations per getter.  After a
  * two-stream tick (chd_tick with emit, or chd_begin_interest + chd_tick) the lists are copied in the order they become
@@ -730,6 +796,7 @@ enum { CHD_STAGE_BUILD = 0, CHD_STAGE_INTEREST, CHD_STAGE_EMIT, CHD_STAGE_EMIT_K
        CHD_STAGE_READBACK,                                     /* chd_fetch_results_async: the PCIe hop (snapshot -> pinned host) */
        CHD_STAGE_VISIBLE_DELTA,                                /* chd_visible_delta / CHD_TICK_VISIBLE_DELTA */
        CHD_STAGE_ENTITY_EVENTS,                                /* chd_spawn_entities* / chd_move_entities* / chd_despawn_entities */
+       CHD_STAGE_FOLLOW,                                       /* chd_follow_queries */
        CHD_STAGE_COUNT };
 uint64_t chd_launch_count(const chd_engine* e);
 /* The launch-bound stages (build, interest update, emit preparation, fan-out) are replayed as CUDA graphs once
