@@ -14,6 +14,89 @@
 namespace chd {
 
 
+// Block-aggregated append of the entities whose cell changed (the prefix of Notify, spatial.go:612-626): one global atomic per
+// block and call, which every thread of the block makes.  Entity i moved from key p to key c; the list holds channel ids, 0 =
+// outside the world (GetChannelId error, spatial.go:613-622).  reset: zero the block's counter for the next call.
+__device__ __forceinline__ void handover_append(const GridDev& g, const HandoverOut& ho, uint32_t& s_cnt, uint32_t& s_base, bool moved,
+                                                uint32_t i, uint32_t p, uint32_t c, bool reset) {
+    uint32_t my = 0;
+    if (moved) my = atomicAdd(&s_cnt, 1u);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        if (s_cnt) s_base = atomicAdd(ho.count, s_cnt);
+        if (reset) s_cnt = 0;
+    }
+    __syncthreads();
+    if (moved) {
+        const uint32_t slot = s_base + my;
+        if (slot < ho.cap) {
+            ho.entity[slot] = i;
+            ho.src_cell[slot] = p >= g.cells ? 0u : p + g.id_start;
+            ho.dst_cell[slot] = c >= g.cells ? 0u : c + g.id_start;
+        }
+    }
+}
+
+// A block's digit histogram in shared memory: cleared, then (after a barrier) written to column blockIdx.x of hist[digit][block]
+template <int BINS>
+__device__ __forceinline__ void hist_clear(uint32_t* s_hist) {
+    for (int d = threadIdx.x; d < BINS; d += BUILD_THREADS) s_hist[d] = 0;
+}
+template <int BINS>
+__device__ __forceinline__ void hist_flush(const uint32_t* s_hist, uint32_t* __restrict__ hist, uint32_t nblocks) {
+    __syncthreads();
+    for (int d = threadIdx.x; d < BINS; d += BUILD_THREADS) hist[(uint32_t)d * nblocks + blockIdx.x] = s_hist[d];
+}
+
+// Digit d's scanned base in block `block`'s column of hist_scanned.  Block 0's bases are the global exclusive counts per digit, so
+// in a single-pass sort (digit == key) they are the cell CSR offsets: with ex.cell_start set, block 0 publishes them (keys ==
+// cells mark out-of-world entities, so cell_start[cells] is the in-world count).  cell_start[cells + 1] = n is the caller's.
+__device__ __forceinline__ uint32_t load_base(const uint32_t* __restrict__ hist_scanned, uint32_t d, uint32_t nblocks, uint32_t block,
+                                              const ScatterExtras& ex) {
+    const uint32_t b = hist_scanned[d * nblocks + block];
+    if (ex.cell_start && block == 0) {
+        if (d <= ex.cells) ex.cell_start[d] = b;
+        if (d == ex.cells) *ex.n_in_world = b;
+    }
+    return b;
+}
+
+// A scatter block's bases (load_base of every digit) into s_base, and block 0 publishes the end of the cell CSR.
+template <int BINS>
+__device__ __forceinline__ void load_bases(uint32_t* s_base, const uint32_t* __restrict__ hist_scanned, uint32_t nblocks, uint32_t n,
+                                           const ScatterExtras& ex) {
+    for (int d = threadIdx.x; d < BINS; d += BUILD_THREADS) s_base[d] = load_base(hist_scanned, d, nblocks, blockIdx.x, ex);
+    if (ex.cell_start && blockIdx.x == 0 && threadIdx.x == 0) ex.cell_start[ex.cells + 1] = n;
+}
+
+// Loads a tile's keys and values (warp w: the run of 32 * BUILD_ROUNDS from tile + w * 32 * BUILD_ROUNDS, one element per lane and
+// round; val_in == nullptr: value = index) and ranks each element among the warp's earlier ones with the same digit: rk = the
+// warp's count of the digit so far (wcnt, the warp's row of counters, which the lowest lane holding the digit advances) + the
+// lane's rank among its peers.  Lanes past hi take part in the match only.
+template <typename Cnt>
+__device__ __forceinline__ void load_and_rank(const uint32_t* __restrict__ key_in, const uint32_t* __restrict__ val_in, uint32_t tile, uint32_t hi,
+                                              uint32_t shift, uint32_t mask, Cnt* wcnt, uint32_t (&k)[BUILD_ROUNDS], uint32_t (&v)[BUILD_ROUNDS],
+                                              uint32_t (&rk)[BUILD_ROUNDS]) {
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const uint32_t lt_mask = (1u << lane) - 1u;
+#pragma unroll
+    for (int r = 0; r < BUILD_ROUNDS; r++) {
+        const uint32_t i = tile + w * (32 * BUILD_ROUNDS) + r * 32 + lane;
+        const bool valid = i < hi;
+        k[r] = valid ? key_in[i] : 0u;
+        v[r] = valid ? (val_in ? val_in[i] : i) : 0u;
+        const uint32_t d = valid ? ((k[r] >> shift) & mask) : 0xFFFFFFFFu;
+        const uint32_t peers = __match_any_sync(0xffffffffu, d);
+        const uint32_t rank = __popc(peers & lt_mask);
+        uint32_t cnt = 0;
+        if (valid) cnt = wcnt[d];
+        __syncwarp();
+        if (valid && rank == 0) wcnt[d] = (Cnt)(cnt + __popc(peers));
+        __syncwarp();
+        rk[r] = cnt + rank;
+    }
+}
+
 // cell key per entity (+ optional handover detection against the previous build's keys:
 // the prefix of Notify, spatial.go:612-626: GetChannelId(old) != GetChannelId(new)).
 __global__ void __launch_bounds__(256) assign_cells_kernel(GridDev g, const double* __restrict__ x, const double* __restrict__ z,
@@ -27,7 +110,7 @@ __global__ void __launch_bounds__(256) assign_cells_kernel(GridDev g, const doub
         if (threadIdx.x == 0) s_cnt = 0;
         __syncthreads();
     }
-    uint32_t c = g.cells, p = g.cells, my = 0;
+    uint32_t c = g.cells, p = g.cells;
     bool moved = false;
     if (i < n) {
         c = cell_index(g, x[i], z[i]);
@@ -38,21 +121,7 @@ __global__ void __launch_bounds__(256) assign_cells_kernel(GridDev g, const doub
             moved = p != c;
         }
     }
-    if (prev_key) {
-        // block-aggregated append: one global atomic per block instead of one per crossing entity
-        if (moved) my = atomicAdd(&s_cnt, 1u);
-        __syncthreads();
-        if (threadIdx.x == 0 && s_cnt) s_base = atomicAdd(ho.count, s_cnt);
-        __syncthreads();
-        if (moved) {
-            const uint32_t slot = s_base + my;
-            if (slot < ho.cap) {  // channel ids; 0 = outside the world (GetChannelId error, spatial.go:613-622)
-                ho.entity[slot] = i;
-                ho.src_cell[slot] = p >= g.cells ? 0u : p + g.id_start;
-                ho.dst_cell[slot] = c >= g.cells ? 0u : c + g.id_start;
-            }
-        }
-    }
+    if (prev_key) handover_append(g, ho, s_cnt, s_base, moved, i, p, c, false);
 }
 
 // assign_cells_kernel + the first pass's radix_hist_kernel in ONE launch (single-GPU build: one launch and one pass over the keys
@@ -66,14 +135,14 @@ __global__ void __launch_bounds__(BUILD_THREADS)
     __shared__ uint32_t s_hist[BINS];
     __shared__ uint32_t s_cnt, s_base;
     if (bump_epoch && blockIdx.x == 0 && threadIdx.x == 0) *bump_epoch = chd_next_epoch(*bump_epoch);
-    for (int d = threadIdx.x; d < BINS; d += BUILD_THREADS) s_hist[d] = 0;
+    hist_clear<BINS>(s_hist);
     if (threadIdx.x == 0) s_cnt = 0;
     __syncthreads();
     const uint32_t lo = min(n, blockIdx.x * per_block);
     const uint32_t hi = min(n, lo + per_block);
     for (uint32_t base = lo; base < hi; base += BUILD_THREADS) {
         const uint32_t i = base + threadIdx.x;
-        uint32_t c = g.cells, p = g.cells, my = 0;
+        uint32_t c = g.cells, p = g.cells;
         bool moved = false;
         if (i < hi) {
             c = cell_index(g, x[i], z[i]);
@@ -85,27 +154,12 @@ __global__ void __launch_bounds__(BUILD_THREADS)
                 moved = p != c;
             }
         }
-        if (prev_key) {  // block-aggregated append of the entities whose cell changed (prefix of Notify, spatial.go:612-626)
-            if (moved) my = atomicAdd(&s_cnt, 1u);
-            __syncthreads();
-            if (threadIdx.x == 0) {
-                s_base = s_cnt ? atomicAdd(ho.count, s_cnt) : 0u;
-                s_cnt = 0;
-            }
-            __syncthreads();
-            if (moved) {
-                const uint32_t slot = s_base + my;
-                if (slot < ho.cap) {
-                    ho.entity[slot] = i;
-                    ho.src_cell[slot] = p >= g.cells ? 0u : p + g.id_start;
-                    ho.dst_cell[slot] = c >= g.cells ? 0u : c + g.id_start;
-                }
-            }
+        if (prev_key) {
+            handover_append(g, ho, s_cnt, s_base, moved, i, p, c, true);
             __syncthreads();  // s_base is rewritten in the next step
         }
     }
-    __syncthreads();
-    for (int d = threadIdx.x; d < BINS; d += BUILD_THREADS) hist[(uint32_t)d * nblocks + blockIdx.x] = s_hist[d];
+    hist_flush<BINS>(s_hist, hist, nblocks);
 }
 
 // per-block digit histogram; hist layout [digit][block]
@@ -117,13 +171,12 @@ __global__ void __launch_bounds__(BUILD_THREADS)
     // first kernel of the build stage: opens a new epoch for the stage's look-back scans (chd_scan.cuh)
     if (bump_epoch && blockIdx.x == 0 && threadIdx.x == 0) *bump_epoch = chd_next_epoch(*bump_epoch);
     if (n_ptr) n = min(n, *n_ptr);  // live length on the device (multi-GPU: own + halo entities)
-    for (int d = threadIdx.x; d < BINS; d += BUILD_THREADS) s_hist[d] = 0;
+    hist_clear<BINS>(s_hist);
     __syncthreads();
     const uint32_t lo = min(n, blockIdx.x * per_block);
     const uint32_t hi = min(n, lo + per_block);
     for (uint32_t i = lo + threadIdx.x; i < hi; i += BUILD_THREADS) atomicAdd(&s_hist[(key[i] >> shift) & mask], 1u);
-    __syncthreads();
-    for (int d = threadIdx.x; d < BINS; d += BUILD_THREADS) hist[(uint32_t)d * nblocks + blockIdx.x] = s_hist[d];
+    hist_flush<BINS>(s_hist, hist, nblocks);
 }
 
 // stable scatter of one pass.  val_in == nullptr means "value = index" (first pass).
@@ -136,39 +189,15 @@ __global__ void __launch_bounds__(BUILD_THREADS)
     __shared__ uint32_t s_tot[BINS];
     __shared__ uint32_t s_wcnt[BUILD_WARPS][BINS];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const uint32_t lt_mask = (1u << lane) - 1u;
     if (n_ptr) n = min(n, *n_ptr);
-    for (int d = threadIdx.x; d < BINS; d += BUILD_THREADS) {
-        const uint32_t b = hist_scanned[(uint32_t)d * nblocks + blockIdx.x];
-        s_base[d] = b;
-        if (ex.cell_start && blockIdx.x == 0) {  // block 0's bases are the global exclusive counts per key
-            if ((uint32_t)d <= ex.cells) ex.cell_start[d] = b;
-            if ((uint32_t)d == ex.cells) *ex.n_in_world = b;  // keys == cells mark out-of-world entities
-            if (d == 0) ex.cell_start[ex.cells + 1] = n;
-        }
-    }
+    load_bases<BINS>(s_base, hist_scanned, nblocks, n, ex);
     const uint32_t lo = min(n, blockIdx.x * per_block);
     const uint32_t hi = min(n, lo + per_block);
     for (uint32_t tile = lo; tile < hi; tile += BUILD_TILE) {
         for (int d = threadIdx.x; d < BINS * BUILD_WARPS; d += BUILD_THREADS) (&s_wcnt[0][0])[d] = 0;
         __syncthreads();
         uint32_t k[BUILD_ROUNDS], v[BUILD_ROUNDS], rk[BUILD_ROUNDS];
-#pragma unroll
-        for (int r = 0; r < BUILD_ROUNDS; r++) {
-            const uint32_t i = tile + w * (32 * BUILD_ROUNDS) + r * 32 + lane;
-            const bool valid = i < hi;
-            k[r] = valid ? key_in[i] : 0u;
-            v[r] = valid ? (val_in ? val_in[i] : i) : 0u;
-            const uint32_t d = valid ? ((k[r] >> shift) & mask) : 0xFFFFFFFFu;
-            const uint32_t peers = __match_any_sync(0xffffffffu, d);
-            const uint32_t rank = __popc(peers & lt_mask);
-            uint32_t cnt = 0;
-            if (valid) cnt = s_wcnt[w][d];
-            __syncwarp();
-            if (valid && rank == 0) s_wcnt[w][d] = cnt + __popc(peers);
-            __syncwarp();
-            rk[r] = cnt + rank;
-        }
+        load_and_rank(key_in, val_in, tile, hi, shift, mask, s_wcnt[w], k, v, rk);
         __syncthreads();
         for (int d = threadIdx.x; d < BINS; d += BUILD_THREADS) {
             uint32_t run = 0;
@@ -212,40 +241,16 @@ __global__ void __launch_bounds__(BUILD_THREADS)
     __shared__ uint32_t s_key[BUILD_TILE], s_val[BUILD_TILE];
     __shared__ uint32_t s_scan[BUILD_WARPS];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const uint32_t lt_mask = (1u << lane) - 1u;
     constexpr int DPT = BINS / BUILD_THREADS;  // digits per thread in the prefix step
     if (n_ptr) n = min(n, *n_ptr);
-    for (int d = threadIdx.x; d < BINS; d += BUILD_THREADS) {
-        const uint32_t b = hist_scanned[(uint32_t)d * nblocks + blockIdx.x];
-        s_base[d] = b;
-        if (ex.cell_start && blockIdx.x == 0) {
-            if ((uint32_t)d <= ex.cells) ex.cell_start[d] = b;
-            if ((uint32_t)d == ex.cells) *ex.n_in_world = b;
-            if (d == 0) ex.cell_start[ex.cells + 1] = n;
-        }
-    }
+    load_bases<BINS>(s_base, hist_scanned, nblocks, n, ex);
     const uint32_t lo = min(n, blockIdx.x * per_block);
     const uint32_t hi = min(n, lo + per_block);
     for (uint32_t tile = lo; tile < hi; tile += BUILD_TILE) {
         for (int d = threadIdx.x; d < BINS * BUILD_WARPS; d += BUILD_THREADS) (&s_wcnt[0][0])[d] = 0;
         __syncthreads();
         uint32_t k[BUILD_ROUNDS], v[BUILD_ROUNDS], rk[BUILD_ROUNDS];
-#pragma unroll
-        for (int r = 0; r < BUILD_ROUNDS; r++) {
-            const uint32_t i = tile + w * (32 * BUILD_ROUNDS) + r * 32 + lane;
-            const bool valid = i < hi;
-            k[r] = valid ? key_in[i] : 0u;
-            v[r] = valid ? (val_in ? val_in[i] : i) : 0u;
-            const uint32_t d = valid ? ((k[r] >> shift) & mask) : 0xFFFFFFFFu;
-            const uint32_t peers = __match_any_sync(0xffffffffu, d);
-            const uint32_t rank = __popc(peers & lt_mask);
-            uint32_t cnt = 0;
-            if (valid) cnt = s_wcnt[w][d];
-            __syncwarp();
-            if (valid && rank == 0) s_wcnt[w][d] = (uint16_t)(cnt + __popc(peers));
-            __syncwarp();
-            rk[r] = cnt + rank;
-        }
+        load_and_rank(key_in, val_in, tile, hi, shift, mask, s_wcnt[w], k, v, rk);
         __syncthreads();
         // per digit: warp counts -> exclusive offsets across warps; tile totals -> exclusive prefix across digits
         uint32_t tot[DPT], sum = 0;
@@ -307,19 +312,14 @@ __global__ void __launch_bounds__(BUILD_THREADS)
     }
 }
 
-// single-pass builds: the cell CSR offsets straight from the scanned histogram (block 0's bases are the global exclusive counts
-// per key), published BEFORE the scatter runs so that the emit preparation can overlap it
-__global__ void __launch_bounds__(256) publish_cell_start_kernel(const uint32_t* __restrict__ hist_scanned, uint32_t nblocks, uint32_t cells, uint32_t n,
-                                                                 const uint32_t* __restrict__ n_ptr, uint32_t* __restrict__ cell_start,
-                                                                 uint32_t* __restrict__ n_in_world) {
+// single-pass builds: the cell CSR offsets straight from the scanned histogram (load_base of block 0), published BEFORE the
+// scatter runs so that the emit preparation can overlap it
+__global__ void __launch_bounds__(256) publish_cell_start_kernel(const uint32_t* __restrict__ hist_scanned, uint32_t nblocks, uint32_t n,
+                                                                 const uint32_t* __restrict__ n_ptr, ScatterExtras ex) {
     const uint32_t d = blockIdx.x * blockDim.x + threadIdx.x;
     if (n_ptr) n = min(n, *n_ptr);
-    if (d <= cells) {
-        const uint32_t b = hist_scanned[d * nblocks];
-        cell_start[d] = b;
-        if (d == cells) *n_in_world = b;  // keys == cells mark out-of-world entities
-    }
-    if (d == 0) cell_start[cells + 1] = n;
+    if (d <= ex.cells) load_base(hist_scanned, d, nblocks, 0, ex);
+    if (d == 0) ex.cell_start[ex.cells + 1] = n;
 }
 
 // cell_start[c] = first sorted position whose key >= c, for c in [0, C+1]; cell_start[C+1] = n.

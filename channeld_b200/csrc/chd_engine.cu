@@ -186,6 +186,16 @@ static bool alloc_pairbuf(chd_engine* e, PairBuf& pb) {
            dalloc(e, &pb.last_index, P);
 }
 
+// a sort by cell on `blocks` blocks, its scans in `stage`.  The caller allocates the temporaries in their place in chd_create's
+// order: where the large buffers land moves the emit kernel's time (moving the entity sort's here cost 1.5 % of bench.py's
+// benchmark config on an H100 80GB HBM3 at 700 W)
+static bool alloc_cell_sort(chd_engine* e, CellSort& cs, uint32_t blocks, bool whole_grid, int stage) {
+    const uint64_t bins = (uint64_t)BUILD_MAX_BINS * blocks;
+    cs.blocks = blocks;
+    cs.whole_grid = whole_grid;
+    return dalloc(e, &cs.hist, bins + 2) && chd_make_site(e, cs.site[0], bins + 1, stage) && chd_make_site(e, cs.site[1], bins + 1, stage);
+}
+
 chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int device, chd_engine** out) {
     if (!cfg || !out) {
         g_create_error = "null argument";
@@ -267,16 +277,8 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     g.default_interval_ms = L.default_fanout_interval_ms; g.default_delay_ms = L.default_fanout_delay_ms;
 
     const uint64_t N = L.max_entities, S = L.max_subscribers, Q = L.max_queries, P = L.max_pairs, C = g.cells;
-    e->build_blocks = (uint32_t)e->sm_count * 4;
-    e->pc_blocks = (uint32_t)std::min<uint64_t>(4096, (P + BUILD_TILE - 1) / BUILD_TILE);
-    if (e->pc_blocks == 0) e->pc_blocks = 1;
     e->ho_cap = L.max_entities;
     e->max_tiles = (L.max_visible + EMIT_WARP_TILE - 1) / EMIT_WARP_TILE + 1;  // (the smaller of the two tile sizes)
-    uint64_t scan_n = (uint64_t)BUILD_MAX_BINS * e->build_blocks + 1;
-    if (P + 1 > scan_n) scan_n = P + 1;
-    if (Q + 1 > scan_n) scan_n = Q + 1;
-    if (S + 1 > scan_n) scan_n = S + 1;
-    if (N + 1 > scan_n) scan_n = N + 1;
     // the aux stream carries short latency-bound kernels that should slot in ahead of the long emit kernel
     bool ok = chd_make_stream(e, &e->aux_stream) && chd_make_stream(e, &e->dl_stream) && chd_make_stream(e, &e->dl_stream_b) &&
               chd_make_stream(e, &e->prep_stream);
@@ -286,15 +288,13 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     e->pf_pos.next = 1;
     ok = ok && dalloc(e, &e->d_x, N) && dalloc(e, &e->d_z, N) && (e->d_xb[0] = e->d_x, e->d_zb[0] = e->d_z, true) &&
          dalloc(e, &e->d_gid, N) && dalloc(e, &e->d_key, N) &&
-         dalloc(e, &e->d_prev_key, N) && dalloc(e, &e->d_tmp_key, N) && dalloc(e, &e->d_tmp_val, N) &&
+         dalloc(e, &e->d_prev_key, N) && dalloc(e, &e->ent_sort.tmp_key, N) && dalloc(e, &e->ent_sort.tmp_val, N) &&
          dalloc(e, &e->d_sorted_key, N) &&
          // padded: an emit chunk that starts m != 0 entries into an aligned 16-byte chunk also loads the next aligned chunk,
          // which near the end of the array lies past N (chd_emit.cuh)
          dalloc(e, &e->d_sorted_ent, ((N + 3) / 4) * 4 + 8) && dalloc(e, &e->d_cell_start, C + 2) &&
-         dalloc(e, &e->d_hist, (uint64_t)BUILD_MAX_BINS * e->build_blocks + 2) &&
          dalloc(e, &e->d_epoch, EP_COUNT) && chd_init_epochs(e) &&
-         chd_make_site(e, e->site_hist, (uint64_t)BUILD_MAX_BINS * e->build_blocks + 1, EP_BUILD) &&
-         chd_make_site(e, e->site_hist_b, (uint64_t)BUILD_MAX_BINS * e->build_blocks + 1, EP_BUILD) &&
+         alloc_cell_sort(e, e->ent_sort, (uint32_t)e->sm_count * 4, false, EP_BUILD) &&
          chd_make_site(e, e->site_qoff, Q + 1, EP_QUERY) && chd_make_site(e, e->site_slot, S + 1, EP_QUERY) &&
          chd_make_site(e, e->site_voff, P + 1, EP_EMIT) &&
          chd_make_site(e, e->site_border, N + 1, EP_BORDER) &&
@@ -319,9 +319,8 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     ok = ok && dalloc(e, &e->d_ring_off, C + 1) && dalloc(e, &e->d_ring_arrival, (uint64_t)L.max_ring_entries) &&
          dalloc(e, &e->d_ring_sender, (uint64_t)L.max_ring_entries) && dalloc(e, &e->d_ring_index, (uint64_t)L.max_ring_entries) &&
          dalloc(e, &e->d_ch_msg_index, C) && dalloc(e, &e->d_by_cell, P) &&
-         dalloc(e, &e->d_pc_hist, (uint64_t)BUILD_MAX_BINS * e->pc_blocks + 2) && dalloc(e, &e->d_pc_tmp_key, P) && dalloc(e, &e->d_pc_tmp_val, P) &&
-         chd_make_site(e, e->site_pchist, (uint64_t)BUILD_MAX_BINS * e->pc_blocks + 1, EP_QUERY) &&
-         chd_make_site(e, e->site_pchist_b, (uint64_t)BUILD_MAX_BINS * e->pc_blocks + 1, EP_QUERY) &&
+         alloc_cell_sort(e, e->pair_sort, (uint32_t)std::min<uint64_t>(4096, (P + BUILD_TILE - 1) / BUILD_TILE), true, EP_QUERY) &&
+         dalloc(e, &e->pair_sort.tmp_key, P) && dalloc(e, &e->pair_sort.tmp_val, P) &&
          dalloc(e, &e->d_due, (uint64_t)L.max_due) && dalloc(e, &e->d_due_key, (uint64_t)L.max_due) && dalloc(e, &e->d_ctr, 1) && dalloc(e, &e->d_time, 2) &&
          dalloc(e, &e->d_ring_total, 1) && dalloc(e, &e->d_n_build, 1);
     if (!ok) {

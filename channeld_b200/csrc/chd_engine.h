@@ -2,7 +2,7 @@
 // Layout of the host code (all device buffers are allocated once in chd_create; the tick path allocates nothing and —
 // apart from chd_summary / the chd_get_* copies — never synchronises with the host):
 //   chd_engine.cu    create / destroy, streams, memory, the prefetch protocol, CUDA-graph stage cache, instrumentation
-//   chd_entities.cu  positions, cell assignment, spatial-hash build, radix sort passes
+//   chd_entities.cu  positions, cell assignment, spatial-hash build, the cell sort (chd_cell_sort)
 //   chd_interest.cu  subscribers (lifecycle), query batches, QueryChannelIds, interest update
 //   chd_tick.cu      emit, rings, fan-out, the batched tick and its two-stream choreography, summary
 //   chd_results.cu   getters, chd_fetch_results, device views
@@ -43,6 +43,18 @@ struct Prefetch {
     bool wait = false;  // the reader of `cur` has not been ordered after its upload yet
     cudaEvent_t ev_upload = nullptr, ev_read[2] = {nullptr, nullptr};
     bool read_recorded[2] = {false, false};
+};
+
+// One stable LSD radix sort by cell (chd_cell_sort), allocated by chd_create: the [digit][block] histogram, one look-back scan
+// site per pass, the grid and pass 0's output when the sort takes two passes.
+struct CellSort {
+    uint32_t* hist = nullptr;  // [BUILD_MAX_BINS * blocks + 2]
+    ScanSite site[2] = {};
+    uint32_t blocks = 0;
+    // true: every launch runs all `blocks` blocks, idle ones included (the pair grouping); false: only the blocks whose slice
+    // starts below the length (the entity build)
+    bool whole_grid = false;
+    uint32_t *tmp_key = nullptr, *tmp_val = nullptr;
 };
 
 struct chd_engine {
@@ -116,15 +128,16 @@ struct chd_engine {
     const double *pos_x = nullptr, *pos_z = nullptr;  // what the kernels read: the staging buffers, or the caller's device arrays
     uint32_t *d_gid = nullptr;            // [max_entities] global ids (multi-GPU) of own + halo
     uint32_t *d_key = nullptr, *d_prev_key = nullptr;  // [max_entities] cell key per entity
-    uint32_t *d_tmp_key = nullptr, *d_tmp_val = nullptr, *d_sorted_key = nullptr, *d_sorted_ent = nullptr;
+    // the build's sort by cell: 4 blocks per SM, N-sized temporaries, which chd_get_rehome and chd_handoff_entities borrow as
+    // scratch between builds
+    CellSort ent_sort;
+    uint32_t *d_sorted_key = nullptr, *d_sorted_ent = nullptr;
     uint32_t *d_cell_start = nullptr;     // [C+2]
-    uint32_t *d_hist = nullptr;           // [BUILD_MAX_BINS * nblocks + 1]
     // one look-back scan site per call site: stages run concurrently on two streams and must not share scan state
     unsigned long long* d_epoch = nullptr;  // [EP_COUNT] stage epochs for the look-back scans
-    ScanSite site_hist_b{}, site_pchist_b{}, site_hist{}, site_qoff{}, site_slot{}, site_pchist{}, site_voff{}, site_border{};
+    ScanSite site_qoff{}, site_slot{}, site_voff{}, site_border{};
     uint64_t stage_execs[10] = {};  // [EP_COUNT]
     std::vector<ScanSite*> sites;  // every scan site (chd_make_site registers them)
-    uint32_t build_blocks = 0;
     bool assigned = false, built = false, have_prev_key = false, entities_dirty = false;
     uint32_t n_sorted = 0;
     bool sorted_dev_n = false;  // the last build's length was d_n_build (own + halo on the device), not n_sorted
@@ -253,8 +266,8 @@ struct chd_engine {
     // and chd_adopt_prefetched.
     RingDev ring{};
 
-    uint32_t *d_by_cell = nullptr, *d_pc_hist = nullptr, *d_pc_tmp_key = nullptr, *d_pc_tmp_val = nullptr;  // pairs grouped by cell
-    uint32_t pc_blocks = 0;
+    uint32_t* d_by_cell = nullptr;  // pairs grouped by cell
+    CellSort pair_sort;             // its sort: one block per tile of max_pairs, at most 4096; P-sized temporaries
     chd_due* d_due = nullptr;
     // counters
     Counters* d_ctr = nullptr;
@@ -500,10 +513,14 @@ chd_status chd_build_on(chd_engine* e, cudaStream_t s);
 chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query_batch* q, int64_t now_ns);
 // what the fan-out / payload kernels read: the host-owned CSR snapshot (staged or zero-copy) or the device-owned rings
 RingDev chd_ring_view(const chd_engine* e);
-// one stable LSD radix pass (histogram, look-back scan, scatter) over 32-bit keys; chd_entities.cu
-chd_status chd_sort_pass_any(chd_engine* e, cudaStream_t s, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in, uint32_t n,
-                             const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits, uint32_t* key_out,
-                             uint32_t* val_out, ScatterExtras ex = ScatterExtras{nullptr, 0, nullptr}, unsigned long long* bump = nullptr);
+// The stable sort by cell on `s` (chd_entities.cu): values val (nullptr: the index) of keys key[0, n) in [0, keys) (n_ptr: the
+// live length on the device) into val_out, in <= 2 passes of <= 10-bit digits.  key_out: where a two-pass sort writes the sorted
+// keys.  csr: the cell CSR to publish (nullptr: none).  bump: the epoch the first kernel opens.  assign: pass 0's histogram also
+// assigns the keys.  part: 0 = the whole sort; single-pass sorts only: 1 = histogram, scan and cell CSR, 2 = scatter.
+struct FusedAssign;
+chd_status chd_cell_sort(chd_engine* e, cudaStream_t s, const CellSort& cs, uint32_t keys, const uint32_t* key, const uint32_t* val, uint32_t n,
+                         const uint32_t* n_ptr, uint32_t* key_out, uint32_t* val_out, const ScatterExtras* csr = nullptr,
+                         unsigned long long* bump = nullptr, const FusedAssign* assign = nullptr, int part = 0);
 // the visible-set delta stage on `s` (chd_delta.cu)
 chd_status chd_delta_on(chd_engine* e, cudaStream_t s);
 // the mode rules (chd_table.cu, numbered as in DESIGN.md §5): CHD_OK, or the error set and CHD_ERR_STATE (6: or CHD_ERR_INVALID)

@@ -11,47 +11,88 @@ struct FusedAssign {
     const uint32_t* prev;
     HandoverOut ho;
 };
+
+// One radix pass: digit (key >> shift) & mask of key[0, n) (n_ptr: the live length on the device), values val (nullptr: the
+// index), block b of nblocks owns the slice [b * per_block, (b + 1) * per_block), histogram hist[digit][block].  Digits of up to
+// 8 bits take 256 bins, wider ones 1024.
+struct SortPass {
+    const uint32_t *key, *val;
+    uint32_t n;
+    const uint32_t* n_ptr;
+    uint32_t per_block, nblocks, shift, mask;
+    uint32_t* hist;
+};
+
+// The pass's digit histogram (with assign: the cell assignment computes the keys and counts them in the same launch) and its
+// exclusive scan, which leaves every block's base per digit
 template <int BINS>
-static chd_status sort_pass(chd_engine* e, cudaStream_t s, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in, uint32_t n,
-                            const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits, uint32_t* key_out,
-                            uint32_t* val_out, ScatterExtras ex, unsigned long long* bump, const FusedAssign* assign = nullptr, int half = 0) {
-    // half: 0 = the whole pass, 1 = histogram + scan only, 2 = scatter only (single-pass builds are split so that the emit
-    // preparation, which needs only the cell counts, overlaps the scatter)
-    const uint32_t mask = (1u << bits) - 1u;
-    if (half == 2) goto scatter;
+static chd_status count_digits(chd_engine* e, cudaStream_t s, const SortPass& p, const ScanSite& site, unsigned long long* bump,
+                               const FusedAssign* assign) {
     if (assign)
-        assign_hist_kernel<BINS><<<nblocks, BUILD_THREADS, 0, s>>>(e->g, assign->x, assign->z, n, assign->key, assign->prev, assign->ho, per_block, mask,
-                                                                   hist, nblocks, bump);
+        assign_hist_kernel<BINS><<<p.nblocks, BUILD_THREADS, 0, s>>>(e->g, assign->x, assign->z, p.n, assign->key, assign->prev, assign->ho, p.per_block,
+                                                                     p.mask, p.hist, p.nblocks, bump);
     else
-        radix_hist_kernel<BINS><<<nblocks, BUILD_THREADS, 0, s>>>(key_in, n, n_ptr, per_block, shift, mask, hist, nblocks, bump);
+        radix_hist_kernel<BINS><<<p.nblocks, BUILD_THREADS, 0, s>>>(p.key, p.n, p.n_ptr, p.per_block, p.shift, p.mask, p.hist, p.nblocks, bump);
     KCHECK(e);
-    SCAN(e, exclusive_scan_1p<uint32_t, uint32_t>(hist, hist, (uint64_t)BINS * nblocks, site, s));
-    if (half == 1) return CHD_OK;
-scatter:
-    // bandwidth-bound regime: reorder each tile by digit in shared memory first (coalesced runs); small inputs are latency-bound
-    // and take the plain scatter (fewer barriers per tile)
-    if (n > (2u << 20))
-        radix_scatter_sorted_kernel<BINS><<<nblocks, BUILD_THREADS, 0, s>>>(key_in, val_in, n, n_ptr, per_block, shift, mask, hist, nblocks,
-                                                                           key_out, val_out, ex);
+    SCAN(e, exclusive_scan_1p<uint32_t, uint32_t>(p.hist, p.hist, (uint64_t)BINS * p.nblocks, site, s));
+    return CHD_OK;
+}
+
+// The pass's stable scatter from the scanned histogram.  Bandwidth-bound regime: each tile is reordered by digit in shared memory
+// first (coalesced runs); small inputs are latency-bound and take the plain scatter (fewer barriers per tile).
+template <int BINS>
+static chd_status scatter_digits(chd_engine* e, cudaStream_t s, const SortPass& p, uint32_t* key_out, uint32_t* val_out, ScatterExtras ex) {
+    if (p.n > (2u << 20))
+        radix_scatter_sorted_kernel<BINS><<<p.nblocks, BUILD_THREADS, 0, s>>>(p.key, p.val, p.n, p.n_ptr, p.per_block, p.shift, p.mask, p.hist,
+                                                                             p.nblocks, key_out, val_out, ex);
     else
-        radix_scatter_kernel<BINS><<<nblocks, BUILD_THREADS, 0, s>>>(key_in, val_in, n, n_ptr, per_block, shift, mask, hist, nblocks,
-                                                                    key_out, val_out, ex);
+        radix_scatter_kernel<BINS><<<p.nblocks, BUILD_THREADS, 0, s>>>(p.key, p.val, p.n, p.n_ptr, p.per_block, p.shift, p.mask, p.hist, p.nblocks,
+                                                                      key_out, val_out, ex);
     KCHECK(e);
     return CHD_OK;
 }
 
-static chd_status sort_pass_fused(chd_engine* e, cudaStream_t s, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in,
-                                  uint32_t n, const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits, uint32_t* key_out,
-                                  uint32_t* val_out, ScatterExtras ex, unsigned long long* bump, const FusedAssign* assign, int half = 0) {
-    if (bits <= 8) return sort_pass<256>(e, s, hist, site, key_in, val_in, n, n_ptr, per_block, nblocks, shift, bits, key_out, val_out, ex, bump, assign, half);
-    return sort_pass<1024>(e, s, hist, site, key_in, val_in, n, n_ptr, per_block, nblocks, shift, bits, key_out, val_out, ex, bump, assign, half);
+static chd_status count_pass(chd_engine* e, cudaStream_t s, const SortPass& p, const ScanSite& site, unsigned long long* bump,
+                             const FusedAssign* assign) {
+    return p.mask < 256 ? count_digits<256>(e, s, p, site, bump, assign) : count_digits<1024>(e, s, p, site, bump, assign);
+}
+static chd_status scatter_pass(chd_engine* e, cudaStream_t s, const SortPass& p, uint32_t* key_out, uint32_t* val_out, ScatterExtras ex = {}) {
+    return p.mask < 256 ? scatter_digits<256>(e, s, p, key_out, val_out, ex) : scatter_digits<1024>(e, s, p, key_out, val_out, ex);
 }
 
-chd_status chd_sort_pass_any(chd_engine* e, cudaStream_t s, uint32_t* hist, const ScanSite& site, const uint32_t* key_in, const uint32_t* val_in,
-                                uint32_t n, const uint32_t* n_ptr, uint32_t per_block, uint32_t nblocks, uint32_t shift, uint32_t bits,
-                                uint32_t* key_out, uint32_t* val_out, ScatterExtras ex,
-                                unsigned long long* bump) {
-    return sort_pass_fused(e, s, hist, site, key_in, val_in, n, n_ptr, per_block, nblocks, shift, bits, key_out, val_out, ex, bump, nullptr);
+chd_status chd_cell_sort(chd_engine* e, cudaStream_t s, const CellSort& cs, uint32_t keys, const uint32_t* key, const uint32_t* val, uint32_t n,
+                         const uint32_t* n_ptr, uint32_t* key_out, uint32_t* val_out, const ScatterExtras* csr, unsigned long long* bump,
+                         const FusedAssign* assign, int part) {
+    uint32_t bits = 1;
+    while ((1u << bits) < keys) bits++;
+    const uint32_t bits0 = bits <= 10 ? bits : (bits + 1) / 2;  // <= 2 passes of <= 10-bit digits
+    // contiguous slice per block: a whole number of tiles, at least one
+    const uint32_t slice = (uint32_t)(((uint64_t)n + cs.blocks - 1) / cs.blocks);
+    const uint32_t per_block = std::max<uint32_t>(BUILD_TILE, (slice + BUILD_TILE - 1) / BUILD_TILE * BUILD_TILE);
+    const uint32_t nblocks = cs.whole_grid ? cs.blocks : std::max(1u, (n + per_block - 1) / per_block);
+    const SortPass p0{key, val, n, n_ptr, per_block, nblocks, 0, (1u << bits0) - 1u, cs.hist};
+    chd_status st = CHD_OK;
+    if (bits0 == bits) {  // one pass: digit == key, so block 0's scanned bases are the cell CSR offsets
+        if (part != 2) {
+            st = count_pass(e, s, p0, cs.site[0], bump, assign);
+            if (st != CHD_OK) return st;
+        }
+        if (part != 1) return scatter_pass(e, s, p0, nullptr, val_out, part == 0 && csr ? *csr : ScatterExtras{});
+        if (csr) {  // published before the scatter, so that the emit preparation can overlap it
+            publish_cell_start_kernel<<<blocks_for((uint64_t)csr->cells + 2, 256), 256, 0, s>>>(cs.hist, nblocks, n, n_ptr, *csr);
+            KCHECK(e);
+        }
+        return CHD_OK;
+    }
+    const SortPass p1{cs.tmp_key, cs.tmp_val, n, n_ptr, per_block, nblocks, bits0, (1u << (bits - bits0)) - 1u, cs.hist};
+    st = count_pass(e, s, p0, cs.site[0], bump, assign);
+    if (st == CHD_OK) st = scatter_pass(e, s, p0, cs.tmp_key, cs.tmp_val);
+    if (st == CHD_OK) st = count_pass(e, s, p1, cs.site[1], nullptr, nullptr);
+    if (st == CHD_OK) st = scatter_pass(e, s, p1, key_out, val_out);
+    if (st != CHD_OK || !csr) return st;
+    cell_bounds_kernel<<<blocks_for((uint64_t)n + 1, 256), 256, 0, s>>>(key_out, n, n_ptr, csr->cells, csr->cell_start, csr->n_in_world);
+    KCHECK(e);
+    return CHD_OK;
 }
 
 extern "C" {
@@ -294,49 +335,10 @@ static chd_status build_enqueue(chd_engine* e, cudaStream_t s, bool with_assign,
     // the entity capacity and blocks beyond the live length idle.
     const uint32_t* n_ptr = e->halo_on_device ? e->d_n_build : nullptr;
     const uint32_t n = e->halo_on_device ? e->lim.max_entities : e->n_own + e->n_halo;
-    const uint32_t C = e->g.cells;
-    uint32_t bits = 1;
-    while ((1u << bits) < C + 1) bits++;  // keys are in [0, C]
-    const uint32_t passes = bits <= 10 ? 1 : 2;
-    const uint32_t bits0 = passes == 1 ? bits : (bits + 1) / 2, bits1 = bits - bits0;
-    // contiguous slice per block, multiple of the tile
-    uint32_t per_block = (n + e->build_blocks - 1) / e->build_blocks;
-    per_block = ((per_block + BUILD_TILE - 1) / BUILD_TILE) * BUILD_TILE;
-    if (per_block == 0) per_block = BUILD_TILE;
-    uint32_t nblocks = (n + per_block - 1) / per_block;
-    if (nblocks == 0) nblocks = 1;
-    const uint32_t* vals = e->have_gid ? e->d_gid : nullptr;
-    if (passes == 1 && part != 0) {
-        if (part == 1) {
-            st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent,
-                                 ScatterExtras{nullptr, C, nullptr}, e->d_epoch + EP_BUILD, fap, 1);
-            if (st != CHD_OK) return st;
-            publish_cell_start_kernel<<<blocks_for((uint64_t)C + 2, 256), 256, 0, s>>>(e->d_hist, nblocks, C, n, n_ptr, e->d_cell_start,
-                                                                                         &e->d_ctr->n_entities_in_world);
-            KCHECK(e);
-            return CHD_OK;
-        }
-        st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent,
-                             ScatterExtras{nullptr, C, nullptr}, nullptr, nullptr, 2);
-        if (st != CHD_OK) return st;
-    } else if (passes == 1) {
-        // single pass: digit == key, so the scatter also publishes the CSR offsets
-        ScatterExtras ex{e->d_cell_start, C, &e->d_ctr->n_entities_in_world};
-        st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, nullptr, e->d_sorted_ent, ex,
-                             e->d_epoch + EP_BUILD, fap);
-        if (st != CHD_OK) return st;
-    } else {
-        st = sort_pass_fused(e, s, e->d_hist, e->site_hist, e->d_key, vals, n, n_ptr, per_block, nblocks, 0, bits0, e->d_tmp_key, e->d_tmp_val,
-                             ScatterExtras{nullptr, 0, nullptr}, e->d_epoch + EP_BUILD, fap);
-        if (st != CHD_OK) return st;
-        st = chd_sort_pass_any(e, s, e->d_hist, e->site_hist_b, e->d_tmp_key, e->d_tmp_val, n, n_ptr, per_block, nblocks, bits0, bits1, e->d_sorted_key,
-                               e->d_sorted_ent, ScatterExtras{nullptr, C, nullptr});
-        if (st != CHD_OK) return st;
-        cell_bounds_kernel<<<blocks_for((uint64_t)n + 1, 256), 256, 0, s>>>(e->d_sorted_key, n, n_ptr, C, e->d_cell_start,
-                                                                              &e->d_ctr->n_entities_in_world);
-        KCHECK(e);
-    }
-    return CHD_OK;
+    const ScatterExtras csr{e->d_cell_start, e->g.cells, &e->d_ctr->n_entities_in_world};
+    // keys are in [0, C]: C marks an out-of-world entity
+    return chd_cell_sort(e, s, e->ent_sort, e->g.cells + 1, e->d_key, e->have_gid ? e->d_gid : nullptr, n, n_ptr, e->d_sorted_key, e->d_sorted_ent,
+                         &csr, e->d_epoch + EP_BUILD, fap, part);
 }
 
 chd_status chd_build(chd_engine* e) {

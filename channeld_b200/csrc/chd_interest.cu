@@ -278,31 +278,9 @@ static chd_status interest_enqueue(chd_engine* e, cudaStream_t s, const QueryDev
     }
     return CHD_OK;
     }  // part 0
-    // pairs grouped by cell for the fan-out pass (= every channel's subscriber list): a stable radix sort of pair
-    // indices by cell with the same kernels as the entity build (no global atomics), device-side length
-    {
-        const uint32_t C = e->g.cells;
-        uint32_t bits = 1;
-        while ((1u << bits) < C) bits++;
-        const uint32_t passes = bits <= 10 ? 1 : 2;
-        const uint32_t bits0 = passes == 1 ? bits : (bits + 1) / 2, bits1 = bits - bits0;
-        const uint32_t nb = e->pc_blocks;
-        uint32_t per_block = (uint32_t)((P + nb - 1) / nb);
-        per_block = ((per_block + BUILD_TILE - 1) / BUILD_TILE) * BUILD_TILE;
-        if (passes == 1) {
-            st = chd_sort_pass_any(e, s, e->d_pc_hist, e->site_pchist, cur.cell, nullptr, (uint32_t)P, cur.off + S, per_block, nb, 0, bits0, nullptr,
-                               e->d_by_cell);
-            if (st != CHD_OK) return st;
-        } else {
-            st = chd_sort_pass_any(e, s, e->d_pc_hist, e->site_pchist, cur.cell, nullptr, (uint32_t)P, cur.off + S, per_block, nb, 0, bits0,
-                               e->d_pc_tmp_key, e->d_pc_tmp_val);
-            if (st != CHD_OK) return st;
-            st = chd_sort_pass_any(e, s, e->d_pc_hist, e->site_pchist_b, e->d_pc_tmp_key, e->d_pc_tmp_val, (uint32_t)P, cur.off + S, per_block, nb, bits0,
-                               bits1, nullptr, e->d_by_cell);
-            if (st != CHD_OK) return st;
-        }
-    }
-    return CHD_OK;
+    // pairs grouped by cell for the fan-out pass (= every channel's subscriber list): a stable radix sort of pair indices by cell
+    // (cells are in [0, C)) with the same kernels as the entity build (no global atomics), device-side length
+    return chd_cell_sort(e, s, e->pair_sort, e->g.cells, cur.cell, nullptr, (uint32_t)P, cur.off + S, nullptr, e->d_by_cell);
 }
 
 chd_status chd_update_interest(chd_engine* e, const chd_query_batch* q, int64_t now_ns) {

@@ -463,15 +463,15 @@ chd_status chd_get_rehome(chd_engine* e, uint32_t* global_id, uint32_t* dst_rank
     CU(e, cudaMemsetAsync(e->d_boff, 0, 4, s));
     if (n) {
         // (own entities only: in entity-table mode each carries the table id of its slot)
-        rehome_kernel<<<blocks_for(n, 256), 256, 0, s>>>(e->g, e->d_key, chd_entity_ids(e), n, world, e->d_tmp_key, e->d_tmp_val,
+        rehome_kernel<<<blocks_for(n, 256), 256, 0, s>>>(e->g, e->d_key, chd_entity_ids(e), n, world, e->ent_sort.tmp_key, e->ent_sort.tmp_val,
                                                          e->lim.max_entities, e->d_boff);
         KCHECK(e);
     }
     chd_status st = chd_read_u32(e, e->d_boff, count);
     if (st != CHD_OK) return st;
     const uint32_t m = *count < cap ? *count : cap;
-    if (m && global_id) CU(e, cudaMemcpyAsync(global_id, e->d_tmp_key, 4ull * m, cudaMemcpyDefault, s));
-    if (m && dst_rank) CU(e, cudaMemcpyAsync(dst_rank, e->d_tmp_val, 4ull * m, cudaMemcpyDefault, s));
+    if (m && global_id) CU(e, cudaMemcpyAsync(global_id, e->ent_sort.tmp_key, 4ull * m, cudaMemcpyDefault, s));
+    if (m && dst_rank) CU(e, cudaMemcpyAsync(dst_rank, e->ent_sort.tmp_val, 4ull * m, cudaMemcpyDefault, s));
     CU(e, cudaStreamSynchronize(s));
     return CHD_OK;
 }

@@ -453,7 +453,7 @@ chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank,
     const uint64_t N = e->lim.max_entities;
     const uint32_t world = e->comm ? (uint32_t)e->comm_world : 1u;
     // the list goes to the event staging (free between calls: every user is on this stream) and the radix sort's temporaries
-    uint32_t *d_id = t.d_ev, *d_slot = t.d_ev + N, *d_dst = e->d_tmp_val;
+    uint32_t *d_id = t.d_ev, *d_slot = t.d_ev + N, *d_dst = e->ent_sort.tmp_val;
     double *d_hx = t.d_ev_pos, *d_hz = t.d_ev_pos + N;
     chd_status st = chd_epoch_tick(e, s, EP_BORDER);
     if (st != CHD_OK) return st;

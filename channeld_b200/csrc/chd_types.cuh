@@ -151,9 +151,9 @@ struct HandoverOut {
     uint32_t cap;
 };
 
-// Extras of the FINAL pass of the entity build, fused into the scatter:
-//   cell_start != null: single-pass sorts only (digit == key): block 0 publishes the cell CSR offsets straight from
-//                       the scanned histogram (cell_start[c] = #keys < c), replacing a separate boundaries kernel
+// The cell CSR a sort by cell publishes (chd_cell_sort).  A single-pass sort (digit == key) publishes it straight from the
+// scanned histogram (cell_start[c] = #keys < c, load_base): fused into the scatter when cell_start != null, or by
+// publish_cell_start_kernel in a split build, replacing a separate boundaries kernel
 struct ScatterExtras {
     uint32_t* cell_start;
     uint32_t cells;
