@@ -168,6 +168,18 @@ chd_status chd_visible_delta(chd_engine* e) {
     return st != CHD_OK ? st : chd_delta_on(e, e->stream);
 }
 
+chd_status chd_read_delta_lengths(chd_engine* e, cudaStream_t s, DeltaLengths* out) {
+    const chd_engine::Delta& D = e->dl;
+    uint64_t* h64 = (uint64_t*)e->h_get;
+    h64[2] = 0;
+    CU(e, cudaMemcpyAsync(h64, D.enter_off + D.n_out, 8, cudaMemcpyDeviceToHost, s));
+    CU(e, cudaMemcpyAsync(h64 + 1, D.leave_off + D.n_out, 8, cudaMemcpyDeviceToHost, s));
+    if (D.ids) CU(e, cudaMemcpyAsync(h64 + 2, D.bad_ids, 4, cudaMemcpyDeviceToHost, s));
+    CU(e, cudaStreamSynchronize(s));
+    *out = DeltaLengths{h64[0], h64[1], (uint32_t)h64[2] != 0};
+    return CHD_OK;
+}
+
 chd_status chd_get_visible_delta(chd_engine* e, uint64_t* enter_off, uint32_t* enter_entity, uint64_t* leave_off, uint32_t* leave_entity,
                                  uint64_t cap, uint64_t* n_entered, uint64_t* n_left, uint32_t* n_slots) {
     if (!e) return CHD_ERR_INVALID;
@@ -179,26 +191,22 @@ chd_status chd_get_visible_delta(chd_engine* e, uint64_t* enter_off, uint32_t* e
     CU(e, cudaSetDevice(e->device));
     cudaStream_t s = e->stream;  // (a tick's delta on prep_stream is joined into the engine stream)
     const uint32_t S = D.n_out;
-    uint64_t* h64 = (uint64_t*)e->h_get;
-    CU(e, cudaMemcpyAsync(h64, D.enter_off + S, 8, cudaMemcpyDeviceToHost, s));
-    CU(e, cudaMemcpyAsync(h64 + 1, D.leave_off + S, 8, cudaMemcpyDeviceToHost, s));
-    if (D.ids) CU(e, cudaMemcpyAsync(h64 + 2, D.bad_ids, 4, cudaMemcpyDeviceToHost, s));
-    CU(e, cudaStreamSynchronize(s));
-    const uint64_t ne = h64[0], nl = h64[1];
-    const bool bad_ids = D.ids && (uint32_t)h64[2] != 0;
+    DeltaLengths dn;
+    const chd_status st = chd_read_delta_lengths(e, s, &dn);
+    if (st != CHD_OK) return st;
+    const uint64_t ne = dn.n_entered, nl = dn.n_left;
     if (n_entered) *n_entered = ne;
     if (n_left) *n_left = nl;
     if (n_slots) *n_slots = S;
     if (enter_off) CU(e, cudaMemcpyAsync(enter_off, D.enter_off, 8ull * (S + 1ull), cudaMemcpyDefault, s));
     if (leave_off) CU(e, cudaMemcpyAsync(leave_off, D.leave_off, 8ull * (S + 1ull), cudaMemcpyDefault, s));
     if (enter_entity || leave_entity) {
-        if (bad_ids) {
+        if (chd_delta_overflowed(ne, nl, D.enter_cap, D.leave_cap, dn.bad_ids)) {
             CU(e, cudaStreamSynchronize(s));
-            e->fail("the last visible delta met an id >= id_space %u or an id held twice (CHD_OVF_DELTA_IDS): no lists", D.id_space);
-            return CHD_ERR_INVALID;
-        }
-        if (ne > D.enter_cap || nl > D.leave_cap) {
-            CU(e, cudaStreamSynchronize(s));
+            if (dn.bad_ids) {
+                e->fail("the last visible delta met an id >= id_space %u or an id held twice (CHD_OVF_DELTA_IDS): no lists", D.id_space);
+                return CHD_ERR_INVALID;
+            }
             e->fail("the last visible delta overflowed (CHD_OVF_DELTA): %llu entered / %llu left > capacity %llu",
                     (unsigned long long)ne, (unsigned long long)nl, (unsigned long long)std::min(D.enter_cap, D.leave_cap));
             return CHD_ERR_CAPACITY;

@@ -523,6 +523,13 @@ chd_status chd_cell_sort(chd_engine* e, cudaStream_t s, const CellSort& cs, uint
                          unsigned long long* bump = nullptr, const FusedAssign* assign = nullptr, int part = 0);
 // the visible-set delta stage on `s` (chd_delta.cu)
 chd_status chd_delta_on(chd_engine* e, cudaStream_t s);
+// The last visible delta's list lengths and its id-mode error flag (CHD_OVF_DELTA_IDS), read on `s` once the delta has finished
+// there: one host round trip (chd_delta.cu)
+struct DeltaLengths {
+    uint64_t n_entered, n_left;
+    bool bad_ids;
+};
+chd_status chd_read_delta_lengths(chd_engine* e, cudaStream_t s, DeltaLengths* out);
 // the mode rules (chd_table.cu, numbered as in DESIGN.md §5): CHD_OK, or the error set and CHD_ERR_STATE (6: or CHD_ERR_INVALID)
 chd_status chd_rule_not_table(chd_engine* e, const char* fn);
 chd_status chd_rule_table_on_slab(chd_engine* e, const char* fn);
@@ -542,6 +549,12 @@ chd_status chd_follow_drop(chd_engine* e, const uint32_t* slot, const uint32_t* 
 chd_status chd_table_after_build(chd_engine* e, cudaStream_t s);
 chd_status chd_table_delta_ids(chd_engine* e, cudaStream_t s);
 void chd_table_observe(chd_engine* e, uint32_t delta_build);
+}
+
+// The visible delta overflowed: a list outgrew its capacity (CHD_OVF_DELTA) or an id-mode delta met a bad id (CHD_OVF_DELTA_IDS).
+// Its lists are not complete, and no read-back copies them.
+__host__ __device__ inline bool chd_delta_overflowed(uint64_t n_entered, uint64_t n_left, uint64_t enter_cap, uint64_t leave_cap, bool bad_ids) {
+    return n_entered > enter_cap || n_left > leave_cap || bad_ids;
 }
 
 // What the cell CSR's sorted_entity, the visible lists and the read-back report: entity indices, or ids in entity-table mode.  The

@@ -16,38 +16,15 @@ struct PackSeg {
     uint32_t count_is_u64;
 };
 struct PackArgs {
-    PackSeg seg[16];
+    PackSeg seg[16];  // the most one launch takes: phase A's hop 1, its 14 lists and 2 snapshots of their counts
     int n;
     uint32_t* truncated;  // pinned: set to 1 if a list did not fit its buffer
 };
-__global__ void __launch_bounds__(256) pack_kernel(PackArgs a) {
-    const PackSeg sg = a.seg[blockIdx.y];
-    uint64_t n = sg.fixed;
-    if (sg.count_ptr) n = sg.count_is_u64 ? *reinterpret_cast<const unsigned long long*>(sg.count_ptr) : (uint64_t)*reinterpret_cast<const uint32_t*>(sg.count_ptr);
-    if (n > sg.cap) {
-        if (blockIdx.x == 0 && threadIdx.x == 0) *a.truncated = 1;
-        n = sg.cap;
-    }
-    const uint64_t words = n * sg.elem_words;
-    const uint32_t* __restrict__ s = reinterpret_cast<const uint32_t*>(sg.src);
-    uint32_t* __restrict__ d = reinterpret_cast<uint32_t*>(sg.dst);
-    const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, nthr = (uint64_t)gridDim.x * blockDim.x;
-    if ((((uintptr_t)s | (uintptr_t)d) & 15) == 0) {  // 16-byte moves: full PCIe write bursts
-        const uint64_t q = words / 4;
-        const uint4* __restrict__ s4 = reinterpret_cast<const uint4*>(s);
-        uint4* __restrict__ d4 = reinterpret_cast<uint4*>(d);
-        for (uint64_t i = tid; i < q; i += nthr) d4[i] = s4[i];
-        for (uint64_t i = q * 4 + tid; i < words; i += nthr) d[i] = s[i];
-    } else {
-        for (uint64_t i = tid; i < words; i += nthr) d[i] = s[i];
-    }
-}
-// The visible-set delta's read-back moves up to hundreds of MB per tick (DESIGN §8), more than pack_kernel's fixed 24 blocks per
-// segment are sized for: a grid sized from the capacity, each segment read and written in 16-byte vectors once the destination is
-// 16-byte aligned (when the source is aligned the same way), with a scalar head and tail.  Streaming loads and stores: the data is
-// read once and should not evict what the emit kernel beside it keeps in L2.
+// One segment per blockIdx.y: its count, clamped to the capacity, in 16-byte vectors (full PCIe write bursts) once the destination
+// is 16-byte aligned (when the source is aligned the same way), with a scalar head and tail.  Streaming loads and stores: the data is read once and should
+// not evict what the emit kernel beside it keeps in L2.
 constexpr unsigned COPY_THREADS = 256;
-__global__ void __launch_bounds__(COPY_THREADS) bulk_copy_kernel(PackArgs a) {
+__device__ __forceinline__ void copy_segment(const PackArgs& a) {
     const PackSeg sg = a.seg[blockIdx.y];
     uint64_t n = sg.fixed;
     if (sg.count_ptr) n = sg.count_is_u64 ? *reinterpret_cast<const unsigned long long*>(sg.count_ptr) : (uint64_t)*reinterpret_cast<const uint32_t*>(sg.count_ptr);
@@ -71,6 +48,10 @@ __global__ void __launch_bounds__(COPY_THREADS) bulk_copy_kernel(PackArgs a) {
     for (uint64_t i = tid; i < q; i += nthr) __stcs(d4 + i, __ldcs(s4 + i));
     for (uint64_t i = head + q * 4 + tid; i < words; i += nthr) d[i] = s[i];
 }
+// Two names for one copy, so that a trace tells the delta's hops apart from the other lists': pack_kernel copies the phase A / B
+// lists (24 blocks per segment), bulk_copy_kernel the visible delta's, up to hundreds of MB per tick (DESIGN §8, bulk_copy_grid).
+__global__ void __launch_bounds__(COPY_THREADS) pack_kernel(PackArgs a) { copy_segment(a); }
+__global__ void __launch_bounds__(COPY_THREADS) bulk_copy_kernel(PackArgs a) { copy_segment(a); }
 // x blocks per segment: enough for one 16-byte vector per thread, at most `per_sm4` quarters of the SM count; y: the segments.
 // Hop 1 (HBM -> HBM) takes 8 (2 CTAs per SM and segment: a launch of the four delta segments holds at most 8 per SM), hop 2 (HBM ->
 // PCIe) 1: its CTAs stay resident for the whole transfer (4 ms on the all-entities-move workload); at 8 the pipelined tick took
@@ -91,7 +72,7 @@ static_assert(sizeof(Counters) <= DELTA_HEADER_WORD * 4 && DELTA_HEADER_WORD * 4
 __global__ void delta_head_kernel(const unsigned long long* n_entered, const unsigned long long* n_left, uint64_t enter_cap, uint64_t leave_cap,
                                   const uint32_t* bad_ids, uint32_t n_out, DeltaHead* h) {
     const unsigned long long ne = *n_entered, nl = *n_left;
-    const bool ovf = ne > enter_cap || nl > leave_cap || (bad_ids && *bad_ids);
+    const bool ovf = chd_delta_overflowed(ne, nl, enter_cap, leave_cap, bad_ids && *bad_ids);
     h->n_entered = ne;
     h->n_left = nl;
     h->overflow = ovf;
@@ -99,6 +80,12 @@ __global__ void delta_head_kernel(const unsigned long long* n_entered, const uns
     h->copy_left = ovf ? 0 : nl;
     h->copy_offsets = ovf ? 0 : (unsigned long long)n_out + 1;
 }
+// The start of a fetch set's staging buffer: the counts hop 2 sizes its copies by, as hop 1 (or delta_head_kernel) saw them
+struct StageHead {
+    Counters a, b;     // the counters when phase A / phase B is final (b also travels to the pinned header)
+    uint32_t n_pairs;  // the pair lists' length, pair_off[n_slots]
+    DeltaHead delta;
+};
 bool is_pinned_host(const void* p) {
     if (!p) return true;
     cudaPointerAttributes at;
@@ -117,18 +104,32 @@ uint32_t take_deltas(chd_engine* e, bool want) {
 }
 // Synchronous form: the last delta's list lengths, read on `s` once it has finished there; *overflow: no lists to copy
 chd_status read_delta_counts(chd_engine* e, cudaStream_t s, uint32_t deltas, chd_delta_counts* dc, bool* overflow) {
-    chd_engine::Delta& D = e->dl;
+    const chd_engine::Delta& D = e->dl;
     *dc = chd_delta_counts{};
     *overflow = false;
     if (!deltas) return CHD_OK;
-    uint64_t* h64 = (uint64_t*)e->h_get;
-    h64[2] = 0;
-    CU(e, cudaMemcpyAsync(h64, D.enter_off + D.n_out, 8, cudaMemcpyDeviceToHost, s));
-    CU(e, cudaMemcpyAsync(h64 + 1, D.leave_off + D.n_out, 8, cudaMemcpyDeviceToHost, s));
-    if (D.ids) CU(e, cudaMemcpyAsync(h64 + 2, D.bad_ids, 4, cudaMemcpyDeviceToHost, s));
-    CU(e, cudaStreamSynchronize(s));
-    *dc = chd_delta_counts{h64[0], h64[1], D.n_out, deltas};
-    *overflow = h64[0] > D.enter_cap || h64[1] > D.leave_cap || (uint32_t)h64[2] != 0;
+    DeltaLengths dn;
+    const chd_status st = chd_read_delta_lengths(e, s, &dn);
+    if (st != CHD_OK) return st;
+    *dc = chd_delta_counts{dn.n_entered, dn.n_left, D.n_out, deltas};
+    *overflow = chd_delta_overflowed(dn.n_entered, dn.n_left, D.enter_cap, D.leave_cap, dn.bad_ids);
+    return CHD_OK;
+}
+// When a tick's results are final, for the read-back streams of both fetches (the synchronous one's early form and the asynchronous
+// one).  Phase A: after the interest fill (ev_pairs) and the build: pairs, interest diff, query statuses, handover list, cell CSR.
+chd_status wait_phase_a(chd_engine* e, cudaStream_t s) {
+    CU(e, cudaStreamWaitEvent(s, e->ev_pairs, 0));
+    if (e->build_done_recorded) CU(e, cudaStreamWaitEvent(s, e->ev_build_done, 0));
+    return CHD_OK;
+}
+// Phase B: after the aux chain (ev_join: fan-out) and the emit preparation (ev_prep_done): due list, visible offsets, counters.  And
+// after the visible delta, because its CHD_OVF_DELTA belongs to this tick's summary: a tick's delta off the engine stream (ev_done)
+// and, when the fetch reads deltas back, the last delta wherever it ran (ev_end; a standalone one runs on the engine stream).
+chd_status wait_phase_b(chd_engine* e, cudaStream_t s, bool deltas) {
+    CU(e, cudaStreamWaitEvent(s, e->ev_join, 0));
+    CU(e, cudaStreamWaitEvent(s, e->ev_prep_done, 0));
+    if (e->dl.done_recorded) CU(e, cudaStreamWaitEvent(s, e->dl.ev_done, 0));
+    if (deltas) CU(e, cudaStreamWaitEvent(s, e->dl.ev_end, 0));
     return CHD_OK;
 }
 }  // namespace
@@ -311,15 +312,12 @@ chd_status chd_fetch_results_delta(chd_engine* e, const chd_result_buffers* b, c
     };
     Counters ca{};  // counters as of phase A
     if (early) {
-        // The tick is probably still running.  Read back on a separate stream, in the order in which results become final:
-        //   phase A  after the interest fill (ev_pairs) and the build: pairs, interest diff, query statuses, handover list, cell CSR
-        //   phase B  after the aux chain (ev_join: fan-out) and the emit preparation (ev_prep_done): due list, visible offsets
-        //            (and after the visible delta of a CHD_TICK_VISIBLE_DELTA tick: the counters carry its overflow bit)
-        // while the emit kernel is still writing the expanded list.
+        // The tick is probably still running.  Read back on separate streams, phase A and then phase B, each as soon as its results
+        // are final (wait_phase_a / wait_phase_b), while the emit kernel is still writing the expanded list.
         CU(e, cudaSetDevice(e->device));
         s = e->dl_stream;
-        CU(e, cudaStreamWaitEvent(s, e->ev_pairs, 0));
-        if (e->build_done_recorded) CU(e, cudaStreamWaitEvent(s, e->ev_build_done, 0));
+        st = wait_phase_a(e, s);
+        if (st != CHD_OK) return st;
         CU(e, cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
         CU(e, cudaStreamSynchronize(s));  // sync A
         ca = *e->h_ctr;
@@ -386,10 +384,8 @@ chd_status chd_fetch_results_delta(chd_engine* e, const chd_result_buffers* b, c
     cudaStream_t sa = s;  // stream carrying the phase-A copies
     if (early) {  // phase B, on its own stream: its counter read-back must not queue behind the phase-A copies
         s = e->dl_stream_b;
-        CU(e, cudaStreamWaitEvent(s, e->ev_join, 0));
-        CU(e, cudaStreamWaitEvent(s, e->ev_prep_done, 0));
-        if (e->dl.done_recorded) CU(e, cudaStreamWaitEvent(s, e->dl.ev_done, 0));  // the visible delta (its overflow bit)
-        if (deltas) CU(e, cudaStreamWaitEvent(s, e->dl.ev_end, 0));  // the delta read back here (a standalone one: on the engine stream)
+        st = wait_phase_b(e, s, deltas);
+        if (st != CHD_OK) return st;
         CU(e, cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
         CU(e, cudaStreamSynchronize(s));  // sync B
         st = chd_decode_summary(e, summary);
@@ -466,133 +462,102 @@ chd_status chd_fetch_results_async_delta(chd_engine* e, const chd_result_buffers
     const uint32_t S = e->n_slots;
     Counters* ctr = e->d_ctr;
     uint32_t* hdr = reinterpret_cast<uint32_t*>(pinned_header);
-    hdr[CHD_FETCH_HEADER_BYTES / 4 - 1] = 0;  // truncation flag (host write, ordered before the kernels are launched)
+    uint32_t* truncated = hdr + CHD_FETCH_HEADER_BYTES / 4 - 1;
+    *truncated = 0;  // (host write, ordered before the kernels are launched)
     memset(hdr + DELTA_HEADER_WORD, 0, 24);  // the delta's counts (stay 0 when this fetch carries none)
-    auto seg = [](const void* src, void* dst, const void* cnt, uint64_t fixed, uint64_t cap, uint32_t words, uint32_t is64) {
-        return PackSeg{src, dst, cnt, fixed, cap, words, is64};
-    };
-    // phase A: final once the interest fill and the build are done
-    PackArgs A{};
-    A.truncated = hdr + CHD_FETCH_HEADER_BYTES / 4 - 1;
-    if (b->pair_off) A.seg[A.n++] = seg(pb.off, b->pair_off, nullptr, (uint64_t)S + 1, (uint64_t)S + 1, 1, 0);
-    if (b->pair_channel) A.seg[A.n++] = seg(e->d_pair_ch, b->pair_channel, pb.off + S, 0, b->pair_cap, 1, 0);
-    if (b->pair_dist) A.seg[A.n++] = seg(pb.dist, b->pair_dist, pb.off + S, 0, b->pair_cap, 1, 0);
-    if (b->pair_interval_ms) A.seg[A.n++] = seg(pb.interval, b->pair_interval_ms, pb.off + S, 0, b->pair_cap, 1, 0);
-    if (b->new_sub) A.seg[A.n++] = seg(e->d_new_sub, b->new_sub, &ctr->n_sub_new, 0, b->diff_cap, 1, 0);
-    if (b->new_channel) A.seg[A.n++] = seg(e->d_new_ch, b->new_channel, &ctr->n_sub_new, 0, b->diff_cap, 1, 0);
-    if (b->unsub_sub) A.seg[A.n++] = seg(e->d_gone_sub, b->unsub_sub, &ctr->n_unsub, 0, b->diff_cap, 1, 0);
-    if (b->unsub_channel) A.seg[A.n++] = seg(e->d_gone_ch, b->unsub_channel, &ctr->n_unsub, 0, b->diff_cap, 1, 0);
-    if (b->query_status) A.seg[A.n++] = seg(e->d_status, b->query_status, nullptr, std::min<uint64_t>(e->last_nq, b->status_cap), b->status_cap, 1, 0);
-    if (b->cell_start) A.seg[A.n++] = seg(e->d_cell_start, b->cell_start, nullptr, (uint64_t)e->g.cells + 1, (uint64_t)e->g.cells + 1, 1, 0);
-    if (b->sorted_entity) A.seg[A.n++] = seg(chd_sorted_out(e), b->sorted_entity, &ctr->n_entities_in_world, 0, b->entity_cap, 1, 0);
-    PackArgs A2{};  // (the handover triple: a second launch keeps PackArgs small)
-    A2.truncated = A.truncated;
-    const uint64_t hcap = std::min<uint64_t>(b->handover_cap, e->ho_cap);
-    if (b->handover_entity) A2.seg[A2.n++] = seg(e->d_ho_entity, b->handover_entity, &ctr->n_handover, 0, hcap, 1, 0);
-    if (b->handover_src) A2.seg[A2.n++] = seg(e->d_ho_src, b->handover_src, &ctr->n_handover, 0, hcap, 1, 0);
-    if (b->handover_dst) A2.seg[A2.n++] = seg(e->d_ho_dst, b->handover_dst, &ctr->n_handover, 0, hcap, 1, 0);
-    // phase B: final after the fan-out pass and the emit preparation; the counters travel last
-    PackArgs B{};
-    B.truncated = A.truncated;
-    if (b->due) B.seg[B.n++] = seg(e->d_due, b->due, &ctr->n_due, 0, std::min<uint64_t>(b->due_cap, e->lim.max_due), sizeof(chd_due) / 4, 0);
-    if (b->vis_off) B.seg[B.n++] = seg(e->d_vis_off, b->vis_off, nullptr, (uint64_t)S + 1, (uint64_t)S + 1, 2, 0);
-    B.seg[B.n++] = seg(ctr, pinned_header, nullptr, sizeof(Counters) / 4, sizeof(Counters) / 4, 1, 0);
     // ---- hop 1: snapshot into device staging (microseconds: the next tick is ordered after THIS, not after the PCIe transfer);
-    //      hop 2: staging -> the caller's pinned buffers on a stream of its own, sized by the snapshot's own copy of the counts
+    //      hop 2: staging -> the caller's pinned buffers on a stream of its own, sized by the snapshot's own copy of the counts.
+    // Each list is declared once, and its staging slice, hop-1 segment and hop-2 segment all come from that declaration.  Staging
+    // addresses are byte offsets until the buffer has been sized.
+    enum { HOP_A, HOP_B, HOP_DELTA };  // the hop-1 launch that snapshots a list: phase A, phase B, the visible delta
+    struct Count {
+        const void* live;  // what hop 1 reads (nullptr: the snapshot's, which delta_head_kernel writes before hop 1; or `fixed`)
+        int64_t snap;      // what hop 2 reads: offset in StageHead (-1: `fixed`)
+        uint32_t is64;
+        uint64_t fixed;
+    };
+    struct List {
+        int hop;
+        const void* src;  // nullptr: no hop 1 (delta_head_kernel writes the slice)
+        void* dst;        // nullptr: no hop 2 (a count only hop 2 reads)
+        Count n;
+        uint64_t cap;
+        uint32_t words;   // element size in 32-bit words
+        uint64_t slice;   // offset in the staging buffer
+    };
+    List lists[24];
+    int nl = 0;
     auto up16 = [](uint64_t v) { return (v + 15) & ~(uint64_t)15; };
-    uint64_t need = 0;
-    PackArgs* sets[3] = {&A, &A2, &B};
-    for (PackArgs* pa : sets)
-        for (int k = 0; k < pa->n; k++) need += up16(std::max<uint64_t>(pa->seg[k].cap, pa->seg[k].fixed) * pa->seg[k].elem_words * 4);
-    need += 2 * up16(sizeof(Counters)) + 64;
-    if (deltas) {
-        need += up16(sizeof(DeltaHead));
-        for (const void* p : {(const void*)db.enter_off, (const void*)db.leave_off}) need += p ? up16(8 * db.slot_cap) : 0;
-        for (const void* p : {(const void*)db.enter_entity, (const void*)db.leave_entity}) need += p ? up16(4 * db.entity_cap) : 0;
+    uint64_t stage_bytes = up16(sizeof(StageHead));
+    auto list = [&](int hop, const void* src, void* dst, Count n, uint64_t cap, uint32_t words) {  // a requested list: a slice of its own
+        if (!dst) return;
+        lists[nl++] = List{hop, src, dst, n, cap, words, stage_bytes};
+        stage_bytes += up16(std::max(cap, n.fixed) * words * 4);
+    };
+    auto count = [&](int hop, const void* src, void* dst, uint64_t at, uint32_t words) {  // a count: its slice is its place in StageHead
+        lists[nl++] = List{hop, src, dst, Count{nullptr, -1, 0, words}, words, 1, at};
+    };
+    auto fixed = [](uint64_t n) { return Count{nullptr, -1, 0, n}; };
+#define SNAP(field) (int64_t)offsetof(StageHead, field)
+    const uint64_t S1 = (uint64_t)S + 1, C1 = (uint64_t)e->g.cells + 1, hcap = std::min<uint64_t>(b->handover_cap, e->ho_cap);
+    // list(hop, device source, pinned destination, count: live and in the snapshot, capacity, element words)
+    list(HOP_A, pb.off, b->pair_off, fixed(S1), S1, 1);
+    list(HOP_A, e->d_pair_ch, b->pair_channel, {pb.off + S, SNAP(n_pairs)}, b->pair_cap, 1);
+    list(HOP_A, pb.dist, b->pair_dist, {pb.off + S, SNAP(n_pairs)}, b->pair_cap, 1);
+    list(HOP_A, pb.interval, b->pair_interval_ms, {pb.off + S, SNAP(n_pairs)}, b->pair_cap, 1);
+    list(HOP_A, e->d_new_sub, b->new_sub, {&ctr->n_sub_new, SNAP(a.n_sub_new)}, b->diff_cap, 1);
+    list(HOP_A, e->d_new_ch, b->new_channel, {&ctr->n_sub_new, SNAP(a.n_sub_new)}, b->diff_cap, 1);
+    list(HOP_A, e->d_gone_sub, b->unsub_sub, {&ctr->n_unsub, SNAP(a.n_unsub)}, b->diff_cap, 1);
+    list(HOP_A, e->d_gone_ch, b->unsub_channel, {&ctr->n_unsub, SNAP(a.n_unsub)}, b->diff_cap, 1);
+    list(HOP_A, e->d_status, b->query_status, fixed(std::min<uint64_t>(e->last_nq, b->status_cap)), b->status_cap, 1);
+    list(HOP_A, e->d_cell_start, b->cell_start, fixed(C1), C1, 1);
+    list(HOP_A, chd_sorted_out(e), b->sorted_entity, {&ctr->n_entities_in_world, SNAP(a.n_entities_in_world)}, b->entity_cap, 1);
+    list(HOP_A, e->d_ho_entity, b->handover_entity, {&ctr->n_handover, SNAP(a.n_handover)}, hcap, 1);
+    list(HOP_A, e->d_ho_src, b->handover_src, {&ctr->n_handover, SNAP(a.n_handover)}, hcap, 1);
+    list(HOP_A, e->d_ho_dst, b->handover_dst, {&ctr->n_handover, SNAP(a.n_handover)}, hcap, 1);
+    list(HOP_B, e->d_due, b->due, {&ctr->n_due, SNAP(b.n_due)}, std::min<uint64_t>(b->due_cap, e->lim.max_due), sizeof(chd_due) / 4);
+    list(HOP_B, e->d_vis_off, b->vis_off, fixed(S1), S1, 2);
+    count(HOP_A, ctr, nullptr, SNAP(a), sizeof(Counters) / 4);
+    count(HOP_A, pb.off + S, nullptr, SNAP(n_pairs), 1);
+    count(HOP_B, ctr, pinned_header, SNAP(b), sizeof(Counters) / 4);
+    if (deltas) {  // the lengths each delta copy moves are 0 after an overflow
+        list(HOP_DELTA, D.enter_off, db.enter_off, {nullptr, SNAP(delta.copy_offsets), 1}, db.slot_cap, 2);
+        list(HOP_DELTA, D.leave_off, db.leave_off, {nullptr, SNAP(delta.copy_offsets), 1}, db.slot_cap, 2);
+        list(HOP_DELTA, D.enter, db.enter_entity, {nullptr, SNAP(delta.copy_entered), 1}, db.entity_cap, 1);
+        list(HOP_DELTA, D.leave, db.leave_entity, {nullptr, SNAP(delta.copy_left), 1}, db.entity_cap, 1);
+        count(HOP_DELTA, nullptr, hdr + DELTA_HEADER_WORD, SNAP(delta), 6);  // its lengths and overflow
         if (!e->dl_stream_d && !chd_make_stream(e, &e->dl_stream_d)) return CHD_ERR_CUDA;
     }
-    if (!ensure_cap(e, &e->d_fetch_stage[fi], &e->fetch_stage_bytes[fi], need, need)) return CHD_ERR_CUDA;
+#undef SNAP
+    if (!ensure_cap(e, &e->d_fetch_stage[fi], &e->fetch_stage_bytes[fi], stage_bytes, stage_bytes)) return CHD_ERR_CUDA;
     if (!e->dl_stream_c && !chd_make_stream(e, &e->dl_stream_c)) return CHD_ERR_CUDA;
     if (!e->ev_fetch_done[fi] && !chd_make_event(e, &e->ev_fetch_done[fi])) return CHD_ERR_CUDA;
-    uint8_t* cursor = e->d_fetch_stage[fi];
-    auto carve = [&](uint64_t bytes) {
-        uint8_t* p = cursor;
-        cursor += up16(bytes);
-        return p;
-    };
-    Counters* ctr_a = reinterpret_cast<Counters*>(carve(sizeof(Counters)));  // the counts as they stand when phase A / B is final
-    Counters* ctr_b = reinterpret_cast<Counters*>(carve(sizeof(Counters)));
-    uint32_t* npairs_s = reinterpret_cast<uint32_t*>(carve(16));
-    auto staged_count = [&](const void* cnt, Counters* snap) -> const void* {
-        if (!cnt) return nullptr;
-        if (cnt == (const void*)(pb.off + S)) return npairs_s;
-        const uintptr_t o = (uintptr_t)cnt - (uintptr_t)ctr;
-        return o < sizeof(Counters) ? (const void*)((const uint8_t*)snap + o) : cnt;
-    };
-    PackArgs H[3] = {};  // hop 2 of A, A2, B
-    for (int j = 0; j < 3; j++) {
-        PackArgs* pa = sets[j];
-        H[j].truncated = pa->truncated;
-        H[j].n = pa->n;
-        for (int k = 0; k < pa->n; k++) {
-            PackSeg& d1 = pa->seg[k];
-            void* st = carve(std::max<uint64_t>(d1.cap, d1.fixed) * d1.elem_words * 4);
-            H[j].seg[k] = d1;
-            H[j].seg[k].src = st;
-            H[j].seg[k].count_ptr = staged_count(d1.count_ptr, j == 2 ? ctr_b : ctr_a);
-            d1.dst = st;  // hop 1 writes the snapshot
-        }
+    uint8_t* const stage = e->d_fetch_stage[fi];
+    PackArgs hop1[3] = {}, hop2[3] = {};
+    for (int k = 0; k < nl; k++) {
+        const List& l = lists[k];
+        void* slice = stage + l.slice;
+        const void* snap = l.n.snap < 0 ? nullptr : stage + l.n.snap;
+        PackArgs &h1 = hop1[l.hop], &h2 = hop2[l.hop];
+        if (l.src) h1.seg[h1.n++] = PackSeg{l.src, slice, l.n.live ? l.n.live : snap, l.n.fixed, l.cap, l.words, l.n.is64};
+        if (l.dst) h2.seg[h2.n++] = PackSeg{slice, l.dst, snap, l.n.fixed, l.cap, l.words, l.n.is64};
     }
-    // hop 1 also snapshots the counts themselves
-    A.seg[A.n++] = seg(ctr, ctr_a, nullptr, sizeof(Counters) / 4, sizeof(Counters) / 4, 1, 0);
-    A.seg[A.n++] = seg(pb.off + S, npairs_s, nullptr, 1, 1, 1, 0);
-    B.seg[B.n++] = seg(ctr, ctr_b, nullptr, sizeof(Counters) / 4, sizeof(Counters) / 4, 1, 0);
-    // (B's own copy of the counters to the pinned header reads the snapshot in hop 2)
-    for (int k = 0; k < H[2].n; k++)
-        if (H[2].seg[k].dst == pinned_header) H[2].seg[k].src = ctr_b;
-    // the visible delta: hop 1 (DL) snapshots its lengths (DeltaHead) and lists, hop 2 (DH) moves them and the lengths to the host;
-    // both copy the lengths DeltaHead gives (0 after an overflow)
-    PackArgs DL{}, DH{};
-    DL.truncated = DH.truncated = A.truncated;
-    DeltaHead* dhead = nullptr;
-    if (deltas) {
-        dhead = reinterpret_cast<DeltaHead*>(carve(sizeof(DeltaHead)));
-        auto both = [&](const void* src, void* dst, const unsigned long long* cnt, uint64_t cap, uint32_t words) {
-            if (!dst) return;
-            void* st = carve(cap * words * 4);
-            DL.seg[DL.n++] = seg(src, st, cnt, 0, cap, words, 1);
-            DH.seg[DH.n++] = seg(st, dst, cnt, 0, cap, words, 1);
-        };
-        both(D.enter_off, db.enter_off, &dhead->copy_offsets, db.slot_cap, 2);
-        both(D.leave_off, db.leave_off, &dhead->copy_offsets, db.slot_cap, 2);
-        both(D.enter, db.enter_entity, &dhead->copy_entered, db.entity_cap, 1);
-        both(D.leave, db.leave_entity, &dhead->copy_left, db.entity_cap, 1);
-        DH.seg[DH.n++] = seg(dhead, hdr + DELTA_HEADER_WORD, nullptr, 6, 6, 1, 0);
-    }
+    for (int h = 0; h < 3; h++) hop1[h].truncated = hop2[h].truncated = truncated;
     cudaStream_t sa = e->dl_stream, sb = e->dl_stream_b, sc = e->dl_stream_c;
-    CU(e, cudaStreamWaitEvent(sa, e->ev_pairs, 0));
-    if (e->build_done_recorded) CU(e, cudaStreamWaitEvent(sa, e->ev_build_done, 0));
-    pack_kernel<<<dim3(24, (unsigned)A.n), 256, 0, sa>>>(A);
+    chd_status st = wait_phase_a(e, sa);
+    if (st != CHD_OK) return st;
+    pack_kernel<<<dim3(24, (unsigned)hop1[HOP_A].n), COPY_THREADS, 0, sa>>>(hop1[HOP_A]);
     KCHECK(e);
-    if (A2.n) {
-        pack_kernel<<<dim3(8, (unsigned)A2.n), 256, 0, sa>>>(A2);
-        KCHECK(e);
-    }
     CU(e, cudaEventRecord(e->ev_fetch_a[fi], sa));
     CU(e, cudaStreamWaitEvent(sc, e->ev_fetch_a[fi], 0));
     const bool prof = e->profiling == 1;
     if (prof) CU(e, cudaEventRecord(e->evt(CHD_STAGE_READBACK, e->stage_n[CHD_STAGE_READBACK], 0), sc));
-    if (H[0].n) {
-        pack_kernel<<<dim3(24, (unsigned)H[0].n), 256, 0, sc>>>(H[0]);
+    if (hop2[HOP_A].n) {
+        pack_kernel<<<dim3(24, (unsigned)hop2[HOP_A].n), COPY_THREADS, 0, sc>>>(hop2[HOP_A]);
         KCHECK(e);
     }
-    if (H[1].n) {
-        pack_kernel<<<dim3(8, (unsigned)H[1].n), 256, 0, sc>>>(H[1]);
-        KCHECK(e);
-    }
-    CU(e, cudaStreamWaitEvent(sb, e->ev_join, 0));
-    CU(e, cudaStreamWaitEvent(sb, e->ev_prep_done, 0));
-    if (e->dl.done_recorded) CU(e, cudaStreamWaitEvent(sb, e->dl.ev_done, 0));  // the visible delta (its overflow bit)
+    st = wait_phase_b(e, sb, deltas);
+    if (st != CHD_OK) return st;
     if (deltas) {
         // hop 1 of the delta on a stream of its own, from the delta's end on: beside the expanded-list kernel, and only the next delta
         // waits for it (D.read_guard), not the next tick's other stages
@@ -600,26 +565,25 @@ chd_status chd_fetch_results_async_delta(chd_engine* e, const chd_result_buffers
         CU(e, cudaStreamWaitEvent(sd, D.ev_end, 0));
         delta_head_kernel<<<1, 1, 0, sd>>>(reinterpret_cast<const unsigned long long*>(D.enter_off + D.n_out),
                                           reinterpret_cast<const unsigned long long*>(D.leave_off + D.n_out), D.enter_cap, D.leave_cap,
-                                          D.ids ? D.bad_ids : nullptr, D.n_out, dhead);
+                                          D.ids ? D.bad_ids : nullptr, D.n_out, &reinterpret_cast<StageHead*>(stage)->delta);
         KCHECK(e);
-        if (DL.n) {
-            bulk_copy_kernel<<<bulk_copy_grid(e, DL, 8), COPY_THREADS, 0, sd>>>(DL);
+        if (hop1[HOP_DELTA].n) {
+            bulk_copy_kernel<<<bulk_copy_grid(e, hop1[HOP_DELTA], 8), COPY_THREADS, 0, sd>>>(hop1[HOP_DELTA]);
             KCHECK(e);
         }
         CU(e, cudaEventRecord(D.ev_read[fi], sd));
         D.read_guard = true;
         D.read_fi = fi;
-        CU(e, cudaStreamWaitEvent(sb, D.ev_end, 0));  // (a standalone delta's overflow bit belongs to this summary too)
     }
-    pack_kernel<<<dim3(24, (unsigned)B.n), 256, 0, sb>>>(B);
+    pack_kernel<<<dim3(24, (unsigned)hop1[HOP_B].n), COPY_THREADS, 0, sb>>>(hop1[HOP_B]);
     KCHECK(e);
     CU(e, cudaEventRecord(e->ev_fetch_b[fi], sb));
     CU(e, cudaStreamWaitEvent(sc, e->ev_fetch_b[fi], 0));
-    pack_kernel<<<dim3(24, (unsigned)H[2].n), 256, 0, sc>>>(H[2]);
+    pack_kernel<<<dim3(24, (unsigned)hop2[HOP_B].n), COPY_THREADS, 0, sc>>>(hop2[HOP_B]);
     KCHECK(e);
     if (deltas) {
         CU(e, cudaStreamWaitEvent(sc, D.ev_read[fi], 0));
-        bulk_copy_kernel<<<bulk_copy_grid(e, DH, 1), COPY_THREADS, 0, sc>>>(DH);
+        bulk_copy_kernel<<<bulk_copy_grid(e, hop2[HOP_DELTA], 1), COPY_THREADS, 0, sc>>>(hop2[HOP_DELTA]);
         KCHECK(e);
     }
     CU(e, cudaEventRecord(e->ev_fetch_done[fi], sc));
