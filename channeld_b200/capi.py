@@ -27,6 +27,7 @@ TICK_VISIBLE_DELTA = 16
 TICK_FOLLOW = 32  # the tick's batch is the one chd_follow_queries generated (batch None)
 FOLLOW_ALL, FOLLOW_MOVED = 0, 1
 FOLLOW_NOT_SELECTED, FOLLOW_NO_ENTITY = 16, 17  # beside Q_* in chd_get_follow's status
+FOLLOW_OVERRIDDEN = 18  # the slot's host entry in chd_follow_queries_with's batch replaced its generated query
 OVF_PAIRS, OVF_WINDOW, OVF_VISIBLE, OVF_DUE, OVF_BORDER, OVF_RING = 1, 2, 4, 8, 16, 32
 OVF_DELTA = 64
 OVF_DELTA_IDS = 128
@@ -158,7 +159,7 @@ SYMBOLS = [
     "chd_fetch_results_delta", "chd_fetch_results_async_delta", "chd_fetch_wait_delta",
     "chd_entity_table_init", "chd_spawn_entities", "chd_spawn_entities_f32", "chd_despawn_entities", "chd_move_entities", "chd_move_entities_f32",
     "chd_get_entity_stats", "chd_handoff_entities",
-    "chd_follow_bind", "chd_follow_unbind", "chd_follow_queries", "chd_get_follow",
+    "chd_follow_bind", "chd_follow_unbind", "chd_follow_queries", "chd_get_follow", "chd_follow_queries_with",
 ]
 STAGE_BUILD, STAGE_INTEREST, STAGE_EMIT, STAGE_EMIT_KERNEL, STAGE_FANOUT, STAGE_TICK, STAGE_EXPORT, STAGE_EXCHANGE, STAGE_IMPORT, STAGE_READBACK, STAGE_VISIBLE_DELTA, STAGE_ENTITY_EVENTS, STAGE_FOLLOW = range(13)
 
@@ -368,6 +369,8 @@ def lib():
     L.chd_follow_unbind.argtypes = [vp, vp, C.c_uint32]
     L.chd_follow_queries.restype = C.c_int
     L.chd_follow_queries.argtypes = [vp, C.c_uint32]
+    L.chd_follow_queries_with.restype = C.c_int
+    L.chd_follow_queries_with.argtypes = [vp, C.c_uint32, C.POINTER(QueryBatch)]
     L.chd_get_follow.restype = C.c_int
     L.chd_get_follow.argtypes = [vp, vp, vp, vp, vp, vp, C.c_uint32, u32p, u32p]
     _lib = L

@@ -273,13 +273,20 @@ class GpuStaticGrid2DSpatialController:
         self.engine.follow_unbind(conn_slots)
 
     # -- Tick()   (channel.go:358-387 for all spatial channels at once).  follow = capi.FOLLOW_ALL / FOLLOW_MOVED with batch None:
-    # the batch is generated from the FollowEntities bindings.
-    def Tick(self, batch, t_ns, flags=capi.TICK_ALL, follow=None):
+    # the batch is generated from the FollowEntities bindings.  explicit = the UPDATE_SPATIAL_INTEREST batch of the connections that
+    # send their own queries this tick (spectators, SpotsAOI, ...): merged in front of the generated one, and a following
+    # connection that sent one uses it for this tick.
+    def Tick(self, batch, t_ns, flags=capi.TICK_ALL, follow=None, explicit=None):
         if follow is not None:
             if batch is not None:
                 raise SpatialError("a followed tick generates its own batch")
-            self.engine.follow_queries(follow)
+            if explicit is not None:
+                self.engine.follow_queries_with(follow, explicit)
+            else:
+                self.engine.follow_queries(follow)
             flags |= capi.TICK_FOLLOW
+        elif explicit is not None:
+            raise SpatialError("explicit queries are merged into a followed tick: pass follow=")
         return self.engine.tick(batch, t_ns, flags)
 
     # -- per client, the entities to spawn / despawn since the last delta: the net effect of the FULL data a new subscription

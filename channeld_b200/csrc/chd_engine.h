@@ -166,6 +166,7 @@ struct chd_engine {
     // pf_q.cur: the adopted batch the next interest update with q == NULL consumes (-1 once consumed).
     QStage dq_pf[2] = {};
     QueryDev dq_pf_view[2] = {};  // the batch each set holds
+    uint32_t dq_pf_spots[2] = {0, 0};  // and its spot total
     Prefetch pf_q;
     struct RStage {
         uint32_t *off, *sender; int64_t* arrival; uint64_t *index, *cmi;
@@ -366,6 +367,9 @@ struct chd_engine {
         uint32_t n_bound = 0;
         FollowDev st{};     // per-slot bindings, [max_subscribers]
         FollowBatch q{};    // the generated batch, [max_queries]; q.n_selected: queries in it
+        uint8_t* spot_buf = nullptr;  // merged batches: q.spot_x | q.spot_z | q.spot_dist, spot_cap spots each, grown on demand
+        uint64_t spot_bytes = 0, spot_cap = 0;
+        uint32_t* hdr = nullptr;  // [1] the host part's length, written before the merged generation's graph
         QueryDev view{};    // the generated batch as the interest stage reads it
         bool ready = false;     // a generated batch waits for the interest update that consumes it
         uint8_t* d_stage = nullptr;  // chd_follow_bind / chd_follow_unbind: staged arguments
@@ -511,6 +515,10 @@ chd_status chd_fetch_guard(chd_engine* e, cudaStream_t s);
 // chd_build / chd_update_interest without the fetch guard, enqueued on `s` (chd_tick runs the interest update on aux_stream)
 chd_status chd_build_on(chd_engine* e, cudaStream_t s);
 chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query_batch* q, int64_t now_ns);
+// Copies a query batch into the engine's device SoA (or a prefetch staging set) on `s`, device arrays in place, and returns the
+// device view; *spots (if given): the batch's spot total
+chd_status chd_upload_queries(chd_engine* e, cudaStream_t s, const chd_query_batch* q, QueryDev* out, bool need_sub,
+                              chd_engine::QStage* stage = nullptr, uint32_t* spots = nullptr);
 // what the fan-out / payload kernels read: the host-owned CSR snapshot (staged or zero-copy) or the device-owned rings
 RingDev chd_ring_view(const chd_engine* e);
 // The stable sort by cell on `s` (chd_entities.cu): values val (nullptr: the index) of keys key[0, n) in [0, keys) (n_ptr: the
@@ -541,6 +549,7 @@ chd_status chd_rule_halo_import(chd_engine* e);
 chd_status chd_rule_follow(chd_engine* e, const char* fn);
 chd_status chd_rule_no_followers(chd_engine* e, const char* fn);
 chd_status chd_rule_one_batch(chd_engine* e, const char* fn);
+chd_status chd_rule_merged_batch(chd_engine* e, bool adopted);
 // followers (chd_follow.cu): the listed slots (n == 0 with slot == nullptr: every slot) follow nothing from now on; d_slot: the
 // same list on the device if the caller uploaded it already
 chd_status chd_follow_drop(chd_engine* e, const uint32_t* slot, const uint32_t* d_slot, uint32_t n);

@@ -6,10 +6,13 @@
 // engine stream too or on the second stream between the tick's fork and its join, which the engine stream waits for before the
 // tick ends.  A generation enqueued after that tick is therefore ordered after the last read of the batch; while a
 // chd_begin_interest is pending (forked, not joined yet) chd_follow_queries is refused.  The generation writes follower-owned
-// arrays only, none of which an asynchronous read-back copies, so it needs no chd_fetch_guard.
+// arrays only, none of which an asynchronous read-back copies, so it needs no chd_fetch_guard.  A merged generation
+// (chd_follow_queries_with) also reads the host part, from the query scratch or an adopted prefetch set, on the same stream; it
+// copies everything into follower-owned arrays, so the prefetch set is released right after it.
 #include "chd_engine.h"
 
 #include "chd_follow.cuh"
+#include "chd_misc.cuh"
 
 namespace {
 
@@ -21,16 +24,19 @@ bool follow_alloc(chd_engine* e) {
     const uint64_t S = e->lim.max_subscribers, Q = e->lim.max_queries;
     FollowDev& d = F.st;
     FollowBatch& q = F.q;
-    bool ok = dalloc(e, &d.entity, S) && dalloc(e, &d.kind, S) && dalloc(e, &d.dirty, S) && dalloc(e, &d.tslot, S) && dalloc(e, &d.res, S);
+    bool ok = dalloc(e, &d.entity, S) && dalloc(e, &d.kind, S) && dalloc(e, &d.dirty, S) && dalloc(e, &d.tslot, S) && dalloc(e, &d.res, S) &&
+              dalloc(e, &d.ovr, S);
     for (double** p : {&d.sph_r, &d.box_ex, &d.box_ez, &d.cone_dx, &d.cone_dz, &d.cone_angle, &d.cone_r, &d.last_x, &d.last_z}) ok = ok && dalloc(e, p, S);
-    ok = ok && dalloc(e, &q.sub, Q) && dalloc(e, &q.kind, Q) && dalloc(e, &q.n_selected, 1);
+    ok = ok && dalloc(e, &q.sub, Q) && dalloc(e, &q.kind, Q) && dalloc(e, &q.n_selected, 1) && dalloc(e, &q.spot_off, Q + 1) &&
+         dalloc(e, &q.spot_ndist, Q) && dalloc(e, &q.missing, Q) && dalloc(e, &F.hdr, 1);
     for (double** p : {&q.sph_cx, &q.sph_cz, &q.sph_r, &q.box_cx, &q.box_cz, &q.box_ex, &q.box_ez, &q.cone_cx, &q.cone_cz, &q.cone_dx, &q.cone_dz,
                        &q.cone_angle, &q.cone_r})
         ok = ok && dalloc(e, p, Q);
     ok = ok && chd_make_site(e, F.site, S + 1, EP_FOLLOW);
     if (!ok) return false;
-    if (cudaMemsetAsync(d.kind, 0, S, e->stream) != cudaSuccess || cudaMemsetAsync(q.n_selected, 0, 4, e->stream) != cudaSuccess)
-        return e->fail("cudaMemsetAsync failed in chd_follow_bind");
+    if (cudaMemsetAsync(d.kind, 0, S, e->stream) != cudaSuccess || cudaMemsetAsync(d.ovr, 0, S, e->stream) != cudaSuccess ||
+        cudaMemsetAsync(q.n_selected, 0, 4, e->stream) != cudaSuccess)
+        return e->fail("cudaMemsetAsync failed allocating the follower state");
     F.h_kind.assign(S, 0);
     F.on = true;
     return true;
@@ -42,6 +48,104 @@ chd_status stage_upload(chd_engine* e, const void* h, uint64_t bytes) {
     if (!ensure_cap(e, &F.d_stage, &F.stage_cap, bytes, bytes + bytes / 2 + 4096)) return CHD_ERR_CUDA;
     CU(e, cudaMemcpyAsync(F.d_stage, h, bytes, cudaMemcpyHostToDevice, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
+    return CHD_OK;
+}
+
+// The size class of a merged batch's host part: 0, or max(256, the next power of two >= n)
+uint64_t host_class(uint32_t n) {
+    if (!n) return 0;
+    uint64_t H = 256;
+    while (H < n) H <<= 1;
+    return H;
+}
+
+// Merged batches: room for `spots` spots (at least one, so that the spot arrays exist whenever the host part has spot_off).  The
+// arrays are replaced, not kept: the merge rewrites them before anything reads them.
+bool spot_alloc(chd_engine* e, uint64_t spots) {
+    chd_engine::Follow& F = e->fw;
+    const uint64_t need = std::max<uint64_t>(spots, 1), cap = std::max<uint64_t>(need + need / 2, 4096);
+    if (need <= F.spot_cap) return true;
+    if (!ensure_cap(e, &F.spot_buf, &F.spot_bytes, 20 * need, 20 * cap)) return false;
+    F.spot_cap = cap;
+    F.q.spot_x = reinterpret_cast<double*>(F.spot_buf);
+    F.q.spot_z = F.q.spot_x + cap;
+    F.q.spot_dist = reinterpret_cast<uint32_t*>(F.q.spot_z + cap);
+    return true;
+}
+
+// The follow stage on the engine stream: the batch generated from the bindings, behind the host part h of n_h entries (spots: its
+// spot total) when n_h > 0.
+chd_status follow_generate(chd_engine* e, uint32_t mode, const QueryDev& h, uint32_t n_h, uint32_t spots) {
+    chd_engine::Follow& F = e->fw;
+    const bool merged = n_h > 0;
+    if (!merged && (!F.on || !F.n_bound)) {  // nothing follows: an empty batch (it still applies pending lifecycle changes)
+        F.view = QueryDev{};
+        F.ready = true;
+        return CHD_OK;
+    }
+    cudaStream_t s = e->stream;
+    StageTimer timer(e, s, CHD_STAGE_FOLLOW);
+    const uint32_t S = e->n_slots, B = F.n_bound, H = (uint32_t)host_class(n_h);
+    const FollowEntities ent = e->tbl.on ? FollowEntities{e->d_x, e->d_z, e->lim.max_entities, e->tbl.d_table, e->tbl.bits, e->tbl.d_id_of_slot}
+                                         : FollowEntities{e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z, e->n_own, nullptr, 0, nullptr};
+    chd_status st = chd_epoch_tick(e, s, EP_FOLLOW);
+    if (st != CHD_OK) return st;
+    const FollowBatch& q = F.q;
+    if (!merged) {
+        // the graph bakes in the slot and follower counts, the mode and where the positions live (the state arrays never move)
+        const uint64_t key = stage_key(0x666f6c6cull, S, B, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub);
+        st = run_stage(e, s, F.g, key, [&]() -> chd_status {
+            // the skip tail: entries behind the selected count name no slot and no kind
+            CU(e, cudaMemsetAsync(q.sub, 0xFF, 4ull * B, s));
+            CU(e, cudaMemsetAsync(q.kind, 0, B, s));
+            bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_FOLLOW);
+            KCHECK(e);
+            SCAN(e, compact_1p(FollowFlag<false>{F.st, ent, mode}, FollowSink<false>{F.st, q, 0}, S, F.site, s));
+            return CHD_OK;
+        });
+    } else {
+        if (h.spot_off && !spot_alloc(e, spots)) return CHD_ERR_CUDA;
+        // the host count changes from tick to tick inside one size class: it is read from F.hdr, not baked into the graph
+        set_u32_kernel<<<1, 1, 0, s>>>(F.hdr, n_h);
+        KCHECK(e);
+        FollowMerge m{h, F.hdr, H, H + B, S, q, F.st.ovr};
+        m.h.n = 0;
+        const unsigned grid = (unsigned)std::min<uint64_t>(blocks_for(std::max<uint64_t>(H + B + 1ull, F.spot_cap), FOLLOW_THREADS), 4ull * e->sm_count);
+        // ... and so do the host part's arrays (the staging set of the query scratch or a prefetch, or the caller's device arrays) and
+        // the spot buffer's three arrays: a grown buffer may start where the old one did, but its spot_z and spot_dist move with the
+        // capacity
+        const uint64_t key = stage_key(0x666f6c6dull, S, B, H, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub, grid, h.sub, h.kind,
+                                       h.sph_cx, h.sph_cz, h.sph_r, h.box_cx, h.box_cz, h.box_ex, h.box_ez, h.cone_cx, h.cone_cz, h.cone_dx, h.cone_dz,
+                                       h.cone_angle, h.cone_r, h.spot_off, h.spot_ndist, h.spot_x, h.spot_z, h.spot_dist, q.spot_x, q.spot_z,
+                                       q.spot_dist, F.spot_cap);
+        st = run_stage(e, s, F.g, key, [&]() -> chd_status {
+            bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_FOLLOW);
+            KCHECK(e);
+            follow_merge_kernel<<<grid, FOLLOW_THREADS, 0, s>>>(m);
+            KCHECK(e);
+            SCAN(e, compact_1p(FollowFlag<true>{F.st, ent, mode}, FollowSink<true>{F.st, q, H}, S, F.site, s));
+            return CHD_OK;
+        });
+    }
+    if (st != CHD_OK) return st;
+    if (!e->tbl.on) {  // the positions were read: a prefetch may refill their buffers after this
+        st = chd_note_pos_read(e, s);
+        if (st != CHD_OK) return st;
+    }
+    QueryDev v{};
+    v.n = H + B;
+    v.sub = q.sub; v.kind = q.kind;
+    v.sph_cx = q.sph_cx; v.sph_cz = q.sph_cz; v.sph_r = q.sph_r;
+    v.box_cx = q.box_cx; v.box_cz = q.box_cz; v.box_ex = q.box_ex; v.box_ez = q.box_ez;
+    v.cone_cx = q.cone_cx; v.cone_cz = q.cone_cz; v.cone_dx = q.cone_dx; v.cone_dz = q.cone_dz; v.cone_angle = q.cone_angle; v.cone_r = q.cone_r;
+    if (merged) {
+        v.missing = q.missing;
+        if (h.spot_off) {
+            v.spot_off = q.spot_off; v.spot_ndist = q.spot_ndist; v.spot_x = q.spot_x; v.spot_z = q.spot_z; v.spot_dist = q.spot_dist;
+        }
+    }
+    F.view = v;
+    F.ready = true;
     return CHD_OK;
 }
 
@@ -166,45 +270,44 @@ chd_status chd_follow_queries(chd_engine* e, uint32_t mode) {
     if (chd_rule_follow(e, "chd_follow_queries") != CHD_OK || chd_rule_one_batch(e, "chd_follow_queries") != CHD_OK) return CHD_ERR_STATE;
     std::lock_guard<std::recursive_mutex> lk(e->mu);
     CU(e, cudaSetDevice(e->device));
+    return follow_generate(e, mode, QueryDev{}, 0, 0);
+}
+
+chd_status chd_follow_queries_with(chd_engine* e, uint32_t mode, const chd_query_batch* q) {
+    if (!e || (mode != CHD_FOLLOW_ALL && mode != CHD_FOLLOW_MOVED)) return CHD_ERR_INVALID;
+    if (chd_rule_follow(e, "chd_follow_queries_with") != CHD_OK || chd_rule_merged_batch(e, !q) != CHD_OK) return CHD_ERR_STATE;
+    std::lock_guard<std::recursive_mutex> lk(e->mu);
+    CU(e, cudaSetDevice(e->device));
     chd_engine::Follow& F = e->fw;
-    if (!F.on || !F.n_bound) {  // nothing follows: an empty batch (it still applies pending lifecycle changes)
-        F.view = QueryDev{};
-        F.ready = true;
-        return CHD_OK;
+    const int set = q ? -1 : e->pf_q.cur;  // the adopted prefetch set holding the host part
+    const QueryDev* adopted = q ? nullptr : &e->dq_pf_view[set];
+    if (q ? !q->sub : !adopted->sub) {
+        e->fail("chd_follow_queries_with: the host part is an identity batch (sub == NULL), which cannot be merged");
+        return CHD_ERR_INVALID;
     }
-    cudaStream_t s = e->stream;
-    StageTimer timer(e, s, CHD_STAGE_FOLLOW);
-    const uint32_t S = e->n_slots, B = F.n_bound;
-    const FollowEntities ent = e->tbl.on ? FollowEntities{e->d_x, e->d_z, e->lim.max_entities, e->tbl.d_table, e->tbl.bits, e->tbl.d_id_of_slot}
-                                         : FollowEntities{e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z, e->n_own, nullptr, 0, nullptr};
-    chd_status st = chd_epoch_tick(e, s, EP_FOLLOW);
-    if (st != CHD_OK) return st;
-    const FollowBatch& q = F.q;
-    // the graph bakes in the slot and follower counts, the mode and where the positions live (the state arrays never move)
-    const uint64_t key = stage_key(0x666f6c6cull, S, B, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub);
-    st = run_stage(e, s, F.g, key, [&]() -> chd_status {
-        // the skip tail: entries behind the selected count name no slot and no kind
-        CU(e, cudaMemsetAsync(q.sub, 0xFF, 4ull * B, s));
-        CU(e, cudaMemsetAsync(q.kind, 0, B, s));
-        bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_FOLLOW);
-        KCHECK(e);
-        SCAN(e, compact_1p(FollowFlag{F.st, ent, mode}, FollowSink{F.st, q}, S, F.site, s));
-        return CHD_OK;
-    });
-    if (st != CHD_OK) return st;
-    if (!e->tbl.on) {  // the positions were read: a prefetch may refill their buffers after this
-        st = chd_note_pos_read(e, s);
-        if (st != CHD_OK) return st;
+    const uint32_t n_h = q ? q->n : adopted->n;
+    const uint64_t len = host_class(n_h) + (F.on ? F.n_bound : 0);
+    if (len > e->lim.max_queries) {
+        e->fail("chd_follow_queries_with: merged batch of %llu entries (%u host entries in a class of %llu, %u followers) > max_queries %u",
+                (unsigned long long)len, n_h, (unsigned long long)host_class(n_h), F.n_bound, e->lim.max_queries);
+        return CHD_ERR_CAPACITY;
     }
-    QueryDev v{};
-    v.n = B;
-    v.sub = q.sub; v.kind = q.kind;
-    v.sph_cx = q.sph_cx; v.sph_cz = q.sph_cz; v.sph_r = q.sph_r;
-    v.box_cx = q.box_cx; v.box_cz = q.box_cz; v.box_ex = q.box_ex; v.box_ez = q.box_ez;
-    v.cone_cx = q.cone_cx; v.cone_cz = q.cone_cz; v.cone_dx = q.cone_dx; v.cone_dz = q.cone_dz; v.cone_angle = q.cone_angle; v.cone_r = q.cone_r;
-    F.view = v;
-    F.ready = true;
-    return CHD_OK;
+    QueryDev h{};
+    uint32_t spots = 0;
+    chd_status st = CHD_OK;
+    if (n_h && q) {
+        st = chd_upload_queries(e, e->stream, q, &h, true, nullptr, &spots);  // into the query scratch, which the merge reads on the same stream
+    } else if (adopted) {  // ordered after the upload like any reader of an adopted set, whether or not the part is empty
+        h = *adopted;
+        spots = e->dq_pf_spots[set];
+        st = chd_pf_wait(e, e->pf_q, e->stream);
+    }
+    if (st != CHD_OK) return st;
+    if (n_h && !follow_alloc(e)) return CHD_ERR_CUDA;
+    st = follow_generate(e, mode, h, n_h, spots);
+    if (st != CHD_OK || set < 0) return st;
+    e->pf_q.cur = -1;  // consumed: the staging set may be refilled once the merge has read it
+    return chd_pf_note_read(e, e->pf_q, set, e->stream);
 }
 
 chd_status chd_get_follow(chd_engine* e, uint32_t* slot, uint32_t* entity, uint32_t* status, double* cx, double* cz, uint32_t cap, uint32_t* count,

@@ -26,11 +26,22 @@ struct FollowEntities {
     const uint32_t* __restrict__ id_of_slot;
 };
 
+// Merged: the batch has a host part (chd_follow_queries_with), whose entries marked their slots in f.ovr.  The flag reads and
+// clears the mark of every slot below the slot count, bound or not, so no mark outlives the generation.
+template <bool Merged>
 struct FollowFlag {
     FollowDev f;
     FollowEntities ent;
     uint32_t mode;
     __device__ __forceinline__ bool operator()(uint64_t s) const {
+        if (Merged && f.ovr[s]) {  // the slot's explicit query wins this tick; the next MOVED generation selects it again
+            f.ovr[s] = 0;
+            if (f.kind[s]) {
+                f.res[s] = FOLLOW_NO_QUERY | (uint32_t)CHD_FOLLOW_OVERRIDDEN;
+                f.dirty[s] = 1;
+            }
+            return false;
+        }
         if (!f.kind[s]) return false;
         uint32_t p = f.entity[s];
         if (ent.table) {
@@ -60,10 +71,14 @@ struct FollowFlag {
     }
 };
 
+// Merged: the followers' entries start at `base` (the host part's size class H).
+template <bool Merged>
 struct FollowSink {
     FollowDev f;
     FollowBatch q;
-    __device__ __forceinline__ void operator()(uint64_t s, uint32_t k) const {
+    uint32_t base;
+    __device__ __forceinline__ void operator()(uint64_t s, uint32_t r) const {
+        const uint32_t k = Merged ? base + r : r;
         const uint32_t kind = f.kind[s];
         const double x = f.last_x[s], z = f.last_z[s];  // (written by this thread's flag call)
         q.sub[k] = (uint32_t)s;
@@ -104,6 +119,66 @@ struct FollowReportSink {
     }
     __device__ __forceinline__ void total(uint32_t c) const { *count = c; }
 };
+
+// chd_follow_queries_with: the host part `h` (h.n is not read: the replayed graph must not bake the host count in; it is hdr[0],
+// written before the graph) copied into the merged arrays q, then skip entries up to H + B.  Grid-stride over the entries and, when
+// the host part has spots, over its spot data.  Only the arrays the host part supplies are copied (kind == NULL: all sphere); an
+// entry whose kind needs an array it did not supply is marked in q.missing, and the slot of every entry below the slot count is
+// marked for FollowFlag.  The compaction that follows writes the selected followers over the skip entries from H on.
+struct FollowMerge {
+    QueryDev h;
+    const uint32_t* __restrict__ hdr;  // [0] host entries n_h
+    uint32_t H, len;                   // size class, H + B
+    uint32_t n_slots;
+    FollowBatch q;
+    uint8_t* __restrict__ ovr;
+};
+__global__ void __launch_bounds__(FOLLOW_THREADS) follow_merge_kernel(FollowMerge m) {
+    const QueryDev& h = m.h;
+    const FollowBatch& q = m.q;
+    const uint32_t n_h = *m.hdr;
+    const uint32_t spots = h.spot_off ? h.spot_off[n_h] : 0u;
+    const uint32_t stride = gridDim.x * blockDim.x;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i <= m.len; i += stride) {
+        if (i < n_h) {
+            const uint32_t sub = h.sub[i], kind = query_kind(h, i);
+            q.sub[i] = sub;
+            q.kind[i] = (uint8_t)kind;
+            q.missing[i] = query_arrays_missing(h, kind);
+            if (h.sph_cx) q.sph_cx[i] = h.sph_cx[i];
+            if (h.sph_cz) q.sph_cz[i] = h.sph_cz[i];
+            if (h.sph_r) q.sph_r[i] = h.sph_r[i];
+            if (h.box_cx) q.box_cx[i] = h.box_cx[i];
+            if (h.box_cz) q.box_cz[i] = h.box_cz[i];
+            if (h.box_ex) q.box_ex[i] = h.box_ex[i];
+            if (h.box_ez) q.box_ez[i] = h.box_ez[i];
+            if (h.cone_cx) q.cone_cx[i] = h.cone_cx[i];
+            if (h.cone_cz) q.cone_cz[i] = h.cone_cz[i];
+            if (h.cone_dx) q.cone_dx[i] = h.cone_dx[i];
+            if (h.cone_dz) q.cone_dz[i] = h.cone_dz[i];
+            if (h.cone_angle) q.cone_angle[i] = h.cone_angle[i];
+            if (h.cone_r) q.cone_r[i] = h.cone_r[i];
+            if (h.spot_off) {
+                q.spot_off[i] = h.spot_off[i];
+                q.spot_ndist[i] = h.spot_ndist[i];
+            }
+            if (sub < m.n_slots) m.ovr[sub] = 1;
+        } else {
+            if (i < m.len) {
+                q.sub[i] = 0xFFFFFFFFu;
+                q.kind[i] = 0;
+                q.missing[i] = 0;
+                if (h.spot_off) q.spot_ndist[i] = 0;
+            }
+            if (h.spot_off) q.spot_off[i] = spots;
+        }
+    }
+    for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < spots; k += stride) {
+        q.spot_x[k] = h.spot_x[k];
+        q.spot_z[k] = h.spot_z[k];
+        q.spot_dist[k] = h.spot_dist[k];
+    }
+}
 
 // chd_follow_bind: scatter m staged bindings (one per slot: the host keeps the last of a slot named twice) into the per-slot state.
 // A bound slot starts dirty, with no query generated yet.

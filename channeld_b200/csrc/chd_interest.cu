@@ -7,9 +7,6 @@
 
 extern "C" {
 
-static chd_status upload_queries(chd_engine* e, cudaStream_t s, const chd_query_batch* q, QueryDev* out, bool need_sub,
-                                 chd_engine::QStage* stage = nullptr);
-
 chd_status chd_prefetch_queries(chd_engine* e, const chd_query_batch* q) {
     if (!e || !q) return CHD_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lk(e->mu);
@@ -19,7 +16,7 @@ chd_status chd_prefetch_queries(chd_engine* e, const chd_query_batch* q) {
     if (st != CHD_OK) return st;
     chd_engine::QStage& qs = e->dq_pf[set];
     if (!qs.spot_dist && !alloc_qstage(e, qs)) return CHD_ERR_CUDA;  // (spot_dist is allocated last)
-    st = upload_queries(e, e->up_stream, q, &e->dq_pf_view[set], true, &qs);
+    st = chd_upload_queries(e, e->up_stream, q, &e->dq_pf_view[set], true, &qs, &e->dq_pf_spots[set]);
     return st != CHD_OK ? st : chd_pf_end(e, e->pf_q);
 }
 
@@ -108,9 +105,8 @@ chd_status chd_remove_subscribers(chd_engine* e, const uint32_t* slot, uint32_t 
     return chd_follow_drop(e, slot, e->d_lc_slot, n);  // a removed slot follows nothing
 }
 
-// copies the batch into the engine's device SoA (or a prefetch staging set) on `s` and returns the device view
-static chd_status upload_queries(chd_engine* e, cudaStream_t s, const chd_query_batch* q, QueryDev* out, bool need_sub,
-                                 chd_engine::QStage* stage) {
+chd_status chd_upload_queries(chd_engine* e, cudaStream_t s, const chd_query_batch* q, QueryDev* out, bool need_sub, chd_engine::QStage* stage,
+                              uint32_t* spots) {
     if (!q) return CHD_ERR_INVALID;
     chd_engine::QStage& dq = stage ? *stage : e->dq;
     const uint32_t n = q->n;
@@ -120,6 +116,7 @@ static chd_status upload_queries(chd_engine* e, cudaStream_t s, const chd_query_
     }
     QueryDev d{};
     d.n = n;
+    if (spots) *spots = 0;
 #define UP(field, T)                                                                                      \
     if (q->field) {                                                                                       \
         if (chd_is_device_ptr(e, q->field)) {                                                                 \
@@ -153,6 +150,7 @@ static chd_status upload_queries(chd_engine* e, cudaStream_t s, const chd_query_
         CU(e, cudaMemcpyAsync(e->h_u32, dq.spot_off + n, 4, cudaMemcpyDeviceToHost, s));
         CU(e, cudaStreamSynchronize(s));
         total = *e->h_u32;
+        if (spots) *spots = total;
         if (total > e->lim.max_spots) {
             e->fail("%u spots > max_spots %u", total, e->lim.max_spots);
             return CHD_ERR_CAPACITY;
@@ -191,7 +189,7 @@ chd_status chd_query_channel_ids(chd_engine* e, const chd_query_batch* q, uint32
     CU(e, cudaSetDevice(e->device));
     CU(e, cudaStreamSynchronize(e->aux_stream));  // an in-flight interest update shares the query scratch
     QueryDev d;
-    chd_status st = upload_queries(e, e->stream, q, &d, false);
+    chd_status st = chd_upload_queries(e, e->stream, q, &d, false);
     if (st != CHD_OK) return st;
     const uint32_t n = d.n;
     if (n == 0) {
@@ -314,7 +312,7 @@ chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query
         st = chd_pf_wait(e, e->pf_q, s);
         if (st != CHD_OK) return st;
     } else {
-        st = upload_queries(e, s, q, &d, true);  // H2D / D2D copies into the engine's SoA: outside the graph
+        st = chd_upload_queries(e, s, q, &d, true);  // H2D / D2D copies into the engine's SoA: outside the graph
         if (st != CHD_OK) return st;
     }
     // (outside the replayed graphs: the tick time is a launch argument) tick time, new scan epoch, zeroed counters
@@ -325,7 +323,7 @@ chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query
     // the graph bakes in which staging arrays are live, the batch size and the pair-buffer parity
     const uint64_t key = stage_key(0x696e74ull, d.n, e->n_slots, e->cur, e->lifecycle_used, e->mig.base, e->have_cell_start, d.sub, d.kind, d.sph_cx,
                                    d.sph_cz, d.sph_r, d.box_cx, d.box_cz, d.box_ex, d.box_ez, d.cone_cx, d.cone_cz, d.cone_dx, d.cone_dz, d.cone_angle,
-                                   d.cone_r, d.spot_off, d.spot_ndist, d.spot_x, d.spot_z, d.spot_dist);
+                                   d.cone_r, d.spot_off, d.spot_ndist, d.spot_x, d.spot_z, d.spot_dist, d.missing);
     st = run_stage(e, s, e->g_interest, key, [&]() { return interest_enqueue(e, s, d, 0); });
     if (st != CHD_OK) return st;
     CU(e, cudaEventRecord(e->ev_pairs, s));  // the new pairs exist: emit may start (chd_tick waits on this)

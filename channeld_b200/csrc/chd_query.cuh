@@ -49,8 +49,6 @@ struct BboxAcc {
     }
 };
 
-__device__ __forceinline__ uint32_t query_kind(const QueryDev& q, uint32_t i) { return q.kind ? q.kind[i] : (uint32_t)CHD_AOI_SPHERE; }
-
 // Q1: bounding box of the cells a query's lattice samples can reach.
 __device__ __forceinline__ Bbox query_bbox(const GridDev& g, const QueryDev& q, uint32_t i, uint32_t kind) {
     BboxAcc acc;
@@ -96,7 +94,8 @@ struct WinRef {
 // cursor (zeroed by the stage's first kernel) instead of a device-wide prefix sum (two launches less per tick).
 // A query whose window does not fit the scratch gets CHD_Q_ERR_CAPACITY: like any failed query it leaves the subscriber's
 // subscriptions untouched; CHD_OVF_WINDOW is raised and the cursor's final value is the required capacity.
-// A query that sets a kind bit without supplying that kind's arrays gets CHD_Q_ERR_MISSING_ARRAY.
+// A query that sets a kind bit without supplying that kind's arrays gets CHD_Q_ERR_MISSING_ARRAY; in a merged batch the host
+// part's entries are judged by the arrays the host part supplied (q.missing, written by follow_merge_kernel).
 __global__ void __launch_bounds__(128)
     query_kernel(GridDev g, QueryDev q, Bbox* __restrict__ bbox, uint64_t* __restrict__ win_off, uint64_t win_cap,
                  unsigned long long* __restrict__ win_cursor, uint32_t* __restrict__ window, uint32_t* __restrict__ side_cell,
@@ -111,10 +110,7 @@ __global__ void __launch_bounds__(128)
     win.b.gx0 = win.b.gy0 = win.b.bw = win.b.bh = 0;
     if (i < q.n) {
         kind = query_kind(q, i);
-        missing = ((kind & CHD_AOI_BOX) && (!q.box_cx || !q.box_cz || !q.box_ex || !q.box_ez)) ||
-                  ((kind & CHD_AOI_SPHERE) && (!q.sph_cx || !q.sph_cz || !q.sph_r)) ||
-                  ((kind & CHD_AOI_CONE) && (!q.cone_cx || !q.cone_cz || !q.cone_dx || !q.cone_dz || !q.cone_angle || !q.cone_r)) ||
-                  ((kind & CHD_AOI_SPOTS) && q.spot_off && (!q.spot_x || !q.spot_z || !q.spot_dist));
+        missing = query_arrays_missing(q, kind) || (q.missing && q.missing[i]);
         if (!missing) win.b = query_bbox(g, q, i, kind);
     }
     const uint32_t wn = win.b.bw * win.b.bh;

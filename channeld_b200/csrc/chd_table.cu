@@ -320,6 +320,18 @@ chd_status chd_rule_one_batch(chd_engine* e, const char* fn) {
     return CHD_OK;
 }
 
+// ... except that chd_follow_queries_with merges the two into one batch: the host part is q or (adopted) the adopted prefetched batch,
+// which it consumes.  So an adopted batch is required with q == NULL and refused beside a q.
+chd_status chd_rule_merged_batch(chd_engine* e, bool adopted) {
+    const char* fn = "chd_follow_queries_with";
+    if (e->fw.ready) return refuse(e, "%s: the batch generated by chd_follow_queries has not been consumed by an interest update yet", fn);
+    if (e->interest_pending) return refuse(e, "%s: chd_begin_interest is pending (not joined by chd_tick yet)", fn);
+    if (adopted && e->pf_q.cur < 0) return refuse(e, "%s: q == NULL needs chd_prefetch_queries + chd_adopt_prefetched first", fn);
+    if (!adopted && e->pf_q.cur >= 0)
+        return refuse(e, "%s: the adopted prefetched query batch has not been consumed (pass q == NULL to merge it)", fn);
+    return CHD_OK;
+}
+
 chd_status chd_entity_table_init(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_fresh_engine(e) != CHD_OK) return CHD_ERR_STATE;

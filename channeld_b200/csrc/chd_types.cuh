@@ -66,7 +66,20 @@ struct QueryDev {
     const uint32_t *spot_off, *spot_ndist;
     const double *spot_x, *spot_z;
     const uint32_t* spot_dist;
+    // nullptr except in a merged batch (chd_follow_queries_with): [n], entry i names a kind whose arrays the host part lacked
+    const uint8_t* missing;
 };
+
+// (query_kernel, and follow_merge_kernel for a merged batch's host part)
+__device__ __forceinline__ uint32_t query_kind(const QueryDev& q, uint32_t i) { return q.kind ? q.kind[i] : (uint32_t)CHD_AOI_SPHERE; }
+
+// A kind bit whose arrays the batch does not supply (CHD_Q_ERR_MISSING_ARRAY).  Spots without spot_off are ignored, not missing.
+__device__ __forceinline__ bool query_arrays_missing(const QueryDev& q, uint32_t kind) {
+    return ((kind & CHD_AOI_BOX) && (!q.box_cx || !q.box_cz || !q.box_ex || !q.box_ez)) ||
+           ((kind & CHD_AOI_SPHERE) && (!q.sph_cx || !q.sph_cz || !q.sph_r)) ||
+           ((kind & CHD_AOI_CONE) && (!q.cone_cx || !q.cone_cz || !q.cone_dx || !q.cone_dz || !q.cone_angle || !q.cone_r)) ||
+           ((kind & CHD_AOI_SPOTS) && q.spot_off && (!q.spot_x || !q.spot_z || !q.spot_dist));
+}
 
 struct Bbox {
     uint32_t gx0, gy0, bw, bh;  // bw == 0 => empty
@@ -198,14 +211,19 @@ struct FollowDev {
     uint8_t* dirty;           // bound or re-bound since the last batch that selected the slot, or its entity was missing then
     uint32_t* tslot;          // entity-table mode: the table slot the id was last found in (validated against slot -> id on use)
     uint32_t* res;            // what the last generation did with the slot: batch entry, or FOLLOW_NO_QUERY | reason
+    uint8_t* ovr;             // a host entry of the merged batch names the slot (set by follow_merge_kernel, cleared by FollowFlag)
 };
 
-// The generated batch: a query batch's SoA (chd_query_batch without spots) in device memory.
+// The generated batch: a query batch's SoA in device memory.  The spot arrays and `missing` are used by merged batches only.
 struct FollowBatch {
     uint32_t* sub;
     uint8_t* kind;
     double *sph_cx, *sph_cz, *sph_r, *box_cx, *box_cz, *box_ex, *box_ez, *cone_cx, *cone_cz, *cone_dx, *cone_dz, *cone_angle, *cone_r;
     uint32_t* n_selected;
+    uint32_t *spot_off, *spot_ndist;  // [Q + 1], [Q]
+    double *spot_x, *spot_z;          // [spot capacity], grown on demand
+    uint32_t* spot_dist;
+    uint8_t* missing;                 // [Q]
 };
 
 struct BcastDev {

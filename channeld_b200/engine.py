@@ -59,6 +59,13 @@ def make_batch(n, sub=None, kind=None, sphere=None, box=None, cone=None, spots=N
     return b, keep
 
 
+def host_part_size(n_h):
+    """H of chd_follow_queries_with: the size class of a host part of n_h entries (0, or max(256, the next power of two >= n_h)).
+    The followers' entries of the merged batch, and of its status list, start at H."""
+    n_h = int(n_h)
+    return 0 if n_h == 0 else max(256, 1 << (n_h - 1).bit_length())
+
+
 class Engine:
     def __init__(self, cfg, n_entities, n_subscribers, device=0, **limit_overrides):
         self.L = capi.lib()
@@ -426,6 +433,12 @@ class Engine:
         """Generates the tick's query batch from the bindings (asynchronous); the next begin_interest(None) /
         update_interest(None) or tick(None, flags | TICK_FOLLOW) consumes it."""
         self._ck(self.L.chd_follow_queries(self.h, int(mode)))
+
+    def follow_queries_with(self, mode=capi.FOLLOW_ALL, batch=None):
+        """follow_queries(mode) with the tick's explicit queries in front: `batch` (a chd_query_batch, sub required), or with
+        batch None the batch handed over by prefetch_queries + adopt_prefetched.  The merged batch has host_part_size(n) + followers
+        entries; it is consumed like follow_queries' batch."""
+        self._ck(self.L.chd_follow_queries_with(self.h, int(mode), C.byref(batch) if batch is not None else None))
 
     def get_follow(self):
         """-> dict(slot, entity, status, cx, cz: one entry per follower in slot order; n_selected)."""

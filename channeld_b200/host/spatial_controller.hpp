@@ -333,6 +333,12 @@ class GpuStaticGrid2DSpatialController {
     void FollowEntities(const chd_follow_batch& b) { check(chd_follow_bind(engine_, &b)); }
     void UnfollowEntities(const std::vector<uint32_t>& slot) { check(chd_follow_unbind(engine_, slot.data(), (uint32_t)slot.size())); }
     void FollowQueries(uint32_t mode = CHD_FOLLOW_MOVED) { check(chd_follow_queries(engine_, mode)); }
+    // A mixed world: the tick's explicit queries (connections that follow nothing, or a follower's own query for this tick) merged in
+    // front of the generated ones into one batch.  explicit == nullptr: the batch PrefetchQueries uploaded and AdoptPrefetched handed
+    // over.  Consumed like FollowQueries' batch; the followers' statuses start at the explicit part's size class (chd_gpu.h).
+    void FollowQueriesWith(const chd_query_batch* explicit_part, uint32_t mode = CHD_FOLLOW_MOVED) {
+        check(chd_follow_queries_with(engine_, mode, explicit_part));
+    }
     chd_entity_stats GetEntityStats() {
         chd_entity_stats s{};
         check(chd_get_entity_stats(engine_, &s));

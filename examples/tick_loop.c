@@ -168,6 +168,7 @@ int main(void) {
     /* The same world without a position mirror on the host: entities are events keyed by id (entity-table mode) and every
      * subscriber follows its pawn, so each tick is  move -> chd_follow_queries(MOVED) -> chd_begin_interest(NULL) -> chd_tick.
      * Only the moved entities go up; the queries are generated on the device for the followers whose pawn moved. */
+    lim.max_queries = 2 * n_subs; /* room for the mixed world below: the explicit part's size class + the followers */
     CHECK(chd_create(&cfg, &lim, 0, &e));
     CHECK(chd_set_subscribers(e, conn, n_subs));
     CHECK(chd_entity_table_init(e));
@@ -200,6 +201,47 @@ int main(void) {
         uint32_t followers = 0, selected = 0;
         CHECK(chd_get_follow(e, NULL, NULL, NULL, NULL, NULL, 0, &followers, &selected));
         printf("followers: %u bound, %u queries generated for the last tick, %llu pairs\n", followers, selected, (unsigned long long)sum.n_pairs);
+
+        /* A mixed world: every 4th connection is a spectator that sends its own UPDATE_SPATIAL_INTEREST each tick (a sphere
+         * anywhere, not on a pawn); the others keep following.  The explicit part is prefetched a tick ahead like any batch, and
+         * chd_follow_queries_with(.., NULL) merges the adopted part in front of the generated queries: one interest update, one diff
+         * and one read-back per tick, pipelined as above. */
+        const uint32_t n_x = (n_subs + 3) / 4;
+        uint32_t* xslot = malloc(4ull * n_x);
+        for (uint32_t j = 0; j < n_x; j++) xslot[j] = 4 * j;
+        CHECK(chd_follow_unbind(e, xslot, n_x));
+        double* xq = chd_alloc_pinned(2 * 3 * 8ull * n_x); /* two staging sets of cx | cz | r */
+#define PREFETCH_EXPLICIT(k, t)                                                                                           \
+    do {                                                                                                                  \
+        double* q_ = xq + (uint64_t)(k) * 3 * n_x;                                                                        \
+        for (uint32_t j = 0; j < n_x; j++) {                                                                             \
+            q_[j] = st[0].x[((uint64_t)j * 7 + (uint32_t)(t)) % n_entities]; /* stand-in camera positions */              \
+            q_[n_x + j] = st[0].z[((uint64_t)j * 7 + (uint32_t)(t)) % n_entities];                                        \
+            q_[2 * n_x + j] = st[0].r[0];                                                                                 \
+        }                                                                                                                 \
+        chd_query_batch xb_;                                                                                              \
+        memset(&xb_, 0, sizeof xb_);                                                                                      \
+        xb_.n = n_x; xb_.sub = xslot; /* sub is required: the part names its slots */                                     \
+        xb_.sph_cx = q_; xb_.sph_cz = q_ + n_x; xb_.sph_r = q_ + 2 * n_x;                                                 \
+        CHECK(chd_prefetch_queries(e, &xb_));                                                                             \
+    } while (0)
+        PREFETCH_EXPLICIT(0, 0);
+        for (int tick = 0; tick < 20; tick++) {
+            const int64_t now = (int64_t)(tick + 21) * tick_ns;
+            for (uint32_t i = 0; i < n_moved; i++) mid[i] = id[((uint64_t)i * 100 + (uint32_t)tick) % n_entities];
+            CHECK(chd_move_entities(e, mid, st[tick & 1].x, st[tick & 1].z, n_moved));
+            CHECK(chd_adopt_prefetched(e));                                /* this tick's explicit part */
+            CHECK(chd_follow_queries_with(e, CHD_FOLLOW_MOVED, NULL));     /* ... merged with the followers' queries */
+            if (tick + 1 < 20) PREFETCH_EXPLICIT((tick + 1) & 1, tick + 1); /* the adopted set is free again: fill the other */
+            CHECK(chd_tick(e, NULL, now, CHD_TICK_BUILD | CHD_TICK_EMIT | CHD_TICK_FOLLOW, NULL));
+            CHECK(chd_fetch_results_async(e, &rb[tick & 1], hdr[tick & 1]));
+            if (tick) CHECK(chd_fetch_wait(e, &sum)); /* tick - 1: statuses [0, n_x) are the spectators', followers from H on */
+        }
+        CHECK(chd_fetch_wait(e, &sum));
+        printf("mixed world: %u spectators, %llu pairs\n", n_x, (unsigned long long)sum.n_pairs);
+#undef PREFETCH_EXPLICIT
+        chd_free_pinned(xq);
+        free(xslot);
         chd_free_pinned(mid);
         free(id); free(slot); free(pawn);
     }

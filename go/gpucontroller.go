@@ -537,6 +537,17 @@ func (ctl *GpuStaticGrid2DSpatialController) FollowQueries(mode uint32) error {
 	return nil
 }
 
+// FollowQueriesWith merges the tick's explicit queries (connections that follow nothing, such as spectators and SpotsAOI users, or a
+// follower's own query for this tick) in front of the generated ones, so one interest update covers both.  explicit == nil: the batch
+// PrefetchQueries uploaded and AdoptPrefetched handed over (the pipelined form); otherwise a batch as UpdateInterest takes it, with
+// sub set.  Consumed like FollowQueries' batch; chd_gpu.h gives the layout of the statuses.  UN-RUN like the rest of this file.
+func (ctl *GpuStaticGrid2DSpatialController) FollowQueriesWith(mode uint32, explicit *C.chd_query_batch) error {
+	if st := C.chd_follow_queries_with(ctl.engine, C.uint32_t(mode), explicit); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
 // MoveEntities: netIds / x / z in C memory, valid until the next Summary / FetchResults.  The last move of an id in one call wins;
 // moves of ids that are not live are ignored (counted in EntityStats).
 func (ctl *GpuStaticGrid2DSpatialController) MoveEntities(netIds []uint32, x, z []float32) error {

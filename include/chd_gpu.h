@@ -282,7 +282,8 @@ typedef struct chd_tick_summary {
  *                   subscribers untouched; the rest of the batch was applied; required_window_cells = scratch needed
  *                   (either of these two on a tick whose batch came from chd_follow_queries(CHD_FOLLOW_MOVED): the followers'
  *                   stored centres advanced when the batch was generated, not when it was applied, so re-issue the tick's queries
- *                   with chd_follow_queries(CHD_FOLLOW_ALL))
+ *                   with chd_follow_queries(CHD_FOLLOW_ALL); after chd_follow_queries_with(CHD_FOLLOW_MOVED, q), re-issue
+ *                   chd_follow_queries_with(CHD_FOLLOW_ALL) with the same host part)
  *   CHD_OVF_VISIBLE the expanded visible list was not written (offsets are valid); required_visible = entries needed
  *   CHD_OVF_DUE     the pairs whose decisions did not fit were left untouched (still due: they catch up at the next
  *                   chd_fanout_tick); the list holds the decisions that did fit plus CHD_DUE_VOID holes; required_due
@@ -514,11 +515,38 @@ chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out);
  *                       chd_update_interest with q == NULL, or chd_tick with CHD_TICK_FOLLOW, consumes it.  One batch per interest
  *                       update: CHD_ERR_STATE while an adopted prefetched batch or an earlier generated one is unconsumed, and
  *                       while a chd_begin_interest is pending; chd_adopt_prefetched of a query batch is refused while a generated
- *                       one is unconsumed.  Queries of subscribers that follow nothing go through chd_update_interest in an
- *                       update of their own.
+ *                       one is unconsumed.  Queries of subscribers that follow nothing join the batch through
+ *                       chd_follow_queries_with.
+ *   chd_follow_queries_with
+ *                       chd_follow_queries(mode) plus a HOST PART: the explicit queries of the tick (spectators, free cameras,
+ *                       SpotsAOI, cones that do not look along the pawn), merged with the generated ones into ONE batch on the
+ *                       engine stream, so one interest update, one diff, one status list and one read-back cover the whole tick.
+ *                       The host part is q, a batch exactly as chd_update_interest takes it (host or device arrays; device arrays
+ *                       are read in place; sub must not be NULL), or, with q == NULL, the batch handed over by
+ *                       chd_adopt_prefetched, which this call consumes.  The merged batch owns copies of everything it reads, so
+ *                       the adopted staging set is free for the next chd_prefetch_queries once the merge has run.  Layout, with
+ *                       n_h host entries, B followers, H = 0 if n_h == 0 else max(256, the next power of two >= n_h):
+ *                         [0, n_h)               the host part, in the host's order
+ *                         [n_h, H)               skip entries (sub = 0xFFFFFFFF, kind = 0, status CHD_Q_OK, no spots)
+ *                         [H, H + n_selected)    the selected followers, in ascending slot order
+ *                         [H + n_selected, H+B)  skip entries
+ *                       The batch length, and the length of its status list, is H + B (size classes keep the length, and so the
+ *                       stages' CUDA graphs, constant while the explicit count varies).  With n_h == 0 the call is
+ *                       chd_follow_queries(mode), bit for bit.  A host entry behaves as it does in a batch of its own (statuses,
+ *                       removed or unknown slots, spots, at most one entry per slot); an entry whose kind names arrays the host
+ *                       part did not supply gets CHD_Q_ERR_MISSING_ARRAY even though the followers supply them.  A follower slot
+ *                       with a host entry is OVERRIDDEN for this tick: its explicit query wins, it gets no generated query
+ *                       (chd_get_follow reports CHD_FOLLOW_OVERRIDDEN), its stored centre stays, and it counts as moved, so the
+ *                       next CHD_FOLLOW_MOVED generation selects it again and its subscriptions return to the follow shape (unbind
+ *                       the slot to keep the explicit query).  Consumed like chd_follow_queries' batch.  Refused, changing nothing
+ *                       (an adopted batch stays adopted): CHD_ERR_CAPACITY if H + B > max_queries; CHD_ERR_STATE on a slab,
+ *                       while a generated batch is unconsumed or a chd_begin_interest is pending, with q == NULL and no adopted
+ *                       query batch, and with q != NULL while an adopted one is unconsumed; CHD_ERR_INVALID for a bad mode or a
+ *                       host part with sub == NULL.
  *   chd_get_follow      after the interest update that consumed the batch (and before the next one): per follower, in ascending
  *                       slot order, its slot, entity, the centre of the last query generated for it, and status = the CHD_Q_*
- *                       status of its query, or CHD_FOLLOW_NOT_SELECTED / CHD_FOLLOW_NO_ENTITY.  *count = followers (copies
+ *                       status of its query (its entry in a merged batch is H + its rank), or CHD_FOLLOW_NOT_SELECTED /
+ *                       CHD_FOLLOW_NO_ENTITY / CHD_FOLLOW_OVERRIDDEN.  *count = followers (copies
  *                       min(count, cap)), *n_selected = queries in the last generated batch; this call is where the selected count
  *                       is reported (chd_tick_summary is unchanged).  Synchronous; any pointer may be NULL.
  * Followers are single-GPU: CHD_ERR_STATE on an engine made a slab (chd_set_slab / chd_comm_init; a follower's entity may live on
@@ -533,9 +561,11 @@ typedef struct chd_follow_batch {          /* SoA, HOST arrays */
 } chd_follow_batch;
 enum { CHD_FOLLOW_ALL = 0, CHD_FOLLOW_MOVED = 1 };
 enum { CHD_FOLLOW_NOT_SELECTED = 16, CHD_FOLLOW_NO_ENTITY = 17 }; /* beside CHD_Q_* in chd_get_follow's status */
+enum { CHD_FOLLOW_OVERRIDDEN = 18 };  /* the slot's host entry in chd_follow_queries_with's batch replaced its generated query */
 chd_status chd_follow_bind(chd_engine* e, const chd_follow_batch* b);
 chd_status chd_follow_unbind(chd_engine* e, const uint32_t* slot, uint32_t n);
 chd_status chd_follow_queries(chd_engine* e, uint32_t mode);
+chd_status chd_follow_queries_with(chd_engine* e, uint32_t mode, const chd_query_batch* q);
 chd_status chd_get_follow(chd_engine* e, uint32_t* slot, uint32_t* entity, uint32_t* status, double* cx, double* cz, uint32_t cap,
                           uint32_t* count, uint32_t* n_selected);
 
