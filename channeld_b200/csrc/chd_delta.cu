@@ -51,10 +51,11 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
     const uint64_t N = e->lim.max_entities;
     chd_status st = chd_epoch_tick(e, s, EP_DELTA);
     if (st != CHD_OK) return st;
-    // sizes, the key / pair buffers in use and the ids (the id scatter's, the table lists') are baked into the captured launches
+    // sizes, the key / pair / cell CSR buffers in use and the ids (the id scatter's, the table lists') are baked into the captured
+    // launches
     const EntityIds ids = chd_entity_ids(e);
     uint64_t key = stage_key(0x64656c7461ull, d.n, d.n_slots, D.n_out, e->cur, d.key, d.enter, d.leave, d.enter_cap, d.leave_cap, e->tbl.on,
-                             ids.own_ids, ids.gid, ids.own);
+                             ids.own_ids, ids.gid, ids.own, d.cell_start, d.sorted);  // (the cell CSR: the current copy-input set)
     // id mode: the scatter bakes in the build's length (host count or d_n_build) and the key buffer it reads
     const uint32_t* n_ptr = e->sorted_dev_n ? e->d_n_build : nullptr;
     const uint32_t n_scatter = e->sorted_dev_n ? e->lim.max_entities : e->n_sorted;
@@ -189,6 +190,7 @@ chd_status chd_get_visible_delta(chd_engine* e, uint64_t* enter_off, uint32_t* e
         return CHD_ERR_STATE;
     }
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     cudaStream_t s = e->stream;  // (a tick's delta on prep_stream is joined into the engine stream)
     const uint32_t S = D.n_out;
     DeltaLengths dn;

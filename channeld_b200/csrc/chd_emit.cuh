@@ -24,13 +24,15 @@ struct PairVcountIn {
 };
 
 // tile descriptors + first_pair[t] (the pair whose output interval [voff[p], voff[p+1]) contains entry t*EMIT_TILE);
-// also vis_off[s] = voff[pair_off[s]] and the V / overflow bookkeeping (one launch)
+// also vis_off[s] = voff[pair_off[s]] and the V / overflow bookkeeping (one launch).  V goes to the summary counters and to
+// set_visible, the copy-input set's own V that the copy kernels read.
 __global__ void __launch_bounds__(256)
     emit_partition_kernel(const uint32_t* __restrict__ n_pairs_ptr, uint64_t pair_cap, const uint64_t* __restrict__ voff,
                           const uint32_t* __restrict__ pair_cell, const uint32_t* __restrict__ cell_start, uint32_t* __restrict__ first_pair,
                           TileDesc* __restrict__ desc, uint64_t max_tiles, uint32_t n_slots, const uint32_t* __restrict__ pair_off,
                           uint64_t* __restrict__ vis_off, uint64_t vis_cap, Counters* __restrict__ ctr, unsigned long long* bump_epoch,
-                          uint32_t tile, uint32_t* __restrict__ general_tiles, uint32_t* __restrict__ n_general) {
+                          uint32_t tile, uint32_t* __restrict__ general_tiles, uint32_t* __restrict__ n_general,
+                          unsigned long long* __restrict__ set_visible) {
     const uint64_t n = min((uint64_t)*n_pairs_ptr, pair_cap);
     // last kernel of the emit preparation: open the NEXT execution's scan epoch (the scan of this one has completed)
     if (bump_epoch && blockIdx.x == 0 && threadIdx.x == 0) *bump_epoch = chd_next_epoch(*bump_epoch);
@@ -40,6 +42,7 @@ __global__ void __launch_bounds__(256)
             const uint64_t V = voff[n];
             ctr->n_visible = V;
             ctr->required_visible = V;
+            *set_visible = V;
             if (V > vis_cap) atomicOr(&ctr->overflow, (uint32_t)CHD_OVF_VISIBLE);
         }
     }

@@ -54,17 +54,17 @@ static bool pf_events(chd_engine* e, Prefetch& p) {
     return chd_make_event(e, &p.ev_upload) && chd_make_event(e, &p.ev_read[0]) && chd_make_event(e, &p.ev_read[1]);
 }
 
-chd_status chd_pf_begin(chd_engine* e, Prefetch& p, int* set) {
-    if (!e->up_stream && !chd_make_stream(e, &e->up_stream)) return CHD_ERR_CUDA;
+chd_status chd_pf_begin(chd_engine* e, Prefetch& p, int* set, cudaStream_t s) {
+    if (!s && !e->up_stream && !chd_make_stream(e, &e->up_stream)) return CHD_ERR_CUDA;
     if (!pf_events(e, p)) return CHD_ERR_CUDA;
-    if (p.read_recorded[p.next]) CU(e, cudaStreamWaitEvent(e->up_stream, p.ev_read[p.next], 0));
+    if (p.read_recorded[p.next]) CU(e, cudaStreamWaitEvent(s ? s : e->up_stream, p.ev_read[p.next], 0));
     *set = p.next;
     p.staged = -1;  // a staged upload is in this set: an upload that fails part way leaves nothing staged
     return CHD_OK;
 }
 
-chd_status chd_pf_end(chd_engine* e, Prefetch& p) {
-    CU(e, cudaEventRecord(p.ev_upload, e->up_stream));
+chd_status chd_pf_end(chd_engine* e, Prefetch& p, cudaStream_t s) {
+    CU(e, cudaEventRecord(p.ev_upload, s ? s : e->up_stream));
     p.staged = p.next;
     return CHD_OK;
 }
@@ -91,6 +91,25 @@ chd_status chd_pf_note_read(chd_engine* e, Prefetch& p, int set, cudaStream_t s)
     CU(e, cudaEventRecord(p.ev_read[set], s));
     p.read_recorded[set] = true;
     return CHD_OK;
+}
+
+cudaError_t chd_copy_wait(chd_engine* e) {
+    if (e->copy_pending < 0) return cudaSuccess;
+    const cudaError_t r = cudaStreamWaitEvent(e->stream, e->pf_copy.ev_read[e->copy_pending], 0);
+    if (r == cudaSuccess) e->copy_pending = -1;
+    return r;
+}
+
+void chd_copy_set_select(chd_engine* e, int set) {
+    const CopySet& c = e->copy_set[set];
+    e->d_sorted_ent = c.sorted_ent;
+    e->tbl.d_sorted_id = c.sorted_id;
+    e->d_cell_start = c.cell_start;
+    e->d_voff = c.voff;
+    e->d_first_pair = c.first_pair;
+    e->d_tile_desc = c.tile_desc;
+    e->d_general_tiles = c.general_tiles;
+    e->d_n_general = c.n_general;
 }
 
 chd_status chd_read_u32(chd_engine* e, const uint32_t* d, uint32_t* v) {
@@ -159,7 +178,10 @@ void chd_free_pinned(void* p) {
 void chd_destroy(chd_engine* e) {
     if (!e) return;
     cudaSetDevice(e->device);
-    if (e->stream) cudaStreamSynchronize(e->stream);
+    if (e->stream) {
+        chd_copy_wait(e);
+        cudaStreamSynchronize(e->stream);
+    }
     chd_comm_destroy(e);
     for (cudaStream_t s : e->streams) cudaStreamSynchronize(s);
     for (void* p : e->allocs) cudaFree(p);
@@ -281,7 +303,7 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     e->max_tiles = (L.max_visible + EMIT_WARP_TILE - 1) / EMIT_WARP_TILE + 1;  // (the smaller of the two tile sizes)
     // the aux stream carries short latency-bound kernels that should slot in ahead of the long emit kernel
     bool ok = chd_make_stream(e, &e->aux_stream) && chd_make_stream(e, &e->dl_stream) && chd_make_stream(e, &e->dl_stream_b) &&
-              chd_make_stream(e, &e->prep_stream);
+              chd_make_stream(e, &e->prep_stream) && chd_make_stream(e, &e->build_stream) && chd_make_stream(e, &e->copy_stream, true);
     for (cudaEvent_t* ev : {&e->ev_fork, &e->ev_join, &e->ev_interest, &e->ev_pairs, &e->ev_prep_done, &e->ev_build_done, &e->ev_counts})
         ok = ok && chd_make_event(e, ev);
     e->pf_pos.cur = 0;  // the pair allocated here is the front one; the first prefetch fills the other
@@ -292,7 +314,8 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
          dalloc(e, &e->d_sorted_key, N) &&
          // padded: an emit chunk that starts m != 0 entries into an aligned 16-byte chunk also loads the next aligned chunk,
          // which near the end of the array lies past N (chd_emit.cuh)
-         dalloc(e, &e->d_sorted_ent, ((N + 3) / 4) * 4 + 8) && dalloc(e, &e->d_cell_start, C + 2) &&
+         dalloc(e, &e->copy_set[0].sorted_ent, ((N + 3) / 4) * 4 + 8) && dalloc(e, &e->copy_set[1].sorted_ent, ((N + 3) / 4) * 4 + 8) &&
+         dalloc(e, &e->copy_set[0].cell_start, C + 2) && dalloc(e, &e->copy_set[1].cell_start, C + 2) &&
          dalloc(e, &e->d_epoch, EP_COUNT) && chd_init_epochs(e) &&
          alloc_cell_sort(e, e->ent_sort, (uint32_t)e->sm_count * 4, false, EP_BUILD) &&
          chd_make_site(e, e->site_qoff, Q + 1, EP_QUERY) && chd_make_site(e, e->site_slot, S + 1, EP_QUERY) &&
@@ -311,9 +334,10 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
          dalloc(e, &e->d_slot_query, S);
     ok = ok && dalloc(e, &e->d_new_off, (Q > P ? Q : P) + 2) && dalloc(e, &e->d_new_sub, P) && dalloc(e, &e->d_new_ch, P) && dalloc(e, &e->d_gone_sub, P) &&
          dalloc(e, &e->d_gone_ch, P);
-    ok = ok && dalloc(e, &e->d_pair_ch, P) && dalloc(e, &e->d_vcnt, P) && dalloc(e, &e->d_voff, P + 1) && dalloc(e, &e->d_first_pair, e->max_tiles + 8) && dalloc(e, &e->d_tile_desc, (L.max_visible + EMIT_TILE - 1) / EMIT_TILE + 8) &&
-         dalloc(e, &e->d_general_tiles, (L.max_visible + EMIT_TILE - 1) / EMIT_TILE + 8) && dalloc(e, &e->d_n_general, 4) &&
-         dalloc(e, &e->d_vis_off, S + 1) && dalloc(e, &e->d_vis, L.max_visible);
+    ok = ok && dalloc(e, &e->d_pair_ch, P) && dalloc(e, &e->d_vcnt, P) && dalloc(e, &e->d_vis_off, S + 1) && dalloc(e, &e->d_vis, L.max_visible);
+    for (CopySet& c : e->copy_set)
+        ok = ok && dalloc(e, &c.voff, P + 1) && dalloc(e, &c.first_pair, e->max_tiles + 8) && dalloc(e, &c.tile_desc, (L.max_visible + EMIT_TILE - 1) / EMIT_TILE + 8) &&
+             dalloc(e, &c.general_tiles, (L.max_visible + EMIT_TILE - 1) / EMIT_TILE + 8) && dalloc(e, &c.n_general, 4) && dalloc(e, &c.n_visible, 1);
     ok = ok && dalloc(e, &e->d_cell_max_interval, C) && dalloc(e, &e->d_cell_start_ns, C) && dalloc(e, &e->d_rb_begin, C + 1) && dalloc(e, &e->d_rb_end, C + 1) &&
          dalloc(e, &e->d_ring_flat_off, C + 2) && dalloc(e, &e->d_upd_off, C + 1);
     ok = ok && dalloc(e, &e->d_ring_off, C + 1) && dalloc(e, &e->d_ring_arrival, (uint64_t)L.max_ring_entries) &&
@@ -336,7 +360,14 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     CCU(cudaHostAlloc((void**)&e->h_get, 64, cudaHostAllocDefault));
     CCU(cudaMemsetAsync(e->d_ctr, 0, sizeof(Counters), e->stream));
     CCU(cudaMemsetAsync(e->d_win_cursor, 0, 8, e->stream));
-    CCU(cudaMemsetAsync(e->d_n_general, 0, 16, e->stream));
+    for (CopySet& c : e->copy_set) {
+        CCU(cudaMemsetAsync(c.n_general, 0, 16, e->stream));
+        CCU(cudaMemsetAsync(c.n_visible, 0, 8, e->stream));
+        CCU(cudaMemsetAsync(c.cell_start, 0, (C + 2) * 4, e->stream));
+    }
+    chd_copy_set_select(e, 0);
+    e->pf_copy.cur = 0;  // a build fills set 1 first
+    e->pf_copy.next = 1;
     CCU(cudaMemsetAsync(e->d_slot_ctl, 0, S, e->stream));
     CCU(cudaMemsetAsync(e->d_cell_max_interval, 0, C * 4, e->stream));
     CCU(cudaMemsetAsync(e->d_cell_start_ns, 0, C * 8, e->stream));
@@ -347,7 +378,6 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     CCU(cudaMemsetAsync(e->pairs[0].off, 0, (S + 1) * 4, e->stream));
     CCU(cudaMemsetAsync(e->pairs[1].off, 0, (S + 1) * 4, e->stream));
     CCU(cudaMemsetAsync(e->d_ring_off, 0, (C + 1) * 4, e->stream));
-    CCU(cudaMemsetAsync(e->d_cell_start, 0, (C + 2) * 4, e->stream));
     CCU(cudaMemsetAsync(e->d_vis_off, 0, (S + 1) * 8, e->stream));
     CCU(cudaStreamSynchronize(e->stream));
 #undef CCU
@@ -370,6 +400,7 @@ chd_status chd_set_stream(chd_engine* e, void* cuda_stream) {
 chd_status chd_sync(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     CU(e, cudaStreamSynchronize(e->stream));
     return CHD_OK;
 }
@@ -389,6 +420,7 @@ uint64_t chd_graph_launch_count(const chd_engine* e) { return e ? e->graph_launc
 chd_status chd_profile_enable(chd_engine* e, int on) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     if (on && !e->ev) {
         const size_t n = (size_t)CHD_STAGE_COUNT * chd_engine::EV_RING * 2;
         e->ev = new cudaEvent_t[n]();
@@ -403,6 +435,7 @@ chd_status chd_profile_enable(chd_engine* e, int on) {
 chd_status chd_profile_timeline(chd_engine* e, int stage, double* start_ms, double* stop_ms) {
     if (!e || stage < 0 || stage >= CHD_STAGE_COUNT || !start_ms || !stop_ms || !e->ev) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     CU(e, cudaStreamSynchronize(e->stream));
     CU(e, cudaStreamSynchronize(e->aux_stream));
     if (!e->stage_n[CHD_STAGE_TICK] || !e->stage_n[stage]) return CHD_ERR_STATE;
@@ -418,6 +451,7 @@ chd_status chd_profile_timeline(chd_engine* e, int stage, double* start_ms, doub
 chd_status chd_profile_get(chd_engine* e, int stage, double* total_ms, uint64_t* samples) {
     if (!e || stage < 0 || stage >= CHD_STAGE_COUNT || !total_ms || !samples) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     CU(e, cudaStreamSynchronize(e->stream));
     const uint64_t n = e->stage_n[stage];
     const uint64_t m = n < (uint64_t)chd_engine::EV_RING ? n : (uint64_t)chd_engine::EV_RING;

@@ -57,6 +57,18 @@ struct CellSort {
     uint32_t *tmp_key = nullptr, *tmp_val = nullptr;
 };
 
+// Everything the visible-list copy kernels read besides the pairs: the cell CSR of a build and the emit preparation's outputs.
+// Two sets, so that the next tick's build and preparation write one while the copy kernel of this tick still reads the other.
+struct CopySet {
+    uint32_t *sorted_ent = nullptr, *sorted_id = nullptr;  // sorted_id: entity-table mode only (chd_entity_table_init)
+    uint32_t* cell_start = nullptr;                        // [C+2]
+    uint64_t* voff = nullptr;
+    uint32_t* first_pair = nullptr;
+    TileDesc* tile_desc = nullptr;
+    uint32_t *general_tiles = nullptr, *n_general = nullptr;
+    unsigned long long* n_visible = nullptr;  // V of this set's preparation (the summary keeps its own copy in Counters)
+};
+
 struct chd_engine {
     chd_grid_cfg cfg;
     chd_limits lim;
@@ -133,6 +145,16 @@ struct chd_engine {
     CellSort ent_sort;
     uint32_t *d_sorted_key = nullptr, *d_sorted_ent = nullptr;
     uint32_t *d_cell_start = nullptr;     // [C+2]
+    // d_sorted_ent, d_cell_start, tbl.d_sorted_id, d_voff, d_first_pair, d_tile_desc, d_general_tiles and d_n_general point into
+    // copy_set[pf_copy.cur] (chd_copy_set_select).  Each build takes the set the last copy kernel did not read (chd_pf_begin orders
+    // the build after the last copy that read it); chd_pf_note_read records each copy kernel's read.
+    CopySet copy_set[2];
+    Prefetch pf_copy;
+    // Two-stream ticks: the build runs on build_stream (highest priority), the copy kernel on copy_stream (lowest priority), so
+    // that the next tick's head runs beside it.  copy_pending: the set read by a copy kernel on copy_stream that the engine stream
+    // is not ordered after yet (-1: none; chd_copy_wait).
+    cudaStream_t build_stream = nullptr, copy_stream = nullptr;
+    int copy_pending = -1;
     // one look-back scan site per call site: stages run concurrently on two streams and must not share scan state
     unsigned long long* d_epoch = nullptr;  // [EP_COUNT] stage epochs for the look-back scans
     ScanSite site_qoff{}, site_slot{}, site_voff{}, site_border{};
@@ -266,6 +288,11 @@ struct chd_engine {
     // arrays (zero-copy), an adopted prefetch set or the device-owned rings.  Set by chd_create, chd_set_rings, chd_rings_init
     // and chd_adopt_prefetched.
     RingDev ring{};
+    // the entry count of host-owned rings (chd_set_rings, an adopted prefetch), written to d_ring_total by the next pass that reads
+    // the rings, on that pass's stream (chd_ring_total_flush): a kernel on the engine stream between ticks would queue behind the
+    // copy kernel's grid, and the next tick's head would wait for it
+    uint32_t ring_total = 0;
+    bool ring_total_pending = false;
 
     uint32_t* d_by_cell = nullptr;  // pairs grouped by cell
     CellSort pair_sort;             // its sort: one block per tile of max_pairs, at most 4096; P-sized temporaries
@@ -443,12 +470,13 @@ static bool dalloc(chd_engine* e, T** p, uint64_t count) {
     return true;
 }
 
-// Every secondary stream: non-blocking and at the device's highest priority, so that its short kernels and copies do not queue
-// behind the emit kernel's grid.  chd_destroy releases it.
-static inline bool chd_make_stream(chd_engine* e, cudaStream_t* s) {
+// Every secondary stream: non-blocking, at the device's highest priority so that its short kernels and copies do not queue
+// behind the emit kernel's grid, or at the lowest (`lowest`: the copy stream, whose grid yields to the next tick's head).
+// chd_destroy releases it.
+static inline bool chd_make_stream(chd_engine* e, cudaStream_t* s, bool lowest = false) {
     int lo = 0, hi = 0;
     cudaError_t r = cudaDeviceGetStreamPriorityRange(&lo, &hi);
-    if (r == cudaSuccess) r = cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, hi);
+    if (r == cudaSuccess) r = cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, lowest ? lo : hi);
     if (r != cudaSuccess) return e->fail("cudaStreamCreateWithPriority failed: %s", cudaGetErrorString(r));
     e->streams.push_back(*s);
     return true;
@@ -486,15 +514,21 @@ bool chd_is_device_ptr(const chd_engine* e, const void* p);
 void chd_dfree(chd_engine* e, void* p);
 // The prefetch protocol (struct Prefetch).  begin: creates up_stream and the events on first use, orders up_stream after the
 // last recorded read of the set the prefetch fills and returns that set; the caller then enqueues the upload on up_stream.
-// end: records the upload and stages the set (a second prefetch before an adoption refills it).  adopt: makes the staged set
+// end: records the upload and stages the set (a second prefetch before an adoption refills it).  Both take the writer's stream
+// instead of up_stream when one is given (the copy-input sets: the build writes them).  adopt: makes the staged set
 // the one read (false: nothing staged).  wait: orders reader stream `s` after the upload, once per adoption.  note_read:
 // records a read of `set` (-1: none) on `s`, outside any graph capture, so that no prefetch overwrites it before that read.
-chd_status chd_pf_begin(chd_engine* e, Prefetch& p, int* set);
-chd_status chd_pf_end(chd_engine* e, Prefetch& p);
+chd_status chd_pf_begin(chd_engine* e, Prefetch& p, int* set, cudaStream_t s = nullptr);
+chd_status chd_pf_end(chd_engine* e, Prefetch& p, cudaStream_t s = nullptr);
 bool chd_pf_adopt(Prefetch& p);
 chd_status chd_pf_wait(chd_engine* e, Prefetch& p, cudaStream_t s);
 chd_status chd_pf_note_read(chd_engine* e, Prefetch& p, int set, cudaStream_t s);
 chd_status chd_read_u32(chd_engine* e, const uint32_t* d, uint32_t* v);
+// Orders the engine stream after the copy kernel a two-stream chd_tick left running on copy_stream (device-side, no host sync).
+// Every entry point that reads the expanded list, hands out device memory or is a documented completion point calls it first.
+cudaError_t chd_copy_wait(chd_engine* e);
+// Points the engine's copy-input pointers at copy_set[set].
+void chd_copy_set_select(chd_engine* e, int set);
 chd_status chd_decode_summary(chd_engine* e, chd_tick_summary* out);
 chd_status chd_assign_cells_impl(chd_engine* e, cudaStream_t s);
 // Host half of a cell assignment: the key buffers swap (handover detection compares against the keys of the previous
@@ -521,6 +555,7 @@ chd_status chd_upload_queries(chd_engine* e, cudaStream_t s, const chd_query_bat
                               chd_engine::QStage* stage = nullptr, uint32_t* spots = nullptr);
 // what the fan-out / payload kernels read: the host-owned CSR snapshot (staged or zero-copy) or the device-owned rings
 RingDev chd_ring_view(const chd_engine* e);
+chd_status chd_ring_total_flush(chd_engine* e, cudaStream_t s);
 // The stable sort by cell on `s` (chd_entities.cu): values val (nullptr: the index) of keys key[0, n) in [0, keys) (n_ptr: the
 // live length on the device) into val_out, in <= 2 passes of <= 10-bit digits.  key_out: where a two-pass sort writes the sorted
 // keys.  csr: the cell CSR to publish (nullptr: none).  bump: the epoch the first kernel opens.  assign: pass 0's histogram also

@@ -344,20 +344,27 @@ static chd_status build_enqueue(chd_engine* e, cudaStream_t s, bool with_assign,
 chd_status chd_build(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     chd_status st = chd_fetch_guard(e, e->stream);
     return st != CHD_OK ? st : chd_build_on(e, e->stream);
 }
 
 chd_status chd_build_on(chd_engine* e, cudaStream_t s) {
     StageTimer timer(e, s, CHD_STAGE_BUILD);
-    chd_status st = chd_epoch_tick(e, s, EP_BUILD);
+    // The cell CSR goes to the copy-input set the last copy kernel did not read, once every copy kernel that read it has finished.
+    // X-slabs keep one set: chd_tick_sharded joins its copy kernel inside the tick, so nothing of the next tick runs beside it.
+    int set = e->pf_copy.cur;
+    chd_status st = e->slab ? CHD_OK : chd_pf_begin(e, e->pf_copy, &set, s);
+    if (st != CHD_OK) return st;
+    chd_copy_set_select(e, set);
+    st = chd_epoch_tick(e, s, EP_BUILD);
     if (st != CHD_OK) return st;
     bool counts_recorded = false;
     if (!e->assigned && !e->halo_on_device) {
         // single-GPU flow: assign + sort as one replayable graph.  The key buffers swap every assignment (handover detection
         // compares against the previous keys); the graph bakes in the sizes, the buffer the new keys go to and the positions.
         const uint64_t key = stage_key(0x6275696c64ull, e->n_own, e->have_gid, e->have_prev_key, e->have_prev_key ? e->d_prev_key : e->d_key,
-                                       e->pos_x, e->pos_z);
+                                       e->pos_x, e->pos_z, set);
         // single-pass builds (<= 1023 cells) run as two replayable halves with an event in between: the cell CSR offsets are
         // final after the first (assignment + histogram + scan), so the emit preparation overlaps the scatter
         const bool split = e->g.cells + 1 <= BUILD_MAX_BINS && e->n_own > 0;
@@ -372,7 +379,7 @@ chd_status chd_build_on(chd_engine* e, cudaStream_t s) {
     } else if (e->assigned && e->halo_on_device) {
         // multi-GPU flow: cells were assigned by chd_export_border and the halo appended on the device; the sort over
         // own + halo entities is sized by capacity (device-side length) and therefore replayable as well.
-        const uint64_t key = stage_key(0x736f7274ull, e->lim.max_entities, e->have_gid, e->d_key);
+        const uint64_t key = stage_key(0x736f7274ull, e->lim.max_entities, e->have_gid, e->d_key, set);
         st = run_stage(e, s, e->g_build, key, [&]() { return build_enqueue(e, s, false); });
     } else {
         const bool with_assign = !e->assigned;
@@ -383,6 +390,11 @@ chd_status chd_build_on(chd_engine* e, cudaStream_t s) {
     st = chd_table_after_build(e, s);  // (entity-table mode only)
     if (st != CHD_OK) return st;
     if (!counts_recorded) CU(e, cudaEventRecord(e->ev_counts, s));  // (cell counts final = build done)
+    if (!e->slab) {
+        st = chd_pf_end(e, e->pf_copy, s);
+        if (st != CHD_OK) return st;
+        chd_pf_adopt(e->pf_copy);
+    }
     e->n_sorted = e->n_own + e->n_halo;
     e->sorted_dev_n = e->halo_on_device;
     e->built = true;

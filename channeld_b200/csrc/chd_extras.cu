@@ -13,6 +13,7 @@ chd_status chd_due_classes(chd_engine* e, uint32_t* out_class_of, uint32_t* out_
                            uint32_t* out_n_classes) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     cudaStream_t s = e->stream;
     uint32_t n_due = 0;
     chd_status st = chd_read_u32(e, &e->d_ctr->n_due, &n_due);
@@ -97,6 +98,7 @@ chd_status chd_adjacent_broadcast(chd_engine* e, const chd_broadcast_batch* b, u
         return CHD_ERR_STATE;
     }
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     const uint32_t n = b->n;
     if (out_status)
         for (uint32_t m = 0; m < n; m++)

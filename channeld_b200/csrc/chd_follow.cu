@@ -324,6 +324,7 @@ chd_status chd_get_follow(chd_engine* e, uint32_t* slot, uint32_t* entity, uint3
     if (!F.on || !F.n_bound) return CHD_OK;
     std::lock_guard<std::recursive_mutex> lk(e->mu);
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     cudaStream_t s = e->stream;
     const uint64_t Q = e->lim.max_queries;
     if (!F.g_count && !(dalloc(e, &F.g_slot, Q) && dalloc(e, &F.g_entity, Q) && dalloc(e, &F.g_status, Q) && dalloc(e, &F.g_cx, Q) && dalloc(e, &F.g_cz, Q) &&

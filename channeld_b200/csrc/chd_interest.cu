@@ -29,6 +29,7 @@ chd_status chd_set_subscribers(chd_engine* e, const uint32_t* conn_id, uint32_t 
         return CHD_ERR_CAPACITY;
     }
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     CU(e, cudaMemcpyAsync(e->d_conn, conn_id, sizeof(uint32_t) * n, cudaMemcpyDefault, e->stream));
     CU(e, cudaMemsetAsync(e->pairs[0].off, 0, ((uint64_t)e->lim.max_subscribers + 1) * 4, e->stream));
     CU(e, cudaMemsetAsync(e->pairs[1].off, 0, ((uint64_t)e->lim.max_subscribers + 1) * 4, e->stream));
@@ -63,6 +64,7 @@ static chd_status upload_slot_list(chd_engine* e, const uint32_t* slot, const ui
 
 chd_status chd_grow_slots(chd_engine* e, uint32_t new_n) {
     if (new_n <= e->n_slots) return CHD_OK;
+    CU(e, chd_copy_wait(e));  // the copy kernel reads the pair offsets
     const uint32_t old_n = e->n_slots;
     extend_offsets_kernel<<<blocks_for(new_n - old_n, 256), 256, 0, e->stream>>>(e->pairs[e->cur].off, old_n, new_n);
     KCHECK(e);
@@ -284,6 +286,7 @@ static chd_status interest_enqueue(chd_engine* e, cudaStream_t s, const QueryDev
 chd_status chd_update_interest(chd_engine* e, const chd_query_batch* q, int64_t now_ns) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     chd_status st = chd_fetch_guard(e, e->stream);
     return st != CHD_OK ? st : chd_update_interest_on(e, e->stream, q, now_ns);
 }

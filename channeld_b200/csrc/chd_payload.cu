@@ -29,6 +29,7 @@ chd_status chd_set_payload_bytes(chd_engine* e, const uint64_t* entry_off, uint3
     if (!e || !entry_off || !full_off || !type_url) return CHD_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lk(e->mu);
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     cudaStream_t s = e->stream;
     chd_engine::Payload& P = e->pl;
     const uint64_t C = e->g.cells;
@@ -59,6 +60,7 @@ chd_status chd_assemble_payloads(chd_engine* e, uint32_t* out_n_classes, uint64_
     if (!e) return CHD_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lk(e->mu);
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     chd_engine::Payload& P = e->pl;
     if (!P.have_input) {
         e->fail("chd_assemble_payloads before chd_set_payload_bytes");
@@ -86,6 +88,8 @@ chd_status chd_assemble_payloads(chd_engine* e, uint32_t* out_n_classes, uint64_
         e->fail("chd_assemble_payloads needs host-owned rings (chd_set_rings): payload bytes are indexed by ring position");
         return CHD_ERR_STATE;
     }
+    st = chd_ring_total_flush(e, s);
+    if (st != CHD_OK) return st;
     const RingDev ring = chd_ring_view(e);
     const PayloadIn in{(const unsigned long long*)P.d_entry_off, P.d_entry_bytes, (const unsigned long long*)P.d_full_off, P.d_full_bytes, P.d_url, P.url_len,
                        P.msg_type};
@@ -129,6 +133,7 @@ chd_status chd_frame_packets(chd_engine* e, const uint8_t* compression, uint64_t
     if (!e) return CHD_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lk(e->mu);
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     chd_engine::Payload& P = e->pl;
     if (!P.assembled) {
         e->fail("chd_frame_packets before chd_assemble_payloads");

@@ -139,6 +139,7 @@ extern "C" {
 chd_status chd_get_cells(chd_engine* e, uint32_t* cell_start, uint32_t* sorted_entity) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     const uint32_t C = e->g.cells;
     if (cell_start) CU(e, cudaMemcpyAsync(cell_start, e->d_cell_start, sizeof(uint32_t) * ((uint64_t)C + 1), cudaMemcpyDefault, e->stream));
     if (sorted_entity) {
@@ -155,6 +156,7 @@ chd_status chd_get_pairs(chd_engine* e, uint32_t* pair_off, uint32_t* channel_id
                          int64_t* last_fanout_ns, uint64_t* last_message_index) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     PairBuf& pb = e->pairs[e->cur];
     const uint32_t S = e->n_slots;
     uint32_t P = 0;
@@ -180,6 +182,7 @@ chd_status chd_get_pairs(chd_engine* e, uint32_t* pair_off, uint32_t* channel_id
 chd_status chd_get_query_status(chd_engine* e, uint32_t* status, uint32_t n) {
     if (!e || !status) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     if (n > e->last_nq) n = e->last_nq;
     CU(e, cudaMemcpyAsync(status, e->d_status, sizeof(uint32_t) * n, cudaMemcpyDefault, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
@@ -189,6 +192,7 @@ chd_status chd_get_query_status(chd_engine* e, uint32_t* status, uint32_t n) {
 chd_status chd_get_diff(chd_engine* e, uint32_t* new_sub, uint32_t* new_channel, uint32_t* unsub_sub, uint32_t* unsub_channel) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     CU(e, cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
     const uint32_t nn = e->h_ctr->n_sub_new, nu = e->h_ctr->n_unsub;
@@ -204,6 +208,7 @@ chd_status chd_get_diff(chd_engine* e, uint32_t* new_sub, uint32_t* new_channel,
 chd_status chd_get_visible(chd_engine* e, uint64_t* vis_off, uint32_t* vis_entity) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     const uint32_t S = e->n_slots;
     cudaStream_t s = e->stream;
     if (vis_off) CU(e, cudaMemcpyAsync(vis_off, e->d_vis_off, sizeof(uint64_t) * ((uint64_t)S + 1), cudaMemcpyDefault, s));
@@ -222,6 +227,7 @@ chd_status chd_get_visible(chd_engine* e, uint64_t* vis_off, uint32_t* vis_entit
 chd_status chd_get_visible_slot(chd_engine* e, uint32_t slot, uint32_t* out, uint64_t cap, uint64_t* count) {
     if (!e || !count || slot >= e->n_slots) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     uint64_t* h64 = (uint64_t*)e->h_get;
     CU(e, cudaMemcpyAsync(h64, e->d_vis_off + slot, 16, cudaMemcpyDeviceToHost, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
@@ -239,6 +245,7 @@ chd_status chd_get_visible_slot(chd_engine* e, uint32_t slot, uint32_t* out, uin
 chd_status chd_get_due(chd_engine* e, chd_due* out, uint32_t cap) {
     if (!e || !out) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     CU(e, cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
     uint32_t n = e->h_ctr->n_due;
@@ -252,6 +259,7 @@ chd_status chd_get_due(chd_engine* e, chd_due* out, uint32_t cap) {
 chd_status chd_get_handover(chd_engine* e, uint32_t* entity, uint32_t* src_channel, uint32_t* dst_channel, uint32_t cap) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     uint32_t n = 0;
     chd_status st = chd_read_u32(e, &e->d_ctr->n_handover, &n);
     if (st != CHD_OK) return st;
@@ -276,6 +284,9 @@ chd_status chd_fetch_results_delta(chd_engine* e, const chd_result_buffers* b, c
         e->fail("chd_fetch_results_delta: delta buffers before chd_reserve_visible_delta");
         return CHD_ERR_STATE;
     }
+    CU(e, cudaSetDevice(e->device));
+    // only a fetch of the expanded list waits for the copy kernel: the other results are final once the tick's head has run
+    if (b->vis_entity) CU(e, chd_copy_wait(e));
     chd_status st;
     cudaStream_t s = e->stream;
     cudaStream_t main_stream = e->stream;
@@ -632,6 +643,8 @@ chd_status chd_fetch_wait_delta(chd_engine* e, chd_tick_summary* summary, chd_de
 
 chd_status chd_device_view(chd_engine* e, int which, void** d_ptr, uint64_t* count) {
     if (!e || !d_ptr) return CHD_ERR_INVALID;
+    CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));  // work the caller orders after this on the engine stream sees the final arrays
     PairBuf& pb = e->pairs[e->cur];
     uint64_t c = 0;
     void* p = nullptr;

@@ -337,6 +337,8 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
         e->fail("chd_tick_sharded before chd_comm_init");
         return CHD_ERR_STATE;
     }
+    CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     {
         chd_status gs_ = chd_fetch_guard(e, e->stream);
         if (gs_ != CHD_OK) return gs_;
@@ -382,7 +384,9 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
         }
     }
     if (st != CHD_OK) return st;
-    return chd_tick(e, nullptr, t_ns, flags, out);
+    st = chd_tick(e, nullptr, t_ns, flags, out);
+    CU(e, chd_copy_wait(e));  // slabs keep the copy kernel inside their tick: the exchange adds dependencies of its own
+    return st;
 }
 
 /* ---- subscriber migration between ranks (state travels in the tick's all-gather) */
@@ -453,6 +457,7 @@ chd_status chd_migrate_in(chd_engine* e, uint32_t src_rank, uint32_t first_index
 chd_status chd_get_rehome(chd_engine* e, uint32_t* global_id, uint32_t* dst_rank, uint32_t cap, uint32_t* count) {
     if (!e || !count) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     if (!e->assigned) {
         e->fail("chd_get_rehome before the tick's cell assignment");
         return CHD_ERR_STATE;

@@ -341,11 +341,13 @@ chd_status chd_entity_table_init(chd_engine* e) {
     uint32_t bits = 4;
     while ((1ull << bits) < 2 * N) bits++;
     const bool ok = dalloc(e, &t.d_table, 1ull << bits) && dalloc(e, &t.d_id_of_slot, N) && dalloc(e, &t.d_snap_id, N) &&
-                    dalloc(e, &t.d_sorted_id, ((N + 3) / 4) * 4 + 8) &&  // the padding and alignment of d_sorted_ent (the emit kernels read it)
+                    // the padding and alignment of d_sorted_ent (the emit kernels read it), one per copy-input set
+                    dalloc(e, &e->copy_set[0].sorted_id, ((N + 3) / 4) * 4 + 8) && dalloc(e, &e->copy_set[1].sorted_id, ((N + 3) / 4) * 4 + 8) &&
                     dalloc(e, &t.d_winner, N) && dalloc(e, &t.d_mslot, N) && dalloc(e, &t.d_ho_tmp, 3 * N) && dalloc(e, &t.d_build_seq, 2) &&
                     dalloc(e, &t.d_flag, N) && dalloc(e, &t.d_stats, 3) && dalloc(e, &t.d_ev, 2 * N) && dalloc(e, &t.d_ev_pos, 2 * N) &&
                     chd_make_event(e, &t.ev_stage[0]) && chd_make_event(e, &t.ev_stage[1]);
     if (!ok) return CHD_ERR_CUDA;
+    t.d_sorted_id = e->copy_set[e->pf_copy.cur].sorted_id;
     cudaStream_t s = e->stream;
     CU(e, cudaMemsetAsync(t.d_table, 0, 8ull << bits, s));
     CU(e, cudaMemsetAsync(t.d_id_of_slot, 0, 4 * N, s));
@@ -435,6 +437,7 @@ chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out) {
     if (!e || !out) return CHD_ERR_INVALID;
     if (chd_rule_table(e, "chd_get_entity_stats") != CHD_OK) return CHD_ERR_STATE;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     const chd_engine::Table& t = e->tbl;
     uint64_t* h64 = reinterpret_cast<uint64_t*>(e->h_get);
     CU(e, cudaMemcpyAsync(h64, t.d_stats, 24, cudaMemcpyDeviceToHost, e->stream));

@@ -28,7 +28,11 @@ static chd_status emit_prep_enqueue(chd_engine* e, cudaStream_t s, bool cta_tile
     const uint64_t P = e->lim.max_pairs;
     const unsigned grid = (unsigned)e->sm_count * 8;
     const uint32_t tile = cta_tiles ? (uint32_t)EMIT_TILE : (uint32_t)EMIT_WARP_TILE;
-    const uint64_t key = stage_key(0x656d6974ull, S, e->cur, cta_tiles, s);
+    const int set = e->pf_copy.cur;
+    const uint64_t key = stage_key(0x656d6974ull, S, e->cur, cta_tiles, s, set);
+    // the preparation rewrites its copy-input set: after the last copy kernel that read it (a tick without a build reuses the set
+    // of the copy before it; after a build this is the copy the build already waited for)
+    if (e->pf_copy.read_recorded[set]) CU(e, cudaStreamWaitEvent(s, e->pf_copy.ev_read[set], 0));
     chd_status st = chd_epoch_tick(e, s, EP_EMIT);
     if (st != CHD_OK) return st;
     return run_stage(e, s, e->g_emit_prep, key, [&]() -> chd_status {
@@ -36,16 +40,22 @@ static chd_status emit_prep_enqueue(chd_engine* e, cudaStream_t s, bool cta_tile
         SCAN(e, exclusive_scan_fn<PairVcountIn, uint64_t>(PairVcountIn{pb.cell, e->d_cell_start}, e->d_voff, P, e->site_voff, s, pb.off + S));
         emit_partition_kernel<<<grid, 256, 0, s>>>(pb.off + S, P, e->d_voff, pb.cell, e->d_cell_start, e->d_first_pair, cta_tiles ? e->d_tile_desc : nullptr,
                                                    e->max_tiles, S, pb.off, e->d_vis_off, e->lim.max_visible, e->d_ctr, e->d_epoch + EP_EMIT, tile,
-                                                   e->d_general_tiles, e->d_n_general);
+                                                   e->d_general_tiles, e->d_n_general, e->copy_set[set].n_visible);
         KCHECK(e);
         return CHD_OK;
     });
 }
 
+// the copy kernels on `s`; they read V from their set, which the next tick's preparation does not rewrite while they run
 static chd_status emit_kernel_enqueue(chd_engine* e, cudaStream_t s, bool cta_tiles) {
     PairBuf& pb = e->pairs[e->cur];
     const uint32_t S = e->n_slots;
     const uint64_t P = e->lim.max_pairs;
+    const int set = e->pf_copy.cur;
+    const unsigned long long* V = e->copy_set[set].n_visible;
+    chd_status st = chd_pf_wait(e, e->pf_copy, s);
+    if (st != CHD_OK) return st;
+    {
     StageTimer kt(e, s, CHD_STAGE_EMIT_KERNEL);
     if (cta_tiles) {
         // EMIT_TILES_PER_CTA tiles per CTA, dispatched by the hardware block scheduler.  The tile count lives on the device; the grid is
@@ -56,9 +66,9 @@ static chd_status emit_kernel_enqueue(chd_engine* e, cudaStream_t s, bool cta_ti
         if (tiles == 0) tiles = 1;
         if (tiles > 0x7fffffffull) tiles = 0x7fffffffull;
         tiles = (tiles + EMIT_TILES_PER_CTA - 1) / EMIT_TILES_PER_CTA;
-        emit_visible_kernel<<<(unsigned)tiles, EMIT_THREADS, CHD_EMIT_DYN_SMEM, s>>>(&e->d_ctr->n_visible, chd_sorted_out(e), e->d_tile_desc, e->d_vis, e->lim.max_visible);
+        emit_visible_kernel<<<(unsigned)tiles, EMIT_THREADS, CHD_EMIT_DYN_SMEM, s>>>(V, chd_sorted_out(e), e->d_tile_desc, e->d_vis, e->lim.max_visible);
         KCHECK(e);
-        emit_visible_general_kernel<<<(unsigned)e->sm_count * 2, EMIT_THREADS, 0, s>>>(e->d_general_tiles, e->d_n_general, pb.off + S, P, &e->d_ctr->n_visible,
+        emit_visible_general_kernel<<<(unsigned)e->sm_count * 2, EMIT_THREADS, 0, s>>>(e->d_general_tiles, e->d_n_general, pb.off + S, P, V,
                                                                                        e->d_voff, pb.cell, e->d_cell_start, chd_sorted_out(e),
                                                                                        e->d_first_pair, e->d_vis, e->lim.max_visible);
     } else {
@@ -66,13 +76,18 @@ static chd_status emit_kernel_enqueue(chd_engine* e, cudaStream_t s, bool cta_ti
                                                                                     e->d_first_pair, e->d_vis, e->lim.max_visible);
     }
     KCHECK(e);
+    }
+    st = chd_pf_note_read(e, e->pf_copy, set, s);
+    if (st != CHD_OK) return st;
+    e->copy_pending = s == e->stream ? -1 : set;
     return CHD_OK;
 }
 
 // The emit: the preparation (ending with ev_prep_done), then the copy kernel on `s`, after `kernel_ev` if one is given.  Without
 // `pairs_ev` the preparation runs on `s` too.  In a two-stream tick it needs only the new pairs (`pairs_ev`, second stream) and
 // the cell CSR OFFSETS (ev_counts: recorded between the two halves of a single-pass build), not the sorted entity array — it runs
-// on prep_stream next to the build's scatter; the copy kernel follows on `s` when both are done.
+// on prep_stream next to the build's scatter; the copy kernel follows on `s` (copy_stream) when both and the build
+// (ev_build_done) are done.
 static chd_status emit_enqueue(chd_engine* e, cudaStream_t s, cudaEvent_t pairs_ev, cudaEvent_t kernel_ev) {
     if (!e->built) {
         e->fail("emit before any chd_build");
@@ -82,14 +97,16 @@ static chd_status emit_enqueue(chd_engine* e, cudaStream_t s, cudaEvent_t pairs_
     StageTimer timer(e, s, CHD_STAGE_EMIT);
     const cudaStream_t ps = pairs_ev ? e->prep_stream : s;
     if (pairs_ev) {
-        CU(e, cudaStreamWaitEvent(ps, e->ev_fork, 0));    // the previous tick's copy kernel (it reads what the preparation rewrites)
         CU(e, cudaStreamWaitEvent(ps, e->ev_counts, 0));
         CU(e, cudaStreamWaitEvent(ps, pairs_ev, 0));
     }
     chd_status st = emit_prep_enqueue(e, ps, cta_tiles);
     if (st != CHD_OK) return st;
     CU(e, cudaEventRecord(e->ev_prep_done, ps));  // visible offsets + counters are final; only the expanded list is still to come
-    if (pairs_ev) CU(e, cudaStreamWaitEvent(s, e->ev_prep_done, 0));
+    if (pairs_ev) {
+        CU(e, cudaStreamWaitEvent(s, e->ev_prep_done, 0));
+        CU(e, cudaStreamWaitEvent(s, e->ev_build_done, 0));
+    }
     if (kernel_ev) CU(e, cudaStreamWaitEvent(s, kernel_ev, 0));
     return emit_kernel_enqueue(e, s, cta_tiles);
 }
@@ -97,6 +114,7 @@ static chd_status emit_enqueue(chd_engine* e, cudaStream_t s, cudaEvent_t pairs_
 chd_status chd_emit_visible(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     chd_status st = chd_fetch_guard(e, e->stream);
     return st != CHD_OK ? st : emit_enqueue(e, e->stream, nullptr, nullptr);
 }
@@ -158,8 +176,8 @@ chd_status chd_set_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_ent
     e->pf_ring.cur = -1;
     e->pf_ring.wait = false;
     // the fan-out kernel clamps ring_off to this: a lying caller cannot cause out-of-bounds reads
-    set_u32_kernel<<<1, 1, 0, e->stream>>>(e->d_ring_total, total);
-    KCHECK(e);
+    e->ring_total = total;
+    e->ring_total_pending = true;
     return CHD_OK;
 }
 
@@ -182,6 +200,7 @@ chd_status chd_rings_init(chd_engine* e, uint32_t capacity_per_cell) {
     CU(e, cudaMemsetAsync(e->d_ch_msg_index, 0, (uint64_t)e->g.cells * 8, s));
     set_u32_kernel<<<1, 1, 0, s>>>(e->d_ring_total, (uint32_t)need);
     KCHECK(e);
+    e->ring_total_pending = false;
     e->rings_owned = true;
     e->ring_cap = capacity_per_cell;
     e->ring = RingDev{e->d_rb_begin, e->d_rb_end, e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, e->d_ch_msg_index, e->d_ring_total, nullptr};
@@ -223,6 +242,7 @@ chd_status chd_get_rings(chd_engine* e, uint32_t* ring_off, int64_t* arrival_ns,
         return CHD_ERR_STATE;
     }
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     cudaStream_t s = e->stream;
     const uint32_t C = e->g.cells;
     // (control-plane call: a plain two-pass scan through scratch that is free between ticks)
@@ -273,6 +293,14 @@ chd_status chd_set_channel_start_times(chd_engine* e, const int64_t* start_ns) {
     return CHD_OK;
 }
 
+chd_status chd_ring_total_flush(chd_engine* e, cudaStream_t s) {
+    if (!e->ring_total_pending) return CHD_OK;
+    set_u32_kernel<<<1, 1, 0, s>>>(e->d_ring_total, e->ring_total);
+    KCHECK(e);
+    e->ring_total_pending = false;
+    return CHD_OK;
+}
+
 RingDev chd_ring_view(const chd_engine* e) {
     RingDev ring = e->ring;
     ring.start = e->have_cell_start ? e->d_cell_start_ns : nullptr;
@@ -285,6 +313,7 @@ static chd_status fanout_enqueue(chd_engine* e, cudaStream_t s, int64_t t_ns) {
     const uint64_t P = e->lim.max_pairs;
     StageTimer timer(e, s, CHD_STAGE_FANOUT);
     chd_status st = chd_pf_wait(e, e->pf_ring, s);  // rings handed over by chd_adopt_prefetched: ordered after their upload
+    if (st == CHD_OK) st = chd_ring_total_flush(e, s);
     if (st != CHD_OK) return st;
     chd_epoch_tick(e, s, EP_FANOUT);
     stage_begin_kernel<<<1, 1, 0, s>>>(e->d_time + 1, t_ns, e->d_epoch + EP_FANOUT, &e->d_ctr->n_due, 1, nullptr);
@@ -307,6 +336,7 @@ static chd_status fanout_enqueue(chd_engine* e, cudaStream_t s, int64_t t_ns) {
 chd_status chd_fanout_tick(chd_engine* e, int64_t t_ns) {
     if (!e) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     chd_status st = chd_fetch_guard(e, e->stream);
     return st != CHD_OK ? st : fanout_enqueue(e, e->stream, t_ns);
 }
@@ -343,8 +373,8 @@ chd_status chd_adopt_prefetched(chd_engine* e) {
     if (chd_pf_adopt(e->pf_ring)) {
         const chd_engine::RStage& r = e->ring_pf[e->pf_ring.cur];
         e->ring = staged_ring(e, r);
-        set_u32_kernel<<<1, 1, 0, e->stream>>>(e->d_ring_total, r.total);
-        KCHECK(e);
+        e->ring_total = r.total;
+        e->ring_total_pending = true;
     }
     if (!chd_pf_adopt(e->pf_pos)) return CHD_OK;
     chd_status st = chd_pf_wait(e, e->pf_pos, e->stream);
@@ -360,6 +390,7 @@ chd_status chd_adopt_prefetched(chd_engine* e) {
 chd_status chd_summary(chd_engine* e, chd_tick_summary* out) {
     if (!e || !out) return CHD_ERR_INVALID;
     CU(e, cudaSetDevice(e->device));
+    CU(e, chd_copy_wait(e));
     CU(e, cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
     return chd_decode_summary(e, out);
@@ -432,11 +463,13 @@ chd_status chd_fetch_guard(chd_engine* e, cudaStream_t s) {
     return CHD_OK;
 }
 
-// Dependency graph of a tick:   build ----------------+--> emit
-//                               interest --> fan-out  |      (emit needs the cell CSR and the new pairs)
-// The build / emit chain (HBM-bound) runs on the main stream `s`, the interest / fan-out chain (latency-bound, disjoint state)
-// on aux_stream, started here or earlier by chd_begin_interest; the streams are joined before the summary.  A tick with nothing
-// to overlap runs its stages one after the other on `s`.
+// Dependency graph of a tick:   build ----------------+--> emit preparation --> copy kernel
+//                               interest --> fan-out  |      (the emit needs the cell CSR and the new pairs)
+// The build runs on build_stream, the interest / fan-out chain on aux_stream (started here or earlier by chd_begin_interest),
+// the emit preparation on prep_stream: the tick's head, all forked from the engine stream `s` (= e->stream) at high priority.
+// The copy kernel (HBM-bound) runs on copy_stream at the lowest priority.  `s` joins everything but the copy kernel, and the
+// previous tick's copy kernel: the next tick's head runs beside this tick's copy, and `s` is never more than one copy behind
+// (chd_copy_wait joins the rest).  A tick with nothing to overlap runs its stages one after the other on `s`.
 static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_batch* q, int64_t t_ns, uint32_t flags) {
     CU(e, cudaSetDevice(e->device));
     chd_status st = chd_fetch_guard(e, s);
@@ -462,6 +495,7 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
     }
     if (do_delta && chd_delta_check(e, need_build) != CHD_OK) return CHD_ERR_STATE;
     if (!started && !((interest || do_fanout) && (need_build || do_emit))) {
+        CU(e, chd_copy_wait(e));
         if (need_build) {
             st = chd_build_on(e, s);
             if (st != CHD_OK) return st;
@@ -486,18 +520,25 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
     }
     const bool fanout_done = started ? e->pending_fanout : do_fanout;
     e->interest_pending = false;
+    // the build forks off `s` onto build_stream: left on `s`, it would queue behind the previous copy kernel's grid
+    const cudaStream_t bs = e->build_stream;
+    CU(e, cudaEventRecord(e->ev_fork, s));
+    CU(e, cudaStreamWaitEvent(bs, e->ev_fork, 0));
+    CU(e, chd_copy_wait(e));  // `s` (not the head, forked above) waits for the previous tick's copy kernel
     if (need_build) {
-        st = chd_build_on(e, s);
+        st = chd_build_on(e, bs);
         if (st != CHD_OK) return st;
-        CU(e, cudaEventRecord(e->ev_build_done, s));
         e->build_done_recorded = true;
     }
-    if (do_delta) CU(e, cudaEventRecord(e->dl.ev_in, s));  // the cell CSR and keys of this tick (or of the last build) are final
+    CU(e, cudaEventRecord(e->ev_build_done, bs));
+    if (do_delta) CU(e, cudaEventRecord(e->dl.ev_in, bs));  // the cell CSR and keys of this tick (or of the last build) are final
     if (do_emit) {
         // the preparation waits for the new pairs (for the fork when this tick updates no interest); CHD_TICK_EARLY_RESULTS: the
         // copy kernel starts after the whole aux chain, so every host-facing result is final while it is still streaming
-        st = emit_enqueue(e, s, (started || interest) ? e->ev_pairs : e->ev_interest, (flags & CHD_TICK_EARLY_RESULTS) ? e->ev_join : nullptr);
+        st = emit_enqueue(e, e->copy_stream, (started || interest) ? e->ev_pairs : e->ev_interest,
+                          (flags & CHD_TICK_EARLY_RESULTS) ? e->ev_join : nullptr);
         if (st != CHD_OK) return st;
+        CU(e, cudaStreamWaitEvent(s, e->ev_prep_done, 0));
     }
     if (do_delta) {
         // latency-bound: on prep_stream (after the emit preparation), next to the expanded-list kernel and the aux chain; it needs
@@ -511,6 +552,7 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
         e->dl.done_recorded = true;  // the early read-back's counters wait for it (CHD_OVF_DELTA belongs to this tick's summary)
         CU(e, cudaStreamWaitEvent(s, e->dl.ev_done, 0));
     }
+    CU(e, cudaStreamWaitEvent(s, e->ev_build_done, 0));
     CU(e, cudaStreamWaitEvent(s, e->ev_join, 0));
     if (do_fanout && !fanout_done) {
         st = fanout_enqueue(e, s, t_ns);
@@ -525,8 +567,10 @@ chd_status chd_tick(chd_engine* e, const chd_query_batch* q, int64_t t_ns, uint3
     if (!e) return CHD_ERR_INVALID;
     chd_status st;
     {
-        StageTimer whole(e, e->stream, CHD_STAGE_TICK);  // main-stream span of the tick (without the summary read-back)
+        // from the tick's first head kernel to the end of its copy kernel (without the summary read-back)
+        StageTimer whole(e, e->stream, CHD_STAGE_TICK);
         st = tick_enqueue(e, e->stream, q, t_ns, flags);
+        if (e->copy_pending >= 0) whole.s = e->copy_stream;
     }
     if (st != CHD_OK) return st;
     if (out) return chd_summary(e, out);

@@ -326,6 +326,14 @@ enum {
  * q == NULL (here and in chd_update_interest) = the batch uploaded by chd_prefetch_queries and handed over by
  * chd_adopt_prefetched, or the batch generated by chd_follow_queries; CHD_ERR_STATE if there is none. */
 chd_status chd_begin_interest(chd_engine* e, const chd_query_batch* q, int64_t t_ns, int with_fanout);
+/* Completion: after chd_tick returns, work the caller enqueues on the engine stream is ordered after every result of the tick
+ * except the expanded list (vis_entity): in a two-stream tick the expanded-list kernel keeps running on a low-priority stream of
+ * its own, next to the following tick's build, interest update and emit preparation.  The expanded list is final once any of
+ * these has been called: chd_summary (also through out != NULL), chd_sync, any chd_get_*, chd_device_view, chd_fetch_results
+ * with vis_entity != NULL, chd_build, chd_emit_visible, chd_update_interest, chd_fanout_tick, the payload, broadcast and
+ * window-class calls, chd_tick_sharded, chd_destroy — or once the next chd_tick has returned.  The tick-path inputs
+ * (chd_set_entities*, chd_set_rings, chd_prefetch_*, chd_adopt_prefetched, chd_begin_interest, chd_follow_queries*, the entity
+ * events), chd_tick itself and chd_fetch_results_async* / chd_fetch_wait* do not wait for it. */
 chd_status chd_tick(chd_engine* e, const chd_query_batch* q, int64_t t_ns, uint32_t flags, chd_tick_summary* out);
 
 /* ---- results.  Each copies to caller memory (host or device) on the engine stream and synchronises.
