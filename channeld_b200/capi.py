@@ -28,6 +28,7 @@ TICK_FOLLOW = 32  # the tick's batch is the one chd_follow_queries generated (ba
 FOLLOW_ALL, FOLLOW_MOVED = 0, 1
 FOLLOW_NOT_SELECTED, FOLLOW_NO_ENTITY = 16, 17  # beside Q_* in chd_get_follow's status
 FOLLOW_OVERRIDDEN = 18  # the slot's host entry in chd_follow_queries_with's batch replaced its generated query
+FOLLOW_OUTSIDE_SLAB = 19  # the generated query would reach columns the slab does not serve: no query this tick
 OVF_PAIRS, OVF_WINDOW, OVF_VISIBLE, OVF_DUE, OVF_BORDER, OVF_RING = 1, 2, 4, 8, 16, 32
 OVF_DELTA = 64
 OVF_DELTA_IDS = 128

@@ -240,6 +240,8 @@ class GpuStaticGrid2DSpatialController:
     # follow=...) builds the UPDATE_SPATIAL_INTEREST batch (message_spatial.go:41-129) on the device from the entities' positions.
     # queries[i] gives the AOI SHAPE of connection slot i (SphereAOI / BoxAOI / ConeAOI, any combination); its Center is ignored,
     # the centre is entity net_ids[i] (entity index without SpawnObjects).  SpotsAOI is absolute and cannot follow an entity.
+    # On a slab (entity-table mode only) a follower lives on its entity's owner (sharding.FollowerRegistry); a follower whose query
+    # would reach columns the slab does not serve reports capi.FOLLOW_OUTSIDE_SLAB.
     def FollowEntities(self, conn_slots, net_ids, queries: Sequence[SpatialInterestQuery]) -> None:
         n = len(queries)
         kind = np.zeros(n, np.uint8)

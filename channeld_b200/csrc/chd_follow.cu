@@ -88,19 +88,28 @@ chd_status follow_generate(chd_engine* e, uint32_t mode, const QueryDev& h, uint
     const uint32_t S = e->n_slots, B = F.n_bound, H = (uint32_t)host_class(n_h);
     const FollowEntities ent = e->tbl.on ? FollowEntities{e->d_x, e->d_z, e->lim.max_entities, e->tbl.d_table, e->tbl.bits, e->tbl.d_id_of_slot}
                                          : FollowEntities{e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z, e->n_own, nullptr, 0, nullptr};
+    // on a slab (entity-table mode: every followed entity is an own one) the columns it serves, with the world's edges left open
+    const uint32_t lo = e->slab && e->g.col_lo > e->g.halo ? e->g.col_lo - e->g.halo : 0u;
+    const uint32_t hi = e->slab ? (uint32_t)std::min<uint64_t>((uint64_t)e->g.col_hi + e->g.halo, e->g.cols) : e->g.cols;
+    const FollowSlab slab{e->g.off_x, e->g.w, (double)e->g.cols, lo > 0 ? (double)lo : -INFINITY, hi < e->g.cols ? (double)hi : INFINITY};
+    const bool check = lo > 0 || hi < e->g.cols;
     chd_status st = chd_epoch_tick(e, s, EP_FOLLOW);
     if (st != CHD_OK) return st;
     const FollowBatch& q = F.q;
     if (!merged) {
-        // the graph bakes in the slot and follower counts, the mode and where the positions live (the state arrays never move)
-        const uint64_t key = stage_key(0x666f6c6cull, S, B, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub);
+        // the graph bakes in the slot and follower counts, the mode, where the positions live (the state arrays never move) and the
+        // served columns
+        const uint64_t key = stage_key(0x666f6c6cull, S, B, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub, lo, hi);
         st = run_stage(e, s, F.g, key, [&]() -> chd_status {
             // the skip tail: entries behind the selected count name no slot and no kind
             CU(e, cudaMemsetAsync(q.sub, 0xFF, 4ull * B, s));
             CU(e, cudaMemsetAsync(q.kind, 0, B, s));
             bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_FOLLOW);
             KCHECK(e);
-            SCAN(e, compact_1p(FollowFlag<false>{F.st, ent, mode}, FollowSink<false>{F.st, q, 0}, S, F.site, s));
+            if (check)
+                SCAN(e, compact_1p(FollowFlag<false, true>{F.st, ent, slab, mode}, FollowSink<false>{F.st, q, 0}, S, F.site, s));
+            else
+                SCAN(e, compact_1p(FollowFlag<false, false>{F.st, ent, slab, mode}, FollowSink<false>{F.st, q, 0}, S, F.site, s));
             return CHD_OK;
         });
     } else {
@@ -114,7 +123,7 @@ chd_status follow_generate(chd_engine* e, uint32_t mode, const QueryDev& h, uint
         // ... and so do the host part's arrays (the staging set of the query scratch or a prefetch, or the caller's device arrays) and
         // the spot buffer's three arrays: a grown buffer may start where the old one did, but its spot_z and spot_dist move with the
         // capacity
-        const uint64_t key = stage_key(0x666f6c6dull, S, B, H, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub, grid, h.sub, h.kind,
+        const uint64_t key = stage_key(0x666f6c6dull, S, B, H, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub, lo, hi, grid, h.sub, h.kind,
                                        h.sph_cx, h.sph_cz, h.sph_r, h.box_cx, h.box_cz, h.box_ex, h.box_ez, h.cone_cx, h.cone_cz, h.cone_dx, h.cone_dz,
                                        h.cone_angle, h.cone_r, h.spot_off, h.spot_ndist, h.spot_x, h.spot_z, h.spot_dist, q.spot_x, q.spot_z,
                                        q.spot_dist, F.spot_cap);
@@ -123,7 +132,10 @@ chd_status follow_generate(chd_engine* e, uint32_t mode, const QueryDev& h, uint
             KCHECK(e);
             follow_merge_kernel<<<grid, FOLLOW_THREADS, 0, s>>>(m);
             KCHECK(e);
-            SCAN(e, compact_1p(FollowFlag<true>{F.st, ent, mode}, FollowSink<true>{F.st, q, H}, S, F.site, s));
+            if (check)
+                SCAN(e, compact_1p(FollowFlag<true, true>{F.st, ent, slab, mode}, FollowSink<true>{F.st, q, H}, S, F.site, s));
+            else
+                SCAN(e, compact_1p(FollowFlag<true, false>{F.st, ent, slab, mode}, FollowSink<true>{F.st, q, H}, S, F.site, s));
             return CHD_OK;
         });
     }

@@ -13,8 +13,8 @@
 namespace chd {
 
 constexpr int FOLLOW_THREADS = 256;
-// res[] of a slot that is bound but has no query in the generated batch: FOLLOW_NO_QUERY | CHD_FOLLOW_NOT_SELECTED / _NO_ENTITY
-// (a selected follower's res is its batch entry, below 2^31)
+// res[] of a slot that is bound but has no query in the generated batch: FOLLOW_NO_QUERY | CHD_FOLLOW_NOT_SELECTED / _NO_ENTITY /
+// _OVERRIDDEN / _OUTSIDE_SLAB (a selected follower's res is its batch entry, below 2^31)
 constexpr uint32_t FOLLOW_NO_QUERY = 0x80000000u;
 
 // Where a followed entity's position comes from: the arrays the build reads; in entity-table mode through the id table.
@@ -26,12 +26,36 @@ struct FollowEntities {
     const uint32_t* __restrict__ id_of_slot;
 };
 
+// The columns a slab serves: its queries may touch cells in columns [col_lo - halo, col_hi + halo) (chd_import_halo brings in no
+// other entity).  A follower's centre never reaches the host, so the device decides whether the generated query fits: the union
+// over the bound kinds of the column span floor((cx - reach - off_x) / w) .. floor((cx + reach - off_x) / w) (reach = sph_r, box_ex,
+// cone_r), in the rounded f64 steps of grid_coord, clipped to the world's columns [0, cols) because samples outside the world are
+// skipped.  A bounding box, not the samples: conservative.  lo / hi are -inf / +inf on a side where the served range reaches the
+// world's edge.  Only slabs whose served range is not the whole world run it (FollowFlag<_, true>).
+struct FollowSlab {
+    double off_x, w, fcols, lo, hi;
+    __device__ __forceinline__ bool outside(const FollowDev& f, uint64_t s, uint32_t kind, double cx) const {
+        double a = INFINITY, b = -INFINITY;
+        auto span = [&](double r) {
+            a = fmin(a, floor(f64div(f64sub(f64sub(cx, r), off_x), w)));
+            b = fmax(b, floor(f64div(f64sub(f64add(cx, r), off_x), w)));
+        };
+        if (kind & CHD_AOI_SPHERE) span(f.sph_r[s]);
+        if (kind & CHD_AOI_BOX) span(f.box_ex[s]);
+        if (kind & CHD_AOI_CONE) span(f.cone_r[s]);
+        // the clipped span is empty (entirely outside the world, or no finite reach): the query path reports that entry itself
+        return b >= 0.0 && a < fcols && a <= b && (a < lo || b >= hi);
+    }
+};
+
 // Merged: the batch has a host part (chd_follow_queries_with), whose entries marked their slots in f.ovr.  The flag reads and
-// clears the mark of every slot below the slot count, bound or not, so no mark outlives the generation.
-template <bool Merged>
+// clears the mark of every slot below the slot count, bound or not, so no mark outlives the generation.  Slab: the served-range
+// check runs (a separate instantiation: its f64 divisions would raise the register count of every engine's compaction).
+template <bool Merged, bool Slab>
 struct FollowFlag {
     FollowDev f;
     FollowEntities ent;
+    FollowSlab slab;
     uint32_t mode;
     __device__ __forceinline__ bool operator()(uint64_t s) const {
         if (Merged && f.ovr[s]) {  // the slot's explicit query wins this tick; the next MOVED generation selects it again
@@ -62,6 +86,11 @@ struct FollowFlag {
         const bool moved = __double_as_longlong(x) != __double_as_longlong(f.last_x[s]) || __double_as_longlong(z) != __double_as_longlong(f.last_z[s]);
         if (mode == (uint32_t)CHD_FOLLOW_MOVED && !f.dirty[s] && !moved) {
             f.res[s] = FOLLOW_NO_QUERY | (uint32_t)CHD_FOLLOW_NOT_SELECTED;
+            return false;
+        }
+        if (Slab && slab.outside(f, s, f.kind[s], x)) {  // no query; the centre stays the last generated one, and it counts as moved
+            f.res[s] = FOLLOW_NO_QUERY | (uint32_t)CHD_FOLLOW_OUTSIDE_SLAB;
+            f.dirty[s] = 1;
             return false;
         }
         f.last_x[s] = x;

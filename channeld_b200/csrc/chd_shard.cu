@@ -337,6 +337,14 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
         e->fail("chd_tick_sharded before chd_comm_init");
         return CHD_ERR_STATE;
     }
+    // CHD_TICK_FOLLOW: the batch is the one chd_follow_queries(_with) generated, started below like a host batch
+    const bool follow = flags & CHD_TICK_FOLLOW;
+    if (follow && q) return CHD_ERR_INVALID;
+    if (follow && !e->fw.ready) {
+        e->fail("chd_tick_sharded: CHD_TICK_FOLLOW without a batch generated by chd_follow_queries");
+        return CHD_ERR_STATE;
+    }
+    flags &= ~(uint32_t)CHD_TICK_FOLLOW;  // (chd_tick below joins the update this call begins)
     CU(e, cudaSetDevice(e->device));
     CU(e, chd_copy_wait(e));
     {
@@ -344,7 +352,7 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
         if (gs_ != CHD_OK) return gs_;
     }
     chd_status st;
-    const bool has_batch = q || e->pf_q.cur >= 0;
+    const bool has_batch = q || e->pf_q.cur >= 0 || follow;
     // Without subscriber migration the interest update does not depend on the exchange: it starts first and overlaps it.
     // With migration the immigrants' previous state arrives in the all-gather, so the update starts right after it.
     if (has_batch && !e->mig_subs) {
@@ -424,7 +432,10 @@ chd_status chd_migrate_out(chd_engine* e, const uint32_t* slot, uint32_t n) {
     }
     e->mig_packed = true;
     e->lifecycle_used = true;
-    return CHD_OK;
+    // An emigrant follows nothing here any more: this rank generates no query for it.  The binding does not ride in the blob: the
+    // follow stage runs on the engine stream before the exchange that carries the blob, so the blob would arrive too late for this
+    // tick's generation on the destination.  The destination binds the slot again (chd_follow_bind after chd_migrate_in).
+    return chd_follow_drop(e, slot, e->d_lc_slot, n);
 }
 
 chd_status chd_migrate_in(chd_engine* e, uint32_t src_rank, uint32_t first_index, const uint32_t* slot, const uint32_t* conn_id, uint32_t n) {

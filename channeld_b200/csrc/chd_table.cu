@@ -301,14 +301,18 @@ chd_status chd_rule_halo_import(chd_engine* e) {
     return e->have_gid || e->tbl.on ? CHD_OK : refuse(e, "chd_import_halo requires global entity ids (chd_set_entity_ids or entity-table mode)");
 }
 
-// 9. Followers (chd_follow_*) are single-GPU: a follower's entity may live on another rank, and border records carry no
-// positions.  So they are refused on a slab, and an engine with followers cannot become one.  `entity` of a binding is the table
-// id in entity-table mode and the entity index otherwise (chd_set_entity_ids does not change that).
+// 9. Followers (chd_follow_*) on a slab need entity-table mode: there a follower lives on the rank that owns its entity, which
+// the id resolves to through the rank's own table (halo ids never enter it), so the exact position is local.  Index-mode and
+// id-mode slabs refuse them (an entity's index there is its place in the host's array plus the halo import order), and an engine
+// with followers cannot become a slab (the slab comes first, then chd_entity_table_init, rule 4).  `entity` of a binding is the
+// table id in entity-table mode and the entity index otherwise (chd_set_entity_ids does not change that).
 chd_status chd_rule_follow(chd_engine* e, const char* fn) {
-    return e->slab ? refuse(e, "%s: followers are not available on an engine made a slab (chd_set_slab / chd_comm_init)", fn) : CHD_OK;
+    if (!e->slab || e->tbl.on) return CHD_OK;
+    return refuse(e, "%s: followers on an engine made a slab (chd_set_slab / chd_comm_init) need entity-table mode (chd_entity_table_init after the slab)", fn);
 }
 chd_status chd_rule_no_followers(chd_engine* e, const char* fn) {
-    return e->fw.n_bound ? refuse(e, "%s: %u subscriber slots follow entities (chd_follow_bind); followers are single-GPU", fn, e->fw.n_bound) : CHD_OK;
+    return e->fw.n_bound ? refuse(e, "%s: %u subscriber slots follow entities (chd_follow_bind); the slab comes before the followers", fn, e->fw.n_bound)
+                         : CHD_OK;
 }
 
 // ... and one query batch per interest update: a generated batch (chd_follow_queries) and an adopted prefetched one

@@ -330,6 +330,9 @@ class GpuStaticGrid2DSpatialController {
     // Connections whose interest follows their pawn: bound once (FollowEntities; kind == nullptr: all sphere, shape arrays of unused
     // kinds nullptr), then FollowQueries builds each tick's UPDATE_SPATIAL_INTEREST batch on the device; BeginInterest(nullptr, ..)
     // or Tick(nullptr, .., flags | CHD_TICK_FOLLOW) consumes it.  net_id: the entity index outside entity-table mode.
+    // On N GPUs (entity-table mode on slabs) a follower lives on the rank that owns its entity: TickSharded(nullptr, .., flags |
+    // CHD_TICK_FOLLOW) consumes the batch, MigrateOut unbinds the emigrants and the destination binds them again after MigrateIn.
+    // GetFollow reports CHD_FOLLOW_OUTSIDE_SLAB for a follower whose query would reach columns the slab does not serve.
     void FollowEntities(const chd_follow_batch& b) { check(chd_follow_bind(engine_, &b)); }
     void UnfollowEntities(const std::vector<uint32_t>& slot) { check(chd_follow_unbind(engine_, slot.data(), (uint32_t)slot.size())); }
     void FollowQueries(uint32_t mode = CHD_FOLLOW_MOVED) { check(chd_follow_queries(engine_, mode)); }

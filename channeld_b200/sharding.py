@@ -173,3 +173,73 @@ class EntityRouter:
                 out[d][1].append(xi)
                 out[d][2].append(zi)
         return [(np.asarray(a, np.uint32), np.asarray(b, np.float64), np.asarray(c, np.float64)) for a, b, c in out]
+
+
+class FollowerRegistry:
+    """Followers on a sharded entity-table host (chd_follow_bind on X-slabs).  A follower lives on the rank that owns its entity, so
+    its centre is always an own entity of that rank's table and its exact position is local.  Every process keeps the registry of
+    ALL ranks, as it keeps the EntityRouter: connection -> (entity id, kind, shape), and the connections' slots in a SlotTable.
+
+    After each tick's EntityRouter.handoff, plan(router) moves every follower to router.owner[entity] through plan_migrations and
+    returns, per destination, the chd_follow_bind batch of its arriving slots (first placements and immigrants).  A follower whose
+    entity the router does not know (despawned, not spawned yet) stays where it is; its rank reports CHD_FOLLOW_NO_ENTITY.
+
+    Per tick, on every rank: route the entity events; adopt the hand-offs (spawn); chd_migrate_out / chd_migrate_in (and
+    chd_add_subscribers for first placements); bind the arrivals; chd_follow_queries(_with)(CHD_FOLLOW_MOVED);
+    chd_tick_sharded(NULL, .., flags | CHD_TICK_FOLLOW); chd_handoff_entities.  chd_migrate_out unbinds the emigrants on the source;
+    the binding does not travel in the migration blob, so the destination binds them again."""
+
+    SHAPE = ("sph_r", "box_ex", "box_ez", "cone_dx", "cone_dz", "cone_angle", "cone_r")
+
+    def __init__(self, world: int):
+        self.world = int(world)
+        self.slots = SlotTable(world)
+        self.bind = {}  # connection -> (entity id, kind, shape: 7 floats in SHAPE order)
+        self._rebind = set()  # connections bound since the last plan()
+
+    def follow(self, conn, entity, kind, shape):
+        """Binds (or re-binds) a connection; it is placed or re-bound by the next plan()."""
+        shape = tuple(float(v) for v in shape)
+        if len(shape) != 7:
+            raise ValueError("a follower's shape is 7 values: " + ", ".join(self.SHAPE))
+        self.bind[conn] = (int(entity), int(kind), shape)
+        self._rebind.add(conn)
+
+    def unfollow(self, conn):
+        """Forgets a connection -> (rank, slot) it occupied (chd_remove_subscribers there), or None if it was never placed."""
+        self.bind.pop(conn, None)
+        self._rebind.discard(conn)
+        return self.slots.remove(conn) if conn in self.slots.owner else None
+
+    def owner_of(self, conn):
+        return self.slots.owner.get(conn)
+
+    def batch(self, conns):
+        """The chd_follow_bind arrays of `conns` (placed connections): dict(slot u32, entity u32, kind u8, shape f64 [7][m])."""
+        conns = list(conns)
+        m = len(conns)
+        out = dict(slot=np.array([self.slots.slot[c] for c in conns], np.uint32),
+                   entity=np.array([self.bind[c][0] for c in conns], np.uint32),
+                   kind=np.array([self.bind[c][1] for c in conns], np.uint8),
+                   shape=np.array([self.bind[c][2] for c in conns], np.float64).reshape(m, 7).T.copy())
+        out["conn"] = conns
+        return out
+
+    def plan(self, router):
+        """One tick's placement: -> (arrivals, out_lists, in_calls, vacated, binds) where the first four are plan_migrations' (by
+        connection) and binds[rank] is the chd_follow_bind batch (FollowerRegistry.batch) of the connections that arrive on `rank`
+        this tick, or were re-bound there with follow(), in connection order."""
+        conns = sorted(c for c, (e, _, _) in self.bind.items() if e in router.owner)
+        new_owner = {c: router.owner[self.bind[c][0]] for c in conns}
+        arrivals, out_lists, in_calls, vacated = plan_migrations(self.slots, new_owner)
+        fresh = [set() for _ in range(self.world)]
+        for r in range(self.world):
+            fresh[r] |= {c for c, _ in arrivals[r]}
+        for dst, _, _, pairs in in_calls:
+            fresh[dst] |= {c for c, _ in pairs}
+        for c in self._rebind:
+            if c in self.slots.owner:
+                fresh[self.slots.owner[c]].add(c)
+        self._rebind = {c for c in self._rebind if c not in self.slots.owner}  # (not placed yet: its entity is unknown)
+        binds = [self.batch(sorted(fresh[r])) for r in range(self.world)]
+        return arrivals, out_lists, in_calls, vacated, binds

@@ -491,11 +491,17 @@ func (ctl *GpuStaticGrid2DSpatialController) DestroyObjects(netIds []uint32) ([]
 	return status, nil
 }
 
+// FollowOutsideSlab: the follower status (chd_get_follow) of a generated query that would reach columns the slab does not serve.
+const FollowOutsideSlab = uint32(C.CHD_FOLLOW_OUTSIDE_SLAB)
+
 // FollowEntities binds connection slots to the entities they stand on (chd_follow_bind); kind[i] is a CHD_AOI_SPHERE | BOX | CONE
 // mask (nil: all sphere) and shape the per-binding parameters in the order sph_r, box_ex, box_ez, cone_dx, cone_dz, cone_angle,
 // cone_r (a nil entry: no binding uses that kind).  The arrays are copied before the call returns, so Go slices are fine.
 // FollowQueries then generates each tick's interest batch on the device (mode CHD_FOLLOW_ALL / CHD_FOLLOW_MOVED); BeginInterest(nil)
 // or a Tick with CHD_TICK_FOLLOW consumes it.  Clients with a pawn are bound; server connections keep sending explicit queries.
+// On N GPUs (entity-table mode on slabs) a follower lives on the rank that owns its entity: TickSharded with CHD_TICK_FOLLOW consumes
+// the batch, MigrateOut unbinds the emigrants and the destination binds them again after MigrateIn; a follower whose query would reach
+// columns the slab does not serve gets FollowOutsideSlab.
 // UN-RUN like the rest of this file.
 func (ctl *GpuStaticGrid2DSpatialController) FollowEntities(slots, netIds []uint32, kind []uint8, shape [7][]float64) error {
 	if len(netIds) != len(slots) || len(slots) == 0 {

@@ -513,7 +513,16 @@ chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out);
  *                       fan-out state and interval, subscription.go:44-57).  A follower whose entity does not exist (index >= the
  *                       entity count; id not live in the table — a slot reused by another id is not followed) gets no query and
  *                       keeps its subscriptions, like a connection that sent no update; when the id is spawned again the follower
- *                       resumes and counts as moved.  An entity outside the world gives CHD_Q_ERR_OUT_OF_WORLD from the query
+ *                       resumes and counts as moved.  On a slab (entity-table mode) the id resolves through the rank's own table,
+ *                       which holds its own entities only, so "the entity exists" means "this rank owns it": a follower whose id is
+ *                       a halo entity, or was handed off (chd_handoff_entities), gets CHD_FOLLOW_NO_ENTITY, keeps its
+ *                       subscriptions, and counts as moved when the id is own again.  Also on a slab, a selected follower whose
+ *                       query would reach columns the slab does not serve gets no query and CHD_FOLLOW_OUTSIDE_SLAB: the served
+ *                       columns are [col_lo - halo, col_hi + halo); the query's span is the union over its kinds of the columns
+ *                       floor((cx - reach - off_x) / w) .. floor((cx + reach - off_x) / w) (reach = sph_r, box_ex, cone_r), clipped
+ *                       to [0, cols) because samples outside the world are skipped.  The check is conservative (a bounding box,
+ *                       not the samples).  Such a follower keeps its subscriptions and its last centre, and counts as moved.  An
+ *                       engine that is not a slab never makes this check.  An entity outside the world gives CHD_Q_ERR_OUT_OF_WORLD from the query
  *                       path as for any batch.  The batch has one entry per FOLLOWER (B): entries behind the selected ones are
  *                       skip entries (sub = 0xFFFFFFFF, kind = 0, status CHD_Q_OK), so the batch length the interest stage and
  *                       chd_get_query_status / the status list of chd_fetch_results* see is B, and entry i below the selected
@@ -547,19 +556,24 @@ chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out);
  *                       (chd_get_follow reports CHD_FOLLOW_OVERRIDDEN), its stored centre stays, and it counts as moved, so the
  *                       next CHD_FOLLOW_MOVED generation selects it again and its subscriptions return to the follow shape (unbind
  *                       the slot to keep the explicit query).  Consumed like chd_follow_queries' batch.  Refused, changing nothing
- *                       (an adopted batch stays adopted): CHD_ERR_CAPACITY if H + B > max_queries; CHD_ERR_STATE on a slab,
+ *                       (an adopted batch stays adopted): CHD_ERR_CAPACITY if H + B > max_queries; CHD_ERR_STATE on an index-mode or id-mode slab,
  *                       while a generated batch is unconsumed or a chd_begin_interest is pending, with q == NULL and no adopted
  *                       query batch, and with q != NULL while an adopted one is unconsumed; CHD_ERR_INVALID for a bad mode or a
  *                       host part with sub == NULL.
  *   chd_get_follow      after the interest update that consumed the batch (and before the next one): per follower, in ascending
  *                       slot order, its slot, entity, the centre of the last query generated for it, and status = the CHD_Q_*
  *                       status of its query (its entry in a merged batch is H + its rank), or CHD_FOLLOW_NOT_SELECTED /
- *                       CHD_FOLLOW_NO_ENTITY / CHD_FOLLOW_OVERRIDDEN.  *count = followers (copies
+ *                       CHD_FOLLOW_NO_ENTITY / CHD_FOLLOW_OVERRIDDEN / CHD_FOLLOW_OUTSIDE_SLAB.  *count = followers (copies
  *                       min(count, cap)), *n_selected = queries in the last generated batch; this call is where the selected count
  *                       is reported (chd_tick_summary is unchanged).  Synchronous; any pointer may be NULL.
- * Followers are single-GPU: CHD_ERR_STATE on an engine made a slab (chd_set_slab / chd_comm_init; a follower's entity may live on
- * another rank, and border records carry no positions), and those two calls are refused once a slot follows.  Not supported:
- * centre offsets, cone directions taken from an entity's rotation, spots relative to an entity. */
+ * Followers on a slab need entity-table mode (the slab first, then chd_entity_table_init): a follower lives on the rank that owns
+ * its entity, whose exact position is local there (border records carry no positions).  CHD_ERR_STATE on an index-mode or id-mode
+ * slab, and chd_set_slab / chd_comm_init are refused once a slot follows.  chd_tick_sharded(e, NULL, .., flags | CHD_TICK_FOLLOW)
+ * consumes the generated batch as chd_tick does.  A follower moves with its entity: chd_migrate_out unbinds the emigrants, and the
+ * destination binds them again with chd_follow_bind after chd_migrate_in (the binding does not travel in the migration blob).
+ * Halo: halo_cols >= ceil(max reach / w) + the columns an entity can cross in one tick keeps the tick on which an entity crosses
+ * into a neighbour's slab exact (its old owner still generates the query); a smaller halo reports CHD_FOLLOW_OUTSIDE_SLAB there.
+ * Not supported: centre offsets, cone directions taken from an entity's rotation, spots relative to an entity. */
 typedef struct chd_follow_batch {          /* SoA, HOST arrays */
     uint32_t n;
     const uint32_t* slot;                  /* [n] subscriber slot */
@@ -570,6 +584,7 @@ typedef struct chd_follow_batch {          /* SoA, HOST arrays */
 enum { CHD_FOLLOW_ALL = 0, CHD_FOLLOW_MOVED = 1 };
 enum { CHD_FOLLOW_NOT_SELECTED = 16, CHD_FOLLOW_NO_ENTITY = 17 }; /* beside CHD_Q_* in chd_get_follow's status */
 enum { CHD_FOLLOW_OVERRIDDEN = 18 };  /* the slot's host entry in chd_follow_queries_with's batch replaced its generated query */
+enum { CHD_FOLLOW_OUTSIDE_SLAB = 19 }; /* the generated query would reach columns the slab does not serve: no query this tick */
 chd_status chd_follow_bind(chd_engine* e, const chd_follow_batch* b);
 chd_status chd_follow_unbind(chd_engine* e, const uint32_t* slot, uint32_t n);
 chd_status chd_follow_queries(chd_engine* e, uint32_t mode);
