@@ -8,6 +8,8 @@
 // Grouping = open-addressing hash table keyed by the full 192-bit identity (window_hi, lo, word): a slot is claimed with
 // one atomicCAS by the first record that reaches it and identified by THAT record's key from then on, so equal keys
 // always meet in the same slot and unequal keys never share one — exact, no reliance on hash quality.
+// A CHD_DUE_VOID hole (a slot an overflowed fan-out reserved but did not fill, chd_fanout.cuh) is not a decision: its key and
+// window are whatever an earlier tick left there, so it probes nothing, gets class_of = CHD_DUE_VOID and is in no class.
 #pragma once
 #include "chd_types.cuh"
 
@@ -26,6 +28,10 @@ __global__ void __launch_bounds__(256)
     const uint32_t n = min(*n_due_ptr, due_cap);
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    if (due[i].kind == CHD_DUE_VOID) {
+        slot_of[i] = CHD_DUE_VOID;
+        return;
+    }
     const int64_t hi = due[i].window_hi;
     const DueKey k = key[i];
     const bool full = !((k.word >> 33) & 1ull);  // FULL sends of a channel share one payload whatever their window
@@ -59,7 +65,10 @@ __global__ void __launch_bounds__(256)
     const uint32_t n = min(*n_due_ptr, due_cap);
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i == 0) *bump_epoch = chd_next_epoch(*bump_epoch);
-    if (i < n) flag[i] = rep_min[slot_of[i]] == i ? 1u : 0u;
+    if (i < n) {
+        const uint32_t h = slot_of[i];
+        flag[i] = h != CHD_DUE_VOID && rep_min[h] == i ? 1u : 0u;
+    }
 }
 
 // rank[] = exclusive scan of flag[]: class ids are numbered by their lowest member
@@ -70,7 +79,12 @@ __global__ void __launch_bounds__(256)
     const uint32_t n = min(*n_due_ptr, due_cap);
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const uint32_t h = slot_of[i], rep = rep_min[h], id = rank[rep];
+    const uint32_t h = slot_of[i];
+    if (h == CHD_DUE_VOID) {
+        class_of[i] = CHD_DUE_VOID;
+        return;
+    }
+    const uint32_t rep = rep_min[h], id = rank[rep];
     class_of[i] = id;
     if (rep == i) {
         class_rep[id] = i;

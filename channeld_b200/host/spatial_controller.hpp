@@ -263,6 +263,7 @@ class GpuStaticGrid2DSpatialController {
     }
 
     // Window classes of the last fan-out pass (data.go:248-252: which decisions share one merged payload).
+    // A CHD_DUE_VOID hole of an overflowed list has class_of == CHD_DUE_VOID and belongs to no class.
     struct DueClasses {
         std::vector<uint32_t> class_of, rep, count;
     };

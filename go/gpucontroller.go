@@ -392,6 +392,7 @@ func (ctl *GpuStaticGrid2DSpatialController) AdjacentBroadcast(channelIds []comm
 
 // DueClasses groups the due list of the last tick by payload identity (data.go:248-252 merges afresh per subscriber):
 // the host merges / marshals the window of due record rep[k] once and sends it to every record i with classOf[i] == k.
+// A CHD_DUE_VOID hole of an overflowed list has classOf[i] == CHD_DUE_VOID (0xFFFFFFFF) and belongs to no class.
 func (ctl *GpuStaticGrid2DSpatialController) DueClasses(nDue int) (classOf, rep, count []uint32, err error) {
 	if nDue == 0 {
 		return nil, nil, nil, nil

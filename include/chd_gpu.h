@@ -768,6 +768,8 @@ chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank,
  *   - an UPDATE decision whose subscriber had own updates inside the window is a class of its own.
  * out_class_of[i] = class of due record i (index into the list chd_get_due / chd_fetch_results return, same order),
  * out_class_rep[k] = lowest due index of class k (classes are numbered by it), out_class_count[k] = its size.
+ * A CHD_DUE_VOID hole (a list that overflowed, CHD_OVF_DUE) has class CHD_DUE_VOID and is in no class: the classes, their
+ * numbering, reps and counts cover the real decisions only.
  * Any output may be NULL.  CHD_ERR_CAPACITY if there are more than cap_classes classes.  Synchronous. */
 chd_status chd_due_classes(chd_engine* e, uint32_t* out_class_of, uint32_t* out_class_rep, uint32_t* out_class_count,
                            uint32_t cap_classes, uint32_t* out_n_classes);

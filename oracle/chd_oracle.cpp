@@ -510,6 +510,27 @@ uint64_t orc_channels_tick_data(orc_channel* const* ch, uint32_t n_ch, int64_t t
     return total;
 }
 
+uint64_t orc_channels_tick_data_ex(orc_channel* const* ch, uint32_t n_ch, int64_t t_ns, orc_send* out, uint64_t cap, uint64_t* out_off,
+                                   int64_t* window_lo, uint32_t* self_skipped, uint64_t* sel_off, uint32_t* sel_pos, uint64_t sel_cap) {
+    uint64_t total = 0, n_sel = 0;
+    out_off[0] = 0;
+    sel_off[0] = 0;
+    std::vector<uint32_t> off1;  // one channel's selection offsets, relative to its first selected position
+    for (uint32_t c = 0; c < n_ch; c++) {
+        const uint64_t room = cap - total, sel_room = sel_cap - n_sel;
+        const uint32_t r = room > 0xFFFFFFFEull ? 0xFFFFFFFEu : uint32_t(room);
+        off1.resize(uint64_t(r) + 1);
+        const uint32_t k = orc_channel_tick_data_ex(ch[c], t_ns, out + total, r, window_lo + total, self_skipped + total, off1.data(),
+                                                    sel_pos + n_sel, sel_room > 0xFFFFFFFEull ? 0xFFFFFFFEu : uint32_t(sel_room));
+        if (k == uint32_t(-1)) return uint64_t(-1);
+        for (uint32_t j = 1; j <= k; j++) sel_off[total + j] = n_sel + off1[j];
+        n_sel += off1[k];
+        total += k;
+        out_off[c + 1] = total;
+    }
+    return total;
+}
+
 void orc_channels_get_state(orc_channel* const* ch, const uint32_t* chan, const uint32_t* conn_id, uint64_t n, int64_t* last_fanout,
                             uint8_t* had_first, uint64_t* last_msg_index, uint8_t* found) {
     for (uint64_t i = 0; i < n; i++) {

@@ -159,6 +159,11 @@ void orc_channels_on_update(orc_channel* const* ch, const uint32_t* chan, const 
 /* tick_data of channels 0 .. n_ch-1 in turn; the sends of channel c are out[out_off[c] .. out_off[c+1]).  Returns the total,
  * or (uint64_t)-1 when `cap` is too small or a channel's iteration bound trips. */
 uint64_t orc_channels_tick_data(orc_channel* const* ch, uint32_t n_ch, int64_t t_ns, orc_send* out, uint64_t cap, uint64_t* out_off);
+/* The same with orc_channel_tick_data_ex's identities for every send (window_lo[cap], self_skipped[cap]); the ring positions merged
+ * into send i are sel_pos[sel_off[i] .. sel_off[i+1]) (positions within its channel's ring), one CSR across all channels
+ * (sel_off[cap+1]).  Returns the total, or (uint64_t)-1 when `cap` or `sel_cap` is too small or an iteration bound trips. */
+uint64_t orc_channels_tick_data_ex(orc_channel* const* ch, uint32_t n_ch, int64_t t_ns, orc_send* out, uint64_t cap, uint64_t* out_off,
+                                   int64_t* window_lo, uint32_t* self_skipped, uint64_t* sel_off, uint32_t* sel_pos, uint64_t sel_cap);
 /* found[i] = 0 when conn_id[i] is not subscribed to chan[i] (the state outputs are then left as they were) */
 void orc_channels_get_state(orc_channel* const* ch, const uint32_t* chan, const uint32_t* conn_id, uint64_t n, int64_t* last_fanout,
                             uint8_t* had_first, uint64_t* last_msg_index, uint8_t* found);

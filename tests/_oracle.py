@@ -103,6 +103,9 @@ class Oracle:
         L.orc_channels_on_update.argtypes = [vp, u32p, C.POINTER(C.c_int64), u32p, C.c_uint64]
         L.orc_channels_tick_data.restype = C.c_uint64
         L.orc_channels_tick_data.argtypes = [vp, C.c_uint32, C.c_int64, C.POINTER(Send), C.c_uint64, u64p]
+        L.orc_channels_tick_data_ex.restype = C.c_uint64
+        L.orc_channels_tick_data_ex.argtypes = [vp, C.c_uint32, C.c_int64, C.POINTER(Send), C.c_uint64, u64p, C.POINTER(C.c_int64), u32p, u64p,
+                                                u32p, C.c_uint64]
         L.orc_channels_get_state.restype = None
         L.orc_channels_get_state.argtypes = [vp, u32p, u32p, C.c_uint64, C.POINTER(C.c_int64), C.POINTER(C.c_uint8), u64p,
                                              C.POINTER(C.c_uint8)]
@@ -371,6 +374,21 @@ class OracleChannels:
         k = self.L.orc_channels_tick_data(self._hp(), self.n, int(t_ns), out.ctypes.data_as(C.POINTER(Send)), int(cap), _p(off, u64p))
         assert k != 2 ** 64 - 1, "oracle tick_data: capacity/iteration bound"
         return out[:k], off
+
+    def tick_data_ex(self, t_ns, cap, sel_cap):
+        """tick_data + per send its window_lo, self_skipped and the ring positions merged (positions within its channel's ring)
+        -> (sends, off[n+1], window_lo, self_skipped, sel_off u64[len(sends)+1], sel_pos): send i merged sel_pos[sel_off[i]:sel_off[i+1]]"""
+        cap = max(int(cap), 1)
+        out = np.zeros(cap, SEND_DTYPE)
+        off = np.zeros(self.n + 1, np.uint64)
+        lo = np.zeros(cap, np.int64)
+        sk = np.zeros(cap, np.uint32)
+        so = np.zeros(cap + 1, np.uint64)
+        sp = np.zeros(max(int(sel_cap), 1), np.uint32)
+        k = self.L.orc_channels_tick_data_ex(self._hp(), self.n, int(t_ns), out.ctypes.data_as(C.POINTER(Send)), cap, _p(off, u64p),
+                                             lo.ctypes.data_as(C.POINTER(C.c_int64)), _p(sk, u32p), _p(so, u64p), _p(sp, u32p), len(sp))
+        assert k != 2 ** 64 - 1, "oracle tick_data_ex: capacity/iteration bound"
+        return out[:k], off, lo[:k], sk[:k], so[:k + 1], sp[:int(so[k])]
 
     def state(self, chan, conn):
         """-> (last[n], had_first[n], last_index[n], found[n])"""
