@@ -6,12 +6,13 @@
 static DeltaDev delta_view(chd_engine* e) {
     chd_engine::Delta& D = e->dl;
     const PairBuf& pb = e->pairs[e->cur];
+    const CopySet& c = chd_copy_in(e);
     DeltaDev d{};
     d.cells = e->g.cells;
     d.key = e->d_key;
     d.n = e->n_sorted;
-    d.cell_start = e->d_cell_start;
-    d.sorted = e->d_sorted_ent;
+    d.cell_start = c.cell_start;
+    d.sorted = c.sorted_ent;
     d.pair_off = pb.off;
     d.pair_cell = pb.cell;
     d.n_slots = e->n_slots;
@@ -24,7 +25,7 @@ static DeltaDev delta_view(chd_engine* e) {
     d.overflow = &e->d_ctr->overflow;
     d.bad_ids = nullptr;
     if (D.ids) {
-        // Id mode: the cell CSRs (now: the build's d_sorted_ent, sorted with d_gid as values; snapshot: its copy) hold global ids, so
+        // Id mode: the cell CSRs (now: the build's sorted_ent, sorted with d_gid as values; snapshot: its copy) hold global ids, so
         // the kernels must look an entity's cell up by global id.  now_gkey is that lookup for the current state and snap_key, copied
         // from it by the advance, for the snapshot; snap_hdr[0] = n = id_space once a delta has succeeded (0 before: nothing).
         // The kernels treat `e < n ? key[e] : cells` and `ent >= other_n` as "absent"; that stays right because
@@ -34,8 +35,8 @@ static DeltaDev delta_view(chd_engine* e) {
         d.key = D.now_gkey;
         d.n = D.id_space;
         d.bad_ids = D.bad_ids;
-        // the CSR by id: d_sorted_ent, or in entity-table mode (where it holds build positions) the table pass's id-valued copy
-        d.sorted = chd_sorted_out(e);
+        // the CSR by id: sorted_ent, or in entity-table mode (where it holds build positions) the table pass's id-valued copy
+        d.sorted = chd_sorted_out(e, c);
     }
     return d;
 }

@@ -57,7 +57,7 @@ static bool pf_events(chd_engine* e, Prefetch& p) {
 chd_status chd_pf_begin(chd_engine* e, Prefetch& p, int* set, cudaStream_t s) {
     if (!s && !e->up_stream && !chd_make_stream(e, &e->up_stream)) return CHD_ERR_CUDA;
     if (!pf_events(e, p)) return CHD_ERR_CUDA;
-    if (p.read_recorded[p.next]) CU(e, cudaStreamWaitEvent(s ? s : e->up_stream, p.ev_read[p.next], 0));
+    if (chd_pf_after_read(e, p, p.next, s ? s : e->up_stream) != CHD_OK) return CHD_ERR_CUDA;
     *set = p.next;
     p.staged = -1;  // a staged upload is in this set: an upload that fails part way leaves nothing staged
     return CHD_OK;
@@ -93,23 +93,16 @@ chd_status chd_pf_note_read(chd_engine* e, Prefetch& p, int set, cudaStream_t s)
     return CHD_OK;
 }
 
+chd_status chd_pf_after_read(chd_engine* e, const Prefetch& p, int set, cudaStream_t s) {
+    if (p.read_recorded[set]) CU(e, cudaStreamWaitEvent(s, p.ev_read[set], 0));
+    return CHD_OK;
+}
+
 cudaError_t chd_copy_wait(chd_engine* e) {
     if (e->copy_pending < 0) return cudaSuccess;
     const cudaError_t r = cudaStreamWaitEvent(e->stream, e->pf_copy.ev_read[e->copy_pending], 0);
     if (r == cudaSuccess) e->copy_pending = -1;
     return r;
-}
-
-void chd_copy_set_select(chd_engine* e, int set) {
-    const CopySet& c = e->copy_set[set];
-    e->d_sorted_ent = c.sorted_ent;
-    e->tbl.d_sorted_id = c.sorted_id;
-    e->d_cell_start = c.cell_start;
-    e->d_voff = c.voff;
-    e->d_first_pair = c.first_pair;
-    e->d_tile_desc = c.tile_desc;
-    e->d_general_tiles = c.general_tiles;
-    e->d_n_general = c.n_general;
 }
 
 chd_status chd_read_u32(chd_engine* e, const uint32_t* d, uint32_t* v) {
@@ -308,8 +301,7 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
         ok = ok && chd_make_event(e, ev);
     e->pf_pos.cur = 0;  // the pair allocated here is the front one; the first prefetch fills the other
     e->pf_pos.next = 1;
-    ok = ok && dalloc(e, &e->d_x, N) && dalloc(e, &e->d_z, N) && (e->d_xb[0] = e->d_x, e->d_zb[0] = e->d_z, true) &&
-         dalloc(e, &e->d_gid, N) && dalloc(e, &e->d_key, N) &&
+    ok = ok && dalloc(e, &e->pos[0].x, N) && dalloc(e, &e->pos[0].z, N) && dalloc(e, &e->d_gid, N) && dalloc(e, &e->d_key, N) &&
          dalloc(e, &e->d_prev_key, N) && dalloc(e, &e->ent_sort.tmp_key, N) && dalloc(e, &e->ent_sort.tmp_val, N) &&
          dalloc(e, &e->d_sorted_key, N) &&
          // padded: an emit chunk that starts m != 0 entries into an aligned 16-byte chunk also loads the next aligned chunk,
@@ -365,7 +357,6 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
         CCU(cudaMemsetAsync(c.n_visible, 0, 8, e->stream));
         CCU(cudaMemsetAsync(c.cell_start, 0, (C + 2) * 4, e->stream));
     }
-    chd_copy_set_select(e, 0);
     e->pf_copy.cur = 0;  // a build fills set 1 first
     e->pf_copy.next = 1;
     CCU(cudaMemsetAsync(e->d_slot_ctl, 0, S, e->stream));

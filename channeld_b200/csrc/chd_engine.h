@@ -36,6 +36,8 @@ using namespace chd;
 // while a tick is in flight, and hands to the next tick with chd_adopt_prefetched.  The sets' buffers stay with their kind; this
 // holds which set is free, which is staged and which is read, and the events that order the uploads against the reads.  A
 // prefetch fills the set other than the one adopted last, after the last recorded read of it (chd_pf_*).
+// A double-buffered kind's sets are reached only through its Prefetch: readers use set `cur`, the writer uses the set that
+// chd_pf_begin returned.  No member of chd_engine points into a set.
 struct Prefetch {
     int next = 0;      // the set the next prefetch fills
     int staged = -1;   // the set holding an upload not adopted yet (-1: none)
@@ -64,10 +66,19 @@ struct CopySet {
     uint32_t* cell_start = nullptr;                        // [C+2]
     uint64_t* voff = nullptr;
     uint32_t* first_pair = nullptr;
-    TileDesc* tile_desc = nullptr;
-    uint32_t *general_tiles = nullptr, *n_general = nullptr;
+    TileDesc* tile_desc = nullptr;  // per-tile copy descriptors (chd_emit.cuh)
+    uint32_t *general_tiles = nullptr, *n_general = nullptr;  // tiles with more than two segments: list, {length, consumer ticket}
     unsigned long long* n_visible = nullptr;  // V of this set's preparation (the summary keeps its own copy in Counters)
 };
+
+// One pair of position buffers: chd_create allocates set 0, the first chd_prefetch_entities set 1.
+struct PosSet {
+    double *x = nullptr, *z = nullptr;
+    uint32_t n = 0;  // entities a prefetch uploaded into it
+};
+
+// Positions as the kernels read them (chd_positions).
+struct Positions { const double *x = nullptr, *z = nullptr; };
 
 struct chd_engine {
     chd_grid_cfg cfg;
@@ -128,26 +139,21 @@ struct chd_engine {
     bool halo_on_device = false;     // multi-GPU: the build length (own + halo) lives in d_n_build
     uint32_t* d_n_build = nullptr;
     bool have_gid = false;
-    double *d_x = nullptr, *d_z = nullptr;        // engine-owned staging for host inputs (the FRONT buffers: d_xb / d_zb[pf_pos.cur])
-    // position pairs: [0] is allocated by chd_create, [1] by the first chd_prefetch_entities; a prefetch fills the BACK pair and
-    // chd_adopt_prefetched makes it the front one.  pos_n: entities a prefetch uploaded into each pair.
-    double *d_xb[2] = {nullptr, nullptr}, *d_zb[2] = {nullptr, nullptr};
-    uint32_t pos_n[2] = {0, 0};
-    Prefetch pf_pos;  // pf_pos.cur = the front pair (chd_create sets it to 0)
-    uint32_t *d_general_tiles = nullptr, *d_n_general = nullptr;  // tiles with more than two segments: list, {length, consumer ticket}
+    // position pairs: the set calls, chd_entity_buffers and the table-mode kernels use the front pair pos[pf_pos.cur] (chd_pos_front;
+    // chd_create makes it 0), a prefetch fills the back one and chd_adopt_prefetched makes it the front one
+    PosSet pos[2];
+    Prefetch pf_pos;
+    Positions in_place;  // the caller's device arrays the last set call reads in place (x == nullptr: the front pair)
     float* d_pos_f32[2] = {nullptr, nullptr};  // float staging of chd_set_entities_f32 [0] / chd_prefetch_entities_f32 [1]: x then z
     cudaStream_t up_stream = nullptr;  // every prefetch upload
-    const double *pos_x = nullptr, *pos_z = nullptr;  // what the kernels read: the staging buffers, or the caller's device arrays
     uint32_t *d_gid = nullptr;            // [max_entities] global ids (multi-GPU) of own + halo
     uint32_t *d_key = nullptr, *d_prev_key = nullptr;  // [max_entities] cell key per entity
     // the build's sort by cell: 4 blocks per SM, N-sized temporaries, which chd_get_rehome and chd_handoff_entities borrow as
     // scratch between builds
     CellSort ent_sort;
-    uint32_t *d_sorted_key = nullptr, *d_sorted_ent = nullptr;
-    uint32_t *d_cell_start = nullptr;     // [C+2]
-    // d_sorted_ent, d_cell_start, tbl.d_sorted_id, d_voff, d_first_pair, d_tile_desc, d_general_tiles and d_n_general point into
-    // copy_set[pf_copy.cur] (chd_copy_set_select).  Each build takes the set the last copy kernel did not read (chd_pf_begin orders
-    // the build after the last copy that read it); chd_pf_note_read records each copy kernel's read.
+    uint32_t* d_sorted_key = nullptr;
+    // Readers use copy_set[pf_copy.cur] (chd_copy_in).  Each build writes the set the last copy kernel did not read (chd_pf_begin
+    // orders the build after the last copy that read it) and adopts it when it ends; chd_pf_note_read records each copy kernel's read.
     CopySet copy_set[2];
     Prefetch pf_copy;
     // Two-stream ticks: the build runs on build_stream (highest priority), the copy kernel on copy_stream (lowest priority), so
@@ -183,12 +189,12 @@ struct chd_engine {
         uint32_t *sub; uint8_t* kind;
         double *sph_cx, *sph_cz, *sph_r, *box_cx, *box_cz, *box_ex, *box_ez, *cone_cx, *cone_cz, *cone_dx, *cone_dz, *cone_angle, *cone_r;
         uint32_t *spot_off, *spot_ndist; double *spot_x, *spot_z; uint32_t* spot_dist;
+        QueryDev view;   // a prefetch set: the batch it holds
+        uint32_t spots;  // and its spot total
     } dq{};
     // chd_prefetch_queries / chd_prefetch_rings: two staging sets each, allocated by the first prefetch that fills them.
     // pf_q.cur: the adopted batch the next interest update with q == NULL consumes (-1 once consumed).
     QStage dq_pf[2] = {};
-    QueryDev dq_pf_view[2] = {};  // the batch each set holds
-    uint32_t dq_pf_spots[2] = {0, 0};  // and its spot total
     Prefetch pf_q;
     struct RStage {
         uint32_t *off, *sender; int64_t* arrival; uint64_t *index, *cmi;
@@ -211,8 +217,7 @@ struct chd_engine {
     uint32_t *d_new_off = nullptr;  // scratch for u64 -> u32 offset narrowing (stateless query path)
     uint32_t *d_new_sub = nullptr, *d_new_ch = nullptr, *d_gone_sub = nullptr, *d_gone_ch = nullptr;
     // emit
-    uint32_t *d_vcnt = nullptr, *d_first_pair = nullptr, *d_vis = nullptr;
-    TileDesc* d_tile_desc = nullptr;  // per-tile copy descriptors (chd_emit.cuh)
+    uint32_t *d_vcnt = nullptr, *d_vis = nullptr;
     uint32_t* d_pair_ch = nullptr;  // channel id of every current pair (written by interest_fill_kernel)
     // ---- window classes of the due list (chd_due_classes): keys written by the fan-out kernel, scratch allocated on first use
     DueKey* d_due_key = nullptr;
@@ -266,7 +271,7 @@ struct chd_engine {
     uint64_t fetch_issued = 0, fetch_waited = 0;
     bool fetch_guard = false;
     bool early_ready = false;  // ev_join + ev_prep_done of the last tick are recorded
-    uint64_t *d_voff = nullptr, *d_vis_off = nullptr;
+    uint64_t* d_vis_off = nullptr;
     uint64_t max_tiles = 0;
     uint64_t vis_estimate = 0;  // n_visible of the last summary the host decoded (0 = none yet): sizes the emit grid
     // fanout
@@ -374,7 +379,7 @@ struct chd_engine {
         uint64_t rebuilds = 0, builds = 0;  // builds: table-mode builds so far (the device counts them too: d_build_seq)
         bool ho_raw = false;   // the handover list holds slots of a fresh cell assignment (chd_assign_host)
         uint64_t* d_table = nullptr;
-        uint32_t *d_id_of_slot = nullptr, *d_snap_id = nullptr, *d_sorted_id = nullptr, *d_winner = nullptr, *d_mslot = nullptr;
+        uint32_t *d_id_of_slot = nullptr, *d_snap_id = nullptr, *d_winner = nullptr, *d_mslot = nullptr;
         uint32_t *d_ho_tmp = nullptr, *d_build_seq = nullptr;  // d_build_seq[0] = builds, [1] = stashed handover count
         uint8_t* d_flag = nullptr;                             // slot spawned / despawned since the last cell assignment
         unsigned long long* d_stats = nullptr;                 // moves applied, to unknown ids, superseded within a call
@@ -518,17 +523,17 @@ void chd_dfree(chd_engine* e, void* p);
 // instead of up_stream when one is given (the copy-input sets: the build writes them).  adopt: makes the staged set
 // the one read (false: nothing staged).  wait: orders reader stream `s` after the upload, once per adoption.  note_read:
 // records a read of `set` (-1: none) on `s`, outside any graph capture, so that no prefetch overwrites it before that read.
+// after_read: orders `s` after the last recorded read of `set` (a writer of that set).
 chd_status chd_pf_begin(chd_engine* e, Prefetch& p, int* set, cudaStream_t s = nullptr);
 chd_status chd_pf_end(chd_engine* e, Prefetch& p, cudaStream_t s = nullptr);
 bool chd_pf_adopt(Prefetch& p);
 chd_status chd_pf_wait(chd_engine* e, Prefetch& p, cudaStream_t s);
 chd_status chd_pf_note_read(chd_engine* e, Prefetch& p, int set, cudaStream_t s);
+chd_status chd_pf_after_read(chd_engine* e, const Prefetch& p, int set, cudaStream_t s);
 chd_status chd_read_u32(chd_engine* e, const uint32_t* d, uint32_t* v);
 // Orders the engine stream after the copy kernel a two-stream chd_tick left running on copy_stream (device-side, no host sync).
 // Every entry point that reads the expanded list, hands out device memory or is a documented completion point calls it first.
 cudaError_t chd_copy_wait(chd_engine* e);
-// Points the engine's copy-input pointers at copy_set[set].
-void chd_copy_set_select(chd_engine* e, int set);
 chd_status chd_decode_summary(chd_engine* e, chd_tick_summary* out);
 chd_status chd_assign_cells_impl(chd_engine* e, cudaStream_t s);
 // Host half of a cell assignment: the key buffers swap (handover detection compares against the keys of the previous
@@ -538,7 +543,6 @@ uint32_t* chd_assign_host(chd_engine* e);
 // the current positions were replaced by n others (a set call, chd_set_entity_count, an adopted prefetch): nothing is assigned
 // or built for them yet
 void chd_entities_replaced(chd_engine* e, uint32_t n);
-chd_status chd_note_pos_read(chd_engine* e, cudaStream_t s);
 // Called on the host wherever a stage's epoch is about to be bumped on the device: every 2^20 executions of a stage the
 // descriptors of its scan sites are cleared, so no descriptor can survive until the 22-bit epoch repeats.  `s` is the
 // stream the stage runs on, so the clear is ordered before the stage's scans.
@@ -588,9 +592,9 @@ chd_status chd_rule_merged_batch(chd_engine* e, bool adopted);
 // followers (chd_follow.cu): the listed slots (n == 0 with slot == nullptr: every slot) follow nothing from now on; d_slot: the
 // same list on the device if the caller uploaded it already
 chd_status chd_follow_drop(chd_engine* e, const uint32_t* slot, const uint32_t* d_slot, uint32_t n);
-// entity-table mode (chd_table.cu): the pass after every table-mode build (sorted ids, handover list in ids); the delta's
-// translation to ids, inside its stage; a decoded summary's last successful delta
-chd_status chd_table_after_build(chd_engine* e, cudaStream_t s);
+// entity-table mode (chd_table.cu): the pass after every table-mode build into copy-input set `c` (sorted ids, handover list
+// in ids); the delta's translation to ids, inside its stage; a decoded summary's last successful delta
+chd_status chd_table_after_build(chd_engine* e, cudaStream_t s, const CopySet& c);
 chd_status chd_table_delta_ids(chd_engine* e, cudaStream_t s);
 void chd_table_observe(chd_engine* e, uint32_t delta_build);
 }
@@ -601,9 +605,20 @@ __host__ __device__ inline bool chd_delta_overflowed(uint64_t n_entered, uint64_
     return n_entered > enter_cap || n_left > leave_cap || bad_ids;
 }
 
-// What the cell CSR's sorted_entity, the visible lists and the read-back report: entity indices, or ids in entity-table mode.  The
-// slot-valued d_sorted_ent stays what the delta reads.
-static inline const uint32_t* chd_sorted_out(const chd_engine* e) { return e->tbl.on ? e->tbl.d_sorted_id : e->d_sorted_ent; }
+// The copy-input set the readers use: the one the last successful build adopted.
+static inline const CopySet& chd_copy_in(const chd_engine* e) { return e->copy_set[e->pf_copy.cur]; }
+
+// What set c's sorted_entity, the visible lists and the read-back report: entity indices, or ids in entity-table mode.  The
+// slot-valued sorted_ent stays what the delta reads.
+static inline const uint32_t* chd_sorted_out(const chd_engine* e, const CopySet& c) { return e->tbl.on ? c.sorted_id : c.sorted_ent; }
+
+// The front position pair: what the set calls and the table-mode kernels write.
+static inline const PosSet& chd_pos_front(const chd_engine* e) { return e->pos[e->pf_pos.cur]; }
+
+// The positions the kernels read: the caller's arrays a set call reads in place, else the front pair.  chd_note_pos_read records
+// (outside any graph capture) a kernel's read of the front pair, so that a prefetch into it is ordered after that read.
+static inline Positions chd_positions(const chd_engine* e) { return e->in_place.x ? e->in_place : Positions{chd_pos_front(e).x, chd_pos_front(e).z}; }
+static inline chd_status chd_note_pos_read(chd_engine* e, cudaStream_t s) { return chd_pf_note_read(e, e->pf_pos, e->in_place.x ? -1 : e->pf_pos.cur, s); }
 
 // The ids build positions carry: entity-table slots by the table and the halo after them by d_gid, else d_gid or the index.
 static inline EntityIds chd_entity_ids(const chd_engine* e) {

@@ -6,7 +6,7 @@
 
 // assign: when set, the pass's histogram kernel also computes the keys from the positions (first pass of a single-GPU build)
 struct FusedAssign {
-    const double *x, *z;
+    Positions pos;
     uint32_t* key;
     const uint32_t* prev;
     HandoverOut ho;
@@ -29,7 +29,7 @@ template <int BINS>
 static chd_status count_digits(chd_engine* e, cudaStream_t s, const SortPass& p, const ScanSite& site, unsigned long long* bump,
                                const FusedAssign* assign) {
     if (assign)
-        assign_hist_kernel<BINS><<<p.nblocks, BUILD_THREADS, 0, s>>>(e->g, assign->x, assign->z, p.n, assign->key, assign->prev, assign->ho, p.per_block,
+        assign_hist_kernel<BINS><<<p.nblocks, BUILD_THREADS, 0, s>>>(e->g, assign->pos.x, assign->pos.z, p.n, assign->key, assign->prev, assign->ho, p.per_block,
                                                                      p.mask, p.hist, p.nblocks, bump);
     else
         radix_hist_kernel<BINS><<<p.nblocks, BUILD_THREADS, 0, s>>>(p.key, p.n, p.n_ptr, p.per_block, p.shift, p.mask, p.hist, p.nblocks, bump);
@@ -177,33 +177,26 @@ static chd_status upload_positions(chd_engine* e, const char* fn, const void* x,
         return CHD_ERR_CAPACITY;
     }
     CU(e, cudaSetDevice(e->device));
-    cudaStream_t s = e->stream;
-    double *dx = e->d_x, *dz = e->d_z;
-    int set = 0;
-    chd_status st;
-    if (prefetch) {
-        st = chd_pf_begin(e, e->pf_pos, &set);
-        if (st != CHD_OK) return st;
-        // the second pair of position buffers exists only for hosts that prefetch
-        if (!e->d_zb[set] && !(dalloc(e, &e->d_xb[set], e->lim.max_entities) && dalloc(e, &e->d_zb[set], e->lim.max_entities))) return CHD_ERR_CUDA;
-        s = e->up_stream;
-        dx = e->d_xb[set];
-        dz = e->d_zb[set];
-    }
+    int set = e->pf_pos.cur;
+    chd_status st = prefetch ? chd_pf_begin(e, e->pf_pos, &set) : CHD_OK;
+    if (st != CHD_OK) return st;
+    cudaStream_t s = prefetch ? e->up_stream : e->stream;
+    PosSet& p = e->pos[set];
+    // the second pair of position buffers exists only for hosts that prefetch
+    if (!p.z && !(dalloc(e, &p.x, e->lim.max_entities) && dalloc(e, &p.z, e->lim.max_entities))) return CHD_ERR_CUDA;
     const bool in_place = !f32 && !prefetch && n && chd_is_device_ptr(e, x) && chd_is_device_ptr(e, z);
     if (f32) {
-        st = widen_upload(e, prefetch ? 1 : 0, (const float*)x, (const float*)z, n, dx, dz, s);
+        st = widen_upload(e, prefetch ? 1 : 0, (const float*)x, (const float*)z, n, p.x, p.z, s);
         if (st != CHD_OK) return st;
     } else if (!in_place) {
-        CU(e, cudaMemcpyAsync(dx, x, sizeof(double) * n, cudaMemcpyDefault, s));
-        CU(e, cudaMemcpyAsync(dz, z, sizeof(double) * n, cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(p.x, x, sizeof(double) * n, cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(p.z, z, sizeof(double) * n, cudaMemcpyDefault, s));
     }
     if (prefetch) {
-        e->pos_n[set] = n;
+        p.n = n;
         return chd_pf_end(e, e->pf_pos);
     }
-    e->pos_x = in_place ? (const double*)x : e->d_x;  // device-resident producer: read in place
-    e->pos_z = in_place ? (const double*)z : e->d_z;
+    e->in_place = in_place ? Positions{(const double*)x, (const double*)z} : Positions{};  // device-resident producer: read in place
     chd_entities_replaced(e, n);
     return CHD_OK;
 }
@@ -221,14 +214,13 @@ chd_status chd_prefetch_entities_f32(chd_engine* e, const float* x, const float*
     return upload_positions(e, "chd_prefetch_entities_f32", x, z, n, true, true);
 }
 
-chd_status chd_entity_buffers(chd_engine* e, double** d_x, double** d_z, uint32_t* n) {
+chd_status chd_entity_buffers(chd_engine* e, double** x, double** z, uint32_t* n) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_not_table(e, "chd_entity_buffers") != CHD_OK) return CHD_ERR_STATE;
-    if (d_x) *d_x = e->d_x;
-    if (d_z) *d_z = e->d_z;
+    if (x) *x = chd_pos_front(e).x;
+    if (z) *z = chd_pos_front(e).z;
     if (n) *n = e->n_own;
-    e->pos_x = e->d_x;
-    e->pos_z = e->d_z;
+    e->in_place = {};
     e->assigned = false;  // the caller may write positions
     e->entities_dirty = true;
     return CHD_OK;
@@ -254,12 +246,6 @@ chd_status chd_set_entity_ids(chd_engine* e, const uint32_t* gid, uint32_t n) {
     e->have_gid = true;
     e->entities_dirty = true;
     return CHD_OK;
-}
-
-// The engine's position buffers are double-buffered for chd_prefetch_entities: remember (outside any graph capture)
-// the last kernel that read the front pair, so an upload into it can be ordered after that read.
-chd_status chd_note_pos_read(chd_engine* e, cudaStream_t s) {
-    return chd_pf_note_read(e, e->pf_pos, e->pos_x == e->d_x ? e->pf_pos.cur : -1, s);
 }
 
 chd_status chd_assign_cells(chd_engine* e) {
@@ -303,17 +289,17 @@ chd_status chd_assign_cells_impl(chd_engine* e, cudaStream_t s) {
     chd_status st = assign_prepare(e, s, &prev, &ho);
     if (st != CHD_OK) return st;
     if (e->n_own) {
-        assign_cells_kernel<<<blocks_for(e->n_own, 256), 256, 0, s>>>(e->g, e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z,
-                                                                      e->n_own, e->d_key, prev, ho, e->assign_bump);
+        const Positions p = chd_positions(e);
+        assign_cells_kernel<<<blocks_for(e->n_own, 256), 256, 0, s>>>(e->g, p.x, p.z, e->n_own, e->d_key, prev, ho, e->assign_bump);
         KCHECK(e);
         e->assign_bump = nullptr;  // consumed
     }
     return CHD_OK;
 }
 
-// part: 0 = the whole build; single-pass builds only: 1 = cell assignment + histogram + scan + CSR offsets, 2 = scatter.  The
-// cell CSR offsets are final after part 1.
-static chd_status build_enqueue(chd_engine* e, cudaStream_t s, bool with_assign, int part = 0) {
+// The cell CSR into copy-input set `out`.  part: 0 = the whole build; single-pass builds only: 1 = cell assignment + histogram +
+// scan + CSR offsets, 2 = scatter.  The cell CSR offsets are final after part 1.
+static chd_status build_enqueue(chd_engine* e, cudaStream_t s, const CopySet& out, bool with_assign, int part = 0) {
     chd_status st;
     FusedAssign fa{};
     const FusedAssign* fap = nullptr;
@@ -324,7 +310,7 @@ static chd_status build_enqueue(chd_engine* e, cudaStream_t s, bool with_assign,
             HandoverOut ho{};
             st = assign_prepare(e, s, &prev, &ho);
             if (st != CHD_OK) return st;
-            fa = FusedAssign{e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z, e->d_key, prev, ho};
+            fa = FusedAssign{chd_positions(e), e->d_key, prev, ho};
             fap = &fa;
         } else {
             st = chd_assign_cells_impl(e, s);
@@ -335,9 +321,9 @@ static chd_status build_enqueue(chd_engine* e, cudaStream_t s, bool with_assign,
     // the entity capacity and blocks beyond the live length idle.
     const uint32_t* n_ptr = e->halo_on_device ? e->d_n_build : nullptr;
     const uint32_t n = e->halo_on_device ? e->lim.max_entities : e->n_own + e->n_halo;
-    const ScatterExtras csr{e->d_cell_start, e->g.cells, &e->d_ctr->n_entities_in_world};
+    const ScatterExtras csr{out.cell_start, e->g.cells, &e->d_ctr->n_entities_in_world};
     // keys are in [0, C]: C marks an out-of-world entity
-    return chd_cell_sort(e, s, e->ent_sort, e->g.cells + 1, e->d_key, e->have_gid ? e->d_gid : nullptr, n, n_ptr, e->d_sorted_key, e->d_sorted_ent,
+    return chd_cell_sort(e, s, e->ent_sort, e->g.cells + 1, e->d_key, e->have_gid ? e->d_gid : nullptr, n, n_ptr, e->d_sorted_key, out.sorted_ent,
                          &csr, e->d_epoch + EP_BUILD, fap, part);
 }
 
@@ -356,7 +342,7 @@ chd_status chd_build_on(chd_engine* e, cudaStream_t s) {
     int set = e->pf_copy.cur;
     chd_status st = e->slab ? CHD_OK : chd_pf_begin(e, e->pf_copy, &set, s);
     if (st != CHD_OK) return st;
-    chd_copy_set_select(e, set);
+    const CopySet& out = e->copy_set[set];
     st = chd_epoch_tick(e, s, EP_BUILD);
     if (st != CHD_OK) return st;
     bool counts_recorded = false;
@@ -364,30 +350,30 @@ chd_status chd_build_on(chd_engine* e, cudaStream_t s) {
         // single-GPU flow: assign + sort as one replayable graph.  The key buffers swap every assignment (handover detection
         // compares against the previous keys); the graph bakes in the sizes, the buffer the new keys go to and the positions.
         const uint64_t key = stage_key(0x6275696c64ull, e->n_own, e->have_gid, e->have_prev_key, e->have_prev_key ? e->d_prev_key : e->d_key,
-                                       e->pos_x, e->pos_z, set);
+                                       chd_positions(e).x, chd_positions(e).z, set);
         // single-pass builds (<= 1023 cells) run as two replayable halves with an event in between: the cell CSR offsets are
         // final after the first (assignment + histogram + scan), so the emit preparation overlaps the scatter
         const bool split = e->g.cells + 1 <= BUILD_MAX_BINS && e->n_own > 0;
-        st = run_stage(e, s, e->g_build, key, [&]() { return build_enqueue(e, s, true, split ? 1 : 0); });
+        st = run_stage(e, s, e->g_build, key, [&]() { return build_enqueue(e, s, out, true, split ? 1 : 0); });
         if (st == CHD_OK && !e->assigned) chd_assign_host(e);  // replayed graph
         if (st == CHD_OK && split) {
             CU(e, cudaEventRecord(e->ev_counts, s));
             counts_recorded = true;
-            st = run_stage(e, s, e->g_build_b, stage_key(key, 0x62), [&]() { return build_enqueue(e, s, false, 2); });
+            st = run_stage(e, s, e->g_build_b, stage_key(key, 0x62), [&]() { return build_enqueue(e, s, out, false, 2); });
         }
         if (st == CHD_OK) st = chd_note_pos_read(e, s);
     } else if (e->assigned && e->halo_on_device) {
         // multi-GPU flow: cells were assigned by chd_export_border and the halo appended on the device; the sort over
         // own + halo entities is sized by capacity (device-side length) and therefore replayable as well.
         const uint64_t key = stage_key(0x736f7274ull, e->lim.max_entities, e->have_gid, e->d_key, set);
-        st = run_stage(e, s, e->g_build, key, [&]() { return build_enqueue(e, s, false); });
+        st = run_stage(e, s, e->g_build, key, [&]() { return build_enqueue(e, s, out, false); });
     } else {
         const bool with_assign = !e->assigned;
-        st = build_enqueue(e, s, with_assign);
+        st = build_enqueue(e, s, out, with_assign);
         if (st == CHD_OK && with_assign) st = chd_note_pos_read(e, s);
     }
     if (st != CHD_OK) return st;
-    st = chd_table_after_build(e, s);  // (entity-table mode only)
+    st = chd_table_after_build(e, s, out);  // (entity-table mode only)
     if (st != CHD_OK) return st;
     if (!counts_recorded) CU(e, cudaEventRecord(e->ev_counts, s));  // (cell counts final = build done)
     if (!e->slab) {

@@ -86,8 +86,9 @@ chd_status follow_generate(chd_engine* e, uint32_t mode, const QueryDev& h, uint
     cudaStream_t s = e->stream;
     StageTimer timer(e, s, CHD_STAGE_FOLLOW);
     const uint32_t S = e->n_slots, B = F.n_bound, H = (uint32_t)host_class(n_h);
-    const FollowEntities ent = e->tbl.on ? FollowEntities{e->d_x, e->d_z, e->lim.max_entities, e->tbl.d_table, e->tbl.bits, e->tbl.d_id_of_slot}
-                                         : FollowEntities{e->pos_x ? e->pos_x : e->d_x, e->pos_z ? e->pos_z : e->d_z, e->n_own, nullptr, 0, nullptr};
+    const Positions p = chd_positions(e);  // (entity-table mode: the front pair)
+    const FollowEntities ent = e->tbl.on ? FollowEntities{p.x, p.z, e->lim.max_entities, e->tbl.d_table, e->tbl.bits, e->tbl.d_id_of_slot}
+                                         : FollowEntities{p.x, p.z, e->n_own, nullptr, 0, nullptr};
     // on a slab (entity-table mode: every followed entity is an own one) the columns it serves, with the world's edges left open
     const uint32_t lo = e->slab && e->g.col_lo > e->g.halo ? e->g.col_lo - e->g.halo : 0u;
     const uint32_t hi = e->slab ? (uint32_t)std::min<uint64_t>((uint64_t)e->g.col_hi + e->g.halo, e->g.cols) : e->g.cols;
@@ -292,7 +293,7 @@ chd_status chd_follow_queries_with(chd_engine* e, uint32_t mode, const chd_query
     CU(e, cudaSetDevice(e->device));
     chd_engine::Follow& F = e->fw;
     const int set = q ? -1 : e->pf_q.cur;  // the adopted prefetch set holding the host part
-    const QueryDev* adopted = q ? nullptr : &e->dq_pf_view[set];
+    const QueryDev* adopted = q ? nullptr : &e->dq_pf[set].view;
     if (q ? !q->sub : !adopted->sub) {
         e->fail("chd_follow_queries_with: the host part is an identity batch (sub == NULL), which cannot be merged");
         return CHD_ERR_INVALID;
@@ -311,7 +312,7 @@ chd_status chd_follow_queries_with(chd_engine* e, uint32_t mode, const chd_query
         st = chd_upload_queries(e, e->stream, q, &h, true, nullptr, &spots);  // into the query scratch, which the merge reads on the same stream
     } else if (adopted) {  // ordered after the upload like any reader of an adopted set, whether or not the part is empty
         h = *adopted;
-        spots = e->dq_pf_spots[set];
+        spots = e->dq_pf[set].spots;
         st = chd_pf_wait(e, e->pf_q, e->stream);
     }
     if (st != CHD_OK) return st;

@@ -16,7 +16,7 @@ chd_status chd_prefetch_queries(chd_engine* e, const chd_query_batch* q) {
     if (st != CHD_OK) return st;
     chd_engine::QStage& qs = e->dq_pf[set];
     if (!qs.spot_dist && !alloc_qstage(e, qs)) return CHD_ERR_CUDA;  // (spot_dist is allocated last)
-    st = chd_upload_queries(e, e->up_stream, q, &e->dq_pf_view[set], true, &qs, &e->dq_pf_spots[set]);
+    st = chd_upload_queries(e, e->up_stream, q, &qs.view, true, &qs, &qs.spots);
     return st != CHD_OK ? st : chd_pf_end(e, e->pf_q);
 }
 
@@ -306,7 +306,7 @@ chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query
             return CHD_ERR_STATE;
         }
         pf_set = e->pf_q.cur;
-        d = e->dq_pf_view[pf_set];
+        d = e->dq_pf[pf_set].view;
         e->pf_q.cur = -1;  // consumed
         if (d.n > e->n_slots && !d.sub) {
             e->fail("identity query batch (sub == NULL) of %u queries > %u subscribers", d.n, e->n_slots);

@@ -141,12 +141,13 @@ chd_status chd_get_cells(chd_engine* e, uint32_t* cell_start, uint32_t* sorted_e
     CU(e, cudaSetDevice(e->device));
     CU(e, chd_copy_wait(e));
     const uint32_t C = e->g.cells;
-    if (cell_start) CU(e, cudaMemcpyAsync(cell_start, e->d_cell_start, sizeof(uint32_t) * ((uint64_t)C + 1), cudaMemcpyDefault, e->stream));
+    const CopySet& c = chd_copy_in(e);
+    if (cell_start) CU(e, cudaMemcpyAsync(cell_start, c.cell_start, sizeof(uint32_t) * ((uint64_t)C + 1), cudaMemcpyDefault, e->stream));
     if (sorted_entity) {
         uint32_t nin = 0;
-        chd_status st = chd_read_u32(e, e->d_cell_start + C, &nin);
+        chd_status st = chd_read_u32(e, c.cell_start + C, &nin);
         if (st != CHD_OK) return st;
-        CU(e, cudaMemcpyAsync(sorted_entity, chd_sorted_out(e), sizeof(uint32_t) * nin, cudaMemcpyDefault, e->stream));
+        CU(e, cudaMemcpyAsync(sorted_entity, chd_sorted_out(e, c), sizeof(uint32_t) * nin, cudaMemcpyDefault, e->stream));
     }
     CU(e, cudaStreamSynchronize(e->stream));
     return CHD_OK;
@@ -387,10 +388,10 @@ chd_status chd_fetch_results_delta(chd_engine* e, const chd_result_buffers* b, c
         const uint32_t n = e->last_nq < b->status_cap ? e->last_nq : b->status_cap;
         CU(e, cudaMemcpyAsync(b->query_status, e->d_status, sizeof(uint32_t) * n, cudaMemcpyDefault, s));
     }
-    if (b->cell_start) CU(e, cudaMemcpyAsync(b->cell_start, e->d_cell_start, sizeof(uint32_t) * ((uint64_t)e->g.cells + 1), cudaMemcpyDefault, s));
+    if (b->cell_start) CU(e, cudaMemcpyAsync(b->cell_start, chd_copy_in(e).cell_start, sizeof(uint32_t) * ((uint64_t)e->g.cells + 1), cudaMemcpyDefault, s));
     if (b->sorted_entity) {
         if (ca.n_entities_in_world > b->entity_cap) return drain(CHD_ERR_CAPACITY);
-        CU(e, cudaMemcpyAsync(b->sorted_entity, chd_sorted_out(e), sizeof(uint32_t) * (uint64_t)ca.n_entities_in_world, cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(b->sorted_entity, chd_sorted_out(e, chd_copy_in(e)), sizeof(uint32_t) * (uint64_t)ca.n_entities_in_world, cudaMemcpyDefault, s));
     }
     cudaStream_t sa = s;  // stream carrying the phase-A copies
     if (early) {  // phase B, on its own stream: its counter read-back must not queue behind the phase-A copies
@@ -521,8 +522,8 @@ chd_status chd_fetch_results_async_delta(chd_engine* e, const chd_result_buffers
     list(HOP_A, e->d_gone_sub, b->unsub_sub, {&ctr->n_unsub, SNAP(a.n_unsub)}, b->diff_cap, 1);
     list(HOP_A, e->d_gone_ch, b->unsub_channel, {&ctr->n_unsub, SNAP(a.n_unsub)}, b->diff_cap, 1);
     list(HOP_A, e->d_status, b->query_status, fixed(std::min<uint64_t>(e->last_nq, b->status_cap)), b->status_cap, 1);
-    list(HOP_A, e->d_cell_start, b->cell_start, fixed(C1), C1, 1);
-    list(HOP_A, chd_sorted_out(e), b->sorted_entity, {&ctr->n_entities_in_world, SNAP(a.n_entities_in_world)}, b->entity_cap, 1);
+    list(HOP_A, chd_copy_in(e).cell_start, b->cell_start, fixed(C1), C1, 1);
+    list(HOP_A, chd_sorted_out(e, chd_copy_in(e)), b->sorted_entity, {&ctr->n_entities_in_world, SNAP(a.n_entities_in_world)}, b->entity_cap, 1);
     list(HOP_A, e->d_ho_entity, b->handover_entity, {&ctr->n_handover, SNAP(a.n_handover)}, hcap, 1);
     list(HOP_A, e->d_ho_src, b->handover_src, {&ctr->n_handover, SNAP(a.n_handover)}, hcap, 1);
     list(HOP_A, e->d_ho_dst, b->handover_dst, {&ctr->n_handover, SNAP(a.n_handover)}, hcap, 1);
@@ -649,8 +650,8 @@ chd_status chd_device_view(chd_engine* e, int which, void** d_ptr, uint64_t* cou
     uint64_t c = 0;
     void* p = nullptr;
     switch (which) {
-        case CHD_VIEW_CELL_START: p = e->d_cell_start; c = (uint64_t)e->g.cells + 2; break;
-        case CHD_VIEW_SORTED_ENTITY: p = (void*)chd_sorted_out(e); c = e->n_sorted; break;
+        case CHD_VIEW_CELL_START: p = chd_copy_in(e).cell_start; c = (uint64_t)e->g.cells + 2; break;
+        case CHD_VIEW_SORTED_ENTITY: p = (void*)chd_sorted_out(e, chd_copy_in(e)); c = e->n_sorted; break;
         case CHD_VIEW_ENT_CELL: p = e->d_key; c = e->n_own + e->n_halo; break;
         case CHD_VIEW_PAIR_OFF: p = pb.off; c = (uint64_t)e->n_slots + 1; break;
         case CHD_VIEW_PAIR_CHANNEL: p = pb.cell; c = e->lim.max_pairs; break;

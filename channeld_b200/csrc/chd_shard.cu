@@ -116,7 +116,8 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
     if (!e->assigned) {
         // replayable: cell assignment + border selection of one tick.  The graph bakes in the sizes, the key buffer the new keys
         // go to, the positions, the ids the records carry, the records, the slab and the exchange path.
-        const uint64_t key = stage_key(0x6578706full, n, e->have_gid, e->have_prev_key, e->have_prev_key ? e->d_prev_key : e->d_key, e->pos_x, e->pos_z,
+        const Positions p = chd_positions(e);
+        const uint64_t key = stage_key(0x6578706full, n, e->have_gid, e->have_prev_key, e->have_prev_key ? e->d_prev_key : e->d_key, p.x, p.z,
                                        ids.own_ids, ids.gid, ids.own, d_records, cap_records, e->g.col_lo, e->g.col_hi, e->g.halo, to_peers);
         st = run_stage(e, s, e->g_export, key, enqueue);
         if (st == CHD_OK && !e->assigned) chd_assign_host(e);  // replayed graph

@@ -177,7 +177,7 @@ chd_status spawn(chd_engine* e, const char* fn, const uint32_t* id_in, const voi
         st = upload_events(e, aid, aslot, &ax, &az);
         if (st != CHD_OK) return st;
         tbl_spawn_kernel<<<grid_for(e, m), TBL_THREADS, 0, e->stream>>>(t.d_table, t.bits, t.d_ev, t.d_ev + m, t.d_ev_pos, t.d_ev_pos + m, (uint32_t)m,
-                                                                       t.d_id_of_slot, e->d_x, e->d_z, t.d_flag);
+                                                                       t.d_id_of_slot, chd_pos_front(e).x, chd_pos_front(e).z, t.d_flag);
         KCHECK(e);
         touched(e);
     }
@@ -195,6 +195,7 @@ chd_status move(chd_engine* e, const char* fn, const uint32_t* id, const void* x
     if (!n) return CHD_OK;
     CU(e, cudaSetDevice(e->device));
     chd_engine::Table& t = e->tbl;
+    const PosSet& front = chd_pos_front(e);
     cudaStream_t s = e->stream;
     StageTimer timer(e, s, CHD_STAGE_ENTITY_EVENTS);
     // host inputs are copied into the event staging, device inputs read in place
@@ -216,9 +217,9 @@ chd_status move(chd_engine* e, const char* fn, const uint32_t* id, const void* x
     tbl_move_resolve_kernel<<<grid, TBL_THREADS, 0, s>>>(t.d_table, t.bits, did, n, t.d_mslot, t.d_winner, t.d_stats);
     KCHECK(e);
     if (f32)
-        tbl_move_apply_kernel<float><<<grid, TBL_THREADS, 0, s>>>(t.d_mslot, t.d_winner, (const float*)dx, (const float*)dz, n, e->d_x, e->d_z, t.d_stats);
+        tbl_move_apply_kernel<float><<<grid, TBL_THREADS, 0, s>>>(t.d_mslot, t.d_winner, (const float*)dx, (const float*)dz, n, front.x, front.z, t.d_stats);
     else
-        tbl_move_apply_kernel<double><<<grid, TBL_THREADS, 0, s>>>(t.d_mslot, t.d_winner, (const double*)dx, (const double*)dz, n, e->d_x, e->d_z, t.d_stats);
+        tbl_move_apply_kernel<double><<<grid, TBL_THREADS, 0, s>>>(t.d_mslot, t.d_winner, (const double*)dx, (const double*)dz, n, front.x, front.z, t.d_stats);
     KCHECK(e);
     touched(e);
     return CHD_OK;
@@ -345,13 +346,12 @@ chd_status chd_entity_table_init(chd_engine* e) {
     uint32_t bits = 4;
     while ((1ull << bits) < 2 * N) bits++;
     const bool ok = dalloc(e, &t.d_table, 1ull << bits) && dalloc(e, &t.d_id_of_slot, N) && dalloc(e, &t.d_snap_id, N) &&
-                    // the padding and alignment of d_sorted_ent (the emit kernels read it), one per copy-input set
+                    // the padding and alignment of sorted_ent (the emit kernels read it), one per copy-input set
                     dalloc(e, &e->copy_set[0].sorted_id, ((N + 3) / 4) * 4 + 8) && dalloc(e, &e->copy_set[1].sorted_id, ((N + 3) / 4) * 4 + 8) &&
                     dalloc(e, &t.d_winner, N) && dalloc(e, &t.d_mslot, N) && dalloc(e, &t.d_ho_tmp, 3 * N) && dalloc(e, &t.d_build_seq, 2) &&
                     dalloc(e, &t.d_flag, N) && dalloc(e, &t.d_stats, 3) && dalloc(e, &t.d_ev, 2 * N) && dalloc(e, &t.d_ev_pos, 2 * N) &&
                     chd_make_event(e, &t.ev_stage[0]) && chd_make_event(e, &t.ev_stage[1]);
     if (!ok) return CHD_ERR_CUDA;
-    t.d_sorted_id = e->copy_set[e->pf_copy.cur].sorted_id;
     cudaStream_t s = e->stream;
     CU(e, cudaMemsetAsync(t.d_table, 0, 8ull << bits, s));
     CU(e, cudaMemsetAsync(t.d_id_of_slot, 0, 4 * N, s));
@@ -361,11 +361,10 @@ chd_status chd_entity_table_init(chd_engine* e) {
     CU(e, cudaMemsetAsync(t.d_stats, 0, 24, s));
     CU(e, cudaMemsetAsync(t.d_build_seq, 0, 8, s));
     CU(e, cudaMemsetAsync(&e->d_ctr->delta_build, 0, 4, s));
-    tbl_park_kernel<<<grid_for(e, N), TBL_THREADS, 0, s>>>(e->d_x, e->d_z, (uint32_t)N);  // every slot starts outside the world
+    tbl_park_kernel<<<grid_for(e, N), TBL_THREADS, 0, s>>>(chd_pos_front(e).x, chd_pos_front(e).z, (uint32_t)N);  // every slot starts outside the world
     KCHECK(e);
     CU(e, cudaStreamSynchronize(s));
-    e->pos_x = e->d_x;
-    e->pos_z = e->d_z;
+    e->in_place = {};
     t.bits = bits;
     t.on = true;
     return CHD_OK;
@@ -383,6 +382,7 @@ chd_status chd_despawn_entities(chd_engine* e, const uint32_t* id_in, uint32_t n
     if (chd_rule_table(e, "chd_despawn_entities") != CHD_OK) return CHD_ERR_STATE;
     CU(e, cudaSetDevice(e->device));
     chd_engine::Table& t = e->tbl;
+    const PosSet& front = chd_pos_front(e);
     std::vector<uint32_t> kid;
     const uint32_t* ids = nullptr;
     chd_status st = host_view(e, id_in, n, kid, &ids);
@@ -423,7 +423,7 @@ chd_status chd_despawn_entities(chd_engine* e, const uint32_t* id_in, uint32_t n
         StageTimer timer(e, e->stream, CHD_STAGE_ENTITY_EVENTS);
         st = upload_events(e, aid, aslot, nullptr, nullptr);
         if (st != CHD_OK) return st;
-        tbl_despawn_kernel<<<grid_for(e, m), TBL_THREADS, 0, e->stream>>>(t.d_table, t.bits, t.d_ev, t.d_ev + m, m, t.d_id_of_slot, e->d_x, e->d_z, t.d_flag);
+        tbl_despawn_kernel<<<grid_for(e, m), TBL_THREADS, 0, e->stream>>>(t.d_table, t.bits, t.d_ev, t.d_ev + m, m, t.d_id_of_slot, front.x, front.z, t.d_flag);
         KCHECK(e);
         touched(e);
     }
@@ -468,6 +468,7 @@ chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank,
     }
     CU(e, cudaSetDevice(e->device));
     chd_engine::Table& t = e->tbl;
+    const PosSet& front = chd_pos_front(e);
     cudaStream_t s = e->stream;
     const uint64_t N = e->lim.max_entities;
     const uint32_t world = e->comm ? (uint32_t)e->comm_world : 1u;
@@ -479,7 +480,7 @@ chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank,
     bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_BORDER);
     KCHECK(e);
     SCAN(e, compact_1p(HandoffFlag{e->g, e->d_key},
-                       HandoffSink{e->g, world, e->d_key, chd_entity_ids(e), e->d_x, e->d_z, d_id, d_slot, d_dst, d_hx, d_hz, e->d_boff}, e->n_own,
+                       HandoffSink{e->g, world, e->d_key, chd_entity_ids(e), front.x, front.z, d_id, d_slot, d_dst, d_hx, d_hz, e->d_boff}, e->n_own,
                        e->site_border, s));
     st = chd_read_u32(e, e->d_boff, count);
     if (st != CHD_OK) return st;
@@ -504,15 +505,15 @@ chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank,
         t.free_fifo.push_back(hslot[j]);
     }
     StageTimer timer(e, s, CHD_STAGE_ENTITY_EVENTS);
-    tbl_despawn_kernel<<<grid_for(e, m), TBL_THREADS, 0, s>>>(t.d_table, t.bits, d_id, d_slot, m, t.d_id_of_slot, e->d_x, e->d_z, t.d_flag);
+    tbl_despawn_kernel<<<grid_for(e, m), TBL_THREADS, 0, s>>>(t.d_table, t.bits, d_id, d_slot, m, t.d_id_of_slot, front.x, front.z, t.d_flag);
     KCHECK(e);
     touched(e);
     return CHD_OK;
 }
 
-// After every table-mode build, on the build's stream: the id-valued copy of the sorted entity array and, after a fresh cell
-// assignment, the handover list in ids without the slots spawned or despawned since the previous one (then the flags clear).
-chd_status chd_table_after_build(chd_engine* e, cudaStream_t s) {
+// After every table-mode build into copy-input set `c`, on the build's stream: its id-valued sorted entity array and, after a fresh
+// cell assignment, the handover list in ids without the slots spawned or despawned since the previous one (then the flags clear).
+chd_status chd_table_after_build(chd_engine* e, cudaStream_t s, const CopySet& c) {
     chd_engine::Table& t = e->tbl;
     if (!t.on) return CHD_OK;
     // on slabs the build's length (own slots + halo records) lives on the device
@@ -520,10 +521,10 @@ chd_status chd_table_after_build(chd_engine* e, cudaStream_t s) {
     const uint32_t n = e->halo_on_device ? e->lim.max_entities : e->n_own + e->n_halo;
     const EntityIds ids = chd_entity_ids(e);
     const bool raw = t.ho_raw;
-    const uint64_t key = stage_key(0x7461626c65ull, n, n_ptr, ids.own, ids.gid, raw, e->d_sorted_ent, t.d_sorted_id, ids.own_ids, e->ho_cap);
+    const uint64_t key = stage_key(0x7461626c65ull, n, n_ptr, ids.own, ids.gid, raw, c.sorted_ent, c.sorted_id, ids.own_ids, e->ho_cap);
     const unsigned grid = (unsigned)e->sm_count * 4;
     chd_status st = run_stage(e, s, t.g_post, key, [&]() -> chd_status {
-        tbl_gather_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(e->d_sorted_ent, ids, n, n_ptr, t.d_sorted_id, t.d_build_seq);
+        tbl_gather_ids_kernel<<<grid, TBL_THREADS, 0, s>>>(c.sorted_ent, ids, n, n_ptr, c.sorted_id, t.d_build_seq);
         KCHECK(e);
         if (!raw) return CHD_OK;
         const HandoverOut ho{e->d_ho_entity, e->d_ho_src, e->d_ho_dst, &e->d_ctr->n_handover, e->ho_cap};

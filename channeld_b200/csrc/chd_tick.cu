@@ -29,18 +29,19 @@ static chd_status emit_prep_enqueue(chd_engine* e, cudaStream_t s, bool cta_tile
     const unsigned grid = (unsigned)e->sm_count * 8;
     const uint32_t tile = cta_tiles ? (uint32_t)EMIT_TILE : (uint32_t)EMIT_WARP_TILE;
     const int set = e->pf_copy.cur;
+    const CopySet& c = chd_copy_in(e);
     const uint64_t key = stage_key(0x656d6974ull, S, e->cur, cta_tiles, s, set);
     // the preparation rewrites its copy-input set: after the last copy kernel that read it (a tick without a build reuses the set
     // of the copy before it; after a build this is the copy the build already waited for)
-    if (e->pf_copy.read_recorded[set]) CU(e, cudaStreamWaitEvent(s, e->pf_copy.ev_read[set], 0));
-    chd_status st = chd_epoch_tick(e, s, EP_EMIT);
+    chd_status st = chd_pf_after_read(e, e->pf_copy, set, s);
+    if (st == CHD_OK) st = chd_epoch_tick(e, s, EP_EMIT);
     if (st != CHD_OK) return st;
     return run_stage(e, s, e->g_emit_prep, key, [&]() -> chd_status {
         // per-pair visible counts are computed by the scan itself; the partition pass opens the next epoch
-        SCAN(e, exclusive_scan_fn<PairVcountIn, uint64_t>(PairVcountIn{pb.cell, e->d_cell_start}, e->d_voff, P, e->site_voff, s, pb.off + S));
-        emit_partition_kernel<<<grid, 256, 0, s>>>(pb.off + S, P, e->d_voff, pb.cell, e->d_cell_start, e->d_first_pair, cta_tiles ? e->d_tile_desc : nullptr,
+        SCAN(e, exclusive_scan_fn<PairVcountIn, uint64_t>(PairVcountIn{pb.cell, c.cell_start}, c.voff, P, e->site_voff, s, pb.off + S));
+        emit_partition_kernel<<<grid, 256, 0, s>>>(pb.off + S, P, c.voff, pb.cell, c.cell_start, c.first_pair, cta_tiles ? c.tile_desc : nullptr,
                                                    e->max_tiles, S, pb.off, e->d_vis_off, e->lim.max_visible, e->d_ctr, e->d_epoch + EP_EMIT, tile,
-                                                   e->d_general_tiles, e->d_n_general, e->copy_set[set].n_visible);
+                                                   c.general_tiles, c.n_general, c.n_visible);
         KCHECK(e);
         return CHD_OK;
     });
@@ -52,7 +53,7 @@ static chd_status emit_kernel_enqueue(chd_engine* e, cudaStream_t s, bool cta_ti
     const uint32_t S = e->n_slots;
     const uint64_t P = e->lim.max_pairs;
     const int set = e->pf_copy.cur;
-    const unsigned long long* V = e->copy_set[set].n_visible;
+    const CopySet& c = chd_copy_in(e);
     chd_status st = chd_pf_wait(e, e->pf_copy, s);
     if (st != CHD_OK) return st;
     {
@@ -66,14 +67,14 @@ static chd_status emit_kernel_enqueue(chd_engine* e, cudaStream_t s, bool cta_ti
         if (tiles == 0) tiles = 1;
         if (tiles > 0x7fffffffull) tiles = 0x7fffffffull;
         tiles = (tiles + EMIT_TILES_PER_CTA - 1) / EMIT_TILES_PER_CTA;
-        emit_visible_kernel<<<(unsigned)tiles, EMIT_THREADS, CHD_EMIT_DYN_SMEM, s>>>(V, chd_sorted_out(e), e->d_tile_desc, e->d_vis, e->lim.max_visible);
+        emit_visible_kernel<<<(unsigned)tiles, EMIT_THREADS, CHD_EMIT_DYN_SMEM, s>>>(c.n_visible, chd_sorted_out(e, c), c.tile_desc, e->d_vis, e->lim.max_visible);
         KCHECK(e);
-        emit_visible_general_kernel<<<(unsigned)e->sm_count * 2, EMIT_THREADS, 0, s>>>(e->d_general_tiles, e->d_n_general, pb.off + S, P, V,
-                                                                                       e->d_voff, pb.cell, e->d_cell_start, chd_sorted_out(e),
-                                                                                       e->d_first_pair, e->d_vis, e->lim.max_visible);
+        emit_visible_general_kernel<<<(unsigned)e->sm_count * 2, EMIT_THREADS, 0, s>>>(c.general_tiles, c.n_general, pb.off + S, P, c.n_visible,
+                                                                                       c.voff, pb.cell, c.cell_start, chd_sorted_out(e, c),
+                                                                                       c.first_pair, e->d_vis, e->lim.max_visible);
     } else {
-        emit_visible_warp_kernel<<<(unsigned)e->sm_count * 4, EMIT_THREADS, 0, s>>>(pb.off + S, P, e->d_voff, pb.cell, e->d_cell_start, chd_sorted_out(e),
-                                                                                    e->d_first_pair, e->d_vis, e->lim.max_visible);
+        emit_visible_warp_kernel<<<(unsigned)e->sm_count * 4, EMIT_THREADS, 0, s>>>(pb.off + S, P, c.voff, pb.cell, c.cell_start, chd_sorted_out(e, c),
+                                                                                    c.first_pair, e->d_vis, e->lim.max_visible);
     }
     KCHECK(e);
     }
@@ -379,11 +380,8 @@ chd_status chd_adopt_prefetched(chd_engine* e) {
     if (!chd_pf_adopt(e->pf_pos)) return CHD_OK;
     chd_status st = chd_pf_wait(e, e->pf_pos, e->stream);
     if (st != CHD_OK) return st;
-    e->d_x = e->d_xb[e->pf_pos.cur];
-    e->d_z = e->d_zb[e->pf_pos.cur];
-    e->pos_x = e->d_x;
-    e->pos_z = e->d_z;
-    chd_entities_replaced(e, e->pos_n[e->pf_pos.cur]);
+    e->in_place = {};
+    chd_entities_replaced(e, chd_pos_front(e).n);
     return CHD_OK;
 }
 
