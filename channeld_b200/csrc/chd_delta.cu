@@ -108,7 +108,6 @@ chd_status chd_delta_on(chd_engine* e, cudaStream_t s) {
 
 // The first reserve picks the mode (ids: id mode over [0, id_space)) and allocates; every later one only grows the lists.
 static chd_status delta_reserve(chd_engine* e, uint64_t cap_entries, bool ids, uint32_t id_space) {
-    CU(e, cudaSetDevice(e->device));
     // a delta of an earlier tick may still be running (on the engine stream or, inside a tick, on prep_stream)
     CU(e, cudaStreamSynchronize(e->stream));
     CU(e, cudaStreamSynchronize(e->prep_stream));
@@ -153,21 +152,23 @@ static chd_status delta_reserve(chd_engine* e, uint64_t cap_entries, bool ids, u
 chd_status chd_reserve_visible_delta(chd_engine* e, uint64_t cap_entries) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_index_delta(e) != CHD_OK) return CHD_ERR_STATE;
+    CHD_ENTER(e, ENTRY_DEVICE);
     return delta_reserve(e, cap_entries, e->dl.ids, e->dl.id_space);  // (id mode: grows the lists only)
 }
 
 chd_status chd_reserve_visible_delta_ids(chd_engine* e, uint64_t cap_entries, uint32_t id_space) {
     if (!e || id_space == 0) return CHD_ERR_INVALID;
     const chd_status st = chd_rule_id_delta(e, id_space);
-    return st != CHD_OK ? st : delta_reserve(e, cap_entries, true, id_space);
+    if (st != CHD_OK) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    return delta_reserve(e, cap_entries, true, id_space);
 }
 
 chd_status chd_visible_delta(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_delta_check(e, false) != CHD_OK) return CHD_ERR_STATE;
-    CU(e, cudaSetDevice(e->device));
-    const chd_status st = chd_fetch_guard(e, e->stream);
-    return st != CHD_OK ? st : chd_delta_on(e, e->stream);
+    CHD_ENTER(e, ENTRY_FETCH_GUARD);
+    return chd_delta_on(e, e->stream);
 }
 
 chd_status chd_read_delta_lengths(chd_engine* e, cudaStream_t s, DeltaLengths* out) {
@@ -190,8 +191,7 @@ chd_status chd_get_visible_delta(chd_engine* e, uint64_t* enter_off, uint32_t* e
         e->fail("chd_get_visible_delta before chd_reserve_visible_delta");
         return CHD_ERR_STATE;
     }
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     cudaStream_t s = e->stream;  // (a tick's delta on prep_stream is joined into the engine stream)
     const uint32_t S = D.n_out;
     DeltaLengths dn;

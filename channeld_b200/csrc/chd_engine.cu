@@ -105,6 +105,14 @@ cudaError_t chd_copy_wait(chd_engine* e) {
     return r;
 }
 
+chd_status chd_enter(chd_engine* e, unsigned needs, std::unique_lock<std::recursive_mutex>& lock) {
+    if (needs & ENTRY_LOCK) lock = std::unique_lock<std::recursive_mutex>(e->mu);
+    if (!(needs & (ENTRY_DEVICE | ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD))) return CHD_OK;
+    CU(e, cudaSetDevice(e->device));
+    if (needs & ENTRY_COPY_WAIT) CU(e, chd_copy_wait(e));
+    return needs & ENTRY_FETCH_GUARD ? chd_fetch_guard(e, e->stream) : CHD_OK;
+}
+
 chd_status chd_read_u32(chd_engine* e, const uint32_t* d, uint32_t* v) {
     CU(e, cudaMemcpyAsync(e->h_get, d, 4, cudaMemcpyDeviceToHost, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
@@ -170,6 +178,7 @@ void chd_free_pinned(void* p) {
 
 void chd_destroy(chd_engine* e) {
     if (!e) return;
+    // device and copy wait without CHD_ENTER: the engine is released whatever fails (a void call has no status to return)
     cudaSetDevice(e->device);
     if (e->stream) {
         chd_copy_wait(e);
@@ -378,7 +387,7 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
 
 chd_status chd_set_stream(chd_engine* e, void* cuda_stream) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     CU(e, cudaStreamSynchronize(e->stream));
     if (e->own_stream) {
         cudaStreamDestroy(e->stream);
@@ -390,8 +399,7 @@ chd_status chd_set_stream(chd_engine* e, void* cuda_stream) {
 
 chd_status chd_sync(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     CU(e, cudaStreamSynchronize(e->stream));
     return CHD_OK;
 }
@@ -402,6 +410,7 @@ uint64_t chd_launch_count(const chd_engine* e) { return e ? e->n_launch : 0; }
 
 chd_status chd_enable_graphs(chd_engine* e, int on) {
     if (!e) return CHD_ERR_INVALID;
+    CHD_ENTER(e, 0);
     e->use_graphs = on != 0;
     return CHD_OK;
 }
@@ -410,8 +419,7 @@ uint64_t chd_graph_launch_count(const chd_engine* e) { return e ? e->graph_launc
 
 chd_status chd_profile_enable(chd_engine* e, int on) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     if (on && !e->ev) {
         const size_t n = (size_t)CHD_STAGE_COUNT * chd_engine::EV_RING * 2;
         e->ev = new cudaEvent_t[n]();
@@ -425,8 +433,7 @@ chd_status chd_profile_enable(chd_engine* e, int on) {
 
 chd_status chd_profile_timeline(chd_engine* e, int stage, double* start_ms, double* stop_ms) {
     if (!e || stage < 0 || stage >= CHD_STAGE_COUNT || !start_ms || !stop_ms || !e->ev) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     CU(e, cudaStreamSynchronize(e->stream));
     CU(e, cudaStreamSynchronize(e->aux_stream));
     if (!e->stage_n[CHD_STAGE_TICK] || !e->stage_n[stage]) return CHD_ERR_STATE;
@@ -441,8 +448,7 @@ chd_status chd_profile_timeline(chd_engine* e, int stage, double* start_ms, doub
 
 chd_status chd_profile_get(chd_engine* e, int stage, double* total_ms, uint64_t* samples) {
     if (!e || stage < 0 || stage >= CHD_STAGE_COUNT || !total_ms || !samples) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     CU(e, cudaStreamSynchronize(e->stream));
     const uint64_t n = e->stage_n[stage];
     const uint64_t m = n < (uint64_t)chd_engine::EV_RING ? n : (uint64_t)chd_engine::EV_RING;

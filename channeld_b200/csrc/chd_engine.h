@@ -444,6 +444,23 @@ struct chd_engine {
         CU(e, cudaGetLastError());                    \
     } while (0)
 
+// What an entry point of include/chd_gpu.h needs before it touches the engine.  Each one declares it once, with CHD_ENTER after
+// its argument and mode-rule checks, and the steps always run in the order of the list:
+//   ENTRY_LOCK         holds e->mu until the entry point returns: the entry points that may run on any thread (chd_cell_of*,
+//                      chd_query_channel_ids, chd_adjacent_broadcast) and those that share state with them: h_u32, the query
+//                      scratch, the engine stream while a graph is being captured (run_stage).
+//   ENTRY_DEVICE       makes e->device the calling thread's current device: every entry point that makes a CUDA call.
+//   ENTRY_COPY_WAIT    chd_copy_wait: every entry point that reads the expanded list, hands out device memory, rewrites something
+//                      the pending copy kernel reads or is a documented completion point (chd_sync, chd_summary, the getters).
+//   ENTRY_FETCH_GUARD  chd_fetch_guard on the engine stream: every entry point that rewrites arrays an outstanding asynchronous
+//                      read-back may still be copying.
+// COPY_WAIT and FETCH_GUARD imply DEVICE, and CHD_ENTER(e, 0) marks an entry point that needs none.  A failed step returns CHD_ERR_CUDA.
+enum : unsigned { ENTRY_DEVICE = 1, ENTRY_LOCK = 2, ENTRY_COPY_WAIT = 4, ENTRY_FETCH_GUARD = 8 };
+chd_status chd_enter(chd_engine* e, unsigned needs, std::unique_lock<std::recursive_mutex>& lock);  // CHD_ENTER's steps
+#define CHD_ENTER(e, needs)                                   \
+    std::unique_lock<std::recursive_mutex> chd_entry_lock_;   \
+    if (const chd_status chd_entry_st_ = chd_enter((e), (needs), chd_entry_lock_); chd_entry_st_ != CHD_OK) return chd_entry_st_
+
 struct StageTimer {  // records a CUDA-event pair around a stage on stream `s` when profiling is on
     chd_engine* e;
     cudaStream_t s;
@@ -532,7 +549,7 @@ chd_status chd_pf_note_read(chd_engine* e, Prefetch& p, int set, cudaStream_t s)
 chd_status chd_pf_after_read(chd_engine* e, const Prefetch& p, int set, cudaStream_t s);
 chd_status chd_read_u32(chd_engine* e, const uint32_t* d, uint32_t* v);
 // Orders the engine stream after the copy kernel a two-stream chd_tick left running on copy_stream (device-side, no host sync).
-// Every entry point that reads the expanded list, hands out device memory or is a documented completion point calls it first.
+// Which entry points call it: ENTRY_COPY_WAIT.
 cudaError_t chd_copy_wait(chd_engine* e);
 chd_status chd_decode_summary(chd_engine* e, chd_tick_summary* out);
 chd_status chd_assign_cells_impl(chd_engine* e, cudaStream_t s);

@@ -105,8 +105,7 @@ chd_status chd_cell_of(chd_engine* e, const double* x, const double* z, uint32_t
 
 chd_status chd_cell_of_valid(chd_engine* e, const double* x, const double* z, uint32_t n, uint32_t* out, uint8_t* out_valid) {
     if (!e || (n && (!x || !z || !out))) return CHD_ERR_INVALID;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     // chunked through the tmp buffers (they are free outside chd_build)
     double *dx = nullptr, *dz = nullptr;
     uint32_t* dk = nullptr;
@@ -167,16 +166,20 @@ void chd_entities_replaced(chd_engine* e, uint32_t n) {
     e->entities_dirty = true;
 }
 
-// Every position upload, f64 or f32: into the front pair on the engine stream (set), or into the pair the next prefetch fills on
-// up_stream (prefetch).  Device-resident doubles given to a set are read in place.
-static chd_status upload_positions(chd_engine* e, const char* fn, const void* x, const void* z, uint32_t n, bool f32, bool prefetch) {
+// argument checks of every position upload
+static chd_status check_positions(chd_engine* e, const char* fn, const void* x, const void* z, uint32_t n) {
     if (!e || (n && (!x || !z))) return CHD_ERR_INVALID;
     if (chd_rule_not_table(e, fn) != CHD_OK) return CHD_ERR_STATE;
     if (n > e->lim.max_entities) {
         e->fail("%s: %u > max_entities %u", fn, n, e->lim.max_entities);
         return CHD_ERR_CAPACITY;
     }
-    CU(e, cudaSetDevice(e->device));
+    return CHD_OK;
+}
+
+// Every position upload, f64 or f32: into the front pair on the engine stream (set), or into the pair the next prefetch fills on
+// up_stream (prefetch).  Device-resident doubles given to a set are read in place.
+static chd_status upload_positions(chd_engine* e, const void* x, const void* z, uint32_t n, bool f32, bool prefetch) {
     int set = e->pf_pos.cur;
     chd_status st = prefetch ? chd_pf_begin(e, e->pf_pos, &set) : CHD_OK;
     if (st != CHD_OK) return st;
@@ -202,21 +205,34 @@ static chd_status upload_positions(chd_engine* e, const char* fn, const void* x,
 }
 
 chd_status chd_set_entities(chd_engine* e, const double* x, const double* z, uint32_t n) {
-    return upload_positions(e, "chd_set_entities", x, z, n, false, false);
+    const chd_status st = check_positions(e, "chd_set_entities", x, z, n);
+    if (st != CHD_OK) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    return upload_positions(e, x, z, n, false, false);
 }
 chd_status chd_prefetch_entities(chd_engine* e, const double* x, const double* z, uint32_t n) {
-    return upload_positions(e, "chd_prefetch_entities", x, z, n, false, true);
+    const chd_status st = check_positions(e, "chd_prefetch_entities", x, z, n);
+    if (st != CHD_OK) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    return upload_positions(e, x, z, n, false, true);
 }
 chd_status chd_set_entities_f32(chd_engine* e, const float* x, const float* z, uint32_t n) {
-    return upload_positions(e, "chd_set_entities_f32", x, z, n, true, false);
+    const chd_status st = check_positions(e, "chd_set_entities_f32", x, z, n);
+    if (st != CHD_OK) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    return upload_positions(e, x, z, n, true, false);
 }
 chd_status chd_prefetch_entities_f32(chd_engine* e, const float* x, const float* z, uint32_t n) {
-    return upload_positions(e, "chd_prefetch_entities_f32", x, z, n, true, true);
+    const chd_status st = check_positions(e, "chd_prefetch_entities_f32", x, z, n);
+    if (st != CHD_OK) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    return upload_positions(e, x, z, n, true, true);
 }
 
 chd_status chd_entity_buffers(chd_engine* e, double** x, double** z, uint32_t* n) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_not_table(e, "chd_entity_buffers") != CHD_OK) return CHD_ERR_STATE;
+    CHD_ENTER(e, 0);
     if (x) *x = chd_pos_front(e).x;
     if (z) *z = chd_pos_front(e).z;
     if (n) *n = e->n_own;
@@ -229,6 +245,7 @@ chd_status chd_entity_buffers(chd_engine* e, double** x, double** z, uint32_t* n
 chd_status chd_set_entity_count(chd_engine* e, uint32_t n) {
     if (!e || n > e->lim.max_entities) return CHD_ERR_INVALID;
     if (chd_rule_not_table(e, "chd_set_entity_count") != CHD_OK) return CHD_ERR_STATE;
+    CHD_ENTER(e, 0);
     chd_entities_replaced(e, n);
     return CHD_OK;
 }
@@ -236,7 +253,7 @@ chd_status chd_set_entity_count(chd_engine* e, uint32_t n) {
 chd_status chd_set_entity_ids(chd_engine* e, const uint32_t* gid, uint32_t n) {
     if (!e || n > e->lim.max_entities) return CHD_ERR_INVALID;
     if (chd_rule_not_table(e, "chd_set_entity_ids") != CHD_OK) return CHD_ERR_STATE;
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     e->delta_blocked = true;  // global ids: the multi-GPU flow (index-mode visible deltas are single-GPU only)
     if (!gid) {
         e->have_gid = false;
@@ -250,10 +267,7 @@ chd_status chd_set_entity_ids(chd_engine* e, const uint32_t* gid, uint32_t n) {
 
 chd_status chd_assign_cells(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
-    {
-        chd_status gs_ = chd_fetch_guard(e, e->stream);
-        if (gs_ != CHD_OK) return gs_;
-    }
+    CHD_ENTER(e, ENTRY_FETCH_GUARD);
     const bool was_assigned = e->assigned;
     chd_status st = chd_assign_cells_impl(e, e->stream);
     if (st == CHD_OK && !was_assigned) st = chd_note_pos_read(e, e->stream);
@@ -282,7 +296,6 @@ static chd_status assign_prepare(chd_engine* e, cudaStream_t s, uint32_t** prev_
 }
 
 chd_status chd_assign_cells_impl(chd_engine* e, cudaStream_t s) {
-    CU(e, cudaSetDevice(e->device));
     if (e->assigned) return CHD_OK;
     uint32_t* prev = nullptr;
     HandoverOut ho{};
@@ -329,10 +342,8 @@ static chd_status build_enqueue(chd_engine* e, cudaStream_t s, const CopySet& ou
 
 chd_status chd_build(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
-    chd_status st = chd_fetch_guard(e, e->stream);
-    return st != CHD_OK ? st : chd_build_on(e, e->stream);
+    CHD_ENTER(e, ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
+    return chd_build_on(e, e->stream);
 }
 
 chd_status chd_build_on(chd_engine* e, cudaStream_t s) {

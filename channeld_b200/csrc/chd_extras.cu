@@ -12,8 +12,7 @@ extern "C" {
 chd_status chd_due_classes(chd_engine* e, uint32_t* out_class_of, uint32_t* out_class_rep, uint32_t* out_class_count, uint32_t cap_classes,
                            uint32_t* out_n_classes) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     cudaStream_t s = e->stream;
     uint32_t n_due = 0;
     chd_status st = chd_read_u32(e, &e->d_ctr->n_due, &n_due);
@@ -75,8 +74,7 @@ __global__ void bcast_msgoff_kernel(const uint32_t* __restrict__ off9, uint32_t 
 
 chd_status chd_set_subscriber_types(chd_engine* e, const uint8_t* conn_type, uint32_t n) {
     if (!e || n > e->lim.max_subscribers) return CHD_ERR_INVALID;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     if (!conn_type) {
         e->have_conn_type = false;
         return CHD_OK;
@@ -92,13 +90,11 @@ chd_status chd_set_subscriber_types(chd_engine* e, const uint8_t* conn_type, uin
 chd_status chd_adjacent_broadcast(chd_engine* e, const chd_broadcast_batch* b, uint32_t* out_status, uint32_t* out_off, uint32_t* out_slot,
                                   uint64_t cap) {
     if (!e || !b || (b->n && (!b->channel_id || !b->broadcast)) || !out_off) return CHD_ERR_INVALID;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
     if (e->interest_pending) {
         e->fail("chd_adjacent_broadcast while a chd_begin_interest is pending (call chd_tick first)");
         return CHD_ERR_STATE;
     }
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT);
     const uint32_t n = b->n;
     if (out_status)
         for (uint32_t m = 0; m < n; m++)

@@ -5,8 +5,7 @@
 // tick is in flight): the generation runs on the engine stream, and the interest update that reads the batch is either on the
 // engine stream too or on the second stream between the tick's fork and its join, which the engine stream waits for before the
 // tick ends.  A generation enqueued after that tick is therefore ordered after the last read of the batch; while a
-// chd_begin_interest is pending (forked, not joined yet) chd_follow_queries is refused.  The generation writes follower-owned
-// arrays only, none of which an asynchronous read-back copies, so it needs no chd_fetch_guard.  A merged generation
+// chd_begin_interest is pending (forked, not joined yet) chd_follow_queries is refused.  A merged generation
 // (chd_follow_queries_with) also reads the host part, from the query scratch or an adopted prefetch set, on the same stream; it
 // copies everything into follower-owned arrays, so the prefetch set is released right after it.
 #include "chd_engine.h"
@@ -171,8 +170,7 @@ chd_status chd_follow_bind(chd_engine* e, const chd_follow_batch* b) {
     if (chd_rule_follow(e, "chd_follow_bind") != CHD_OK) return CHD_ERR_STATE;
     const uint32_t n = b->n;
     if (!n) return CHD_OK;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     // argument checks first: a refused call binds nothing
     std::unordered_map<uint32_t, uint32_t> last;  // slot -> its last binding in the call
     last.reserve(n);
@@ -268,8 +266,7 @@ chd_status chd_follow_unbind(chd_engine* e, const uint32_t* slot, uint32_t n) {
     if (!e || (n && !slot)) return CHD_ERR_INVALID;
     if (chd_rule_follow(e, "chd_follow_unbind") != CHD_OK) return CHD_ERR_STATE;
     if (!n) return CHD_OK;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     for (uint32_t i = 0; i < n; i++)
         if (slot[i] >= e->lim.max_subscribers) {
             e->fail("chd_follow_unbind: slot %u >= max_subscribers %u", slot[i], e->lim.max_subscribers);
@@ -281,16 +278,14 @@ chd_status chd_follow_unbind(chd_engine* e, const uint32_t* slot, uint32_t n) {
 chd_status chd_follow_queries(chd_engine* e, uint32_t mode) {
     if (!e || (mode != CHD_FOLLOW_ALL && mode != CHD_FOLLOW_MOVED)) return CHD_ERR_INVALID;
     if (chd_rule_follow(e, "chd_follow_queries") != CHD_OK || chd_rule_one_batch(e, "chd_follow_queries") != CHD_OK) return CHD_ERR_STATE;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     return follow_generate(e, mode, QueryDev{}, 0, 0);
 }
 
 chd_status chd_follow_queries_with(chd_engine* e, uint32_t mode, const chd_query_batch* q) {
     if (!e || (mode != CHD_FOLLOW_ALL && mode != CHD_FOLLOW_MOVED)) return CHD_ERR_INVALID;
     if (chd_rule_follow(e, "chd_follow_queries_with") != CHD_OK || chd_rule_merged_batch(e, !q) != CHD_OK) return CHD_ERR_STATE;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     chd_engine::Follow& F = e->fw;
     const int set = q ? -1 : e->pf_q.cur;  // the adopted prefetch set holding the host part
     const QueryDev* adopted = q ? nullptr : &e->dq_pf[set].view;
@@ -335,9 +330,7 @@ chd_status chd_get_follow(chd_engine* e, uint32_t* slot, uint32_t* entity, uint3
     if (count) *count = 0;
     if (n_selected) *n_selected = 0;
     if (!F.on || !F.n_bound) return CHD_OK;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT);
     cudaStream_t s = e->stream;
     const uint64_t Q = e->lim.max_queries;
     if (!F.g_count && !(dalloc(e, &F.g_slot, Q) && dalloc(e, &F.g_entity, Q) && dalloc(e, &F.g_status, Q) && dalloc(e, &F.g_cx, Q) && dalloc(e, &F.g_cz, Q) &&

@@ -9,8 +9,7 @@ extern "C" {
 
 chd_status chd_prefetch_queries(chd_engine* e, const chd_query_batch* q) {
     if (!e || !q) return CHD_ERR_INVALID;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     int set = 0;
     chd_status st = chd_pf_begin(e, e->pf_q, &set);
     if (st != CHD_OK) return st;
@@ -28,8 +27,7 @@ chd_status chd_set_subscribers(chd_engine* e, const uint32_t* conn_id, uint32_t 
         e->fail("chd_set_subscribers: %u > max_subscribers %u", n, e->lim.max_subscribers);
         return CHD_ERR_CAPACITY;
     }
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     CU(e, cudaMemcpyAsync(e->d_conn, conn_id, sizeof(uint32_t) * n, cudaMemcpyDefault, e->stream));
     CU(e, cudaMemsetAsync(e->pairs[0].off, 0, ((uint64_t)e->lim.max_subscribers + 1) * 4, e->stream));
     CU(e, cudaMemsetAsync(e->pairs[1].off, 0, ((uint64_t)e->lim.max_subscribers + 1) * 4, e->stream));
@@ -64,7 +62,7 @@ static chd_status upload_slot_list(chd_engine* e, const uint32_t* slot, const ui
 
 chd_status chd_grow_slots(chd_engine* e, uint32_t new_n) {
     if (new_n <= e->n_slots) return CHD_OK;
-    CU(e, chd_copy_wait(e));  // the copy kernel reads the pair offsets
+    CU(e, chd_copy_wait(e));  // only when the table grows: the copy kernel reads the pair offsets
     const uint32_t old_n = e->n_slots;
     extend_offsets_kernel<<<blocks_for(new_n - old_n, 256), 256, 0, e->stream>>>(e->pairs[e->cur].off, old_n, new_n);
     KCHECK(e);
@@ -76,8 +74,7 @@ chd_status chd_grow_slots(chd_engine* e, uint32_t new_n) {
 chd_status chd_add_subscribers(chd_engine* e, const uint32_t* slot, const uint32_t* conn_id, uint32_t n) {
     if (!e || (n && (!slot || !conn_id))) return CHD_ERR_INVALID;
     if (n == 0) return CHD_OK;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     uint32_t max_slot = 0;
     chd_status st = upload_slot_list(e, slot, conn_id, n, &max_slot);
     if (st != CHD_OK) return st;
@@ -92,8 +89,7 @@ chd_status chd_add_subscribers(chd_engine* e, const uint32_t* slot, const uint32
 chd_status chd_remove_subscribers(chd_engine* e, const uint32_t* slot, uint32_t n) {
     if (!e || (n && !slot)) return CHD_ERR_INVALID;
     if (n == 0) return CHD_OK;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     uint32_t max_slot = 0;
     chd_status st = upload_slot_list(e, slot, nullptr, n, &max_slot);
     if (st != CHD_OK) return st;
@@ -187,8 +183,7 @@ static chd_status run_query_kernel(chd_engine* e, cudaStream_t s, const QueryDev
 chd_status chd_query_channel_ids(chd_engine* e, const chd_query_batch* q, uint32_t* out_status, uint32_t* out_off,
                                  uint32_t* out_channel_id, uint32_t* out_dist, uint64_t cap) {
     if (!e || !q) return CHD_ERR_INVALID;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     CU(e, cudaStreamSynchronize(e->aux_stream));  // an in-flight interest update shares the query scratch
     QueryDev d;
     chd_status st = chd_upload_queries(e, e->stream, q, &d, false);
@@ -285,10 +280,8 @@ static chd_status interest_enqueue(chd_engine* e, cudaStream_t s, const QueryDev
 
 chd_status chd_update_interest(chd_engine* e, const chd_query_batch* q, int64_t now_ns) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
-    chd_status st = chd_fetch_guard(e, e->stream);
-    return st != CHD_OK ? st : chd_update_interest_on(e, e->stream, q, now_ns);
+    CHD_ENTER(e, ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
+    return chd_update_interest_on(e, e->stream, q, now_ns);
 }
 
 chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query_batch* q, int64_t now_ns) {

@@ -27,9 +27,7 @@ extern "C" {
 chd_status chd_set_payload_bytes(chd_engine* e, const uint64_t* entry_off, uint32_t n_entries, const uint8_t* entry_bytes, const uint64_t* full_off,
                                  const uint8_t* full_bytes, const char* type_url, uint32_t msg_type) {
     if (!e || !entry_off || !full_off || !type_url) return CHD_ERR_INVALID;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT);
     cudaStream_t s = e->stream;
     chd_engine::Payload& P = e->pl;
     const uint64_t C = e->g.cells;
@@ -58,9 +56,7 @@ chd_status chd_set_payload_bytes(chd_engine* e, const uint64_t* entry_off, uint3
 chd_status chd_assemble_payloads(chd_engine* e, uint32_t* out_n_classes, uint64_t* out_class_off, uint32_t cap_classes, uint8_t* out_blob,
                                  uint64_t blob_cap, uint64_t* out_blob_len) {
     if (!e) return CHD_ERR_INVALID;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT);
     chd_engine::Payload& P = e->pl;
     if (!P.have_input) {
         e->fail("chd_assemble_payloads before chd_set_payload_bytes");
@@ -131,9 +127,7 @@ chd_status chd_assemble_payloads(chd_engine* e, uint32_t* out_n_classes, uint64_
 chd_status chd_frame_packets(chd_engine* e, const uint8_t* compression, uint64_t* out_conn_off, uint32_t* out_conn_len, uint32_t* out_conn_frames,
                              uint8_t* out_bytes, uint64_t out_cap, uint64_t* out_len, uint32_t* out_dropped) {
     if (!e) return CHD_ERR_INVALID;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT);
     chd_engine::Payload& P = e->pl;
     if (!P.assembled) {
         e->fail("chd_frame_packets before chd_assemble_payloads");

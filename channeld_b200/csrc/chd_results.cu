@@ -138,8 +138,7 @@ extern "C" {
 
 chd_status chd_get_cells(chd_engine* e, uint32_t* cell_start, uint32_t* sorted_entity) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     const uint32_t C = e->g.cells;
     const CopySet& c = chd_copy_in(e);
     if (cell_start) CU(e, cudaMemcpyAsync(cell_start, c.cell_start, sizeof(uint32_t) * ((uint64_t)C + 1), cudaMemcpyDefault, e->stream));
@@ -156,8 +155,7 @@ chd_status chd_get_cells(chd_engine* e, uint32_t* cell_start, uint32_t* sorted_e
 chd_status chd_get_pairs(chd_engine* e, uint32_t* pair_off, uint32_t* channel_id, uint32_t* dist, uint32_t* interval_ms, uint8_t* flags,
                          int64_t* last_fanout_ns, uint64_t* last_message_index) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     PairBuf& pb = e->pairs[e->cur];
     const uint32_t S = e->n_slots;
     uint32_t P = 0;
@@ -182,8 +180,7 @@ chd_status chd_get_pairs(chd_engine* e, uint32_t* pair_off, uint32_t* channel_id
 
 chd_status chd_get_query_status(chd_engine* e, uint32_t* status, uint32_t n) {
     if (!e || !status) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     if (n > e->last_nq) n = e->last_nq;
     CU(e, cudaMemcpyAsync(status, e->d_status, sizeof(uint32_t) * n, cudaMemcpyDefault, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
@@ -192,8 +189,7 @@ chd_status chd_get_query_status(chd_engine* e, uint32_t* status, uint32_t n) {
 
 chd_status chd_get_diff(chd_engine* e, uint32_t* new_sub, uint32_t* new_channel, uint32_t* unsub_sub, uint32_t* unsub_channel) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     CU(e, cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
     const uint32_t nn = e->h_ctr->n_sub_new, nu = e->h_ctr->n_unsub;
@@ -208,8 +204,7 @@ chd_status chd_get_diff(chd_engine* e, uint32_t* new_sub, uint32_t* new_channel,
 
 chd_status chd_get_visible(chd_engine* e, uint64_t* vis_off, uint32_t* vis_entity) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     const uint32_t S = e->n_slots;
     cudaStream_t s = e->stream;
     if (vis_off) CU(e, cudaMemcpyAsync(vis_off, e->d_vis_off, sizeof(uint64_t) * ((uint64_t)S + 1), cudaMemcpyDefault, s));
@@ -227,8 +222,7 @@ chd_status chd_get_visible(chd_engine* e, uint64_t* vis_off, uint32_t* vis_entit
 
 chd_status chd_get_visible_slot(chd_engine* e, uint32_t slot, uint32_t* out, uint64_t cap, uint64_t* count) {
     if (!e || !count || slot >= e->n_slots) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     uint64_t* h64 = (uint64_t*)e->h_get;
     CU(e, cudaMemcpyAsync(h64, e->d_vis_off + slot, 16, cudaMemcpyDeviceToHost, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
@@ -245,8 +239,7 @@ chd_status chd_get_visible_slot(chd_engine* e, uint32_t slot, uint32_t* out, uin
 
 chd_status chd_get_due(chd_engine* e, chd_due* out, uint32_t cap) {
     if (!e || !out) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     CU(e, cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
     uint32_t n = e->h_ctr->n_due;
@@ -259,8 +252,7 @@ chd_status chd_get_due(chd_engine* e, chd_due* out, uint32_t cap) {
 
 chd_status chd_get_handover(chd_engine* e, uint32_t* entity, uint32_t* src_channel, uint32_t* dst_channel, uint32_t cap) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     uint32_t n = 0;
     chd_status st = chd_read_u32(e, &e->d_ctr->n_handover, &n);
     if (st != CHD_OK) return st;
@@ -285,7 +277,7 @@ chd_status chd_fetch_results_delta(chd_engine* e, const chd_result_buffers* b, c
         e->fail("chd_fetch_results_delta: delta buffers before chd_reserve_visible_delta");
         return CHD_ERR_STATE;
     }
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     // only a fetch of the expanded list waits for the copy kernel: the other results are final once the tick's head has run
     if (b->vis_entity) CU(e, chd_copy_wait(e));
     chd_status st;
@@ -326,7 +318,6 @@ chd_status chd_fetch_results_delta(chd_engine* e, const chd_result_buffers* b, c
     if (early) {
         // The tick is probably still running.  Read back on separate streams, phase A and then phase B, each as soon as its results
         // are final (wait_phase_a / wait_phase_b), while the emit kernel is still writing the expanded list.
-        CU(e, cudaSetDevice(e->device));
         s = e->dl_stream;
         st = wait_phase_a(e, s);
         if (st != CHD_OK) return st;
@@ -461,7 +452,7 @@ chd_status chd_fetch_results_async_delta(chd_engine* e, const chd_result_buffers
             e->fail("chd_fetch_results_async: every buffer must be pinned host memory (chd_alloc_pinned)");
             return CHD_ERR_INVALID;
         }
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     if (e->fetch_issued - e->fetch_waited >= 2) {
         e->fail("chd_fetch_results_async: two fetches are already outstanding (call chd_fetch_wait)");
         return CHD_ERR_STATE;
@@ -619,7 +610,7 @@ chd_status chd_fetch_wait_delta(chd_engine* e, chd_tick_summary* summary, chd_de
         e->fail("chd_fetch_wait without a chd_fetch_results_async in flight");
         return CHD_ERR_STATE;
     }
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     const int fi = (int)(e->fetch_waited & 1);  // the OLDEST outstanding fetch
     CU(e, cudaEventSynchronize(e->ev_fetch_done[fi]));
     e->fetch_waited++;
@@ -644,8 +635,7 @@ chd_status chd_fetch_wait_delta(chd_engine* e, chd_tick_summary* summary, chd_de
 
 chd_status chd_device_view(chd_engine* e, int which, void** d_ptr, uint64_t* count) {
     if (!e || !d_ptr) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));  // work the caller orders after this on the engine stream sees the final arrays
+    CHD_ENTER(e, ENTRY_COPY_WAIT);  // work the caller orders after this on the engine stream sees the final arrays
     PairBuf& pb = e->pairs[e->cur];
     uint64_t c = 0;
     void* p = nullptr;

@@ -64,6 +64,7 @@ chd_status chd_set_slab(chd_engine* e, uint32_t col_lo, uint32_t col_hi, uint32_
     // (entity-table mode on slabs: the slab comes first, then chd_entity_table_init; the table's slots do not move with the slab)
     if (e && (chd_rule_not_table(e, "chd_set_slab") != CHD_OK || chd_rule_no_followers(e, "chd_set_slab") != CHD_OK)) return CHD_ERR_STATE;
     if (!e || col_lo >= col_hi || col_hi > e->g.cols) return CHD_ERR_INVALID;
+    CHD_ENTER(e, 0);
     e->slab = true;
     e->g.col_lo = col_lo;
     e->g.col_hi = col_hi;
@@ -76,12 +77,8 @@ chd_status chd_set_slab(chd_engine* e, uint32_t col_lo, uint32_t col_hi, uint32_
 chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_records, uint32_t* out_count) {
     if (e && chd_rule_table_on_slab(e, "chd_export_border") != CHD_OK) return CHD_ERR_STATE;
     if (!e || !d_records) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_FETCH_GUARD);
     cudaStream_t s = e->stream;
-    {
-        chd_status gs_ = chd_fetch_guard(e, s);
-        if (gs_ != CHD_OK) return gs_;
-    }
     const uint32_t n = e->n_own;
     // inside chd_tick_sharded with the peer exchange the records go straight into the peers' windows afterwards: no padding needed
     const bool to_peers = e->peer_push && d_records == e->d_rec_local;
@@ -140,7 +137,7 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
 chd_status chd_import_halo(chd_engine* e, const uint32_t* d_records, uint32_t n_records, uint32_t skip_first, uint32_t skip_count) {
     if (e && chd_rule_table_on_slab(e, "chd_import_halo") != CHD_OK) return CHD_ERR_STATE;
     if (!e || (n_records && !d_records)) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     if (chd_rule_halo_import(e) != CHD_OK) return CHD_ERR_STATE;
     cudaStream_t s = e->stream;
     if (n_records > e->lim.max_entities) {
@@ -203,7 +200,7 @@ chd_status chd_comm_init(chd_engine* e, const void* unique_id, int rank, int wor
         e->fail("chd_comm_init: %d ranks > %u grid columns (a slab is at least one column)", world, e->g.cols);
         return CHD_ERR_INVALID;
     }
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     NcclApi* api = nccl_api();
     if (!api->lib) {
         e->fail("%s", api->err.c_str());
@@ -315,7 +312,7 @@ chd_status chd_comm_info(const chd_engine* e, int* rank, int* world, uint32_t* c
 chd_status chd_comm_destroy(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     if (!e->comm) return CHD_OK;
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     CU(e, cudaStreamSynchronize(e->stream));
     for (int r = 0; r < e->comm_world && r < CHD_MAX_PEERS; r++) {
         if (r != e->comm_rank && e->peer_base[r]) cudaIpcCloseMemHandle(e->peer_base[r]);
@@ -346,12 +343,7 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
         return CHD_ERR_STATE;
     }
     flags &= ~(uint32_t)CHD_TICK_FOLLOW;  // (chd_tick below joins the update this call begins)
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
-    {
-        chd_status gs_ = chd_fetch_guard(e, e->stream);
-        if (gs_ != CHD_OK) return gs_;
-    }
+    CHD_ENTER(e, ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
     chd_status st;
     const bool has_batch = q || e->pf_q.cur >= 0 || follow;
     // Without subscriber migration the interest update does not depend on the exchange: it starts first and overlaps it.
@@ -394,7 +386,7 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
     }
     if (st != CHD_OK) return st;
     st = chd_tick(e, nullptr, t_ns, flags, out);
-    CU(e, chd_copy_wait(e));  // slabs keep the copy kernel inside their tick: the exchange adds dependencies of its own
+    CU(e, chd_copy_wait(e));  // after the tick: slabs keep the copy kernel inside their tick (the exchange adds dependencies of its own)
     return st;
 }
 
@@ -414,8 +406,7 @@ chd_status chd_migrate_out(chd_engine* e, const uint32_t* slot, uint32_t n) {
         e->fail("chd_migrate_out: one call per tick (pass every emigrant at once)");
         return CHD_ERR_STATE;
     }
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     for (uint32_t i = 0; i < n; i++)
         if (slot[i] >= e->n_slots) {
             e->fail("chd_migrate_out: slot %u is not in use (%u slots)", slot[i], e->n_slots);
@@ -447,8 +438,7 @@ chd_status chd_migrate_in(chd_engine* e, uint32_t src_rank, uint32_t first_index
     }
     if ((int)src_rank >= e->comm_world || (uint64_t)first_index + n > e->mig_subs) return CHD_ERR_INVALID;
     if (n == 0) return CHD_OK;
-    std::lock_guard<std::recursive_mutex> lk(e->mu);
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
     uint32_t max_slot = 0;
     for (uint32_t i = 0; i < n; i++) {
         if (slot[i] >= e->lim.max_subscribers) return CHD_ERR_INVALID;
@@ -468,8 +458,7 @@ chd_status chd_migrate_in(chd_engine* e, uint32_t src_rank, uint32_t first_index
 
 chd_status chd_get_rehome(chd_engine* e, uint32_t* global_id, uint32_t* dst_rank, uint32_t cap, uint32_t* count) {
     if (!e || !count) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     if (!e->assigned) {
         e->fail("chd_get_rehome before the tick's cell assignment");
         return CHD_ERR_STATE;
@@ -503,6 +492,7 @@ chd_status chd_comm_use_collective(chd_engine* e, int on) {
         e->fail("chd_comm_use_collective before chd_comm_init");
         return CHD_ERR_STATE;
     }
+    CHD_ENTER(e, 0);
     e->peer_push = !on && e->peer_mapped;
     return CHD_OK;
 }

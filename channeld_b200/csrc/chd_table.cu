@@ -113,10 +113,18 @@ chd_status rebuild_table(chd_engine* e) {
 
 bool reserved_id(uint32_t id) { return id == 0u || id == 0xFFFFFFFFu; }
 
-chd_status spawn(chd_engine* e, const char* fn, const uint32_t* id_in, const void* x_in, const void* z_in, bool f32, uint32_t n, uint8_t* out_status) {
-    if (!e || (n && (!id_in || !x_in || !z_in))) return CHD_ERR_INVALID;
+// argument checks of a spawn or a move (at most max_entities moves per call)
+chd_status check_events(chd_engine* e, const char* fn, const uint32_t* id, const void* x, const void* z, uint32_t n, bool is_move) {
+    if (!e || (n && (!id || !x || !z))) return CHD_ERR_INVALID;
     if (chd_rule_table(e, fn) != CHD_OK) return CHD_ERR_STATE;
-    CU(e, cudaSetDevice(e->device));
+    if (is_move && n > e->lim.max_entities) {
+        e->fail("%s: %u moves in one call > max_entities %llu", fn, n, (unsigned long long)e->lim.max_entities);
+        return CHD_ERR_CAPACITY;
+    }
+    return CHD_OK;
+}
+
+chd_status spawn(chd_engine* e, const uint32_t* id_in, const void* x_in, const void* z_in, bool f32, uint32_t n, uint8_t* out_status) {
     chd_engine::Table& t = e->tbl;
     std::vector<uint32_t> kid;
     const uint32_t* ids = nullptr;
@@ -184,16 +192,8 @@ chd_status spawn(chd_engine* e, const char* fn, const uint32_t* id_in, const voi
     return put_status(e, out_status, status);
 }
 
-chd_status move(chd_engine* e, const char* fn, const uint32_t* id, const void* x, const void* z, bool f32, uint32_t n) {
-    if (!e || (n && (!id || !x || !z))) return CHD_ERR_INVALID;
-    if (chd_rule_table(e, fn) != CHD_OK) return CHD_ERR_STATE;
+chd_status move(chd_engine* e, const uint32_t* id, const void* x, const void* z, bool f32, uint32_t n) {
     const uint64_t N = e->lim.max_entities;
-    if (n > N) {
-        e->fail("%s: %u moves in one call > max_entities %llu", fn, n, (unsigned long long)N);
-        return CHD_ERR_CAPACITY;
-    }
-    if (!n) return CHD_OK;
-    CU(e, cudaSetDevice(e->device));
     chd_engine::Table& t = e->tbl;
     const PosSet& front = chd_pos_front(e);
     cudaStream_t s = e->stream;
@@ -341,7 +341,7 @@ chd_status chd_entity_table_init(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_fresh_engine(e) != CHD_OK) return CHD_ERR_STATE;
     chd_engine::Table& t = e->tbl;
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     const uint64_t N = e->lim.max_entities;
     uint32_t bits = 4;
     while ((1ull << bits) < 2 * N) bits++;
@@ -371,16 +371,22 @@ chd_status chd_entity_table_init(chd_engine* e) {
 }
 
 chd_status chd_spawn_entities(chd_engine* e, const uint32_t* id, const double* x, const double* z, uint32_t n, uint8_t* out_status) {
-    return spawn(e, "chd_spawn_entities", id, x, z, false, n, out_status);
+    const chd_status st = check_events(e, "chd_spawn_entities", id, x, z, n, false);
+    if (st != CHD_OK) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    return spawn(e, id, x, z, false, n, out_status);
 }
 chd_status chd_spawn_entities_f32(chd_engine* e, const uint32_t* id, const float* x, const float* z, uint32_t n, uint8_t* out_status) {
-    return spawn(e, "chd_spawn_entities_f32", id, x, z, true, n, out_status);
+    const chd_status st = check_events(e, "chd_spawn_entities_f32", id, x, z, n, false);
+    if (st != CHD_OK) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    return spawn(e, id, x, z, true, n, out_status);
 }
 
 chd_status chd_despawn_entities(chd_engine* e, const uint32_t* id_in, uint32_t n, uint8_t* out_status) {
     if (!e || (n && !id_in)) return CHD_ERR_INVALID;
     if (chd_rule_table(e, "chd_despawn_entities") != CHD_OK) return CHD_ERR_STATE;
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     chd_engine::Table& t = e->tbl;
     const PosSet& front = chd_pos_front(e);
     std::vector<uint32_t> kid;
@@ -431,17 +437,22 @@ chd_status chd_despawn_entities(chd_engine* e, const uint32_t* id_in, uint32_t n
 }
 
 chd_status chd_move_entities(chd_engine* e, const uint32_t* id, const double* x, const double* z, uint32_t n) {
-    return move(e, "chd_move_entities", id, x, z, false, n);
+    const chd_status st = check_events(e, "chd_move_entities", id, x, z, n, true);
+    if (st != CHD_OK || !n) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    return move(e, id, x, z, false, n);
 }
 chd_status chd_move_entities_f32(chd_engine* e, const uint32_t* id, const float* x, const float* z, uint32_t n) {
-    return move(e, "chd_move_entities_f32", id, x, z, true, n);
+    const chd_status st = check_events(e, "chd_move_entities_f32", id, x, z, n, true);
+    if (st != CHD_OK || !n) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    return move(e, id, x, z, true, n);
 }
 
 chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out) {
     if (!e || !out) return CHD_ERR_INVALID;
     if (chd_rule_table(e, "chd_get_entity_stats") != CHD_OK) return CHD_ERR_STATE;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     const chd_engine::Table& t = e->tbl;
     uint64_t* h64 = reinterpret_cast<uint64_t*>(e->h_get);
     CU(e, cudaMemcpyAsync(h64, t.d_stats, 24, cudaMemcpyDeviceToHost, e->stream));
@@ -466,7 +477,7 @@ chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank,
                 "chd_assign_cells, chd_build or a tick)");
         return CHD_ERR_STATE;
     }
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     chd_engine::Table& t = e->tbl;
     const PosSet& front = chd_pos_front(e);
     cudaStream_t s = e->stream;

@@ -114,10 +114,8 @@ static chd_status emit_enqueue(chd_engine* e, cudaStream_t s, cudaEvent_t pairs_
 
 chd_status chd_emit_visible(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
-    chd_status st = chd_fetch_guard(e, e->stream);
-    return st != CHD_OK ? st : emit_enqueue(e, e->stream, nullptr, nullptr);
+    CHD_ENTER(e, ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
+    return emit_enqueue(e, e->stream, nullptr, nullptr);
 }
 
 // argument checks of one tick's host-owned rings (chd_set_rings / chd_prefetch_rings)
@@ -162,7 +160,7 @@ chd_status chd_set_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_ent
                          const uint64_t* index, const uint64_t* ch_msg_index) {
     chd_status st = check_rings(e, "chd_set_rings", ring_off, n_entries, arrival, sender, index);
     if (st != CHD_OK) return st;
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     const uint32_t total = n_entries;
     const bool in_place = chd_is_device_ptr(e, ring_off) && (!total || (chd_is_device_ptr(e, arrival) && chd_is_device_ptr(e, sender) && chd_is_device_ptr(e, index))) &&
                           (!ch_msg_index || chd_is_device_ptr(e, ch_msg_index));
@@ -194,7 +192,7 @@ chd_status chd_rings_init(chd_engine* e, uint32_t capacity_per_cell) {
         e->fail("chd_rings_init: %u cells x %u entries > max_ring_entries %u", e->g.cells, capacity_per_cell, e->lim.max_ring_entries);
         return CHD_ERR_CAPACITY;
     }
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     cudaStream_t s = e->stream;
     rings_init_kernel<<<blocks_for((uint64_t)e->g.cells + 1, 128), 128, 0, s>>>(e->g.cells, capacity_per_cell, e->d_rb_begin, e->d_rb_end);
     KCHECK(e);
@@ -217,7 +215,7 @@ chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_u
         e->fail("chd_rings_append before chd_rings_init");
         return CHD_ERR_STATE;
     }
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     cudaStream_t s = e->stream;
     const uint32_t C = e->g.cells;
     const uint64_t grown = (uint64_t)n_updates + n_updates / 2 + 1024;
@@ -242,8 +240,7 @@ chd_status chd_get_rings(chd_engine* e, uint32_t* ring_off, int64_t* arrival_ns,
         e->fail("chd_get_rings: the rings are host-owned (chd_set_rings)");
         return CHD_ERR_STATE;
     }
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     cudaStream_t s = e->stream;
     const uint32_t C = e->g.cells;
     // (control-plane call: a plain two-pass scan through scratch that is free between ticks)
@@ -283,7 +280,7 @@ chd_status chd_get_rings(chd_engine* e, uint32_t* ring_off, int64_t* arrival_ns,
 
 chd_status chd_set_channel_start_times(chd_engine* e, const int64_t* start_ns) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     if (!start_ns) {
         e->have_cell_start = false;
         return CHD_OK;
@@ -336,17 +333,15 @@ static chd_status fanout_enqueue(chd_engine* e, cudaStream_t s, int64_t t_ns) {
 
 chd_status chd_fanout_tick(chd_engine* e, int64_t t_ns) {
     if (!e) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
-    chd_status st = chd_fetch_guard(e, e->stream);
-    return st != CHD_OK ? st : fanout_enqueue(e, e->stream, t_ns);
+    CHD_ENTER(e, ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
+    return fanout_enqueue(e, e->stream, t_ns);
 }
 
 chd_status chd_prefetch_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
                               const uint64_t* index, const uint64_t* ch_msg_index) {
     chd_status st = check_rings(e, "chd_prefetch_rings", ring_off, n_entries, arrival, sender, index);
     if (st != CHD_OK) return st;
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     int set = 0;
     st = chd_pf_begin(e, e->pf_ring, &set);
     if (st != CHD_OK) return st;
@@ -369,7 +364,7 @@ chd_status chd_adopt_prefetched(chd_engine* e) {
                 "interest update yet (one batch per update)");
         return CHD_ERR_STATE;
     }
-    CU(e, cudaSetDevice(e->device));
+    CHD_ENTER(e, ENTRY_DEVICE);
     chd_pf_adopt(e->pf_q);  // consumed by the next chd_begin_interest / chd_update_interest called with q == NULL
     if (chd_pf_adopt(e->pf_ring)) {
         const chd_engine::RStage& r = e->ring_pf[e->pf_ring.cur];
@@ -387,8 +382,7 @@ chd_status chd_adopt_prefetched(chd_engine* e) {
 
 chd_status chd_summary(chd_engine* e, chd_tick_summary* out) {
     if (!e || !out) return CHD_ERR_INVALID;
-    CU(e, cudaSetDevice(e->device));
-    CU(e, chd_copy_wait(e));
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
     CU(e, cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, e->stream));
     CU(e, cudaStreamSynchronize(e->stream));
     return chd_decode_summary(e, out);
@@ -441,9 +435,8 @@ chd_status chd_begin_interest(chd_engine* e, const chd_query_batch* q, int64_t t
         e->fail("chd_begin_interest: the previous one has not been joined by chd_tick yet");
         return CHD_ERR_STATE;
     }
-    CU(e, cudaSetDevice(e->device));
-    chd_status st = chd_fetch_guard(e, e->stream);
-    if (st == CHD_OK) st = aux_chain_enqueue(e, e->stream, q, true, t_ns, with_fanout != 0);
+    CHD_ENTER(e, ENTRY_FETCH_GUARD);
+    const chd_status st = aux_chain_enqueue(e, e->stream, q, true, t_ns, with_fanout != 0);
     if (st != CHD_OK) return st;
     e->interest_pending = true;
     e->pending_fanout = with_fanout != 0;
@@ -469,9 +462,7 @@ chd_status chd_fetch_guard(chd_engine* e, cudaStream_t s) {
 // previous tick's copy kernel: the next tick's head runs beside this tick's copy, and `s` is never more than one copy behind
 // (chd_copy_wait joins the rest).  A tick with nothing to overlap runs its stages one after the other on `s`.
 static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_batch* q, int64_t t_ns, uint32_t flags) {
-    CU(e, cudaSetDevice(e->device));
-    chd_status st = chd_fetch_guard(e, s);
-    if (st != CHD_OK) return st;
+    chd_status st;
     const bool need_build = (flags & CHD_TICK_BUILD) && (e->entities_dirty || !e->built);
     const bool do_emit = flags & CHD_TICK_EMIT;
     const bool do_fanout = flags & CHD_TICK_FANOUT;
@@ -493,7 +484,7 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
     }
     if (do_delta && chd_delta_check(e, need_build) != CHD_OK) return CHD_ERR_STATE;
     if (!started && !((interest || do_fanout) && (need_build || do_emit))) {
-        CU(e, chd_copy_wait(e));
+        CU(e, chd_copy_wait(e));  // one stream: the whole tick runs after the previous tick's copy kernel
         if (need_build) {
             st = chd_build_on(e, s);
             if (st != CHD_OK) return st;
@@ -567,6 +558,7 @@ chd_status chd_tick(chd_engine* e, const chd_query_batch* q, int64_t t_ns, uint3
     {
         // from the tick's first head kernel to the end of its copy kernel (without the summary read-back)
         StageTimer whole(e, e->stream, CHD_STAGE_TICK);
+        CHD_ENTER(e, ENTRY_FETCH_GUARD);
         st = tick_enqueue(e, e->stream, q, t_ns, flags);
         if (e->copy_pending >= 0) whole.s = e->copy_stream;
     }
