@@ -18,16 +18,17 @@ __global__ void __launch_bounds__(128)
     if (c <= cells) begin[c] = end[c] = min(c, cells) * cap;  // ([cells]: sentinel)
 }
 
-// one thread per cell applies the cell's updates of this tick in the order given (upd_off: CSR by cell)
+// one thread per cell applies the cell's updates of this tick in the order given (upd_off: CSR by cell, clamped to n_updates: a
+// lying caller cannot make it read past the uploaded updates)
 __global__ void __launch_bounds__(128)
-    rings_append_kernel(uint32_t cells, uint32_t cap, const uint32_t* __restrict__ upd_off, const int64_t* __restrict__ upd_arrival,
+    rings_append_kernel(uint32_t cells, uint32_t cap, const uint32_t* __restrict__ upd_off, uint32_t n_updates, const int64_t* __restrict__ upd_arrival,
                         const uint32_t* __restrict__ upd_sender, uint32_t* __restrict__ begin, uint32_t* __restrict__ end, int64_t* __restrict__ arrival,
                         uint32_t* __restrict__ sender, uint64_t* __restrict__ index, uint64_t* __restrict__ msg_index,
                         const uint32_t* __restrict__ max_interval_ms, uint32_t* __restrict__ overflow) {
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= cells) return;
-    const uint32_t u0 = upd_off[c], u1 = upd_off[c + 1];
-    if (u0 == u1) return;
+    const uint32_t u0 = min(upd_off[c], n_updates), u1 = min(upd_off[c + 1], n_updates);
+    if (u0 >= u1) return;
     const uint32_t base = c * cap;
     uint32_t b = begin[c], e = end[c];
     uint64_t mi = msg_index[c];
@@ -40,6 +41,7 @@ __global__ void __launch_bounds__(128)
                 b++;
                 n--;
             }
+#pragma unroll 1  // (unrolled, ptxas spills 16 bytes of this kernel to the stack)
             for (uint32_t i = 0; i < n; i++) {
                 arrival[base + i] = arrival[b + i];
                 sender[base + i] = sender[b + i];

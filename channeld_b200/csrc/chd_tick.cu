@@ -118,6 +118,16 @@ chd_status chd_emit_visible(chd_engine* e) {
     return emit_enqueue(e, e->stream, nullptr, nullptr);
 }
 
+// Ring inputs go before chd_begin_interest.  The chain it forks onto aux_stream reads what they write, and nothing on the engine
+// stream is ordered against that chain until chd_tick joins it: the interest update reads the channel start times and raises the
+// per-cell maxFanOutIntervalMs that chd_rings_append reads, the fan-out reads the rings and the start times.  `fanout_only`: the
+// input is read by the fan-out alone (chd_set_rings), so a begun chain without the fan-out does not exclude it.
+static chd_status rings_before_interest(chd_engine* e, const char* fn, bool fanout_only) {
+    if (!e->interest_pending || (fanout_only && !e->pending_fanout)) return CHD_OK;
+    e->fail("%s while a chd_begin_interest is pending: ring inputs go before it (or after the chd_tick that joins it)", fn);
+    return CHD_ERR_STATE;
+}
+
 // argument checks of one tick's host-owned rings (chd_set_rings / chd_prefetch_rings)
 static chd_status check_rings(chd_engine* e, const char* fn, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
                               const uint64_t* index) {
@@ -160,6 +170,7 @@ chd_status chd_set_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_ent
                          const uint64_t* index, const uint64_t* ch_msg_index) {
     chd_status st = check_rings(e, "chd_set_rings", ring_off, n_entries, arrival, sender, index);
     if (st != CHD_OK) return st;
+    if (rings_before_interest(e, "chd_set_rings", true) != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_DEVICE);
     const uint32_t total = n_entries;
     const bool in_place = chd_is_device_ptr(e, ring_off) && (!total || (chd_is_device_ptr(e, arrival) && chd_is_device_ptr(e, sender) && chd_is_device_ptr(e, index))) &&
@@ -187,6 +198,7 @@ chd_status chd_rings_init(chd_engine* e, uint32_t capacity_per_cell) {
         if (e) e->fail("chd_rings_init: capacity_per_cell must exceed %u (MaxUpdateMsgBufferSize: the reference's buffer may grow beyond it)", RING_MAX_BUFFER);
         return CHD_ERR_INVALID;
     }
+    if (rings_before_interest(e, "chd_rings_init", false) != CHD_OK) return CHD_ERR_STATE;
     const uint64_t need = (uint64_t)e->g.cells * capacity_per_cell;
     if (need > e->lim.max_ring_entries) {
         e->fail("chd_rings_init: %u cells x %u entries > max_ring_entries %u", e->g.cells, capacity_per_cell, e->lim.max_ring_entries);
@@ -215,6 +227,7 @@ chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_u
         e->fail("chd_rings_append before chd_rings_init");
         return CHD_ERR_STATE;
     }
+    if (rings_before_interest(e, "chd_rings_append", false) != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_DEVICE);
     cudaStream_t s = e->stream;
     const uint32_t C = e->g.cells;
@@ -226,7 +239,7 @@ chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_u
         CU(e, cudaMemcpyAsync(e->d_upd_arrival, arrival_ns, sizeof(int64_t) * n_updates, cudaMemcpyDefault, s));
         CU(e, cudaMemcpyAsync(e->d_upd_sender, sender_conn_id, sizeof(uint32_t) * n_updates, cudaMemcpyDefault, s));
     }
-    rings_append_kernel<<<blocks_for(C, 128), 128, 0, s>>>(C, e->ring_cap, e->d_upd_off, e->d_upd_arrival, e->d_upd_sender, e->d_rb_begin, e->d_rb_end,
+    rings_append_kernel<<<blocks_for(C, 128), 128, 0, s>>>(C, e->ring_cap, e->d_upd_off, n_updates, e->d_upd_arrival, e->d_upd_sender, e->d_rb_begin, e->d_rb_end,
                                                            e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, e->d_ch_msg_index, e->d_cell_max_interval,
                                                            &e->d_ctr->overflow);
     KCHECK(e);
@@ -280,6 +293,7 @@ chd_status chd_get_rings(chd_engine* e, uint32_t* ring_off, int64_t* arrival_ns,
 
 chd_status chd_set_channel_start_times(chd_engine* e, const int64_t* start_ns) {
     if (!e) return CHD_ERR_INVALID;
+    if (rings_before_interest(e, "chd_set_channel_start_times", false) != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_DEVICE);
     if (!start_ns) {
         e->have_cell_start = false;

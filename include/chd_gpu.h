@@ -207,7 +207,8 @@ chd_status chd_emit_visible(chd_engine* e);
 /* ---- update rings: the per-channel updateMsgBuffer metadata (data.go:46-51) in insertion order, CSR by cell
  * index (channel id - channel_id_start): ring_off[cells+1], n_entries = ring_off[cells].  channel_msg_index[cells] = ChannelData.msgIndex
  * (data.go:25,158) or NULL for zeros.  The host owns OnUpdate/eviction (data.go:149-173): payload merging is
- * opaque protobuf work. */
+ * opaque protobuf work.  Call order: before chd_begin_interest(..., with_fanout = 1), whose fan-out reads the rings on the
+ * engine's second stream until chd_tick joins it; in between it returns CHD_ERR_STATE (with with_fanout = 0 it is accepted). */
 chd_status chd_set_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival_ns,
                          const uint32_t* sender_conn_id, const uint64_t* message_index, const uint64_t* channel_msg_index);
 /* The same for the other per-tick inputs: the query batch (consumed by the next chd_begin_interest / chd_update_interest
@@ -229,7 +230,10 @@ chd_status chd_prefetch_rings(chd_engine* e, const uint32_t* ring_off, uint32_t 
  * channel's maxFanOutIntervalMs (tracked on the device: it grows when a subscription with a longer interval is created,
  * subscription.go:84-86) — pop that one.  Merging the update into the channel's data message (opaque protobuf) stays with the
  * host.  chd_get_rings reads the live rings back as the CSR chd_set_rings takes (tests, recovery).  Stream-ordered except
- * chd_get_rings. */
+ * chd_get_rings.  Offsets past n_updates are read as n_updates.  Call order: chd_rings_init, chd_rings_append and
+ * chd_set_channel_start_times go before chd_begin_interest (the interest update and the fan-out it starts read the rings, the
+ * start times and maxFanOutIntervalMs) or after the chd_tick that joins it; in between they return CHD_ERR_STATE and change
+ * nothing. */
 chd_status chd_rings_init(chd_engine* e, uint32_t capacity_per_cell);
 chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_updates, const int64_t* arrival_ns, const uint32_t* sender_conn_id);
 chd_status chd_get_rings(chd_engine* e, uint32_t* ring_off, int64_t* arrival_ns, uint32_t* sender_conn_id, uint64_t* message_index,

@@ -531,6 +531,29 @@ uint64_t orc_channels_tick_data_ex(orc_channel* const* ch, uint32_t n_ch, int64_
     return total;
 }
 
+uint64_t orc_channels_get_rings(orc_channel* const* ch, uint32_t n_ch, uint64_t* ring_off, int64_t* arrival_ns, uint32_t* sender_conn_id,
+                                uint64_t* message_index, uint64_t cap, uint64_t* msg_index, uint32_t* max_interval_ms) {
+    uint64_t total = 0;
+    ring_off[0] = 0;
+    for (uint32_t c = 0; c < n_ch; c++) {
+        total += ch[c]->ring.size();
+        ring_off[c + 1] = total;
+        if (msg_index) msg_index[c] = ch[c]->msg_index;
+        if (max_interval_ms) max_interval_ms[c] = ch[c]->max_interval_ms;
+    }
+    if (total > cap) return total;
+    for (uint32_t c = 0; c < n_ch; c++) {
+        uint64_t k = ring_off[c];
+        for (const RingEl& r : ch[c]->ring) {
+            if (arrival_ns) arrival_ns[k] = r.arrival;
+            if (sender_conn_id) sender_conn_id[k] = r.sender;
+            if (message_index) message_index[k] = r.index;
+            k++;
+        }
+    }
+    return total;
+}
+
 void orc_channels_get_state(orc_channel* const* ch, const uint32_t* chan, const uint32_t* conn_id, uint64_t n, int64_t* last_fanout,
                             uint8_t* had_first, uint64_t* last_msg_index, uint8_t* found) {
     for (uint64_t i = 0; i < n; i++) {

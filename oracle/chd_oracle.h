@@ -164,6 +164,12 @@ uint64_t orc_channels_tick_data(orc_channel* const* ch, uint32_t n_ch, int64_t t
  * (sel_off[cap+1]).  Returns the total, or (uint64_t)-1 when `cap` or `sel_cap` is too small or an iteration bound trips. */
 uint64_t orc_channels_tick_data_ex(orc_channel* const* ch, uint32_t n_ch, int64_t t_ns, orc_send* out, uint64_t cap, uint64_t* out_off,
                                    int64_t* window_lo, uint32_t* self_skipped, uint64_t* sel_off, uint32_t* sel_pos, uint64_t sel_cap);
+/* Every channel's updateMsgBuffer (data.go:46-51) as a CSR by channel: ring_off[n_ch+1], the entries of channel c in insertion
+ * order at [ring_off[c], ring_off[c+1]) of arrival_ns / sender_conn_id / message_index; msg_index[n_ch] = ChannelData.msgIndex
+ * (data.go:25,158), max_interval_ms[n_ch] = ChannelData.maxFanOutIntervalMs (subscription.go:84-86).  Any output but ring_off may
+ * be NULL.  Returns the total; when it exceeds `cap` only the offsets and the per-channel outputs are written. */
+uint64_t orc_channels_get_rings(orc_channel* const* ch, uint32_t n_ch, uint64_t* ring_off, int64_t* arrival_ns, uint32_t* sender_conn_id,
+                                uint64_t* message_index, uint64_t cap, uint64_t* msg_index, uint32_t* max_interval_ms);
 /* found[i] = 0 when conn_id[i] is not subscribed to chan[i] (the state outputs are then left as they were) */
 void orc_channels_get_state(orc_channel* const* ch, const uint32_t* chan, const uint32_t* conn_id, uint64_t n, int64_t* last_fanout,
                             uint8_t* had_first, uint64_t* last_msg_index, uint8_t* found);

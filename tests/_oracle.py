@@ -106,6 +106,8 @@ class Oracle:
         L.orc_channels_tick_data_ex.restype = C.c_uint64
         L.orc_channels_tick_data_ex.argtypes = [vp, C.c_uint32, C.c_int64, C.POINTER(Send), C.c_uint64, u64p, C.POINTER(C.c_int64), u32p, u64p,
                                                 u32p, C.c_uint64]
+        L.orc_channels_get_rings.restype = C.c_uint64
+        L.orc_channels_get_rings.argtypes = [vp, C.c_uint32, u64p, C.POINTER(C.c_int64), u32p, u64p, C.c_uint64, u64p, u32p]
         L.orc_channels_get_state.restype = None
         L.orc_channels_get_state.argtypes = [vp, u32p, u32p, C.c_uint64, C.POINTER(C.c_int64), C.POINTER(C.c_uint8), u64p,
                                              C.POINTER(C.c_uint8)]
@@ -343,6 +345,8 @@ class OracleChannels:
         self.h = np.array([self.L.orc_channel_new() for _ in range(n)], np.uint64)
 
     def __del__(self):
+        if getattr(self, "_owner", None) is not None:
+            return  # a view: its owner frees the channels
         try:
             for h in self.h:
                 self.L.orc_channel_free(C.c_void_p(int(h)))
@@ -389,6 +393,25 @@ class OracleChannels:
                                              lo.ctypes.data_as(C.POINTER(C.c_int64)), _p(sk, u32p), _p(so, u64p), _p(sp, u32p), len(sp))
         assert k != 2 ** 64 - 1, "oracle tick_data_ex: capacity/iteration bound"
         return out[:k], off, lo[:k], sk[:k], so[:k + 1], sp[:int(so[k])]
+
+    def get_rings(self):
+        """Every channel's updateMsgBuffer as a CSR by channel -> dict(off u64[n+1], arrival, sender, index (insertion order per
+        channel), msg_index u64[n] (ChannelData.msgIndex), max_interval_ms u32[n] (ChannelData.maxFanOutIntervalMs))"""
+        off = np.zeros(self.n + 1, np.uint64)
+        mi = np.zeros(self.n, np.uint64)
+        mx = np.zeros(self.n, np.uint32)
+        total = int(self.L.orc_channels_get_rings(self._hp(), self.n, _p(off, u64p), None, None, None, 0, _p(mi, u64p), _p(mx, u32p)))
+        arr, snd, idx = np.zeros(max(total, 1), np.int64), np.zeros(max(total, 1), np.uint32), np.zeros(max(total, 1), np.uint64)
+        k = self.L.orc_channels_get_rings(self._hp(), self.n, _p(off, u64p), arr.ctypes.data_as(C.POINTER(C.c_int64)), _p(snd, u32p),
+                                          _p(idx, u64p), total, None, None)
+        assert k == total
+        return dict(off=off, arrival=arr[:total], sender=snd[:total], index=idx[:total], msg_index=mi, max_interval_ms=mx)
+
+    def view(self, chans):
+        """The channels chans (indices into this set) as a set of their own (the same handles: calls on the view change them)."""
+        v = OracleChannels.__new__(OracleChannels)
+        v.L, v.h, v.n, v._owner = self.L, np.ascontiguousarray(self.h[np.asarray(chans, np.int64)]), len(chans), self
+        return v
 
     def state(self, chan, conn):
         """-> (last[n], had_first[n], last_index[n], found[n])"""
