@@ -93,7 +93,9 @@ struct WinRef {
 // its location does not matter: the block's windows are carved out of `window` with one atomicAdd per block on a bump
 // cursor (zeroed by the stage's first kernel) instead of a device-wide prefix sum (two launches less per tick).
 // A query whose window does not fit the scratch gets CHD_Q_ERR_CAPACITY: like any failed query it leaves the subscriber's
-// subscriptions untouched; CHD_OVF_WINDOW is raised and the cursor's final value is the required capacity.
+// subscriptions untouched; CHD_OVF_WINDOW is raised and the cursor's final value is the required capacity.  A query with an
+// empty window (spots only, or shapes that miss the grid) needs no scratch and is never refused: its offset may lie past the
+// scratch once the cursor has run over, but it writes nothing there, so it runs its spots or fails with its own status.
 // A query that sets a kind bit without supplying that kind's arrays gets CHD_Q_ERR_MISSING_ARRAY; in a merged batch the host
 // part's entries are judged by the arrays the host part supplied (q.missing, written by follow_merge_kernel).
 __global__ void __launch_bounds__(128)
@@ -133,7 +135,7 @@ __global__ void __launch_bounds__(128)
     if (i >= q.n) return;
     bbox[i] = win.b;
     win_off[i] = off;
-    if (missing || off + wn > win_cap) {
+    if (missing || (wn != 0 && off + wn > win_cap)) {
         if (!missing) atomicOr(overflow, (uint32_t)CHD_OVF_WINDOW);
         status[i] = missing ? CHD_Q_ERR_MISSING_ARRAY : CHD_Q_ERR_CAPACITY;
         count[i] = 0;

@@ -182,7 +182,9 @@ enum {
                                    lattice walk of more than 2^24 samples (cut off: a documented deviation) */
     CHD_Q_ERR_ANGLE_RANGE = 6,  /* |cone angle| >= 2^29: Go switches to Payne-Hanek reduction, not reproduced */
     CHD_Q_ERR_CAPACITY = 7,     /* the query's cell window did not fit chd_limits.max_window_cells (CHD_OVF_WINDOW is raised):
-                                   like every failed query it leaves the subscriber's subscriptions untouched */
+                                   like every failed query it leaves the subscriber's subscriptions untouched.  Only a query that
+                                   needs a window can get it: one whose window is empty (spots only, or shapes that miss the
+                                   grid) runs its spots or fails with its own status however full the scratch is */
     CHD_Q_ERR_MISSING_ARRAY = 8 /* a kind bit is set but that kind's arrays were not supplied in the batch */
 };
 
@@ -283,7 +285,8 @@ typedef struct chd_tick_summary {
  *   CHD_OVF_PAIRS   the interest update was NOT applied: every subscriber keeps its previous subscriptions and fan-out state,
  *                   the diff lists are empty; required_pairs = the total the update would have needed
  *   CHD_OVF_WINDOW  the queries whose cell windows did not fit got CHD_Q_ERR_CAPACITY and, like any failed query, left their
- *                   subscribers untouched; the rest of the batch was applied; required_window_cells = scratch needed
+ *                   subscribers untouched; the rest of the batch was applied, including every query with an empty window (spots
+ *                   only, or shapes that miss the grid), which needs no scratch; required_window_cells = scratch needed
  *                   (either of these two on a tick whose batch came from chd_follow_queries(CHD_FOLLOW_MOVED): the followers'
  *                   stored centres advanced when the batch was generated, not when it was applied, so re-issue the tick's queries
  *                   with chd_follow_queries(CHD_FOLLOW_ALL); after chd_follow_queries_with(CHD_FOLLOW_MOVED, q), re-issue

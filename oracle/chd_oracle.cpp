@@ -4,10 +4,12 @@
 #include "chd_oracle.h"
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <condition_variable>
 #include <cstring>
 #include <functional>
+#include <initializer_list>
 #include <mutex>
 #include <list>
 #include <map>
@@ -879,6 +881,71 @@ int orc_visible_delta(uint32_t cells, const uint32_t* prev_cell, uint32_t prev_n
     }
     if ((enter && enter_off[n_out] > enter_cap) || (leave && leave_off[n_out] > leave_cap)) return ORC_ERR_CAPACITY;
     if (enter || leave) pass(true);
+    return ORC_OK;
+}
+
+/* ------------------------------------------------------------------ batched QueryChannelIds ------ */
+int orc_query_batch(const orc_grid* g, const orc_query_soa* b, uint32_t* status, uint64_t* out_off, uint32_t* out_ids,
+                    uint32_t* out_dists, uint64_t cap, int n_threads) {
+    const uint32_t n = b->n;
+    const auto has = [](std::initializer_list<const void*> ps) {
+        for (const void* p : ps)
+            if (!p) return false;
+        return true;
+    };
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t k = b->kind ? b->kind[i] : uint32_t(ORC_AOI_SPHERE);
+        if (((k & ORC_AOI_SPOTS) && !has({b->spot_off, b->spot_x, b->spot_z})) ||
+            ((k & ORC_AOI_BOX) && !has({b->box_cx, b->box_cz, b->box_ex, b->box_ez})) ||
+            ((k & ORC_AOI_SPHERE) && !has({b->sph_cx, b->sph_cz, b->sph_r})) ||
+            ((k & ORC_AOI_CONE) && !has({b->cone_cx, b->cone_cz, b->cone_dx, b->cone_dz, b->cone_angle, b->cone_r})))
+            return ORC_ERR_NIL;
+    }
+    if (n_threads < 1) n_threads = 1;
+    std::vector<std::vector<std::pair<uint32_t, uint32_t>>> res(n);
+    std::atomic<uint32_t> next{0};
+    const uint32_t chunk = 64;
+    Pool::get().run(n_threads, [&](int) {
+        std::map<uint32_t, uint32_t> m;
+        for (uint32_t lo; (lo = next.fetch_add(chunk)) < n;) {
+            for (uint32_t i = lo; i < std::min(n, lo + chunk); i++) {
+                orc_query q;
+                std::memset(&q, 0, sizeof(q));
+                q.kind_mask = b->kind ? b->kind[i] : uint32_t(ORC_AOI_SPHERE);
+                if (q.kind_mask & ORC_AOI_SPOTS) {
+                    const uint32_t s0 = b->spot_off[i];
+                    q.n_spots = b->spot_off[i + 1] - s0;
+                    q.n_spot_dists = b->spot_ndist ? b->spot_ndist[i] : 0u;
+                    if (!b->spot_dist) q.n_spot_dists = 0;  // no dists given: every spot has dist 0
+                    q.spot_x = b->spot_x + s0;
+                    q.spot_z = b->spot_z + s0;
+                    q.spot_dist = b->spot_dist ? b->spot_dist + s0 : nullptr;
+                }
+                if (q.kind_mask & ORC_AOI_BOX) {
+                    q.box_cx = b->box_cx[i]; q.box_cz = b->box_cz[i]; q.box_ex = b->box_ex[i]; q.box_ez = b->box_ez[i];
+                }
+                if (q.kind_mask & ORC_AOI_SPHERE) {
+                    q.sph_cx = b->sph_cx[i]; q.sph_cz = b->sph_cz[i]; q.sph_r = b->sph_r[i];
+                }
+                if (q.kind_mask & ORC_AOI_CONE) {
+                    q.cone_cx = b->cone_cx[i]; q.cone_cz = b->cone_cz[i]; q.cone_dx = b->cone_dx[i]; q.cone_dz = b->cone_dz[i];
+                    q.cone_angle = b->cone_angle[i]; q.cone_r = b->cone_r[i];
+                }
+                m.clear();
+                status[i] = uint32_t(query_into(g, &q, m));
+                if (status[i] == ORC_OK) res[i].assign(m.begin(), m.end());
+            }
+        }
+    });
+    out_off[0] = 0;
+    for (uint32_t i = 0; i < n; i++) out_off[i + 1] = out_off[i] + res[i].size();
+    if (!out_ids) return ORC_OK;
+    if (out_off[n] > cap) return ORC_ERR_CAPACITY;
+    for (uint32_t i = 0; i < n; i++)
+        for (size_t k = 0; k < res[i].size(); k++) {
+            out_ids[out_off[i] + k] = res[i][k].first;
+            out_dists[out_off[i] + k] = res[i][k].second;
+        }
     return ORC_OK;
 }
 

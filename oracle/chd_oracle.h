@@ -84,6 +84,28 @@ void orc_cell_of(const orc_grid* g, const double* x, const double* z, uint32_t n
 int orc_query_channel_ids(const orc_grid* g, const orc_query* q, uint32_t* out_ids, uint32_t* out_dists,
                           uint32_t cap, uint32_t* out_n);
 
+/* A batch of queries in the layout of chd_query_batch (include/chd_gpu.h), without the subscriber slots: kind[n] (NULL = all
+ * sphere), the shape arrays (a kind no query uses may be NULL), spots as a CSR spot_off[n+1] into spot_x / spot_z / spot_dist with
+ * spot_ndist[n] = len(Dists) of each query (NULL = 0; spot_dist NULL = every dist 0). */
+typedef struct orc_query_soa {
+    uint32_t n;
+    const uint8_t* kind;
+    const double *sph_cx, *sph_cz, *sph_r;
+    const double *box_cx, *box_cz, *box_ex, *box_ez;
+    const double *cone_cx, *cone_cz, *cone_dx, *cone_dz, *cone_angle, *cone_r;
+    const uint32_t* spot_off;
+    const uint32_t* spot_ndist;
+    const double *spot_x, *spot_z;
+    const uint32_t* spot_dist;
+} orc_query_soa;
+
+/* orc_query_channel_ids for every query of a batch, spread over n_threads threads of the pool.  status[n]; the results as a CSR
+ * (out_off[n+1], u64) of (channel id, dist), each query's entries in orc_query_channel_ids' order; a failed query has none.
+ * out_ids / out_dists NULL: only status and out_off are written.  Returns ORC_OK, ORC_ERR_CAPACITY when out_off[n] > cap (status
+ * and out_off are written, nothing else), or ORC_ERR_NIL when a query sets a kind bit whose arrays are NULL (nothing written). */
+int orc_query_batch(const orc_grid* g, const orc_query_soa* b, uint32_t* status, uint64_t* out_off, uint32_t* out_ids,
+                    uint32_t* out_dists, uint64_t cap, int n_threads);
+
 /* spatial.go:358-381; order as the reference emits (row-major y,x).  Returns count (<=8). */
 uint32_t orc_get_adjacent_channels(const orc_grid* g, uint32_t channel_id, uint32_t* out8);
 

@@ -38,6 +38,12 @@ class Query(C.Structure):
     ]
 
 
+class QuerySoA(C.Structure):
+    _fields_ = [("n", C.c_uint32), ("kind", C.c_void_p)] + [(k, f64p) for k in (
+        "sph_cx", "sph_cz", "sph_r", "box_cx", "box_cz", "box_ex", "box_ez", "cone_cx", "cone_cz", "cone_dx", "cone_dz", "cone_angle",
+        "cone_r")] + [("spot_off", u32p), ("spot_ndist", u32p), ("spot_x", f64p), ("spot_z", f64p), ("spot_dist", u32p)]
+
+
 class Send(C.Structure):
     _fields_ = [
         ("conn_id", C.c_uint32), ("kind", C.c_uint32), ("n_selected", C.c_uint32),
@@ -68,6 +74,8 @@ class Oracle:
         L.orc_cell_of.argtypes = [C.POINTER(Grid), f64p, f64p, C.c_uint32, u32p]
         L.orc_query_channel_ids.restype = C.c_int
         L.orc_query_channel_ids.argtypes = [C.POINTER(Grid), C.POINTER(Query), u32p, u32p, C.c_uint32, u32p]
+        L.orc_query_batch.restype = C.c_int
+        L.orc_query_batch.argtypes = [C.POINTER(Grid), C.POINTER(QuerySoA), u32p, u64p, u32p, u32p, C.c_uint64, C.c_int]
         L.orc_get_adjacent_channels.restype = C.c_uint32
         L.orc_get_adjacent_channels.argtypes = [C.POINTER(Grid), C.c_uint32, u32p]
         L.orc_adjacent_broadcast.restype = C.c_uint32
@@ -170,6 +178,49 @@ class Oracle:
         if st != OK:
             return None, st
         return {int(ids[i]): int(dists[i]) for i in range(n.value)}, st
+
+    def query_batch(self, g, n, kind=None, sphere=None, box=None, cone=None, spots=None, n_threads=None):
+        """orc_query_batch on a batch in engine.make_batch's form: kind[n] masks (None = all sphere), sphere=(cx,cz,r)
+        box=(cx,cz,ex,ez) cone=(cx,cz,dx,dz,angle,r) tuples of arrays, spots=(spot_off, spot_ndist, x, z, dist).
+        -> (status u32[n], off u64[n+1], channel_id u32[], dist u32[])"""
+        b = QuerySoA()
+        b.n = int(n)
+        keep = []
+
+        def arr(a, dt, t):
+            a = np.ascontiguousarray(a, dt)
+            keep.append(a)
+            return _p(a, t)
+
+        if kind is not None:
+            k = np.ascontiguousarray(kind, np.uint8)
+            keep.append(k)
+            b.kind = k.ctypes.data
+        for names, vals in ((("sph_cx", "sph_cz", "sph_r"), sphere), (("box_cx", "box_cz", "box_ex", "box_ez"), box),
+                            (("cone_cx", "cone_cz", "cone_dx", "cone_dz", "cone_angle", "cone_r"), cone)):
+            if vals is not None:
+                for name, v in zip(names, vals):
+                    setattr(b, name, arr(v, np.float64, f64p))
+        if spots is not None:
+            off, ndist, x, z, dist = spots
+            b.spot_off, b.spot_x, b.spot_z = arr(off, np.uint32, u32p), arr(x, np.float64, f64p), arr(z, np.float64, f64p)
+            if ndist is not None:
+                b.spot_ndist = arr(ndist, np.uint32, u32p)
+            if dist is not None:
+                b.spot_dist = arr(dist, np.uint32, u32p)
+        status = np.zeros(max(n, 1), np.uint32)
+        off = np.zeros(n + 1, np.uint64)
+        nt = int(n_threads or os.cpu_count() or 1)
+        cap = 64 * n + 1024
+        while True:
+            ids, dist = np.zeros(cap, np.uint32), np.zeros(cap, np.uint32)
+            rc = self.lib.orc_query_batch(C.byref(g), C.byref(b), _p(status, u32p), _p(off, u64p), _p(ids, u32p), _p(dist, u32p), cap, nt)
+            if rc != ERR_CAPACITY:
+                break
+            cap = int(off[n])
+        assert rc == OK, rc
+        t = int(off[n])
+        return status[:n], off, ids[:t], dist[:t]
 
     def adjacent(self, g, channel_id):
         out = np.zeros(8, np.uint32)
