@@ -162,6 +162,19 @@ SYMBOLS = [
     "chd_get_entity_stats", "chd_handoff_entities",
     "chd_follow_bind", "chd_follow_unbind", "chd_follow_queries", "chd_get_follow", "chd_follow_queries_with",
 ]
+# every symbol include/chd_gpu_subs.h declares (explicit subscriptions; checked by tests/test_subs_host.py against that header)
+SUB_SYMBOLS = ["chd_apply_subscriptions"]
+SUBOP_SUB, SUBOP_UNSUB = 0, 1
+SUBOPT_INTERVAL, SUBOPT_DELAY, SUBOPT_SKIP_SELF, SUBOPT_SKIP_FIRST = 1, 2, 4, 8
+SUB_NEW, SUB_MERGED, SUB_UNSUBSCRIBED, SUB_NOT_SUBSCRIBED, SUB_ERR_SLOT, SUB_ERR_CHANNEL, SUB_ERR_CAPACITY = range(7)
+DIST_EXPLICIT = 0xFFFFFFFF
+
+
+class SubBatch(C.Structure):
+    _fields_ = [("n", C.c_uint32), ("slot", C.c_void_p), ("channel_id", C.c_void_p), ("op", C.c_void_p), ("present", C.c_void_p),
+                ("interval_ms", C.c_void_p), ("delay_ms", C.c_void_p), ("skip_self", C.c_void_p), ("skip_first", C.c_void_p)]
+
+
 STAGE_BUILD, STAGE_INTEREST, STAGE_EMIT, STAGE_EMIT_KERNEL, STAGE_FANOUT, STAGE_TICK, STAGE_EXPORT, STAGE_EXCHANGE, STAGE_IMPORT, STAGE_READBACK, STAGE_VISIBLE_DELTA, STAGE_ENTITY_EVENTS, STAGE_FOLLOW = range(13)
 
 _lib = None
@@ -374,6 +387,8 @@ def lib():
     L.chd_follow_queries_with.argtypes = [vp, C.c_uint32, C.POINTER(QueryBatch)]
     L.chd_get_follow.restype = C.c_int
     L.chd_get_follow.argtypes = [vp, vp, vp, vp, vp, vp, C.c_uint32, u32p, u32p]
+    L.chd_apply_subscriptions.restype = C.c_int
+    L.chd_apply_subscriptions.argtypes = [vp, C.POINTER(SubBatch), C.c_int64, vp]
     _lib = L
     return L
 

@@ -21,6 +21,14 @@ class SpatialError(Exception):
 
 
 @dataclass
+class ChannelSubscriptionOptions:  # channeld.proto ChannelSubscriptionOptions: the fan-out fields (None = not set in the message)
+    FanOutIntervalMs: Optional[int] = None
+    FanOutDelayMs: Optional[int] = None
+    SkipSelfUpdateFanOut: Optional[bool] = None
+    SkipFirstFanOut: Optional[bool] = None
+
+
+@dataclass
 class SpatialInfo:  # pkg/common/common.go:20-24
     X: float = 0.0
     Y: float = 0.0
@@ -290,6 +298,30 @@ class GpuStaticGrid2DSpatialController:
         elif explicit is not None:
             raise SpatialError("explicit queries are merged into a followed tick: pass follow=")
         return self.engine.tick(batch, t_ns, flags)
+
+    # -- SubscribeToChannel / UnsubscribeFromChannel for spatial channels (subscription.go:34-125), batched: what handleSubToChannel /
+    # handleUnsubFromChannel (message.go:488-605) and a server's subscriptions to its own cells after CreateChannels
+    # (message_spatial.go:167-173) do to the fan-out state.  options[i] (None = no options) carries the fields the message set;
+    # DataAccess and DataFieldMasks stay with the host.  Applied between ticks, at channel time t_ns; returns capi.SUB_* per op.
+    def SubscribeToChannelBatch(self, conn_slots, channel_ids, options: Sequence[Optional["ChannelSubscriptionOptions"]], t_ns) -> np.ndarray:
+        n = len(conn_slots)
+        present = np.zeros(n, np.uint8)
+        iv, dl = np.zeros(n, np.uint32), np.zeros(n, np.int32)
+        ss, sf = np.zeros(n, np.uint8), np.zeros(n, np.uint8)
+        for i, o in enumerate(options):
+            if o is None:
+                continue
+            for v, arr, bit in ((o.FanOutIntervalMs, iv, capi.SUBOPT_INTERVAL), (o.FanOutDelayMs, dl, capi.SUBOPT_DELAY),
+                                (o.SkipSelfUpdateFanOut, ss, capi.SUBOPT_SKIP_SELF), (o.SkipFirstFanOut, sf, capi.SUBOPT_SKIP_FIRST)):
+                if v is not None:
+                    arr[i] = v
+                    present[i] |= bit
+        return self.engine.apply_subscriptions(conn_slots, channel_ids, np.full(n, capi.SUBOP_SUB, np.uint8), interval=iv, delay=dl, skip_self=ss,
+                                               skip_first=sf, now_ns=t_ns, present=present)
+
+    def UnsubscribeFromChannelBatch(self, conn_slots, channel_ids) -> np.ndarray:
+        n = len(conn_slots)
+        return self.engine.apply_subscriptions(conn_slots, channel_ids, np.full(n, capi.SUBOP_UNSUB, np.uint8))
 
     # -- per client, the entities to spawn / despawn since the last delta: the net effect of the FULL data a new subscription
     # sends, the despawns of an unsubscription and the handovers between cells (spatial.go:612-858,

@@ -411,6 +411,16 @@ struct chd_engine {
         ScanSite site{};
         GraphSet g;
     } fw;
+    // ---- explicit subscriptions (chd_subs.cu): scratch allocated on first use, op arrays grown on demand
+    struct Subs {
+        uint64_t op_cap = 0;  // ops every op array below holds
+        uint32_t *slot = nullptr, *channel = nullptr, *interval = nullptr;
+        int32_t* delay = nullptr;
+        uint8_t *op = nullptr, *present = nullptr, *skip_self = nullptr, *skip_first = nullptr, *status = nullptr;
+        // sort keys and values (first pass by cell, second by slot), each op's slot (S if rejected) and cell index
+        uint32_t *key = nullptr, *key_out = nullptr, *idx1 = nullptr, *idx2 = nullptr, *eff_slot = nullptr, *cell = nullptr;
+        uint32_t *beg = nullptr, *cnt = nullptr, *noff = nullptr;  // [max_subscribers (+2)]: per touched slot its first op / new run length
+    } subs;
 
     bool fail(const char* fmt, ...) const {
         char buf[512];
@@ -606,6 +616,7 @@ chd_status chd_rule_follow(chd_engine* e, const char* fn);
 chd_status chd_rule_no_followers(chd_engine* e, const char* fn);
 chd_status chd_rule_one_batch(chd_engine* e, const char* fn);
 chd_status chd_rule_merged_batch(chd_engine* e, bool adopted);
+chd_status chd_rule_explicit_subs(chd_engine* e, const char* fn);
 // followers (chd_follow.cu): the listed slots (n == 0 with slot == nullptr: every slot) follow nothing from now on; d_slot: the
 // same list on the device if the caller uploaded it already
 chd_status chd_follow_drop(chd_engine* e, const uint32_t* slot, const uint32_t* d_slot, uint32_t n);

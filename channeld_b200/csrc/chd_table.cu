@@ -337,6 +337,14 @@ chd_status chd_rule_merged_batch(chd_engine* e, bool adopted) {
     return CHD_OK;
 }
 
+// 10. Explicit subscriptions (chd_apply_subscriptions) are single-GPU: a slab engine's slots migrate between ranks with their pairs,
+// and the ops would have to follow them.  Refused, like the interest-stage inputs, between chd_begin_interest and its chd_tick.
+chd_status chd_rule_explicit_subs(chd_engine* e, const char* fn) {
+    if (e->slab) return refuse(e, "%s: explicit subscriptions are not available on an engine made a slab (chd_set_slab / chd_comm_init)", fn);
+    if (e->interest_pending) return refuse(e, "%s: chd_begin_interest is pending (not joined by chd_tick yet)", fn);
+    return CHD_OK;
+}
+
 chd_status chd_entity_table_init(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_fresh_engine(e) != CHD_OK) return CHD_ERR_STATE;

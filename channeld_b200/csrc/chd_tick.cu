@@ -35,12 +35,15 @@ static chd_status emit_prep_enqueue(chd_engine* e, cudaStream_t s, bool cta_tile
     // of the copy before it; after a build this is the copy the build already waited for)
     chd_status st = chd_pf_after_read(e, e->pf_copy, set, s);
     if (st == CHD_OK) st = chd_epoch_tick(e, s, EP_EMIT);
+    // the tiles the partition may describe: tile_desc / general_tiles hold one entry per CTA tile of max_visible (+ 8), first_pair
+    // one per warp tile, so a visible count far above max_visible (CHD_OVF_VISIBLE) never writes past either
+    const uint64_t tile_cap = cta_tiles ? (e->lim.max_visible + EMIT_TILE - 1) / EMIT_TILE + 1 : e->max_tiles;
     if (st != CHD_OK) return st;
     return run_stage(e, s, e->g_emit_prep, key, [&]() -> chd_status {
         // per-pair visible counts are computed by the scan itself; the partition pass opens the next epoch
         SCAN(e, exclusive_scan_fn<PairVcountIn, uint64_t>(PairVcountIn{pb.cell, c.cell_start}, c.voff, P, e->site_voff, s, pb.off + S));
         emit_partition_kernel<<<grid, 256, 0, s>>>(pb.off + S, P, c.voff, pb.cell, c.cell_start, c.first_pair, cta_tiles ? c.tile_desc : nullptr,
-                                                   e->max_tiles, S, pb.off, e->d_vis_off, e->lim.max_visible, e->d_ctr, e->d_epoch + EP_EMIT, tile,
+                                                   tile_cap, S, pb.off, e->d_vis_off, e->lim.max_visible, e->d_ctr, e->d_epoch + EP_EMIT, tile,
                                                    c.general_tiles, c.n_general, c.n_visible);
         KCHECK(e);
         return CHD_OK;

@@ -190,6 +190,29 @@ class Engine:
         slots = np.ascontiguousarray(slots, np.uint32)
         self._ck(self.L.chd_remove_subscribers(self.h, ptr(slots), len(slots)))
 
+    def apply_subscriptions(self, slots, channel_ids, ops, interval=None, delay=None, skip_self=None, skip_first=None, now_ns=0, present=None,
+                            status=True):
+        """SUB_TO_CHANNEL / UNSUB_FROM_CHANNEL for spatial channels (include/chd_gpu_subs.h), applied in array order at now_ns.
+        Each option is None (no op carries it) or one value per op; `present` (CHD_SUBOPT_* per op) says which ops carry which
+        option, and defaults to every given option on every op.  Returns the CHD_SUB_* status per op (None with status=False, which
+        adds no host synchronisation)."""
+        slots = np.ascontiguousarray(slots, np.uint32)
+        n = len(slots)
+        arrs = dict(slot=slots, channel_id=np.ascontiguousarray(channel_ids, np.uint32), op=np.ascontiguousarray(ops, np.uint8))
+        mask = np.zeros(n, np.uint8)
+        for name, v, dt, bit in (("interval_ms", interval, np.uint32, capi.SUBOPT_INTERVAL), ("delay_ms", delay, np.int32, capi.SUBOPT_DELAY),
+                                 ("skip_self", skip_self, np.uint8, capi.SUBOPT_SKIP_SELF), ("skip_first", skip_first, np.uint8, capi.SUBOPT_SKIP_FIRST)):
+            if v is not None:
+                arrs[name] = np.ascontiguousarray(np.broadcast_to(np.asarray(v).astype(dt), (n,)))
+                mask |= bit
+        arrs["present"] = mask if present is None else np.ascontiguousarray(present, np.uint8)
+        assert all(len(a) == n for a in arrs.values())
+        b = capi.SubBatch(n=n, **{k: ptr(a) for k, a in arrs.items()})
+        self._keep_subs = arrs  # (the copies are asynchronous without out_status)
+        out = np.zeros(n, np.uint8) if status else None
+        self._ck(self.L.chd_apply_subscriptions(self.h, C.byref(b), int(now_ns), ptr(out)))
+        return out
+
     def query_channel_ids(self, batch, cap=None):
         """-> (status[n], off[n+1], channel_id[], dist[])"""
         n = batch.n

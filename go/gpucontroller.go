@@ -14,6 +14,7 @@ package channeld
 #cgo LDFLAGS: -L${SRCDIR}/../../channeld_b200 -lchd_b200 -Wl,-rpath,${SRCDIR}/../../channeld_b200
 #include <stdlib.h>
 #include "chd_gpu.h"
+#include "chd_gpu_subs.h"
 */
 import "C"
 
@@ -657,6 +658,62 @@ func (ctl *GpuStaticGrid2DSpatialController) RemoveSubscribers(slots []uint32) e
 		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
 	}
 	return nil
+}
+
+// SubOps: the SUB_TO_CHANNEL / UNSUB_FROM_CHANNEL messages of spatial channels collected since the last tick, in arrival order
+// (include/chd_gpu_subs.h).  handleSubToChannel / handleUnsubFromChannel (message.go:488-605) append one row per message whose
+// channel is SPATIAL instead of calling SubscribeToChannel / UnsubscribeFromChannel, and so does the server's subscription to
+// each cell it owns right after CreateChannels (message_spatial.go:167-173, with the server's SubOptions).  Present carries the
+// proto presence of FanOutIntervalMs / FanOutDelayMs / SkipSelfUpdateFanOut / SkipFirstFanOut (CHD_SUBOPT_*); DataAccess and
+// DataFieldMasks stay in the Go ChannelSubscription.  Slot, ChannelId and Op have one entry per op; the other arrays may be left
+// empty when no op carries that field (Present empty: no op carries any).
+type SubOps struct {
+	Slot, ChannelId []uint32
+	Op, Present     []uint8
+	IntervalMs      []uint32
+	DelayMs         []int32
+	SkipSelf        []uint8
+	SkipFirst       []uint8
+}
+
+// ApplySubscriptions applies the ops between two ticks (never between BeginInterest and the tick that joins it) at channel time
+// `now` and returns a CHD_SUB_* status per op, from which the host sends its SubscribedToChannel / UnsubscribedFromChannel replies.
+// The statuses are written before the call returns, so plain Go slices are fine.
+func (ctl *GpuStaticGrid2DSpatialController) ApplySubscriptions(ops *SubOps, now ChannelTime) ([]uint8, error) {
+	n := len(ops.Slot)
+	if n == 0 {
+		return nil, nil
+	}
+	// &b is Go memory holding Go pointers: legal while they are pinned (as in QueryChannelIds); the call is synchronous here
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	// an optional array no op carries may be left empty: it goes to C as NULL
+	u32 := func(s []uint32) *C.uint32_t {
+		if len(s) == 0 {
+			return nil
+		}
+		pin.Pin(&s[0])
+		return (*C.uint32_t)(unsafe.Pointer(&s[0]))
+	}
+	u8 := func(s []uint8) *C.uint8_t {
+		if len(s) == 0 {
+			return nil
+		}
+		pin.Pin(&s[0])
+		return (*C.uint8_t)(unsafe.Pointer(&s[0]))
+	}
+	var delay *C.int32_t
+	if len(ops.DelayMs) > 0 {
+		pin.Pin(&ops.DelayMs[0])
+		delay = (*C.int32_t)(unsafe.Pointer(&ops.DelayMs[0]))
+	}
+	b := C.chd_sub_batch{n: C.uint32_t(n), slot: u32(ops.Slot), channel_id: u32(ops.ChannelId), op: u8(ops.Op), present: u8(ops.Present),
+		interval_ms: u32(ops.IntervalMs), delay_ms: delay, skip_self: u8(ops.SkipSelf), skip_first: u8(ops.SkipFirst)}
+	status := make([]uint8, n)
+	if st := C.chd_apply_subscriptions(ctl.engine, &b, C.int64_t(now), u8(status)); st != C.CHD_OK {
+		return nil, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return status, nil
 }
 
 // CommUniqueId / CommInit / TickSharded: multi-GPU, one channeld process per GPU.  Rank 0 creates the id and ships the 128 bytes to
