@@ -175,6 +175,16 @@ class SubBatch(C.Structure):
                 ("interval_ms", C.c_void_p), ("delay_ms", C.c_void_p), ("skip_self", C.c_void_p), ("skip_first", C.c_void_p)]
 
 
+# every symbol include/chd_gpu_facing.h declares (facings and follower frames; checked by tests/test_facing_host.py against that header)
+FACING_SYMBOLS = ["chd_spawn_entities_facing", "chd_spawn_entities_facing_f32", "chd_move_entities_facing", "chd_move_entities_facing_f32",
+                  "chd_handoff_entities_facing", "chd_follow_set_frame", "chd_get_follow_frame"]
+
+
+class FollowFrameBatch(C.Structure):
+    _fields_ = [("n", C.c_uint32), ("slot", C.c_void_p), ("off_fwd", C.c_void_p), ("off_right", C.c_void_p), ("rot_cos", C.c_void_p),
+                ("rot_sin", C.c_void_p)]
+
+
 STAGE_BUILD, STAGE_INTEREST, STAGE_EMIT, STAGE_EMIT_KERNEL, STAGE_FANOUT, STAGE_TICK, STAGE_EXPORT, STAGE_EXCHANGE, STAGE_IMPORT, STAGE_READBACK, STAGE_VISIBLE_DELTA, STAGE_ENTITY_EVENTS, STAGE_FOLLOW = range(13)
 
 _lib = None
@@ -389,6 +399,18 @@ def lib():
     L.chd_get_follow.argtypes = [vp, vp, vp, vp, vp, vp, C.c_uint32, u32p, u32p]
     L.chd_apply_subscriptions.restype = C.c_int
     L.chd_apply_subscriptions.argtypes = [vp, C.POINTER(SubBatch), C.c_int64, vp]
+    for f in (L.chd_spawn_entities_facing, L.chd_spawn_entities_facing_f32):
+        f.restype = C.c_int
+        f.argtypes = [vp, vp, vp, vp, vp, vp, C.c_uint32, vp]
+    for f in (L.chd_move_entities_facing, L.chd_move_entities_facing_f32):
+        f.restype = C.c_int
+        f.argtypes = [vp, vp, vp, vp, vp, vp, C.c_uint32]
+    L.chd_handoff_entities_facing.restype = C.c_int
+    L.chd_handoff_entities_facing.argtypes = [vp, vp, vp, vp, vp, vp, vp, C.c_uint32, u32p]
+    L.chd_follow_set_frame.restype = C.c_int
+    L.chd_follow_set_frame.argtypes = [vp, C.POINTER(FollowFrameBatch)]
+    L.chd_get_follow_frame.restype = C.c_int
+    L.chd_get_follow_frame.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, u32p]
     _lib = L
     return L
 

@@ -391,6 +391,9 @@ struct chd_engine {
         cudaEvent_t ev_stage[2] = {nullptr, nullptr};
         int next_stage = 0;
         GraphSet g_post;
+        // facings (include/chd_gpu_facing.h), allocated by the first facing call: d_fx / d_fz [N] per slot (0, 0: none), written by
+        // the event kernels and read by the follow stage, both on the engine stream; d_ev_face: [2N] staging of the events' facings
+        double *d_fx = nullptr, *d_fz = nullptr, *d_ev_face = nullptr;
     } tbl;
     // ---- followers (chd_follow.cu): everything is allocated by the first chd_follow_bind
     struct Follow {
@@ -410,6 +413,13 @@ struct chd_engine {
         double *g_cx = nullptr, *g_cz = nullptr;
         ScanSite site{};
         GraphSet g;
+        // frames (chd_follow_set_frame): device state allocated by the first frame; h_frame mirrors fr.on; n_framed counts the bound
+        // followers with a frame, and the generation runs the Frame instantiations only while it is not zero
+        FollowFrame fr{};
+        std::vector<uint8_t> h_frame;
+        uint32_t n_framed = 0;
+        uint32_t* g_fslot = nullptr;  // chd_get_follow_frame's lists: [max_queries] slots, [6][max_queries] doubles
+        double* g_fval = nullptr;
     } fw;
     // ---- explicit subscriptions (chd_subs.cu): scratch allocated on first use, op arrays grown on demand
     struct Subs {
@@ -617,6 +627,7 @@ chd_status chd_rule_no_followers(chd_engine* e, const char* fn);
 chd_status chd_rule_one_batch(chd_engine* e, const char* fn);
 chd_status chd_rule_merged_batch(chd_engine* e, bool adopted);
 chd_status chd_rule_explicit_subs(chd_engine* e, const char* fn);
+chd_status chd_rule_facing(chd_engine* e, const char* fn);
 // followers (chd_follow.cu): the listed slots (n == 0 with slot == nullptr: every slot) follow nothing from now on; d_slot: the
 // same list on the device if the caller uploaded it already
 chd_status chd_follow_drop(chd_engine* e, const uint32_t* slot, const uint32_t* d_slot, uint32_t n);

@@ -11,6 +11,7 @@
 #include "chd_engine.h"
 
 #include "chd_follow.cuh"
+#include "chd_gpu_facing.h"
 #include "chd_misc.cuh"
 
 namespace {
@@ -39,6 +40,45 @@ bool follow_alloc(chd_engine* e) {
     F.h_kind.assign(S, 0);
     F.on = true;
     return true;
+}
+
+// The frame state, at the first chd_follow_set_frame: no slot has a frame yet.
+bool frame_alloc(chd_engine* e) {
+    chd_engine::Follow& F = e->fw;
+    if (F.fr.on) return true;
+    const uint64_t S = e->lim.max_subscribers;
+    FollowFrame d{};
+    bool ok = dalloc(e, &d.on, S);
+    for (double** p : {&d.off_fwd, &d.off_right, &d.rot_cos, &d.rot_sin, &d.last_fx, &d.last_fz, &d.cx, &d.cz, &d.dx, &d.dz}) ok = ok && dalloc(e, p, S);
+    if (!ok) return false;
+    if (cudaMemsetAsync(d.on, 0, S, e->stream) != cudaSuccess) return e->fail("cudaMemsetAsync failed allocating the frame state");
+    F.h_frame.assign(S, 0);
+    F.fr = d;
+    return true;
+}
+
+// The slot's follower is plain again (its device mark is cleared by the caller's kernel)
+void frame_forget(chd_engine::Follow& F, uint32_t s) {
+    if (F.h_frame.empty() || !F.h_frame[s]) return;
+    F.h_frame[s] = 0;
+    F.n_framed--;
+}
+
+// The follow compaction of the generation: the instantiation for the engine's state (served-range check, frames)
+template <bool Merged>
+chd_status follow_compact(chd_engine* e, cudaStream_t s, bool check, bool frame, const FollowEntities& ent, const FollowSlab& slab, uint32_t mode,
+                          uint32_t base) {
+    chd_engine::Follow& F = e->fw;
+    const uint32_t S = e->n_slots;
+    if (frame && check)
+        SCAN(e, compact_1p(FollowFlag<Merged, true, true>{F.st, ent, slab, mode, F.fr}, FollowSink<Merged, true>{F.st, F.q, base, F.fr}, S, F.site, s));
+    else if (frame)
+        SCAN(e, compact_1p(FollowFlag<Merged, false, true>{F.st, ent, slab, mode, F.fr}, FollowSink<Merged, true>{F.st, F.q, base, F.fr}, S, F.site, s));
+    else if (check)
+        SCAN(e, compact_1p(FollowFlag<Merged, true>{F.st, ent, slab, mode}, FollowSink<Merged>{F.st, F.q, base}, S, F.site, s));
+    else
+        SCAN(e, compact_1p(FollowFlag<Merged, false>{F.st, ent, slab, mode}, FollowSink<Merged>{F.st, F.q, base}, S, F.site, s));
+    return CHD_OK;
 }
 
 // `bytes` of host data into the follower staging buffer, before the call returns (the caller's arrays are plain host memory)
@@ -86,8 +126,9 @@ chd_status follow_generate(chd_engine* e, uint32_t mode, const QueryDev& h, uint
     StageTimer timer(e, s, CHD_STAGE_FOLLOW);
     const uint32_t S = e->n_slots, B = F.n_bound, H = (uint32_t)host_class(n_h);
     const Positions p = chd_positions(e);  // (entity-table mode: the front pair)
-    const FollowEntities ent = e->tbl.on ? FollowEntities{p.x, p.z, e->lim.max_entities, e->tbl.d_table, e->tbl.bits, e->tbl.d_id_of_slot}
-                                         : FollowEntities{p.x, p.z, e->n_own, nullptr, 0, nullptr};
+    const FollowEntities ent = e->tbl.on ? FollowEntities{p.x, p.z, e->lim.max_entities, e->tbl.d_table, e->tbl.bits, e->tbl.d_id_of_slot, e->tbl.d_fx, e->tbl.d_fz}
+                                         : FollowEntities{p.x, p.z, e->n_own, nullptr, 0, nullptr, nullptr, nullptr};
+    const bool frame = F.n_framed > 0;  // (entity-table mode only, rule 11)
     // on a slab (entity-table mode: every followed entity is an own one) the columns it serves, with the world's edges left open
     const uint32_t lo = e->slab && e->g.col_lo > e->g.halo ? e->g.col_lo - e->g.halo : 0u;
     const uint32_t hi = e->slab ? (uint32_t)std::min<uint64_t>((uint64_t)e->g.col_hi + e->g.halo, e->g.cols) : e->g.cols;
@@ -97,20 +138,17 @@ chd_status follow_generate(chd_engine* e, uint32_t mode, const QueryDev& h, uint
     if (st != CHD_OK) return st;
     const FollowBatch& q = F.q;
     if (!merged) {
-        // the graph bakes in the slot and follower counts, the mode, where the positions live (the state arrays never move) and the
-        // served columns
-        const uint64_t key = stage_key(0x666f6c6cull, S, B, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub, lo, hi);
+        // the graph bakes in the slot and follower counts, the mode, where the positions and facings live (the state arrays never
+        // move), the served columns and whether frames run
+        const uint64_t key = stage_key(0x666f6c6cull, S, B, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub, lo, hi, frame, ent.fx,
+                                       F.fr.on);
         st = run_stage(e, s, F.g, key, [&]() -> chd_status {
             // the skip tail: entries behind the selected count name no slot and no kind
             CU(e, cudaMemsetAsync(q.sub, 0xFF, 4ull * B, s));
             CU(e, cudaMemsetAsync(q.kind, 0, B, s));
             bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_FOLLOW);
             KCHECK(e);
-            if (check)
-                SCAN(e, compact_1p(FollowFlag<false, true>{F.st, ent, slab, mode}, FollowSink<false>{F.st, q, 0}, S, F.site, s));
-            else
-                SCAN(e, compact_1p(FollowFlag<false, false>{F.st, ent, slab, mode}, FollowSink<false>{F.st, q, 0}, S, F.site, s));
-            return CHD_OK;
+            return follow_compact<false>(e, s, check, frame, ent, slab, mode, 0);
         });
     } else {
         if (h.spot_off && !spot_alloc(e, spots)) return CHD_ERR_CUDA;
@@ -123,7 +161,8 @@ chd_status follow_generate(chd_engine* e, uint32_t mode, const QueryDev& h, uint
         // ... and so do the host part's arrays (the staging set of the query scratch or a prefetch, or the caller's device arrays) and
         // the spot buffer's three arrays: a grown buffer may start where the old one did, but its spot_z and spot_dist move with the
         // capacity
-        const uint64_t key = stage_key(0x666f6c6dull, S, B, H, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub, lo, hi, grid, h.sub, h.kind,
+        const uint64_t key = stage_key(0x666f6c6dull, S, B, H, mode, ent.px, ent.pz, ent.n, ent.table, ent.bits, F.st.kind, q.sub, lo, hi, frame, ent.fx,
+                                       F.fr.on, grid, h.sub, h.kind,
                                        h.sph_cx, h.sph_cz, h.sph_r, h.box_cx, h.box_cz, h.box_ex, h.box_ez, h.cone_cx, h.cone_cz, h.cone_dx, h.cone_dz,
                                        h.cone_angle, h.cone_r, h.spot_off, h.spot_ndist, h.spot_x, h.spot_z, h.spot_dist, q.spot_x, q.spot_z,
                                        q.spot_dist, F.spot_cap);
@@ -132,11 +171,7 @@ chd_status follow_generate(chd_engine* e, uint32_t mode, const QueryDev& h, uint
             KCHECK(e);
             follow_merge_kernel<<<grid, FOLLOW_THREADS, 0, s>>>(m);
             KCHECK(e);
-            if (check)
-                SCAN(e, compact_1p(FollowFlag<true, true>{F.st, ent, slab, mode}, FollowSink<true>{F.st, q, H}, S, F.site, s));
-            else
-                SCAN(e, compact_1p(FollowFlag<true, false>{F.st, ent, slab, mode}, FollowSink<true>{F.st, q, H}, S, F.site, s));
-            return CHD_OK;
+            return follow_compact<true>(e, s, check, frame, ent, slab, mode, H);
         });
     }
     if (st != CHD_OK) return st;
@@ -225,11 +260,12 @@ chd_status chd_follow_bind(chd_engine* e, const chd_follow_batch* b) {
     const uint8_t* d = F.d_stage;
     const FollowStage stage{reinterpret_cast<const uint32_t*>(d + 56 * m), reinterpret_cast<const uint32_t*>(d + 60 * m), d + 64 * m,
                             reinterpret_cast<const double*>(d)};
-    follow_bind_kernel<<<blocks_for(m, FOLLOW_THREADS), FOLLOW_THREADS, 0, e->stream>>>(stage, (uint32_t)m, F.st);
+    follow_bind_kernel<<<blocks_for(m, FOLLOW_THREADS), FOLLOW_THREADS, 0, e->stream>>>(stage, (uint32_t)m, F.st, F.fr.on);
     KCHECK(e);
     for (uint64_t k = 0; k < m; k++) {
         F.n_bound += !F.h_kind[hs[k]];
         F.h_kind[hs[k]] = hk[k];
+        frame_forget(F, hs[k]);
     }
     return CHD_OK;
 }
@@ -240,14 +276,18 @@ chd_status chd_follow_drop(chd_engine* e, const uint32_t* slot, const uint32_t* 
     const uint32_t S = e->lim.max_subscribers;
     if (!slot) {  // every slot
         CU(e, cudaMemsetAsync(F.st.kind, 0, S, e->stream));
+        if (F.fr.on) CU(e, cudaMemsetAsync(F.fr.on, 0, S, e->stream));
         std::fill(F.h_kind.begin(), F.h_kind.end(), (uint8_t)0);
+        std::fill(F.h_frame.begin(), F.h_frame.end(), (uint8_t)0);
         F.n_bound = 0;
+        F.n_framed = 0;
         return CHD_OK;
     }
     uint32_t hit = 0;
     for (uint32_t i = 0; i < n; i++)
         if (slot[i] < S && F.h_kind[slot[i]]) {
             F.h_kind[slot[i]] = 0;
+            frame_forget(F, slot[i]);
             hit++;
         }
     if (!hit) return CHD_OK;
@@ -257,7 +297,7 @@ chd_status chd_follow_drop(chd_engine* e, const uint32_t* slot, const uint32_t* 
         if (st != CHD_OK) return st;
         d_slot = reinterpret_cast<const uint32_t*>(F.d_stage);
     }
-    follow_unbind_kernel<<<blocks_for(n, FOLLOW_THREADS), FOLLOW_THREADS, 0, e->stream>>>(d_slot, n, S, F.st.kind);
+    follow_unbind_kernel<<<blocks_for(n, FOLLOW_THREADS), FOLLOW_THREADS, 0, e->stream>>>(d_slot, n, S, F.st.kind, F.fr.on);
     KCHECK(e);
     return CHD_OK;
 }
@@ -357,6 +397,96 @@ chd_status chd_get_follow(chd_engine* e, uint32_t* slot, uint32_t* entity, uint3
     if (status) CU(e, cudaMemcpyAsync(status, F.g_status, 4 * k, cudaMemcpyDefault, s));
     if (cx) CU(e, cudaMemcpyAsync(cx, F.g_cx, 8 * k, cudaMemcpyDefault, s));
     if (cz) CU(e, cudaMemcpyAsync(cz, F.g_cz, 8 * k, cudaMemcpyDefault, s));
+    CU(e, cudaStreamSynchronize(s));
+    return CHD_OK;
+}
+
+// ---- frames (include/chd_gpu_facing.h)
+
+chd_status chd_follow_set_frame(chd_engine* e, const chd_follow_frame_batch* b) {
+    if (!e || !b || (b->n && !b->slot) || (!b->rot_cos != !b->rot_sin)) return CHD_ERR_INVALID;
+    if (chd_rule_facing(e, "chd_follow_set_frame") != CHD_OK || chd_rule_follow(e, "chd_follow_set_frame") != CHD_OK) return CHD_ERR_STATE;
+    const uint32_t n = b->n;
+    if (!n) return CHD_OK;
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_DEVICE);
+    chd_engine::Follow& F = e->fw;
+    // argument checks first: a refused call frames nothing
+    std::unordered_map<uint32_t, uint32_t> last;  // slot -> its last frame in the call
+    last.reserve(n);
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t s = b->slot[i];
+        if (!F.on || s >= e->lim.max_subscribers || !F.h_kind[s]) {
+            e->fail("chd_follow_set_frame: slot %u follows nothing (chd_follow_bind first)", s);
+            return CHD_ERR_INVALID;
+        }
+        const double v[4] = {b->off_fwd ? b->off_fwd[i] : 0.0, b->off_right ? b->off_right[i] : 0.0, b->rot_cos ? b->rot_cos[i] : 1.0,
+                             b->rot_sin ? b->rot_sin[i] : 0.0};
+        for (double a : v)
+            if (!std::isfinite(a)) {
+                e->fail("chd_follow_set_frame: frame %u (slot %u) has a non-finite offset or rotation", i, s);
+                return CHD_ERR_INVALID;
+            }
+        last[s] = i;
+    }
+    if (!frame_alloc(e)) return CHD_ERR_CUDA;
+    // staged SoA of the m winners: [4][m] doubles (off_fwd, off_right, rot_cos, rot_sin) | slot [m]
+    const uint64_t m = last.size();
+    std::vector<uint8_t> h(m * (4 * 8 + 4));
+    double* v = reinterpret_cast<double*>(h.data());
+    uint32_t* hs = reinterpret_cast<uint32_t*>(h.data() + 32 * m);
+    uint64_t j = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        if (last[b->slot[i]] != i) continue;
+        hs[j] = b->slot[i];
+        v[j] = b->off_fwd ? b->off_fwd[i] : 0.0;
+        v[m + j] = b->off_right ? b->off_right[i] : 0.0;
+        v[2 * m + j] = b->rot_cos ? b->rot_cos[i] : 1.0;
+        v[3 * m + j] = b->rot_sin ? b->rot_sin[i] : 0.0;
+        j++;
+    }
+    chd_status st = stage_upload(e, h.data(), h.size());
+    if (st != CHD_OK) return st;
+    const FollowFrameStage stage{reinterpret_cast<const uint32_t*>(F.d_stage + 32 * m), reinterpret_cast<const double*>(F.d_stage)};
+    follow_frame_kernel<<<blocks_for(m, FOLLOW_THREADS), FOLLOW_THREADS, 0, e->stream>>>(stage, (uint32_t)m, F.st, F.fr);
+    KCHECK(e);
+    for (uint64_t k = 0; k < m; k++) {
+        F.n_framed += !F.h_frame[hs[k]];
+        F.h_frame[hs[k]] = 1;
+    }
+    return CHD_OK;
+}
+
+chd_status chd_get_follow_frame(chd_engine* e, uint32_t* slot, double* fx, double* fz, double* cx, double* cz, double* dx, double* dz, uint32_t cap,
+                                uint32_t* count) {
+    if (!e) return CHD_ERR_INVALID;
+    if (chd_rule_facing(e, "chd_get_follow_frame") != CHD_OK || chd_rule_follow(e, "chd_get_follow_frame") != CHD_OK) return CHD_ERR_STATE;
+    chd_engine::Follow& F = e->fw;
+    if (F.ready || e->interest_pending) {
+        e->fail("chd_get_follow_frame: the generated batch has not been consumed by an interest update yet (or chd_begin_interest is not joined)");
+        return CHD_ERR_STATE;
+    }
+    if (count) *count = 0;
+    if (!F.on || !F.n_framed) return CHD_OK;
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT);
+    cudaStream_t s = e->stream;
+    const uint64_t Q = e->lim.max_queries;
+    if (!F.g_fval && !(dalloc(e, &F.g_fslot, Q + 1) && dalloc(e, &F.g_fval, 6 * Q))) return CHD_ERR_CUDA;  // (g_fval is allocated last)
+    uint32_t* d_count = F.g_fslot + Q;
+    chd_status st = chd_epoch_tick(e, s, EP_FOLLOW);
+    if (st != CHD_OK) return st;
+    bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_FOLLOW);
+    KCHECK(e);
+    SCAN(e, compact_1p(FollowFramedFlag{F.st.kind, F.fr.on}, FollowFrameReportSink{F.fr, F.g_fslot, F.g_fval, (uint32_t)Q, d_count}, e->n_slots, F.site, s));
+    uint32_t m = 0;
+    st = chd_read_u32(e, d_count, &m);
+    if (st != CHD_OK) return st;
+    if (count) *count = m;
+    const uint64_t k = std::min(m, cap);
+    if (!k) return CHD_OK;
+    if (slot) CU(e, cudaMemcpyAsync(slot, F.g_fslot, 4 * k, cudaMemcpyDefault, s));
+    double* out[6] = {fx, fz, cx, cz, dx, dz};
+    for (int a = 0; a < 6; a++)
+        if (out[a]) CU(e, cudaMemcpyAsync(out[a], F.g_fval + a * Q, 8 * k, cudaMemcpyDefault, s));
     CU(e, cudaStreamSynchronize(s));
     return CHD_OK;
 }

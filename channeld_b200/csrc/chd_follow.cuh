@@ -24,6 +24,7 @@ struct FollowEntities {
     const uint64_t* __restrict__ table;  // nullptr: index mode
     uint32_t bits;
     const uint32_t* __restrict__ id_of_slot;
+    const double *__restrict__ fx, *__restrict__ fz;  // the table's facings (include/chd_gpu_facing.h), nullptr: no entity has one
 };
 
 // The columns a slab serves: its queries may touch cells in columns [col_lo - halo, col_hi + halo) (chd_import_halo brings in no
@@ -48,15 +49,33 @@ struct FollowSlab {
     }
 };
 
+// A framed follower's query from its entity at (x, z) with facing (fx, fz), not (0, 0): the centre offset along and across the
+// unit facing and the cone direction turned by the frame's rotation, each step rounded on its own (include/chd_gpu_facing.h).
+struct FramedQuery {
+    double cx, cz, dx, dz;
+    __device__ __forceinline__ FramedQuery(const FollowFrame& fr, uint64_t s, double x, double z, double fx, double fz) {
+        const double m = f64sqrt(f64add(f64mul(fx, fx), f64mul(fz, fz)));
+        const double ux = f64div(fx, m), uz = f64div(fz, m);
+        const double fwd = fr.off_fwd[s], right = fr.off_right[s], rc = fr.rot_cos[s], rs = fr.rot_sin[s];
+        cx = f64sub(f64add(x, f64mul(fwd, ux)), f64mul(right, uz));
+        cz = f64add(f64add(z, f64mul(fwd, uz)), f64mul(right, ux));
+        dx = f64sub(f64mul(fx, rc), f64mul(fz, rs));
+        dz = f64add(f64mul(fx, rs), f64mul(fz, rc));
+    }
+};
+
 // Merged: the batch has a host part (chd_follow_queries_with), whose entries marked their slots in f.ovr.  The flag reads and
 // clears the mark of every slot below the slot count, bound or not, so no mark outlives the generation.  Slab: the served-range
 // check runs (a separate instantiation: its f64 divisions would raise the register count of every engine's compaction).
-template <bool Merged, bool Slab>
+// Frame: some follower has a frame (chd_follow_set_frame).  A framed slot's facing joins the MOVED test, its query is generated
+// from the frame and recorded in fr for FollowSink and chd_get_follow_frame.  Engines without frames run the other instantiations.
+template <bool Merged, bool Slab, bool Frame = false>
 struct FollowFlag {
     FollowDev f;
     FollowEntities ent;
     FollowSlab slab;
     uint32_t mode;
+    FollowFrame fr;  // (Frame only)
     __device__ __forceinline__ bool operator()(uint64_t s) const {
         if (Merged && f.ovr[s]) {  // the slot's explicit query wins this tick; the next MOVED generation selects it again
             f.ovr[s] = 0;
@@ -83,15 +102,48 @@ struct FollowFlag {
             return false;
         }
         const double x = ent.px[p], z = ent.pz[p];
-        const bool moved = __double_as_longlong(x) != __double_as_longlong(f.last_x[s]) || __double_as_longlong(z) != __double_as_longlong(f.last_z[s]);
+        bool moved = __double_as_longlong(x) != __double_as_longlong(f.last_x[s]) || __double_as_longlong(z) != __double_as_longlong(f.last_z[s]);
+        const bool framed = Frame && fr.on[s];
+        double fx = 0.0, fz = 0.0;  // no facing: zero, or a non-finite component
+        if (framed) {
+            if (ent.fx) {
+                fx = ent.fx[p];
+                fz = ent.fz[p];
+                if (!isfinite(fx) || !isfinite(fz) || (fx == 0.0 && fz == 0.0)) fx = fz = 0.0;
+            }
+            moved = moved || __double_as_longlong(fx) != __double_as_longlong(fr.last_fx[s]) || __double_as_longlong(fz) != __double_as_longlong(fr.last_fz[s]);
+        }
         if (mode == (uint32_t)CHD_FOLLOW_MOVED && !f.dirty[s] && !moved) {
             f.res[s] = FOLLOW_NO_QUERY | (uint32_t)CHD_FOLLOW_NOT_SELECTED;
             return false;
         }
-        if (Slab && slab.outside(f, s, f.kind[s], x)) {  // no query; the centre stays the last generated one, and it counts as moved
-            f.res[s] = FOLLOW_NO_QUERY | (uint32_t)CHD_FOLLOW_OUTSIDE_SLAB;
-            f.dirty[s] = 1;
-            return false;
+        double cx = x;
+        if (!Frame) {
+            if (Slab && slab.outside(f, s, f.kind[s], x)) {  // no query; the centre stays the last generated one, and it counts as moved
+                f.res[s] = FOLLOW_NO_QUERY | (uint32_t)CHD_FOLLOW_OUTSIDE_SLAB;
+                f.dirty[s] = 1;
+                return false;
+            }
+        } else {
+            double cz = z, dx = 0.0, dz = 0.0;
+            if (framed) {
+                if (fx != 0.0 || fz != 0.0) {
+                    const FramedQuery g(fr, s, x, z, fx, fz);
+                    cx = g.cx; cz = g.cz; dx = g.dx; dz = g.dz;
+                } else {  // no facing: the plain query
+                    dx = f.cone_dx[s];
+                    dz = f.cone_dz[s];
+                }
+            }
+            if (Slab && slab.outside(f, s, f.kind[s], cx)) {  // (the offset centre)
+                f.res[s] = FOLLOW_NO_QUERY | (uint32_t)CHD_FOLLOW_OUTSIDE_SLAB;
+                f.dirty[s] = 1;
+                return false;
+            }
+            if (framed) {
+                fr.last_fx[s] = fx; fr.last_fz[s] = fz;
+                fr.cx[s] = cx; fr.cz[s] = cz; fr.dx[s] = dx; fr.dz[s] = dz;
+            }
         }
         f.last_x[s] = x;
         f.last_z[s] = z;
@@ -100,16 +152,19 @@ struct FollowFlag {
     }
 };
 
-// Merged: the followers' entries start at `base` (the host part's size class H).
-template <bool Merged>
+// Merged: the followers' entries start at `base` (the host part's size class H).  Frame: a framed slot's centre and cone direction
+// are the ones its flag call recorded in fr.
+template <bool Merged, bool Frame = false>
 struct FollowSink {
     FollowDev f;
     FollowBatch q;
     uint32_t base;
+    FollowFrame fr;  // (Frame only)
     __device__ __forceinline__ void operator()(uint64_t s, uint32_t r) const {
         const uint32_t k = Merged ? base + r : r;
         const uint32_t kind = f.kind[s];
-        const double x = f.last_x[s], z = f.last_z[s];  // (written by this thread's flag call)
+        const bool framed = Frame && fr.on[s];
+        const double x = framed ? fr.cx[s] : f.last_x[s], z = framed ? fr.cz[s] : f.last_z[s];  // (written by this thread's flag call)
         q.sub[k] = (uint32_t)s;
         q.kind[k] = (uint8_t)kind;
         if (kind & CHD_AOI_SPHERE) {
@@ -119,7 +174,9 @@ struct FollowSink {
             q.box_cx[k] = x; q.box_cz[k] = z; q.box_ex[k] = f.box_ex[s]; q.box_ez[k] = f.box_ez[s];
         }
         if (kind & CHD_AOI_CONE) {
-            q.cone_cx[k] = x; q.cone_cz[k] = z; q.cone_dx[k] = f.cone_dx[s]; q.cone_dz[k] = f.cone_dz[s];
+            q.cone_cx[k] = x; q.cone_cz[k] = z;
+            q.cone_dx[k] = framed ? fr.dx[s] : f.cone_dx[s];
+            q.cone_dz[k] = framed ? fr.dz[s] : f.cone_dz[s];
             q.cone_angle[k] = f.cone_angle[s]; q.cone_r[k] = f.cone_r[s];
         }
         f.res[s] = k;
@@ -145,6 +202,29 @@ struct FollowReportSink {
         status[k] = (r & FOLLOW_NO_QUERY) ? (r & ~FOLLOW_NO_QUERY) : qstatus[r];
         cx[k] = f.last_x[s];
         cz[k] = f.last_z[s];
+    }
+    __device__ __forceinline__ void total(uint32_t c) const { *count = c; }
+};
+
+// chd_get_follow_frame: the framed followers in ascending slot order with the facing, centre and direction of their last query.
+struct FollowFramedFlag {
+    const uint8_t *__restrict__ kind, *__restrict__ on;
+    __device__ __forceinline__ bool operator()(uint64_t s) const { return kind[s] != 0 && on[s] != 0; }
+};
+struct FollowFrameReportSink {
+    FollowFrame fr;
+    uint32_t* __restrict__ slot;
+    double* __restrict__ out;  // [6][cap]: fx, fz, cx, cz, dx, dz
+    uint32_t cap;
+    uint32_t* __restrict__ count;
+    __device__ __forceinline__ void operator()(uint64_t s, uint32_t k) const {
+        slot[k] = (uint32_t)s;
+        out[k] = fr.last_fx[s];
+        out[(uint64_t)cap + k] = fr.last_fz[s];
+        out[2ull * cap + k] = fr.cx[s];
+        out[3ull * cap + k] = fr.cz[s];
+        out[4ull * cap + k] = fr.dx[s];
+        out[5ull * cap + k] = fr.dz[s];
     }
     __device__ __forceinline__ void total(uint32_t c) const { *count = c; }
 };
@@ -216,7 +296,8 @@ struct FollowStage {
     const uint8_t* __restrict__ kind;
     const double* __restrict__ shape;  // [7][m]: sph_r, box_ex, box_ez, cone_dx, cone_dz, cone_angle, cone_r
 };
-__global__ void __launch_bounds__(FOLLOW_THREADS) follow_bind_kernel(FollowStage st, uint32_t m, FollowDev f) {
+// frame_on: the frame marks once frames exist (a re-bind makes the slot plain), else nullptr
+__global__ void __launch_bounds__(FOLLOW_THREADS) follow_bind_kernel(FollowStage st, uint32_t m, FollowDev f, uint8_t* __restrict__ frame_on) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
     const uint32_t s = st.slot[i];
@@ -234,12 +315,38 @@ __global__ void __launch_bounds__(FOLLOW_THREADS) follow_bind_kernel(FollowStage
     f.dirty[s] = 1;
     f.tslot[s] = TBL_NONE;
     f.res[s] = FOLLOW_NO_QUERY | (uint32_t)CHD_FOLLOW_NOT_SELECTED;
+    if (frame_on) frame_on[s] = 0;
 }
 
-// chd_follow_unbind / chd_remove_subscribers: the listed slots follow nothing (slots beyond the state are ignored)
-__global__ void __launch_bounds__(FOLLOW_THREADS) follow_unbind_kernel(const uint32_t* __restrict__ slot, uint32_t n, uint32_t n_state, uint8_t* __restrict__ kind) {
+// chd_follow_unbind / chd_remove_subscribers: the listed slots follow nothing (slots beyond the state are ignored); frame_on as
+// for follow_bind_kernel
+__global__ void __launch_bounds__(FOLLOW_THREADS) follow_unbind_kernel(const uint32_t* __restrict__ slot, uint32_t n, uint32_t n_state, uint8_t* __restrict__ kind,
+                                                                       uint8_t* __restrict__ frame_on) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && slot[i] < n_state) kind[slot[i]] = 0;
+    if (i < n && slot[i] < n_state) {
+        kind[slot[i]] = 0;
+        if (frame_on) frame_on[slot[i]] = 0;
+    }
+}
+
+// chd_follow_set_frame: scatter m staged frames (one per slot) into the frame state.  The slot turns dirty, so the next MOVED
+// generation selects it, and its read-back is zero until then.
+struct FollowFrameStage {
+    const uint32_t* __restrict__ slot;
+    const double* __restrict__ v;  // [4][m]: off_fwd, off_right, rot_cos, rot_sin
+};
+__global__ void __launch_bounds__(FOLLOW_THREADS) follow_frame_kernel(FollowFrameStage st, uint32_t m, FollowDev f, FollowFrame fr) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const uint32_t s = st.slot[i];
+    fr.on[s] = 1;
+    fr.off_fwd[s] = st.v[i];
+    fr.off_right[s] = st.v[(uint64_t)m + i];
+    fr.rot_cos[s] = st.v[2ull * m + i];
+    fr.rot_sin[s] = st.v[3ull * m + i];
+    fr.last_fx[s] = fr.last_fz[s] = 0.0;
+    fr.cx[s] = fr.cz[s] = fr.dx[s] = fr.dz[s] = 0.0;
+    f.dirty[s] = 1;
 }
 
 }  // namespace chd

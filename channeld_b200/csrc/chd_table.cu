@@ -3,6 +3,7 @@
 // high-volume path, resolve their ids on the device.
 #include "chd_engine.h"
 
+#include "chd_gpu_facing.h"
 #include "chd_table.cuh"
 
 #include <unordered_set>
@@ -64,23 +65,44 @@ chd_status put_status(chd_engine* e, uint8_t* out, const std::vector<uint8_t>& s
     return CHD_OK;
 }
 
-// Uploads m (id, slot) pairs and, with positions, their x / z (as doubles) into the device event staging on the engine stream.
+// The facing storage (include/chd_gpu_facing.h), at the first facing call: every slot has no facing.
+chd_status facing_alloc(chd_engine* e) {
+    chd_engine::Table& t = e->tbl;
+    if (t.d_fx) return CHD_OK;
+    const uint64_t N = e->lim.max_entities;
+    double *fx = nullptr, *ev = nullptr;
+    if (!dalloc(e, &fx, 2 * N) || !dalloc(e, &ev, 2 * N)) return CHD_ERR_CUDA;
+    CU(e, cudaMemsetAsync(fx, 0, 16 * N, e->stream));
+    t.d_fx = fx;
+    t.d_fz = fx + N;
+    t.d_ev_face = ev;
+    return CHD_OK;
+}
+
+// Uploads m (id, slot) pairs and, with positions, their x / z (as doubles) into the device event staging on the engine stream; with
+// facings (fx != nullptr) their fx / fz into the facing staging.
 chd_status upload_events(chd_engine* e, const std::vector<uint32_t>& id, const std::vector<uint32_t>& slot, const std::vector<double>* x,
-                         const std::vector<double>* z) {
+                         const std::vector<double>* z, const std::vector<double>* fx = nullptr, const std::vector<double>* fz = nullptr) {
     chd_engine::Table& t = e->tbl;
     const uint64_t m = id.size();
     if (!m) return CHD_OK;
     int k = 0;
     uint8_t* h = nullptr;
-    chd_status st = take_stage(e, m * (x ? 24 : 8), &k, &h);
+    const uint64_t lead = (x ? 16 * m : 0) + (fx ? 16 * m : 0);  // x | z | fx | fz, then id | slot
+    chd_status st = take_stage(e, lead + 8 * m, &k, &h);
     if (st != CHD_OK) return st;
-    uint32_t* hi = reinterpret_cast<uint32_t*>(h + (x ? 16 * m : 0));
+    uint32_t* hi = reinterpret_cast<uint32_t*>(h + lead);
     memcpy(hi, id.data(), 4 * m);
     memcpy(hi + m, slot.data(), 4 * m);
     if (x) {
         memcpy(h, x->data(), 8 * m);
         memcpy(h + 8 * m, z->data(), 8 * m);
         CU(e, cudaMemcpyAsync(t.d_ev_pos, h, 16 * m, cudaMemcpyHostToDevice, e->stream));
+    }
+    if (fx) {
+        memcpy(h + 16 * m, fx->data(), 8 * m);
+        memcpy(h + 24 * m, fz->data(), 8 * m);
+        CU(e, cudaMemcpyAsync(t.d_ev_face, h + 16 * m, 16 * m, cudaMemcpyHostToDevice, e->stream));
     }
     CU(e, cudaMemcpyAsync(t.d_ev, hi, 8 * m, cudaMemcpyHostToDevice, e->stream));
     CU(e, cudaEventRecord(t.ev_stage[k], e->stream));
@@ -124,32 +146,38 @@ chd_status check_events(chd_engine* e, const char* fn, const uint32_t* id, const
     return CHD_OK;
 }
 
-chd_status spawn(chd_engine* e, const uint32_t* id_in, const void* x_in, const void* z_in, bool f32, uint32_t n, uint8_t* out_status) {
+// n values of a host or device array as doubles: the float form widens exactly, as chd_set_entities_f32 does
+chd_status widened(chd_engine* e, const void* in, bool f32, uint32_t n, std::vector<double>& out) {
+    out.resize(n);
+    chd_status st = CHD_OK;
+    if (f32) {
+        std::vector<float> keep;
+        const float* p = nullptr;
+        if ((st = host_view(e, (const float*)in, n, keep, &p)) != CHD_OK) return st;
+        for (uint32_t i = 0; i < n; i++) out[i] = (double)p[i];
+    } else {
+        std::vector<double> keep;
+        const double* p = nullptr;
+        if ((st = host_view(e, (const double*)in, n, keep, &p)) != CHD_OK) return st;
+        std::copy(p, p + n, out.begin());
+    }
+    return CHD_OK;
+}
+
+// fx_in == nullptr: no facing (chd_spawn_entities); the facings are written once the storage exists
+chd_status spawn(chd_engine* e, const uint32_t* id_in, const void* x_in, const void* z_in, bool f32, uint32_t n, uint8_t* out_status,
+                 const void* fx_in = nullptr, const void* fz_in = nullptr) {
     chd_engine::Table& t = e->tbl;
     std::vector<uint32_t> kid;
     const uint32_t* ids = nullptr;
     chd_status st = host_view(e, id_in, n, kid, &ids);
     if (st != CHD_OK) return st;
-    // positions as doubles: the float form widens exactly, as chd_set_entities_f32 does
-    std::vector<double> px(n), pz(n);
-    if (f32) {
-        std::vector<float> kx, kz;
-        const float *fx = nullptr, *fz = nullptr;
-        if ((st = host_view(e, (const float*)x_in, n, kx, &fx)) != CHD_OK || (st = host_view(e, (const float*)z_in, n, kz, &fz)) != CHD_OK) return st;
-        for (uint32_t i = 0; i < n; i++) {
-            px[i] = (double)fx[i];
-            pz[i] = (double)fz[i];
-        }
-    } else {
-        std::vector<double> kx, kz;
-        const double *dx = nullptr, *dz = nullptr;
-        if ((st = host_view(e, (const double*)x_in, n, kx, &dx)) != CHD_OK || (st = host_view(e, (const double*)z_in, n, kz, &dz)) != CHD_OK) return st;
-        std::copy(dx, dx + n, px.begin());
-        std::copy(dz, dz + n, pz.begin());
-    }
+    std::vector<double> px, pz, pfx, pfz;
+    if ((st = widened(e, x_in, f32, n, px)) != CHD_OK || (st = widened(e, z_in, f32, n, pz)) != CHD_OK) return st;
+    if (fx_in && ((st = widened(e, fx_in, f32, n, pfx)) != CHD_OK || (st = widened(e, fz_in, f32, n, pfz)) != CHD_OK)) return st;
     std::vector<uint8_t> status(n, (uint8_t)CHD_EV_OK);
     std::vector<uint32_t> aid, aslot;
-    std::vector<double> ax, az;
+    std::vector<double> ax, az, afx, afz;
     std::unordered_set<uint32_t> seen;
     seen.reserve(n);
     for (uint32_t i = 0; i < n; i++) {
@@ -172,6 +200,10 @@ chd_status spawn(chd_engine* e, const uint32_t* id_in, const void* x_in, const v
         aslot.push_back(slot);
         ax.push_back(px[i]);
         az.push_back(pz[i]);
+        if (fx_in) {
+            afx.push_back(pfx[i]);
+            afz.push_back(pfz[i]);
+        }
     }
     const uint64_t m = aid.size();
     if (m) {
@@ -182,17 +214,19 @@ chd_status spawn(chd_engine* e, const uint32_t* id_in, const void* x_in, const v
         }
         for (uint64_t j = 0; j < m; j++) t.slot_of[aid[j]] = aslot[j];
         t.used += m;
-        st = upload_events(e, aid, aslot, &ax, &az);
+        st = upload_events(e, aid, aslot, &ax, &az, fx_in ? &afx : nullptr, fx_in ? &afz : nullptr);
         if (st != CHD_OK) return st;
         tbl_spawn_kernel<<<grid_for(e, m), TBL_THREADS, 0, e->stream>>>(t.d_table, t.bits, t.d_ev, t.d_ev + m, t.d_ev_pos, t.d_ev_pos + m, (uint32_t)m,
-                                                                       t.d_id_of_slot, chd_pos_front(e).x, chd_pos_front(e).z, t.d_flag);
+                                                                       t.d_id_of_slot, chd_pos_front(e).x, chd_pos_front(e).z, t.d_flag,
+                                                                       fx_in ? t.d_ev_face : nullptr, fx_in ? t.d_ev_face + m : nullptr, t.d_fx, t.d_fz);
         KCHECK(e);
         touched(e);
     }
     return put_status(e, out_status, status);
 }
 
-chd_status move(chd_engine* e, const uint32_t* id, const void* x, const void* z, bool f32, uint32_t n) {
+// fx == nullptr: the facings stay (chd_move_entities)
+chd_status move(chd_engine* e, const uint32_t* id, const void* x, const void* z, bool f32, uint32_t n, const void* fx = nullptr, const void* fz = nullptr) {
     const uint64_t N = e->lim.max_entities;
     chd_engine::Table& t = e->tbl;
     const PosSet& front = chd_pos_front(e);
@@ -213,10 +247,24 @@ chd_status move(chd_engine* e, const uint32_t* id, const void* x, const void* z,
         dx = base;
         dz = base + w * N;
     }
+    const void *dfx = fx, *dfz = fz;
+    if (fx && !(chd_is_device_ptr(e, fx) && chd_is_device_ptr(e, fz))) {
+        uint8_t* base = reinterpret_cast<uint8_t*>(t.d_ev_face);
+        CU(e, cudaMemcpyAsync(base, fx, w * n, cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(base + w * N, fz, w * n, cudaMemcpyDefault, s));
+        dfx = base;
+        dfz = base + w * N;
+    }
     const unsigned grid = grid_for(e, n);
     tbl_move_resolve_kernel<<<grid, TBL_THREADS, 0, s>>>(t.d_table, t.bits, did, n, t.d_mslot, t.d_winner, t.d_stats);
     KCHECK(e);
-    if (f32)
+    if (f32 && fx)
+        tbl_move_apply_kernel<float, true><<<grid, TBL_THREADS, 0, s>>>(t.d_mslot, t.d_winner, (const float*)dx, (const float*)dz, n, front.x, front.z, t.d_stats,
+                                                                        (const float*)dfx, (const float*)dfz, t.d_fx, t.d_fz);
+    else if (fx)
+        tbl_move_apply_kernel<double, true><<<grid, TBL_THREADS, 0, s>>>(t.d_mslot, t.d_winner, (const double*)dx, (const double*)dz, n, front.x, front.z,
+                                                                         t.d_stats, (const double*)dfx, (const double*)dfz, t.d_fx, t.d_fz);
+    else if (f32)
         tbl_move_apply_kernel<float><<<grid, TBL_THREADS, 0, s>>>(t.d_mslot, t.d_winner, (const float*)dx, (const float*)dz, n, front.x, front.z, t.d_stats);
     else
         tbl_move_apply_kernel<double><<<grid, TBL_THREADS, 0, s>>>(t.d_mslot, t.d_winner, (const double*)dx, (const double*)dz, n, front.x, front.z, t.d_stats);
@@ -224,6 +272,10 @@ chd_status move(chd_engine* e, const uint32_t* id, const void* x, const void* z,
     touched(e);
     return CHD_OK;
 }
+
+chd_status handoff_check(chd_engine* e, const char* fn);
+chd_status handoff(chd_engine* e, const char* fn, uint32_t* id, uint32_t* dst_rank, double* x, double* z, double* fx, double* fz, uint32_t cap,
+                   uint32_t* count);
 
 template <typename... A>
 chd_status refuse(const chd_engine* e, const char* fmt, A... a) {
@@ -343,6 +395,12 @@ chd_status chd_rule_explicit_subs(chd_engine* e, const char* fn) {
     if (e->slab) return refuse(e, "%s: explicit subscriptions are not available on an engine made a slab (chd_set_slab / chd_comm_init)", fn);
     if (e->interest_pending) return refuse(e, "%s: chd_begin_interest is pending (not joined by chd_tick yet)", fn);
     return CHD_OK;
+}
+
+// 11. Facings and frames (include/chd_gpu_facing.h) need entity-table mode: index mode's positions come from host snapshots and the
+// prefetch pair, and a facing there would be a third pipelined input.  The frame calls follow rule 9 as well.
+chd_status chd_rule_facing(chd_engine* e, const char* fn) {
+    return e->tbl.on ? CHD_OK : refuse(e, "%s: facings and follower frames need entity-table mode (chd_entity_table_init)", fn);
 }
 
 chd_status chd_entity_table_init(chd_engine* e) {
@@ -478,14 +536,78 @@ chd_status chd_get_entity_stats(chd_engine* e, chd_entity_stats* out) {
 
 chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank, double* x, double* z, uint32_t cap, uint32_t* count) {
     if (!e || !count || (cap && (!id || !dst_rank || !x || !z))) return CHD_ERR_INVALID;
-    if (chd_rule_table(e, "chd_handoff_entities") != CHD_OK) return CHD_ERR_STATE;
+    if (handoff_check(e, "chd_handoff_entities") != CHD_OK) return CHD_ERR_STATE;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    return handoff(e, "chd_handoff_entities", id, dst_rank, x, z, nullptr, nullptr, cap, count);
+}
+
+chd_status chd_handoff_entities_facing(chd_engine* e, uint32_t* id, uint32_t* dst_rank, double* x, double* z, double* fx, double* fz, uint32_t cap,
+                                       uint32_t* count) {
+    if (!e || !count || (cap && (!id || !dst_rank || !x || !z || !fx || !fz))) return CHD_ERR_INVALID;
+    if (chd_rule_facing(e, "chd_handoff_entities_facing") != CHD_OK || handoff_check(e, "chd_handoff_entities_facing") != CHD_OK) return CHD_ERR_STATE;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    const chd_status st = facing_alloc(e);
+    if (st != CHD_OK) return st;
+    return handoff(e, "chd_handoff_entities_facing", id, dst_rank, x, z, fx, fz, cap, count);
+}
+
+// ---- facings (include/chd_gpu_facing.h)
+
+chd_status chd_spawn_entities_facing(chd_engine* e, const uint32_t* id, const double* x, const double* z, const double* fx, const double* fz, uint32_t n,
+                                     uint8_t* out_status) {
+    if (e && n && (!fx || !fz)) return CHD_ERR_INVALID;
+    chd_status st = check_events(e, "chd_spawn_entities_facing", id, x, z, n, false);
+    if (st != CHD_OK) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    if ((st = facing_alloc(e)) != CHD_OK) return st;
+    return spawn(e, id, x, z, false, n, out_status, fx, fz);
+}
+chd_status chd_spawn_entities_facing_f32(chd_engine* e, const uint32_t* id, const float* x, const float* z, const float* fx, const float* fz, uint32_t n,
+                                         uint8_t* out_status) {
+    if (e && n && (!fx || !fz)) return CHD_ERR_INVALID;
+    chd_status st = check_events(e, "chd_spawn_entities_facing_f32", id, x, z, n, false);
+    if (st != CHD_OK) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    if ((st = facing_alloc(e)) != CHD_OK) return st;
+    return spawn(e, id, x, z, true, n, out_status, fx, fz);
+}
+
+chd_status chd_move_entities_facing(chd_engine* e, const uint32_t* id, const double* x, const double* z, const double* fx, const double* fz, uint32_t n) {
+    if (e && n && (!fx || !fz)) return CHD_ERR_INVALID;
+    chd_status st = check_events(e, "chd_move_entities_facing", id, x, z, n, true);
+    if (st != CHD_OK) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    if ((st = facing_alloc(e)) != CHD_OK || !n) return st;
+    return move(e, id, x, z, false, n, fx, fz);
+}
+chd_status chd_move_entities_facing_f32(chd_engine* e, const uint32_t* id, const float* x, const float* z, const float* fx, const float* fz, uint32_t n) {
+    if (e && n && (!fx || !fz)) return CHD_ERR_INVALID;
+    chd_status st = check_events(e, "chd_move_entities_facing_f32", id, x, z, n, true);
+    if (st != CHD_OK) return st;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    if ((st = facing_alloc(e)) != CHD_OK || !n) return st;
+    return move(e, id, x, z, true, n, fx, fz);
+}
+
+}  // extern "C"
+
+namespace {
+
+// the mode rule and the call order of a hand-off
+chd_status handoff_check(chd_engine* e, const char* fn) {
+    if (chd_rule_table(e, fn) != CHD_OK) return CHD_ERR_STATE;
     if (!e->assigned) {
         // the keys must describe the current positions: a spawn, move, despawn or hand-off since the last assignment changed them
-        e->fail("chd_handoff_entities needs a cell assignment after the last spawn / move / despawn / hand-off (chd_export_border, "
-                "chd_assign_cells, chd_build or a tick)");
+        e->fail("%s needs a cell assignment after the last spawn / move / despawn / hand-off (chd_export_border, chd_assign_cells, chd_build or a "
+                "tick)", fn);
         return CHD_ERR_STATE;
     }
-    CHD_ENTER(e, ENTRY_DEVICE);
+    return CHD_OK;
+}
+
+// chd_handoff_entities(_facing), named fn in errors: fx == nullptr lists no facings
+chd_status handoff(chd_engine* e, const char* fn, uint32_t* id, uint32_t* dst_rank, double* x, double* z, double* fx, double* fz, uint32_t cap,
+                   uint32_t* count) {
     chd_engine::Table& t = e->tbl;
     const PosSet& front = chd_pos_front(e);
     cudaStream_t s = e->stream;
@@ -498,14 +620,19 @@ chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank,
     if (st != CHD_OK) return st;
     bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_BORDER);
     KCHECK(e);
-    SCAN(e, compact_1p(HandoffFlag{e->g, e->d_key},
-                       HandoffSink{e->g, world, e->d_key, chd_entity_ids(e), front.x, front.z, d_id, d_slot, d_dst, d_hx, d_hz, e->d_boff}, e->n_own,
-                       e->site_border, s));
+    HandoffSink sink{e->g, world, e->d_key, chd_entity_ids(e), front.x, front.z, d_id, d_slot, d_dst, d_hx, d_hz, e->d_boff};
+    if (fx) {  // the facings go to the facing staging, copied out before the despawn pass below removes the entities
+        sink.pfx = t.d_fx;
+        sink.pfz = t.d_fz;
+        sink.fx = t.d_ev_face;
+        sink.fz = t.d_ev_face + N;
+    }
+    SCAN(e, compact_1p(HandoffFlag{e->g, e->d_key}, sink, e->n_own, e->site_border, s));
     st = chd_read_u32(e, e->d_boff, count);
     if (st != CHD_OK) return st;
     const uint32_t m = *count;
     if (m > cap) {  // transactional: nothing removed, a repeat call with a larger buffer lists the same entities
-        e->fail("chd_handoff_entities: %u entities to hand off > cap %u", m, cap);
+        e->fail("%s: %u entities to hand off > cap %u", fn, m, cap);
         return CHD_ERR_CAPACITY;
     }
     if (!m) return CHD_OK;
@@ -513,6 +640,10 @@ chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank,
     CU(e, cudaMemcpyAsync(dst_rank, d_dst, 4ull * m, cudaMemcpyDefault, s));
     CU(e, cudaMemcpyAsync(x, d_hx, 8ull * m, cudaMemcpyDefault, s));
     CU(e, cudaMemcpyAsync(z, d_hz, 8ull * m, cudaMemcpyDefault, s));
+    if (fx) {
+        CU(e, cudaMemcpyAsync(fx, t.d_ev_face, 8ull * m, cudaMemcpyDefault, s));
+        CU(e, cudaMemcpyAsync(fz, t.d_ev_face + N, 8ull * m, cudaMemcpyDefault, s));
+    }
     std::vector<uint32_t> hid(m), hslot(m);
     CU(e, cudaMemcpyAsync(hid.data(), d_id, 4ull * m, cudaMemcpyDeviceToHost, s));
     CU(e, cudaMemcpyAsync(hslot.data(), d_slot, 4ull * m, cudaMemcpyDeviceToHost, s));
@@ -529,6 +660,10 @@ chd_status chd_handoff_entities(chd_engine* e, uint32_t* id, uint32_t* dst_rank,
     touched(e);
     return CHD_OK;
 }
+
+}  // namespace
+
+extern "C" {
 
 // After every table-mode build into copy-input set `c`, on the build's stream: its id-valued sorted entity array and, after a fresh
 // cell assignment, the handover list in ids without the slots spawned or despawned since the previous one (then the flags clear).

@@ -13,10 +13,12 @@ namespace chd {
 
 constexpr int TBL_THREADS = 256;
 
-// Spawn apply (x != nullptr): insert (id, slot), slot -> id, the position, flag the slot.  Rebuild (x == nullptr): insert only.
+// Spawn apply (x != nullptr): insert (id, slot), slot -> id, the position, flag the slot, and once facings exist (pfx != nullptr)
+// the facing (fx == nullptr: none).  Rebuild (x == nullptr): insert only.
 __global__ void __launch_bounds__(TBL_THREADS) tbl_spawn_kernel(uint64_t* table, uint32_t bits, const uint32_t* __restrict__ id, const uint32_t* __restrict__ slot,
                                                                 const double* __restrict__ x, const double* __restrict__ z, uint32_t n, uint32_t* id_of_slot,
-                                                                double* px, double* pz, uint8_t* flag) {
+                                                                double* px, double* pz, uint8_t* flag, const double* __restrict__ fx = nullptr,
+                                                                const double* __restrict__ fz = nullptr, double* pfx = nullptr, double* pfz = nullptr) {
     const uint64_t mask = (1ull << bits) - 1ull;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint64_t w = (uint64_t)id[i] << 32 | slot[i];
@@ -27,6 +29,10 @@ __global__ void __launch_bounds__(TBL_THREADS) tbl_spawn_kernel(uint64_t* table,
         px[slot[i]] = x[i];
         pz[slot[i]] = z[i];
         flag[slot[i]] = 1;
+        if (pfx) {
+            pfx[slot[i]] = fx ? fx[i] : 0.0;
+            pfz[slot[i]] = fx ? fz[i] : 0.0;
+        }
     }
 }
 
@@ -65,11 +71,13 @@ __global__ void __launch_bounds__(TBL_THREADS) tbl_move_resolve_kernel(const uin
     tbl_block_count(stats + 1, unknown);
 }
 
-// Move, pass 2: the winner of each slot writes the position (f32 widened exactly, as widen_positions_kernel does) and clears its
-// election for the next call; the others count as superseded.
-template <typename T>
+// Move, pass 2: the winner of each slot writes the position (f32 widened exactly, as widen_positions_kernel does) and, with Facing,
+// its facing, and clears its election for the next call; the others count as superseded.
+template <typename T, bool Facing = false>
 __global__ void __launch_bounds__(TBL_THREADS) tbl_move_apply_kernel(const uint32_t* __restrict__ mslot, uint32_t* winner, const T* __restrict__ x,
-                                                                     const T* __restrict__ z, uint32_t n, double* px, double* pz, unsigned long long* stats) {
+                                                                     const T* __restrict__ z, uint32_t n, double* px, double* pz, unsigned long long* stats,
+                                                                     const T* __restrict__ fx = nullptr, const T* __restrict__ fz = nullptr,
+                                                                     double* pfx = nullptr, double* pfz = nullptr) {
     uint32_t applied = 0, superseded = 0;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint32_t s = mslot[i];
@@ -77,6 +85,10 @@ __global__ void __launch_bounds__(TBL_THREADS) tbl_move_apply_kernel(const uint3
         if (winner[s] == i + 1) {
             px[s] = (double)x[i];
             pz[s] = (double)z[i];
+            if (Facing) {
+                pfx[s] = (double)fx[i];
+                pfz[s] = (double)fz[i];
+            }
             winner[s] = 0;
             applied++;
         } else {
@@ -97,7 +109,7 @@ __global__ void __launch_bounds__(TBL_THREADS) tbl_gather_ids_kernel(const uint3
 }
 
 // chd_handoff_entities, one compaction (compact_1p): the own in-world slots whose column lies outside this rank's slab, with their
-// id, the rank owning that column, their slot and their position.
+// id, the rank owning that column, their slot and their position (chd_handoff_entities_facing: and their facing).
 struct HandoffFlag {
     GridDev g;
     const uint32_t* __restrict__ key;
@@ -117,12 +129,18 @@ struct HandoffSink {
     uint32_t *__restrict__ id, *__restrict__ slot, *__restrict__ dst;
     double *__restrict__ x, *__restrict__ z;
     uint32_t* __restrict__ count;
+    const double *__restrict__ pfx = nullptr, *__restrict__ pfz = nullptr;  // facings to copy out (nullptr: none)
+    double *__restrict__ fx = nullptr, *__restrict__ fz = nullptr;
     __device__ __forceinline__ void operator()(uint64_t i, uint32_t k) const {
         id[k] = ids.at((uint32_t)i);
         slot[k] = (uint32_t)i;
         dst[k] = slab_owner(key[i] % g.cols, g.cols, world);
         x[k] = px[i];
         z[k] = pz[i];
+        if (pfx) {
+            fx[k] = pfx[i];
+            fz[k] = pfz[i];
+        }
     }
     __device__ __forceinline__ void total(uint32_t c) const { *count = c; }
 };

@@ -214,6 +214,15 @@ struct FollowDev {
     uint8_t* ovr;             // a host entry of the merged batch names the slot (set by follow_merge_kernel, cleared by FollowFlag)
 };
 
+// Frames of followers (chd_follow_set_frame, include/chd_gpu_facing.h), [max_subscribers] each, allocated by the first frame.
+// on == 0: the slot's follower is plain.
+struct FollowFrame {
+    uint8_t* on;
+    double *off_fwd, *off_right, *rot_cos, *rot_sin;
+    double *last_fx, *last_fz;  // the facing the last query was generated from (0, 0: none)
+    double *cx, *cz, *dx, *dz;  // that query's centre and cone direction (chd_get_follow_frame)
+};
+
 // The generated batch: a query batch's SoA in device memory.  The spot arrays and `missing` are used by merged batches only.
 struct FollowBatch {
     uint32_t* sub;

@@ -420,6 +420,33 @@ class Engine:
     def move_entities_f32(self, ids, x, z):
         self._events(self.L.chd_move_entities_f32, ids, x, z, np.float32, status=False)
 
+    # facings (include/chd_gpu_facing.h, entity-table mode): (fx, fz) per id, (cos yaw, sin yaw); (0, 0) or non-finite = none
+    def spawn_entities_facing(self, ids, x, z, fx, fz):
+        """-> per-event status (capi.EV_*)."""
+        return self._facing_events(self.L.chd_spawn_entities_facing, ids, x, z, fx, fz, np.float64, True)
+
+    def spawn_entities_facing_f32(self, ids, x, z, fx, fz):
+        return self._facing_events(self.L.chd_spawn_entities_facing_f32, ids, x, z, fx, fz, np.float32, True)
+
+    def move_entities_facing(self, ids, x, z, fx, fz):
+        """Position and facing together; the facing of an id's last move in the call wins with its position."""
+        self._facing_events(self.L.chd_move_entities_facing, ids, x, z, fx, fz, np.float64, False)
+
+    def move_entities_facing_f32(self, ids, x, z, fx, fz):
+        self._facing_events(self.L.chd_move_entities_facing_f32, ids, x, z, fx, fz, np.float32, False)
+
+    def _facing_events(self, fn, ids, x, z, fx, fz, dtype, status):
+        arrs = [a if hasattr(a, "data_ptr") else np.ascontiguousarray(a, dt) for a, dt in
+                ((ids, np.uint32), (x, dtype), (z, dtype), (fx, dtype), (fz, dtype))]
+        n = len(arrs[0])
+        if not status:
+            self._keep_moves = arrs  # the H2D copy is asynchronous: referenced until the next move
+            self._ck(fn(self.h, *(ptr(a) for a in arrs), n))
+            return None
+        st = np.zeros(n, np.uint8)
+        self._ck(fn(self.h, *(ptr(a) for a in arrs), n, ptr(st)))
+        return st
+
     def entity_stats(self):
         s = capi.EntityStats()
         self._ck(self.L.chd_get_entity_stats(self.h, C.byref(s)))
@@ -473,6 +500,36 @@ class Engine:
         if k:
             self._ck(self.L.chd_get_follow(self.h, ptr(slot), ptr(ent), ptr(st), ptr(cx), ptr(cz), k, None, None))
         return dict(slot=slot, entity=ent, status=st, cx=cx, cz=cz, n_selected=sel.value)
+
+    def follow_set_frame(self, slots, off_fwd=None, off_right=None, rot=None):
+        """Frames of bound followers (include/chd_gpu_facing.h): centre offsets along / to the right of the entity's facing, and
+        rot=(cos, sin) arrays turning the cone relative to the facing (None: the identity)."""
+        slots = np.ascontiguousarray(slots, np.uint32)
+        n = len(slots)
+        keep = [slots]
+
+        def arr(a):
+            if a is None:
+                return None
+            a = np.ascontiguousarray(np.broadcast_to(np.asarray(a, np.float64), (n,)))
+            keep.append(a)
+            return ptr(a)
+
+        b = capi.FollowFrameBatch(n=n, slot=ptr(slots), off_fwd=arr(off_fwd), off_right=arr(off_right))
+        if rot is not None:
+            b.rot_cos, b.rot_sin = arr(rot[0]), arr(rot[1])
+        self._ck(self.L.chd_follow_set_frame(self.h, C.byref(b)))
+
+    def get_follow_frame(self):
+        """-> dict(slot, fx, fz, cx, cz, dx, dz): every framed follower in slot order with the facing, centre and cone direction
+        of its last query."""
+        n = C.c_uint32()
+        self._ck(self.L.chd_get_follow_frame(self.h, None, None, None, None, None, None, None, 0, C.byref(n)))
+        k = n.value
+        out = dict(slot=np.zeros(k, np.uint32), **{a: np.zeros(k) for a in ("fx", "fz", "cx", "cz", "dx", "dz")})
+        if k:
+            self._ck(self.L.chd_get_follow_frame(self.h, *(ptr(out[a]) for a in ("slot", "fx", "fz", "cx", "cz", "dx", "dz")), k, C.byref(n)))
+        return out
 
     def device_view(self, which):
         p, n = C.c_void_p(), C.c_uint64()
@@ -547,6 +604,21 @@ class Engine:
         self._ck(st)
         k = n.value
         return ids[:k].copy(), dst[:k].copy(), x[:k].copy(), z[:k].copy()
+
+    def handoff_entities_facing(self, cap=1 << 16):
+        """handoff_entities with each entity's facing -> (id, dst_rank, x, z, fx, fz); the receiving rank adopts them with
+        spawn_entities_facing(id, x, z, fx, fz)."""
+        n = C.c_uint32()
+        while True:
+            ids, dst = np.zeros(cap, np.uint32), np.zeros(cap, np.uint32)
+            x, z, fx, fz = np.zeros(cap), np.zeros(cap), np.zeros(cap), np.zeros(cap)
+            st = self.L.chd_handoff_entities_facing(self.h, ptr(ids), ptr(dst), ptr(x), ptr(z), ptr(fx), ptr(fz), int(cap), C.byref(n))
+            if st != capi.ERR_CAPACITY or n.value <= cap:
+                break
+            cap = n.value
+        self._ck(st)
+        k = n.value
+        return ids[:k].copy(), dst[:k].copy(), x[:k].copy(), z[:k].copy(), fx[:k].copy(), fz[:k].copy()
 
     def comm_info(self):
         r, w, ver = C.c_int(), C.c_int(), C.c_int()

@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "../../include/chd_gpu.h"
+#include "../../include/chd_gpu_facing.h"
 
 namespace channeld {
 
@@ -240,6 +241,29 @@ class GpuStaticGrid2DSpatialController {
             return h;
         }
     }
+    // HandoffEntities with each entity's facing (include/chd_gpu_facing.h, 0, 0: none); the destination adopts with SpawnObjectsFacing
+    struct HandoffFacing {
+        std::vector<uint32_t> net_id, dst_rank;
+        std::vector<double> x, z, fx, fz;
+    };
+    HandoffFacing HandoffEntitiesFacing(uint32_t cap = 1024) {
+        for (;;) {
+            const size_t c = cap ? cap : 1;
+            HandoffFacing h{std::vector<uint32_t>(c), std::vector<uint32_t>(c), std::vector<double>(c), std::vector<double>(c), std::vector<double>(c),
+                            std::vector<double>(c)};
+            uint32_t n = 0;
+            const chd_status st =
+                chd_handoff_entities_facing(engine_, h.net_id.data(), h.dst_rank.data(), h.x.data(), h.z.data(), h.fx.data(), h.fz.data(), cap, &n);
+            if (st == CHD_ERR_CAPACITY && n > cap) {  // nothing was removed: ask again with room for the whole list
+                cap = n;
+                continue;
+            }
+            check(st);
+            for (auto* v : {&h.x, &h.z, &h.fx, &h.fz}) v->resize(n);
+            h.net_id.resize(n), h.dst_rank.resize(n);
+            return h;
+        }
+    }
 
     // Recipients of BroadcastType_ADJACENT_CHANNELS messages (message.go:188-239), batched: CSR of subscriber slots.
     struct BroadcastSets {
@@ -342,6 +366,35 @@ class GpuStaticGrid2DSpatialController {
     // over.  Consumed like FollowQueries' batch; the followers' statuses start at the explicit part's size class (chd_gpu.h).
     void FollowQueriesWith(const chd_query_batch* explicit_part, uint32_t mode = CHD_FOLLOW_MOVED) {
         check(chd_follow_queries_with(engine_, mode, explicit_part));
+    }
+    // Followers that turn with their pawn (entity-table mode, include/chd_gpu_facing.h): the moves carry the facing (cos yaw, sin
+    // yaw) of FRepMovement.rotation, and a framed follower is centred off_fwd ahead of / off_right to the right of its pawn, its cone
+    // along the facing turned by (rot_cos, rot_sin).  A bind clears the frame: SetFollowFrames after every FollowEntities of the slot.
+    void SpawnObjectsFacing(const std::vector<uint32_t>& net_id, const std::vector<float>& x, const std::vector<float>& z, const std::vector<float>& fx,
+                            const std::vector<float>& fz, std::vector<uint8_t>* status = nullptr) {
+        Table();
+        std::vector<uint8_t> st(net_id.size());
+        check(chd_spawn_entities_facing_f32(engine_, net_id.data(), x.data(), z.data(), fx.data(), fz.data(), (uint32_t)net_id.size(), st.data()));
+        if (status) *status = std::move(st);
+    }
+    // stream-ordered like MoveEntities
+    void MoveEntitiesFacing(const uint32_t* net_id, const float* x, const float* z, const float* fx, const float* fz, uint32_t n) {
+        Table();
+        check(chd_move_entities_facing_f32(engine_, net_id, x, z, fx, fz, n));
+    }
+    void SetFollowFrames(const chd_follow_frame_batch& b) { check(chd_follow_set_frame(engine_, &b)); }
+    struct FollowFrames {
+        std::vector<uint32_t> slot;
+        std::vector<double> fx, fz, cx, cz, dx, dz;
+    };
+    FollowFrames GetFollowFrames() {
+        FollowFrames f;
+        uint32_t n = 0;
+        check(chd_get_follow_frame(engine_, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, &n));
+        f.slot.resize(n);
+        for (auto* v : {&f.fx, &f.fz, &f.cx, &f.cz, &f.dx, &f.dz}) v->resize(n);
+        if (n) check(chd_get_follow_frame(engine_, f.slot.data(), f.fx.data(), f.fz.data(), f.cx.data(), f.cz.data(), f.dx.data(), f.dz.data(), n, &n));
+        return f;
     }
     chd_entity_stats GetEntityStats() {
         chd_entity_stats s{};

@@ -139,20 +139,25 @@ class EntityRouter:
     def _rank_of_ids(self, ids):
         return np.array([self.owner.get(int(i), -1) for i in ids], np.int64)
 
-    def spawn(self, ids, x, z):
-        """-> per rank (ids u32, x, z).  An id that is already live goes to its owner (which reports it as a duplicate)."""
+    @staticmethod
+    def _facing(fx, fz):
+        return () if fx is None else (np.asarray(fx), np.asarray(fz))
+
+    def spawn(self, ids, x, z, fx=None, fz=None):
+        """-> per rank (ids u32, x, z), or (ids, x, z, fx, fz) for chd_spawn_entities_facing when facings are given.  An id that is
+        already live goes to its owner (which reports it as a duplicate)."""
         ids = np.asarray(ids, np.uint32)
         rank = self.owner_of_x(x)
         known = self._rank_of_ids(ids)
         rank = np.where(known >= 0, known, rank)
         for i, r in zip(ids.tolist(), rank.tolist()):
             self.owner.setdefault(i, r)
-        return self._split(rank, ids, np.asarray(x, np.float64), np.asarray(z, np.float64))
+        return self._split(rank, ids, np.asarray(x, np.float64), np.asarray(z, np.float64), *self._facing(fx, fz))
 
-    def move(self, ids, x, z):
-        """-> per rank (ids u32, x, z) for chd_move_entities."""
+    def move(self, ids, x, z, fx=None, fz=None):
+        """-> per rank (ids u32, x, z) for chd_move_entities, or (ids, x, z, fx, fz) for chd_move_entities_facing."""
         ids = np.asarray(ids, np.uint32)
-        return self._split(self._rank_of_ids(ids), ids, np.asarray(x), np.asarray(z))
+        return self._split(self._rank_of_ids(ids), ids, np.asarray(x), np.asarray(z), *self._facing(fx, fz))
 
     def despawn(self, ids):
         """-> per rank ids u32; the ids leave the map."""
@@ -164,15 +169,24 @@ class EntityRouter:
 
     def handoff(self, lists):
         """lists[r] = rank r's chd_handoff_entities result (id, dst_rank, x, z) -> per rank (ids u32, x, z) to adopt with
-        chd_spawn_entities; every listed id is owned by its destination from now on."""
-        out = [([], [], []) for _ in range(self.world)]
-        for ids, dst, x, z in lists:
-            for i, d, xi, zi in zip(np.asarray(ids).tolist(), np.asarray(dst).tolist(), np.asarray(x), np.asarray(z)):
+        chd_spawn_entities; every listed id is owned by its destination from now on.  With chd_handoff_entities_facing results
+        (id, dst_rank, x, z, fx, fz) the batches are (ids, x, z, fx, fz) for chd_spawn_entities_facing; when only some lists carry
+        facings, the entities of the others get none (0, 0)."""
+        facing = any(len(l) == 6 for l in lists)
+        out = [tuple([] for _ in range(5 if facing else 3)) for _ in range(self.world)]
+        for l in lists:
+            if len(l) not in (4, 6):
+                raise ValueError("a hand-off list is (id, dst_rank, x, z) or (id, dst_rank, x, z, fx, fz)")
+            ids, dst = l[0], l[1]
+            cols = [np.asarray(a) for a in l[2:4]]
+            if facing:
+                cols += [np.asarray(a) for a in l[4:6]] if len(l) == 6 else [np.zeros(len(cols[0]))] * 2
+            for k, (i, d) in enumerate(zip(np.asarray(ids).tolist(), np.asarray(dst).tolist())):
                 self.owner[i] = d
                 out[d][0].append(i)
-                out[d][1].append(xi)
-                out[d][2].append(zi)
-        return [(np.asarray(a, np.uint32), np.asarray(b, np.float64), np.asarray(c, np.float64)) for a, b, c in out]
+                for c, a in enumerate(cols):
+                    out[d][1 + c].append(a[k])
+        return [(np.asarray(o[0], np.uint32),) + tuple(np.asarray(a, np.float64) for a in o[1:]) for o in out]
 
 
 class FollowerRegistry:
@@ -190,24 +204,36 @@ class FollowerRegistry:
     the binding does not travel in the migration blob, so the destination binds them again."""
 
     SHAPE = ("sph_r", "box_ex", "box_ez", "cone_dx", "cone_dz", "cone_angle", "cone_r")
+    FRAME = ("off_fwd", "off_right", "rot_cos", "rot_sin")
 
     def __init__(self, world: int):
         self.world = int(world)
         self.slots = SlotTable(world)
         self.bind = {}  # connection -> (entity id, kind, shape: 7 floats in SHAPE order)
+        self.frame = {}  # connection -> 4 floats in FRAME order (chd_follow_set_frame), for framed followers only
         self._rebind = set()  # connections bound since the last plan()
 
-    def follow(self, conn, entity, kind, shape):
-        """Binds (or re-binds) a connection; it is placed or re-bound by the next plan()."""
+    def follow(self, conn, entity, kind, shape, frame=None):
+        """Binds (or re-binds) a connection; it is placed or re-bound by the next plan().  frame: (off_fwd, off_right) or
+        (off_fwd, off_right, rot_cos, rot_sin) for a follower that turns with its entity (include/chd_gpu_facing.h), None: plain."""
         shape = tuple(float(v) for v in shape)
         if len(shape) != 7:
             raise ValueError("a follower's shape is 7 values: " + ", ".join(self.SHAPE))
         self.bind[conn] = (int(entity), int(kind), shape)
+        self.frame.pop(conn, None)
+        if frame is not None:
+            frame = tuple(float(v) for v in frame)
+            if len(frame) == 2:
+                frame += (1.0, 0.0)
+            if len(frame) != 4:
+                raise ValueError("a follower's frame is 2 or 4 values: " + ", ".join(self.FRAME))
+            self.frame[conn] = frame
         self._rebind.add(conn)
 
     def unfollow(self, conn):
         """Forgets a connection -> (rank, slot) it occupied (chd_remove_subscribers there), or None if it was never placed."""
         self.bind.pop(conn, None)
+        self.frame.pop(conn, None)
         self._rebind.discard(conn)
         return self.slots.remove(conn) if conn in self.slots.owner else None
 
@@ -215,7 +241,9 @@ class FollowerRegistry:
         return self.slots.owner.get(conn)
 
     def batch(self, conns):
-        """The chd_follow_bind arrays of `conns` (placed connections): dict(slot u32, entity u32, kind u8, shape f64 [7][m])."""
+        """The chd_follow_bind arrays of `conns` (placed connections): dict(slot u32, entity u32, kind u8, shape f64 [7][m]), and,
+        when some of them have a frame, frame: their chd_follow_set_frame arrays, dict(slot u32, off_fwd, off_right, rot_cos,
+        rot_sin), to apply after the bind."""
         conns = list(conns)
         m = len(conns)
         out = dict(slot=np.array([self.slots.slot[c] for c in conns], np.uint32),
@@ -223,12 +251,19 @@ class FollowerRegistry:
                    kind=np.array([self.bind[c][1] for c in conns], np.uint8),
                    shape=np.array([self.bind[c][2] for c in conns], np.float64).reshape(m, 7).T.copy())
         out["conn"] = conns
+        framed = [c for c in conns if c in self.frame]
+        if not framed:
+            return out
+        fr = np.array([self.frame[c] for c in framed], np.float64).reshape(len(framed), 4).T
+        out["frame"] = dict(slot=np.array([self.slots.slot[c] for c in framed], np.uint32),
+                            **{k: fr[i].copy() for i, k in enumerate(self.FRAME)})
         return out
 
     def plan(self, router):
         """One tick's placement: -> (arrivals, out_lists, in_calls, vacated, binds) where the first four are plan_migrations' (by
         connection) and binds[rank] is the chd_follow_bind batch (FollowerRegistry.batch) of the connections that arrive on `rank`
-        this tick, or were re-bound there with follow(), in connection order."""
+        this tick, or were re-bound there with follow(), in connection order, with the frames to set after it when it has framed
+        followers (binds[rank]["frame"]: a bind clears a slot's frame, and frames do not travel with migrations either)."""
         conns = sorted(c for c, (e, _, _) in self.bind.items() if e in router.owner)
         new_owner = {c: router.owner[self.bind[c][0]] for c in conns}
         arrivals, out_lists, in_calls, vacated = plan_migrations(self.slots, new_owner)

@@ -15,6 +15,7 @@ package channeld
 #include <stdlib.h>
 #include "chd_gpu.h"
 #include "chd_gpu_subs.h"
+#include "chd_gpu_facing.h"
 */
 import "C"
 
@@ -572,6 +573,74 @@ func (ctl *GpuStaticGrid2DSpatialController) MoveEntities(netIds []uint32, x, z 
 	return nil
 }
 
+// MoveEntitiesFacing is MoveEntities with each move's facing (cos yaw, sin yaw of FRepMovement.rotation; include/chd_gpu_facing.h):
+// the Merge hook appends it beside the location, 20 bytes per move.  The facing of an id's winning move wins with its position; a
+// facing of (0, 0) or with a non-finite component is none.  Arrays in C memory as for MoveEntities.  UN-RUN like the rest of this file.
+func (ctl *GpuStaticGrid2DSpatialController) MoveEntitiesFacing(netIds []uint32, x, z, fx, fz []float32) error {
+	n := len(netIds)
+	if len(x) != n || len(z) != n || len(fx) != n || len(fz) != n {
+		return errors.New("MoveEntitiesFacing: array sizes differ")
+	}
+	if err := ctl.entityTable(); err != nil || n == 0 {
+		return err
+	}
+	if st := C.chd_move_entities_facing_f32(ctl.engine, (*C.uint32_t)(unsafe.Pointer(&netIds[0])), (*C.float)(unsafe.Pointer(&x[0])),
+		(*C.float)(unsafe.Pointer(&z[0])), (*C.float)(unsafe.Pointer(&fx[0])), (*C.float)(unsafe.Pointer(&fz[0])), C.uint32_t(n)); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
+// SpawnObjectsFacing is SpawnObjects with each entity's facing; it returns one CHD_EV_* status per entity.
+func (ctl *GpuStaticGrid2DSpatialController) SpawnObjectsFacing(netIds []uint32, x, z, fx, fz []float32) ([]uint8, error) {
+	n := len(netIds)
+	if len(x) != n || len(z) != n || len(fx) != n || len(fz) != n {
+		return nil, errors.New("SpawnObjectsFacing: array sizes differ")
+	}
+	if err := ctl.entityTable(); err != nil || n == 0 {
+		return nil, err
+	}
+	st := make([]uint8, n)
+	if r := C.chd_spawn_entities_facing_f32(ctl.engine, (*C.uint32_t)(unsafe.Pointer(&netIds[0])), (*C.float)(unsafe.Pointer(&x[0])),
+		(*C.float)(unsafe.Pointer(&z[0])), (*C.float)(unsafe.Pointer(&fx[0])), (*C.float)(unsafe.Pointer(&fz[0])), C.uint32_t(n),
+		(*C.uint8_t)(unsafe.Pointer(&st[0]))); r != C.CHD_OK {
+		return nil, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return st, nil
+}
+
+// SetFollowFrames gives bound followers a frame (chd_follow_set_frame): the centre offFwd ahead of and offRight to the right of the
+// pawn, the cone along its facing turned by (rotCos, rotSin) (nil: the identity).  A bind clears the frame.  UN-RUN like the rest of
+// this file.
+func (ctl *GpuStaticGrid2DSpatialController) SetFollowFrames(slots []uint32, offFwd, offRight, rotCos, rotSin []float64) error {
+	n := len(slots)
+	if len(offFwd) != n || len(offRight) != n || (rotCos == nil) != (rotSin == nil) || (rotCos != nil && (len(rotCos) != n || len(rotSin) != n)) {
+		return errors.New("SetFollowFrames: array sizes differ")
+	}
+	if n == 0 {
+		return nil
+	}
+	cs := (*C.uint32_t)(C.malloc(C.size_t(4 * n)))
+	cv := (*C.double)(C.malloc(C.size_t(8 * 4 * n)))
+	defer C.free(unsafe.Pointer(cs))
+	defer C.free(unsafe.Pointer(cv))
+	copy(unsafe.Slice((*uint32)(unsafe.Pointer(cs)), n), slots)
+	v := unsafe.Slice((*float64)(unsafe.Pointer(cv)), 4*n)
+	copy(v[:n], offFwd)
+	copy(v[n:2*n], offRight)
+	at := func(k int) *C.double { return (*C.double)(unsafe.Add(unsafe.Pointer(cv), 8*k*n)) }
+	b := C.chd_follow_frame_batch{n: C.uint32_t(n), slot: cs, off_fwd: at(0), off_right: at(1)}
+	if rotCos != nil {
+		copy(v[2*n:3*n], rotCos)
+		copy(v[3*n:], rotSin)
+		b.rot_cos, b.rot_sin = at(2), at(3)
+	}
+	if st := C.chd_follow_set_frame(ctl.engine, &b); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
 func (ctl *GpuStaticGrid2DSpatialController) EntityStats() (C.chd_entity_stats, error) {
 	var s C.chd_entity_stats
 	if st := C.chd_get_entity_stats(ctl.engine, &s); st != C.CHD_OK {
@@ -805,6 +874,59 @@ func (ctl *GpuStaticGrid2DSpatialController) HandoffEntities(capEntities int) (n
 		k := int(n)
 		return netIds[:k], dstRank[:k], x[:k], z[:k], nil
 	}
+}
+
+// HandoffEntitiesFacing is HandoffEntities with each entity's facing (include/chd_gpu_facing.h; 0, 0: none).  The destination adopts
+// the entities with SpawnObjectsFacing, so the tick after a slab crossing is exact.  UN-RUN like the rest of this file.
+func (ctl *GpuStaticGrid2DSpatialController) HandoffEntitiesFacing(capEntities int) (netIds, dstRank []uint32, x, z, fx, fz []float64, err error) {
+	for {
+		netIds, dstRank = make([]uint32, capEntities+1), make([]uint32, capEntities+1)
+		x, z = make([]float64, capEntities+1), make([]float64, capEntities+1)
+		fx, fz = make([]float64, capEntities+1), make([]float64, capEntities+1)
+		var n C.uint32_t
+		st := C.chd_handoff_entities_facing(ctl.engine, (*C.uint32_t)(unsafe.Pointer(&netIds[0])), (*C.uint32_t)(unsafe.Pointer(&dstRank[0])),
+			(*C.double)(unsafe.Pointer(&x[0])), (*C.double)(unsafe.Pointer(&z[0])), (*C.double)(unsafe.Pointer(&fx[0])),
+			(*C.double)(unsafe.Pointer(&fz[0])), C.uint32_t(capEntities), &n)
+		if st == C.CHD_ERR_CAPACITY && int(n) > capEntities {
+			capEntities = int(n)
+			continue
+		}
+		if st != C.CHD_OK {
+			return nil, nil, nil, nil, nil, nil, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+		}
+		k := int(n)
+		return netIds[:k], dstRank[:k], x[:k], z[:k], fx[:k], fz[:k], nil
+	}
+}
+
+// FollowFrames is chd_get_follow_frame: every framed follower in slot order with the facing its last query used (0, 0: none), that
+// query's centre and its cone direction.
+type FollowFrames struct {
+	Slot                   []uint32
+	Fx, Fz, Cx, Cz, Dx, Dz []float64
+}
+
+func (ctl *GpuStaticGrid2DSpatialController) GetFollowFrames() (FollowFrames, error) {
+	var f FollowFrames
+	var n C.uint32_t
+	if st := C.chd_get_follow_frame(ctl.engine, nil, nil, nil, nil, nil, nil, nil, 0, &n); st != C.CHD_OK {
+		return f, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	k := int(n)
+	if k == 0 {
+		return f, nil
+	}
+	f.Slot = make([]uint32, k)
+	vals := [6]*[]float64{&f.Fx, &f.Fz, &f.Cx, &f.Cz, &f.Dx, &f.Dz}
+	for _, v := range vals {
+		*v = make([]float64, k)
+	}
+	d := func(v []float64) *C.double { return (*C.double)(unsafe.Pointer(&v[0])) }
+	if st := C.chd_get_follow_frame(ctl.engine, (*C.uint32_t)(unsafe.Pointer(&f.Slot[0])), d(f.Fx), d(f.Fz), d(f.Cx), d(f.Cz), d(f.Dx), d(f.Dz),
+		C.uint32_t(k), &n); st != C.CHD_OK {
+		return FollowFrames{}, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return f, nil
 }
 
 // RingsInit / RingsAppend: ChannelData.OnUpdate's buffer on the GPU (data.go:149-173); updOff is the CSR by cell of this tick's
