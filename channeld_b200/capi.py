@@ -185,6 +185,10 @@ class FollowFrameBatch(C.Structure):
                 ("rot_sin", C.c_void_p)]
 
 
+# every symbol include/chd_gpu_rings.h declares (ring limits across slabs; checked by tests/test_rings_host.py against that header)
+RING_SYMBOLS = ["chd_export_ring_limits", "chd_import_ring_limits"]
+
+
 STAGE_BUILD, STAGE_INTEREST, STAGE_EMIT, STAGE_EMIT_KERNEL, STAGE_FANOUT, STAGE_TICK, STAGE_EXPORT, STAGE_EXCHANGE, STAGE_IMPORT, STAGE_READBACK, STAGE_VISIBLE_DELTA, STAGE_ENTITY_EVENTS, STAGE_FOLLOW = range(13)
 
 _lib = None
@@ -411,6 +415,10 @@ def lib():
     L.chd_follow_set_frame.argtypes = [vp, C.POINTER(FollowFrameBatch)]
     L.chd_get_follow_frame.restype = C.c_int
     L.chd_get_follow_frame.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, C.c_uint32, u32p]
+    L.chd_export_ring_limits.restype = C.c_int
+    L.chd_export_ring_limits.argtypes = [vp, vp, C.c_uint32, u32p]
+    L.chd_import_ring_limits.restype = C.c_int
+    L.chd_import_ring_limits.argtypes = [vp, vp, C.c_uint32]
     _lib = L
     return L
 

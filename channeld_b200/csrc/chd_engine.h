@@ -287,6 +287,14 @@ struct chd_engine {
     uint64_t upd_arrival_cap = 0, upd_sender_cap = 0;
     uint32_t* d_ring_scan_scratch = nullptr;
     uint32_t* d_cell_max_interval = nullptr;  // [C] ChannelData.maxFanOutIntervalMs (subscription.go:84-86)
+    // ring limits on slabs (include/chd_gpu_rings.h), allocated by their first use: the exported shadow of d_cell_max_interval [C],
+    // the record count of an export through chd_export_ring_limits, the export compaction's scan site
+    uint32_t *d_ring_lim_x = nullptr, *d_ring_lim_n = nullptr;
+    ScanSite site_ring_lim{};
+    // a communicator engine's chd_rings_append only uploads its updates into d_upd_*: chd_tick_sharded appends them after the
+    // ring-limit import (rule 12)
+    bool rings_staged = false;
+    uint32_t staged_updates = 0;
     int64_t* d_cell_start_ns = nullptr;       // [C] per-channel ChannelTime origin (chd_set_channel_start_times) or nullptr
     bool have_cell_start = false;
     // the rings the fan-out and payload kernels read (chd_ring_view adds `start`): the staging copies above, the caller's device
@@ -313,6 +321,10 @@ struct chd_engine {
     uint64_t rec_stride_words = 0;    // words one rank contributes to the all-gather (border records + migration blob)
     uint32_t mig_subs = 0, mig_pairs = 0;  // migration blob capacities (0: no subscriber migration)
     bool mig_packed = false;          // chd_migrate_out was called for the coming tick
+    // the ring-limit section of a contribution (after the migration blob): its word offset and its record capacity, the largest
+    // served-cell count of any rank.  Layout: [count, 3 words of padding, 2 x u32 per record]
+    uint64_t ring_sec_off = 0;
+    uint32_t ring_sec_cap = 0;
     uint32_t *d_rec_local = nullptr, *d_rec_all = nullptr;
     unsigned long long* assign_bump = nullptr;  // epoch the next assign_cells_kernel launch bumps for its caller (border export)
     // peer exchange (chd_shard.cuh): this rank's window, the peers' windows mapped with CUDA IPC, device-side sequence / counts
@@ -628,6 +640,10 @@ chd_status chd_rule_one_batch(chd_engine* e, const char* fn);
 chd_status chd_rule_merged_batch(chd_engine* e, bool adopted);
 chd_status chd_rule_explicit_subs(chd_engine* e, const char* fn);
 chd_status chd_rule_facing(chd_engine* e, const char* fn);
+chd_status chd_rule_ring_limits(chd_engine* e, const char* fn);
+chd_status chd_rule_rings_staged(chd_engine* e, const char* fn);
+// device-owned rings (chd_tick.cu): the append kernel on `s` over n_updates updates already uploaded into d_upd_*
+chd_status chd_rings_apply(chd_engine* e, cudaStream_t s, uint32_t n_updates);
 // followers (chd_follow.cu): the listed slots (n == 0 with slot == nullptr: every slot) follow nothing from now on; d_slot: the
 // same list on the device if the caller uploaded it already
 chd_status chd_follow_drop(chd_engine* e, const uint32_t* slot, const uint32_t* d_slot, uint32_t n);

@@ -280,6 +280,7 @@ static chd_status interest_enqueue(chd_engine* e, cudaStream_t s, const QueryDev
 
 chd_status chd_update_interest(chd_engine* e, const chd_query_batch* q, int64_t now_ns) {
     if (!e) return CHD_ERR_INVALID;
+    if (chd_rule_rings_staged(e, "chd_update_interest") != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
     return chd_update_interest_on(e, e->stream, q, now_ns);
 }

@@ -9,6 +9,8 @@
 #include <dlfcn.h>
 #include <nccl.h>  // types and prototypes only; every call goes through the table below
 
+#include "chd_gpu_rings.h"
+
 #include "chd_shard.cuh"
 
 namespace {
@@ -100,10 +102,10 @@ chd_status chd_export_border(chd_engine* e, uint32_t* d_records, uint32_t cap_re
         if (to_peers) {
             PeerWindows pw{};
             for (int r = 0; r < e->comm_world; r++) pw.base[r] = (uint32_t*)e->peer_base[r];
-            const uint64_t blob_words = e->rec_stride_words - 2ull * e->rec_per_rank;
+            const uint64_t blob_words = e->ring_sec_off - 2ull * e->rec_per_rank;
             peer_push_kernel<<<(unsigned)std::min<uint64_t>((uint64_t)e->sm_count, 8 + (2ull * cap_records * e->comm_world) / 8192), 256, 0, s>>>(
-                d_records, e->d_boff + n, cap_records, blob_words, e->rec_stride_words, pw, (uint32_t)e->comm_world, (uint32_t)e->comm_rank, e->d_xchg_seq,
-                e->d_push_done, e->d_epoch + EP_BORDER);
+                d_records, e->d_boff + n, cap_records, blob_words, e->ring_sec_cap, e->rec_stride_words, pw, (uint32_t)e->comm_world, (uint32_t)e->comm_rank,
+                e->d_xchg_seq, e->d_push_done, e->d_epoch + EP_BORDER);
             KCHECK(e);
         }
         return CHD_OK;
@@ -174,6 +176,74 @@ chd_status chd_import_halo(chd_engine* e, const uint32_t* d_records, uint32_t n_
     return CHD_OK;
 }
 
+/* ---- ring limits (include/chd_gpu_rings.h): maxFanOutIntervalMs across slabs, exchanged as (cell, value) records */
+
+}  // extern "C"
+
+// the shadow, the count word of the public export and the export's scan site: allocated by the first use
+static chd_status ring_limits_alloc(chd_engine* e) {
+    if (e->d_ring_lim_x) return CHD_OK;
+    const uint64_t C = e->g.cells;
+    if (!dalloc(e, &e->d_ring_lim_n, 1) || !chd_make_site(e, e->site_ring_lim, C + 1, EP_BORDER)) return CHD_ERR_CUDA;
+    CU(e, cudaStreamSynchronize(0));  // (chd_make_site clears its descriptors on the default stream)
+    uint32_t* x = nullptr;
+    if (!dalloc(e, &x, C)) return CHD_ERR_CUDA;
+    CU(e, cudaMemsetAsync(x, 0, C * 4, e->stream));
+    e->d_ring_lim_x = x;
+    return CHD_OK;
+}
+
+// On `s`: the records (cell, limit) of every served cell whose limit rose above the shadow, at most `cap` of them into `out`, their
+// count into *count (ctr: a count above cap raises CHD_OVF_BORDER there); then the shadow takes the exported values if they fit.
+static chd_status ring_limits_export(chd_engine* e, cudaStream_t s, uint32_t* out, uint32_t cap, uint32_t* count, Counters* ctr) {
+    chd_status st = chd_epoch_tick(e, s, EP_BORDER);
+    if (st != CHD_OK) return st;
+    bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_BORDER);
+    KCHECK(e);
+    SCAN(e, compact_1p(RingLimitFlag{e->g, e->d_cell_max_interval, e->d_ring_lim_x}, RingLimitSink{e->d_cell_max_interval, out, cap, count, ctr},
+                       e->g.cells, e->site_ring_lim, s));
+    if (cap) {
+        ring_limit_advance_kernel<<<blocks_for(cap, 256), 256, 0, s>>>(out, count, cap, e->d_ring_lim_x);
+        KCHECK(e);
+    }
+    return CHD_OK;
+}
+
+// On `s`: every record of `ranks` sections raises the limit and the shadow of its cell.
+static chd_status ring_limits_import(chd_engine* e, cudaStream_t s, const RingLimitView& v, uint32_t ranks) {
+    const uint64_t n = (uint64_t)ranks * v.per_rank;
+    if (!n) return CHD_OK;
+    ring_limit_import_kernel<<<blocks_for(n, 256), 256, 0, s>>>(v, ranks, e->g.cells, e->d_cell_max_interval, e->d_ring_lim_x);
+    KCHECK(e);
+    return CHD_OK;
+}
+
+extern "C" {
+
+chd_status chd_export_ring_limits(chd_engine* e, uint32_t* d_records, uint32_t cap, uint32_t* out_count) {
+    if (!e || (cap && !d_records)) return CHD_ERR_INVALID;
+    if (chd_rule_ring_limits(e, "chd_export_ring_limits") != CHD_OK) return CHD_ERR_STATE;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    chd_status st = ring_limits_alloc(e);
+    if (st == CHD_OK) st = ring_limits_export(e, e->stream, d_records, cap, e->d_ring_lim_n, out_count ? nullptr : e->d_ctr);
+    if (st != CHD_OK || !out_count) return st;
+    st = chd_read_u32(e, e->d_ring_lim_n, out_count);
+    if (st != CHD_OK) return st;
+    if (*out_count > cap) {
+        e->fail("ring-limit export needs %u records > capacity %u (nothing was advanced)", *out_count, cap);
+        return CHD_ERR_CAPACITY;
+    }
+    return CHD_OK;
+}
+
+chd_status chd_import_ring_limits(chd_engine* e, const uint32_t* d_records, uint32_t n) {
+    if (!e || (n && !d_records)) return CHD_ERR_INVALID;
+    if (chd_rule_ring_limits(e, "chd_import_ring_limits") != CHD_OK) return CHD_ERR_STATE;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    chd_status st = ring_limits_alloc(e);
+    return st != CHD_OK ? st : ring_limits_import(e, e->stream, RingLimitView{d_records, n, 2ull * n, false}, 1);
+}
+
 /* ------------------------------------------------------------------ the exchange behind the ABI ---- */
 
 chd_status chd_comm_unique_id(void* out_id) {
@@ -226,7 +296,17 @@ chd_status chd_comm_init(chd_engine* e, const void* unique_id, int rank, int wor
     if (e->mig_subs && !e->mig_pairs) e->mig_pairs = 16 * e->mig_subs;
     const uint64_t blob_words = e->mig_subs ? ((MigView::words(e->mig_subs, e->mig_pairs) + 3ull) & ~3ull) : 0ull;
     e->rec_per_rank = border_capacity;
-    e->rec_stride_words = 2ull * border_capacity + blob_words;
+    // ... and its ring-limit section (include/chd_gpu_rings.h), reserved here because chd_rings_init may come later: room for the
+    // served cells of the widest rank, as every contribution has the same size
+    uint32_t served_cols = 0;
+    for (int r = 0; r < world; r++) {
+        const uint64_t lo = ((uint64_t)r * e->g.cols) / (uint64_t)world, hi = ((uint64_t)(r + 1) * e->g.cols) / (uint64_t)world;
+        const uint64_t a = lo > halo_cols ? lo - halo_cols : 0, b = std::min<uint64_t>(e->g.cols, hi + halo_cols);
+        served_cols = std::max(served_cols, (uint32_t)(b - a));
+    }
+    e->ring_sec_cap = served_cols * e->g.rows;
+    e->ring_sec_off = 2ull * border_capacity + blob_words;
+    e->rec_stride_words = e->ring_sec_off + 4ull + ((2ull * e->ring_sec_cap + 3ull) & ~3ull);
     if (!dalloc(e, &e->d_rec_local, e->rec_stride_words) || !dalloc(e, &e->d_rec_all, e->rec_stride_words * (uint64_t)world)) return CHD_ERR_CUDA;
     CU(e, cudaMemsetAsync(e->d_rec_local, 0, e->rec_stride_words * 4, e->stream));
     CU(e, cudaMemsetAsync(e->d_rec_all, 0, e->rec_stride_words * 4 * (uint64_t)world, e->stream));
@@ -343,13 +423,28 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
         return CHD_ERR_STATE;
     }
     flags &= ~(uint32_t)CHD_TICK_FOLLOW;  // (chd_tick below joins the update this call begins)
+    // device rings: the interest update raises the ring limits, so it starts inside this call, after their exchange
+    const bool rings = e->rings_owned;
+    if (rings && e->interest_pending) {
+        e->fail("chd_tick_sharded with device rings while a chd_begin_interest is pending: the interest update starts inside the tick");
+        return CHD_ERR_STATE;
+    }
     CHD_ENTER(e, ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
     chd_status st;
     const bool has_batch = q || e->pf_q.cur >= 0 || follow;
-    // Without subscriber migration the interest update does not depend on the exchange: it starts first and overlaps it.
-    // With migration the immigrants' previous state arrives in the all-gather, so the update starts right after it.
-    if (has_batch && !e->mig_subs) {
+    // Without subscriber migration and device rings the interest update does not depend on the exchange: it starts first and
+    // overlaps it.  With migration the immigrants' previous state arrives in the all-gather; with device rings the staged updates
+    // are appended with the ring limits of every rank as of the previous tick's end, and this tick's raises come after.  Then the
+    // update starts right after the import.
+    const bool late_interest = e->mig_subs || rings;
+    if (has_batch && !late_interest) {
         st = chd_begin_interest(e, q, t_ns, (flags & CHD_TICK_FANOUT) ? 1 : 0);
+        if (st != CHD_OK) return st;
+    }
+    if (rings) {  // before anything forks: the limits as of the previous tick's end, into this rank's contribution
+        st = ring_limits_alloc(e);
+        uint32_t* sec = e->d_rec_local + e->ring_sec_off;
+        if (st == CHD_OK) st = ring_limits_export(e, e->stream, sec + 4, e->ring_sec_cap, sec, e->d_ctr);
         if (st != CHD_OK) return st;
     }
     const uint32_t cap = e->border_cap;
@@ -375,16 +470,20 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
         // immigrants' state (read by the interest update below) sits in the same window
         StageTimer tm(e, e->stream, CHD_STAGE_IMPORT);
         st = chd_import_halo(e, gathered, cap * (uint32_t)e->comm_world, (uint32_t)e->comm_rank * cap, cap);
+        if (st == CHD_OK && rings)
+            st = ring_limits_import(e, e->stream, RingLimitView{gathered + e->ring_sec_off, e->ring_sec_cap, e->rec_stride_words, true},
+                                    (uint32_t)e->comm_world);
     }
     if (st != CHD_OK) return st;
-    if (e->mig_subs) {
-        e->mig = MigView{const_cast<uint32_t*>(gathered) + 2ull * cap, e->rec_stride_words, e->mig_subs, e->mig_pairs};
-        if (has_batch) {
-            st = chd_begin_interest(e, q, t_ns, (flags & CHD_TICK_FANOUT) ? 1 : 0);
-            if (st != CHD_OK) return st;
-        }
+    if (e->rings_staged) {
+        st = chd_rings_apply(e, e->stream, e->staged_updates);
+        if (st != CHD_OK) return st;
     }
-    if (st != CHD_OK) return st;
+    if (e->mig_subs) e->mig = MigView{const_cast<uint32_t*>(gathered) + 2ull * cap, e->rec_stride_words, e->mig_subs, e->mig_pairs};
+    if (has_batch && late_interest) {
+        st = chd_begin_interest(e, q, t_ns, (flags & CHD_TICK_FANOUT) ? 1 : 0);
+        if (st != CHD_OK) return st;
+    }
     st = chd_tick(e, nullptr, t_ns, flags, out);
     CU(e, chd_copy_wait(e));  // after the tick: slabs keep the copy kernel inside their tick (the exchange adds dependencies of its own)
     return st;

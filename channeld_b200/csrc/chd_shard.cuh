@@ -92,6 +92,73 @@ struct HaloSink {
     }
 };
 
+// ---- ring limits on slabs (include/chd_gpu_rings.h).  L = maxFanOutIntervalMs per cell (d_cell_max_interval), raised by this
+// rank's interest updates; X = its exported shadow.  Records are (cell, value) pairs of u32.
+// Export: (c, L[c]) for every served cell with L[c] > X[c], then X[c] = L[c] (ring_limit_advance_kernel, only if the records fit).
+// Import: L[c] = max(L[c], v) and X[c] = max(X[c], v) for every gathered record (c, v).
+// Claim: after an exchange in which every rank exports and then imports every record, each rank serving c holds M = max_r L_r[c] as
+// of the exports.  Proof: X_r <= L_r always (both rise together on import, X is set to L on export).  Every value ever written to
+// some X_s[c] was either exported by s or imported by s, and so was exported in some exchange; every rank serving c imported it
+// there and L never falls, so every such rank holds L >= it.  Now take the rank s with L_s[c] = M at this export: if L_s[c] > X_s[c]
+// it exports M now and every rank imports it; otherwise M = X_s[c] and the first sentence covers it.  Nothing above M is ever
+// written, so every rank serving c ends at exactly M: the one-GPU value, since each (subscriber, cell) pair is created on the one
+// rank that holds the subscriber, which serves every cell its query reaches.
+struct RingLimitFlag {
+    GridDev g;  // served columns: [col_lo - halo, col_hi + halo) clipped to the grid
+    const uint32_t* __restrict__ lim;
+    const uint32_t* __restrict__ shadow;
+    __device__ __forceinline__ bool operator()(uint64_t c) const {
+        const uint32_t col = (uint32_t)c % g.cols;
+        return col + g.halo >= g.col_lo && col < g.col_hi + g.halo && lim[c] > shadow[c];
+    }
+};
+struct RingLimitSink {
+    const uint32_t* __restrict__ lim;
+    uint32_t* __restrict__ out;
+    uint32_t cap;
+    uint32_t* __restrict__ count_out;
+    Counters* __restrict__ ctr;  // nullptr: the caller reads the count and reports an overflow itself
+    __device__ __forceinline__ void operator()(uint64_t c, uint32_t k) const {
+        if (k < cap) {
+            out[2 * k] = (uint32_t)c;
+            out[2 * k + 1] = lim[c];
+        }
+    }
+    __device__ __forceinline__ void total(uint32_t n) const {
+        *count_out = n;
+        if (n > cap && ctr) atomicOr(&ctr->overflow, (uint32_t)CHD_OVF_BORDER);
+    }
+};
+// X[c] = exported value, for every exported record; nothing if the export did not fit (it is repeated in full next time)
+__global__ void __launch_bounds__(256) ring_limit_advance_kernel(const uint32_t* __restrict__ rec, const uint32_t* __restrict__ count, uint32_t cap,
+                                                                 uint32_t* __restrict__ shadow) {
+    const uint32_t n = *count, k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (n > cap || k >= n) return;
+    shadow[rec[2 * k]] = rec[2 * k + 1];
+}
+
+// Gathered ring-limit records: rank r's section starts at word r * stride_words of `base`.  headed: the section is [count, 3 words of
+// padding, records] (chd_tick_sharded's contribution); otherwise `base` holds per_rank records of one rank, all live.
+struct RingLimitView {
+    const uint32_t* base;
+    uint32_t per_rank;
+    uint64_t stride_words;
+    bool headed;
+};
+__global__ void __launch_bounds__(256) ring_limit_import_kernel(RingLimitView v, uint32_t ranks, uint32_t cells, uint32_t* __restrict__ lim,
+                                                                uint32_t* __restrict__ shadow) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (uint64_t)ranks * v.per_rank) return;
+    const uint32_t r = (uint32_t)(i / v.per_rank), k = (uint32_t)(i % v.per_rank);
+    const uint32_t* sec = v.base + r * v.stride_words;
+    if (v.headed && k >= min(sec[0], v.per_rank)) return;
+    const uint32_t* rec = sec + (v.headed ? 4 : 0) + 2ull * k;
+    const uint32_t c = rec[0], val = rec[1];
+    if (c >= cells) return;
+    if (lim[c] < val) atomicMax(&lim[c], val);
+    if (shadow[c] < val) atomicMax(&shadow[c], val);
+}
+
 // ---- the exchange itself over peer memory (NVLink): no collective library call on the tick path.
 // Every rank owns a WINDOW = 2 buffers (tick parity) x world x stride words + 2 x world 64-bit flags, mapped into every peer with
 // CUDA IPC at chd_comm_init.  peer_push_kernel copies this rank's live border records (and its migration blob) straight into
@@ -108,9 +175,10 @@ __device__ __forceinline__ unsigned long long* peer_flags(uint32_t* win_base, ui
     return reinterpret_cast<unsigned long long*>(win_base + 2ull * world * stride_words);
 }
 
+// After the migration blob comes the ring-limit section ([count, 3 words of padding, records]): its header and live records move.
 __global__ void __launch_bounds__(256) peer_push_kernel(const uint32_t* __restrict__ local, const uint32_t* __restrict__ count_ptr, uint32_t cap,
-                                                        uint64_t blob_words, uint64_t stride_words, PeerWindows peers, uint32_t world, uint32_t rank,
-                                                        unsigned long long* __restrict__ seq_ctr, uint32_t* __restrict__ done_ctr,
+                                                        uint64_t blob_words, uint32_t ring_cap, uint64_t stride_words, PeerWindows peers, uint32_t world,
+                                                        uint32_t rank, unsigned long long* __restrict__ seq_ctr, uint32_t* __restrict__ done_ctr,
                                                         unsigned long long* bump_epoch) {
     __shared__ bool s_last;
     const unsigned long long seq = *seq_ctr + 1ull;  // (the last block advances the counter after every block has read it)
@@ -118,6 +186,8 @@ __global__ void __launch_bounds__(256) peer_push_kernel(const uint32_t* __restri
     const uint32_t count = min(*count_ptr, cap);
     const uint64_t rec_words = 2ull * count;
     const uint64_t rec_q = rec_words / 4, blob_q = blob_words / 4;  // 16-byte moves; the blob starts 16-byte aligned (cap is even)
+    const uint64_t ring_off = 2ull * cap + blob_words;                // (16-byte aligned: blob_words is a multiple of 4)
+    const uint64_t ring_q = (4ull + 2ull * min(local[ring_off], ring_cap) + 3ull) / 4;
     const uint64_t slot_off = ((uint64_t)parity * world + rank) * stride_words;
     const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x, nthr = (uint64_t)gridDim.x * blockDim.x;
     for (uint32_t r = 0; r < world; r++) {
@@ -129,6 +199,9 @@ __global__ void __launch_bounds__(256) peer_push_kernel(const uint32_t* __restri
         const uint4* b4 = reinterpret_cast<const uint4*>(local + 2ull * cap);
         uint4* e4 = reinterpret_cast<uint4*>(dst + 2ull * cap);
         for (uint64_t i = tid; i < blob_q; i += nthr) e4[i] = b4[i];
+        const uint4* r4 = reinterpret_cast<const uint4*>(local + ring_off);
+        uint4* q4 = reinterpret_cast<uint4*>(dst + ring_off);
+        for (uint64_t i = tid; i < ring_q; i += nthr) q4[i] = r4[i];
     }
     __threadfence_system();
     __syncthreads();

@@ -403,6 +403,20 @@ chd_status chd_rule_facing(chd_engine* e, const char* fn) {
     return e->tbl.on ? CHD_OK : refuse(e, "%s: facings and follower frames need entity-table mode (chd_entity_table_init)", fn);
 }
 
+// 12. Ring limits (include/chd_gpu_rings.h) need device-owned rings on a slab and, like the other ring inputs, go before a
+// chd_begin_interest (its chain raises the limits).  A communicator engine stages its one chd_rings_append per tick for
+// chd_tick_sharded, which appends after the ring-limit import; until then the calls that would append, read or raise around the
+// staged updates are refused.
+chd_status chd_rule_ring_limits(chd_engine* e, const char* fn) {
+    if (!e->rings_owned || !e->slab) return refuse(e, "%s needs device-owned rings (chd_rings_init) on a slab (chd_set_slab / chd_comm_init)", fn);
+    if (e->interest_pending) return refuse(e, "%s: chd_begin_interest is pending (not joined by chd_tick yet)", fn);
+    return CHD_OK;
+}
+chd_status chd_rule_rings_staged(chd_engine* e, const char* fn) {
+    if (!e->rings_staged) return CHD_OK;
+    return refuse(e, "%s: ring updates are staged for the next chd_tick_sharded (one chd_rings_append per tick on a communicator engine)", fn);
+}
+
 chd_status chd_entity_table_init(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_fresh_engine(e) != CHD_OK) return CHD_ERR_STATE;

@@ -230,7 +230,7 @@ chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_u
         e->fail("chd_rings_append before chd_rings_init");
         return CHD_ERR_STATE;
     }
-    if (rings_before_interest(e, "chd_rings_append", false) != CHD_OK) return CHD_ERR_STATE;
+    if (rings_before_interest(e, "chd_rings_append", false) != CHD_OK || chd_rule_rings_staged(e, "chd_rings_append") != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_DEVICE);
     cudaStream_t s = e->stream;
     const uint32_t C = e->g.cells;
@@ -242,10 +242,21 @@ chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_u
         CU(e, cudaMemcpyAsync(e->d_upd_arrival, arrival_ns, sizeof(int64_t) * n_updates, cudaMemcpyDefault, s));
         CU(e, cudaMemcpyAsync(e->d_upd_sender, sender_conn_id, sizeof(uint32_t) * n_updates, cudaMemcpyDefault, s));
     }
+    if (e->comm) {  // rule 12: chd_tick_sharded appends them once the other ranks' ring limits are in
+        e->rings_staged = true;
+        e->staged_updates = n_updates;
+        return CHD_OK;
+    }
+    return chd_rings_apply(e, s, n_updates);
+}
+
+chd_status chd_rings_apply(chd_engine* e, cudaStream_t s, uint32_t n_updates) {
+    const uint32_t C = e->g.cells;
     rings_append_kernel<<<blocks_for(C, 128), 128, 0, s>>>(C, e->ring_cap, e->d_upd_off, n_updates, e->d_upd_arrival, e->d_upd_sender, e->d_rb_begin, e->d_rb_end,
                                                            e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, e->d_ch_msg_index, e->d_cell_max_interval,
                                                            &e->d_ctr->overflow);
     KCHECK(e);
+    e->rings_staged = false;
     return CHD_OK;
 }
 
@@ -256,6 +267,7 @@ chd_status chd_get_rings(chd_engine* e, uint32_t* ring_off, int64_t* arrival_ns,
         e->fail("chd_get_rings: the rings are host-owned (chd_set_rings)");
         return CHD_ERR_STATE;
     }
+    if (chd_rule_rings_staged(e, "chd_get_rings") != CHD_OK) return CHD_ERR_STATE;  // (its length pass reuses d_upd_off)
     CHD_ENTER(e, ENTRY_COPY_WAIT);
     cudaStream_t s = e->stream;
     const uint32_t C = e->g.cells;
@@ -452,6 +464,7 @@ chd_status chd_begin_interest(chd_engine* e, const chd_query_batch* q, int64_t t
         e->fail("chd_begin_interest: the previous one has not been joined by chd_tick yet");
         return CHD_ERR_STATE;
     }
+    if (chd_rule_rings_staged(e, "chd_begin_interest") != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_FETCH_GUARD);
     const chd_status st = aux_chain_enqueue(e, e->stream, q, true, t_ns, with_fanout != 0);
     if (st != CHD_OK) return st;
@@ -571,6 +584,7 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
 
 chd_status chd_tick(chd_engine* e, const chd_query_batch* q, int64_t t_ns, uint32_t flags, chd_tick_summary* out) {
     if (!e) return CHD_ERR_INVALID;
+    if (chd_rule_rings_staged(e, "chd_tick") != CHD_OK) return CHD_ERR_STATE;
     chd_status st;
     {
         // from the tick's first head kernel to the end of its copy kernel (without the summary read-back)

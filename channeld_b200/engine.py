@@ -657,3 +657,17 @@ class Engine:
 
     def import_halo(self, d_records, n_records, skip_first, skip_count):
         self._ck(self.L.chd_import_halo(self.h, ptr(d_records), int(n_records), int(skip_first), int(skip_count)))
+
+    # ---- ring limits across slabs (include/chd_gpu_rings.h): device record buffers, 2 x u32 (cell, maxFanOutIntervalMs) each
+    def export_ring_limits(self, d_records, cap, want_count=True):
+        """Records of the served cells whose limit rose since their last export or import -> their count (None with
+        want_count=False: no host synchronisation, an overflow shows up in the next summary)."""
+        if not want_count:
+            self._ck(self.L.chd_export_ring_limits(self.h, ptr(d_records), int(cap), None))
+            return None
+        n = C.c_uint32()
+        self._ck(self.L.chd_export_ring_limits(self.h, ptr(d_records), int(cap), C.byref(n)))
+        return n.value
+
+    def import_ring_limits(self, d_records, n):
+        self._ck(self.L.chd_import_ring_limits(self.h, ptr(d_records), int(n)))

@@ -16,6 +16,7 @@ package channeld
 #include "chd_gpu.h"
 #include "chd_gpu_subs.h"
 #include "chd_gpu_facing.h"
+#include "chd_gpu_rings.h"
 */
 import "C"
 
@@ -940,6 +941,25 @@ func (ctl *GpuStaticGrid2DSpatialController) RingsInit(capacityPerCell uint32) e
 
 func (ctl *GpuStaticGrid2DSpatialController) RingsAppend(updOff *C.uint32_t, n uint32, arrival *C.int64_t, sender *C.uint32_t) error {
 	if st := C.chd_rings_append(ctl.engine, updOff, C.uint32_t(n), arrival, sender); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
+// ExportRingLimits / ImportRingLimits (include/chd_gpu_rings.h): each channel's maxFanOutIntervalMs across slabs, for hosts that
+// join slabs themselves.  Records are (cell, maxFanOutIntervalMs) u32 pairs in device memory.  After its tick every rank exports;
+// every rank imports every rank's records before its next RingsAppend.  A communicator engine (chd_comm_init) needs neither:
+// chd_tick_sharded exchanges the limits and appends the updates RingsAppend staged.
+func (ctl *GpuStaticGrid2DSpatialController) ExportRingLimits(dRecords *C.uint32_t, capRecords uint32) (uint32, error) {
+	var n C.uint32_t
+	if st := C.chd_export_ring_limits(ctl.engine, dRecords, C.uint32_t(capRecords), &n); st != C.CHD_OK {
+		return uint32(n), errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return uint32(n), nil
+}
+
+func (ctl *GpuStaticGrid2DSpatialController) ImportRingLimits(dRecords *C.uint32_t, n uint32) error {
+	if st := C.chd_import_ring_limits(ctl.engine, dRecords, C.uint32_t(n)); st != C.CHD_OK {
 		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
 	}
 	return nil
