@@ -8,7 +8,7 @@
 //   chd_results.cu   getters, chd_fetch_results, device views
 //   chd_shard.cu     multi-GPU X-slabs: border export, halo import, the NCCL exchange
 //   chd_extras.cu    window classes, ADJACENT_CHANNELS broadcast sets, config-plane helpers
-//   chd_table.cu     the mode rules; entity-table mode: spawn / move / despawn by id, the id-valued results
+//   chd_table.cu     the mode and call-order rules; entity-table mode: spawn / move / despawn by id, the id-valued results
 //   chd_follow.cu    followers: slot -> entity bindings and the query batch generated from them
 #pragma once
 #include <cuda_runtime.h>
@@ -626,7 +626,7 @@ struct DeltaLengths {
     bool bad_ids;
 };
 chd_status chd_read_delta_lengths(chd_engine* e, cudaStream_t s, DeltaLengths* out);
-// the mode rules (chd_table.cu, numbered as in DESIGN.md §5): CHD_OK, or the error set and CHD_ERR_STATE (6: or CHD_ERR_INVALID)
+// the mode and call-order rules (chd_table.cu, numbered as in DESIGN.md §5): CHD_OK, or the error set and CHD_ERR_STATE (6: or CHD_ERR_INVALID)
 chd_status chd_rule_not_table(chd_engine* e, const char* fn);
 chd_status chd_rule_table_on_slab(chd_engine* e, const char* fn);
 chd_status chd_rule_table(chd_engine* e, const char* fn);
@@ -636,12 +636,15 @@ chd_status chd_delta_check(chd_engine* e, bool will_build);
 chd_status chd_rule_halo_import(chd_engine* e);
 chd_status chd_rule_follow(chd_engine* e, const char* fn);
 chd_status chd_rule_no_followers(chd_engine* e, const char* fn);
+chd_status chd_rule_no_generated_batch(chd_engine* e, const char* fn);
 chd_status chd_rule_one_batch(chd_engine* e, const char* fn);
 chd_status chd_rule_merged_batch(chd_engine* e, bool adopted);
+chd_status chd_rule_batch_waiting(chd_engine* e, const char* fn, bool generated);
 chd_status chd_rule_explicit_subs(chd_engine* e, const char* fn);
 chd_status chd_rule_facing(chd_engine* e, const char* fn);
 chd_status chd_rule_ring_limits(chd_engine* e, const char* fn);
 chd_status chd_rule_rings_staged(chd_engine* e, const char* fn);
+chd_status chd_rule_no_chain(chd_engine* e, const char* fn, bool fanout_only);
 // device-owned rings (chd_tick.cu): the append kernel on `s` over n_updates updates already uploaded into d_upd_*
 chd_status chd_rings_apply(chd_engine* e, cudaStream_t s, uint32_t n_updates);
 // followers (chd_follow.cu): the listed slots (n == 0 with slot == nullptr: every slot) follow nothing from now on; d_slot: the

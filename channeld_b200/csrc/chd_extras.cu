@@ -90,10 +90,7 @@ chd_status chd_set_subscriber_types(chd_engine* e, const uint8_t* conn_type, uin
 chd_status chd_adjacent_broadcast(chd_engine* e, const chd_broadcast_batch* b, uint32_t* out_status, uint32_t* out_off, uint32_t* out_slot,
                                   uint64_t cap) {
     if (!e || !b || (b->n && (!b->channel_id || !b->broadcast)) || !out_off) return CHD_ERR_INVALID;
-    if (e->interest_pending) {
-        e->fail("chd_adjacent_broadcast while a chd_begin_interest is pending (call chd_tick first)");
-        return CHD_ERR_STATE;
-    }
+    if (chd_rule_no_chain(e, "chd_adjacent_broadcast", false) != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT);
     const uint32_t n = b->n;
     if (out_status)

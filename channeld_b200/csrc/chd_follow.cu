@@ -362,11 +362,8 @@ chd_status chd_get_follow(chd_engine* e, uint32_t* slot, uint32_t* entity, uint3
                           uint32_t* n_selected) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_follow(e, "chd_get_follow") != CHD_OK) return CHD_ERR_STATE;
+    if (chd_rule_no_generated_batch(e, "chd_get_follow") != CHD_OK || chd_rule_no_chain(e, "chd_get_follow", false) != CHD_OK) return CHD_ERR_STATE;
     chd_engine::Follow& F = e->fw;
-    if (F.ready || e->interest_pending) {
-        e->fail("chd_get_follow: the generated batch has not been consumed by an interest update yet (or chd_begin_interest is not joined)");
-        return CHD_ERR_STATE;
-    }
     if (count) *count = 0;
     if (n_selected) *n_selected = 0;
     if (!F.on || !F.n_bound) return CHD_OK;
@@ -460,11 +457,9 @@ chd_status chd_get_follow_frame(chd_engine* e, uint32_t* slot, double* fx, doubl
                                 uint32_t* count) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_facing(e, "chd_get_follow_frame") != CHD_OK || chd_rule_follow(e, "chd_get_follow_frame") != CHD_OK) return CHD_ERR_STATE;
-    chd_engine::Follow& F = e->fw;
-    if (F.ready || e->interest_pending) {
-        e->fail("chd_get_follow_frame: the generated batch has not been consumed by an interest update yet (or chd_begin_interest is not joined)");
+    if (chd_rule_no_generated_batch(e, "chd_get_follow_frame") != CHD_OK || chd_rule_no_chain(e, "chd_get_follow_frame", false) != CHD_OK)
         return CHD_ERR_STATE;
-    }
+    chd_engine::Follow& F = e->fw;
     if (count) *count = 0;
     if (!F.on || !F.n_framed) return CHD_OK;
     CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT);

@@ -418,17 +418,11 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
     // CHD_TICK_FOLLOW: the batch is the one chd_follow_queries(_with) generated, started below like a host batch
     const bool follow = flags & CHD_TICK_FOLLOW;
     if (follow && q) return CHD_ERR_INVALID;
-    if (follow && !e->fw.ready) {
-        e->fail("chd_tick_sharded: CHD_TICK_FOLLOW without a batch generated by chd_follow_queries");
-        return CHD_ERR_STATE;
-    }
+    if (follow && chd_rule_batch_waiting(e, "chd_tick_sharded", true) != CHD_OK) return CHD_ERR_STATE;
     flags &= ~(uint32_t)CHD_TICK_FOLLOW;  // (chd_tick below joins the update this call begins)
     // device rings: the interest update raises the ring limits, so it starts inside this call, after their exchange
     const bool rings = e->rings_owned;
-    if (rings && e->interest_pending) {
-        e->fail("chd_tick_sharded with device rings while a chd_begin_interest is pending: the interest update starts inside the tick");
-        return CHD_ERR_STATE;
-    }
+    if (rings && chd_rule_no_chain(e, "chd_tick_sharded with device rings", false) != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
     chd_status st;
     const bool has_batch = q || e->pf_q.cur >= 0 || follow;

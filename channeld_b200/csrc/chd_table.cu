@@ -288,7 +288,9 @@ chd_status refuse(const chd_engine* e, const char* fmt, A... a) {
 extern "C" {
 
 // ---- The mode rules (DESIGN.md §5, same numbers): entities are named by index, by global id (chd_set_entity_ids) or by table id
-// (entity-table mode), visible deltas by index or by global id (id mode).  Entry points call their rule after the argument checks.
+// (entity-table mode), visible deltas by index or by global id (id mode).  With them the call-order rules: one query batch per
+// interest update (9) and nothing rewritten under a begun chd_begin_interest (13).  Entry points call their rule after the
+// argument checks.
 
 // 1. Refused in entity-table mode: the calls that bypass the table (positions, counts, global ids, a slab).
 chd_status chd_rule_not_table(chd_engine* e, const char* fn) {
@@ -370,31 +372,41 @@ chd_status chd_rule_no_followers(chd_engine* e, const char* fn) {
 
 // ... and one query batch per interest update: a generated batch (chd_follow_queries) and an adopted prefetched one
 // (chd_prefetch_queries + chd_adopt_prefetched) exclude each other until the update that consumes the first has been enqueued.
+// A generated batch also holds off the reports of the followers it was generated from (chd_get_follow, chd_get_follow_frame).
+chd_status chd_rule_no_generated_batch(chd_engine* e, const char* fn) {
+    if (!e->fw.ready) return CHD_OK;
+    return refuse(e, "%s: the batch generated by chd_follow_queries has not been consumed by an interest update yet (one batch per update)", fn);
+}
 chd_status chd_rule_one_batch(chd_engine* e, const char* fn) {
-    if (e->fw.ready) return refuse(e, "%s: the batch generated by chd_follow_queries has not been consumed by an interest update yet", fn);
+    if (chd_rule_no_generated_batch(e, fn) != CHD_OK) return CHD_ERR_STATE;
     if (e->pf_q.cur >= 0) return refuse(e, "%s: the adopted prefetched query batch has not been consumed by an interest update yet", fn);
-    if (e->interest_pending) return refuse(e, "%s: chd_begin_interest is pending (not joined by chd_tick yet)", fn);
-    return CHD_OK;
+    return chd_rule_no_chain(e, fn, false);
 }
 
 // ... except that chd_follow_queries_with merges the two into one batch: the host part is q or (adopted) the adopted prefetched batch,
 // which it consumes.  So an adopted batch is required with q == NULL and refused beside a q.
 chd_status chd_rule_merged_batch(chd_engine* e, bool adopted) {
     const char* fn = "chd_follow_queries_with";
-    if (e->fw.ready) return refuse(e, "%s: the batch generated by chd_follow_queries has not been consumed by an interest update yet", fn);
-    if (e->interest_pending) return refuse(e, "%s: chd_begin_interest is pending (not joined by chd_tick yet)", fn);
+    if (chd_rule_no_generated_batch(e, fn) != CHD_OK || chd_rule_no_chain(e, fn, false) != CHD_OK) return CHD_ERR_STATE;
     if (adopted && e->pf_q.cur < 0) return refuse(e, "%s: q == NULL needs chd_prefetch_queries + chd_adopt_prefetched first", fn);
     if (!adopted && e->pf_q.cur >= 0)
         return refuse(e, "%s: the adopted prefetched query batch has not been consumed (pass q == NULL to merge it)", fn);
     return CHD_OK;
 }
 
+// ... and an interest update that takes the waiting batch (q == NULL) needs one: with `generated` (CHD_TICK_FOLLOW) the generated
+// batch, otherwise either kind.
+chd_status chd_rule_batch_waiting(chd_engine* e, const char* fn, bool generated) {
+    if (generated) return e->fw.ready ? CHD_OK : refuse(e, "%s: CHD_TICK_FOLLOW without a batch generated by chd_follow_queries", fn);
+    if (e->fw.ready || e->pf_q.cur >= 0) return CHD_OK;
+    return refuse(e, "%s: q == NULL needs chd_prefetch_queries + chd_adopt_prefetched, or chd_follow_queries, first", fn);
+}
+
 // 10. Explicit subscriptions (chd_apply_subscriptions) are single-GPU: a slab engine's slots migrate between ranks with their pairs,
-// and the ops would have to follow them.  Refused, like the interest-stage inputs, between chd_begin_interest and its chd_tick.
+// and the ops would have to follow them.  Rule 13 as well.
 chd_status chd_rule_explicit_subs(chd_engine* e, const char* fn) {
     if (e->slab) return refuse(e, "%s: explicit subscriptions are not available on an engine made a slab (chd_set_slab / chd_comm_init)", fn);
-    if (e->interest_pending) return refuse(e, "%s: chd_begin_interest is pending (not joined by chd_tick yet)", fn);
-    return CHD_OK;
+    return chd_rule_no_chain(e, fn, false);
 }
 
 // 11. Facings and frames (include/chd_gpu_facing.h) need entity-table mode: index mode's positions come from host snapshots and the
@@ -403,18 +415,27 @@ chd_status chd_rule_facing(chd_engine* e, const char* fn) {
     return e->tbl.on ? CHD_OK : refuse(e, "%s: facings and follower frames need entity-table mode (chd_entity_table_init)", fn);
 }
 
-// 12. Ring limits (include/chd_gpu_rings.h) need device-owned rings on a slab and, like the other ring inputs, go before a
-// chd_begin_interest (its chain raises the limits).  A communicator engine stages its one chd_rings_append per tick for
-// chd_tick_sharded, which appends after the ring-limit import; until then the calls that would append, read or raise around the
-// staged updates are refused.
+// 12. Ring limits (include/chd_gpu_rings.h) need device-owned rings on a slab, and rule 13 (the chain raises the limits).  A
+// communicator engine stages its one chd_rings_append per tick for chd_tick_sharded, which appends after the ring-limit import;
+// until then the calls that would append, read or raise around the staged updates are refused.
 chd_status chd_rule_ring_limits(chd_engine* e, const char* fn) {
     if (!e->rings_owned || !e->slab) return refuse(e, "%s needs device-owned rings (chd_rings_init) on a slab (chd_set_slab / chd_comm_init)", fn);
-    if (e->interest_pending) return refuse(e, "%s: chd_begin_interest is pending (not joined by chd_tick yet)", fn);
-    return CHD_OK;
+    return chd_rule_no_chain(e, fn, false);
 }
 chd_status chd_rule_rings_staged(chd_engine* e, const char* fn) {
     if (!e->rings_staged) return CHD_OK;
     return refuse(e, "%s: ring updates are staged for the next chd_tick_sharded (one chd_rings_append per tick on a communicator engine)", fn);
+}
+
+// 13. chd_begin_interest forks the interest update (and, with_fanout, the fan-out) onto aux_stream, and nothing on the engine
+// stream is ordered against that chain until the chd_tick that joins it.  Until then the calls that rewrite what the chain reads,
+// or read what it writes, are refused: the interest update reads the query batches, the subscriptions and the channel start times
+// and raises the per-cell maxFanOutIntervalMs that chd_rings_append and the ring limits read; the fan-out reads the rings and the
+// start times; the follower reports and the adjacent broadcast read the pairs the update rewrites.  `fanout_only`: the call's
+// input is read by the fan-out alone (chd_set_rings), so a chain without the fan-out does not exclude it.
+chd_status chd_rule_no_chain(chd_engine* e, const char* fn, bool fanout_only) {
+    if (!e->interest_pending || (fanout_only && !e->pending_fanout)) return CHD_OK;
+    return refuse(e, "%s: chd_begin_interest is pending (not joined by chd_tick yet)", fn);
 }
 
 chd_status chd_entity_table_init(chd_engine* e) {

@@ -121,16 +121,6 @@ chd_status chd_emit_visible(chd_engine* e) {
     return emit_enqueue(e, e->stream, nullptr, nullptr);
 }
 
-// Ring inputs go before chd_begin_interest.  The chain it forks onto aux_stream reads what they write, and nothing on the engine
-// stream is ordered against that chain until chd_tick joins it: the interest update reads the channel start times and raises the
-// per-cell maxFanOutIntervalMs that chd_rings_append reads, the fan-out reads the rings and the start times.  `fanout_only`: the
-// input is read by the fan-out alone (chd_set_rings), so a begun chain without the fan-out does not exclude it.
-static chd_status rings_before_interest(chd_engine* e, const char* fn, bool fanout_only) {
-    if (!e->interest_pending || (fanout_only && !e->pending_fanout)) return CHD_OK;
-    e->fail("%s while a chd_begin_interest is pending: ring inputs go before it (or after the chd_tick that joins it)", fn);
-    return CHD_ERR_STATE;
-}
-
 // argument checks of one tick's host-owned rings (chd_set_rings / chd_prefetch_rings)
 static chd_status check_rings(chd_engine* e, const char* fn, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
                               const uint64_t* index) {
@@ -173,7 +163,7 @@ chd_status chd_set_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_ent
                          const uint64_t* index, const uint64_t* ch_msg_index) {
     chd_status st = check_rings(e, "chd_set_rings", ring_off, n_entries, arrival, sender, index);
     if (st != CHD_OK) return st;
-    if (rings_before_interest(e, "chd_set_rings", true) != CHD_OK) return CHD_ERR_STATE;
+    if (chd_rule_no_chain(e, "chd_set_rings", true) != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_DEVICE);
     const uint32_t total = n_entries;
     const bool in_place = chd_is_device_ptr(e, ring_off) && (!total || (chd_is_device_ptr(e, arrival) && chd_is_device_ptr(e, sender) && chd_is_device_ptr(e, index))) &&
@@ -201,7 +191,7 @@ chd_status chd_rings_init(chd_engine* e, uint32_t capacity_per_cell) {
         if (e) e->fail("chd_rings_init: capacity_per_cell must exceed %u (MaxUpdateMsgBufferSize: the reference's buffer may grow beyond it)", RING_MAX_BUFFER);
         return CHD_ERR_INVALID;
     }
-    if (rings_before_interest(e, "chd_rings_init", false) != CHD_OK) return CHD_ERR_STATE;
+    if (chd_rule_no_chain(e, "chd_rings_init", false) != CHD_OK) return CHD_ERR_STATE;
     const uint64_t need = (uint64_t)e->g.cells * capacity_per_cell;
     if (need > e->lim.max_ring_entries) {
         e->fail("chd_rings_init: %u cells x %u entries > max_ring_entries %u", e->g.cells, capacity_per_cell, e->lim.max_ring_entries);
@@ -230,7 +220,7 @@ chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_u
         e->fail("chd_rings_append before chd_rings_init");
         return CHD_ERR_STATE;
     }
-    if (rings_before_interest(e, "chd_rings_append", false) != CHD_OK || chd_rule_rings_staged(e, "chd_rings_append") != CHD_OK) return CHD_ERR_STATE;
+    if (chd_rule_no_chain(e, "chd_rings_append", false) != CHD_OK || chd_rule_rings_staged(e, "chd_rings_append") != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_DEVICE);
     cudaStream_t s = e->stream;
     const uint32_t C = e->g.cells;
@@ -308,7 +298,7 @@ chd_status chd_get_rings(chd_engine* e, uint32_t* ring_off, int64_t* arrival_ns,
 
 chd_status chd_set_channel_start_times(chd_engine* e, const int64_t* start_ns) {
     if (!e) return CHD_ERR_INVALID;
-    if (rings_before_interest(e, "chd_set_channel_start_times", false) != CHD_OK) return CHD_ERR_STATE;
+    if (chd_rule_no_chain(e, "chd_set_channel_start_times", false) != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_DEVICE);
     if (!start_ns) {
         e->have_cell_start = false;
@@ -388,11 +378,7 @@ chd_status chd_adopt_prefetched(chd_engine* e) {
         e->fail("chd_adopt_prefetched without a preceding chd_prefetch_entities / chd_prefetch_queries / chd_prefetch_rings");
         return CHD_ERR_STATE;
     }
-    if (e->pf_q.staged >= 0 && e->fw.ready) {
-        e->fail("chd_adopt_prefetched: a query batch was prefetched, but the batch generated by chd_follow_queries has not been consumed by an "
-                "interest update yet (one batch per update)");
-        return CHD_ERR_STATE;
-    }
+    if (e->pf_q.staged >= 0 && chd_rule_no_generated_batch(e, "chd_adopt_prefetched of a query batch") != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_DEVICE);
     chd_pf_adopt(e->pf_q);  // consumed by the next chd_begin_interest / chd_update_interest called with q == NULL
     if (chd_pf_adopt(e->pf_ring)) {
@@ -456,15 +442,8 @@ static chd_status aux_chain_enqueue(chd_engine* e, cudaStream_t s, const chd_que
 
 chd_status chd_begin_interest(chd_engine* e, const chd_query_batch* q, int64_t t_ns, int with_fanout) {
     if (!e) return CHD_ERR_INVALID;
-    if (!q && e->pf_q.cur < 0 && !e->fw.ready) {
-        e->fail("chd_begin_interest: q == NULL needs chd_prefetch_queries + chd_adopt_prefetched, or chd_follow_queries, first");
-        return CHD_ERR_STATE;
-    }
-    if (e->interest_pending) {
-        e->fail("chd_begin_interest: the previous one has not been joined by chd_tick yet");
-        return CHD_ERR_STATE;
-    }
-    if (chd_rule_rings_staged(e, "chd_begin_interest") != CHD_OK) return CHD_ERR_STATE;
+    if (!q && chd_rule_batch_waiting(e, "chd_begin_interest", false) != CHD_OK) return CHD_ERR_STATE;
+    if (chd_rule_no_chain(e, "chd_begin_interest", false) != CHD_OK || chd_rule_rings_staged(e, "chd_begin_interest") != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_FETCH_GUARD);
     const chd_status st = aux_chain_enqueue(e, e->stream, q, true, t_ns, with_fanout != 0);
     if (st != CHD_OK) return st;
@@ -500,10 +479,7 @@ static chd_status tick_enqueue(chd_engine* e, cudaStream_t s, const chd_query_ba
     const bool started = e->interest_pending;  // the aux chain of this tick was started by chd_begin_interest
     const bool follow = flags & CHD_TICK_FOLLOW;  // the batch is the generated one (q == NULL)
     if (follow && q) return CHD_ERR_INVALID;
-    if (follow && !started && !e->fw.ready) {
-        e->fail("chd_tick: CHD_TICK_FOLLOW without a batch generated by chd_follow_queries");
-        return CHD_ERR_STATE;
-    }
+    if (follow && !started && chd_rule_batch_waiting(e, "chd_tick", true) != CHD_OK) return CHD_ERR_STATE;
     const bool interest = q || follow;  // this tick has an interest update of its own
     e->early_ready = false;
     e->build_done_recorded = false;

@@ -1,7 +1,6 @@
 """CPU-side checks of facings and follower frames (include/chd_gpu_facing.h): the header is plain C99 next to chd_gpu.h, the library
-exports what it declares, every entry point refuses a NULL engine and declares its needs once (the rules of
-tests/test_entry_points.py), the numpy restatement of the generation gives the answers derived by hand, and the sharding helpers
-pass facings and frames through.  No GPU needed."""
+exports what it declares, every entry point refuses a NULL engine, the numpy restatement of the generation gives the answers derived
+by hand, and the sharding helpers pass facings and frames through.  No GPU needed."""
 import ctypes as C
 import os
 import re
@@ -10,33 +9,14 @@ import sys
 
 import numpy as np
 
-from tests import test_entry_points as tep
 from tests._facing import frame_query
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = os.path.join(ROOT, "include", "chd_gpu_facing.h")
 
-# the inventory of chd_gpu_facing.h's entry points: the event calls as their chd_gpu.h counterparts, set-frame as chd_follow_bind,
-# get-frame as chd_get_follow
-NEEDS = {
-    "chd_spawn_entities_facing": "DEVICE",
-    "chd_spawn_entities_facing_f32": "DEVICE",
-    "chd_move_entities_facing": "DEVICE",
-    "chd_move_entities_facing_f32": "DEVICE",
-    "chd_handoff_entities_facing": "DEVICE",
-    "chd_follow_set_frame": "LOCK|DEVICE",
-    "chd_get_follow_frame": "LOCK|COPY_WAIT",
-}
-
-
 def _declared():
     src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
     return sorted(set(re.findall(r"\b(chd_[a-z0-9_]+)\s*\(", src)))
-
-
-def _entry_points():
-    hdr = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
-    return {m.group(1) for m in re.finditer(r"^chd_status\s+(chd_[a-z0-9_]+)\s*\(\s*chd_engine\s*\*", hdr, flags=re.M)}
 
 
 def test_header_is_plain_c_and_frame_batch_matches(tmp_path):
@@ -92,18 +72,6 @@ print("BAD", bad)
     out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0, out.stderr[-2000:]
     assert "BAD []" in out.stdout, out.stdout
-
-
-def test_every_entry_point_is_in_the_table():
-    assert _entry_points() == set(NEEDS)
-
-
-def test_each_entry_point_declares_its_needs_once():
-    bodies = tep._bodies()
-    for name, want in NEEDS.items():
-        enters = re.findall(r"\bCHD_ENTER\s*\(\s*e\s*,([^;]*)\)\s*;", bodies[name])
-        assert len(enters) == 1, "%s: %d CHD_ENTER" % (name, len(enters))
-        assert tep._flags(enters[0]) == tep._flags(want), "%s declares %s, the table says %s" % (name, enters[0].strip(), want)
 
 
 # ---- the numpy restatement against answers derived by hand

@@ -1,6 +1,6 @@
 """CPU-side checks of explicit subscriptions (include/chd_gpu_subs.h): the header is plain C99 next to chd_gpu.h, the library exports
-what it declares, every entry point refuses a NULL engine and declares its needs once (the rules of tests/test_entry_points.py), and
-the oracle's presence-mask merge gives the answers derived by hand from subscription.go:34-125.  No GPU needed."""
+what it declares, every entry point refuses a NULL engine, and the oracle's presence-mask merge gives the answers derived by hand
+from subscription.go:34-125.  No GPU needed."""
 import ctypes as C
 import os
 import re
@@ -10,27 +10,15 @@ import sys
 import numpy as np
 import pytest
 
-from tests import test_entry_points as tep
 from tests._subs_oracle import (ERR_CHANNEL, ERR_SLOT, MERGED, NEW, NOT_SUBSCRIBED, OPT_DELAY, OPT_INTERVAL, OPT_SKIP_FIRST, OPT_SKIP_SELF,
                                 SUB, UNSUB, UNSUBSCRIBED, DIST_EXPLICIT, SubsOracle)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = os.path.join(ROOT, "include", "chd_gpu_subs.h")
 
-# the inventory of chd_gpu_subs.h's entry points (what each declares with CHD_ENTER; the rules: ENTRY_* in csrc/chd_engine.h).
-# chd_apply_subscriptions takes the lock besides chd_update_interest's needs: it opens epochs of the query stage's scan sites, which
-# chd_query_channel_ids bumps from any thread.
-NEEDS = {"chd_apply_subscriptions": "LOCK|COPY_WAIT|FETCH_GUARD"}
-
-
 def _declared():
     src = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
     return sorted(set(re.findall(r"\b(chd_[a-z0-9_]+)\s*\(", src)))
-
-
-def _entry_points():
-    hdr = re.sub(r"/\*.*?\*/", "", open(HEADER).read(), flags=re.S)
-    return {m.group(1) for m in re.finditer(r"^chd_status\s+(chd_[a-z0-9_]+)\s*\(\s*chd_engine\s*\*", hdr, flags=re.M)}
 
 
 def test_header_is_plain_c_and_sub_batch_matches(tmp_path):
@@ -88,18 +76,6 @@ print("BAD", bad)
     out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=120)
     assert out.returncode == 0, out.stderr[-2000:]
     assert "BAD []" in out.stdout, out.stdout
-
-
-def test_every_entry_point_is_in_the_table():
-    assert _entry_points() == set(NEEDS)
-
-
-def test_each_entry_point_declares_its_needs_once():
-    bodies = tep._bodies()
-    for name, want in NEEDS.items():
-        enters = re.findall(r"\bCHD_ENTER\s*\(\s*e\s*,([^;]*)\)\s*;", bodies[name])
-        assert len(enters) == 1, "%s: %d CHD_ENTER" % (name, len(enters))
-        assert tep._flags(enters[0]) == tep._flags(want), "%s declares %s, the table says %s" % (name, enters[0].strip(), want)
 
 
 # ---- the oracle's merge, against answers derived by hand from subscription.go:34-125 (conn 7 on slot 0, channel 0x10000 = cell 0)
