@@ -187,6 +187,9 @@ class FollowFrameBatch(C.Structure):
 
 # every symbol include/chd_gpu_rings.h declares (ring limits across slabs; checked by tests/test_rings_host.py against that header)
 RING_SYMBOLS = ["chd_export_ring_limits", "chd_import_ring_limits"]
+# every symbol include/chd_gpu_subs_sharded.h declares (explicit subscriptions on slabs; checked by tests/test_subs_sharded_host.py)
+SUB_SHARDED_SYMBOLS = ["chd_apply_subscriptions_sharded"]
+SUB_ERR_OUTSIDE_SLAB = 7  # beside SUB_* above: a SUB of a cell in a column the slab does not serve
 
 
 STAGE_BUILD, STAGE_INTEREST, STAGE_EMIT, STAGE_EMIT_KERNEL, STAGE_FANOUT, STAGE_TICK, STAGE_EXPORT, STAGE_EXCHANGE, STAGE_IMPORT, STAGE_READBACK, STAGE_VISIBLE_DELTA, STAGE_ENTITY_EVENTS, STAGE_FOLLOW = range(13)
@@ -401,8 +404,9 @@ def lib():
     L.chd_follow_queries_with.argtypes = [vp, C.c_uint32, C.POINTER(QueryBatch)]
     L.chd_get_follow.restype = C.c_int
     L.chd_get_follow.argtypes = [vp, vp, vp, vp, vp, vp, C.c_uint32, u32p, u32p]
-    L.chd_apply_subscriptions.restype = C.c_int
-    L.chd_apply_subscriptions.argtypes = [vp, C.POINTER(SubBatch), C.c_int64, vp]
+    for f in (L.chd_apply_subscriptions, L.chd_apply_subscriptions_sharded):
+        f.restype = C.c_int
+        f.argtypes = [vp, C.POINTER(SubBatch), C.c_int64, vp]
     for f in (L.chd_spawn_entities_facing, L.chd_spawn_entities_facing_f32):
         f.restype = C.c_int
         f.argtypes = [vp, vp, vp, vp, vp, vp, C.c_uint32, vp]

@@ -29,6 +29,9 @@ struct GridDev {
     uint32_t col_lo, col_hi, halo;
     uint32_t default_interval_ms;
     int32_t default_delay_ms;
+    // a column this slab serves: [col_lo - halo, col_hi + halo), clipped to the grid (col < cols); the halo import keeps the
+    // records of these columns, the ring limits are exchanged for them, and explicit subscriptions may name them
+    __device__ __forceinline__ bool serves_column(uint32_t col) const { return col + halo >= col_lo && col < col_hi + halo; }
 };
 
 // The rank owning grid column `col` when `world` ranks split the columns into X-slabs (chd_comm_init): the largest rank r with

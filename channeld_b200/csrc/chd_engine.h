@@ -641,6 +641,7 @@ chd_status chd_rule_one_batch(chd_engine* e, const char* fn);
 chd_status chd_rule_merged_batch(chd_engine* e, bool adopted);
 chd_status chd_rule_batch_waiting(chd_engine* e, const char* fn, bool generated);
 chd_status chd_rule_explicit_subs(chd_engine* e, const char* fn);
+chd_status chd_rule_explicit_subs_slab(chd_engine* e, const char* fn);
 chd_status chd_rule_facing(chd_engine* e, const char* fn);
 chd_status chd_rule_ring_limits(chd_engine* e, const char* fn);
 chd_status chd_rule_rings_staged(chd_engine* e, const char* fn);

@@ -64,9 +64,7 @@ struct HaloFlag {
         if (counts && (uint32_t)(i % rec.per_rank) >= counts[i / rec.per_rank]) return false;
         if (i >= skip_first && i - skip_first < skip_count) return false;
         const uint32_t cell = rec.at(i)[1];
-        if (cell >= g.cells) return false;
-        const uint32_t col = cell % g.cols;
-        return (col + g.halo >= g.col_lo) && (col < g.col_hi + g.halo);
+        return cell < g.cells && g.serves_column(cell % g.cols);
     }
 };
 // appends the kept records after the `base` own entities and publishes the build length (own + halo) on the device:
@@ -104,13 +102,10 @@ struct HaloSink {
 // written, so every rank serving c ends at exactly M: the one-GPU value, since each (subscriber, cell) pair is created on the one
 // rank that holds the subscriber, which serves every cell its query reaches.
 struct RingLimitFlag {
-    GridDev g;  // served columns: [col_lo - halo, col_hi + halo) clipped to the grid
+    GridDev g;  // served columns: GridDev::serves_column
     const uint32_t* __restrict__ lim;
     const uint32_t* __restrict__ shadow;
-    __device__ __forceinline__ bool operator()(uint64_t c) const {
-        const uint32_t col = (uint32_t)c % g.cols;
-        return col + g.halo >= g.col_lo && col < g.col_hi + g.halo && lim[c] > shadow[c];
-    }
+    __device__ __forceinline__ bool operator()(uint64_t c) const { return g.serves_column((uint32_t)c % g.cols) && lim[c] > shadow[c]; }
 };
 struct RingLimitSink {
     const uint32_t* __restrict__ lim;

@@ -1,5 +1,5 @@
-// chd_subs.cu — explicit subscriptions to spatial channels (include/chd_gpu_subs.h): a stage of its own on the engine stream,
-// between ticks.  Kernels: chd_subs.cuh.
+// chd_subs.cu — explicit subscriptions to spatial channels (include/chd_gpu_subs.h, and on slabs include/chd_gpu_subs_sharded.h):
+// a stage of its own on the engine stream, between ticks.  Kernels: chd_subs.cuh.
 #include "chd_engine.h"
 
 #include "chd_subs.cuh"
@@ -41,28 +41,22 @@ void open_epoch(chd_engine* e, cudaStream_t s) {
     bump_epoch_kernel<<<1, 1, 0, s>>>(e->d_epoch + EP_QUERY);
 }
 
-}  // namespace
-
-extern "C" {
-
-chd_status chd_apply_subscriptions(chd_engine* e, const chd_sub_batch* b, int64_t now_ns, uint8_t* out_status) {
-    if (!e || !b) return CHD_ERR_INVALID;
-    const uint32_t n = b->n;
-    if (n && (!b->slot || !b->channel_id || !b->op)) return CHD_ERR_INVALID;
-    if (chd_rule_explicit_subs(e, "chd_apply_subscriptions") != CHD_OK) return CHD_ERR_STATE;
+// the batch limits, checked after the call's rule: CHD_ERR_CAPACITY, nothing applied
+chd_status check_batch(chd_engine* e, uint32_t n, const char* fn) {
     if (n > e->lim.max_pairs) {
-        e->fail("chd_apply_subscriptions: %u ops > max_pairs %llu", n, (unsigned long long)e->lim.max_pairs);
+        e->fail("%s: %u ops > max_pairs %llu", fn, n, (unsigned long long)e->lim.max_pairs);
         return CHD_ERR_CAPACITY;
     }
     if (e->n_slots >= (1u << 20)) {  // the sort by slot takes <= 2 passes of <= 10-bit digits
-        e->fail("chd_apply_subscriptions: %u subscriber slots (at most 2^20 - 1)", e->n_slots);
+        e->fail("%s: %u subscriber slots (at most 2^20 - 1)", fn, e->n_slots);
         return CHD_ERR_CAPACITY;
     }
-    if (n == 0) return CHD_OK;
-    // LOCK: this stage opens epochs of the query stage's scan sites, which chd_query_channel_ids (any thread) also bumps.
-    // COPY_WAIT: the pair buffer written here is the one the pending copy kernel's tick will overwrite next.
-    // FETCH_GUARD: the pairs, their channel ids and the by-cell grouping are read-back sources.
-    CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
+    return CHD_OK;
+}
+
+// Both entry points after their rule, their checks and CHD_ENTER: `slab` rejects SUBs of cells the slab does not serve.
+chd_status apply(chd_engine* e, const chd_sub_batch* b, int64_t now_ns, uint8_t* out_status, bool slab) {
+    const uint32_t n = b->n;
     if (!subs_reserve(e, n)) return CHD_ERR_CUDA;
     chd_engine::Subs& x = e->subs;
     cudaStream_t s = e->stream;
@@ -77,8 +71,11 @@ chd_status chd_apply_subscriptions(chd_engine* e, const chd_sub_batch* b, int64_
         return st;
     const uint32_t S = e->n_slots, C = e->g.cells;
     // 1. validate
-    subs_validate_kernel<<<blocks_for(n, 256), 256, 0, s>>>(ops, S, C, e->g.id_start, e->d_conn, e->lifecycle_used ? e->d_slot_ctl : nullptr, x.key,
-                                                            x.eff_slot, x.cell, x.status);
+    const uint8_t* ctl = e->lifecycle_used ? e->d_slot_ctl : nullptr;
+    if (slab)
+        subs_validate_kernel<true><<<blocks_for(n, 256), 256, 0, s>>>(ops, S, e->g, e->d_conn, ctl, x.key, x.eff_slot, x.cell, x.status);
+    else
+        subs_validate_kernel<false><<<blocks_for(n, 256), 256, 0, s>>>(ops, S, e->g, e->d_conn, ctl, x.key, x.eff_slot, x.cell, x.status);
     KCHECK(e);
     if (S > 0) {
         PairBuf& prev = e->pairs[e->cur];
@@ -121,6 +118,37 @@ chd_status chd_apply_subscriptions(chd_engine* e, const chd_sub_batch* b, int64_
         CU(e, cudaStreamSynchronize(s));
     }
     return CHD_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+chd_status chd_apply_subscriptions(chd_engine* e, const chd_sub_batch* b, int64_t now_ns, uint8_t* out_status) {
+    if (!e || !b) return CHD_ERR_INVALID;
+    const uint32_t n = b->n;
+    if (n && (!b->slot || !b->channel_id || !b->op)) return CHD_ERR_INVALID;
+    if (chd_rule_explicit_subs(e, "chd_apply_subscriptions") != CHD_OK) return CHD_ERR_STATE;
+    const chd_status st = check_batch(e, n, "chd_apply_subscriptions");
+    if (st != CHD_OK || n == 0) return st;
+    // LOCK: this stage opens epochs of the query stage's scan sites, which chd_query_channel_ids (any thread) also bumps.
+    // COPY_WAIT: the pair buffer written here is the one the pending copy kernel's tick will overwrite next.
+    // FETCH_GUARD: the pairs, their channel ids and the by-cell grouping are read-back sources.
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
+    return apply(e, b, now_ns, out_status, false);
+}
+
+chd_status chd_apply_subscriptions_sharded(chd_engine* e, const chd_sub_batch* b, int64_t now_ns, uint8_t* out_status) {
+    if (!e || !b) return CHD_ERR_INVALID;
+    const uint32_t n = b->n;
+    if (n && (!b->slot || !b->channel_id || !b->op)) return CHD_ERR_INVALID;
+    const char* fn = "chd_apply_subscriptions_sharded";
+    if (chd_rule_explicit_subs_slab(e, fn) != CHD_OK || chd_rule_rings_staged(e, fn) != CHD_OK) return CHD_ERR_STATE;
+    const chd_status st = check_batch(e, n, fn);
+    if (st != CHD_OK || n == 0) return st;
+    // the needs of chd_apply_subscriptions, for the same reasons
+    CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
+    return apply(e, b, now_ns, out_status, true);
 }
 
 }  // extern "C"

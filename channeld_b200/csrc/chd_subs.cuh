@@ -3,7 +3,7 @@
 // into its sorted pair run, scan the new run lengths, write the new pair buffer.  Semantics: include/chd_gpu_subs.h.
 #pragma once
 #include "chd_types.cuh"
-#include "../../include/chd_gpu_subs.h"
+#include "../../include/chd_gpu_subs_sharded.h"
 
 namespace chd {
 
@@ -36,19 +36,23 @@ struct SubMerge {
 
 constexpr uint32_t SUB_UNTOUCHED = 0xFFFFFFFFu;
 
-// 1. statuses of the rejected ops; sort keys: the cell (C for a rejected op, sorted behind every valid one) and the slot (S)
-__global__ void __launch_bounds__(256) subs_validate_kernel(SubOps ops, uint32_t n_slots, uint32_t cells, uint32_t id_start,
-                                                            const uint32_t* __restrict__ conn_id, const uint8_t* __restrict__ slot_ctl,
-                                                            uint32_t* __restrict__ key_cell, uint32_t* __restrict__ eff_slot,
-                                                            uint32_t* __restrict__ cell, uint8_t* __restrict__ status) {
+// 1. statuses of the rejected ops; sort keys: the cell (C for a rejected op, sorted behind every valid one) and the slot (S).
+// Slab (chd_apply_subscriptions_sharded): a SUB of a cell in a column the slab does not serve is rejected as well (after the slot
+// and channel tests); an UNSUB of any cell is not.
+template <bool Slab>
+__global__ void __launch_bounds__(256) subs_validate_kernel(SubOps ops, uint32_t n_slots, const GridDev g, const uint32_t* __restrict__ conn_id,
+                                                            const uint8_t* __restrict__ slot_ctl, uint32_t* __restrict__ key_cell,
+                                                            uint32_t* __restrict__ eff_slot, uint32_t* __restrict__ cell, uint8_t* __restrict__ status) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= ops.n) return;
     const uint32_t s = ops.slot[i], ch = ops.channel[i];
+    const uint32_t cells = g.cells, id_start = g.id_start;
     // a free slot (never added, or released: connection id 0) or one with a removal / migration pending
     const bool slot_ok = s < n_slots && conn_id[s] != 0u && (!slot_ctl || slot_ctl[s] == SLOT_NORMAL);
     const bool ch_ok = ch >= id_start && ch - id_start < cells;
-    const bool ok = slot_ok && ch_ok;
-    if (!ok) status[i] = slot_ok ? (uint8_t)CHD_SUB_ERR_CHANNEL : (uint8_t)CHD_SUB_ERR_SLOT;
+    const bool served = !Slab || (ops.op[i] & 1u) || !ch_ok || g.serves_column((ch - id_start) % g.cols);
+    const bool ok = slot_ok && ch_ok && served;
+    if (!ok) status[i] = !slot_ok ? (uint8_t)CHD_SUB_ERR_SLOT : (Slab && ch_ok) ? (uint8_t)CHD_SUB_ERR_OUTSIDE_SLAB : (uint8_t)CHD_SUB_ERR_CHANNEL;
     key_cell[i] = ok ? ch - id_start : cells;
     eff_slot[i] = ok ? s : n_slots;
     cell[i] = ok ? ch - id_start : 0u;

@@ -402,10 +402,15 @@ chd_status chd_rule_batch_waiting(chd_engine* e, const char* fn, bool generated)
     return refuse(e, "%s: q == NULL needs chd_prefetch_queries + chd_adopt_prefetched, or chd_follow_queries, first", fn);
 }
 
-// 10. Explicit subscriptions (chd_apply_subscriptions) are single-GPU: a slab engine's slots migrate between ranks with their pairs,
-// and the ops would have to follow them.  Rule 13 as well.
+// 10. Explicit subscriptions: chd_apply_subscriptions is the whole-world call and chd_apply_subscriptions_sharded the slab call
+// (its ops must name cells the slab serves, and reach each rank before the ring limits are exchanged).  Rule 13 as well; the slab
+// call follows rule 12's staged updates too (chd_rule_rings_staged, at its call site).
 chd_status chd_rule_explicit_subs(chd_engine* e, const char* fn) {
-    if (e->slab) return refuse(e, "%s: explicit subscriptions are not available on an engine made a slab (chd_set_slab / chd_comm_init)", fn);
+    if (e->slab) return refuse(e, "%s: explicit subscriptions on an engine made a slab (chd_set_slab / chd_comm_init) use chd_apply_subscriptions_sharded", fn);
+    return chd_rule_no_chain(e, fn, false);
+}
+chd_status chd_rule_explicit_subs_slab(chd_engine* e, const char* fn) {
+    if (!e->slab) return refuse(e, "%s needs an engine made a slab (chd_set_slab / chd_comm_init); one engine uses chd_apply_subscriptions", fn);
     return chd_rule_no_chain(e, fn, false);
 }
 

@@ -196,6 +196,17 @@ class Engine:
         Each option is None (no op carries it) or one value per op; `present` (CHD_SUBOPT_* per op) says which ops carry which
         option, and defaults to every given option on every op.  Returns the CHD_SUB_* status per op (None with status=False, which
         adds no host synchronisation)."""
+        return self._subs(self.L.chd_apply_subscriptions, slots, channel_ids, ops, interval, delay, skip_self, skip_first, now_ns, present,
+                          status)
+
+    def apply_subscriptions_sharded(self, slots, channel_ids, ops, interval=None, delay=None, skip_self=None, skip_first=None, now_ns=0,
+                                    present=None, status=True):
+        """apply_subscriptions on a slab engine (include/chd_gpu_subs_sharded.h): a SUB of a cell outside the served columns gets
+        SUB_ERR_OUTSIDE_SLAB.  sharding.route_sub_ops splits a batch named by subscriber keys into the ranks' batches."""
+        return self._subs(self.L.chd_apply_subscriptions_sharded, slots, channel_ids, ops, interval, delay, skip_self, skip_first, now_ns,
+                          present, status)
+
+    def _subs(self, fn, slots, channel_ids, ops, interval, delay, skip_self, skip_first, now_ns, present, status):
         slots = np.ascontiguousarray(slots, np.uint32)
         n = len(slots)
         arrs = dict(slot=slots, channel_id=np.ascontiguousarray(channel_ids, np.uint32), op=np.ascontiguousarray(ops, np.uint8))
@@ -210,7 +221,7 @@ class Engine:
         b = capi.SubBatch(n=n, **{k: ptr(a) for k, a in arrs.items()})
         self._keep_subs = arrs  # (the copies are asynchronous without out_status)
         out = np.zeros(n, np.uint8) if status else None
-        self._ck(self.L.chd_apply_subscriptions(self.h, C.byref(b), int(now_ns), ptr(out)))
+        self._ck(fn(self.h, C.byref(b), int(now_ns), ptr(out)))
         return out
 
     def query_channel_ids(self, batch, cap=None):

@@ -103,6 +103,37 @@ def plan_migrations(table: SlotTable, new_owner):
     return arrivals, out_lists, [tuple(c) for c in in_calls], vacated
 
 
+def route_sub_ops(table: SlotTable, subscribers):
+    """Splits a batch of explicit subscription ops (include/chd_gpu_subs_sharded.h) whose ops name subscriber keys into one batch per
+    rank: -> [(op indices int64, slots u32)] per rank, the ops of each rank in array order (so several ops on one pair keep theirs).
+    Give rank r's batch the op arrays indexed by its op indices and its slots, and put the ranks' statuses back in the batch's order
+    with merge_sub_status.  A key the table does not hold is routed nowhere and gets SUB_ERR_SLOT there.
+
+    A slab accepts SUBs of the cells it serves only (columns [col_lo - halo, col_hi + halo)).  A spatial server whose region plus
+    border spans more than one rank's served columns is therefore placed once per rank it needs, under one key per (connection,
+    rank): SlotTable keys are arbitrary, e.g. ("server", conn, r) placed on rank r.  Each of its ops names the key on the owner of the
+    cell's column, owner_of_column((channel - channel_id_start) % cols, cols, world); that rank serves the cell."""
+    keys = list(subscribers)
+    rank = np.array([table.owner.get(k, -1) for k in keys], np.int64)
+    slot = np.array([table.slot.get(k, 0) for k in keys], np.uint32)
+    out = []
+    for r in range(table.world):
+        idx = np.nonzero(rank == r)[0]
+        out.append((idx, slot[idx]))
+    return out
+
+
+def merge_sub_status(routes, statuses, n: int):
+    """route_sub_ops' inverse for the statuses: statuses[r] = rank r's CHD_SUB_* per op of its batch -> u8[n] in the batch's order,
+    SUB_ERR_SLOT for the ops no rank received (unknown keys)."""
+    from .capi import SUB_ERR_SLOT
+
+    out = np.full(int(n), SUB_ERR_SLOT, np.uint8)
+    for (idx, _), st in zip(routes, statuses):
+        out[idx] = np.asarray(st, np.uint8)
+    return out
+
+
 def net_migrant_delta(leave_src, enter_dst):
     """A connection migrated from rank A to rank B (plan_migrations' in_calls), as id-mode visible deltas see it: A's delta
     reports its old slot leaving everything A's snapshot held, B's reports its new slot entering everything it sees now.  The

@@ -17,6 +17,7 @@ package channeld
 #include "chd_gpu_subs.h"
 #include "chd_gpu_facing.h"
 #include "chd_gpu_rings.h"
+#include "chd_gpu_subs_sharded.h"
 */
 import "C"
 
@@ -750,6 +751,18 @@ type SubOps struct {
 // `now` and returns a CHD_SUB_* status per op, from which the host sends its SubscribedToChannel / UnsubscribedFromChannel replies.
 // The statuses are written before the call returns, so plain Go slices are fine.
 func (ctl *GpuStaticGrid2DSpatialController) ApplySubscriptions(ops *SubOps, now ChannelTime) ([]uint8, error) {
+	return ctl.applySubscriptions(ops, now, false)
+}
+
+// ApplySubscriptionsSharded is ApplySubscriptions on a slab engine (CommInit): each process applies the ops of the slots it holds,
+// after the TickSharded that ends a tick and before RingsAppend, migrations and the next TickSharded.  A SUB of a cell outside the
+// slab's served columns gets CHD_SUB_ERR_OUTSIDE_SLAB; a server whose cells span several slabs holds one slot per process and sends
+// each op to the process that owns the cell's column (include/chd_gpu_subs_sharded.h).
+func (ctl *GpuStaticGrid2DSpatialController) ApplySubscriptionsSharded(ops *SubOps, now ChannelTime) ([]uint8, error) {
+	return ctl.applySubscriptions(ops, now, true)
+}
+
+func (ctl *GpuStaticGrid2DSpatialController) applySubscriptions(ops *SubOps, now ChannelTime, sharded bool) ([]uint8, error) {
 	n := len(ops.Slot)
 	if n == 0 {
 		return nil, nil
@@ -780,7 +793,13 @@ func (ctl *GpuStaticGrid2DSpatialController) ApplySubscriptions(ops *SubOps, now
 	b := C.chd_sub_batch{n: C.uint32_t(n), slot: u32(ops.Slot), channel_id: u32(ops.ChannelId), op: u8(ops.Op), present: u8(ops.Present),
 		interval_ms: u32(ops.IntervalMs), delay_ms: delay, skip_self: u8(ops.SkipSelf), skip_first: u8(ops.SkipFirst)}
 	status := make([]uint8, n)
-	if st := C.chd_apply_subscriptions(ctl.engine, &b, C.int64_t(now), u8(status)); st != C.CHD_OK {
+	var st C.chd_status
+	if sharded {
+		st = C.chd_apply_subscriptions_sharded(ctl.engine, &b, C.int64_t(now), u8(status))
+	} else {
+		st = C.chd_apply_subscriptions(ctl.engine, &b, C.int64_t(now), u8(status))
+	}
+	if st != C.CHD_OK {
 		return nil, errors.New(C.GoString(C.chd_last_error(ctl.engine)))
 	}
 	return status, nil

@@ -46,7 +46,8 @@
  * into engine scratch on the engine stream, under the pointer rules of the other batch inputs (chd_gpu.h: pinned host memory
  * makes the copy asynchronous and is reusable after the next synchronising call).  out_status (host or device) == NULL adds no
  * host synchronisation; otherwise the statuses (one CHD_SUB_* per op) are written before the call returns.  Slab engines
- * (chd_set_slab / chd_comm_init) return CHD_ERR_STATE: explicit subscriptions across slabs are not supported.
+ * (chd_set_slab / chd_comm_init) return CHD_ERR_STATE: they apply explicit subscriptions with chd_apply_subscriptions_sharded
+ * (chd_gpu_subs_sharded.h).
  */
 #ifndef CHD_GPU_SUBS_H
 #define CHD_GPU_SUBS_H
