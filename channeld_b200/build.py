@@ -1,5 +1,5 @@
 """In-tree build of libchd_b200.so (hand-written CUDA for sm_90a, the H100 + the C ABI of include/chd_gpu.h,
-include/chd_gpu_subs.h, include/chd_gpu_facing.h, include/chd_gpu_rings.h and include/chd_gpu_subs_sharded.h).
+include/chd_gpu_subs.h, include/chd_gpu_facing.h, include/chd_gpu_rings.h, include/chd_gpu_subs_sharded.h and include/chd_gpu_ring_bytes.h).
 
 nvcc cross-compiles without a GPU.  The .so is a build product: git-ignored, rebuilt when a source is newer.
 """
@@ -30,7 +30,8 @@ def sources():
 def deps():
     out = [os.path.join(ROOT, "include", "chd_gpu.h"), os.path.join(ROOT, "include", "chd_gpu_subs.h"),
            os.path.join(ROOT, "include", "chd_gpu_facing.h"), os.path.join(ROOT, "include", "chd_gpu_rings.h"),
-           os.path.join(ROOT, "include", "chd_gpu_subs_sharded.h"), os.path.abspath(__file__)]
+           os.path.join(ROOT, "include", "chd_gpu_subs_sharded.h"), os.path.join(ROOT, "include", "chd_gpu_ring_bytes.h"),
+           os.path.abspath(__file__)]
     for f in os.listdir(CSRC):
         out.append(os.path.join(CSRC, f))
     return out

@@ -190,6 +190,8 @@ RING_SYMBOLS = ["chd_export_ring_limits", "chd_import_ring_limits"]
 # every symbol include/chd_gpu_subs_sharded.h declares (explicit subscriptions on slabs; checked by tests/test_subs_sharded_host.py)
 SUB_SHARDED_SYMBOLS = ["chd_apply_subscriptions_sharded"]
 SUB_ERR_OUTSIDE_SLAB = 7  # beside SUB_* above: a SUB of a cell in a column the slab does not serve
+# every symbol include/chd_gpu_ring_bytes.h declares (byte-carrying device rings; checked by tests/test_ring_bytes_host.py)
+RING_BYTES_SYMBOLS = ["chd_rings_reserve_bytes", "chd_rings_append_bytes", "chd_get_ring_bytes"]
 
 
 STAGE_BUILD, STAGE_INTEREST, STAGE_EMIT, STAGE_EMIT_KERNEL, STAGE_FANOUT, STAGE_TICK, STAGE_EXPORT, STAGE_EXCHANGE, STAGE_IMPORT, STAGE_READBACK, STAGE_VISIBLE_DELTA, STAGE_ENTITY_EVENTS, STAGE_FOLLOW = range(13)
@@ -423,6 +425,12 @@ def lib():
     L.chd_export_ring_limits.argtypes = [vp, vp, C.c_uint32, u32p]
     L.chd_import_ring_limits.restype = C.c_int
     L.chd_import_ring_limits.argtypes = [vp, vp, C.c_uint32]
+    L.chd_rings_reserve_bytes.restype = C.c_int
+    L.chd_rings_reserve_bytes.argtypes = [vp, C.c_uint32]
+    L.chd_rings_append_bytes.restype = C.c_int
+    L.chd_rings_append_bytes.argtypes = [vp, vp, C.c_uint32, vp, vp, vp, vp]
+    L.chd_get_ring_bytes.restype = C.c_int
+    L.chd_get_ring_bytes.argtypes = [vp, vp, vp, C.c_uint64, u64p]
     _lib = L
     return L
 

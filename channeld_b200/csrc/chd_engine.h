@@ -295,6 +295,21 @@ struct chd_engine {
     // ring-limit import (rule 12)
     bool rings_staged = false;
     uint32_t staged_updates = 0;
+    // rule 14: an append was made since chd_rings_init (the byte reservation comes before it); an append was applied, or the rings
+    // were emptied, after the last fan-out pass (chd_assemble_payloads replays that pass's windows over the rings it read)
+    bool rings_appended = false, rings_after_fanout = false;
+    // byte-carrying device rings (include/chd_gpu_ring_bytes.h, allocated by chd_rings_reserve_bytes): each cell's slab of per_cell
+    // bytes in `slab`, every entry slot's byte position (relative to its cell's slab) and length beside d_ring_arrival, each cell's
+    // live byte range (bb, be) in `cur`; the staged bytes of an append (upd_boff: [n_updates + 1] offsets into upd_bytes)
+    struct RingBytes {
+        bool on = false;
+        uint32_t per_cell = 0;
+        uint8_t* slab = nullptr;
+        uint32_t *pos = nullptr, *len = nullptr, *cur = nullptr;
+        unsigned long long* upd_boff = nullptr;
+        uint8_t* upd_bytes = nullptr;
+        uint64_t upd_boff_cap = 0, upd_bytes_cap = 0;
+    } rbytes;
     int64_t* d_cell_start_ns = nullptr;       // [C] per-channel ChannelTime origin (chd_set_channel_start_times) or nullptr
     bool have_cell_start = false;
     // the rings the fan-out and payload kernels read (chd_ring_view adds `start`): the staging copies above, the caller's device
@@ -646,7 +661,12 @@ chd_status chd_rule_facing(chd_engine* e, const char* fn);
 chd_status chd_rule_ring_limits(chd_engine* e, const char* fn);
 chd_status chd_rule_rings_staged(chd_engine* e, const char* fn);
 chd_status chd_rule_no_chain(chd_engine* e, const char* fn, bool fanout_only);
-// device-owned rings (chd_tick.cu): the append kernel on `s` over n_updates updates already uploaded into d_upd_*
+chd_status chd_rule_ring_bytes_reserve(chd_engine* e);
+chd_status chd_rule_ring_append(chd_engine* e, bool bytes);
+chd_status chd_rule_assemble_rings(chd_engine* e);
+chd_status chd_rule_payload_entries(chd_engine* e, uint32_t n_entries);
+// device-owned rings (chd_tick.cu): the append kernel on `s` over n_updates updates already uploaded into d_upd_* (and, on a
+// byte-carrying engine, their bytes into rbytes.upd_*)
 chd_status chd_rings_apply(chd_engine* e, cudaStream_t s, uint32_t n_updates);
 // followers (chd_follow.cu): the listed slots (n == 0 with slot == nullptr: every slot) follow nothing from now on; d_slot: the
 // same list on the device if the caller uploaded it already

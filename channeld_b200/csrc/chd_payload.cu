@@ -27,6 +27,7 @@ extern "C" {
 chd_status chd_set_payload_bytes(chd_engine* e, const uint64_t* entry_off, uint32_t n_entries, const uint8_t* entry_bytes, const uint64_t* full_off,
                                  const uint8_t* full_bytes, const char* type_url, uint32_t msg_type) {
     if (!e || !entry_off || !full_off || !type_url) return CHD_ERR_INVALID;
+    if (chd_rule_payload_entries(e, n_entries) != CHD_OK) return CHD_ERR_INVALID;
     CHD_ENTER(e, ENTRY_LOCK | ENTRY_COPY_WAIT);
     cudaStream_t s = e->stream;
     chd_engine::Payload& P = e->pl;
@@ -62,6 +63,7 @@ chd_status chd_assemble_payloads(chd_engine* e, uint32_t* out_n_classes, uint64_
         e->fail("chd_assemble_payloads before chd_set_payload_bytes");
         return CHD_ERR_STATE;
     }
+    if (chd_rule_assemble_rings(e) != CHD_OK) return CHD_ERR_STATE;
     // window classes of the last fan-out pass (results stay on the device)
     uint32_t n_classes = 0;
     chd_status st = chd_due_classes(e, nullptr, nullptr, nullptr, 0, &n_classes);
@@ -80,15 +82,13 @@ chd_status chd_assemble_payloads(chd_engine* e, uint32_t* out_n_classes, uint64_
     ENSURE(e, P.d_cls_off, P.cap_cls_off, (uint64_t)n_classes + 2);
     st = remake_site(e, P.site_cls, &P.cap_site_cls, (uint64_t)n_classes + 1, EP_PAYLOAD);
     if (st != CHD_OK) return st;
-    if (e->rings_owned) {
-        e->fail("chd_assemble_payloads needs host-owned rings (chd_set_rings): payload bytes are indexed by ring position");
-        return CHD_ERR_STATE;
-    }
     st = chd_ring_total_flush(e, s);
     if (st != CHD_OK) return st;
     const RingDev ring = chd_ring_view(e);
+    const chd_engine::RingBytes& rb = e->rbytes;
+    const bool dev = e->rings_owned;  // (byte-carrying: rule 14)
     const PayloadIn in{(const unsigned long long*)P.d_entry_off, P.d_entry_bytes, (const unsigned long long*)P.d_full_off, P.d_full_bytes, P.d_url, P.url_len,
-                       P.msg_type};
+                       P.msg_type, dev ? rb.slab : nullptr, dev ? rb.pos : nullptr, dev ? rb.len : nullptr, rb.per_cell};
     st = chd_epoch_tick(e, s, EP_PAYLOAD);
     if (st != CHD_OK) return st;
     payload_size_kernel<<<blocks_for(n_classes, 128), 128, 0, s>>>(n_classes, e->d_cls_out_rep, e->d_due, e->d_due_key, ring, e->d_conn, in, P.d_cls_len,

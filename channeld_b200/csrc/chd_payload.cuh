@@ -6,7 +6,7 @@
 // (data.go:246-256), anypb.New (data.go:295), proto.Marshal(ChannelDataUpdateMessage) (connection.go:58), proto.Marshal(Packet)
 // (connection.go:671), snappy.Encode (:678-681), 5-byte tag (:684-688).
 // Here: the host supplies the serialized bytes of every ring entry's updateMsg (and of each channel's full data message for
-// FULL sends).  Parsing the concatenation of serialized protobuf messages IS merging them (protobuf encoding rule: last scalar
+// FULL sends), or, on byte-carrying device rings (include/chd_gpu_ring_bytes.h), the rings keep each entry's bytes beside it.  Parsing the concatenation of serialized protobuf messages IS merging them (protobuf encoding rule: last scalar
 // wins, repeated fields append, embedded messages merge), so the merged payload of a window = the concatenation of its selected
 // entries' bytes, wrapped in the fixed field headers of Any / ChannelDataUpdateMessage / MessagePack / Packet:
 //   entry  = 0x0A len(mp) mp                                   (Packet.messages, channeld.proto:10-12)
@@ -36,7 +36,23 @@ struct PayloadIn {
     const uint8_t* type_url;              // Any.type_url of the channel data type
     uint32_t url_len;
     uint32_t msg_type;                    // MessageType_CHANNEL_DATA_UPDATE = 8
+    // byte-carrying device rings (chd_rings_reserve_bytes) instead of entry_off / entry_bytes, or ring_bytes == nullptr: entry k
+    // of cell c is ring_len[k] bytes at ring_bytes + c * bytes_per_cell + ring_pos[k]
+    const uint8_t* ring_bytes;
+    const uint32_t* ring_pos;
+    const uint32_t* ring_len;
+    uint64_t bytes_per_cell;
 };
+
+struct ByteSpan {
+    const uint8_t* p;
+    uint64_t n;
+};
+// the serialized updateMsg of ring entry k of `cell`
+__device__ __forceinline__ ByteSpan entry_span(const PayloadIn& in, uint32_t cell, uint32_t k) {
+    if (in.ring_bytes) return ByteSpan{in.ring_bytes + cell * in.bytes_per_cell + in.ring_pos[k], in.ring_len[k]};
+    return ByteSpan{in.entry_bytes + in.entry_off[k], in.entry_off[k + 1] - in.entry_off[k]};
+}
 
 __device__ __forceinline__ uint32_t varint_len(uint64_t v) {
     uint32_t n = 1;
@@ -103,7 +119,7 @@ __global__ void __launch_bounds__(128)
         const bool skipped = (dk.word >> 32) & 1ull;
         const uint32_t me = skipped ? conn_id[(uint32_t)dk.word] : 0u;
         for_each_selected(ring, *ring.total, cell, dk.lo, d.window_hi, skipped, me,
-                          [&](uint32_t e) { value += in.entry_off[e + 1] - in.entry_off[e]; });
+                          [&](uint32_t e) { value += entry_span(in, cell, e).n; });
     }
     const MsgSizes s = msg_sizes(value, in.url_len, d.channel_id, in.msg_type);
     cls_len[k] = s.entry > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)s.entry;
@@ -127,7 +143,7 @@ __global__ void __launch_bounds__(128)
     const uint32_t ring_total = *ring.total;
     uint64_t value = 0;
     if (d.kind == 0) value = in.full_off[cell + 1] - in.full_off[cell];
-    else for_each_selected(ring, ring_total, cell, dk.lo, d.window_hi, skipped, me, [&](uint32_t e) { value += in.entry_off[e + 1] - in.entry_off[e]; });
+    else for_each_selected(ring, ring_total, cell, dk.lo, d.window_hi, skipped, me, [&](uint32_t e) { value += entry_span(in, cell, e).n; });
     // all lanes copy the url and the value; lane 0 then writes the field headers in front of them (zero / empty fields
     // omitted like msg_sizes counts them).  The entry ends with the url bytes and the value field, so the sizes give the
     // header lengths.
@@ -143,10 +159,9 @@ __global__ void __launch_bounds__(128)
         for (uint64_t b = lane; b < value; b += 32) p[b] = src[b];
     } else {
         for_each_selected(ring, ring_total, cell, dk.lo, d.window_hi, skipped, me, [&](uint32_t e) {
-            const uint8_t* src = in.entry_bytes + in.entry_off[e];
-            const uint64_t len = in.entry_off[e + 1] - in.entry_off[e];
-            for (uint64_t b = lane; b < len; b += 32) p[b] = src[b];
-            p += len;
+            const ByteSpan sp = entry_span(in, cell, e);
+            for (uint64_t b = lane; b < sp.n; b += 32) p[b] = sp.p[b];
+            p += sp.n;
         });
     }
     if (lane == 0) {

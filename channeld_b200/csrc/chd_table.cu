@@ -443,6 +443,38 @@ chd_status chd_rule_no_chain(chd_engine* e, const char* fn, bool fanout_only) {
     return refuse(e, "%s: chd_begin_interest is pending (not joined by chd_tick yet)", fn);
 }
 
+// 14. Byte-carrying device rings (include/chd_gpu_ring_bytes.h).  chd_rings_reserve_bytes comes after chd_rings_init and before any
+// append since it, staged or applied (rules 12 and 13 as well).  A byte-carrying engine appends through chd_rings_append_bytes only, so that every entry carries
+// its bytes, and an engine without the reservation through chd_rings_append only.  chd_assemble_payloads replays the windows of
+// the last fan-out pass over the rings (for_each_selected), so on device rings it needs the reservation and rings that pass read:
+// no append applied and no chd_rings_init since it (an append staged on a communicator engine is applied by the next
+// chd_tick_sharded, before its fan-out).  The entries' bytes are in the rings, so chd_set_payload_bytes then carries none
+// (CHD_ERR_INVALID).
+chd_status chd_rule_ring_bytes_reserve(chd_engine* e) {
+    const char* fn = "chd_rings_reserve_bytes";
+    if (!e->rings_owned) return refuse(e, "%s before chd_rings_init", fn);
+    if (e->rings_appended) return refuse(e, "%s after an append: the reservation comes between chd_rings_init and the first append", fn);
+    return chd_rule_no_chain(e, fn, false);
+}
+chd_status chd_rule_ring_append(chd_engine* e, bool bytes) {
+    if (e->rbytes.on == bytes) return CHD_OK;
+    return bytes ? refuse(e, "chd_rings_append_bytes needs byte-carrying rings (chd_rings_reserve_bytes)")
+                 : refuse(e, "chd_rings_append on byte-carrying rings (chd_rings_reserve_bytes): every entry carries its bytes (chd_rings_append_bytes)");
+}
+chd_status chd_rule_assemble_rings(chd_engine* e) {
+    if (!e->rings_owned) return CHD_OK;
+    if (!e->rbytes.on)
+        return refuse(e, "chd_assemble_payloads needs host-owned rings (chd_set_rings): payload bytes are indexed by ring position "
+                         "(or byte-carrying device rings, chd_rings_reserve_bytes)");
+    if (e->rings_after_fanout) return refuse(e, "chd_assemble_payloads: the rings changed after the last fan-out pass (an append or chd_rings_init)");
+    return CHD_OK;
+}
+chd_status chd_rule_payload_entries(chd_engine* e, uint32_t n_entries) {
+    if (!n_entries || !e->rings_owned || !e->rbytes.on) return CHD_OK;
+    e->fail("chd_set_payload_bytes: %u entries on byte-carrying rings (chd_rings_reserve_bytes), whose entries carry their bytes: pass 0", n_entries);
+    return CHD_ERR_INVALID;
+}
+
 chd_status chd_entity_table_init(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_fresh_engine(e) != CHD_OK) return CHD_ERR_STATE;

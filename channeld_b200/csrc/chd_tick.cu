@@ -2,6 +2,7 @@
 // two-stream tick.
 #include "chd_engine.h"
 
+#include "chd_gpu_ring_bytes.h"
 #include "chd_emit.cuh"
 #include "chd_fanout.cuh"
 #include "chd_misc.cuh"
@@ -202,10 +203,13 @@ chd_status chd_rings_init(chd_engine* e, uint32_t capacity_per_cell) {
     rings_init_kernel<<<blocks_for((uint64_t)e->g.cells + 1, 128), 128, 0, s>>>(e->g.cells, capacity_per_cell, e->d_rb_begin, e->d_rb_end);
     KCHECK(e);
     CU(e, cudaMemsetAsync(e->d_ch_msg_index, 0, (uint64_t)e->g.cells * 8, s));
+    if (e->rbytes.on) CU(e, cudaMemsetAsync(e->rbytes.cur, 0, 8ull * e->g.cells, s));  // empty byte slabs, the reservation kept
     set_u32_kernel<<<1, 1, 0, s>>>(e->d_ring_total, (uint32_t)need);
     KCHECK(e);
     e->ring_total_pending = false;
     e->rings_owned = true;
+    e->rings_appended = e->rings_staged;  // (a staged append is still to come: the next chd_tick_sharded applies it to these rings)
+    e->rings_after_fanout = true;
     e->ring_cap = capacity_per_cell;
     e->ring = RingDev{e->d_rb_begin, e->d_rb_end, e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, e->d_ch_msg_index, e->d_ring_total, nullptr};
     e->pf_ring.cur = -1;
@@ -214,14 +218,8 @@ chd_status chd_rings_init(chd_engine* e, uint32_t capacity_per_cell) {
     return CHD_OK;
 }
 
-chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_updates, const int64_t* arrival_ns, const uint32_t* sender_conn_id) {
-    if (!e || !upd_off || (n_updates && (!arrival_ns || !sender_conn_id))) return CHD_ERR_INVALID;
-    if (!e->rings_owned) {
-        e->fail("chd_rings_append before chd_rings_init");
-        return CHD_ERR_STATE;
-    }
-    if (chd_rule_no_chain(e, "chd_rings_append", false) != CHD_OK || chd_rule_rings_staged(e, "chd_rings_append") != CHD_OK) return CHD_ERR_STATE;
-    CHD_ENTER(e, ENTRY_DEVICE);
+// one append's updates into d_upd_* on the engine stream
+static chd_status rings_upload(chd_engine* e, const uint32_t* upd_off, uint32_t n_updates, const int64_t* arrival_ns, const uint32_t* sender_conn_id) {
     cudaStream_t s = e->stream;
     const uint32_t C = e->g.cells;
     const uint64_t grown = (uint64_t)n_updates + n_updates / 2 + 1024;
@@ -232,21 +230,50 @@ chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_u
         CU(e, cudaMemcpyAsync(e->d_upd_arrival, arrival_ns, sizeof(int64_t) * n_updates, cudaMemcpyDefault, s));
         CU(e, cudaMemcpyAsync(e->d_upd_sender, sender_conn_id, sizeof(uint32_t) * n_updates, cudaMemcpyDefault, s));
     }
+    return CHD_OK;
+}
+
+// then staged for chd_tick_sharded (a communicator engine) or applied
+static chd_status rings_stage_or_apply(chd_engine* e, uint32_t n_updates) {
+    e->rings_appended = true;
     if (e->comm) {  // rule 12: chd_tick_sharded appends them once the other ranks' ring limits are in
         e->rings_staged = true;
         e->staged_updates = n_updates;
         return CHD_OK;
     }
-    return chd_rings_apply(e, s, n_updates);
+    return chd_rings_apply(e, e->stream, n_updates);
+}
+
+chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_updates, const int64_t* arrival_ns, const uint32_t* sender_conn_id) {
+    if (!e || !upd_off || (n_updates && (!arrival_ns || !sender_conn_id))) return CHD_ERR_INVALID;
+    if (!e->rings_owned) {
+        e->fail("chd_rings_append before chd_rings_init");
+        return CHD_ERR_STATE;
+    }
+    if (chd_rule_no_chain(e, "chd_rings_append", false) != CHD_OK || chd_rule_rings_staged(e, "chd_rings_append") != CHD_OK ||
+        chd_rule_ring_append(e, false) != CHD_OK)
+        return CHD_ERR_STATE;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    const chd_status st = rings_upload(e, upd_off, n_updates, arrival_ns, sender_conn_id);
+    return st != CHD_OK ? st : rings_stage_or_apply(e, n_updates);
 }
 
 chd_status chd_rings_apply(chd_engine* e, cudaStream_t s, uint32_t n_updates) {
     const uint32_t C = e->g.cells;
-    rings_append_kernel<<<blocks_for(C, 128), 128, 0, s>>>(C, e->ring_cap, e->d_upd_off, n_updates, e->d_upd_arrival, e->d_upd_sender, e->d_rb_begin, e->d_rb_end,
-                                                           e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, e->d_ch_msg_index, e->d_cell_max_interval,
-                                                           &e->d_ctr->overflow);
+    const chd_engine::RingBytes& rb = e->rbytes;
+    if (rb.on) {
+        rings_append_bytes_kernel<<<blocks_for((uint64_t)C * 32, 128), 128, 0, s>>>(
+            C, e->ring_cap, e->d_upd_off, n_updates, e->d_upd_arrival, e->d_upd_sender, rb.upd_boff, rb.upd_bytes, e->d_rb_begin, e->d_rb_end,
+            e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, rb.pos, rb.len, rb.slab, rb.per_cell, rb.cur, e->d_ch_msg_index, e->d_cell_max_interval,
+            &e->d_ctr->overflow);
+    } else {
+        rings_append_kernel<<<blocks_for(C, 128), 128, 0, s>>>(C, e->ring_cap, e->d_upd_off, n_updates, e->d_upd_arrival, e->d_upd_sender, e->d_rb_begin,
+                                                               e->d_rb_end, e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, e->d_ch_msg_index,
+                                                               e->d_cell_max_interval, &e->d_ctr->overflow);
+    }
     KCHECK(e);
     e->rings_staged = false;
+    e->rings_after_fanout = true;
     return CHD_OK;
 }
 
@@ -296,6 +323,136 @@ chd_status chd_get_rings(chd_engine* e, uint32_t* ring_off, int64_t* arrival_ns,
     return CHD_OK;
 }
 
+/* ---- byte-carrying device rings (include/chd_gpu_ring_bytes.h): each update's serialized updateMsg kept in the ring beside
+   its entry (rings_append_bytes_kernel), read in place by the payload kernels (chd_payload.cuh) */
+
+chd_status chd_rings_reserve_bytes(chd_engine* e, uint32_t bytes_per_cell) {
+    if (!e) return CHD_ERR_INVALID;
+    if (bytes_per_cell == 0) {
+        e->fail("chd_rings_reserve_bytes: bytes_per_cell must be positive");
+        return CHD_ERR_INVALID;
+    }
+    // (rule 12 too: staged updates were checked against the slab they were staged for, and their bytes would be applied to this one)
+    if (chd_rule_ring_bytes_reserve(e) != CHD_OK || chd_rule_rings_staged(e, "chd_rings_reserve_bytes") != CHD_OK) return CHD_ERR_STATE;
+    CHD_ENTER(e, ENTRY_DEVICE);
+    chd_engine::RingBytes& rb = e->rbytes;
+    const uint64_t C = e->g.cells;
+    // a failed allocation changes nothing: the per-slot arrays are kept once made, and a new slab replaces the old one only once it exists
+    const bool slots = (rb.pos || dalloc(e, &rb.pos, (uint64_t)e->lim.max_ring_entries)) && (rb.len || dalloc(e, &rb.len, (uint64_t)e->lim.max_ring_entries)) &&
+                       (rb.cur || dalloc(e, &rb.cur, 2 * C));
+    if (!slots) {
+        cudaGetLastError();  // (an allocation failure is not sticky: clear it for the next launch check)
+        return CHD_ERR_CUDA;
+    }
+    if (!rb.slab || rb.per_cell != bytes_per_cell) {
+        uint8_t* slab = nullptr;
+        if (!dalloc(e, &slab, C * bytes_per_cell)) {
+            cudaGetLastError();
+            e->fail("chd_rings_reserve_bytes: %llu cells x %u bytes cannot be allocated", (unsigned long long)C, bytes_per_cell);
+            return CHD_ERR_CAPACITY;
+        }
+        chd_dfree(e, rb.slab);
+        rb.slab = slab;
+    }
+    CU(e, cudaMemsetAsync(rb.cur, 0, 8 * C, e->stream));
+    rb.per_cell = bytes_per_cell;
+    rb.on = true;
+    return CHD_OK;
+}
+
+chd_status chd_rings_append_bytes(chd_engine* e, const uint32_t* upd_off, uint32_t n_updates, const int64_t* arrival_ns, const uint32_t* sender_conn_id,
+                                  const uint64_t* byte_off, const uint8_t* bytes) {
+    if (!e || !upd_off || !byte_off || (n_updates && (!arrival_ns || !sender_conn_id))) return CHD_ERR_INVALID;
+    if (!e->rings_owned) {
+        e->fail("chd_rings_append_bytes before chd_rings_init");
+        return CHD_ERR_STATE;
+    }
+    if (chd_rule_no_chain(e, "chd_rings_append_bytes", false) != CHD_OK || chd_rule_rings_staged(e, "chd_rings_append_bytes") != CHD_OK ||
+        chd_rule_ring_append(e, true) != CHD_OK)
+        return CHD_ERR_STATE;
+    // byte_off is a host array: its lengths are checked here, before anything is appended
+    for (uint32_t k = 0; k < n_updates; k++) {
+        if (byte_off[k + 1] < byte_off[k] || byte_off[k + 1] - byte_off[k] > e->rbytes.per_cell) {
+            e->fail("chd_rings_append_bytes: update %u has byte offsets %llu .. %llu (bytes_per_cell %u)", k, (unsigned long long)byte_off[k],
+                    (unsigned long long)byte_off[k + 1], e->rbytes.per_cell);
+            return CHD_ERR_INVALID;
+        }
+    }
+    const uint64_t nb = byte_off[n_updates];
+    if (nb && !bytes) {
+        e->fail("chd_rings_append_bytes: %llu bytes and no byte array", (unsigned long long)nb);
+        return CHD_ERR_INVALID;
+    }
+    CHD_ENTER(e, ENTRY_DEVICE);
+    chd_engine::RingBytes& rb = e->rbytes;
+    cudaStream_t s = e->stream;
+    if (!ensure_cap(e, &rb.upd_boff, &rb.upd_boff_cap, (uint64_t)n_updates + 1, (uint64_t)n_updates + n_updates / 2 + 1025) ||
+        !ensure_cap(e, &rb.upd_bytes, &rb.upd_bytes_cap, nb + 1, nb + nb / 2 + 4096))
+        return CHD_ERR_CUDA;
+    chd_status st = rings_upload(e, upd_off, n_updates, arrival_ns, sender_conn_id);
+    if (st != CHD_OK) return st;
+    CU(e, cudaMemcpyAsync(rb.upd_boff, byte_off, 8 * ((uint64_t)n_updates + 1), cudaMemcpyHostToDevice, s));
+    if (nb) CU(e, cudaMemcpyAsync(rb.upd_bytes, bytes, nb, cudaMemcpyDefault, s));
+    return rings_stage_or_apply(e, n_updates);
+}
+
+chd_status chd_get_ring_bytes(chd_engine* e, uint64_t* byte_off, uint8_t* bytes, uint64_t cap_bytes, uint64_t* total) {
+    if (!e) return CHD_ERR_INVALID;
+    if (!e->rings_owned || !e->rbytes.on) {
+        e->fail("chd_get_ring_bytes needs byte-carrying device rings (chd_rings_reserve_bytes)");
+        return CHD_ERR_STATE;
+    }
+    if (chd_rule_rings_staged(e, "chd_get_ring_bytes") != CHD_OK) return CHD_ERR_STATE;  // (its length pass reuses d_upd_off)
+    CHD_ENTER(e, ENTRY_COPY_WAIT);
+    const chd_engine::RingBytes& rb = e->rbytes;
+    cudaStream_t s = e->stream;
+    const uint32_t C = e->g.cells;
+    if (total) *total = 0;
+    // (control-plane call: the entry CSR as chd_get_rings makes it, the cells' byte offsets through temporaries)
+    if (!e->d_ring_scan_scratch && !dalloc(e, &e->d_ring_scan_scratch, scan_scratch_elems(C + 1))) return CHD_ERR_CUDA;
+    ring_len_kernel<<<blocks_for(C, 128), 128, 0, s>>>(C, e->d_rb_begin, e->d_rb_end, e->d_upd_off);
+    KCHECK(e);
+    SCAN(e, exclusive_scan<uint32_t, uint32_t>(e->d_upd_off, e->d_ring_flat_off, C, e->d_ring_scan_scratch, s));
+    uint32_t* blen = nullptr;
+    unsigned long long *cell_boff = nullptr, *scratch = nullptr;
+    CU(e, cudaMallocAsync((void**)&blen, 4ull * C + 4, s));
+    CU(e, cudaMallocAsync((void**)&cell_boff, 8ull * (C + 2), s));
+    CU(e, cudaMallocAsync((void**)&scratch, 8ull * scan_scratch_elems(C + 1), s));
+    ring_bytes_len_kernel<<<blocks_for(C, 128), 128, 0, s>>>(C, rb.cur, blen);
+    KCHECK(e);
+    SCAN(e, exclusive_scan<uint32_t, unsigned long long>(blen, cell_boff, C, scratch, s));
+    uint64_t* h64 = (uint64_t*)e->h_u32;
+    CU(e, cudaMemcpyAsync(h64, cell_boff + C, 8, cudaMemcpyDeviceToHost, s));
+    CU(e, cudaMemcpyAsync(h64 + 1, e->d_ring_flat_off + C, 4, cudaMemcpyDeviceToHost, s));
+    CU(e, cudaStreamSynchronize(s));
+    const uint64_t nb = h64[0];
+    const uint32_t n_live = (uint32_t)h64[1];
+    if (total) *total = nb;
+    chd_status st = CHD_OK;
+    if (bytes && nb > cap_bytes) {
+        e->fail("chd_get_ring_bytes: %llu bytes > cap_bytes %llu", (unsigned long long)nb, (unsigned long long)cap_bytes);
+        st = CHD_ERR_CAPACITY;
+    } else if (byte_off || bytes) {
+        unsigned long long* o_boff = nullptr;
+        uint8_t* o_bytes = nullptr;
+        CU(e, cudaMallocAsync((void**)&o_boff, 8ull * (n_live + 1), s));
+        CU(e, cudaMallocAsync((void**)&o_bytes, nb + 1, s));
+        ring_bytes_gather_kernel<<<C, 128, 0, s>>>(C, e->d_rb_begin, e->d_rb_end, e->d_ring_flat_off, rb.pos, rb.cur, cell_boff, rb.slab, rb.per_cell,
+                                                    o_boff, o_bytes);
+        KCHECK(e);
+        CU(e, cudaMemcpyAsync(o_boff + n_live, cell_boff + C, 8, cudaMemcpyDeviceToDevice, s));
+        if (byte_off) CU(e, cudaMemcpyAsync(byte_off, o_boff, 8ull * (n_live + 1), cudaMemcpyDefault, s));
+        if (bytes && nb) CU(e, cudaMemcpyAsync(bytes, o_bytes, nb, cudaMemcpyDefault, s));
+        CU(e, cudaFreeAsync(o_boff, s));
+        CU(e, cudaFreeAsync(o_bytes, s));
+    }
+    CU(e, cudaFreeAsync(blen, s));
+    CU(e, cudaFreeAsync(cell_boff, s));
+    CU(e, cudaFreeAsync(scratch, s));
+    CU(e, cudaStreamSynchronize(s));
+    return st;
+}
+
 chd_status chd_set_channel_start_times(chd_engine* e, const int64_t* start_ns) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_no_chain(e, "chd_set_channel_start_times", false) != CHD_OK) return CHD_ERR_STATE;
@@ -333,6 +490,7 @@ static chd_status fanout_enqueue(chd_engine* e, cudaStream_t s, int64_t t_ns) {
     if (st == CHD_OK) st = chd_ring_total_flush(e, s);
     if (st != CHD_OK) return st;
     chd_epoch_tick(e, s, EP_FANOUT);
+    e->rings_after_fanout = false;
     stage_begin_kernel<<<1, 1, 0, s>>>(e->d_time + 1, t_ns, e->d_epoch + EP_FANOUT, &e->d_ctr->n_due, 1, nullptr);
     KCHECK(e);
     const RingDev ring = chd_ring_view(e);

@@ -682,3 +682,32 @@ class Engine:
 
     def import_ring_limits(self, d_records, n):
         self._ck(self.L.chd_import_ring_limits(self.h, ptr(d_records), int(n)))
+
+    # ---- byte-carrying device rings (include/chd_gpu_ring_bytes.h)
+    def rings_reserve_bytes(self, bytes_per_cell):
+        """After chd_rings_init and before any append: every ring entry carries its update's serialized bytes, in a slab of
+        bytes_per_cell bytes per cell."""
+        self._ck(self.L.chd_rings_reserve_bytes(self.h, int(bytes_per_cell)))
+
+    def rings_append_bytes(self, upd_off, arrival, sender, byte_off, data):
+        """chd_rings_append with update k carrying data[byte_off[k]:byte_off[k + 1]] (byte_off: host u64, n_updates + 1 offsets;
+        data: bytes, a u8 array or a device tensor)."""
+        upd_off = np.ascontiguousarray(upd_off, np.uint32)
+        arrival = np.ascontiguousarray(arrival, np.int64)
+        sender = np.ascontiguousarray(sender, np.uint32)
+        byte_off = np.ascontiguousarray(byte_off, np.uint64)
+        if isinstance(data, (bytes, bytearray)):
+            data = np.frombuffer(data, np.uint8)
+        n = len(byte_off) - 1
+        self._ck(self.L.chd_rings_append_bytes(self.h, ptr(upd_off), n, ptr(arrival) if n else None, ptr(sender) if n else None, ptr(byte_off),
+                                               ptr(data) if len(data) else None))
+
+    def get_ring_bytes(self):
+        """-> (byte_off u64 [n_live + 1], data u8): every live ring entry's bytes, in the entry order of chd_get_rings"""
+        off = np.zeros(self.n_cells + 1, np.uint32)
+        self._ck(self.L.chd_get_rings(self.h, ptr(off), None, None, None, None, 0))
+        total = C.c_uint64()
+        self._ck(self.L.chd_get_ring_bytes(self.h, None, None, 0, C.byref(total)))
+        byte_off, data = np.zeros(int(off[-1]) + 1, np.uint64), np.zeros(total.value + 1, np.uint8)
+        self._ck(self.L.chd_get_ring_bytes(self.h, ptr(byte_off), ptr(data), total.value, C.byref(total)))
+        return byte_off, data[:total.value]

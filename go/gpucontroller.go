@@ -18,6 +18,7 @@ package channeld
 #include "chd_gpu_facing.h"
 #include "chd_gpu_rings.h"
 #include "chd_gpu_subs_sharded.h"
+#include "chd_gpu_ring_bytes.h"
 */
 import "C"
 
@@ -960,6 +961,24 @@ func (ctl *GpuStaticGrid2DSpatialController) RingsInit(capacityPerCell uint32) e
 
 func (ctl *GpuStaticGrid2DSpatialController) RingsAppend(updOff *C.uint32_t, n uint32, arrival *C.int64_t, sender *C.uint32_t) error {
 	if st := C.chd_rings_append(ctl.engine, updOff, C.uint32_t(n), arrival, sender); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
+// RingsReserveBytes / RingsAppendBytes (include/chd_gpu_ring_bytes.h): every ring entry carries its update's serialized
+// updateMsg, so AssemblePayloads reads the bytes from the device rings.  The reserve goes right after RingsInit; byteOff is a Go
+// slice of n+1 offsets into bytes (C memory on the tick path).  Per tick: TickBatch, the payload calls, then RingsAppendBytes.
+func (ctl *GpuStaticGrid2DSpatialController) RingsReserveBytes(bytesPerCell uint32) error {
+	if st := C.chd_rings_reserve_bytes(ctl.engine, C.uint32_t(bytesPerCell)); st != C.CHD_OK {
+		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
+	}
+	return nil
+}
+
+func (ctl *GpuStaticGrid2DSpatialController) RingsAppendBytes(updOff *C.uint32_t, n uint32, arrival *C.int64_t, sender *C.uint32_t, byteOff []uint64,
+	bytes *C.uint8_t) error {
+	if st := C.chd_rings_append_bytes(ctl.engine, updOff, C.uint32_t(n), arrival, sender, (*C.uint64_t)(unsafe.Pointer(&byteOff[0])), bytes); st != C.CHD_OK {
 		return errors.New(C.GoString(C.chd_last_error(ctl.engine)))
 	}
 	return nil
