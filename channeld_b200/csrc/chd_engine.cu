@@ -339,21 +339,16 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     for (CopySet& c : e->copy_set)
         ok = ok && dalloc(e, &c.voff, P + 1) && dalloc(e, &c.first_pair, e->max_tiles + 8) && dalloc(e, &c.tile_desc, (L.max_visible + EMIT_TILE - 1) / EMIT_TILE + 8) &&
              dalloc(e, &c.general_tiles, (L.max_visible + EMIT_TILE - 1) / EMIT_TILE + 8) && dalloc(e, &c.n_general, 4) && dalloc(e, &c.n_visible, 1);
-    ok = ok && dalloc(e, &e->d_cell_max_interval, C) && dalloc(e, &e->d_cell_start_ns, C) && dalloc(e, &e->d_rb_begin, C + 1) && dalloc(e, &e->d_rb_end, C + 1) &&
-         dalloc(e, &e->d_ring_flat_off, C + 2) && dalloc(e, &e->d_upd_off, C + 1);
-    ok = ok && dalloc(e, &e->d_ring_off, C + 1) && dalloc(e, &e->d_ring_arrival, (uint64_t)L.max_ring_entries) &&
-         dalloc(e, &e->d_ring_sender, (uint64_t)L.max_ring_entries) && dalloc(e, &e->d_ring_index, (uint64_t)L.max_ring_entries) &&
-         dalloc(e, &e->d_ch_msg_index, C) && dalloc(e, &e->d_by_cell, P) &&
+    ok = ok && dalloc(e, &e->d_cell_max_interval, C) && dalloc(e, &e->d_cell_start_ns, C) && chd_rings_create(e) == CHD_OK && dalloc(e, &e->d_by_cell, P) &&
          alloc_cell_sort(e, e->pair_sort, (uint32_t)std::min<uint64_t>(4096, (P + BUILD_TILE - 1) / BUILD_TILE), true, EP_QUERY) &&
          dalloc(e, &e->pair_sort.tmp_key, P) && dalloc(e, &e->pair_sort.tmp_val, P) &&
          dalloc(e, &e->d_due, (uint64_t)L.max_due) && dalloc(e, &e->d_due_key, (uint64_t)L.max_due) && dalloc(e, &e->d_ctr, 1) && dalloc(e, &e->d_time, 2) &&
-         dalloc(e, &e->d_ring_total, 1) && dalloc(e, &e->d_n_build, 1);
+         dalloc(e, &e->d_n_build, 1);
     if (!ok) {
         g_create_error = e->err;
         chd_destroy(e);
         return CHD_ERR_CUDA;
     }
-    e->ring = RingDev{e->d_ring_off, e->d_ring_off + 1, e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, nullptr, e->d_ring_total, nullptr};
     for (ScanSite* site : e->sites)
         site->error = &e->d_ctr->overflow;
     CCU(cudaHostAlloc((void**)&e->h_ctr, sizeof(Counters), cudaHostAllocDefault));
@@ -371,13 +366,10 @@ chd_status chd_create(const chd_grid_cfg* cfg, const chd_limits* lim_in, int dev
     CCU(cudaMemsetAsync(e->d_slot_ctl, 0, S, e->stream));
     CCU(cudaMemsetAsync(e->d_cell_max_interval, 0, C * 4, e->stream));
     CCU(cudaMemsetAsync(e->d_cell_start_ns, 0, C * 8, e->stream));
-    CCU(cudaMemsetAsync(e->d_ch_msg_index, 0, C * 8, e->stream));
     CCU(cudaMemsetAsync(e->d_conn, 0, S * 4, e->stream));
     CCU(cudaMemsetAsync(e->d_time, 0, 16, e->stream));
-    CCU(cudaMemsetAsync(e->d_ring_total, 0, 4, e->stream));
     CCU(cudaMemsetAsync(e->pairs[0].off, 0, (S + 1) * 4, e->stream));
     CCU(cudaMemsetAsync(e->pairs[1].off, 0, (S + 1) * 4, e->stream));
-    CCU(cudaMemsetAsync(e->d_ring_off, 0, (C + 1) * 4, e->stream));
     CCU(cudaMemsetAsync(e->d_vis_off, 0, (S + 1) * 8, e->stream));
     CCU(cudaStreamSynchronize(e->stream));
 #undef CCU

@@ -4,7 +4,8 @@
 //   chd_engine.cu    create / destroy, streams, memory, the prefetch protocol, CUDA-graph stage cache, instrumentation
 //   chd_entities.cu  positions, cell assignment, spatial-hash build, the cell sort (chd_cell_sort)
 //   chd_interest.cu  subscribers (lifecycle), query batches, QueryChannelIds, interest update
-//   chd_tick.cu      emit, rings, fan-out, the batched tick and its two-stream choreography, summary
+//   chd_tick.cu      emit, fan-out, channel start times, prefetch adoption, the batched tick and its two-stream choreography, summary
+//   chd_rings.cu     update rings: host-owned snapshots, prefetched sets, device-owned rings with or without bytes, read-back
 //   chd_results.cu   getters, chd_fetch_results, device views
 //   chd_shard.cu     multi-GPU X-slabs: border export, halo import, the NCCL exchange
 //   chd_extras.cu    window classes, ADJACENT_CHANNELS broadcast sets, config-plane helpers
@@ -126,7 +127,6 @@ struct chd_engine {
     GraphSet g_build, g_build_b, g_interest, g_interest_b, g_emit_prep, g_fanout, g_export, g_import;
     uint64_t graph_launches = 0, graph_captures = 0;
     int64_t* d_time = nullptr;      // [0] = now_ns of the last update_interest, [1] = t_ns of the last fanout_tick
-    uint32_t* d_ring_total = nullptr;
     // optional per-stage CUDA-event timing (chd_profile_*): [stage][0=start,1=stop]
     int profiling = 0;  // 0 off, 1 every stage, 2 the emit kernel only
     static constexpr int EV_RING = 1024;
@@ -192,16 +192,10 @@ struct chd_engine {
         QueryDev view;   // a prefetch set: the batch it holds
         uint32_t spots;  // and its spot total
     } dq{};
-    // chd_prefetch_queries / chd_prefetch_rings: two staging sets each, allocated by the first prefetch that fills them.
+    // chd_prefetch_queries: two staging sets, allocated by the first prefetch that fills them.
     // pf_q.cur: the adopted batch the next interest update with q == NULL consumes (-1 once consumed).
     QStage dq_pf[2] = {};
     Prefetch pf_q;
-    struct RStage {
-        uint32_t *off, *sender; int64_t* arrival; uint64_t *index, *cmi;
-        uint32_t total;  // entries uploaded
-        bool has_cmi;    // cmi holds a channel_msg_index
-    } ring_pf[2] = {};
-    Prefetch pf_ring;  // pf_ring.cur: the set `ring` reads (-1: the rings came from chd_set_rings / chd_rings_init)
     Bbox* d_bbox = nullptr;
     uint32_t *d_window = nullptr, *d_side_cell = nullptr, *d_side_dist = nullptr, *d_side_cnt = nullptr;
     uint64_t* d_win_off = nullptr;
@@ -274,53 +268,59 @@ struct chd_engine {
     uint64_t* d_vis_off = nullptr;
     uint64_t max_tiles = 0;
     uint64_t vis_estimate = 0;  // n_visible of the last summary the host decoded (0 = none yet): sizes the emit grid
-    // fanout
-    uint32_t *d_ring_off = nullptr, *d_ring_sender = nullptr;
-    int64_t* d_ring_arrival = nullptr;
-    uint64_t *d_ring_index = nullptr, *d_ch_msg_index = nullptr;
-    // device-owned rings (chd_rings_init: ChannelData.OnUpdate on the GPU, data.go:149-173): per-cell begin / end cursors into
-    // slabs of ring_cap entries inside d_ring_arrival / d_ring_sender / d_ring_index; d_ch_msg_index = ChannelData.msgIndex
-    bool rings_owned = false;
-    uint32_t ring_cap = 0;
-    uint32_t *d_rb_begin = nullptr, *d_rb_end = nullptr, *d_upd_off = nullptr, *d_upd_sender = nullptr, *d_ring_flat_off = nullptr;
-    int64_t* d_upd_arrival = nullptr;
-    uint64_t upd_arrival_cap = 0, upd_sender_cap = 0;
-    uint32_t* d_ring_scan_scratch = nullptr;
+    // ---- update rings (chd_rings.cu): host-owned (one tick's CSR by cell: chd_set_rings, chd_prefetch_rings) or device-owned
+    // (chd_rings_init: ChannelData.OnUpdate on the GPU, data.go:149-173)
+    struct Rings {
+        struct RStage {
+            uint32_t *off = nullptr, *sender = nullptr; int64_t* arrival = nullptr; uint64_t *index = nullptr, *cmi = nullptr;
+            uint32_t total = 0;    // entries uploaded
+            bool has_cmi = false;  // cmi holds a channel_msg_index
+        };
+        // set: chd_set_rings' staging (chd_create); on device-owned rings arrival / sender / index are the entry slabs and cmi is
+        // ChannelData.msgIndex.  pf_set: chd_prefetch_rings' two sets, allocated by the first prefetch that fills them; pf.cur is
+        // the set `view` reads (-1: the rings came from chd_set_rings / chd_rings_init).
+        RStage set, pf_set[2];
+        Prefetch pf;
+        // device-owned rings: per-cell begin / end cursors into slabs of `cap` entries inside set.arrival / set.sender / set.index;
+        // the updates of one append (upd_off: CSR by cell), grown on demand; the read-back's live-entry CSR and its scan scratch
+        bool owned = false;
+        uint32_t cap = 0;
+        uint32_t *begin = nullptr, *end = nullptr, *upd_off = nullptr, *upd_sender = nullptr, *flat_off = nullptr, *scan_scratch = nullptr;
+        int64_t* upd_arrival = nullptr;
+        uint64_t upd_arrival_cap = 0, upd_sender_cap = 0;
+        // a communicator engine's chd_rings_append only uploads its updates into upd_*: chd_tick_sharded appends them after the
+        // ring-limit import (rule 12)
+        bool staged = false;
+        uint32_t staged_updates = 0;
+        // rule 14: an append was made since chd_rings_init (the byte reservation comes before it); an append was applied, or the
+        // rings were emptied, after the last fan-out pass (chd_assemble_payloads replays that pass's windows over the rings it read)
+        bool appended = false, after_fanout = false;
+        // byte-carrying device rings (include/chd_gpu_ring_bytes.h, allocated by chd_rings_reserve_bytes): each cell's slab of
+        // per_cell bytes in `slab`, every entry slot's byte position (relative to its cell's slab) and length beside set.arrival, each
+        // cell's live byte range (bb, be) in `cur`; the staged bytes of an append (upd_boff: [n_updates + 1] offsets into upd_bytes)
+        struct RingBytes {
+            bool on = false;
+            uint32_t per_cell = 0;
+            uint8_t *slab = nullptr, *upd_bytes = nullptr;
+            uint32_t *pos = nullptr, *len = nullptr, *cur = nullptr;
+            unsigned long long* upd_boff = nullptr;
+            uint64_t upd_boff_cap = 0, upd_bytes_cap = 0;
+        } bytes;
+        // the rings the kernels read (chd_ring_view adds `start`): `set`, the caller's device arrays (zero-copy), an adopted prefetch set
+        // or the device-owned rings; d_total their entry count, written for host-owned rings by the next pass that reads them, on its
+        // stream (chd_ring_total_flush): a kernel on the engine stream between ticks would queue behind the copy kernel's grid
+        RingDev view{};
+        uint32_t* d_total = nullptr;
+        uint32_t total = 0;
+        bool total_pending = false;
+    } rings;
     uint32_t* d_cell_max_interval = nullptr;  // [C] ChannelData.maxFanOutIntervalMs (subscription.go:84-86)
     // ring limits on slabs (include/chd_gpu_rings.h), allocated by their first use: the exported shadow of d_cell_max_interval [C],
     // the record count of an export through chd_export_ring_limits, the export compaction's scan site
     uint32_t *d_ring_lim_x = nullptr, *d_ring_lim_n = nullptr;
     ScanSite site_ring_lim{};
-    // a communicator engine's chd_rings_append only uploads its updates into d_upd_*: chd_tick_sharded appends them after the
-    // ring-limit import (rule 12)
-    bool rings_staged = false;
-    uint32_t staged_updates = 0;
-    // rule 14: an append was made since chd_rings_init (the byte reservation comes before it); an append was applied, or the rings
-    // were emptied, after the last fan-out pass (chd_assemble_payloads replays that pass's windows over the rings it read)
-    bool rings_appended = false, rings_after_fanout = false;
-    // byte-carrying device rings (include/chd_gpu_ring_bytes.h, allocated by chd_rings_reserve_bytes): each cell's slab of per_cell
-    // bytes in `slab`, every entry slot's byte position (relative to its cell's slab) and length beside d_ring_arrival, each cell's
-    // live byte range (bb, be) in `cur`; the staged bytes of an append (upd_boff: [n_updates + 1] offsets into upd_bytes)
-    struct RingBytes {
-        bool on = false;
-        uint32_t per_cell = 0;
-        uint8_t* slab = nullptr;
-        uint32_t *pos = nullptr, *len = nullptr, *cur = nullptr;
-        unsigned long long* upd_boff = nullptr;
-        uint8_t* upd_bytes = nullptr;
-        uint64_t upd_boff_cap = 0, upd_bytes_cap = 0;
-    } rbytes;
     int64_t* d_cell_start_ns = nullptr;       // [C] per-channel ChannelTime origin (chd_set_channel_start_times) or nullptr
     bool have_cell_start = false;
-    // the rings the fan-out and payload kernels read (chd_ring_view adds `start`): the staging copies above, the caller's device
-    // arrays (zero-copy), an adopted prefetch set or the device-owned rings.  Set by chd_create, chd_set_rings, chd_rings_init
-    // and chd_adopt_prefetched.
-    RingDev ring{};
-    // the entry count of host-owned rings (chd_set_rings, an adopted prefetch), written to d_ring_total by the next pass that reads
-    // the rings, on that pass's stream (chd_ring_total_flush): a kernel on the engine stream between ticks would queue behind the
-    // copy kernel's grid, and the next tick's head would wait for it
-    uint32_t ring_total = 0;
-    bool ring_total_pending = false;
 
     uint32_t* d_by_cell = nullptr;  // pairs grouped by cell
     CellSort pair_sort;             // its sort: one block per tile of max_pairs, at most 4096; P-sized temporaries
@@ -621,9 +621,13 @@ chd_status chd_update_interest_on(chd_engine* e, cudaStream_t s, const chd_query
 // device view; *spots (if given): the batch's spot total
 chd_status chd_upload_queries(chd_engine* e, cudaStream_t s, const chd_query_batch* q, QueryDev* out, bool need_sub,
                               chd_engine::QStage* stage = nullptr, uint32_t* spots = nullptr);
-// what the fan-out / payload kernels read: the host-owned CSR snapshot (staged or zero-copy) or the device-owned rings
+// update rings (chd_rings.cu): what the kernels read; chd_create's and chd_adopt_prefetched's parts; the append kernel on `s` over
+// n_updates updates already in rings.upd_* (and, on a byte-carrying engine, their bytes in rings.bytes.upd_*)
 RingDev chd_ring_view(const chd_engine* e);
 chd_status chd_ring_total_flush(chd_engine* e, cudaStream_t s);
+chd_status chd_rings_create(chd_engine* e);
+void chd_rings_adopt(chd_engine* e);
+chd_status chd_rings_apply(chd_engine* e, cudaStream_t s, uint32_t n_updates);
 // The stable sort by cell on `s` (chd_entities.cu): values val (nullptr: the index) of keys key[0, n) in [0, keys) (n_ptr: the
 // live length on the device) into val_out, in <= 2 passes of <= 10-bit digits.  key_out: where a two-pass sort writes the sorted
 // keys.  csr: the cell CSR to publish (nullptr: none).  bump: the epoch the first kernel opens.  assign: pass 0's histogram also
@@ -665,9 +669,6 @@ chd_status chd_rule_ring_bytes_reserve(chd_engine* e);
 chd_status chd_rule_ring_append(chd_engine* e, bool bytes);
 chd_status chd_rule_assemble_rings(chd_engine* e);
 chd_status chd_rule_payload_entries(chd_engine* e, uint32_t n_entries);
-// device-owned rings (chd_tick.cu): the append kernel on `s` over n_updates updates already uploaded into d_upd_* (and, on a
-// byte-carrying engine, their bytes into rbytes.upd_*)
-chd_status chd_rings_apply(chd_engine* e, cudaStream_t s, uint32_t n_updates);
 // followers (chd_follow.cu): the listed slots (n == 0 with slot == nullptr: every slot) follow nothing from now on; d_slot: the
 // same list on the device if the caller uploaded it already
 chd_status chd_follow_drop(chd_engine* e, const uint32_t* slot, const uint32_t* d_slot, uint32_t n);

@@ -85,8 +85,8 @@ chd_status chd_assemble_payloads(chd_engine* e, uint32_t* out_n_classes, uint64_
     st = chd_ring_total_flush(e, s);
     if (st != CHD_OK) return st;
     const RingDev ring = chd_ring_view(e);
-    const chd_engine::RingBytes& rb = e->rbytes;
-    const bool dev = e->rings_owned;  // (byte-carrying: rule 14)
+    const chd_engine::Rings::RingBytes& rb = e->rings.bytes;
+    const bool dev = e->rings.owned;  // (byte-carrying: rule 14)
     const PayloadIn in{(const unsigned long long*)P.d_entry_off, P.d_entry_bytes, (const unsigned long long*)P.d_full_off, P.d_full_bytes, P.d_url, P.url_len,
                        P.msg_type, dev ? rb.slab : nullptr, dev ? rb.pos : nullptr, dev ? rb.len : nullptr, rb.per_cell};
     st = chd_epoch_tick(e, s, EP_PAYLOAD);

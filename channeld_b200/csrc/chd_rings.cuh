@@ -210,17 +210,12 @@ __global__ void __launch_bounds__(128)
     }
 }
 
+// chd_get_rings: live lengths (scanned into a CSR by the caller) and the compacted copy
 __global__ void __launch_bounds__(128) ring_len_kernel(uint32_t cells, const uint32_t* __restrict__ begin, const uint32_t* __restrict__ end,
                                                        uint32_t* __restrict__ len) {
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c < cells) len[c] = end[c] - begin[c];
 }
-
-// chd_get_rings: live lengths (scanned into a CSR by the caller) and the compacted copy
-struct RingLenIn {
-    const uint32_t *begin, *end;
-    __device__ __forceinline__ uint64_t operator()(uint64_t c) const { return end[c] - begin[c]; }
-};
 __global__ void __launch_bounds__(128)
     rings_gather_kernel(uint32_t cells, const uint32_t* __restrict__ begin, const uint32_t* __restrict__ end, const uint32_t* __restrict__ out_off,
                         const int64_t* __restrict__ arrival, const uint32_t* __restrict__ sender, const uint64_t* __restrict__ index,

@@ -421,7 +421,7 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
     if (follow && chd_rule_batch_waiting(e, "chd_tick_sharded", true) != CHD_OK) return CHD_ERR_STATE;
     flags &= ~(uint32_t)CHD_TICK_FOLLOW;  // (chd_tick below joins the update this call begins)
     // device rings: the interest update raises the ring limits, so it starts inside this call, after their exchange
-    const bool rings = e->rings_owned;
+    const bool rings = e->rings.owned;
     if (rings && chd_rule_no_chain(e, "chd_tick_sharded with device rings", false) != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_COPY_WAIT | ENTRY_FETCH_GUARD);
     chd_status st;
@@ -469,8 +469,8 @@ chd_status chd_tick_sharded(chd_engine* e, const chd_query_batch* q, int64_t t_n
                                     (uint32_t)e->comm_world);
     }
     if (st != CHD_OK) return st;
-    if (e->rings_staged) {
-        st = chd_rings_apply(e, e->stream, e->staged_updates);
+    if (e->rings.staged) {
+        st = chd_rings_apply(e, e->stream, e->rings.staged_updates);
         if (st != CHD_OK) return st;
     }
     if (e->mig_subs) e->mig = MigView{const_cast<uint32_t*>(gathered) + 2ull * cap, e->rec_stride_words, e->mig_subs, e->mig_pairs};

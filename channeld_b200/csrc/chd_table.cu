@@ -424,11 +424,11 @@ chd_status chd_rule_facing(chd_engine* e, const char* fn) {
 // communicator engine stages its one chd_rings_append per tick for chd_tick_sharded, which appends after the ring-limit import;
 // until then the calls that would append, read or raise around the staged updates are refused.
 chd_status chd_rule_ring_limits(chd_engine* e, const char* fn) {
-    if (!e->rings_owned || !e->slab) return refuse(e, "%s needs device-owned rings (chd_rings_init) on a slab (chd_set_slab / chd_comm_init)", fn);
+    if (!e->rings.owned || !e->slab) return refuse(e, "%s needs device-owned rings (chd_rings_init) on a slab (chd_set_slab / chd_comm_init)", fn);
     return chd_rule_no_chain(e, fn, false);
 }
 chd_status chd_rule_rings_staged(chd_engine* e, const char* fn) {
-    if (!e->rings_staged) return CHD_OK;
+    if (!e->rings.staged) return CHD_OK;
     return refuse(e, "%s: ring updates are staged for the next chd_tick_sharded (one chd_rings_append per tick on a communicator engine)", fn);
 }
 
@@ -452,25 +452,25 @@ chd_status chd_rule_no_chain(chd_engine* e, const char* fn, bool fanout_only) {
 // (CHD_ERR_INVALID).
 chd_status chd_rule_ring_bytes_reserve(chd_engine* e) {
     const char* fn = "chd_rings_reserve_bytes";
-    if (!e->rings_owned) return refuse(e, "%s before chd_rings_init", fn);
-    if (e->rings_appended) return refuse(e, "%s after an append: the reservation comes between chd_rings_init and the first append", fn);
+    if (!e->rings.owned) return refuse(e, "%s before chd_rings_init", fn);
+    if (e->rings.appended) return refuse(e, "%s after an append: the reservation comes between chd_rings_init and the first append", fn);
     return chd_rule_no_chain(e, fn, false);
 }
 chd_status chd_rule_ring_append(chd_engine* e, bool bytes) {
-    if (e->rbytes.on == bytes) return CHD_OK;
+    if (e->rings.bytes.on == bytes) return CHD_OK;
     return bytes ? refuse(e, "chd_rings_append_bytes needs byte-carrying rings (chd_rings_reserve_bytes)")
                  : refuse(e, "chd_rings_append on byte-carrying rings (chd_rings_reserve_bytes): every entry carries its bytes (chd_rings_append_bytes)");
 }
 chd_status chd_rule_assemble_rings(chd_engine* e) {
-    if (!e->rings_owned) return CHD_OK;
-    if (!e->rbytes.on)
+    if (!e->rings.owned) return CHD_OK;
+    if (!e->rings.bytes.on)
         return refuse(e, "chd_assemble_payloads needs host-owned rings (chd_set_rings): payload bytes are indexed by ring position "
                          "(or byte-carrying device rings, chd_rings_reserve_bytes)");
-    if (e->rings_after_fanout) return refuse(e, "chd_assemble_payloads: the rings changed after the last fan-out pass (an append or chd_rings_init)");
+    if (e->rings.after_fanout) return refuse(e, "chd_assemble_payloads: the rings changed after the last fan-out pass (an append or chd_rings_init)");
     return CHD_OK;
 }
 chd_status chd_rule_payload_entries(chd_engine* e, uint32_t n_entries) {
-    if (!n_entries || !e->rings_owned || !e->rbytes.on) return CHD_OK;
+    if (!n_entries || !e->rings.owned || !e->rings.bytes.on) return CHD_OK;
     e->fail("chd_set_payload_bytes: %u entries on byte-carrying rings (chd_rings_reserve_bytes), whose entries carry their bytes: pass 0", n_entries);
     return CHD_ERR_INVALID;
 }

@@ -1,12 +1,9 @@
-// chd_tick.cu — expanded visible lists, update rings, fan-out, and Channel.Tick for every spatial channel as one batched,
-// two-stream tick.
+// chd_tick.cu — expanded visible lists, fan-out, and Channel.Tick for every spatial channel as one batched, two-stream tick.
 #include "chd_engine.h"
 
-#include "chd_gpu_ring_bytes.h"
 #include "chd_emit.cuh"
 #include "chd_fanout.cuh"
 #include "chd_misc.cuh"
-#include "chd_rings.cuh"
 
 extern "C" {
 
@@ -122,337 +119,6 @@ chd_status chd_emit_visible(chd_engine* e) {
     return emit_enqueue(e, e->stream, nullptr, nullptr);
 }
 
-// argument checks of one tick's host-owned rings (chd_set_rings / chd_prefetch_rings)
-static chd_status check_rings(chd_engine* e, const char* fn, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
-                              const uint64_t* index) {
-    if (!e || !ring_off) return CHD_ERR_INVALID;
-    if (e->rings_owned) {
-        e->fail("%s: the rings are device-owned (chd_rings_init): use chd_rings_append", fn);
-        return CHD_ERR_STATE;
-    }
-    if (n_entries > e->lim.max_ring_entries) {
-        e->fail("%u ring entries > max_ring_entries %u", n_entries, e->lim.max_ring_entries);
-        return CHD_ERR_CAPACITY;
-    }
-    if (n_entries && (!arrival || !sender || !index)) return CHD_ERR_INVALID;
-    return CHD_OK;
-}
-
-// copies one tick's host-owned rings into staging arrays on `s` and records their entry count and whether they carry
-// channel_msg_index
-static chd_status copy_rings(chd_engine* e, cudaStream_t s, chd_engine::RStage& r, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival,
-                             const uint32_t* sender, const uint64_t* index, const uint64_t* ch_msg_index) {
-    const uint64_t C = e->g.cells;
-    CU(e, cudaMemcpyAsync(r.off, ring_off, sizeof(uint32_t) * (C + 1), cudaMemcpyDefault, s));
-    if (n_entries) {
-        CU(e, cudaMemcpyAsync(r.arrival, arrival, sizeof(int64_t) * n_entries, cudaMemcpyDefault, s));
-        CU(e, cudaMemcpyAsync(r.sender, sender, sizeof(uint32_t) * n_entries, cudaMemcpyDefault, s));
-        CU(e, cudaMemcpyAsync(r.index, index, sizeof(uint64_t) * n_entries, cudaMemcpyDefault, s));
-    }
-    if (ch_msg_index) CU(e, cudaMemcpyAsync(r.cmi, ch_msg_index, sizeof(uint64_t) * C, cudaMemcpyDefault, s));
-    r.total = n_entries;
-    r.has_cmi = ch_msg_index != nullptr;
-    return CHD_OK;
-}
-
-// staged host-owned rings as the kernels read them: a CSR by cell
-static RingDev staged_ring(const chd_engine* e, const chd_engine::RStage& r) {
-    return RingDev{r.off, r.off + 1, r.arrival, r.sender, r.index, r.has_cmi ? r.cmi : nullptr, e->d_ring_total, nullptr};
-}
-
-chd_status chd_set_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
-                         const uint64_t* index, const uint64_t* ch_msg_index) {
-    chd_status st = check_rings(e, "chd_set_rings", ring_off, n_entries, arrival, sender, index);
-    if (st != CHD_OK) return st;
-    if (chd_rule_no_chain(e, "chd_set_rings", true) != CHD_OK) return CHD_ERR_STATE;
-    CHD_ENTER(e, ENTRY_DEVICE);
-    const uint32_t total = n_entries;
-    const bool in_place = chd_is_device_ptr(e, ring_off) && (!total || (chd_is_device_ptr(e, arrival) && chd_is_device_ptr(e, sender) && chd_is_device_ptr(e, index))) &&
-                          (!ch_msg_index || chd_is_device_ptr(e, ch_msg_index));
-    if (in_place) {  // device-resident rings: consumed in place
-        e->ring = RingDev{ring_off, ring_off + 1, arrival, sender, index, ch_msg_index, e->d_ring_total, nullptr};
-    } else {
-        chd_engine::RStage r{e->d_ring_off, e->d_ring_sender, e->d_ring_arrival, e->d_ring_index, e->d_ch_msg_index, 0, false};
-        st = copy_rings(e, e->stream, r, ring_off, total, arrival, sender, index, ch_msg_index);
-        if (st != CHD_OK) return st;
-        e->ring = staged_ring(e, r);
-    }
-    e->pf_ring.cur = -1;
-    e->pf_ring.wait = false;
-    // the fan-out kernel clamps ring_off to this: a lying caller cannot cause out-of-bounds reads
-    e->ring_total = total;
-    e->ring_total_pending = true;
-    return CHD_OK;
-}
-
-/* ---- device-owned rings: ChannelData.OnUpdate's buffer maintenance on the GPU (data.go:149-173) */
-
-chd_status chd_rings_init(chd_engine* e, uint32_t capacity_per_cell) {
-    if (!e || capacity_per_cell <= RING_MAX_BUFFER) {
-        if (e) e->fail("chd_rings_init: capacity_per_cell must exceed %u (MaxUpdateMsgBufferSize: the reference's buffer may grow beyond it)", RING_MAX_BUFFER);
-        return CHD_ERR_INVALID;
-    }
-    if (chd_rule_no_chain(e, "chd_rings_init", false) != CHD_OK) return CHD_ERR_STATE;
-    const uint64_t need = (uint64_t)e->g.cells * capacity_per_cell;
-    if (need > e->lim.max_ring_entries) {
-        e->fail("chd_rings_init: %u cells x %u entries > max_ring_entries %u", e->g.cells, capacity_per_cell, e->lim.max_ring_entries);
-        return CHD_ERR_CAPACITY;
-    }
-    CHD_ENTER(e, ENTRY_DEVICE);
-    cudaStream_t s = e->stream;
-    rings_init_kernel<<<blocks_for((uint64_t)e->g.cells + 1, 128), 128, 0, s>>>(e->g.cells, capacity_per_cell, e->d_rb_begin, e->d_rb_end);
-    KCHECK(e);
-    CU(e, cudaMemsetAsync(e->d_ch_msg_index, 0, (uint64_t)e->g.cells * 8, s));
-    if (e->rbytes.on) CU(e, cudaMemsetAsync(e->rbytes.cur, 0, 8ull * e->g.cells, s));  // empty byte slabs, the reservation kept
-    set_u32_kernel<<<1, 1, 0, s>>>(e->d_ring_total, (uint32_t)need);
-    KCHECK(e);
-    e->ring_total_pending = false;
-    e->rings_owned = true;
-    e->rings_appended = e->rings_staged;  // (a staged append is still to come: the next chd_tick_sharded applies it to these rings)
-    e->rings_after_fanout = true;
-    e->ring_cap = capacity_per_cell;
-    e->ring = RingDev{e->d_rb_begin, e->d_rb_end, e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, e->d_ch_msg_index, e->d_ring_total, nullptr};
-    e->pf_ring.cur = -1;
-    e->pf_ring.wait = false;
-    e->pf_ring.staged = -1;  // host-owned rings prefetched before this call are not adopted
-    return CHD_OK;
-}
-
-// one append's updates into d_upd_* on the engine stream
-static chd_status rings_upload(chd_engine* e, const uint32_t* upd_off, uint32_t n_updates, const int64_t* arrival_ns, const uint32_t* sender_conn_id) {
-    cudaStream_t s = e->stream;
-    const uint32_t C = e->g.cells;
-    const uint64_t grown = (uint64_t)n_updates + n_updates / 2 + 1024;
-    if (!ensure_cap(e, &e->d_upd_arrival, &e->upd_arrival_cap, n_updates, grown) || !ensure_cap(e, &e->d_upd_sender, &e->upd_sender_cap, n_updates, grown))
-        return CHD_ERR_CUDA;
-    CU(e, cudaMemcpyAsync(e->d_upd_off, upd_off, sizeof(uint32_t) * ((uint64_t)C + 1), cudaMemcpyDefault, s));
-    if (n_updates) {
-        CU(e, cudaMemcpyAsync(e->d_upd_arrival, arrival_ns, sizeof(int64_t) * n_updates, cudaMemcpyDefault, s));
-        CU(e, cudaMemcpyAsync(e->d_upd_sender, sender_conn_id, sizeof(uint32_t) * n_updates, cudaMemcpyDefault, s));
-    }
-    return CHD_OK;
-}
-
-// then staged for chd_tick_sharded (a communicator engine) or applied
-static chd_status rings_stage_or_apply(chd_engine* e, uint32_t n_updates) {
-    e->rings_appended = true;
-    if (e->comm) {  // rule 12: chd_tick_sharded appends them once the other ranks' ring limits are in
-        e->rings_staged = true;
-        e->staged_updates = n_updates;
-        return CHD_OK;
-    }
-    return chd_rings_apply(e, e->stream, n_updates);
-}
-
-chd_status chd_rings_append(chd_engine* e, const uint32_t* upd_off, uint32_t n_updates, const int64_t* arrival_ns, const uint32_t* sender_conn_id) {
-    if (!e || !upd_off || (n_updates && (!arrival_ns || !sender_conn_id))) return CHD_ERR_INVALID;
-    if (!e->rings_owned) {
-        e->fail("chd_rings_append before chd_rings_init");
-        return CHD_ERR_STATE;
-    }
-    if (chd_rule_no_chain(e, "chd_rings_append", false) != CHD_OK || chd_rule_rings_staged(e, "chd_rings_append") != CHD_OK ||
-        chd_rule_ring_append(e, false) != CHD_OK)
-        return CHD_ERR_STATE;
-    CHD_ENTER(e, ENTRY_DEVICE);
-    const chd_status st = rings_upload(e, upd_off, n_updates, arrival_ns, sender_conn_id);
-    return st != CHD_OK ? st : rings_stage_or_apply(e, n_updates);
-}
-
-chd_status chd_rings_apply(chd_engine* e, cudaStream_t s, uint32_t n_updates) {
-    const uint32_t C = e->g.cells;
-    const chd_engine::RingBytes& rb = e->rbytes;
-    if (rb.on) {
-        rings_append_bytes_kernel<<<blocks_for((uint64_t)C * 32, 128), 128, 0, s>>>(
-            C, e->ring_cap, e->d_upd_off, n_updates, e->d_upd_arrival, e->d_upd_sender, rb.upd_boff, rb.upd_bytes, e->d_rb_begin, e->d_rb_end,
-            e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, rb.pos, rb.len, rb.slab, rb.per_cell, rb.cur, e->d_ch_msg_index, e->d_cell_max_interval,
-            &e->d_ctr->overflow);
-    } else {
-        rings_append_kernel<<<blocks_for(C, 128), 128, 0, s>>>(C, e->ring_cap, e->d_upd_off, n_updates, e->d_upd_arrival, e->d_upd_sender, e->d_rb_begin,
-                                                               e->d_rb_end, e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, e->d_ch_msg_index,
-                                                               e->d_cell_max_interval, &e->d_ctr->overflow);
-    }
-    KCHECK(e);
-    e->rings_staged = false;
-    e->rings_after_fanout = true;
-    return CHD_OK;
-}
-
-chd_status chd_get_rings(chd_engine* e, uint32_t* ring_off, int64_t* arrival_ns, uint32_t* sender_conn_id, uint64_t* message_index,
-                         uint64_t* channel_msg_index, uint32_t cap_entries) {
-    if (!e || !ring_off) return CHD_ERR_INVALID;
-    if (!e->rings_owned) {
-        e->fail("chd_get_rings: the rings are host-owned (chd_set_rings)");
-        return CHD_ERR_STATE;
-    }
-    if (chd_rule_rings_staged(e, "chd_get_rings") != CHD_OK) return CHD_ERR_STATE;  // (its length pass reuses d_upd_off)
-    CHD_ENTER(e, ENTRY_COPY_WAIT);
-    cudaStream_t s = e->stream;
-    const uint32_t C = e->g.cells;
-    // (control-plane call: a plain two-pass scan through scratch that is free between ticks)
-    if (!e->d_ring_scan_scratch && !dalloc(e, &e->d_ring_scan_scratch, scan_scratch_elems(C + 1))) return CHD_ERR_CUDA;
-    ring_len_kernel<<<blocks_for(C, 128), 128, 0, s>>>(C, e->d_rb_begin, e->d_rb_end, e->d_upd_off);
-    KCHECK(e);
-    SCAN(e, exclusive_scan<uint32_t, uint32_t>(e->d_upd_off, e->d_ring_flat_off, C, e->d_ring_scan_scratch, s));
-    uint32_t total = 0;
-    chd_status st = chd_read_u32(e, e->d_ring_flat_off + C, &total);
-    if (st != CHD_OK) return st;
-    CU(e, cudaMemcpyAsync(ring_off, e->d_ring_flat_off, sizeof(uint32_t) * ((uint64_t)C + 1), cudaMemcpyDefault, s));
-    if (channel_msg_index) CU(e, cudaMemcpyAsync(channel_msg_index, e->d_ch_msg_index, sizeof(uint64_t) * C, cudaMemcpyDefault, s));
-    if (arrival_ns || sender_conn_id || message_index) {
-        if (total > cap_entries) {
-            e->fail("chd_get_rings: %u entries > cap_entries %u", total, cap_entries);
-            return CHD_ERR_CAPACITY;
-        }
-        int64_t* ta = nullptr;
-        uint32_t* ts = nullptr;
-        uint64_t* ti = nullptr;
-        CU(e, cudaMallocAsync((void**)&ta, 8ull * (total + 1), s));
-        CU(e, cudaMallocAsync((void**)&ts, 4ull * (total + 1), s));
-        CU(e, cudaMallocAsync((void**)&ti, 8ull * (total + 1), s));
-        rings_gather_kernel<<<C, 128, 0, s>>>(C, e->d_rb_begin, e->d_rb_end, e->d_ring_flat_off, e->d_ring_arrival, e->d_ring_sender, e->d_ring_index, ta, ts,
-                                              ti, total);
-        KCHECK(e);
-        if (arrival_ns) CU(e, cudaMemcpyAsync(arrival_ns, ta, 8ull * total, cudaMemcpyDefault, s));
-        if (sender_conn_id) CU(e, cudaMemcpyAsync(sender_conn_id, ts, 4ull * total, cudaMemcpyDefault, s));
-        if (message_index) CU(e, cudaMemcpyAsync(message_index, ti, 8ull * total, cudaMemcpyDefault, s));
-        CU(e, cudaFreeAsync(ta, s));
-        CU(e, cudaFreeAsync(ts, s));
-        CU(e, cudaFreeAsync(ti, s));
-    }
-    CU(e, cudaStreamSynchronize(s));
-    return CHD_OK;
-}
-
-/* ---- byte-carrying device rings (include/chd_gpu_ring_bytes.h): each update's serialized updateMsg kept in the ring beside
-   its entry (rings_append_bytes_kernel), read in place by the payload kernels (chd_payload.cuh) */
-
-chd_status chd_rings_reserve_bytes(chd_engine* e, uint32_t bytes_per_cell) {
-    if (!e) return CHD_ERR_INVALID;
-    if (bytes_per_cell == 0) {
-        e->fail("chd_rings_reserve_bytes: bytes_per_cell must be positive");
-        return CHD_ERR_INVALID;
-    }
-    // (rule 12 too: staged updates were checked against the slab they were staged for, and their bytes would be applied to this one)
-    if (chd_rule_ring_bytes_reserve(e) != CHD_OK || chd_rule_rings_staged(e, "chd_rings_reserve_bytes") != CHD_OK) return CHD_ERR_STATE;
-    CHD_ENTER(e, ENTRY_DEVICE);
-    chd_engine::RingBytes& rb = e->rbytes;
-    const uint64_t C = e->g.cells;
-    // a failed allocation changes nothing: the per-slot arrays are kept once made, and a new slab replaces the old one only once it exists
-    const bool slots = (rb.pos || dalloc(e, &rb.pos, (uint64_t)e->lim.max_ring_entries)) && (rb.len || dalloc(e, &rb.len, (uint64_t)e->lim.max_ring_entries)) &&
-                       (rb.cur || dalloc(e, &rb.cur, 2 * C));
-    if (!slots) {
-        cudaGetLastError();  // (an allocation failure is not sticky: clear it for the next launch check)
-        return CHD_ERR_CUDA;
-    }
-    if (!rb.slab || rb.per_cell != bytes_per_cell) {
-        uint8_t* slab = nullptr;
-        if (!dalloc(e, &slab, C * bytes_per_cell)) {
-            cudaGetLastError();
-            e->fail("chd_rings_reserve_bytes: %llu cells x %u bytes cannot be allocated", (unsigned long long)C, bytes_per_cell);
-            return CHD_ERR_CAPACITY;
-        }
-        chd_dfree(e, rb.slab);
-        rb.slab = slab;
-    }
-    CU(e, cudaMemsetAsync(rb.cur, 0, 8 * C, e->stream));
-    rb.per_cell = bytes_per_cell;
-    rb.on = true;
-    return CHD_OK;
-}
-
-chd_status chd_rings_append_bytes(chd_engine* e, const uint32_t* upd_off, uint32_t n_updates, const int64_t* arrival_ns, const uint32_t* sender_conn_id,
-                                  const uint64_t* byte_off, const uint8_t* bytes) {
-    if (!e || !upd_off || !byte_off || (n_updates && (!arrival_ns || !sender_conn_id))) return CHD_ERR_INVALID;
-    if (!e->rings_owned) {
-        e->fail("chd_rings_append_bytes before chd_rings_init");
-        return CHD_ERR_STATE;
-    }
-    if (chd_rule_no_chain(e, "chd_rings_append_bytes", false) != CHD_OK || chd_rule_rings_staged(e, "chd_rings_append_bytes") != CHD_OK ||
-        chd_rule_ring_append(e, true) != CHD_OK)
-        return CHD_ERR_STATE;
-    // byte_off is a host array: its lengths are checked here, before anything is appended
-    for (uint32_t k = 0; k < n_updates; k++) {
-        if (byte_off[k + 1] < byte_off[k] || byte_off[k + 1] - byte_off[k] > e->rbytes.per_cell) {
-            e->fail("chd_rings_append_bytes: update %u has byte offsets %llu .. %llu (bytes_per_cell %u)", k, (unsigned long long)byte_off[k],
-                    (unsigned long long)byte_off[k + 1], e->rbytes.per_cell);
-            return CHD_ERR_INVALID;
-        }
-    }
-    const uint64_t nb = byte_off[n_updates];
-    if (nb && !bytes) {
-        e->fail("chd_rings_append_bytes: %llu bytes and no byte array", (unsigned long long)nb);
-        return CHD_ERR_INVALID;
-    }
-    CHD_ENTER(e, ENTRY_DEVICE);
-    chd_engine::RingBytes& rb = e->rbytes;
-    cudaStream_t s = e->stream;
-    if (!ensure_cap(e, &rb.upd_boff, &rb.upd_boff_cap, (uint64_t)n_updates + 1, (uint64_t)n_updates + n_updates / 2 + 1025) ||
-        !ensure_cap(e, &rb.upd_bytes, &rb.upd_bytes_cap, nb + 1, nb + nb / 2 + 4096))
-        return CHD_ERR_CUDA;
-    chd_status st = rings_upload(e, upd_off, n_updates, arrival_ns, sender_conn_id);
-    if (st != CHD_OK) return st;
-    CU(e, cudaMemcpyAsync(rb.upd_boff, byte_off, 8 * ((uint64_t)n_updates + 1), cudaMemcpyHostToDevice, s));
-    if (nb) CU(e, cudaMemcpyAsync(rb.upd_bytes, bytes, nb, cudaMemcpyDefault, s));
-    return rings_stage_or_apply(e, n_updates);
-}
-
-chd_status chd_get_ring_bytes(chd_engine* e, uint64_t* byte_off, uint8_t* bytes, uint64_t cap_bytes, uint64_t* total) {
-    if (!e) return CHD_ERR_INVALID;
-    if (!e->rings_owned || !e->rbytes.on) {
-        e->fail("chd_get_ring_bytes needs byte-carrying device rings (chd_rings_reserve_bytes)");
-        return CHD_ERR_STATE;
-    }
-    if (chd_rule_rings_staged(e, "chd_get_ring_bytes") != CHD_OK) return CHD_ERR_STATE;  // (its length pass reuses d_upd_off)
-    CHD_ENTER(e, ENTRY_COPY_WAIT);
-    const chd_engine::RingBytes& rb = e->rbytes;
-    cudaStream_t s = e->stream;
-    const uint32_t C = e->g.cells;
-    if (total) *total = 0;
-    // (control-plane call: the entry CSR as chd_get_rings makes it, the cells' byte offsets through temporaries)
-    if (!e->d_ring_scan_scratch && !dalloc(e, &e->d_ring_scan_scratch, scan_scratch_elems(C + 1))) return CHD_ERR_CUDA;
-    ring_len_kernel<<<blocks_for(C, 128), 128, 0, s>>>(C, e->d_rb_begin, e->d_rb_end, e->d_upd_off);
-    KCHECK(e);
-    SCAN(e, exclusive_scan<uint32_t, uint32_t>(e->d_upd_off, e->d_ring_flat_off, C, e->d_ring_scan_scratch, s));
-    uint32_t* blen = nullptr;
-    unsigned long long *cell_boff = nullptr, *scratch = nullptr;
-    CU(e, cudaMallocAsync((void**)&blen, 4ull * C + 4, s));
-    CU(e, cudaMallocAsync((void**)&cell_boff, 8ull * (C + 2), s));
-    CU(e, cudaMallocAsync((void**)&scratch, 8ull * scan_scratch_elems(C + 1), s));
-    ring_bytes_len_kernel<<<blocks_for(C, 128), 128, 0, s>>>(C, rb.cur, blen);
-    KCHECK(e);
-    SCAN(e, exclusive_scan<uint32_t, unsigned long long>(blen, cell_boff, C, scratch, s));
-    uint64_t* h64 = (uint64_t*)e->h_u32;
-    CU(e, cudaMemcpyAsync(h64, cell_boff + C, 8, cudaMemcpyDeviceToHost, s));
-    CU(e, cudaMemcpyAsync(h64 + 1, e->d_ring_flat_off + C, 4, cudaMemcpyDeviceToHost, s));
-    CU(e, cudaStreamSynchronize(s));
-    const uint64_t nb = h64[0];
-    const uint32_t n_live = (uint32_t)h64[1];
-    if (total) *total = nb;
-    chd_status st = CHD_OK;
-    if (bytes && nb > cap_bytes) {
-        e->fail("chd_get_ring_bytes: %llu bytes > cap_bytes %llu", (unsigned long long)nb, (unsigned long long)cap_bytes);
-        st = CHD_ERR_CAPACITY;
-    } else if (byte_off || bytes) {
-        unsigned long long* o_boff = nullptr;
-        uint8_t* o_bytes = nullptr;
-        CU(e, cudaMallocAsync((void**)&o_boff, 8ull * (n_live + 1), s));
-        CU(e, cudaMallocAsync((void**)&o_bytes, nb + 1, s));
-        ring_bytes_gather_kernel<<<C, 128, 0, s>>>(C, e->d_rb_begin, e->d_rb_end, e->d_ring_flat_off, rb.pos, rb.cur, cell_boff, rb.slab, rb.per_cell,
-                                                    o_boff, o_bytes);
-        KCHECK(e);
-        CU(e, cudaMemcpyAsync(o_boff + n_live, cell_boff + C, 8, cudaMemcpyDeviceToDevice, s));
-        if (byte_off) CU(e, cudaMemcpyAsync(byte_off, o_boff, 8ull * (n_live + 1), cudaMemcpyDefault, s));
-        if (bytes && nb) CU(e, cudaMemcpyAsync(bytes, o_bytes, nb, cudaMemcpyDefault, s));
-        CU(e, cudaFreeAsync(o_boff, s));
-        CU(e, cudaFreeAsync(o_bytes, s));
-    }
-    CU(e, cudaFreeAsync(blen, s));
-    CU(e, cudaFreeAsync(cell_boff, s));
-    CU(e, cudaFreeAsync(scratch, s));
-    CU(e, cudaStreamSynchronize(s));
-    return st;
-}
-
 chd_status chd_set_channel_start_times(chd_engine* e, const int64_t* start_ns) {
     if (!e) return CHD_ERR_INVALID;
     if (chd_rule_no_chain(e, "chd_set_channel_start_times", false) != CHD_OK) return CHD_ERR_STATE;
@@ -467,30 +133,16 @@ chd_status chd_set_channel_start_times(chd_engine* e, const int64_t* start_ns) {
     return CHD_OK;
 }
 
-chd_status chd_ring_total_flush(chd_engine* e, cudaStream_t s) {
-    if (!e->ring_total_pending) return CHD_OK;
-    set_u32_kernel<<<1, 1, 0, s>>>(e->d_ring_total, e->ring_total);
-    KCHECK(e);
-    e->ring_total_pending = false;
-    return CHD_OK;
-}
-
-RingDev chd_ring_view(const chd_engine* e) {
-    RingDev ring = e->ring;
-    ring.start = e->have_cell_start ? e->d_cell_start_ns : nullptr;
-    return ring;
-}
-
 static chd_status fanout_enqueue(chd_engine* e, cudaStream_t s, int64_t t_ns) {
     PairBuf& pb = e->pairs[e->cur];
     const uint32_t S = e->n_slots;
     const uint64_t P = e->lim.max_pairs;
     StageTimer timer(e, s, CHD_STAGE_FANOUT);
-    chd_status st = chd_pf_wait(e, e->pf_ring, s);  // rings handed over by chd_adopt_prefetched: ordered after their upload
+    chd_status st = chd_pf_wait(e, e->rings.pf, s);  // rings handed over by chd_adopt_prefetched: ordered after their upload
     if (st == CHD_OK) st = chd_ring_total_flush(e, s);
     if (st != CHD_OK) return st;
     chd_epoch_tick(e, s, EP_FANOUT);
-    e->rings_after_fanout = false;
+    e->rings.after_fanout = false;
     stage_begin_kernel<<<1, 1, 0, s>>>(e->d_time + 1, t_ns, e->d_epoch + EP_FANOUT, &e->d_ctr->n_due, 1, nullptr);
     KCHECK(e);
     const RingDev ring = chd_ring_view(e);
@@ -505,7 +157,7 @@ static chd_status fanout_enqueue(chd_engine* e, cudaStream_t s, int64_t t_ns) {
         KCHECK(e);
         return CHD_OK;
     });
-    return st != CHD_OK ? st : chd_pf_note_read(e, e->pf_ring, e->pf_ring.cur, s);
+    return st != CHD_OK ? st : chd_pf_note_read(e, e->rings.pf, e->rings.pf.cur, s);
 }
 
 chd_status chd_fanout_tick(chd_engine* e, int64_t t_ns) {
@@ -514,37 +166,16 @@ chd_status chd_fanout_tick(chd_engine* e, int64_t t_ns) {
     return fanout_enqueue(e, e->stream, t_ns);
 }
 
-chd_status chd_prefetch_rings(chd_engine* e, const uint32_t* ring_off, uint32_t n_entries, const int64_t* arrival, const uint32_t* sender,
-                              const uint64_t* index, const uint64_t* ch_msg_index) {
-    chd_status st = check_rings(e, "chd_prefetch_rings", ring_off, n_entries, arrival, sender, index);
-    if (st != CHD_OK) return st;
-    CHD_ENTER(e, ENTRY_DEVICE);
-    int set = 0;
-    st = chd_pf_begin(e, e->pf_ring, &set);
-    if (st != CHD_OK) return st;
-    chd_engine::RStage& r = e->ring_pf[set];
-    const uint64_t C = e->g.cells, R = e->lim.max_ring_entries;
-    if (!r.cmi && !(dalloc(e, &r.off, C + 1) && dalloc(e, &r.arrival, R) && dalloc(e, &r.sender, R) && dalloc(e, &r.index, R) && dalloc(e, &r.cmi, C)))
-        return CHD_ERR_CUDA;  // (cmi is allocated last)
-    st = copy_rings(e, e->up_stream, r, ring_off, n_entries, arrival, sender, index, ch_msg_index);
-    return st != CHD_OK ? st : chd_pf_end(e, e->pf_ring);
-}
-
 chd_status chd_adopt_prefetched(chd_engine* e) {
     if (!e) return CHD_ERR_INVALID;
-    if (e->pf_pos.staged < 0 && e->pf_q.staged < 0 && e->pf_ring.staged < 0) {
+    if (e->pf_pos.staged < 0 && e->pf_q.staged < 0 && e->rings.pf.staged < 0) {
         e->fail("chd_adopt_prefetched without a preceding chd_prefetch_entities / chd_prefetch_queries / chd_prefetch_rings");
         return CHD_ERR_STATE;
     }
     if (e->pf_q.staged >= 0 && chd_rule_no_generated_batch(e, "chd_adopt_prefetched of a query batch") != CHD_OK) return CHD_ERR_STATE;
     CHD_ENTER(e, ENTRY_DEVICE);
     chd_pf_adopt(e->pf_q);  // consumed by the next chd_begin_interest / chd_update_interest called with q == NULL
-    if (chd_pf_adopt(e->pf_ring)) {
-        const chd_engine::RStage& r = e->ring_pf[e->pf_ring.cur];
-        e->ring = staged_ring(e, r);
-        e->ring_total = r.total;
-        e->ring_total_pending = true;
-    }
+    chd_rings_adopt(e);
     if (!chd_pf_adopt(e->pf_pos)) return CHD_OK;
     chd_status st = chd_pf_wait(e, e->pf_pos, e->stream);
     if (st != CHD_OK) return st;

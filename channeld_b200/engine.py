@@ -255,6 +255,34 @@ class Engine:
     def set_rings(self, ring_off, arrival, sender, index, channel_msg_index=None):
         self._upload_rings(self.L.chd_set_rings, "_keep_ring", ring_off, arrival, sender, index, channel_msg_index)
 
+    # ---- device-owned rings (ChannelData.OnUpdate's buffer maintenance on the device)
+    def rings_init(self, capacity_per_cell):
+        self._ck(self.L.chd_rings_init(self.h, int(capacity_per_cell)))
+
+    def rings_append(self, upd_off, arrival, sender, n=None):
+        """Appends updates given as a CSR by cell (upd_off: C + 1 offsets).  n: the update count, upd_off[-1] by default; the
+        device reads no update at or past n, whatever upd_off says."""
+        upd_off = np.ascontiguousarray(upd_off, np.uint32)
+        arrival = np.ascontiguousarray(arrival, np.int64)
+        sender = np.ascontiguousarray(sender, np.uint32)
+        n = int(upd_off[-1]) if n is None else int(n)
+        self._ck(self.L.chd_rings_append(self.h, ptr(upd_off), n, ptr(arrival) if n else None, ptr(sender) if n else None))
+
+    def _ring_off(self):
+        """the live entries' CSR by cell (C + 1 offsets)"""
+        off = np.zeros(self.n_cells + 1, np.uint32)
+        self._ck(self.L.chd_get_rings(self.h, ptr(off), None, None, None, None, 0))
+        return off
+
+    def get_rings(self):
+        """-> dict(off, arrival, sender, index, msg_index): every live entry in ring order, CSR by cell, and each channel's msgIndex"""
+        off = self._ring_off()
+        n = int(off[-1])
+        arr, snd, idx = np.zeros(n + 1, np.int64), np.zeros(n + 1, np.uint32), np.zeros(n + 1, np.uint64)
+        cmi = np.zeros(self.n_cells, np.uint64)
+        self._ck(self.L.chd_get_rings(self.h, ptr(off), ptr(arr), ptr(snd), ptr(idx), ptr(cmi), n))
+        return dict(off=off, arrival=arr[:n], sender=snd[:n], index=idx[:n], msg_index=cmi)
+
     def fanout_tick(self, t_ns):
         self._ck(self.L.chd_fanout_tick(self.h, int(t_ns)))
 
@@ -703,9 +731,8 @@ class Engine:
                                                ptr(data) if len(data) else None))
 
     def get_ring_bytes(self):
-        """-> (byte_off u64 [n_live + 1], data u8): every live ring entry's bytes, in the entry order of chd_get_rings"""
-        off = np.zeros(self.n_cells + 1, np.uint32)
-        self._ck(self.L.chd_get_rings(self.h, ptr(off), None, None, None, None, 0))
+        """-> (byte_off u64 [n_live + 1], data u8): every live ring entry's bytes, in the entry order of get_rings"""
+        off = self._ring_off()
         total = C.c_uint64()
         self._ck(self.L.chd_get_ring_bytes(self.h, None, None, 0, C.byref(total)))
         byte_off, data = np.zeros(int(off[-1]) + 1, np.uint64), np.zeros(total.value + 1, np.uint8)

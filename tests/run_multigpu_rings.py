@@ -19,25 +19,14 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from channeld_b200 import capi, engine, sharding  # noqa: E402
-from tests.test_gpu_rings_scale import _append  # noqa: E402
 from tests.test_gpu_sharded_rings import COLS, DEFAULT_IV, HALO, ROWS, W, RingWorld, _served  # noqa: E402
 
 
-class _NS:
-    capi = capi
-
-
-def rings_of(e):
-    """chd_get_rings -> per cell (arrival, sender, index) and the msgIndex array"""
-    cells = e.n_cells
-    off = np.zeros(cells + 1, np.uint32)
-    p = capi.ptr
-    e._ck(e.L.chd_get_rings(e.h, p(off), None, None, None, None, 0))
-    n = int(off[-1])
-    arr, snd, idx, cmi = np.zeros(n + 1, np.int64), np.zeros(n + 1, np.uint32), np.zeros(n + 1, np.uint64), np.zeros(cells, np.uint64)
-    e._ck(e.L.chd_get_rings(e.h, p(off), p(arr), p(snd), p(idx), p(cmi), n))
-    o = off.astype(np.int64)
-    return {c: (arr[o[c]:o[c + 1]].tolist(), snd[o[c]:o[c + 1]].tolist(), idx[o[c]:o[c + 1]].tolist(), int(cmi[c])) for c in range(cells)}
+def ring_cells(r):
+    """get_rings() -> per cell (arrival, sender, index) and the msgIndex"""
+    o = r["off"].astype(np.int64)
+    return {c: (r["arrival"][o[c]:o[c + 1]].tolist(), r["sender"][o[c]:o[c + 1]].tolist(), r["index"][o[c]:o[c + 1]].tolist(), int(r["msg_index"][c]))
+            for c in range(len(o) - 1)}
 
 
 def due_of(e, n_due, conn):
@@ -70,33 +59,33 @@ def run(rank, world, local, collective):
     if collective:
         e.use_collective(True)
     e.set_subscribers(my_conn)
-    assert e.L.chd_rings_init(e.h, 620) == capi.OK
+    e.rings_init(620)
     conn_all = np.concatenate(rw.conn)
     whole = None
     if rank == 0:
         whole = engine.Engine(cfg, n_ent, len(conn_all), device=local, default_fanout_interval_ms=DEFAULT_IV)
         whole.set_subscribers(conn_all)
         whole.set_entities(x, z)
-        assert whole.L.chd_rings_init(whole.h, 620) == capi.OK
+        whole.rings_init(620)
     bad = 0
     for tick, t in enumerate(rw.times()):
         upd = rw.updates(tick, t)  # (same seed on every rank: the same whole-grid batch)
         e.set_entities(x[mine], z[mine])
         e.set_entity_ids(mine.astype(np.uint32))
-        assert _append(_NS, e, *upd) == capi.OK
+        e.rings_append(*upd)
         b, keep = engine.make_batch(len(my_conn), sub=np.arange(len(my_conn), dtype=np.uint32),
                                     sphere=tuple(a.copy() for a in rw.queries(hosted, tick)))
         s = e.tick_sharded(b, t, capi.TICK_ALL)
         assert s.overflow == 0
-        mine_out = (rings_of(e), due_of(e, s.n_due, my_conn), pairs_of(e, my_conn))
+        mine_out = (ring_cells(e.get_rings()), due_of(e, s.n_due, my_conn), pairs_of(e, my_conn))
         got = [None] * world
         dist.all_gather_object(got, mine_out)
         if rank == 0:
-            assert _append(_NS, whole, *upd) == capi.OK
+            whole.rings_append(*upd)
             wb, wkeep = engine.make_batch(len(conn_all), sub=np.arange(len(conn_all), dtype=np.uint32),
                                           sphere=tuple(a.copy() for a in rw.queries(range(split), tick)))
             sw = whole.tick(wb, t, capi.TICK_ALL)
-            W_r, W_d, W_p = rings_of(whole), due_of(whole, sw.n_due, conn_all), pairs_of(whole, conn_all)
+            W_r, W_d, W_p = ring_cells(whole.get_rings()), due_of(whole, sw.n_due, conn_all), pairs_of(whole, conn_all)
             for r in range(world):
                 g_r, g_d, g_p = got[r]
                 rl, rh = sharding.slab_columns(COLS, world, r)

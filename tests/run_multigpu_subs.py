@@ -21,8 +21,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from channeld_b200 import capi, engine, sharding  # noqa: E402
-from tests.run_multigpu_rings import rings_of  # noqa: E402
-from tests.test_gpu_rings_scale import _append  # noqa: E402
+from tests.run_multigpu_rings import ring_cells  # noqa: E402
 from tests.test_gpu_sharded_subs import (COLS, DEFAULT_IV, HALO, MS, N_ENT, RING_CAP, ROWS, SERVER, W, SubWorld, _dues, _pairs,  # noqa: E402
                                          _random_ops, _served_cols)
 
@@ -55,14 +54,14 @@ def run(rank, world, local, collective):
     if collective:
         e.use_collective(True)
     e.set_subscribers(sw.conn_of_slot[rank])
-    assert e.L.chd_rings_init(e.h, RING_CAP) == capi.OK
+    e.rings_init(RING_CAP)
     mine = np.nonzero(sw.ent_owner == rank)[0]
     whole = None
     if rank == 0:
         whole = engine.Engine(cfg, N_ENT, len(sw.whole_conns), device=local, default_fanout_interval_ms=DEFAULT_IV)
         whole.set_subscribers(sw.whole_conns)
         whole.set_entities(sw.x, sw.z)
-        assert whole.L.chd_rings_init(whole.h, RING_CAP) == capi.OK
+        whole.rings_init(RING_CAP)
     # the migrants: the first querying connection of each rank moves to the next rank (its centre with it)
     migrants = [next(c for c in sw.regular if sw.table.owner[c] == r and sw.queries[c]) for r in range(world)] if world > 1 else []
     bad = moved = 0
@@ -75,7 +74,7 @@ def run(rank, world, local, collective):
         st = e.apply_subscriptions_sharded(slots, _NS.S0 + cell[idx], op[idx], interval=iv[idx], delay=dl[idx], skip_self=ss[idx],
                                            skip_first=sf[idx], now_ns=t - 7 * MS, present=present[idx])
         upd = sw.updates(tick, t)
-        assert _append(_NS, e, *upd) == capi.OK
+        e.rings_append(*upd)
         if tick == MIGRATE_AT and migrants:
             new_owner = {}
             for r, c in enumerate(migrants):
@@ -100,14 +99,14 @@ def run(rank, world, local, collective):
         s = e.tick_sharded(b, t, capi.TICK_ALL)
         assert s.overflow == 0
         got = [None] * world
-        dist.all_gather_object(got, (idx.tolist(), st.tolist(), rings_of(e), _dues(e, s.n_due, conn_of_slot), _pairs(e, conn_of_slot)))
+        dist.all_gather_object(got, (idx.tolist(), st.tolist(), ring_cells(e.get_rings()), _dues(e, s.n_due, conn_of_slot), _pairs(e, conn_of_slot)))
         if tick == MIGRATE_AT and migrants:
             sw.table.release(rank, vacated[rank])  # (the vacated slots are free from the next tick on)
         if rank != 0:
             continue
         want = whole.apply_subscriptions([sw.whole_slot[k[1] if isinstance(k, tuple) else k] for k in keys], _NS.S0 + cell, op, interval=iv,
                                          delay=dl, skip_self=ss, skip_first=sf, now_ns=t - 7 * MS, present=present)
-        assert _append(_NS, whole, *upd) == capi.OK
+        whole.rings_append(*upd)
         wq = [c for c in sw.regular if sw.queries[c]]
         wb, wkeep = engine.make_batch(len(wq), sub=np.array([sw.whole_slot[c] for c in wq], np.uint32),
                                       sphere=(np.array([sw.cx[c] for c in wq]), np.array([sw.cz[c] for c in wq]), np.full(len(wq), 150.0)))
@@ -118,7 +117,7 @@ def run(rank, world, local, collective):
             statuses[np.array(got[r][0], np.int64)] = got[r][1]
             pairs += got[r][4]
             dues += got[r][3]
-            W_r = rings_of(whole)
+            W_r = ring_cells(whole.get_rings())
             for c in np.nonzero(np.isin(np.arange(COLS * ROWS) % COLS, _served_cols(*sharding.slab_columns(COLS, world, r))))[0]:
                 if got[r][2][c] != W_r[c]:
                     print("tick %d rank %d cell %d: ring differs" % (tick, r, c))

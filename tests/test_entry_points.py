@@ -42,17 +42,18 @@ NEEDS = {
     "chd_update_interest": "COPY_WAIT|FETCH_GUARD",
     # chd_tick.cu
     "chd_emit_visible": "COPY_WAIT|FETCH_GUARD",
-    "chd_set_rings": "DEVICE",
-    "chd_rings_init": "DEVICE",
-    "chd_rings_append": "DEVICE",
-    "chd_get_rings": "COPY_WAIT",
     "chd_set_channel_start_times": "DEVICE",
     "chd_fanout_tick": "COPY_WAIT|FETCH_GUARD",
-    "chd_prefetch_rings": "DEVICE",
     "chd_adopt_prefetched": "DEVICE",
     "chd_summary": "COPY_WAIT",
     "chd_begin_interest": "FETCH_GUARD",
     "chd_tick": "FETCH_GUARD",
+    # chd_rings.cu
+    "chd_set_rings": "DEVICE",
+    "chd_prefetch_rings": "DEVICE",
+    "chd_rings_init": "DEVICE",
+    "chd_rings_append": "DEVICE",
+    "chd_get_rings": "COPY_WAIT",
     # chd_results.cu
     "chd_get_cells": "COPY_WAIT",
     "chd_get_pairs": "COPY_WAIT",

@@ -9,6 +9,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from tests.test_gpu_rings_scale import _status
+
 pytestmark = pytest.mark.gpu
 
 OK, INVALID, STATE = 0, 1, 4  # capi.OK, capi.ERR_INVALID, capi.ERR_STATE
@@ -277,17 +279,6 @@ SETUPS = _setups()
 
 
 # ---------------------------------------------------------------------------------------------------------------- gated calls
-def _status(f):
-    """an Engine method's status (it raises ChdError on anything but OK)"""
-    from channeld_b200.capi import ChdError
-
-    try:
-        f()
-    except ChdError as ex:
-        return ex.status
-    return OK
-
-
 def _calls():
     def p(a):
         from channeld_b200.capi import ptr

@@ -62,32 +62,15 @@ def chd():
     return ns
 
 
-# ---- the C entry points of device-owned rings
+def _status(f):
+    """an Engine method's status (it raises ChdError on anything but OK)"""
+    from channeld_b200.capi import OK, ChdError
 
-def _rings_init(chd, e, cap):
-    return e.L.chd_rings_init(e.h, int(cap))
-
-
-def _append(chd, e, upd_off, arrival, sender, n=None):
-    upd_off = np.ascontiguousarray(upd_off, np.uint32)
-    arrival = np.ascontiguousarray(arrival, np.int64)
-    sender = np.ascontiguousarray(sender, np.uint32)
-    n = int(upd_off[-1]) if n is None else int(n)
-    p = chd.capi.ptr
-    return e.L.chd_rings_append(e.h, p(upd_off), n, p(arrival) if n else None, p(sender) if n else None)
-
-
-def _get_rings(chd, e):
-    """-> dict(off, arrival, sender, index, msg_index) as the oracle's get_rings"""
-    p = chd.capi.ptr
-    cells = e.n_cells
-    off = np.zeros(cells + 1, np.uint32)
-    e._ck(e.L.chd_get_rings(e.h, p(off), None, None, None, None, 0))
-    n = int(off[-1])
-    arr, snd, idx = np.zeros(n + 1, np.int64), np.zeros(n + 1, np.uint32), np.zeros(n + 1, np.uint64)
-    cmi = np.zeros(cells, np.uint64)
-    e._ck(e.L.chd_get_rings(e.h, p(off), p(arr), p(snd), p(idx), p(cmi), n))
-    return dict(off=off, arrival=arr[:n], sender=snd[:n], index=idx[:n], msg_index=cmi)
+    try:
+        f()
+    except ChdError as ex:
+        return ex.status
+    return OK
 
 
 def _assert_rings(got, want, skip=()):
@@ -361,7 +344,7 @@ def _engine(chd, w, cap, graphs=True, n_ent=1, **lim):
     if w.start is not None:
         start = np.ascontiguousarray(w.start)
         assert e.L.chd_set_channel_start_times(e.h, chd.capi.ptr(start)) == chd.capi.OK
-    assert _rings_init(chd, e, cap) == chd.capi.OK, e.L.chd_last_error(e.h)
+    e.rings_init(cap)
     return e
 
 
@@ -387,8 +370,8 @@ def test_rings_scale_parity(chd, oracle, grid, cap, starts):
         s = e.summary()
         r = ref.tick(tick, t, want)
         assert s.n_pairs == r["P"] and s.overflow == 0
-        e._ck(_append(chd, e, r["upd_off"], r["u_arr"], r["u_snd"]))
-        _assert_rings(_get_rings(chd, e), r["rings"])
+        e.rings_append(r["upd_off"], r["u_arr"], r["u_snd"])
+        _assert_rings(e.get_rings(), r["rings"])
         e.fanout_tick(t)
         s = e.summary()
         assert s.overflow == 0 and s.n_due == len(r["due"])
@@ -430,12 +413,12 @@ def test_rings_under_the_two_stream_tick(chd, oracle, graphs):
     e = _engine(chd, w, cap, graphs=graphs, n_ent=2000, max_visible=1 << 24)
     ref_final = None
     for tick, (t, q, r) in enumerate(script):
-        e._ck(_append(chd, e, r["upd_off"], r["u_arr"], r["u_snd"]))
+        e.rings_append(r["upd_off"], r["u_arr"], r["u_snd"])
         batch, keep = chd.engine.make_batch(w.S, sub=None, sphere=q)
         s = e.tick(batch, t, chd.capi.TICK_ALL)
         assert s.overflow == 0 and s.n_pairs == r["P"] and s.n_due == len(r["due"])
         np.testing.assert_array_equal(_due_from(w.conn, e.get_due(s.n_due)), r["due"])
-        _assert_rings(_get_rings(chd, e), r["rings"])
+        _assert_rings(e.get_rings(), r["rings"])
         ref_final = r
     ref.check_pairs(e, ref_final)
     assert (ref.slabs.evictions > 0).sum() >= 10 and ref.slabs.slides.sum() > 0
@@ -470,7 +453,7 @@ def test_rings_in_the_pipelined_loop(chd, oracle):
         np.testing.assert_array_equal(_due_from(w.conn, got), r["due"], err_msg=str(i))
 
     for i, (t, q, r) in enumerate(script):
-        e._ck(_append(chd, e, r["upd_off"], r["u_arr"], r["u_snd"]))
+        e.rings_append(r["upd_off"], r["u_arr"], r["u_snd"])
         batch, kb = chd.engine.make_batch(w.S, sub=None, sphere=q)
         keep.append((batch, kb))
         e.tick(batch, t, chd.capi.TICK_ALL, want_summary=False)
@@ -482,7 +465,7 @@ def test_rings_in_the_pipelined_loop(chd, oracle):
     e._ck(e.L.chd_fetch_wait(e.h, C.byref(s)))
     check(len(script) - 1)
     ref.check_pairs(e, script[-1][2])
-    _assert_rings(_get_rings(chd, e), script[-1][2]["rings"])
+    _assert_rings(e.get_rings(), script[-1][2]["rings"])
     e.close()
 
 
@@ -532,12 +515,12 @@ def test_full_slab_drops_its_oldest_entry(chd, oracle):
     u_arr = np.where(u_cell == X, t, t - rng.integers(0, 100 * MS, len(u_cell))).astype(np.int64)
     u_snd = np.full(len(u_cell), 7, np.uint32)
     ref.chans.on_update(u_cell.astype(np.uint32), u_arr, u_snd)
-    e._ck(_append(chd, e, _csr(n_cell), u_arr, u_snd))
+    e.rings_append(_csr(n_cell), u_arr, u_snd)
     e.fanout_tick(t)
     s = capi.TickSummary()
     assert e.L.chd_summary(e.h, C.byref(s)) == capi.ERR_CAPACITY
     assert s.overflow == capi.OVF_RING
-    got, want = _get_rings(chd, e), ref.chans.get_rings()
+    got, want = e.get_rings(), ref.chans.get_rings()
     _assert_rings(got, want, skip=[X])
     g0, w0 = int(got["off"][X]), int(want["off"][X])
     assert int(got["off"][X + 1]) - g0 == cap and int(want["off"][X + 1]) - w0 == 600
@@ -556,10 +539,10 @@ def test_full_slab_drops_its_oldest_entry(chd, oracle):
     u_arr = (t - rng.integers(0, 100 * MS, len(u_cell))).astype(np.int64)
     u_snd = np.full(len(u_cell), 7, np.uint32)
     ref.chans.on_update(u_cell.astype(np.uint32), u_arr, u_snd)
-    e._ck(_append(chd, e, _csr(n_cell), u_arr, u_snd))
+    e.rings_append(_csr(n_cell), u_arr, u_snd)
     e.fanout_tick(t)
     assert e.L.chd_summary(e.h, C.byref(s)) == capi.OK and s.overflow == 0
-    _assert_rings(_get_rings(chd, e), ref.chans.get_rings(), skip=[X])
+    _assert_rings(e.get_rings(), ref.chans.get_rings(), skip=[X])
     due = _due_from(w.conn, e.get_due(s.n_due))
     np.testing.assert_array_equal(due[due["channel"] != S0 + X], _due_by_cell(ref, t, skip=[X]))
     e.close()
@@ -574,16 +557,16 @@ def test_ring_argument_edges(chd, oracle):
     w = _World(oracle, "b", 12, n_sub=2000, n_hot=0)
     C_ = w.C
     e = chd.engine.Engine(chd.engine.grid_cfg(*w.g), 16, w.S, max_ring_entries=C_ * 1024)
-    assert _rings_init(chd, e, 512) == capi.ERR_INVALID
-    assert _rings_init(chd, e, 1025) == capi.ERR_CAPACITY
-    assert _rings_init(chd, e, 513) == capi.OK
-    assert _rings_init(chd, e, 1024) == capi.OK  # cells x cap == max_ring_entries
+    assert _status(lambda: e.rings_init(512)) == capi.ERR_INVALID
+    assert _status(lambda: e.rings_init(1025)) == capi.ERR_CAPACITY
+    e.rings_init(513)
+    e.rings_init(1024)  # cells x cap == max_ring_entries
     e_one_less = chd.engine.Engine(chd.engine.grid_cfg(*w.g), 16, w.S, max_ring_entries=C_ * 1024 - 1)
-    assert _rings_init(chd, e_one_less, 1024) == capi.ERR_CAPACITY
-    assert _rings_init(chd, e_one_less, 1023) == capi.OK
+    assert _status(lambda: e_one_less.rings_init(1024)) == capi.ERR_CAPACITY
+    e_one_less.rings_init(1023)
     e_one_less.close()
     e2 = chd.engine.Engine(chd.engine.grid_cfg(*w.g), 16, w.S, max_ring_entries=C_ * 1024)
-    assert _rings_init(chd, e2, 1024) == capi.OK
+    e2.rings_init(1024)
     chans = oracle.channels(C_)
 
     def updates(lo, hi, t):
@@ -594,26 +577,26 @@ def test_ring_argument_edges(chd, oracle):
     # an append without updates changes nothing
     zero = np.zeros(C_ + 1, np.uint32)
     assert e.L.chd_rings_append(e.h, p(zero), 0, None, None) == capi.OK
-    assert int(_get_rings(chd, e)["off"][-1]) == 0
+    assert int(e.get_rings()["off"][-1]) == 0
     # two appends in one tick == the same updates concatenated per cell in one append (and == the oracle)
     n1, a1, s1 = updates(0, 30, 1000 * MS)
     n2, a2, s2 = updates(0, 30, 1000 * MS)
     for n_, a_, s_ in ((n1, a1, s1), (n2, a2, s2)):
-        e._ck(_append(chd, e, _csr(n_), a_, s_))
+        e.rings_append(_csr(n_), a_, s_)
         chans.on_update(np.repeat(np.arange(C_, dtype=np.uint32), n_), a_, s_)
     o1, o2 = _csr(n1).astype(np.int64), _csr(n2).astype(np.int64)
     cat = [np.concatenate([x[o1[c]:o1[c + 1]], y[o2[c]:o2[c + 1]]]) for c in range(C_) for x, y in [(a1, a2)]]
     cat_s = [np.concatenate([x[o1[c]:o1[c + 1]], y[o2[c]:o2[c + 1]]]) for c in range(C_) for x, y in [(s1, s2)]]
-    e2._ck(_append(chd, e2, _csr(n1 + n2), np.concatenate(cat), np.concatenate(cat_s)))
-    got = _get_rings(chd, e)
+    e2.rings_append(_csr(n1 + n2), np.concatenate(cat), np.concatenate(cat_s))
+    got = e.get_rings()
     _assert_rings(got, chans.get_rings())
-    _assert_rings(_get_rings(chd, e2), got)
+    _assert_rings(e2.get_rings(), got)
     # an append larger than the upload buffers (they grow), with floods past 512 in every cell
     n3, a3, s3 = updates(600, 700, 1300 * MS)
     assert n3.sum() > 150_000
-    e._ck(_append(chd, e, _csr(n3), a3, s3))
+    e.rings_append(_csr(n3), a3, s3)
     chans.on_update(np.repeat(np.arange(C_, dtype=np.uint32), n3), a3, s3)
-    _assert_rings(_get_rings(chd, e), chans.get_rings())
+    _assert_rings(e.get_rings(), chans.get_rings())
     # a CSR that claims 3 entries more than n_updates (still inside the grown upload buffers, which hold stale updates there):
     # only the first n_updates are appended
     n4, a4, s4 = updates(0, 9, 1500 * MS)
@@ -621,9 +604,9 @@ def test_ring_argument_edges(chd, oracle):
     n_upd = int(off4[-1])
     off4[-1] += 3
     a4p, s4p = np.concatenate([a4, np.full(3, 1500 * MS, np.int64)]), np.concatenate([s4, np.full(3, 99, np.uint32)])
-    e._ck(_append(chd, e, off4, a4p, s4p, n=n_upd))
+    e.rings_append(off4, a4p, s4p, n=n_upd)
     chans.on_update(np.repeat(np.arange(C_, dtype=np.uint32), n4), a4, s4)
-    _assert_rings(_get_rings(chd, e), chans.get_rings())
+    _assert_rings(e.get_rings(), chans.get_rings())
     # chd_assemble_payloads indexes payload bytes by ring position: refused on device-owned rings
     e.set_subscribers(w.conn)
     e.set_entities(np.array([w.g[0] + 1.0]), np.array([w.g[1] + 1.0]))
@@ -660,7 +643,7 @@ def test_ring_inputs_are_refused_while_a_begun_interest_chain_reads_them(chd, or
     n0 = rng.integers(0, 9, C_)
     a0 = (t - rng.integers(0, 100 * MS, n0.sum())).astype(np.int64)
     s0 = np.full(n0.sum(), 7, np.uint32)
-    e._ck(_append(chd, e, _csr(n0), a0, s0))
+    e.rings_append(_csr(n0), a0, s0)
     ref.chans.on_update(np.repeat(np.arange(C_, dtype=np.uint32), n0), a0, s0)
     e.fanout_tick(t)
     s = e.summary()
@@ -670,7 +653,7 @@ def test_ring_inputs_are_refused_while_a_begun_interest_chain_reads_them(chd, or
     n1 = rng.integers(0, 9, C_)
     a1 = (t1 - rng.integers(0, 100 * MS, n1.sum())).astype(np.int64)
     s1 = np.full(n1.sum(), 7, np.uint32)
-    e._ck(_append(chd, e, _csr(n1), a1, s1))
+    e.rings_append(_csr(n1), a1, s1)
     ref.chans.on_update(np.repeat(np.arange(C_, dtype=np.uint32), n1), a1, s1)
     want = oracle.sphere_pairs(w.og, np.array([w.g[0] + 1.0]), np.array([w.g[1] + 1.0]), cx, cz, rad)
     w_sub = np.repeat(np.arange(w.S), np.diff(want["pair_off"].astype(np.int64)))
@@ -681,13 +664,13 @@ def test_ring_inputs_are_refused_while_a_begun_interest_chain_reads_them(chd, or
     bad = rng.integers(1, 5, C_)
     bad_a = np.full(bad.sum(), t1, np.int64)
     bad_s = np.full(bad.sum(), 8, np.uint32)
-    assert _append(chd, e, _csr(bad), bad_a, bad_s) == capi.ERR_STATE
-    assert _rings_init(chd, e, cap) == capi.ERR_STATE
+    assert _status(lambda: e.rings_append(_csr(bad), bad_a, bad_s)) == capi.ERR_STATE
+    assert _status(lambda: e.rings_init(cap)) == capi.ERR_STATE
     start = np.full(C_, 5 * MS, np.int64)
     assert e.L.chd_set_channel_start_times(e.h, p(start)) == capi.ERR_STATE
     s = e.tick(None, t1, capi.TICK_ALL)
     assert s.overflow == 0
-    _assert_rings(_get_rings(chd, e), ref.chans.get_rings())
+    _assert_rings(e.get_rings(), ref.chans.get_rings())
     np.testing.assert_array_equal(_due_from(w.conn, e.get_due(s.n_due)), _due_by_cell(ref, t1))
     e.close()
 

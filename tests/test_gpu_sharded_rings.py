@@ -18,7 +18,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.test_gpu_rings_scale import _append, _get_rings
+from tests.test_gpu_rings_scale import _status
 
 pytestmark = pytest.mark.gpu
 
@@ -160,7 +160,7 @@ def _slab_run(chd, world, cap, exchange, graphs=True):
         served.append(_served(lo, hi))
     for e in engines + [whole]:
         e.enable_graphs(graphs)
-        assert e.L.chd_rings_init(e.h, cap) == chd.capi.OK
+        e.rings_init(cap)
     rec_cap = max(len(s) for s in served)
     recs = [torch.zeros(2 * rec_cap, dtype=torch.int32, device="cuda") for _ in range(world)]
     gathered, n_gathered = None, 0
@@ -170,19 +170,19 @@ def _slab_run(chd, world, cap, exchange, graphs=True):
         if exchange and n_gathered:
             for e in engines:
                 e.import_ring_limits(gathered, n_gathered)
-        assert _append(chd, whole, *upd) == chd.capi.OK
+        whole.rings_append(*upd)
         sw = whole.tick(_batch(chd, *rw.queries(range(world), tick))[0], t, chd.capi.TICK_FANOUT)
         assert sw.overflow == 0
         n_due += sw.n_due
-        W_rings = _get_rings(chd, whole)
+        W_rings = whole.get_rings()
         conn_all = np.concatenate(rw.conn)
         w_due, w_pairs = _due_set(whole, sw.n_due, conn_all), _pair_set(whole, conn_all)
         for r, e in enumerate(engines):
-            assert _append(chd, e, *upd) == chd.capi.OK
+            e.rings_append(*upd)
             b, keep = _batch(chd, *rw.queries([r], tick))
             s = e.tick(b, t, chd.capi.TICK_FANOUT)
             assert s.overflow == 0
-            got = _get_rings(chd, e)
+            got = e.get_rings()
             if not exchange:
                 differ += _ring_difference(got, W_rings, served[r])
                 continue
@@ -236,13 +236,13 @@ def test_slab_refusals(chd):
     cfg = chd.engine.grid_cfg(0.0, 0.0, W, W, COLS, ROWS)
     rec = torch.zeros(2 * COLS * ROWS, dtype=torch.int32, device="cuda")
     plain = chd.engine.Engine(cfg, 16, 4)
-    assert plain.L.chd_rings_init(plain.h, 513) == chd.capi.OK
+    plain.rings_init(513)
     slab = chd.engine.Engine(cfg, 16, 4)
     slab.set_slab(0, 6, HALO)
     for e in (plain, slab):  # no slab / no device rings
         for st in (e.L.chd_export_ring_limits(e.h, chd.capi.ptr(rec), COLS * ROWS, None), e.L.chd_import_ring_limits(e.h, chd.capi.ptr(rec), 1)):
             assert st == chd.capi.ERR_STATE
-    assert slab.L.chd_rings_init(slab.h, 513) == chd.capi.OK
+    slab.rings_init(513)
     slab.set_subscribers(np.arange(1, 5, dtype=np.uint32))
     b, keep = _batch(chd, np.full(4, 50.0), np.full(4, 50.0), np.full(4, 20.0))
     slab.begin_interest(b, MS)
@@ -268,13 +268,13 @@ def _world_one(chd, graphs, n_ent=3000):
     for e in (sh, one):
         e.enable_graphs(graphs)
         e.set_subscribers(conn)
-        assert e.L.chd_rings_init(e.h, 620) == chd.capi.OK
+        e.rings_init(620)
     return rw, sh, one, conn, x, z
 
 
 def _compare(chd, sh, one, s1, s2, conn):
     assert s1.overflow == 0 and s2.overflow == 0 and s1.n_due == s2.n_due
-    a, b = _get_rings(chd, sh), _get_rings(chd, one)
+    a, b = sh.get_rings(), one.get_rings()
     for k in ("off", "arrival", "sender", "index", "msg_index"):
         np.testing.assert_array_equal(a[k], b[k], err_msg=k)
     assert _due_set(sh, s1.n_due, conn) == _due_set(one, s2.n_due, conn)
@@ -296,7 +296,7 @@ def test_tick_sharded_with_device_rings_at_world_one_matches_a_single_engine(chd
         sh.set_entity_ids(np.arange(len(x), dtype=np.uint32))
         one.set_entities(x, z)
         for e in (sh, one):
-            assert _append(chd, e, *upd) == chd.capi.OK
+            e.rings_append(*upd)
         s1 = sh.tick_sharded(b, t, chd.capi.TICK_ALL)
         s2 = one.tick(b, t, chd.capi.TICK_ALL)
         _compare(chd, sh, one, s1, s2, conn)
@@ -326,13 +326,12 @@ def test_staged_updates_on_a_communicator_engine(chd):
             assert L.chd_tick_sharded(sh.h, None, times[tick], chd.capi.TICK_ALL, None) == STATE
             sh.tick(None, times[tick], chd.capi.TICK_ALL)  # (joins it)
             break
-        assert _append(chd, one, *upd) == OK
-        assert _append(chd, sh, *upd) == OK
+        one.rings_append(*upd)
+        sh.rings_append(*upd)
         if tick == 1:
             other = rw.updates(tick, times[tick])  # (a different batch: applying it would show)
-            assert _append(chd, sh, *other) == STATE
-            off = np.zeros(COLS * ROWS + 1, np.uint32)
-            assert L.chd_get_rings(sh.h, chd.capi.ptr(off), None, None, None, None, 0) == STATE
+            assert _status(lambda: sh.rings_append(*other)) == STATE
+            assert _status(sh.get_rings) == STATE
             assert L.chd_tick(sh.h, C.byref(b), times[tick], chd.capi.TICK_ALL, None) == STATE
             assert L.chd_begin_interest(sh.h, C.byref(b), times[tick], 1) == STATE
             assert L.chd_update_interest(sh.h, C.byref(b), times[tick]) == STATE

@@ -13,7 +13,6 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from tests.test_gpu_rings_scale import _append, _get_rings
 
 pytestmark = pytest.mark.gpu
 
@@ -209,7 +208,7 @@ def _make_engines(chd, sw, table_mode, graphs=True):
         whole.set_entities(sw.x, sw.z)
     for e in engines + [whole]:
         e.enable_graphs(graphs)
-        assert e.L.chd_rings_init(e.h, RING_CAP) == chd.capi.OK
+        e.rings_init(RING_CAP)
     return whole, engines
 
 
@@ -252,7 +251,7 @@ def _slab_run(chd, world, table_mode, ticks=12):
         exchanged += _exchange_limits(chd, engines, recs)
         upd = sw.updates(tick, t)
         for e in engines + [whole]:
-            assert _append(chd, e, *upd) == chd.capi.OK
+            e.rings_append(*upd)
         # 3. the tick
         b, keep = sw.query_batch(chd, sw.regular, sw.whole_slot)
         s = whole.tick(b, t, chd.capi.TICK_ALL | DELTA)
@@ -262,7 +261,7 @@ def _slab_run(chd, world, table_mode, ticks=12):
         w_vis = _norm(_per_conn(*whole.get_visible(), sw.whole_conns))
         eo, en, lo, le = whole.get_visible_delta()
         w_enter, w_leave = _norm(_per_conn(eo, en, sw.whole_conns)), _norm(_per_conn(lo, le, sw.whole_conns))
-        W_rings = _get_rings(chd, whole)
+        W_rings = whole.get_rings()
         if not table_mode:
             for r, e in enumerate(engines):
                 m = np.nonzero(sw.ent_owner == r)[0]
@@ -281,7 +280,7 @@ def _slab_run(chd, world, table_mode, ticks=12):
             b, keep = sw.query_batch(chd, mine, sw.table.slot)
             s = e.tick(b, t, chd.capi.TICK_EMIT | chd.capi.TICK_FANOUT | DELTA)
             assert s.overflow == 0
-            got_rings = _get_rings(chd, e)
+            got_rings = e.get_rings()
             for c in served[r]:
                 for k in ("arrival", "sender", "index"):
                     np.testing.assert_array_equal(got_rings[k][got_rings["off"][c]:got_rings["off"][c + 1]],
@@ -369,7 +368,7 @@ def _raise_run(chd, exchange):
         e.set_subscribers(np.array([r + 1], np.uint32))
         engines.append(e)
     for e in engines + [whole]:
-        assert e.L.chd_rings_init(e.h, RING_CAP) == chd.capi.OK
+        e.rings_init(RING_CAP)
     cell = 1 * COLS + 5
     recs = [torch.zeros(2 * CELLS, dtype=torch.int32, device="cuda") for _ in range(2)]
     rng = np.random.default_rng(3)
@@ -386,12 +385,12 @@ def _raise_run(chd, exchange):
         off = np.concatenate([[0], np.cumsum(n)]).astype(np.uint32)
         upd = (off, t - rng.integers(0, 5 * MS, int(off[-1])).astype(np.int64), np.full(int(off[-1]), 9, np.uint32))
         for e in engines + [whole]:
-            assert _append(chd, e, *upd) == chd.capi.OK
+            e.rings_append(*upd)
             assert e.tick(None, t, chd.capi.TICK_FANOUT).overflow == 0
-        W_r = _get_rings(chd, whole)
+        W_r = whole.get_rings()
         want = W_r["index"][W_r["off"][cell]:W_r["off"][cell + 1]]
         for r, e in enumerate(engines):
-            g = _get_rings(chd, e)
+            g = e.get_rings()
             got = g["index"][g["off"][cell]:g["off"][cell + 1]]
             if exchange:
                 np.testing.assert_array_equal(got, want, err_msg="tick %d rank %d" % (tick, r))
@@ -421,7 +420,7 @@ def _comm_world(chd, graphs, migrate=8, rings=True):
         e.enable_graphs(graphs)
         e.set_subscribers(sw.whole_conns)
         if rings:
-            assert e.L.chd_rings_init(e.h, RING_CAP) == chd.capi.OK
+            e.rings_init(RING_CAP)
     one.set_entities(sw.x, sw.z)
     return sw, sh, one
 
@@ -469,7 +468,7 @@ def test_tick_sharded_with_migration_matches_a_single_engine(chd, graphs):
             moved += len(ms)
         upd = sw.updates(tick, t)
         for e in (sh, one):
-            assert _append(chd, e, *upd) == chd.capi.OK
+            e.rings_append(*upd)
         sh.set_entities(sw.x, sw.z)
         sh.set_entity_ids(np.arange(N_ENT, dtype=np.uint32))
         b1, k1 = sw.query_batch(chd, sw.regular, slot_of)
@@ -483,7 +482,7 @@ def test_tick_sharded_with_migration_matches_a_single_engine(chd, graphs):
         assert _pairs(sh, sh_conn) == _pairs(one, one_conn), tick
         assert _dues(sh, s1.n_due, sh_conn) == _dues(one, s2.n_due, one_conn), tick
         assert _norm(_per_conn(*sh.get_visible(), sh_conn)) == _norm(_per_conn(*one.get_visible(), one_conn))
-        a, b = _get_rings(chd, sh), _get_rings(chd, one)
+        a, b = sh.get_rings(), one.get_rings()
         for k in ("off", "arrival", "sender", "index", "msg_index"):
             np.testing.assert_array_equal(a[k], b[k], err_msg=k)
     assert moved == 5
@@ -514,7 +513,7 @@ def test_rules(chd):
     plain.close()
     slab = chd.engine.Engine(cfg, 16, 4)
     slab.set_slab(0, 6, HALO)
-    assert slab.L.chd_rings_init(slab.h, RING_CAP) == chd.capi.OK
+    slab.rings_init(RING_CAP)
     slab.set_subscribers(np.arange(1, 5, dtype=np.uint32))
     refused(slab, "apply_subscriptions")
     b, keep = _batch(chd, [1], [50.0], [50.0])
@@ -527,7 +526,7 @@ def test_rules(chd):
     slab.close()
     sw, sh, one = _comm_world(chd, True)
     upd = sw.updates(0, 1000 * MS)
-    assert _append(chd, sh, *upd) == chd.capi.OK
+    sh.rings_append(*upd)
     refused(sh)
     sh.set_entities(sw.x, sw.z)
     sh.set_entity_ids(np.arange(N_ENT, dtype=np.uint32))

@@ -11,7 +11,7 @@ import pytest
 from tests._subs_oracle import DIST_EXPLICIT, ERR_CAPACITY, OPT_DELAY, OPT_INTERVAL, OPT_SKIP_FIRST, OPT_SKIP_SELF, SubsOracle
 from tests.test_gpu_fanout_scale import _due_table
 from tests.test_gpu_fetch_delta import DeltaSet
-from tests.test_gpu_rings_scale import _append, _assert_rings, _csr, _due_from, _get_rings, _rings_init
+from tests.test_gpu_rings_scale import _assert_rings, _csr, _due_from
 from tests.test_oracle_delta import _cells
 
 pytestmark = pytest.mark.gpu
@@ -134,17 +134,17 @@ def test_fanout_over_explicit_pairs(chd, oracle):
     maximum exactly when the oracle did (at creation only)."""
     rng = np.random.default_rng(2)
     e, conn = _small(chd)
-    assert _rings_init(chd, e, 1024) == chd.capi.OK
+    e.rings_init(1024)
     o = SubsOracle(oracle, C_SMALL, conn, default_interval_ms=e.lim.default_fanout_interval_ms, default_delay_ms=e.lim.default_fanout_delay_ms)
     t_prev, n_due, longest, maxima = 0, 0, 0, set()
     for tick in range(24):
         t = (tick + 1) * 33 * MS
         _apply(e, o, _random_ops(rng, 200, 16, 40), t)
         n_cell, cell, arr, snd = _updates(rng, C_SMALL, t_prev, t, conn, flood=4)
-        assert _append(chd, e, _csr(n_cell), arr, snd) == chd.capi.OK
+        e.rings_append(_csr(n_cell), arr, snd)
         o.ch.on_update(cell, arr, snd)
         want_rings = o.ch.get_rings()
-        _assert_rings(_get_rings(chd, e), want_rings)
+        _assert_rings(e.get_rings(), want_rings)
         longest = max(longest, int(np.diff(want_rings["off"].astype(np.int64))[:4].max()))
         maxima |= set(want_rings["max_interval_ms"][:4].tolist())
         e.fanout_tick(t)
@@ -313,7 +313,7 @@ def test_scale_ops_queries_and_fanout(chd, oracle, graphs):
     e.enable_graphs(graphs)
     e.set_entities(ex, ez)
     e.set_subscribers(conn)
-    assert _rings_init(chd, e, 1024) == chd.capi.OK
+    e.rings_init(1024)
     g = _oracle.make_grid(wc.offx, wc.offz, wc.w, wc.h, wc.cols, wc.rows, wc.server_cols, wc.server_rows)
     o = SubsOracle(oracle, C, conn, default_interval_ms=e.lim.default_fanout_interval_ms, default_delay_ms=e.lim.default_fanout_delay_ms)
     damp = lambda d: oracle.damping(d, e.lim.default_fanout_interval_ms)  # noqa: E731
@@ -329,7 +329,7 @@ def test_scale_ops_queries_and_fanout(chd, oracle, graphs):
         batch, keep = chd.engine.make_batch(len(qs), sub=qs, sphere=(cx[qs], cz[qs], qr))
         q_st, q_off, q_ids, q_dist = oracle.query_batch(g, len(qs), sphere=(cx[qs], cz[qs], qr))
         n_cell, cell, arr, snd = _updates(rng, C, t_prev, t, conn[:64])
-        assert _append(chd, e, _csr(n_cell), arr, snd) == chd.capi.OK
+        e.rings_append(_csr(n_cell), arr, snd)
         s = e.tick(batch, t, chd.capi.TICK_ALL)
         # the oracle in the engine's order: interest update, ring updates, tickData
         qoff = q_off.astype(np.int64)
@@ -409,7 +409,7 @@ def test_scale_pipelined_with_visible_delta(chd, oracle, graphs):
     e.set_entities(ex, ez)
     e.set_subscribers(conn)
     e.reserve_visible_delta(1 << 26)
-    assert _rings_init(chd, e, 1024) == chd.capi.OK
+    e.rings_init(1024)
     g = _oracle.make_grid(wc.offx, wc.offz, wc.w, wc.h, wc.cols, wc.rows, wc.server_cols, wc.server_rows)
     ent_cell = _cells(oracle, g, ex, ez)
     o = SubsOracle(oracle, NC, conn, default_interval_ms=e.lim.default_fanout_interval_ms, default_delay_ms=e.lim.default_fanout_delay_ms)
@@ -432,7 +432,7 @@ def test_scale_pipelined_with_visible_delta(chd, oracle, graphs):
             qr = r[qs] * rng.choice([0.5, 1.0, 2.0, 3.0], len(qs))
             batch, keep = chd.engine.make_batch(len(qs), sub=qs, sphere=(cx[qs], cz[qs], qr))
             n_cell, cell, arr, snd = _updates(rng, NC, t_prev, t, conn[:64])
-            assert _append(chd, e, _csr(n_cell), arr, snd) == chd.capi.OK
+            e.rings_append(_csr(n_cell), arr, snd)
             fs = sets[tick % 2]
             fs.reset()
             assert chd.L.chd_tick(e.h, C.byref(batch), t, chd.capi.TICK_ALL | chd.capi.TICK_VISIBLE_DELTA, None) == 0, chd.L.chd_last_error(e.h)

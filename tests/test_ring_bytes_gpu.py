@@ -23,7 +23,7 @@ import pytest
 
 from tests._ring_bytes import ByteRing, entry_bytes, msg_indices, update_bytes
 from tests.test_gpu_payload_scale import DROP_ENTRY, MP_DROP, Payload, _value_len_for_mp, check_frames, restate_frames
-from tests.test_gpu_rings_scale import (N_TICKS, S0, _append, _assert_rings, _csr, _due_from, _engine, _get_rings, _Reference, _World, chd)  # noqa: F401
+from tests.test_gpu_rings_scale import (N_TICKS, S0, _assert_rings, _csr, _due_from, _engine, _Reference, _status, _World, chd)  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -94,10 +94,10 @@ def test_ring_parity(chd, oracle, grid, cap):
             x.summary()
         r = ref.tick(tick, t, want)
         e._ck(_append_bytes(chd, e, r["upd_off"], r["u_arr"], r["u_snd"], msg_before))
-        plain._ck(_append(chd, plain, r["upd_off"], r["u_arr"], r["u_snd"]))
-        got = _get_rings(chd, e)
+        plain.rings_append(r["upd_off"], r["u_arr"], r["u_snd"])
+        got = e.get_rings()
         _assert_rings(got, r["rings"])
-        _assert_rings(got, _get_rings(chd, plain))
+        _assert_rings(got, plain.get_rings())
         _assert_bytes(e, got)
         # the restatement of the hot cells (every other cell holds a few entries at its slab starts)
         uo = r["upd_off"].astype(np.int64)
@@ -169,7 +169,7 @@ def test_payloads(chd, oracle, mode):
             e.summary()
         r = ref.tick(tick, t, want)
         e._ck(_append_bytes(chd, e, r["upd_off"], r["u_arr"], r["u_snd"], msg_before))
-        rings = _get_rings(chd, e)
+        rings = e.get_rings()
         _assert_rings(rings, r["rings"])
         msg_before = rings["msg_index"].copy()
         eoff, eb = e.get_ring_bytes()
@@ -245,7 +245,7 @@ def test_byte_capacity(chd, oracle):
     e.set_entities(np.array([w.g[0] + 1.0]), np.array([w.g[1] + 1.0]))
     e.set_subscribers(w.conn)
     e.build()
-    e._ck(e.L.chd_rings_init(e.h, cap))
+    e.rings_init(cap)
     e.rings_reserve_bytes(bcap)
     rest = [ByteRing(cap, bcap) for _ in range(w.C)]
     rng = np.random.default_rng(52)
@@ -274,7 +274,7 @@ def test_byte_capacity(chd, oracle):
             dropped_ticks.append(tick)
         e.rings_append_bytes(upd_off, arr, snd, boff, data)
         assert bool(_summary_overflow(chd, e) & capi.OVF_RING) == (drops > 0), tick
-        got = _get_rings(chd, e)
+        got = e.get_rings()
         go = got["off"].astype(np.int64)
         for c in range(w.C):
             ents = rest[c].ents
@@ -288,7 +288,7 @@ def test_byte_capacity(chd, oracle):
         np.testing.assert_array_equal(np.diff(off.astype(np.int64)), [len(x[3]) for r in rest for x in r.ents])
     assert 18 in rest[0].byte_slides and rest[1].drops == 1 and dropped_ticks == [2]
     # an update longer than the slab: CHD_ERR_INVALID, nothing appended, no launch
-    before, before_bytes, launches = _get_rings(chd, e), e.get_ring_bytes(), e.launch_count()
+    before, before_bytes, launches = e.get_rings(), e.get_ring_bytes(), e.launch_count()
     n_cell = np.zeros(w.C, np.int64)
     n_cell[[3, 4]] = 1
     boff = np.array([0, 10, 10 + bcap + 1], np.uint64)
@@ -298,7 +298,7 @@ def test_byte_capacity(chd, oracle):
     arr, snd = np.full(2, t, np.int64), np.ones(2, np.uint32)
     assert e.L.chd_rings_append_bytes(e.h, p(uo), 2, p(arr), p(snd), p(boff), p(data)) == capi.ERR_INVALID
     assert e.launch_count() == launches
-    after = _get_rings(chd, e)
+    after = e.get_rings()
     for k in before:
         np.testing.assert_array_equal(after[k], before[k])
     assert e.get_ring_bytes()[1].tobytes() == before_bytes[1].tobytes()
@@ -321,7 +321,7 @@ def test_rules(chd, oracle):
         e.set_subscribers(w.conn)
         e.build()
         if init:
-            e._ck(e.L.chd_rings_init(e.h, cap))
+            e.rings_init(cap)
         return e
 
     def refused(e, st, call):
@@ -337,14 +337,14 @@ def test_rules(chd, oracle):
     # the reserve: after chd_rings_init, before any append
     e = fresh(init=False)
     refused(e, capi.ERR_STATE, lambda: e.L.chd_rings_reserve_bytes(e.h, 256))
-    e._ck(e.L.chd_rings_init(e.h, cap))
+    e.rings_init(cap)
     refused(e, capi.ERR_INVALID, lambda: e.L.chd_rings_reserve_bytes(e.h, 0))
-    e._ck(_append(chd, e, upd_off, arr, snd))
+    e.rings_append(upd_off, arr, snd)
     refused(e, capi.ERR_STATE, lambda: e.L.chd_rings_reserve_bytes(e.h, 256))
     # an engine without the reservation refuses chd_rings_append_bytes
-    rings = _get_rings(chd, e)
+    rings = e.get_rings()
     refused(e, capi.ERR_STATE, lambda: _append_bytes(chd, e, upd_off, arr, snd, rings["msg_index"]))
-    _assert_rings(_get_rings(chd, e), rings)
+    _assert_rings(e.get_rings(), rings)
     # ... and chd_assemble_payloads on device rings, as before
     pl = Payload(chd, e, w.S)
     pl.set_bytes(np.zeros(1, np.uint64), np.zeros(0, np.uint8), np.zeros(w.C + 1, np.uint64), np.zeros(0, np.uint8))
@@ -359,10 +359,10 @@ def test_rules(chd, oracle):
     e.rings_reserve_bytes(256)
     e.rings_reserve_bytes(512)  # again before any append: accepted
     e._ck(_append_bytes(chd, e, upd_off, arr, snd, zero))
-    rings = _get_rings(chd, e)
-    refused(e, capi.ERR_STATE, lambda: _append(chd, e, upd_off, arr, snd))
+    rings = e.get_rings()
+    refused(e, capi.ERR_STATE, lambda: _status(lambda: e.rings_append(upd_off, arr, snd)))
     refused(e, capi.ERR_STATE, lambda: e.L.chd_rings_reserve_bytes(e.h, 512))
-    _assert_rings(_get_rings(chd, e), rings)
+    _assert_rings(e.get_rings(), rings)
     _assert_bytes(e, rings)
     # chd_set_payload_bytes with entries: CHD_ERR_INVALID
     eo = np.array([0, 1], np.uint64)
@@ -378,22 +378,22 @@ def test_rules(chd, oracle):
     assert e.L.chd_assemble_payloads(e.h, C.byref(ncls), None, 0, None, 0, C.byref(blen)) == capi.OK
     e._ck(_append_bytes(chd, e, upd_off, (arr + 10 * MS).astype(np.int64), snd, rings["msg_index"]))
     refused(e, capi.ERR_STATE, lambda: e.L.chd_assemble_payloads(e.h, C.byref(ncls), None, 0, None, 0, C.byref(blen)))
-    rings = _get_rings(chd, e)
-    e._ck(e.L.chd_rings_init(e.h, cap))
-    empty = _get_rings(chd, e)
+    rings = e.get_rings()
+    e.rings_init(cap)
+    empty = e.get_rings()
     assert int(empty["off"][-1]) == 0
     assert e.get_ring_bytes()[1].size == 0
     refused(e, capi.ERR_STATE, lambda: e.L.chd_assemble_payloads(e.h, C.byref(ncls), None, 0, None, 0, C.byref(blen)))
     e._ck(_append_bytes(chd, e, upd_off, arr, snd, zero))  # the reservation survived chd_rings_init
-    _assert_bytes(e, _get_rings(chd, e))
+    _assert_bytes(e, e.get_rings())
     # rule 13: the reserve and the append are refused while a chd_begin_interest is pending
-    rings = _get_rings(chd, e)
+    rings = e.get_rings()
     batch, keep = chd.engine.make_batch(w.S, sub=None, sphere=(w.cx, w.cz, w.rad))
     e.begin_interest(batch, 20 * MS, with_fanout=True)
     refused(e, capi.ERR_STATE, lambda: _append_bytes(chd, e, upd_off, arr, snd, rings["msg_index"]))
     refused(e, capi.ERR_STATE, lambda: e.L.chd_rings_reserve_bytes(e.h, 512))
     e.tick(None, 20 * MS, capi.TICK_ALL)
-    _assert_rings(_get_rings(chd, e), rings)
+    _assert_rings(e.get_rings(), rings)
     _assert_bytes(e, rings)
     e.close()
     e = fresh()

@@ -12,7 +12,6 @@ import numpy as np
 import pytest
 
 from tests.test_gpu_payload_scale import Payload
-from tests.test_gpu_rings_scale import _append, _get_rings
 from tests.test_gpu_sharded_rings import (COLS, DEFAULT_IV, HALO, ROWS, W, RingWorld, _assert_rings_on, _batch, _compare, _due_set, _served,  # noqa: F401
                                           _world_one, chd)
 from tests.test_ring_bytes_gpu import MAX_LEN, _append_bytes, _assert_bytes, _entries_by_decision
@@ -56,7 +55,7 @@ def test_slab_replicas_carry_the_whole_world_bytes(chd, world):
         engines.append(e)
         served.append(_served(lo, hi))
     for e in engines + [whole]:
-        assert e.L.chd_rings_init(e.h, CAP) == chd.capi.OK
+        e.rings_init(CAP)
         e.rings_reserve_bytes(CAP * (MAX_LEN + 1))
     pls = [Payload(chd, e, len(rw.conn[r])) for r, e in enumerate(engines)]
     pw = Payload(chd, whole, len(conn_all))
@@ -75,7 +74,7 @@ def test_slab_replicas_carry_the_whole_world_bytes(chd, world):
         whole._ck(_append_bytes(chd, whole, *upd, msg_before))
         sw = whole.tick(_batch(chd, *rw.queries(range(world), tick))[0], t, chd.capi.TICK_FANOUT)
         assert sw.overflow == 0
-        W_rings = _get_rings(chd, whole)
+        W_rings = whole.get_rings()
         _assert_bytes(whole, W_rings)
         w_due = _due_set(whole, sw.n_due, conn_all)
         w_entries = _entries(pw, whole, conn_all, sw.n_due, full)
@@ -83,7 +82,7 @@ def test_slab_replicas_carry_the_whole_world_bytes(chd, world):
             e._ck(_append_bytes(chd, e, *upd, msg_before))
             s = e.tick(_batch(chd, *rw.queries([r], tick))[0], t, chd.capi.TICK_FANOUT)
             assert s.overflow == 0
-            got = _get_rings(chd, e)
+            got = e.get_rings()
             _assert_rings_on(got, W_rings, served[r], "tick %d rank %d" % (tick, r))
             _assert_bytes(e, got)  # every entry carries its own bytes; with the rings above, the served cells' bytes are the whole world's
             mine = set(rw.conn[r].tolist())
@@ -143,7 +142,7 @@ def test_tick_sharded_applies_the_staged_bytes(chd, graphs):
         s1 = sh.tick_sharded(b, t, capi.TICK_ALL)
         s2 = one.tick(b, t, capi.TICK_ALL)
         _compare(chd, sh, one, s1, s2, conn)
-        rings = _get_rings(chd, sh)
+        rings = sh.get_rings()
         _assert_bytes(sh, rings)
         _assert_bytes(one, rings)
         msg_before = rings["msg_index"].copy()
@@ -167,8 +166,8 @@ def test_reserve_is_refused_while_updates_are_staged(chd):
     # without the reservation: a staged chd_rings_append, chd_rings_init, then the reserve
     off = np.zeros(cells + 1, np.uint32)
     off[1:] = 1
-    assert _append(chd, sh, off, np.array([5], np.int64), np.array([3], np.uint32)) == capi.OK
-    assert sh.L.chd_rings_init(sh.h, CAP) == capi.OK
+    sh.rings_append(off, np.array([5], np.int64), np.array([3], np.uint32))
+    sh.rings_init(CAP)
     _refused(sh, capi.ERR_STATE, lambda: sh.L.chd_rings_reserve_bytes(sh.h, 1000))
     t = rw.times()[0]
     b, keep = _batch(chd, *rw.queries([0, 1], 0))
@@ -186,13 +185,13 @@ def test_reserve_is_refused_while_updates_are_staged(chd):
     p = capi.ptr
     arr, snd = np.array([t - 1], np.int64), np.array([3], np.uint32)
     assert sh.L.chd_rings_append_bytes(sh.h, p(off), 1, p(arr), p(snd), p(boff), p(data)) == capi.OK
-    assert sh.L.chd_rings_init(sh.h, CAP) == capi.OK
+    sh.rings_init(CAP)
     _refused(sh, capi.ERR_STATE, lambda: sh.L.chd_rings_reserve_bytes(sh.h, 100))
     sh.set_entities(x, z)
     sh.set_entity_ids(np.arange(len(x), dtype=np.uint32))
     s = sh.tick_sharded(b, t, capi.TICK_ALL)
     assert s.overflow == 0
-    rings = _get_rings(chd, sh)
+    rings = sh.get_rings()
     assert int(rings["off"][-1]) == 1 and int(rings["off"][1]) == 1
     got_off, got = sh.get_ring_bytes()
     assert got_off.tolist() == [0, 900] and got.tobytes() == data.tobytes()
