@@ -752,7 +752,9 @@ chd_status chd_comm_use_collective(chd_engine* e, int on);
 chd_status chd_migrate_out(chd_engine* e, const uint32_t* slot, uint32_t n);
 chd_status chd_migrate_in(chd_engine* e, uint32_t src_rank, uint32_t first_index, const uint32_t* slot, const uint32_t* conn_id, uint32_t n);
 /* own entities (of the last cell assignment) whose column lies outside this rank's slab: global id (entity-table mode: table id) +
- * the rank that owns the column now.  Synchronous and read-only.  *count = how many there are (copies min(count, cap)). */
+ * the rank that owns the column now.  Synchronous and read-only.  *count = how many there are (copies min(count, cap)).
+ * The owner is computed from chd_comm_init's world.  An engine made a slab with chd_set_slab alone knows no world and names rank 0
+ * as every destination (here and in chd_handoff_entities): the host that chose the slabs routes each entity by its column. */
 chd_status chd_get_rehome(chd_engine* e, uint32_t* global_id, uint32_t* dst_rank, uint32_t cap, uint32_t* count);
 /* Entity-table mode on slabs: hands the entities chd_get_rehome would list to their new owners.  Lists the own live in-world
  * entities of the last cell assignment whose column lies outside [col_lo, col_hi): id[i], dst_rank[i] (as chd_get_rehome computes
